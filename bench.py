@@ -3,6 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...   # the reference's CPU path, same metric
+    python bench.py ... --dump-outputs DIR                    # also write the last timed step's results as .npy
 
 Workload (config.workload): BASELINE.json configs[2], the one the metric is quoted on -- a 10M-entry
 GFKB of synthetic failures.jsonl-shaped ``signature_text`` rows, a 100k-query batch, the reference's
@@ -14,6 +15,13 @@ fixed): per-shard scan -> one all-gather of partial top-k -> merge.
 scan + merge [+ all-gather + merge]); ``e2e``: queries/s through the public API from host text
 buffers (host featurisation, host->device copies, kernels, device->host read of the result).
 Only the ``cpu_baseline`` / ``--impl reference`` legs execute anything under oracle/.
+
+``--dump-outputs DIR`` writes what the timed path returned in its last timed step: ``scores.npy`` (float32
+[queries, k]) and ``rows.npy`` (the global row ids as float64, -1 = empty slot).  The inputs are generated from
+fixed seeds, so two builds run with the same arguments can be compared output for output.  When the two arrays
+would exceed 64 MB, a fixed, seeded sample of the queries is written instead and ``query_index.npy`` names them.
+Roofline fractions use the H100 SXM data-sheet peaks (3.35 TB/s HBM3, 989 TFLOP/s dense BF16); the line records
+the card's name and power limit beside them.
 """
 from __future__ import annotations
 
@@ -22,6 +30,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 from pathlib import Path
@@ -31,6 +40,9 @@ sys.path.insert(0, str(ROOT))
 
 METRIC = "fingerprint-match queries/sec over 10M-entry GFKB"
 UNIT = "queries/s"
+H100_HBM_GBS = 3350.0       # H100 SXM data sheet, HBM3
+H100_BF16_TFLOPS = 989.0    # H100 SXM data sheet, dense BF16 (700 W card)
+DUMP_LIMIT_BYTES = 64 << 20
 
 
 def parse_args():
@@ -50,7 +62,42 @@ def parse_args():
     ap.add_argument("--shard", default="rows", choices=["rows", "queries", "rows-text"],
                     help="rows: corpus rows sharded over the GPUs by row index (BASELINE configs[2]); rows-text: sharded by ranges of "
                          "the global text order (tighter chunks per shard); queries: index replicated, queries split")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's results (scores.npy float32, rows.npy float64) to DIR")
+    a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
+    return a
+
+
+def dump_outputs(out_dir, scores, rows):
+    """The timed path's result arrays as .npy (float32 scores, float64 row ids); a fixed, seeded sample of the queries
+    when the whole result would exceed DUMP_LIMIT_BYTES."""
+    import numpy as np
+
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    scores = np.asarray(scores, dtype=np.float32)
+    rows = np.asarray(rows).astype(np.float64)
+    per_query = scores[0].nbytes + rows[0].nbytes if len(scores) else 1
+    if scores.nbytes + rows.nbytes > DUMP_LIMIT_BYTES:
+        keep = np.sort(np.random.default_rng(20240915).choice(len(scores), (DUMP_LIMIT_BYTES - 4096) // (per_query + 8), replace=False))  # 4 KB: .npy headers
+        np.save(d / "query_index.npy", keep.astype(np.float64))
+        scores, rows = scores[keep], rows[keep]
+    np.save(d / "scores.npy", scores)
+    np.save(d / "rows.npy", rows)
+
+
+def gpu_info(gpu_index: int):
+    """Name and power limit of the card the numbers were measured on."""
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={gpu_index}", "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader,nounits"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL,
+                             text=True, timeout=30).stdout.strip().split(",")
+        return {"name": out[0].strip(), "power_limit_w": float(out[1]), "sm_max_mhz": float(out[2])}
+    except Exception:
+        import torch
+        return {"name": torch.cuda.get_device_name(gpu_index), "power_limit_w": None, "sm_max_mhz": None}
 
 
 def workload_config(a, world):
@@ -62,7 +109,7 @@ def workload_config(a, world):
         "parallelism": ("corpus rows sharded over %d GPU(s); queries replicated; pruning bounds pushed to peer GPUs over NVLink during the scan; 1 all-gather of partial top-k" % world)
                        if getattr(a, "shard", "rows").startswith("rows") else
                        ("index replicated on %d GPU(s); query batch split; 1 all-gather of the results" % world),
-        "l2": "inputs larger than L2 (column blocks + dense bound matrix >> 126 MB); no explicit flush",
+        "l2": "inputs larger than L2 (column blocks + dense bound matrix >> 50 MB); no explicit flush",
     }
 
 
@@ -128,13 +175,15 @@ def _ref_one(qtext):
 
 def _standalone_synth(seed, count, dup_of_seed=0, dup_rows=0):
     """Synthetic rows from oracle/_build/libkvsynth.so (the generator alone, g++-built by __graft_entry__.build()):
-    the reference arm creates its inputs without loading the product's CUDA library."""
+    the reference arm creates its inputs without loading the product's CUDA library.  Without that build the
+    generator is compiled into a temporary directory (the source tree may be read-only)."""
     import ctypes as C
 
     import numpy as np
 
     so = ROOT / "oracle" / "_build" / "libkvsynth.so"
     if not so.exists():
+        so = Path(tempfile.mkdtemp(prefix="kvsynth-")) / "libkvsynth.so"
         subprocess.run(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-pthread", str(ROOT / "oracle" / "synth_shim.cpp"),
                         "-o", str(so)], check=True)
     lib = C.CDLL(str(so))
@@ -256,7 +305,7 @@ def run_ours(a):
     if world > 1:
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         if os.environ.get("NCCL_DEBUG", "VERSION").upper() == "VERSION":
-            os.environ["NCCL_DEBUG"] = "WARN"   # the version banner goes to stdout, where the driver expects ONE JSON line
+            os.environ["NCCL_DEBUG"] = "WARN"   # the version banner would go to stdout, which carries ONE JSON line
         dist.init_process_group("nccl", device_id=torch.device(f"cuda:{local}"))
     torch.cuda.set_device(local)
     dev = torch.device(f"cuda:{local}")
@@ -334,6 +383,8 @@ def run_ours(a):
     step_ms = max_over_ranks(e0.elapsed_time(e1) / a.steps)
     lay = shard.index.layout()
     checksum = int(r.sum().item()) if r.numel() else 0
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, s.cpu().numpy(), r.cpu().numpy())
     kavg = [sum(x[i] for x in kern_ms) / len(kern_ms) for i in range(5)]   # bound0, seed scan, bound1, scan, merge
     local_kernels_ms = sum(kavg)
     # per-rank attribution of a step (max/min over ranks): own kernels, all-gather, global merge
@@ -397,12 +448,7 @@ def run_ours(a):
     assert int(er.sum()) == checksum, "end-to-end result differs from the resident-path result"
 
     # ---- roofline of the path, SURVEY section 8(d) accounting ----
-    peaks = {}
-    try:
-        peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())
-    except Exception:
-        pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = H100_HBM_GBS
     rows_local = lay["rows"]
     bytes_per_row = (lay["block_bytes"] + lay["norm_bytes"] + lay["directory_bytes"]) / max(1, rows_local)
     tiles = lay["last_tiles"]
@@ -412,20 +458,11 @@ def run_ours(a):
     path_s = local_kernels_ms / 1e3
     compulsory = tiles * rows_local * bytes_per_row + lay["last_upload_bytes"] + a.queries * a.k * 12 * lay["last_splits"]
     achieved = compulsory / path_s / 1e9
-    traffic = ncu_note = None
-    try:  # dram bytes of exactly these launches, from the committed ncu capture (same workload only)
-        tr = json.loads((ROOT / "profiles" / "r2_path_traffic.json").read_text())
-        if (tr["rows"], tr["queries"], tr["k"], tr["n_gpus"]) == (a.rows, a.queries, a.k, world):
-            traffic, ncu_note = tr["traffic_bytes_per_step"], tr.get("note")
-    except Exception:
-        pass
     pairs_all = a.queries * lay["chunks"]
     roofline = {
         "bound": "hbm", "kernel": "GFKB match path = " + " + ".join(names[:4]), "dominant_kernel": names[dom],
-        "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-        "traffic_source": ("profiles/r2_path_traffic.json (ncu capture of this workload, committed; not re-measured in this run)" if traffic else None),
-        "ncu_note": ncu_note,
-        "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)",
+        "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
+        "peak_source": "H100 SXM data sheet (HBM3 3.35 TB/s at up to 700 W; see gpu.power_limit_w)",
         "algorithmic_bytes_per_step": compulsory, "bytes_per_row": bytes_per_row,
         "query_tile": 128, "query_tiles": tiles, "partial_lists_per_query": lay["last_splits"],
         "chunks": lay["chunks"], "chunk_rows": 32,
@@ -568,24 +605,24 @@ def run_ours(a):
         c1_ok = bool(np.allclose(c1_s, np.take_along_axis(c1_ref, c1_r, axis=1), rtol=1e-5, atol=1e-7))
         c1.close()
         dflops = 2.0 * dn * dq * dd
-        tpeak = float(peaks.get("bf16_tflops", 1590.0))
-        tsust = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1590.0)))
+        tpeak = H100_BF16_TFLOPS
         secondary = {
             "k2_dense_cosine_1Mx768_10k_queries": {"kernel": "dense_topk_kernel", "ms": min(dms), "flops": dflops,
                                                    "achieved_tflops": dflops / (min(dms) / 1e3) / 1e12,
-                                                   "frac_of_bf16_burst_peak": dflops / (min(dms) / 1e3) / 1e12 / tpeak,
+                                                   "frac_of_bf16_datasheet_peak": dflops / (min(dms) / 1e3) / 1e12 / tpeak,
                                                    "queries_per_s": dq / (min(dms) / 1e3), "row_splits": int(dsplits),
-                                                   "note": "BASELINE configs[1]; tcgen05 cta_group::1 M128 N256 K16, 3-stage TMA ring, 8 epilogue warps, fused top-16; "
+                                                   "note": "BASELINE configs[1]; wgmma m64n256k16 on two consumer warpgroups (M128 N256), 3-stage TMA ring, "
+                                                           "epilogue on the accumulator registers, fused top-16; "
                                                            "synthetic bf16 embeddings (random sign/mantissa, exponent 2^-7..2^0); parity unpinned"},
             "k2_dense_cosine_10Mx768_100k_queries_1gpu": {"kernel": "dense_topk_kernel", "ms": min(d10ms), "flops": 2.0 * d10 * 100_000 * dd,
                                                           "achieved_tflops": 2.0 * d10 * 100_000 * dd / (min(d10ms) / 1e3) / 1e12,
-                                                          "frac_of_bf16_sustained_peak": 2.0 * d10 * 100_000 * dd / (min(d10ms) / 1e3) / 1e12 / tsust,
+                                                          "frac_of_bf16_datasheet_peak": 2.0 * d10 * 100_000 * dd / (min(d10ms) / 1e3) / 1e12 / tpeak,
                                                           "queries_per_s": 100_000 / (min(d10ms) / 1e3), "row_splits": int(d10splits),
                                                           "note": "BASELINE configs[2] read as 768-d bf16 embeddings (SURVEY 8(d) cfg3, 1-GPU variant): 10M rows = 15.4 GB resident, "
                                                                   "100k-query batch, fused top-16; kernel time only; parity unpinned"},
             "k2_dense_allpairs_1Mx1M_top32": {"kernel": "dense_topk_kernel (self-join, own row excluded)", "ms": min(ams),
                                               "flops": 2.0 * dn * dn * dd, "achieved_tflops": 2.0 * dn * dn * dd / (min(ams) / 1e3) / 1e12,
-                                              "frac_of_bf16_sustained_peak": 2.0 * dn * dn * dd / (min(ams) / 1e3) / 1e12 / tsust,
+                                              "frac_of_bf16_datasheet_peak": 2.0 * dn * dn * dd / (min(ams) / 1e3) / 1e12 / tpeak,
                                               "rows_per_s": dn / (min(ams) / 1e3),
                                               "note": "BASELINE configs[3]: every row's 32 nearest other rows; full N x N (symmetry not exploited); parity unpinned"},
             "k3_jaccard_1M_sets_2048_queries": {"kernel": "jaccard_scan_kernel", "rows": jn, "queries": jq, "ms": min(jms),
@@ -615,7 +652,6 @@ def run_ours(a):
     if world > 1 and not a.no_secondary:
         from kakveda_b200.dist import ShardedDense, ShardedJaccard, shard_bounds
         secondary_multi = {}
-        tsust = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1590.0)))
         dd, d10, dq = 768, 10_000_000, 100_000
 
         def dense_rows(count, seed):
@@ -641,7 +677,7 @@ def run_ours(a):
         secondary_multi["k2_dense_cosine_10Mx768_100k_queries_sharded"] = {
             "n_gpus": world, "ms_step_max_over_ranks": dms, "ms_kernel_max_over_ranks": kms, "flops": 2.0 * d10 * dq * dd,
             "achieved_tflops_whole_job": 2.0 * d10 * dq * dd / (dms / 1e3) / 1e12,
-            "frac_of_bf16_sustained_peak_x_gpus": 2.0 * d10 * dq * dd / (dms / 1e3) / 1e12 / (tsust * world),
+            "frac_of_bf16_datasheet_peak_x_gpus": 2.0 * d10 * dq * dd / (dms / 1e3) / 1e12 / (H100_BF16_TFLOPS * world),
             "queries_per_s": dq / (dms / 1e3), "result_checksum": int(dr_.sum().item()),
             "note": "SURVEY 8(d) cfg3 as specified: rows sharded over the GPUs, queries replicated, K2 per shard, one all-gather of partial top-k + K5; "
                     "step = kernel + exchange + merge (CUDA events, max over ranks); parity unpinned"}
@@ -729,7 +765,7 @@ def run_ours(a):
         line = {
             "metric": METRIC, "value": a.queries / (step_ms / 1e3), "unit": UNIT, "n_gpus": world, "steps": a.steps,
             "warmup": a.warmup, "ms_per_step": step_ms, "higher_is_better": True, "scaling": "strong",
-            "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": cfg, "clocks": clocks,
+            "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": cfg, "gpu": gpu_info(local), "clocks": clocks,
             "e2e": {"value": a.queries / e2e_s, "unit": UNIT, "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
                     "ms_per_step": e2e_s * 1e3, "rank0_split_ms": getattr(shard, "last_e2e_ms", None),
                     "rank0_ms_per_call": e2e_calls},

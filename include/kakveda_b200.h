@@ -1,5 +1,5 @@
 /*
- * kakveda_b200 -- C ABI of the B200-native GFKB fingerprint-match engine.
+ * kakveda_b200 -- C ABI of the H100-native GFKB fingerprint-match engine.
  *
  * The reference (prateekdevisingh/kakveda) is pure Python and has no FFI for this path;
  * its one similarity entry point is the method
@@ -241,7 +241,7 @@ int kv_merge_topk_device_on(int device, const void *d_scores_in, const void *d_r
  * milliseconds on its stream:
  * ms[0] = H2D of the query batch, ms[1] = bound + scan kernels, ms[2] = merge (+ fallbacks), ms[3] = D2H. */
 int kv_index_last_timing(const kv_index *ix, float ms[4]);
-/* ... and of its kernels: ms[0] = bound pass 0 (seeds; tcgen05 GEMM + rare-feature join), ms[1] = seed scan,
+/* ... and of its kernels: ms[0] = bound pass 0 (seeds; wgmma GEMM + rare-feature join), ms[1] = seed scan,
  * ms[2] = bound pass 1 (candidate lists), ms[3] = candidate scan, ms[4] = merge.  Exhaustive mode: only [3], [4]. */
 int kv_index_last_kernel_ms(const kv_index *ix, float ms[5]);
 /* Test hook: runs the resident batch once and returns the numerators (dot-product upper bounds) the bound kernel formed
@@ -272,7 +272,7 @@ int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[17]);
 
 /* ------------------------------------------------------------------------------------
  * K2: dense-embedding cosine index (bf16 rows of `dim` elements, dim a multiple of 64) with the
- * top-k fused into a tcgen05 GEMM epilogue.  The reference has no embedding path (its docs list
+ * top-k fused into a wgmma GEMM epilogue.  The reference has no embedding path (its docs list
  * embeddings as a possible extension, docs/failure-intelligence.md:43-46): parity UNPINNED, oracle =
  * float64 cosine of the same bf16 inputs.  Inputs are bfloat16 bit patterns (uint16), row-major.
  * kv_dense_topk: per query the k (<=32) best rows by (cosine desc, row asc); host outputs

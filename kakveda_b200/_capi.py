@@ -115,7 +115,7 @@ def load():
     p = lib_path()
     if not p.exists():
         raise ImportError(
-            f"{p} not found: build it with `python -m kakveda_b200.build` (nvcc, sm_100a). "
+            f"{p} not found: build it with `python -m kakveda_b200.build` (nvcc, sm_90a). "
             "kakveda_b200 has no CPU fallback."
         )
     lib = C.CDLL(str(p))

@@ -1,4 +1,4 @@
-// K1b-B: upper bounds of every (query, chunk) score on the 5th-gen tensor cores, and the candidate lists they leave.
+// K1b-B: upper bounds of every (query, chunk) score on the Hopper tensor cores, and the candidate lists they leave.
 //
 // For a query q and a chunk c (32 rows), with U_c(t) = largest tf of feature t in the chunk (0 if absent) and
 // Bmin_c = smallest positive row norm of the chunk:
@@ -7,9 +7,12 @@
 // so  score(q, r) <= ub(q, c) = dot_bound / sqrt(|q|^2 (Bmin_c + corrS_q))  for every row r of c  (exact block-max
 // pruning: a chunk whose bound is below a query's k-th best score cannot hold a top-k row for it).
 //   * the sum over the NF = 256 FREQUENT features is a [128 queries x 256] x [256 x 64 chunks] fp16 GEMM (weights
-//     rounded UP to fp16, tf exact): tcgen05.mma cta_group::1 kind::f16, M = 128, N = 64, fp32 accumulators in TMEM
-//     (double buffered), the query operand resident in shared memory for the CTA's life, the chunk operand streamed
-//     by TMA (128B swizzle, mbarrier expect_tx) -- this only computes BOUNDS; scores stay exact integer sums (K1b-S);
+//     rounded UP to fp16, tf exact): one MMA warpgroup issues wgmma.mma_async m64n64k16 (two per K step, one per
+//     64-query half), fp32 accumulators in its registers, the query operand resident in shared memory for the CTA's
+//     life, the chunk operand streamed by TMA (128B swizzle, mbarrier expect_tx; one thread of the warpgroup refills a
+//     stage as soon as the warpgroup's MMAs have read it); the warpgroup adds its accumulators
+//     into R (below) while the workers run the rare join of the same block, so the GEMM of block b + 1 overlaps the
+//     epilogue of block b -- this only computes BOUNDS; scores stay exact integer sums (K1b-S);
 //   * the next NF2 = 1024 features by chunk frequency ("second class": mid-frequency words and bigrams, each shared by
 //     many queries of a tile) are kept per 64-chunk block as two TRANSPOSED presence bitmaps Ubt[feature][tf >= 1,
 //     tf >= 2][64 chunk bits] (16 KB, one bulk-async copy per block, double buffered): a query thread reads ONE word per
@@ -19,13 +22,14 @@
 //     it, largest tf); each query looks ITS OWN <= 32 rare features up -- one shared-memory bit test per (query,
 //     feature, block), and only on a hit a probe of the block's table in L2 -- and adds weight x tf into
 //     R[chunk][query] (shared memory).  1.8k bit tests per tile and block instead of 5.4k entry probes;
-//   * epilogue (16 warps, four threads per query, tcgen05.ld of 16 chunk columns each): bound vs the query's threshold.
+//   * epilogue (16 warps, four threads per query, 16 chunk columns of R each): bound vs the query's threshold.
 //     pass 0 keeps, per thread, the 4 best chunks by bound (16 seeds per query: K1b-S scores them first, which gives
 //     every query a close lower bound theta0 of its k-th best score) and stores every bound as an 8-bit code rounded up
 //     (the selection kernel below builds the candidate lists from the codes); pass 1 (only when the codes do not fit in
 //     memory) recomputes the bounds and appends {chunk, mask of the group's surviving queries} to the scan group's
 //     candidate list (paged pool) for every chunk with ub >= theta0.
-// One CTA = one 128-query tile x one range of 64-chunk blocks; 18 warps: 16 workers (join + epilogue), TMA, MMA.
+// One CTA = one 128-query tile x one range of 64-chunk blocks; 20 warps: 16 workers (join + epilogue) and the MMA +
+// TMA warpgroup (warps 16-19).
 #pragma once
 #include "tfidf_kernels.cuh"
 
@@ -40,7 +44,12 @@ constexpr int B_STAGES = 2;
 constexpr int B_A_SLICE_BYTES = TILE_Q * B_BK * 2;  // 16 KiB: one K slice of the query operand
 constexpr int B_B_SLICE_BYTES = B_BN * B_BK * 2;    // 8 KiB: one K slice of the chunk operand
 constexpr int B_WORKERS = 16;
-constexpr int B_THREADS = (B_WORKERS + 2) * 32;
+constexpr int B_MMA_WARP = B_WORKERS;        // first warp of the MMA warpgroup (a warpgroup starts at a multiple of 4)
+constexpr int B_THREADS = (B_WORKERS + 4) * 32;
+// named barriers (0 is __syncthreads): R complete for the epilogue (workers wait, the MMA warpgroup arrives), R clean
+// again for the next block's accumulators (the MMA warpgroup waits, the workers arrive), the workers among themselves,
+// the MMA warpgroup among itself (a chunk slice has been read by all four warps and may be refilled)
+constexpr int B_BAR_RFULL = 1, B_BAR_RCLEAN = 2, B_BAR_WORKERS = 3, B_BAR_MMA = 4;
 constexpr int B_COLS = B_BN / 4;             // chunk columns per epilogue thread (four threads serve a query)
 constexpr int B_SEEDS = 4;                   // seeds per worker thread
 constexpr int B_SEEDS_PER_QUERY = 4 * B_SEEDS;
@@ -54,30 +63,43 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, u
       : "memory");
 }
 
-// shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups 1024 bytes apart
-__device__ __forceinline__ uint64_t umma_desc_sw128(const void *smem) {
+// wgmma shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups 1024 bytes apart (the operand tile
+// starts on a 1024-byte boundary, so the base offset is 0).  Advancing the start address by 32 bytes selects the next
+// K = 16 step inside the swizzled 128-byte row.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(const void *smem) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr(smem) & 0x3FFFF) >> 4);  // start address
   d |= (uint64_t)1 << 16;                              // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;                    // stride byte offset
-  d |= (uint64_t)1 << 46;                              // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                              // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                              // SWIZZLE_128B
   return d;
 }
 
-// instruction descriptor: D = f32, A = B = f16, both K-major, N = 64, M = 128
-constexpr uint32_t B_IDESC = (1u << 4) | ((uint32_t)(B_BN >> 3) << 17) | ((uint32_t)(TILE_Q >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of an accumulator register across an asynchronous wgmma
+__device__ __forceinline__ void wgmma_reg_fence(float &r) { asm volatile("" : "+f"(r)::"memory"); }
 
-__device__ __forceinline__ void umma_f16_128(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t accumulate) {
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, fp16 in, fp32 accumulators in registers (both operands K-major)
+__device__ __forceinline__ void wgmma_m64n64k16_f16(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(B_IDESC), "r"(accumulate)
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      "%24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d)
       : "memory");
 }
+
 // wait of a single-lane role (TMA producer, MMA issuer): polls with a pause, so that the spinning lane does not
 // take issue slots from the worker warps sharing its scheduler
 __device__ __forceinline__ void mbar_wait_idle(uint64_t *bar, uint32_t parity) {
@@ -103,10 +125,6 @@ __device__ __forceinline__ float rsqrt_approx(float x) {
   float y;
   asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-
-__device__ __forceinline__ void umma_commit_1(uint64_t *bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_addr(bar)) : "memory");
 }
 
 struct BoundParams {
@@ -154,8 +172,7 @@ struct __align__(1024) BoundSmem {
   uint2 q2[Q2CAP][TILE_Q];                       // the queries' second-class lists (bit row | (tfmax - 1) << 16, weight)
   uint2 q3[Q3CAP][TILE_Q];                       // the queries' rare lists (feature id, weight)
   float minB[2][B_BN];
-  uint64_t full_bar[B_STAGES], empty_bar[B_STAGES], a_bar, blk_bar[2], tmem_full[2], tmem_empty[2];
-  uint32_t tmem_base;
+  uint64_t full_bar[B_STAGES], a_bar, blk_bar[2];
   unsigned int lcount[4];
   int pages[1];  // [4][max_pages], sized at launch
 };
@@ -181,16 +198,11 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
   const int64_t blk_lo = n_blocks * bsplit / P.n_bsplits, blk_hi = n_blocks * (bsplit + 1) / P.n_bsplits;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < B_STAGES; i++) { mbar_init(&S.full_bar[i], 1); mbar_init(&S.empty_bar[i], 1); }
+    for (int i = 0; i < B_STAGES; i++) mbar_init(&S.full_bar[i], 1);
     mbar_init(&S.a_bar, 1);
     mbar_init(&S.blk_bar[0], 1);
     mbar_init(&S.blk_bar[1], 1);
-    for (int i = 0; i < 2; i++) { mbar_init(&S.tmem_full[i], 1); mbar_init(&S.tmem_empty[i], B_WORKERS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == B_WORKERS + 1) {  // TMEM: 128 columns = two 128x64 fp32 accumulators
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 128;" ::"r"(smem_addr(&S.tmem_base)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   {  // second-class and rare lists of the tile's queries, R = 0, list state
     const uint4 *src2 = (const uint4 *)(P.q2list + (size_t)tile * Q2CAP * TILE_Q);
@@ -204,58 +216,83 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
     for (int i = threadIdx.x; i < 4 * P.max_pages; i += B_THREADS) S.pages[i] = -1;
     if (threadIdx.x < 4) S.lcount[threadIdx.x] = 0;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = S.tmem_base;
 
-  if (warp == B_WORKERS) {
-    // ===== TMA producer =====
-    if (lane == 0) {
+  if (warp >= B_MMA_WARP) {
+    // ===== MMA warpgroup: frequent part of the block's bounds, added into R =====
+    // accumulator fragment of m64nNk16: warp w of the warpgroup holds rows 16 w + lane / 4 (+ 8) of each 64-query
+    // half, register 4 j + e holds column 8 j + 2 (lane % 4) + (e & 1) of row + 8 (e >> 1)
+    const int wq = warp - B_MMA_WARP;
+    const bool producer = wq == 0 && lane == 0;
+    // chunk slices in global order g = (block - blk_lo) * B_KSLICES + slice; slice g goes to stage g % B_STAGES
+    const int64_t n_slices = (blk_hi - blk_lo) * B_KSLICES;
+    auto load_slice = [&](int64_t g) {
+      const int st = (int)(g % B_STAGES);
+      mbar_expect_tx(&S.full_bar[st], B_B_SLICE_BYTES);
+      tma_load_2d(S.b[st], &map_u, &S.full_bar[st], (int)(g % B_KSLICES) * B_BK, (int)((blk_lo + g / B_KSLICES) * B_BN));
+    };
+    if (producer) {
       mbar_expect_tx(&S.a_bar, B_KSLICES * B_A_SLICE_BYTES);
       for (int s = 0; s < B_KSLICES; s++) tma_load_2d(S.a[s], &map_w, &S.a_bar, s * B_BK, tile * TILE_Q);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int64_t bk = blk_lo; bk < blk_hi; bk++) {
-        for (int s = 0; s < B_KSLICES; s++) {
-          mbar_wait_idle(&S.empty_bar[stage], phase ^ 1);
-          mbar_expect_tx(&S.full_bar[stage], B_B_SLICE_BYTES);
-          tma_load_2d(S.b[stage], &map_u, &S.full_bar[stage], s * B_BK, (int)(bk * B_BN));
-          if (++stage == B_STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
+      for (int64_t g = 0; g < B_STAGES && g < n_slices; g++) load_slice(g);
     }
-  } else if (warp == B_WORKERS + 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      mbar_wait_idle(&S.a_bar, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int64_t it = 0;
-      for (int64_t bk = blk_lo; bk < blk_hi; bk++, it++) {
-        const int as = (int)(it & 1);
-        const uint32_t aphase = (uint32_t)((it >> 1) & 1);
-        mbar_wait_idle(&S.tmem_empty[as], aphase ^ 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tmem_d = tmem_base + (uint32_t)(as * B_BN);
-        for (int s = 0; s < B_KSLICES; s++) {
-          mbar_wait_idle(&S.full_bar[stage], phase);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t da = umma_desc_sw128(S.a[s]);
-          const uint64_t db = umma_desc_sw128(S.b[stage]);
+    // refill the stage of slice g (read by every warp of the warpgroup: wgmma_wait done) with slice g + B_STAGES
+    auto release = [&](int64_t g) {
+      asm volatile("bar.sync %0, 128;" ::"n"(B_BAR_MMA) : "memory");
+      if (producer && g + B_STAGES < n_slices) load_slice(g + B_STAGES);
+    };
+    float acc[2][32] = {};
+    mbar_wait_idle(&S.a_bar, 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    int64_t it = 0, g = 0;
+    for (int64_t bk = blk_lo; bk < blk_hi; bk++, it++) {
+#pragma unroll
+      for (int h = 0; h < 2; h++)
+#pragma unroll
+        for (int i = 0; i < 32; i++) wgmma_reg_fence(acc[h][i]);
+      wgmma_fence();
+      for (int s = 0; s < B_KSLICES; s++, g++) {
+        mbar_wait_idle(&S.full_bar[stage], phase);
+        const uint64_t db = wgmma_desc_sw128(S.b[stage]);
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          const uint64_t da = wgmma_desc_sw128(S.a[s] + h * (B_A_SLICE_BYTES / 2));  // rows 64 h .. 64 h + 63
 #pragma unroll
           for (int kk = 0; kk < B_BK / 16; kk++)  // advance 32 bytes (2 x 16-byte units) per K=16 step inside the swizzle row
-            umma_f16_128(tmem_d, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), (uint32_t)((s | kk) != 0));
-          umma_commit_1(&S.empty_bar[stage]);  // slot free once these MMAs have read it
-          if (++stage == B_STAGES) { stage = 0; phase ^= 1; }
+            wgmma_m64n64k16_f16(acc[h], da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), (uint32_t)((s | kk) != 0));
         }
-        umma_commit_1(&S.tmem_full[as]);  // accumulator complete
+        wgmma_commit();
+        if (s > 0) {  // the previous slice's group is done: its stage may be refilled
+          wgmma_wait<1>();
+          release(g - 1);
+        }
+        if (++stage == B_STAGES) { stage = 0; phase ^= 1; }
       }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int h = 0; h < 2; h++)
+#pragma unroll
+        for (int i = 0; i < 32; i++) wgmma_reg_fence(acc[h][i]);
+      release(g - 1);
+      // R holds the previous block's values until the workers' epilogue has read and cleared them
+      if (it > 0) asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_RCLEAN), "n"(B_THREADS) : "memory");
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int q0 = h * 64 + wq * 16 + (lane >> 2);
+#pragma unroll
+        for (int i = 0; i < 32; i++) {
+          const int c = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+          atomicAdd(&S.R[c][q0 + 8 * ((i >> 1) & 1)], acc[h][i]);  // the workers' rare join adds to R concurrently
+        }
+      }
+      asm volatile("bar.arrive %0, %1;" ::"n"(B_BAR_RFULL), "n"(B_THREADS) : "memory");
     }
+    if (it > 0) asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_RCLEAN), "n"(B_THREADS) : "memory");  // the last block's
   } else {
     // ===== workers: join, then epilogue, per block =====
-    const int qtr = warp & 3;   // TMEM lane quarter = scan group of the tile
-    const int cs = warp >> 2;   // which 32 chunk columns of a block this warp's epilogue covers
+    const int qtr = warp & 3;   // quarter of the tile's queries = scan group of the tile
+    const int cs = warp >> 2;   // which B_COLS chunk columns of a block this warp's epilogue covers
     const int qi = qtr * 32 + lane;
     const int64_t slot = (int64_t)tile * TILE_Q + qi;
     const bool q_in = slot < P.n_q;
@@ -325,9 +362,10 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
         const float th = __int_as_float(__ldcg(&P.gthr[slot]));
         if (th > 0.f) tq = jacc ? th / PRUNE_SLACK : th * th * nq / (PRUNE_SLACK * PRUNE_SLACK);
       }
-      asm volatile("bar.sync 1, 512;" ::: "memory");
-      // ---- epilogue, thread = query, B_COLS chunk columns: rare part (R) + second-class part (bitmaps) + frequent
-      //      part (TMEM) -> bound -> seed / candidate ----
+      // R complete: the workers' rare join and the MMA warpgroup's frequent part of this block
+      asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_RFULL), "n"(B_THREADS) : "memory");
+      // ---- epilogue, thread = query, B_COLS chunk columns: rare + frequent part (R) + second-class part (bitmaps)
+      //      -> bound -> seed / candidate ----
       float x[B_COLS];
       {
         float *Rcol = &S.R[cs * B_COLS][qi];
@@ -356,24 +394,6 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
           }
         }
       }
-      mbar_wait(&S.tmem_full[as], aphase);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      uint32_t v[B_COLS];
-      {
-        static_assert(B_COLS == 16, "the TMEM load below reads 16 columns");
-        const uint32_t taddr = tmem_base + ((uint32_t)(qtr * 32) << 16) + (uint32_t)(as * B_BN + cs * B_COLS);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-            : "r"(taddr)
-            : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&S.tmem_empty[as]);  // the values are in registers: the accumulator may be overwritten
       const float *mb = &S.minB[as][cs * B_COLS];
       const int64_t cbase = c0 + cs * B_COLS;
       uint32_t mymask = 0;
@@ -384,7 +404,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
       for (int j = 0; j < B_COLS / 4; j++) codes[j] = 0;
 #pragma unroll
       for (int j = 0; j < B_COLS; j++) {
-        const float xs = base + __uint_as_float(v[j]) + x[j];
+        const float xs = base + x[j];
         const bool c_ok = j < nv;
         if (dbg && q_in && c_ok) P.dbg_xs[(size_t)slot * P.dbg_stride + cbase + j] = xs;
         const float den = jacc ? (nq + mb[j] - xs) : (mb[j] + corrS);
@@ -442,7 +462,9 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
           }
         }
       }
-      asm volatile("bar.sync 1, 512;" ::: "memory");  // R is clean again and every reader of this block's side data is done
+      // R is clean again (the MMA warpgroup may add the next block) and every reader of this block's side data is done
+      asm volatile("bar.arrive %0, %1;" ::"n"(B_BAR_RCLEAN), "n"(B_THREADS) : "memory");
+      asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_WORKERS), "n"(B_WORKERS * 32) : "memory");
     }
     if (pass == 0) {
       if (q_in) {
@@ -463,12 +485,6 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
         }
       }
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == B_WORKERS + 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 128;" ::"r"(tmem_base) : "memory");
   }
 }
 

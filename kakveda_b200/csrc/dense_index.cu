@@ -1,4 +1,4 @@
-// K2: dense-embedding cosine scan with fused top-k on the 5th-gen tensor cores (BASELINE configs[1]:
+// K2: dense-embedding cosine scan with fused top-k on the Hopper tensor cores (BASELINE configs[1]:
 // "1M-entry GFKB, 768-d embedding cosine, 10k-query batch").
 //
 // The reference has no embedding path (SURVEY.md section 0: only TF-IDF exists, dense embeddings are a
@@ -9,14 +9,16 @@
 // norms applied as fp32 scales in the epilogue, and the top-k fused into the epilogue so that the
 // [Q, N] score matrix never exists.  A work item is one (128-query tile, row split); items are ordered
 // split-major so that the CTAs resident together (one per SM) stream the same corpus rows through L2.  Few, long
-// row splits keep every list's k-th-score threshold high.  Per CTA (320 threads):
-//   warp 0      TMA producer: K-slices (64 elements) of the query tile and of the row tile -> 3-stage
-//               shared-memory ring (128B-swizzled), mbarrier expect_tx / complete_tx
-//   warp 1      MMA issuer: tcgen05.mma cta_group::1 kind::f16, M=128 N=256 K=16, accumulators in TMEM
-//               (2 x 256 columns, double buffered); tcgen05.commit releases ring slots / publishes a tile
-//   warps 2-9   epilogue (two warps per TMEM lane quarter, each scanning half of the 256 columns): tcgen05.ld of
-//               the thread's TMEM lane (= its query), scale, threshold test, insertion into the thread's own sorted
-//               top-k list (k <= 32; ties keep the lower row; a self-join skips the query's own row)
+// row splits keep every list's k-th-score threshold high.  Per CTA (288 threads):
+//   warps 0-7   two consumer warpgroups, one per 64-query half of the tile: wgmma.mma_async m64n256k16 (bf16 in,
+//               fp32 accumulators in registers, 128 per thread), then the epilogue on those registers: one shuffle
+//               per pair of values gives every thread ONE query and half of the 256 columns (interleaved in groups of
+//               two); scale, threshold test, insertion into the thread's own sorted top-k list (k <= 32; ties keep
+//               the lower row; a self-join skips the query's own row)
+//   warp 8      TMA producer: K-slices (64 elements) of the query tile and of the row tile -> 3-stage
+//               shared-memory ring (128B-swizzled), mbarrier expect_tx / complete_tx; a slot is refilled once both
+//               warpgroups' MMAs have read it (empty barrier, one arrival per consumer warp)
+// While the consumers run a tile's epilogue, the producer already fills the ring with the next tile's first slices.
 // Each (query tile, split, column half) writes one partial list; K5 (kv_merge_topk_device) merges them.  CTAs
 // working on the same queries exchange k-th-score lower bounds through global memory (gthr).
 #include "kv_cuda.cuh"
@@ -31,8 +33,8 @@
 
 namespace {
 
-constexpr int BM = 128;        // queries per CTA (TMEM lanes)
-constexpr int BN = 256;        // corpus rows per MMA tile (TMEM columns per accumulator stage)
+constexpr int BM = 128;        // queries per CTA (two 64-row wgmma tiles)
+constexpr int BN = 256;        // corpus rows per MMA tile (the N of the wgmma)
 constexpr int BK = 64;         // K-slice: 64 bf16 = one 128-byte swizzle row
 constexpr int UMMA_K = 16;
 constexpr int STAGES = 3;       // 3 x 48 KiB ring + two list sets fit in 227 KiB
@@ -40,8 +42,8 @@ constexpr int A_BYTES = BM * BK * 2;  // 16 KiB
 constexpr int B_BYTES = BN * BK * 2;  // 32 KiB
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
 constexpr int MAXK = 32;       // per-query list slots: 2 x 32 x 128 x 8 B = 64 KiB beside the 3 x 48 KiB ring (k <= 32)
-constexpr int N_THREADS = 320;  // 10 warps: TMA, MMA, 8 epilogue
-constexpr int EPI_THREADS = 256;
+constexpr int EPI_THREADS = 256;  // the two consumer warpgroups
+constexpr int N_THREADS = EPI_THREADS + 32;  // + the TMA producer warp
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -76,32 +78,55 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, u
       : "memory");
 }
 
-// shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups 1024 bytes apart
-__device__ __forceinline__ uint64_t umma_desc(const void *smem) {
+// wgmma shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups 1024 bytes apart (every operand
+// tile starts on a 1024-byte boundary: base offset 0).  +32 bytes of start address = the next K = 16 step of the row.
+__device__ __forceinline__ uint64_t wgmma_desc(const void *smem) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_u32(smem) & 0x3FFFF) >> 4);  // start address
   d |= (uint64_t)1 << 16;                             // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;                   // stride byte offset
-  d |= (uint64_t)1 << 46;                             // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                             // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                             // SWIZZLE_128B
   return d;
 }
 
-// instruction descriptor: D=f32, A=B=bf16, both K-major, N=256, M=128
-constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+// keeps the compiler from moving accesses of an accumulator register across an asynchronous wgmma
+__device__ __forceinline__ void reg_fence(float &r) { asm volatile("" : "+f"(r)::"memory"); }
 
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t accumulate) {
+// D[64 x 256] (+)= A[64 x 16] * B[256 x 16]^T, bf16 in, fp32 accumulators in registers (both operands K-major)
+__device__ __forceinline__ void wgmma_m64n256k16_bf16(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(IDESC), "r"(accumulate)
+      "setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, "
+      "%22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, "
+      "%42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, "
+      "%62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, "
+      "%82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, "
+      "%101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, "
+      "%117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]),
+        "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]),
+        "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]),
+        "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]),
+        "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]),
+        "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]),
+        "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]),
+        "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]),
+        "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(scale_d)
       : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 struct DenseParams {
@@ -127,8 +152,7 @@ __device__ __forceinline__ float fkey_inv(unsigned int k) {
 
 struct __align__(1024) DenseSmem {
   unsigned char stage[STAGES][STAGE_BYTES];
-  uint64_t full_bar[STAGES], empty_bar[STAGES], tmem_full[2], tmem_empty[2];
-  uint32_t tmem_base;
+  uint64_t full_bar[STAGES], empty_bar[STAGES];
   __align__(16) float inv_c[2][BN];
   float lscore[2][MAXK][BM];  // [column half][slot][query]: the 32 lanes of a warp hit 32 different banks
   int lrow[2][MAXK][BM];
@@ -148,22 +172,15 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
   const int64_t L0 = my_qtile * P.r_tiles + P.r_tiles * my_split / P.n_lists;
   const int64_t L1 = my_qtile * P.r_tiles + P.r_tiles * (my_split + 1) / P.n_lists;
   const int n_kb = P.dim / BK;
+  constexpr unsigned FULL_MASK = 0xFFFFFFFFu;
 
-  if (warp == 0 && lane == 0) {
-    for (int i = 0; i < STAGES; i++) { mbar_init(&S.full_bar[i], 1); mbar_init(&S.empty_bar[i], 1); }
-    for (int i = 0; i < 2; i++) { mbar_init(&S.tmem_full[i], 1); mbar_init(&S.tmem_empty[i], 8); }
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < STAGES; i++) { mbar_init(&S.full_bar[i], 1); mbar_init(&S.empty_bar[i], EPI_THREADS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {  // TMEM: 512 columns = two 128x256 fp32 accumulators
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&S.tmem_base)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = S.tmem_base;
 
-  if (warp == 0) {
+  if (warp == EPI_THREADS / 32) {
     // ===== TMA producer =====
     if (lane == 0) {
       int stage = 0;
@@ -180,39 +197,19 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int64_t it = 0;
-      for (int64_t L = L0; L < L1; L++, it++) {
-        const int as = (int)(it & 1);
-        const uint32_t aphase = (uint32_t)((it >> 1) & 1);
-        mbar_wait(&S.tmem_empty[as], aphase ^ 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tmem_d = tmem_base + (uint32_t)(as * BN);
-        for (int kb = 0; kb < n_kb; kb++) {
-          mbar_wait(&S.full_bar[stage], phase);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t da = umma_desc(S.stage[stage]);
-          const uint64_t db = umma_desc(S.stage[stage] + A_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; k++)  // advance 32 bytes (2 x 16-byte units) per K=16 step inside the swizzle row
-            umma_f16(tmem_d, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (uint32_t)((kb | k) != 0));
-          umma_commit(&S.empty_bar[stage]);  // slot free once these MMAs have read it
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&S.tmem_full[as]);  // accumulator complete
-      }
-    }
   } else {
-    // ===== epilogue: warps 2..9; a warp may only touch TMEM lanes 32*(warp%4) .. +31, so two warps share
-    // each lane quarter and split the 256 columns of a tile between them (half 0 / half 1) =====
-    const int lane_base = 32 * (warp & 3);
-    const int qi = lane_base + lane;            // TMEM lane = query inside the tile
-    const int et = (warp - 2) * 32 + lane;      // 0..255 among the epilogue threads
-    const int half = (warp - 2) >> 2;           // which 128 columns of every tile this thread scans
+    // ===== consumers: MMA, then epilogue on the accumulator registers =====
+    // m64nNk16 accumulator fragment: warp w of the warpgroup holds rows 16 w + lane / 4 (register 4 j + e, e < 2) and
+    // 16 w + lane / 4 + 8 (e >= 2), columns 8 j + 2 (lane % 4) + (e & 1).  After the exchange with lane ^ 2, lanes with
+    // lane % 4 < 2 hold the first of those rows, the others the second, each for columns 8 j + 2 (lane & 1) + {0, 1}
+    // ("lo") and 8 j + 4 + 2 (lane & 1) + {0, 1} ("hi"): one query, half of the columns, ascending in j.
+    const int wg = warp >> 2, wq = warp & 3;
+    const int quad = lane & 3;
+    const bool upper = quad >= 2;
+    const int qi = wg * 64 + wq * 16 + (lane >> 2) + (upper ? 8 : 0);  // query inside the tile
+    const int et = threadIdx.x;                 // 0..255 among the epilogue threads
+    const int half = quad & 1;                  // which interleaved half of every tile's columns this thread scans
+    const int cofs = 2 * half;                  // column of register 4 j + m: 8 j + cofs + (m & 1) + 4 (m >> 1)
     const int k = P.k;
     float *ls = &S.lscore[half][0][qi];         // element j of this thread's list lives at ls[j * BM]
     int *lr = &S.lrow[half][0][qi];
@@ -234,11 +231,38 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
         P.part_rows[o] = j < cnt ? (long long)(P.row_base + lr[j * BM]) : -1LL;
       }
     };
+    float acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; i++) acc[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
     int64_t it = 0;
     for (int64_t L = L0; L < L1; L++, it++) {
       const int qtile = (int)(L / P.r_tiles);
       const int64_t t = L % P.r_tiles;
-      if (qtile != cur_qtile) {  // (warp-uniform) next query tile: publish and restart the lists
+      // ---- MMA over the K slices; a slice's ring slot is released once the next slice's MMAs are issued and the
+      //      slice's own have completed ----
+#pragma unroll
+      for (int i = 0; i < 128; i++) reg_fence(acc[i]);
+      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+      int prev = -1;
+      for (int kb = 0; kb < n_kb; kb++) {
+        mbar_wait(&S.full_bar[stage], phase);
+        const uint64_t da = wgmma_desc(S.stage[stage] + wg * (A_BYTES / 2));  // rows 64 wg .. 64 wg + 63 of the tile
+        const uint64_t db = wgmma_desc(S.stage[stage] + A_BYTES);
+#pragma unroll
+        for (int kk = 0; kk < BK / UMMA_K; kk++)  // advance 32 bytes (2 x 16-byte units) per K=16 step inside the swizzle row
+          wgmma_m64n256k16_bf16(acc, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), (uint32_t)((kb | kk) != 0));
+        asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+        if (prev >= 0) {
+          asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&S.empty_bar[prev]);
+        }
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      if (qtile != cur_qtile) {  // (CTA-uniform) next query tile: publish and restart the lists
         flush();
         cur_qtile = qtile;
         q = (int64_t)qtile * BM + qi;
@@ -254,7 +278,6 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
         for (int j = 0; j < k; j++) { ls[j * BM] = -INFINITY; lr[j * BM] = 0x7fffffff; }
       }
       const int as = (int)(it & 1);
-      const uint32_t aphase = (uint32_t)((it >> 1) & 1);
       // inverse norms of this tile's rows (0 past the end; such rows are rejected by index below)
       const int64_t row0 = t * BN;
       for (int c = et; c < BN; c += EPI_THREADS) S.inv_c[as][c] = (row0 + c < P.n_rows) ? P.inv_norm_c[row0 + c] : -INFINITY;  // 0 * -inf = NaN: never a candidate
@@ -267,73 +290,64 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
         }
       }
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      mbar_wait(&S.tmem_full[as], aphase);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t taddr = tmem_base + ((uint32_t)lane_base << 16) + (uint32_t)(as * BN);
-#pragma unroll 1
-      for (int c0 = half * (BN / 2); c0 < ((P.dbg == 1) ? 0 : (half + 1) * (BN / 2)); c0 += 32) {
-        uint32_t v[32];
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr + (uint32_t)c0)
-            : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (P.dbg == 2) { if (v[0] == 0x12345678u && v[31] == 0x9abcdef0u) thr = 1.f; continue; }
-        // 32 independent scale ops + a max tree: one (rarely taken) branch per 32 rows instead of 32
-        float tv[32];
-        const float4 *ic4 = reinterpret_cast<const float4 *>(&S.inv_c[as][c0]);
+      asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 #pragma unroll
-        for (int j4 = 0; j4 < 8; j4++) {
-          const float4 ic = ic4[j4];
-          tv[4 * j4 + 0] = __uint_as_float(v[4 * j4 + 0]) * ic.x;
-          tv[4 * j4 + 1] = __uint_as_float(v[4 * j4 + 1]) * ic.y;
-          tv[4 * j4 + 2] = __uint_as_float(v[4 * j4 + 2]) * ic.z;
-          tv[4 * j4 + 3] = __uint_as_float(v[4 * j4 + 3]) * ic.w;
+      for (int i = 0; i < 128; i++) reg_fence(acc[i]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&S.empty_bar[prev]);
+      if (P.dbg == 1) continue;
+      // one query per thread: swap the row this thread does not keep with lane ^ 2
+#pragma unroll
+      for (int j = 0; j < 32; j++) {
+        const float s0 = upper ? acc[4 * j + 0] : acc[4 * j + 2], s1 = upper ? acc[4 * j + 1] : acc[4 * j + 3];
+        const float m0 = upper ? acc[4 * j + 2] : acc[4 * j + 0], m1 = upper ? acc[4 * j + 3] : acc[4 * j + 1];
+        const float g0 = __shfl_xor_sync(FULL_MASK, s0, 2), g1 = __shfl_xor_sync(FULL_MASK, s1, 2);
+        acc[4 * j + 0] = upper ? g0 : m0;
+        acc[4 * j + 1] = upper ? g1 : m1;
+        acc[4 * j + 2] = upper ? m0 : g0;
+        acc[4 * j + 3] = upper ? m1 : g1;
+      }
+      if (P.dbg == 2) { if (acc[0] == 1.2345678f && acc[127] == 9.87654321f) thr = 1.f; continue; }
+      // per 8 values (16 columns): scale, max -> one branch; only groups where some query of the warp has a
+      // candidate are walked element by element (`sc > lo` == `sc > thr && sc >= gth`, lo = max(thr, pred(gth)))
+#pragma unroll
+      for (int sb = 0; sb < 16; sb++) {
+        float tv[8];
+#pragma unroll
+        for (int jj = 0; jj < 2; jj++) {
+          const int j = 2 * sb + jj;
+          const float2 icl = *reinterpret_cast<const float2 *>(&S.inv_c[as][8 * j + cofs]);
+          const float2 ich = *reinterpret_cast<const float2 *>(&S.inv_c[as][8 * j + 4 + cofs]);
+          tv[4 * jj + 0] = acc[4 * j + 0] * icl.x;
+          tv[4 * jj + 1] = acc[4 * j + 1] * icl.y;
+          tv[4 * jj + 2] = acc[4 * j + 2] * ich.x;
+          tv[4 * jj + 3] = acc[4 * j + 3] * ich.y;
         }
-        // per 8 columns: max -> one branch; only sub-blocks where some query of the warp has a candidate are
-        // walked element by element (`sc > lo` == `sc > thr && sc >= gth`, lo = max(thr, pred(gth)))
-#pragma unroll
-        for (int sb = 0; sb < 4; sb++) {
-          const float m01 = fmaxf(tv[8 * sb + 0], tv[8 * sb + 1]), m23 = fmaxf(tv[8 * sb + 2], tv[8 * sb + 3]);
-          const float m45 = fmaxf(tv[8 * sb + 4], tv[8 * sb + 5]), m67 = fmaxf(tv[8 * sb + 6], tv[8 * sb + 7]);
-          const float best = fmaxf(fmaxf(m01, m23), fmaxf(m45, m67)) * inv_q;
-          if (best > lo) {
+        const float m01 = fmaxf(tv[0], tv[1]), m23 = fmaxf(tv[2], tv[3]);
+        const float m45 = fmaxf(tv[4], tv[5]), m67 = fmaxf(tv[6], tv[7]);
+        const float best = fmaxf(fmaxf(m01, m23), fmaxf(m45, m67)) * inv_q;
+        if (best > lo) {
 #pragma unroll  // static indices keep tv[] in registers
-            for (int j = 8 * sb; j < 8 * sb + 8; j++) {
-              const float sc = tv[j] * inv_q;
-              if (sc > lo && (int)(row0 + c0 + j) != excl) {
-                int pos = cnt < k ? cnt++ : k - 1;
-                while (pos > 0 && ls[(pos - 1) * BM] < sc) {
-                  ls[pos * BM] = ls[(pos - 1) * BM];
-                  lr[pos * BM] = lr[(pos - 1) * BM];
-                  pos--;
-                }
-                ls[pos * BM] = sc;
-                lr[pos * BM] = (int)(row0 + c0 + j);
-                if (cnt == k) { thr = ls[(k - 1) * BM]; lo = fmaxf(thr, gth_pred); }
+          for (int e = 0; e < 8; e++) {
+            const float sc = tv[e] * inv_q;
+            const int col = 8 * (2 * sb + (e >> 2)) + cofs + (e & 1) + 4 * ((e >> 1) & 1);
+            if (sc > lo && (int)(row0 + col) != excl) {
+              int pos = cnt < k ? cnt++ : k - 1;
+              while (pos > 0 && ls[(pos - 1) * BM] < sc) {
+                ls[pos * BM] = ls[(pos - 1) * BM];
+                lr[pos * BM] = lr[(pos - 1) * BM];
+                pos--;
               }
+              ls[pos * BM] = sc;
+              lr[pos * BM] = (int)(row0 + col);
+              if (cnt == k) { thr = ls[(k - 1) * BM]; lo = fmaxf(thr, gth_pred); }
             }
           }
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&S.tmem_empty[as]);
       if (q_ok && cnt == k && thr > gth) atomicMax(&P.gthr[q], fkey(thr));
     }
     flush();
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
   }
 }
 
@@ -383,7 +397,7 @@ struct kv_dense_index {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[2] = {nullptr, nullptr};
   std::mutex mu;
-  int sm_count = 148;
+  int sm_count = 132;
   DevVec<__nv_bfloat16> rows;
   int64_t n_rows = 0;
   DevBuf<float> d_inv_c, d_inv_q, d_part_s, d_out_s;

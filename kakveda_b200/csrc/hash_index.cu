@@ -101,7 +101,7 @@ struct kv_hash_index {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[2] = {nullptr, nullptr};
   std::mutex mu;
-  int sm_count = 148;
+  int sm_count = 132;
   DevVec<unsigned long long> rows;
   int64_t n_rows = 0;
   DevBuf<unsigned long long> d_keys, d_pairs;

@@ -23,7 +23,7 @@ extern "C" {
 
 const char *kv_last_error(void) { return g_err; }
 
-const char *kv_version(void) { return "kakveda_b200 0.1 (sm_100a)"; }
+const char *kv_version(void) { return "kakveda_b200 0.1 (sm_90a)"; }
 
 int kv_device_count(void) {
   int n = 0;

@@ -43,7 +43,7 @@ struct kv_index {
   cudaEvent_t evp2 = nullptr;  // start of phase 2 of a two-phase batch
   bool two_phase = false;
   std::mutex mu;
-  int sm_count = 148;
+  int sm_count = 132;
 
   // raw CSR: device copy for the statistics kernels and K6, host copy for the sort and the column blocks
   DevVec<int64_t> indptr;  // n_rows + 1 entries once any row exists

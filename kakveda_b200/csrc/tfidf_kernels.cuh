@@ -1,6 +1,6 @@
 // Device code of the TF-IDF cosine index: finalize kernels, query preparation, K1a (one query, float64 scores of
 // every row), K1b-S (exact scan of candidate (query, chunk) pairs with fused top-k), K5 (list merge), K6 (float64
-// re-scoring).  The bound kernel K1b-B (tcgen05) lives in bound_kernel.cuh.  Included by tfidf_index.cu only.
+// re-scoring).  The bound kernel K1b-B (wgmma) lives in bound_kernel.cuh.  Included by tfidf_index.cu only.
 //
 // Math (SURVEY.md section 7, restating sklearn text.py:1650-1739 + pairwise.py:1742-1752 as called
 // by services/shared/similarity.py:14-20).  The reference refits TF-IDF on [query]+corpus per

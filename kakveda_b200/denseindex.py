@@ -1,4 +1,4 @@
-"""Dense-embedding cosine index (K2): bf16 GEMM on the tcgen05 tensor cores with a fused top-k.
+"""Dense-embedding cosine index (K2): bf16 GEMM on the Hopper tensor cores (wgmma) with a fused top-k.
 
 Extension of the reference (which only has TF-IDF; embeddings are listed as a possible upgrade in
 docs/failure-intelligence.md:43-46).  Rows and queries are float arrays rounded to bfloat16 on the way in;

@@ -7,7 +7,7 @@ assignment (services/gfkb/app.py:31,86).  ``GfkbIndex`` is the resident device i
 engine caches between calls, and the batched entry point (``topk``) the GFKB match handler's
 sort/top-5 (services/gfkb/app.py:88-91) maps onto.
 
-All arithmetic runs in libkakveda_b200.so (hand-written sm_100a kernels).  Nothing here falls
+All arithmetic runs in libkakveda_b200.so (hand-written sm_90a kernels).  Nothing here falls
 back to scikit-learn or NumPy math: without the library or without a GPU the calls raise.
 """
 from __future__ import annotations
@@ -190,7 +190,7 @@ class Vocabulary:
 
 
 class GfkbIndex:
-    """Resident TF-IDF index of one row shard of the GFKB on one B200.
+    """Resident TF-IDF index of one row shard of the GFKB on one H100.
 
     ``row_base`` is the global index of the shard's first row; ``vocab`` may be shared between
     shards living in one process.  Usage: ``add_texts`` / ``add_features`` (append-only, like

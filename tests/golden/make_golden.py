@@ -1,13 +1,13 @@
 """Generate the golden vectors under tests/golden/ by RUNNING THE UNMODIFIED REFERENCE.
 
-Run in the authoring container only (needs /root/reference; the GPU box has no copy):
+Needs a checkout of the reference (its directory in KAKVEDA_REFERENCE); the tests only read the JSON output:
 
     python tests/golden/make_golden.py
 
 Everything numerical in the JSON files comes from ``services.shared.similarity.SimilarityEngine``
 (services/shared/similarity.py:14-20), ``services.shared.fingerprint`` (fingerprint.py:51-71) and the
 GFKB handler ``services.gfkb.app.match`` (services/gfkb/app.py:79-102) imported from
-/root/reference; inputs are either the reference's own test / fixture data or seeded synthetic rows
+the reference checkout; inputs are either the reference's own test / fixture data or seeded synthetic rows
 from ``kakveda_b200.synth`` (regenerated, and checksum-verified, at test time).
 """
 from __future__ import annotations
@@ -15,11 +15,12 @@ from __future__ import annotations
 import hashlib
 import json
 import sys
+import os
 from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
 REPO = HERE.parent.parent
-REF = Path("/root/reference")
+REF = Path(os.environ["KAKVEDA_REFERENCE"])
 sys.path.insert(0, str(REPO))
 sys.path.insert(0, str(REF))
 

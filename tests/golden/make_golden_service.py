@@ -1,6 +1,6 @@
 """Golden vectors for the resident-GFKB service layer (kakveda_b200/store.py), made by RUNNING THE UNMODIFIED
 REFERENCE handlers ``/failures/upsert`` and ``/failures/match`` (services/gfkb/app.py:79-147) through FastAPI's
-TestClient in the authoring container (needs /root/reference):
+TestClient (needs a checkout of the reference, its directory in KAKVEDA_REFERENCE):
 
     python tests/golden/make_golden_service.py
 
@@ -16,11 +16,12 @@ import pathlib
 import random
 import sys
 import tempfile
+import os
 from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
 REPO = HERE.parent.parent
-REF = Path("/root/reference")
+REF = Path(os.environ["KAKVEDA_REFERENCE"])
 sys.path.insert(0, str(REPO))
 sys.path.insert(0, str(REF))
 

@@ -1,6 +1,6 @@
 """Golden vectors for the batched warning path (kakveda_b200/store.py::GfkbStore.warn_batch), made by RUNNING THE
-UNMODIFIED REFERENCE handler ``/warn`` (services/warning_policy/app.py:19-72) in the authoring container (needs
-/root/reference):
+UNMODIFIED REFERENCE handler ``/warn`` (services/warning_policy/app.py:19-72) (needs a checkout of the
+reference, its directory in KAKVEDA_REFERENCE):
 
     python tests/golden/make_golden_warn.py
 
@@ -17,11 +17,12 @@ import json
 import pathlib
 import sys
 import tempfile
+import os
 from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
 REPO = HERE.parent.parent
-REF = Path("/root/reference")
+REF = Path(os.environ["KAKVEDA_REFERENCE"])
 sys.path.insert(0, str(REPO))
 sys.path.insert(0, str(REF))
 

@@ -497,7 +497,7 @@ def test_jaccard_token_sets(lib):
 
 
 def test_bound_kernel_numerators_vs_numpy(lib):
-    """K1b-B (tcgen05 GEMM over the frequent features + transposed bitmaps of the second class + rare-feature join): the
+    """K1b-B (wgmma GEMM over the frequent features + transposed bitmaps of the second class + rare-feature join): the
     dot-product upper bound of every (query, chunk) pair equals the exact union bound sum_{t in q and chunk}
     tf_q a(t) max_tf_chunk(t) computed with NumPy -- never below it (the pruning stays exact), and within 0.1 % of
     it for all but a sliver of the pairs (fp16 round-up of weights; a chunk holding tf >= 2 of a second-class
