@@ -22,6 +22,9 @@
 //     it, largest tf); each query looks ITS OWN <= 32 rare features up -- one shared-memory bit test per (query,
 //     feature, block), and only on a hit a probe of the block's table in L2 -- and adds weight x tf into
 //     R[chunk][query] (shared memory).  1.8k bit tests per tile and block instead of 5.4k entry probes;
+//   * R is fixed point, uint32 in units of 1 / s_q per query (s_q: a power of two chosen by prep_queries_kernel so that
+//     R cannot wrap), every term rounded up into it: the MMA warpgroup's and the rare join's adds are native integer
+//     shared atomics (a float shared atomicAdd is a compare-and-swap loop on sm_90a);
 //   * epilogue (16 warps, four threads per query, 16 chunk columns of R each): bound vs the query's threshold.
 //     pass 0 keeps, per thread, the 4 best chunks by bound (16 seeds per query: K1b-S scores them first, which gives
 //     every query a close lower bound theta0 of its k-th best score) and stores every bound as an 8-bit code rounded up
@@ -135,7 +138,7 @@ struct BoundParams {
   const uint32_t *ovf_vals;
   int n_ovf;
   int64_t n_chunks, n_q;
-  const uint2 *q3list;                                    // [n_tiles][Q3CAP][TILE_Q] rare (feature, weight) lists of the queries
+  const uint2 *q3list;                                    // [n_tiles][Q3CAP][TILE_Q] rare (feature, fixed-point weight) lists
   const uint32_t *rbloom;                                 // [n_blocks][RB_BITS / 32]
   const uint32_t *rt_keys;                                // per-block rare tables: feature << 5 | largest tf (31: tfmax[])
   const unsigned long long *rt_masks;                     // ... chunks of the block holding the feature
@@ -144,6 +147,7 @@ struct BoundParams {
   const uint2 *q2list;                                    // [n_tiles][Q2CAP][TILE_Q]
   const uint32_t *ubt;                                    // [n_blocks][NF2][2][B_BN / 32]
   const float *q_nq, *q_dotS, *q_dotX, *q_corrS;          // [n_q] (sorted query order)
+  const float *q_rscale;                                  // [n_q] 1 / s_q, a power of two: the unit of R's fixed point
   const int *gthr;                                        // [n_q] float bits: lower bound of the k-th score
   int pass;                                               // 0: seeds, 1: candidate lists
   int n_bsplits, jaccard;
@@ -168,9 +172,9 @@ struct __align__(1024) BoundSmem {
   unsigned char b[B_STAGES][B_B_SLICE_BYTES];    // chunk slices in flight
   uint32_t ubt[2][NF2][2][B_BN / 32];            // second-class bitmaps (tf >= 1, tf >= 2) of the current / next block of chunks
   uint32_t rbm[2][RB_BITS / 32];                 // rare-feature presence bitmap of the current / next block
-  float R[B_BN][TILE_Q];                         // rare part of the dot bound, [chunk][query]
+  uint32_t R[B_BN][TILE_Q];                      // frequent + rare part of the dot bound in units of 1 / s_q, [chunk][query]
   uint2 q2[Q2CAP][TILE_Q];                       // the queries' second-class lists (bit row | (tfmax - 1) << 16, weight)
-  uint2 q3[Q3CAP][TILE_Q];                       // the queries' rare lists (feature id, weight)
+  uint2 q3[Q3CAP][TILE_Q];                       // the queries' rare lists (feature id, fixed-point weight)
   float minB[2][B_BN];
   uint64_t full_bar[B_STAGES], a_bar, blk_bar[2];
   unsigned int lcount[4];
@@ -211,8 +215,8 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
     const uint4 *src3 = (const uint4 *)(P.q3list + (size_t)tile * Q3CAP * TILE_Q);
     uint4 *dst3 = (uint4 *)&S.q3[0][0];
     for (int i = threadIdx.x; i < Q3CAP * TILE_Q / 2; i += B_THREADS) dst3[i] = src3[i];
-    float4 *r4 = (float4 *)&S.R[0][0];
-    for (int i = threadIdx.x; i < B_BN * TILE_Q / 4; i += B_THREADS) r4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    uint4 *r4 = (uint4 *)&S.R[0][0];
+    for (int i = threadIdx.x; i < B_BN * TILE_Q / 4; i += B_THREADS) r4[i] = make_uint4(0u, 0u, 0u, 0u);
     for (int i = threadIdx.x; i < 4 * P.max_pages; i += B_THREADS) S.pages[i] = -1;
     if (threadIdx.x < 4) S.lcount[threadIdx.x] = 0;
   }
@@ -242,6 +246,15 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
       if (producer && g + B_STAGES < n_slices) load_slice(g + B_STAGES);
     };
     float acc[2][32] = {};
+    // s_q of the four query rows this thread holds (1 / a power of two: exact); padding rows have zero weights
+    float sq[2][2];
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+      for (int r = 0; r < 2; r++) {
+        const int64_t sl = (int64_t)tile * TILE_Q + h * 64 + wq * 16 + (lane >> 2) + 8 * r;
+        sq[h][r] = sl < P.n_q ? __frcp_rn(P.q_rscale[sl]) : 1.f;
+      }
     mbar_wait_idle(&S.a_bar, 0);
     int stage = 0;
     uint32_t phase = 0;
@@ -283,7 +296,8 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
 #pragma unroll
         for (int i = 0; i < 32; i++) {
           const int c = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-          atomicAdd(&S.R[c][q0 + 8 * ((i >> 1) & 1)], acc[h][i]);  // the workers' rare join adds to R concurrently
+          // rounded up into R's fixed point; the workers' rare join adds to R concurrently
+          atomicAdd(&S.R[c][q0 + 8 * ((i >> 1) & 1)], __float2uint_ru(acc[h][i] * sq[h][(i >> 1) & 1]));
         }
       }
       asm volatile("bar.arrive %0, %1;" ::"n"(B_BAR_RFULL), "n"(B_THREADS) : "memory");
@@ -300,6 +314,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
     const bool q_ok = nq > 0.f;
     const float base = q_ok ? P.q_dotS[slot] + P.q_dotX[slot] : 0.f;
     const float corrS = q_ok ? P.q_corrS[slot] : 0.f;
+    const float rs = q_in ? P.q_rscale[slot] : 0.f;  // a power of two: R x rs is exact
     const int list = (tile * 4 + qtr) * P.n_bsplits + bsplit;
     int *my_pages = S.pages + qtr * P.max_pages;
     float sm[B_SEEDS];
@@ -324,35 +339,42 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
       mbar_wait(&S.blk_bar[as], aphase);
       // ---- rare join, inverted: thread (query, quarter of its rare list) tests each feature in the block's presence
       //      bitmap; on a hit it probes the block's table (L2) and adds weight x tf to R[chunk][query] for every chunk
-      //      of the mask.  Rows are text-sorted, so one feature can sit in most chunks of a block: R is dense. ----
+      //      of the mask.  Rows are text-sorted, so one feature can sit in most chunks of a block: R is dense.
+      //      Three phases, each issuing all of its loads before it consumes one (bitmap bits, first-slot keys of the
+      //      hits, masks of the found keys): one or two L2 latencies per thread and block rather than two per hit. ----
       {
+        constexpr int NR = Q3CAP / 4;  // list entries of a thread
         const int jq = threadIdx.x & (TILE_Q - 1), part = threadIdx.x >> 7;  // 512 worker threads = 128 queries x 4
         const uint32_t *bm = S.rbm[as];
         const uint32_t tsize = P.rt_size[bk], toff = P.rt_off[bk];
-#pragma unroll 1
-        for (int i = part; i < Q3CAP; i += 4) {
-          const uint2 f3 = S.q3[i][jq];
-          if (f3.x >= FID_NONE) break;  // the lists are filled from the front (padding queries: all ones)
-          const uint32_t bb = rb_bit(f3.x);
-          if (!((bm[bb >> 5] >> (bb & 31u)) & 1u)) continue;
-          uint32_t h = rt_slot(f3.x, tsize);
-          for (;;) {
-            const uint32_t key = __ldg(P.rt_keys + toff + h);
-            if (key == KEY_EMPTY) break;
-            if ((key >> 5) == f3.x) {
-              uint32_t tf = key & 31u;
-              if (tf == TF_OVF) tf = __ldg(P.tfmax + f3.x);
-              const float x = __fmul_ru(__uint_as_float(f3.y), (float)tf);
-              unsigned long long cm = __ldg(P.rt_masks + toff + h);
-              while (cm) {
-                const int j = __ffsll((long long)cm) - 1;
-                cm &= cm - 1;
-                atomicAdd(&S.R[j][jq], x);
-              }
-              break;
-            }
-            h = h + 1 == tsize ? 0 : h + 1;
+        uint32_t fid[NR], h[NR], key[NR];
+#pragma unroll
+        for (int k = 0; k < NR; k++) {
+          fid[k] = S.q3[part + 4 * k][jq].x;  // FID_NONE past the end of the list (padding queries: all ones)
+          const uint32_t bb = rb_bit(fid[k]);
+          const bool hit = fid[k] < FID_NONE && ((bm[bb >> 5] >> (bb & 31u)) & 1u);
+          h[k] = rt_slot(fid[k], tsize);
+          key[k] = hit ? __ldg(P.rt_keys + toff + h[k]) : KEY_EMPTY;
+        }
+#pragma unroll
+        for (int k = 0; k < NR; k++)  // first slot taken by another feature: continue the linear probe
+          while (key[k] != KEY_EMPTY && (key[k] >> 5) != fid[k]) {
+            h[k] = h[k] + 1 == tsize ? 0 : h[k] + 1;
+            key[k] = __ldg(P.rt_keys + toff + h[k]);
           }
+        unsigned long long cm[NR];
+        uint32_t tf[NR];
+#pragma unroll
+        for (int k = 0; k < NR; k++) {
+          const bool found = key[k] != KEY_EMPTY;
+          cm[k] = found ? __ldg(P.rt_masks + toff + h[k]) : 0ull;
+          tf[k] = key[k] & 31u;
+          if (found && tf[k] == TF_OVF) tf[k] = __ldg(P.tfmax + fid[k]);
+        }
+#pragma unroll
+        for (int k = 0; k < NR; k++) {
+          const uint32_t x = S.q3[part + 4 * k][jq].y * tf[k];  // fixed point, <= 2^30 + tf (prep_queries_kernel)
+          for (unsigned long long m = cm[k]; m; m &= m - 1) atomicAdd(&S.R[__ffsll((long long)m) - 1][jq], x);
         }
       }
       if (threadIdx.x < B_BN) S.minB[as][threadIdx.x] = P.chunk_minB[c0 + threadIdx.x];
@@ -368,9 +390,9 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
       //      -> bound -> seed / candidate ----
       float x[B_COLS];
       {
-        float *Rcol = &S.R[cs * B_COLS][qi];
+        uint32_t *Rcol = &S.R[cs * B_COLS][qi];
 #pragma unroll
-        for (int j = 0; j < B_COLS; j++) { x[j] = Rcol[j * TILE_Q]; Rcol[j * TILE_Q] = 0.f; }
+        for (int j = 0; j < B_COLS; j++) { x[j] = __uint2float_ru(Rcol[j * TILE_Q]) * rs; Rcol[j * TILE_Q] = 0u; }
       }
       const uint32_t bsh = (uint32_t)((cs * B_COLS) & 31), bword = (uint32_t)((cs * B_COLS) >> 5);
       constexpr uint32_t CMASK = B_COLS == 32 ? 0xFFFFFFFFu : ((1u << B_COLS) - 1u);

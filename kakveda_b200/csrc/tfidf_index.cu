@@ -108,7 +108,7 @@ struct kv_index {
   DevBuf<double> d_q_oov;
   DevBuf<int> d_qperm;
   DevBuf<uint8_t> d_flags;
-  DevBuf<float> d_qconst;     // 7 * n_q: nq, dotU, corrU, dotS, corrS, dotX, -inf
+  DevBuf<float> d_qconst;     // 7 * n_q: nq, dotU, corrU, dotS, corrS, dotX, 1 / s_q (fixed-point unit of the bound kernel's R)
   DevBuf<unsigned char> d_qtab;
   DevBuf<uint2> d_q2list, d_q3list;
   DevBuf<__half> d_Wf;
@@ -908,7 +908,7 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   if (const char *e = getenv("KAKVEDA_B200_Q2CAP")) P.q2cap = std::max(0, std::min(Q2CAP, atoi(e)));
   P.fslot = ix->d_fslot.p; P.fslot2 = ix->d_fslot2.p; P.q2list = ix->d_q2list.p; P.jaccard = ix->jaccard; P.corpus_fit = ix->corpus_fit;
   P.q_nq = ix->d_qconst.p; P.q_dotU = P.q_nq + n_q; P.q_corrU = P.q_nq + 2 * n_q; P.q_dotS = P.q_nq + 3 * n_q;
-  P.q_corrS = P.q_nq + 4 * n_q; P.q_dotX = P.q_nq + 5 * n_q;
+  P.q_corrS = P.q_nq + 4 * n_q; P.q_dotX = P.q_nq + 5 * n_q; P.q_rscale = P.q_nq + 6 * n_q;
   P.qtab = ix->d_qtab.p; P.Wf = ix->d_Wf.p; P.q3list = ix->d_q3list.p;
   prep_queries_kernel<<<(unsigned)((n_q + 127) / 128), 128, 0, s>>>(P);
   KV_CUDA(cudaGetLastError());
@@ -1058,6 +1058,7 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
       BP.rbloom = ix->d_rbloom.p; BP.rt_keys = ix->d_rt_keys.p; BP.rt_masks = ix->d_rt_masks.p; BP.rt_off = ix->d_rt_off.p;
       BP.rt_size = ix->d_rt_size.p; BP.tfmax = ix->d_tfmax.p;
       BP.q_nq = qc; BP.q_dotS = qc + 3 * n_q; BP.q_corrS = qc + 4 * n_q; BP.q_dotX = qc + 5 * n_q;
+      BP.q_rscale = qc + 6 * n_q;
       BP.gthr = ix->d_gthr.p; BP.n_bsplits = (int)n_bsplits; BP.jaccard = ix->jaccard;
       BP.seeds = ix->d_seeds.p;
       BP.list_count = ix->d_list_count.p + n_groups; BP.list_pages = ix->d_list_pages.p; BP.max_pages = max_pages;

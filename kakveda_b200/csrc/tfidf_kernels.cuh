@@ -322,9 +322,10 @@ struct PrepParams {
   int jaccard, corpus_fit;
   int q2cap;                // second-class features a query lists itself (<= Q2CAP)
   float *q_nq, *q_dotU, *q_corrU, *q_dotS, *q_corrS, *q_dotX;  // [n_q] by sorted slot
+  float *q_rscale;          // [n_q] 1 / s_q: fixed-point unit of the bound kernel's accumulator R (see below)
   unsigned char *qtab;      // [n_q][QTAB_BYTES]
   __half *Wf;               // [n_q_pad][NF], zeroed by the caller
-  uint2 *q3list;            // [n_tiles][Q3CAP][TILE_Q] (rare feature id, weight tf_q a(t) rounded up as float bits)
+  uint2 *q3list;            // [n_tiles][Q3CAP][TILE_Q] (rare feature id, weight ceil(tf_q a(t) s_q) as an integer)
   uint2 *q2list;            // [n_tiles][Q2CAP][TILE_Q] (bit row | (tfmax(t) - 1) << 16, weight tf_q a(t) as float bits)
 };
 
@@ -346,6 +347,7 @@ __global__ void prep_queries_kernel(PrepParams P) {
   for (int j = 0; j < Q3CAP; j++) q3[(size_t)j * TILE_Q] = make_uint2(FID_NONE, 0u);
   int c3 = 0;
   float dotX = 0.f;
+  double xmax = 0.0;  // upper bound of what the bound kernel sums into R for this query: frequent and listed rare terms
   for (int64_t p = P.q_indptr[q]; p < P.q_indptr[q + 1]; p++) {
     const uint32_t t = P.q_ids[p];
     const double f = (double)P.q_tf[p];
@@ -370,19 +372,38 @@ __global__ void prep_queries_kernel(PrepParams P) {
       feats[cnt++] = qf;
       const int fs = P.fslot[t];
       if (fs >= 0) {
-        P.Wf[(size_t)i * NF + fs] = __float2half_ru(__double2float_ru(f * a));
+        const __half wf = __float2half_ru(__double2float_ru(f * a));
+        P.Wf[(size_t)i * NF + fs] = wf;
+        xmax += (double)__half2float(wf) * tm;
       } else if (P.fslot2[t] != 0xFFFFu && c2 < P.q2cap) {
         const uint32_t tm1 = min(P.tfmax[t] - 1u, 65535u);  // weight of the 'tf >= 2' plane: (largest tf - 1) more times
         q2[(size_t)c2 * TILE_Q] = make_uint2((uint32_t)P.fslot2[t] | (tm1 << 16), __float_as_uint(__double2float_ru(f * a * (1.0 + 1e-6))));
         c2++;
       } else if (P.fslot2[t] == 0xFFFFu && c3 < Q3CAP) {  // rare: looked up per block of chunks by the bound kernel
-        q3[(size_t)c3 * TILE_Q] = make_uint2(t, __float_as_uint(__double2float_ru(f * a * (1.0 + 1e-6))));
+        const float w3 = __double2float_ru(f * a * (1.0 + 1e-6));
+        q3[(size_t)c3 * TILE_Q] = make_uint2(t, __float_as_uint(w3));  // scaled to an integer below, once s_q is known
+        xmax += (double)w3 * tm;
         c3++;
       } else {  // no list slot left: assumed present in every chunk with its largest tf (a valid, loose bound)
         dotX = __fadd_ru(dotX, __double2float_ru(f * a * tm * (1.0 + 1e-6)));
       }
     }
   }
+  // Fixed-point scale of R (the bound kernel's frequent + rare part, summed with integer shared atomics): s_q = 2^(30 - e)
+  // with xmax < 2^e, so xmax s_q <= 2^30, and a power of two, so scaling is exact.  No wrap: R[chunk][query] is one
+  // MMA term ceil(acc s_q) plus at most Q3CAP rare terms w3 tf with w3 = ceil(weight s_q) <= weight s_q + 1.  The
+  // accumulator acc is the fp32 tensor-core sum of fp16 weights times the chunk's largest tf (fp16, within 2^-11 of
+  // it), and every tf is at most tfmax(t) <= 65535, so R <= 1.001 xmax s_q + 1 + Q3CAP 65535 < 2^31.  A wrapped sum
+  // would LOWER a bound and pruning would drop rows.  xmax < 2^31 for a regular query (classify_queries) and 0 for the
+  // others, so s_q and 1 / s_q are normal floats.
+  int e = 0;
+  frexp(xmax, &e);
+  const double s_q = ldexp(1.0, 30 - e);
+  for (int j = 0; j < c3; j++) {
+    uint2 &r = q3[(size_t)j * TILE_Q];
+    r.y = (uint32_t)ceil((double)__uint_as_float(r.y) * s_q);  // <= xmax s_q: fits
+  }
+  P.q_rscale[i] = (float)ldexp(1.0, e - 30);
   P.q_nq[i] = regular ? (float)nq : 0.f;  // nq == 0 switches the query off in the kernels
   P.q_dotU[i] = (float)dotU;
   P.q_corrU[i] = (float)corrU;
