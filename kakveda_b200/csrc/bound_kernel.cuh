@@ -130,6 +130,65 @@ __device__ __forceinline__ float rsqrt_approx(float x) {
   return y;
 }
 
+// The candidate lists of a batch: list l = group * n_bsplits + bsplit holds records {chunk, mask of the group's queries}
+// in pages of PAGE_RECS records taken from one pool.
+struct CandLists {
+  uint32_t *count;          // [n_lists]
+  uint32_t *pages;          // [n_lists][max_pages]
+  int max_pages;
+  uint2 *pool;
+  unsigned int *pool_next;  // pages handed out
+  unsigned int pool_pages;  // capacity
+  int *overflow;            // set when the pool ran out (the batch is rerun with a larger pool)
+};
+
+// Appends the {chunk, mask} of every lane with a non-empty mask to list `list`, warp-aggregated: lane 0 takes the
+// warp's positions from the list's shared counter and allocates the pages its range crosses into, publishing each in the
+// list's shared page table (warps sharing a list wait there for a page another warp is allocating).  All 32 lanes call.
+__device__ __forceinline__ void list_append(const CandLists &L, int list, unsigned int *count, int *pages, uint32_t chunk,
+                                            uint32_t mask, unsigned int &n_pairs, unsigned int &n_recs) {
+  const uint32_t am = __ballot_sync(FULL, mask != 0);
+  if (!am) return;
+  const int n = __popc(am);
+  unsigned int bpos = 0;
+  if ((threadIdx.x & 31) == 0) {
+    bpos = atomicAdd(count, (unsigned int)n);
+    for (unsigned int pg = (bpos + PAGE_RECS - 1) / PAGE_RECS; pg * PAGE_RECS < bpos + n; pg++) {
+      unsigned int np = atomicAdd(L.pool_next, 1u);
+      if (np >= L.pool_pages) { *L.overflow = 1; np = 0; }
+      L.pages[(size_t)list * L.max_pages + pg] = np;
+      __threadfence_block();
+      *(volatile int *)&pages[pg] = (int)np;
+    }
+  }
+  bpos = __shfl_sync(FULL, bpos, 0);
+  if (mask) {
+    const unsigned int pos = bpos + (unsigned int)__popc(am & lanemask_lt());
+    const unsigned int pg = pos / PAGE_RECS;
+    int page;
+    while ((page = *(volatile int *)&pages[pg]) < 0) {}
+    uint2 rec;
+    rec.x = chunk;
+    rec.y = mask;
+    L.pool[(size_t)page * PAGE_RECS + (pos % PAGE_RECS)] = rec;
+    n_pairs += (unsigned int)__popc(mask);
+    n_recs++;
+  }
+}
+
+// adds a warp's appended pairs and records to stats[2] / stats[3]
+__device__ __forceinline__ void flush_list_stats(unsigned long long *stats, unsigned int n_pairs, unsigned int n_recs) {
+  if (!stats) return;
+  for (int o = 16; o; o >>= 1) {
+    n_pairs += __shfl_xor_sync(FULL, n_pairs, o);
+    n_recs += __shfl_xor_sync(FULL, n_recs, o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(&stats[2], (unsigned long long)n_pairs);
+    atomicAdd(&stats[3], (unsigned long long)n_recs);
+  }
+}
+
 struct BoundParams {
   const uint32_t *blk;
   const BlockInfo *binfo;
@@ -150,16 +209,9 @@ struct BoundParams {
   const float *q_rscale;                                  // [n_q] 1 / s_q, a power of two: the unit of R's fixed point
   const int *gthr;                                        // [n_q] float bits: lower bound of the k-th score
   int pass;                                               // 0: seeds, 1: candidate lists
-  int n_bsplits, jaccard;
+  int n_bsplits;
   int *seeds;                                             // pass 0: [n_q][n_bsplits][B_SEEDS_PER_QUERY] chunk ids, -1 = none
-  // pass 1: list l = group * n_bsplits + bsplit
-  uint32_t *list_count;   // [n_lists]
-  uint32_t *list_pages;   // [n_lists][max_pages]
-  int max_pages;
-  uint2 *pool;
-  unsigned int *pool_next;  // pages handed out
-  unsigned int pool_pages;  // capacity
-  int *overflow;            // set when the pool ran out (the batch is rerun with a larger pool)
+  CandLists lists;                                        // pass 1 (max_pages also sizes the shared page tables)
   unsigned long long *stats;  // [2] surviving (query, chunk) pairs, [3] candidate records
   unsigned char *ubq;         // pass 0, optional: every bound as an 8-bit code (rounded up), [n_q][ubq_stride]
   int64_t ubq_stride;
@@ -183,15 +235,14 @@ struct __align__(1024) BoundSmem {
 
 static inline size_t bound_smem_bytes(int max_pages) { return sizeof(BoundSmem) + (size_t)4 * max_pages * sizeof(int) + 1024; }
 
-// FAST = the configuration of the headline path fixed at compile time (pass 0 with bound codes, TF-IDF cosine, no test
-// hook): the epilogue then holds no uniform branches, parameter reloads or dead variants.  FAST = false is the same code
-// with those four switches read from the parameters.
+// FAST = the configuration of the headline path fixed at compile time (pass 0 with bound codes, no test hook): the
+// epilogue then holds no uniform branches, parameter reloads or dead variants.  FAST = false is the same code with
+// those three switches read from the parameters.
 template <bool FAST>
 __global__ void __launch_bounds__(B_THREADS, 1)
 tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_u, BoundParams P) {
   extern __shared__ unsigned char smem_raw[];
   const int pass = FAST ? 0 : P.pass;
-  const bool jacc = FAST ? false : (P.jaccard != 0);
   const bool has_codes = FAST ? true : (P.ubq != nullptr);
   // 1024-byte alignment by an OFFSET into the shared array (not by rounding a generic pointer): the compiler keeps
   // the shared address space, so every access below is LDS/STS/ATOMS instead of a generic load / store / atomic
@@ -217,7 +268,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
     for (int i = threadIdx.x; i < Q3CAP * TILE_Q / 2; i += B_THREADS) dst3[i] = src3[i];
     uint4 *r4 = (uint4 *)&S.R[0][0];
     for (int i = threadIdx.x; i < B_BN * TILE_Q / 4; i += B_THREADS) r4[i] = make_uint4(0u, 0u, 0u, 0u);
-    for (int i = threadIdx.x; i < 4 * P.max_pages; i += B_THREADS) S.pages[i] = -1;
+    for (int i = threadIdx.x; i < 4 * P.lists.max_pages; i += B_THREADS) S.pages[i] = -1;
     if (threadIdx.x < 4) S.lcount[threadIdx.x] = 0;
   }
   __syncthreads();
@@ -316,7 +367,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
     const float corrS = q_ok ? P.q_corrS[slot] : 0.f;
     const float rs = q_in ? P.q_rscale[slot] : 0.f;  // a power of two: R x rs is exact
     const int list = (tile * 4 + qtr) * P.n_bsplits + bsplit;
-    int *my_pages = S.pages + qtr * P.max_pages;
+    int *my_pages = S.pages + qtr * P.lists.max_pages;
     float sm[B_SEEDS];
     int sc[B_SEEDS];
 #pragma unroll
@@ -382,7 +433,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
       float tq = 0.f;
       if (pass == 1 && q_ok) {
         const float th = __int_as_float(__ldcg(&P.gthr[slot]));
-        if (th > 0.f) tq = jacc ? th / PRUNE_SLACK : th * th * nq / (PRUNE_SLACK * PRUNE_SLACK);
+        if (th > 0.f) tq = th * th * nq / (PRUNE_SLACK * PRUNE_SLACK);
       }
       // R complete: the workers' rare join and the MMA warpgroup's frequent part of this block
       asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_RFULL), "n"(B_THREADS) : "memory");
@@ -429,15 +480,14 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
         const float xs = base + x[j];
         const bool c_ok = j < nv;
         if (dbg && q_in && c_ok) P.dbg_xs[(size_t)slot * P.dbg_stride + cbase + j] = xs;
-        const float den = jacc ? (nq + mb[j] - xs) : (mb[j] + corrS);
+        const float den = mb[j] + corrS;
         if (pass == 1) {
-          const float lhs = jacc ? xs : xs * xs;
-          const bool sv = q_ok && c_ok && (tq <= 0.f || den <= 0.f || lhs >= tq * den);
+          const bool sv = q_ok && c_ok && (tq <= 0.f || den <= 0.f || xs * xs >= tq * den);
           const uint32_t m = __ballot_sync(FULL, sv);
           if (lane == j) mymask = m;
         } else if (q_ok && c_ok) {
           // the bound itself (slack included): seeds are ranked by it, and it is stored as a code that only errs upwards
-          float metric = den > 0.f ? (jacc ? __fdividef(xs, den) : xs * rsqrt_approx(nq * den)) * (PRUNE_SLACK * 1.00001f) : INFINITY;
+          float metric = den > 0.f ? xs * rsqrt_approx(nq * den) * (PRUNE_SLACK * 1.00001f) : INFINITY;
           if (has_codes) codes[j >> 2] |= (uint32_t)fminf(255.f, ceilf(metric * UBQ_SCALE)) << ((j & 3) * 8);
           if (metric > sm[B_SEEDS - 1]) {
             int cc = (int)(cbase + j);
@@ -452,38 +502,8 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
       }
       if (pass == 0 && has_codes && q_in)
         *reinterpret_cast<uint4 *>(P.ubq + (size_t)slot * P.ubq_stride + cbase) = make_uint4(codes[0], codes[1], codes[2], codes[3]);
-      if (pass == 1) {
-        // lanes holding a non-empty mask append {chunk, mask} to the group's list (warp-aggregated; four warps share
-        // a list; the warp whose range crosses into a new page allocates it)
-        const uint32_t am = __ballot_sync(FULL, mymask != 0);
-        if (am) {
-          const int n = __popc(am);
-          unsigned int bpos = 0;
-          if (lane == 0) {
-            bpos = atomicAdd(&S.lcount[qtr], (unsigned int)n);
-            for (unsigned int pg = (bpos + PAGE_RECS - 1) / PAGE_RECS; pg * PAGE_RECS < bpos + n; pg++) {
-              unsigned int np = atomicAdd(P.pool_next, 1u);
-              if (np >= P.pool_pages) { *P.overflow = 1; np = 0; }
-              P.list_pages[(size_t)list * P.max_pages + pg] = np;
-              __threadfence_block();
-              *(volatile int *)&my_pages[pg] = (int)np;
-            }
-          }
-          bpos = __shfl_sync(FULL, bpos, 0);
-          if (mymask) {
-            const unsigned int pos = bpos + (unsigned int)__popc(am & lanemask_lt());
-            const unsigned int pg = pos / PAGE_RECS;
-            int page;
-            while ((page = *(volatile int *)&my_pages[pg]) < 0) {}
-            uint2 rec;
-            rec.x = (uint32_t)(cbase + lane);
-            rec.y = mymask;
-            P.pool[(size_t)page * PAGE_RECS + (pos % PAGE_RECS)] = rec;
-            n_pairs += (unsigned int)__popc(mymask);
-            n_recs++;
-          }
-        }
-      }
+      // four warps (one per chunk-column quarter) share the group's list
+      if (pass == 1) list_append(P.lists, list, &S.lcount[qtr], my_pages, (uint32_t)(cbase + lane), mymask, n_pairs, n_recs);
       // R is clean again (the MMA warpgroup may add the next block) and every reader of this block's side data is done
       asm volatile("bar.arrive %0, %1;" ::"n"(B_BAR_RCLEAN), "n"(B_THREADS) : "memory");
       asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_WORKERS), "n"(B_WORKERS * 32) : "memory");
@@ -495,17 +515,8 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
         for (int i = 0; i < B_SEEDS; i++) o[i] = sc[i];
       }
     } else {
-      if (cs == 0 && lane == 0) P.list_count[list] = S.lcount[qtr];
-      if (P.stats) {
-        for (int o = 16; o; o >>= 1) {
-          n_pairs += __shfl_xor_sync(FULL, n_pairs, o);
-          n_recs += __shfl_xor_sync(FULL, n_recs, o);
-        }
-        if (lane == 0) {
-          atomicAdd(&P.stats[2], (unsigned long long)n_pairs);
-          atomicAdd(&P.stats[3], (unsigned long long)n_recs);
-        }
-      }
+      if (cs == 0 && lane == 0) P.lists.count[list] = S.lcount[qtr];
+      flush_list_stats(P.stats, n_pairs, n_recs);
     }
   }
 }
@@ -514,7 +525,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
 // K1b-B2: candidate lists from the stored 8-bit bound codes (second pass without recomputing the bounds).  One CTA =
 // one scan group (32 queries = the lanes) x one chunk range; a warp reads, per query, 32 codes (one 32-byte sector) and
 // compares them with the query's threshold code; ballots give the group's query mask per chunk; non-empty masks are
-// appended to the group's paged candidate list exactly as K1b-B's pass 1 does.  HBM-bound: n_q x chunks bytes read once.
+// appended to the group's paged candidate list by the same list_append as K1b-B's pass 1.  HBM-bound: n_q x chunks bytes read once.
 // ----------------------------------------------------------------------------------------
 struct SelectParams {
   const unsigned char *ubq;
@@ -522,13 +533,7 @@ struct SelectParams {
   const float *q_nq;
   const int *gthr;
   int n_bsplits;
-  uint32_t *list_count;
-  uint32_t *list_pages;
-  int max_pages;
-  uint2 *pool;
-  unsigned int *pool_next;
-  unsigned int pool_pages;
-  int *overflow;
+  CandLists lists;
   unsigned long long *stats;
 };
 
@@ -540,7 +545,7 @@ __global__ void __launch_bounds__(SEL_WARPS * 32) tfidf_select_kernel(SelectPara
   const int group = blockIdx.x, bsplit = blockIdx.y;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int list = group * P.n_bsplits + bsplit;
-  for (int i = threadIdx.x; i < P.max_pages; i += blockDim.x) s_pages[i] = -1;
+  for (int i = threadIdx.x; i < P.lists.max_pages; i += blockDim.x) s_pages[i] = -1;
   if (threadIdx.x == 0) s_count = 0;
   __syncthreads();
   const int64_t slot = (int64_t)group * GROUP_Q + lane;
@@ -565,47 +570,11 @@ __global__ void __launch_bounds__(SEL_WARPS * 32) tfidf_select_kernel(SelectPara
       const uint32_t m = __ballot_sync(FULL, q_ok && code >= tcode && c + j < c_hi);
       if (lane == j) mymask = m;
     }
-    const uint32_t am = __ballot_sync(FULL, mymask != 0);
-    if (am) {
-      const int n = __popc(am);
-      unsigned int bpos = 0;
-      if (lane == 0) {
-        bpos = atomicAdd(&s_count, (unsigned int)n);
-        for (unsigned int pg = (bpos + PAGE_RECS - 1) / PAGE_RECS; pg * PAGE_RECS < bpos + n; pg++) {
-          unsigned int np = atomicAdd(P.pool_next, 1u);
-          if (np >= P.pool_pages) { *P.overflow = 1; np = 0; }
-          P.list_pages[(size_t)list * P.max_pages + pg] = np;
-          __threadfence_block();
-          *(volatile int *)&s_pages[pg] = (int)np;
-        }
-      }
-      bpos = __shfl_sync(FULL, bpos, 0);
-      if (mymask) {
-        const unsigned int pos = bpos + (unsigned int)__popc(am & lanemask_lt());
-        const unsigned int pg = pos / PAGE_RECS;
-        int page;
-        while ((page = *(volatile int *)&s_pages[pg]) < 0) {}
-        uint2 rec;
-        rec.x = (uint32_t)(c + lane);
-        rec.y = mymask;
-        P.pool[(size_t)page * PAGE_RECS + (pos % PAGE_RECS)] = rec;
-        n_pairs += (unsigned int)__popc(mymask);
-        n_recs++;
-      }
-    }
+    list_append(P.lists, list, &s_count, s_pages, (uint32_t)(c + lane), mymask, n_pairs, n_recs);
   }
   __syncthreads();
-  if (threadIdx.x == 0) P.list_count[list] = s_count;
-  if (P.stats) {
-    for (int o = 16; o; o >>= 1) {
-      n_pairs += __shfl_xor_sync(FULL, n_pairs, o);
-      n_recs += __shfl_xor_sync(FULL, n_recs, o);
-    }
-    if (lane == 0) {
-      atomicAdd(&P.stats[2], (unsigned long long)n_pairs);
-      atomicAdd(&P.stats[3], (unsigned long long)n_recs);
-    }
-  }
+  if (threadIdx.x == 0) P.lists.count[list] = s_count;
+  flush_list_stats(P.stats, n_pairs, n_recs);
 }
 
 typedef CUresult (*PFN_encodeTiled_kv)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,

@@ -83,7 +83,7 @@ struct kv_index {
   DevBuf<unsigned long long> d_ovf_keys;
   DevBuf<uint32_t> d_ovf_vals;
   int n_ovf = 0;
-  int64_t rare_table_bytes = 0;
+  int64_t n_rt_slots = 0;  // slots of all blocks' rare tables
   int64_t blk_words = 0, n_chunks = 0, n_chunks_pad = 0, n_entries = 0, n_rare_entries = 0;
   std::vector<uint32_t> h_df, h_tfmax;
   std::vector<short> h_fslot;
@@ -227,6 +227,72 @@ void sort_rows_by_text(const std::vector<int64_t> &indptr, const std::vector<uin
       }
     });
   }
+}
+
+// ---- the scan layout in host memory ----
+// The arrays kv_index_finalize builds on the host cores (row order, column blocks, dense / bitmap / rare-table side
+// structures) with the counts that size them.  A layout file (kv_index_layout_save) is this header followed by univ and
+// then the arrays in each_array's order.
+struct LayoutHeader {
+  uint64_t magic, checksum;
+  int64_t n_rows, nnz, V, n_chunks, n_chunks_pad, blk_words, n_entries, n_rare_entries, n_ovf, n_rt_slots, n_blocks, univ_len;
+  int32_t jaccard, corpus_fit, threads, reserved;
+};
+
+struct ScanLayout {
+  LayoutHeader H{};
+  std::vector<uint8_t> univ;  // the universal features the layout folds into per-query constants (host only)
+  std::vector<short> fslot;
+  std::vector<unsigned short> fslot2;
+  std::vector<int> perm;
+  std::vector<BlockInfo> binfo;
+  std::vector<uint32_t> blk;
+  std::vector<__half> uf;
+  std::vector<uint32_t> ubt, rbloom, rt_off, rt_size, rt_keys;
+  std::vector<unsigned long long> rt_masks, ovf_keys;
+  std::vector<uint32_t> ovf_vals;
+};
+
+// f(host array, device buffer, entries) for every device array of the layout, in file order, until f returns false
+template <class SL, class F>
+bool each_array(SL &L, kv_index *ix, F &&f) {
+  const LayoutHeader &H = L.H;
+  const size_t V = (size_t)H.V, pad = (size_t)H.n_chunks_pad, nb = (size_t)H.n_blocks, slots = (size_t)H.n_rt_slots,
+               n_ovf = (size_t)H.n_ovf;
+  return f(L.fslot, ix->d_fslot, V) && f(L.fslot2, ix->d_fslot2, V) && f(L.perm, ix->d_perm, (size_t)H.n_rows) &&
+         f(L.binfo, ix->d_binfo, pad) && f(L.blk, ix->d_blk, (size_t)H.blk_words) && f(L.uf, ix->d_Uf, pad * NF) &&
+         f(L.ubt, ix->d_ubt, nb * NF2 * 4) && f(L.rbloom, ix->d_rbloom, nb * (RB_BITS / 32)) && f(L.rt_off, ix->d_rt_off, nb) &&
+         f(L.rt_size, ix->d_rt_size, nb) && f(L.rt_keys, ix->d_rt_keys, slots) && f(L.rt_masks, ix->d_rt_masks, slots) &&
+         f(L.ovf_keys, ix->d_ovf_keys, n_ovf) && f(L.ovf_vals, ix->d_ovf_vals, n_ovf);
+}
+
+// Makes L the scan layout on the device: sizes the buffers, copies the arrays, builds invperm and the tensor map of the
+// dense matrix, and takes L's counts.  Row norms and chunk minima are the caller's (they depend on the statistics).
+int upload_layout(kv_index *ix, const ScanLayout &L) {
+  cudaStream_t s = ix->stream;
+  const LayoutHeader &H = L.H;
+  const int64_t nz = std::max<int64_t>(H.n_rows, 1);
+  KV_CUDA(ix->d_invperm.ensure(nz)); KV_CUDA(ix->d_B64.ensure(nz)); KV_CUDA(ix->d_B32.ensure(nz));
+  KV_CUDA(ix->d_cminB.ensure(H.n_chunks_pad)); KV_CUDA(ix->d_blk.ensure(H.blk_words + 64));
+  cudaError_t err = cudaSuccess;
+  each_array(L, ix, [&](const auto &h, auto &d, size_t n) {
+    err = d.ensure(std::max<int64_t>((int64_t)n, 1));
+    if (err == cudaSuccess && n) err = cudaMemcpyAsync(d.p, h.data(), n * sizeof(h[0]), cudaMemcpyHostToDevice, s);
+    return err == cudaSuccess;
+  });
+  KV_CUDA(err);
+  if (H.n_rows) {
+    invperm_kernel<<<(unsigned)((H.n_rows + 255) / 256), 256, 0, s>>>(ix->d_perm.p, H.n_rows, ix->d_invperm.p);
+    KV_CUDA(cudaGetLastError());
+  }
+  KV_CUDA(cudaStreamSynchronize(s));  // the caller's staging vectors may go out of scope
+  int rc = make_map_f16_nf(&ix->map_u, ix->d_Uf.p, H.n_chunks_pad, B_BN);
+  if (rc != KV_OK) return rc;
+  ix->h_fslot = L.fslot; ix->h_fslot2 = L.fslot2;
+  ix->n_chunks = H.n_chunks; ix->n_chunks_pad = H.n_chunks_pad; ix->blk_words = H.blk_words; ix->n_entries = H.n_entries;
+  ix->n_rare_entries = H.n_rare_entries; ix->n_ovf = (int)H.n_ovf; ix->n_rt_slots = H.n_rt_slots;
+  ix->layout_valid = H.n_rows > 0; ix->layout_rows = H.n_rows; ix->layout_univ = L.univ;
+  return KV_OK;
 }
 
 }  // namespace
@@ -528,73 +594,41 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
   }
   ix->layout_valid = false;
   // ---- on the host cores: (norm class, text) order of the rows, then the column blocks ----
-  std::vector<int> perm;
-  sort_rows_by_text(ix->h_indptr, ix->h_ids, n, hB, perm);
-  BlockLayout L;
-  build_blocks(ix->h_indptr.data(), ix->h_ids.data(), ix->h_tf.data(), perm.data(), n, V, ix->h_univ.data(),
-               ix->h_tfmax.data(), host_threads(), L);
-  ix->n_chunks = L.n_chunks;
-  ix->n_chunks_pad = L.n_chunks_pad;
-  ix->blk_words = L.total_words;
-  ix->n_entries = L.n_entries;
-  ix->n_rare_entries = L.n_rare_entries;
-  KV_CUDA(ix->d_blk.ensure(L.total_words + 64));
-  KV_CUDA(ix->d_binfo.ensure(L.n_chunks_pad));
-  KV_CUDA(ix->d_Uf.ensure(L.n_chunks_pad * NF));
-  KV_CUDA(ix->d_fslot.ensure(Vz));
-  KV_CUDA(ix->d_cminB.ensure(L.n_chunks_pad));
+  ScanLayout SL;
+  sort_rows_by_text(ix->h_indptr, ix->h_ids, n, hB, SL.perm);
+  {
+    BlockLayout L;
+    build_blocks(ix->h_indptr.data(), ix->h_ids.data(), ix->h_tf.data(), SL.perm.data(), n, V, ix->h_univ.data(),
+                 ix->h_tfmax.data(), host_threads(), L);
+    LayoutHeader &H = SL.H;
+    H.n_rows = n; H.V = Vz; H.n_chunks = L.n_chunks; H.n_chunks_pad = L.n_chunks_pad; H.n_blocks = L.n_chunks_pad / 64;
+    H.blk_words = L.total_words; H.n_entries = L.n_entries; H.n_rare_entries = L.n_rare_entries;
+    H.n_rt_slots = (int64_t)L.rt_keys.size(); H.n_ovf = (int64_t)L.ovf.size(); H.univ_len = Vz;
+    SL.univ = ix->h_univ;
+    SL.fslot = std::move(L.fslot); SL.fslot2 = std::move(L.fslot2); SL.binfo = std::move(L.binfo); SL.uf = std::move(L.Uf);
+    SL.ubt = std::move(L.Ubt); SL.rbloom = std::move(L.rbloom); SL.rt_off = std::move(L.rt_off); SL.rt_size = std::move(L.rt_size);
+    SL.rt_keys = std::move(L.rt_keys); SL.rt_masks = std::move(L.rt_masks);
+    SL.blk.reserve((size_t)L.total_words);
+    for (auto &part : L.parts) {  // the blocks of each build thread, back to back
+      SL.blk.insert(SL.blk.end(), part.begin(), part.end());
+      std::vector<uint32_t>().swap(part);
+    }
+    for (const auto &o : L.ovf) { SL.ovf_keys.push_back(o.first); SL.ovf_vals.push_back(o.second); }
+  }
+  int rc = upload_layout(ix, SL);
+  if (rc != KV_OK) return rc;
   if (n) {
-    KV_CUDA(cudaMemcpyAsync(ix->d_perm.p, perm.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
-    KV_CUDA(ix->d_invperm.ensure(n));
-    invperm_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(ix->d_perm.p, n, ix->d_invperm.p);
-    KV_CUDA(cudaGetLastError());
     rownorm_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(ix->indptr.p, ix->ids.p, ix->tf.p, ix->d_perm.p, n,
                                                                     ix->d_bb64.p, ix->d_B64.p, ix->d_B32.p);
     KV_CUDA(cudaGetLastError());
   }
-  chunk_meta_kernel<<<(unsigned)((L.n_chunks_pad + 255) / 256), 256, 0, s>>>(ix->d_B32.p, n, L.n_chunks, L.n_chunks_pad, ix->d_cminB.p);
+  chunk_meta_kernel<<<(unsigned)((ix->n_chunks_pad + 255) / 256), 256, 0, s>>>(ix->d_B32.p, n, ix->n_chunks, ix->n_chunks_pad,
+                                                                                ix->d_cminB.p);
   KV_CUDA(cudaGetLastError());
-  for (size_t t = 0; t < L.parts.size(); t++)
-    if (!L.parts[t].empty())
-      KV_CUDA(cudaMemcpyAsync(ix->d_blk.p + L.part_off[t], L.parts[t].data(), L.parts[t].size() * 4, cudaMemcpyHostToDevice, s));
-  KV_CUDA(cudaMemcpyAsync(ix->d_binfo.p, L.binfo.data(), (size_t)L.n_chunks_pad * sizeof(BlockInfo), cudaMemcpyHostToDevice, s));
-  KV_CUDA(cudaMemcpyAsync(ix->d_Uf.p, L.Uf.data(), (size_t)L.n_chunks_pad * NF * sizeof(__half), cudaMemcpyHostToDevice, s));
-  ix->h_fslot = L.fslot;
-  ix->h_fslot2 = L.fslot2;
-  KV_CUDA(cudaMemcpyAsync(ix->d_fslot.p, ix->h_fslot.data(), (size_t)Vz * sizeof(short), cudaMemcpyHostToDevice, s));
-  KV_CUDA(ix->d_fslot2.ensure(Vz));
-  KV_CUDA(cudaMemcpyAsync(ix->d_fslot2.p, ix->h_fslot2.data(), (size_t)Vz * sizeof(short), cudaMemcpyHostToDevice, s));
-  KV_CUDA(ix->d_ubt.ensure((int64_t)L.Ubt.size()));
-  KV_CUDA(cudaMemcpyAsync(ix->d_ubt.p, L.Ubt.data(), L.Ubt.size() * 4, cudaMemcpyHostToDevice, s));
-  KV_CUDA(ix->d_rbloom.ensure((int64_t)L.rbloom.size())); KV_CUDA(ix->d_rt_keys.ensure((int64_t)L.rt_keys.size()));
-  KV_CUDA(ix->d_rt_masks.ensure((int64_t)L.rt_masks.size())); KV_CUDA(ix->d_rt_off.ensure((int64_t)L.rt_off.size()));
-  KV_CUDA(ix->d_rt_size.ensure((int64_t)L.rt_size.size()));
-  KV_CUDA(cudaMemcpyAsync(ix->d_rbloom.p, L.rbloom.data(), L.rbloom.size() * 4, cudaMemcpyHostToDevice, s));
-  KV_CUDA(cudaMemcpyAsync(ix->d_rt_keys.p, L.rt_keys.data(), L.rt_keys.size() * 4, cudaMemcpyHostToDevice, s));
-  KV_CUDA(cudaMemcpyAsync(ix->d_rt_masks.p, L.rt_masks.data(), L.rt_masks.size() * 8, cudaMemcpyHostToDevice, s));
-  KV_CUDA(cudaMemcpyAsync(ix->d_rt_off.p, L.rt_off.data(), L.rt_off.size() * 4, cudaMemcpyHostToDevice, s));
-  KV_CUDA(cudaMemcpyAsync(ix->d_rt_size.p, L.rt_size.data(), L.rt_size.size() * 4, cudaMemcpyHostToDevice, s));
-  ix->rare_table_bytes = (int64_t)(L.rt_keys.size() * 12 + L.rbloom.size() * 4);
-  ix->n_ovf = (int)L.ovf.size();
-  KV_CUDA(ix->d_ovf_keys.ensure(std::max(1, ix->n_ovf))); KV_CUDA(ix->d_ovf_vals.ensure(std::max(1, ix->n_ovf)));
-  std::vector<unsigned long long> ok((size_t)ix->n_ovf);
-  std::vector<uint32_t> ov((size_t)ix->n_ovf);
-  for (int i = 0; i < ix->n_ovf; i++) { ok[(size_t)i] = L.ovf[(size_t)i].first; ov[(size_t)i] = L.ovf[(size_t)i].second; }
-  if (ix->n_ovf) {
-    KV_CUDA(cudaMemcpyAsync(ix->d_ovf_keys.p, ok.data(), (size_t)ix->n_ovf * 8, cudaMemcpyHostToDevice, s));
-    KV_CUDA(cudaMemcpyAsync(ix->d_ovf_vals.p, ov.data(), (size_t)ix->n_ovf * 4, cudaMemcpyHostToDevice, s));
-  }
-  KV_CUDA(cudaStreamSynchronize(s));  // the staging vectors go out of scope
-  {
-    int rc = make_map_f16_nf(&ix->map_u, ix->d_Uf.p, L.n_chunks_pad, B_BN);
-    if (rc != KV_OK) return rc;
-  }
+  KV_CUDA(cudaStreamSynchronize(s));
   ix->V = V;
   ix->finalized = true;
   ix->batch_valid = false;
-  ix->layout_valid = n > 0;
-  ix->layout_rows = n;
-  ix->layout_univ = ix->h_univ;
   ix->last_finalize_kind = 1;
   return KV_OK;
 }
@@ -937,22 +971,160 @@ static int prepare_batch(kv_index *ix, const int64_t *q_indptr, const uint32_t *
 // Device-only half: bounds + scans + merge (+ fallback scans for irregular queries) of the uploaded batch.
 // phase 0: the whole batch.  phase 1: up to the seed scan; the outputs receive the seed top-k (their k-th score is a
 // lower bound of the final k-th score; a row-sharded GFKB exchanges it between the GPUs).  phase 2: the rest.
+// Three device paths: pruned (bound pass 0 -> seed scan -> candidate selection -> scan of the candidates), exhaustive
+// (small indexes, KAKVEDA_B200_NO_PRUNE=1: every chunk is a candidate of every query) and Jaccard (K3).
+struct Batch {
+  int k, phase;
+  float *out_s;  // the outputs, [n_q][k] by original query
+  long long *out_r;
+  int64_t n_q, n_tiles, n_groups, n_bsplits, n_ssplits, n_ssplits_a, n_parts;
+  int max_pages, n_seed, n_peers;
+  bool use_codes;
+  int64_t launches = 0;
+};
+
+// K5: the first n_lists partial lists of the batch, per query -> the outputs, by original query
+static int launch_merge(kv_index *ix, const Batch &b, int64_t n_lists) {
+  merge_topk_kernel<<<(unsigned)((b.n_q * 32 + 255) / 256), 256, 0, ix->stream>>>(
+      ix->d_part_s.p, ix->d_part_r.p, (int)n_lists, b.n_q, b.k, b.n_q * b.k, b.n_q * b.k, ix->d_qperm.p, b.out_s, b.out_r);
+  KV_CUDA(cudaGetLastError());
+  return KV_OK;
+}
+
+// K1b-S parameters shared by every scan of the batch (the caller sets the candidate lists and the splits)
+static ScanParams scan_params(const kv_index *ix, const Batch &b) {
+  const float *qc = ix->d_qconst.p;
+  ScanParams SP{};
+  SP.blk = ix->d_blk.p; SP.binfo = ix->d_binfo.p; SP.B32 = ix->d_B32.p; SP.perm = ix->d_perm.p;
+  SP.n_chunks = ix->n_chunks; SP.n_rows = ix->n_rows; SP.row_base = ix->row_base;
+  SP.ovf_keys = ix->d_ovf_keys.p; SP.ovf_vals = ix->d_ovf_vals.p; SP.n_ovf = ix->n_ovf;
+  SP.qtab = ix->d_qtab.p; SP.q_nq = qc; SP.q_dotU = qc + b.n_q; SP.q_corrU = qc + 2 * b.n_q;
+  SP.q_excl = ix->has_excl ? ix->d_excl_sorted.p : nullptr; SP.gthr = ix->d_gthr.p;
+  for (int i = 0; i < 7; i++) SP.peer_gthr[i] = i < b.n_peers ? ix->peer_gthr[i] : nullptr;
+  SP.n_peers = b.n_peers; SP.stats = ix->d_stats.p; SP.n_q = b.n_q; SP.k = b.k;
+  SP.part_scores = ix->d_part_s.p; SP.part_rows = ix->d_part_r.p; SP.max_pages = b.max_pages;
+  return SP;
+}
+
+// Pruned path.  Phase 0 / 1: bound pass 0 (seeds and bound codes) -> seed scan; phase 1 ends with the seed top-k.
+// Phase 0 / 2: candidate lists -- from the stored codes when they were kept, else by recomputing the bounds (pass 1) --
+// then the scan of the candidates into b.n_parts partial lists.
+static int run_pruned(kv_index *ix, Batch &b) {
+  cudaStream_t s = ix->stream;
+  const float *qc = ix->d_qconst.p; const int64_t n_q = b.n_q;
+  if (b.phase != 2) KV_CUDA(cudaMemsetAsync(ix->d_pool_ctl.p, 0, 2 * sizeof(unsigned int), s));
+  BoundParams BP;
+  BP.blk = ix->d_blk.p; BP.binfo = ix->d_binfo.p; BP.chunk_minB = ix->d_cminB.p;
+  BP.ovf_keys = ix->d_ovf_keys.p; BP.ovf_vals = ix->d_ovf_vals.p; BP.n_ovf = ix->n_ovf;
+  BP.n_chunks = ix->n_chunks; BP.n_q = n_q; BP.q2list = ix->d_q2list.p; BP.q3list = ix->d_q3list.p; BP.ubt = ix->d_ubt.p;
+  BP.rbloom = ix->d_rbloom.p; BP.rt_keys = ix->d_rt_keys.p; BP.rt_masks = ix->d_rt_masks.p; BP.rt_off = ix->d_rt_off.p;
+  BP.rt_size = ix->d_rt_size.p; BP.tfmax = ix->d_tfmax.p;
+  BP.q_nq = qc; BP.q_dotS = qc + 3 * n_q; BP.q_corrS = qc + 4 * n_q; BP.q_dotX = qc + 5 * n_q; BP.q_rscale = qc + 6 * n_q;
+  BP.gthr = ix->d_gthr.p; BP.n_bsplits = (int)b.n_bsplits; BP.seeds = ix->d_seeds.p;
+  BP.lists.count = ix->d_list_count.p + b.n_groups; BP.lists.pages = ix->d_list_pages.p; BP.lists.max_pages = b.max_pages;
+  BP.lists.pool = ix->d_pool.p; BP.lists.pool_next = ix->d_pool_ctl.p; BP.lists.pool_pages = (unsigned int)ix->pool_pages;
+  BP.lists.overflow = (int *)(ix->d_pool_ctl.p + 1); BP.stats = ix->d_stats.p;
+  BP.dbg_xs = ix->dbg_xs; BP.dbg_stride = ix->n_chunks_pad; BP.ubq = b.use_codes ? ix->d_ubq.p : nullptr; BP.ubq_stride = ix->n_chunks_pad;
+  const size_t b_smem = bound_smem_bytes(b.max_pages);
+  const dim3 bgrid((unsigned)b.n_tiles, (unsigned)b.n_bsplits);
+  ScanParams SP = scan_params(ix, b);
+  if (b.phase != 2) {
+    // pass 0: seeds
+    KV_CUDA(cudaEventRecord(ix->evk[0], s));
+    BP.pass = 0;
+    // the headline configuration (bound codes kept, no test hook) runs the specialised instantiation
+    if (BP.ubq && !BP.dbg_xs && !getenv("KAKVEDA_B200_GENERIC_BOUND"))
+      tfidf_bound_kernel<true><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_u, BP);
+    else
+      tfidf_bound_kernel<false><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_u, BP);
+    KV_CUDA(cudaGetLastError());
+    seeds_to_lists_kernel<<<(unsigned)((b.n_groups * GROUP_Q * b.n_seed + 255) / 256), 256, 0, s>>>(
+        ix->d_seeds.p, n_q, b.n_seed, ix->d_direct.p, ix->d_list_count.p);
+    KV_CUDA(cudaGetLastError());
+    KV_CUDA(cudaEventRecord(ix->evk[1], s));
+    // seed scan: gives every query a lower bound of its k-th score
+    SP.list_mode = 1; SP.list_count = ix->d_list_count.p; SP.direct = ix->d_direct.p; SP.direct_stride = GROUP_Q * b.n_seed;
+    SP.n_bsplits = 1; SP.n_ssplits = (int)b.n_ssplits_a;
+    tfidf_scan_kernel<<<dim3((unsigned)b.n_groups, (unsigned)b.n_ssplits_a), S_WARPS * 32, scan_smem_bytes(b.k), s>>>(SP);
+    KV_CUDA(cudaGetLastError());
+    KV_CUDA(cudaEventRecord(ix->evk[2], s));
+    b.launches += 3;
+    if (b.phase == 1) {  // the seed top-k of this shard, by original query
+      b.launches++;
+      return launch_merge(ix, b, b.n_ssplits_a);
+    }
+  }
+  if (b.phase == 2) KV_CUDA(cudaEventRecord(ix->evp2, s));  // the caller's threshold exchange sits between evk[2] and this point
+  if (b.use_codes) {
+    SelectParams LP;
+    LP.ubq = ix->d_ubq.p; LP.ubq_stride = ix->n_chunks_pad; LP.n_chunks = ix->n_chunks; LP.n_q = n_q;
+    LP.q_nq = qc; LP.gthr = ix->d_gthr.p; LP.n_bsplits = (int)b.n_bsplits; LP.lists = BP.lists; LP.stats = BP.stats;
+    tfidf_select_kernel<<<dim3((unsigned)b.n_groups, (unsigned)b.n_bsplits), SEL_WARPS * 32, (size_t)b.max_pages * sizeof(int), s>>>(LP);
+  } else {
+    BP.pass = 1;
+    tfidf_bound_kernel<false><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_u, BP);
+  }
+  KV_CUDA(cudaGetLastError());
+  KV_CUDA(cudaEventRecord(ix->evk[3], s));
+  SP.list_mode = 0; SP.list_count = BP.lists.count; SP.list_pages = ix->d_list_pages.p; SP.pool = ix->d_pool.p;
+  SP.n_bsplits = (int)b.n_bsplits; SP.n_ssplits = (int)b.n_ssplits;
+  tfidf_scan_kernel<<<dim3((unsigned)(b.n_groups * b.n_bsplits), (unsigned)b.n_ssplits), S_WARPS * 32, scan_smem_bytes(b.k), s>>>(SP);
+  KV_CUDA(cudaGetLastError());
+  b.launches += 2;
+  return KV_OK;
+}
+
+// Exhaustive path: every chunk of a list's chunk range x every query of the group
+static int run_exhaustive(kv_index *ix, Batch &b) {
+  ScanParams SP = scan_params(ix, b);
+  SP.list_mode = 2; SP.n_bsplits = (int)b.n_bsplits; SP.n_ssplits = (int)b.n_ssplits;
+  tfidf_scan_kernel<<<dim3((unsigned)(b.n_groups * b.n_bsplits), (unsigned)b.n_ssplits), S_WARPS * 32, scan_smem_bytes(b.k),
+                      ix->stream>>>(SP);
+  KV_CUDA(cudaGetLastError());
+  b.launches++;
+  return KV_OK;
+}
+
+// Jaccard path: token sets have no text structure to prune on -- the dense-regime kernel K3 scores every chunk for a
+// whole scan group at once
+static int run_jaccard(kv_index *ix, Batch &b) {
+  const int64_t n_q = b.n_q, n_groups = b.n_groups;
+  const int64_t jsplits = std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>((4LL * ix->sm_count + n_groups - 1) / n_groups, 256),
+                                                                 std::max<int64_t>(1, ix->n_chunks / 64)));
+  b.n_parts = jsplits * J_WARPS;
+  KV_CUDA(ix->d_part_s.ensure(b.n_parts * n_q * b.k));
+  KV_CUDA(ix->d_part_r.ensure(b.n_parts * n_q * b.k));
+  const float *qc = ix->d_qconst.p;
+  JaccardParams JP;
+  JP.blk = ix->d_blk.p; JP.binfo = ix->d_binfo.p; JP.B32 = ix->d_B32.p; JP.perm = ix->d_perm.p;
+  JP.n_chunks = ix->n_chunks; JP.n_rows = ix->n_rows; JP.row_base = ix->row_base;
+  JP.qtab = ix->d_qtab.p; JP.q_nq = qc; JP.q_dotU = qc + n_q; JP.q_excl = ix->has_excl ? ix->d_excl_sorted.p : nullptr;
+  JP.gthr = ix->d_gthr.p; JP.stats = ix->d_stats.p;
+  JP.n_q = n_q; JP.k = b.k; JP.n_splits = (int)jsplits; JP.part_scores = ix->d_part_s.p; JP.part_rows = ix->d_part_r.p;
+  static bool jattr[64] = {false};
+  if (!jattr[ix->device & 63]) {
+    KV_CUDA(cudaFuncSetAttribute(jaccard_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jaccard_smem_bytes(32)));
+    jattr[ix->device & 63] = true;
+  }
+  jaccard_scan_kernel<<<dim3((unsigned)n_groups, (unsigned)jsplits), J_WARPS * 32, jaccard_smem_bytes(b.k), ix->stream>>>(JP);
+  KV_CUDA(cudaGetLastError());
+  b.launches++;
+  return KV_OK;
+}
+
 static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, int phase = 0) {
   if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_topk_resident: no query batch uploaded");
   if (k < 1 || k > 32) return kv_fail(KV_ERR_INVALID, "kv_topk: k must be 1..32");
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
-  const int64_t n_q = ix->batch_q, n_tiles = ix->batch_tiles;
-  const int64_t n_groups = (n_q + GROUP_Q - 1) / GROUP_Q;
+  Batch b;
+  b.k = k; b.phase = phase; b.out_s = d_out_s; b.out_r = d_out_r;
+  const int64_t n_q = b.n_q = ix->batch_q, n_tiles = b.n_tiles = ix->batch_tiles;
+  const int64_t n_groups = b.n_groups = (n_q + GROUP_Q - 1) / GROUP_Q;
   const int64_t n_blocks = (ix->n_chunks + B_BN - 1) / B_BN;
-  // Pruned mode: bound pass 0 -> seed scan -> bound pass 1 -> scan of the candidates.  Exhaustive mode (small
-  // indexes, KAKVEDA_B200_NO_PRUNE=1): every chunk is a candidate of every query.
   const char *env = getenv("KAKVEDA_B200_NO_PRUNE");
-  // Jaccard mode: token sets have no text structure to prune on -- the dense-regime kernel K3 scores every chunk for a
-  // whole scan group at once (KAKVEDA_B200_JACCARD_GENERIC=1 forces the generic bound + scan path)
-  const bool jdense = ix->jaccard && !getenv("KAKVEDA_B200_JACCARD_GENERIC");
-  const int prune = (env && env[0] == '1') || jdense ? 0 : (ix->n_chunks >= 512 ? 1 : 0);
-  int64_t n_bsplits, n_ssplits;
+  const bool prune = !(env && env[0] == '1') && !ix->jaccard && ix->n_chunks >= 512;
+  int64_t &n_bsplits = b.n_bsplits, &n_ssplits = b.n_ssplits;
   if (prune) {
     n_bsplits = std::max<int64_t>(1, std::min<int64_t>((ix->sm_count + n_tiles - 1) / n_tiles, n_blocks));
     // a bound CTA keeps the page table of its four candidate lists in shared memory: bound the chunks per row range
@@ -964,28 +1136,29 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
                                                         std::min<int64_t>(1024, std::max<int64_t>(1, ix->n_chunks / 4))));
     n_ssplits = 1;
   }
-  const int64_t n_lists = n_groups * n_bsplits, n_parts = n_bsplits * n_ssplits;
-  const int64_t n_ssplits_a = std::max<int64_t>(1, std::min<int64_t>((4LL * ix->sm_count + n_groups - 1) / n_groups, 8));
-  ix->last_tiles = n_tiles; ix->last_splits = n_parts; ix->last_ctas = n_lists * n_ssplits;
+  const int64_t n_lists = n_groups * n_bsplits;
+  b.n_parts = n_bsplits * n_ssplits;
+  b.n_ssplits_a = std::max<int64_t>(1, std::min<int64_t>((4LL * ix->sm_count + n_groups - 1) / n_groups, 8));
+  ix->last_tiles = n_tiles; ix->last_splits = b.n_parts; ix->last_ctas = n_lists * n_ssplits;
   if (n_q > ix->d_gthr.cap && (ix->gthr_exported || ix->n_peers))
     return kv_fail(KV_ERR_STATE, "kv_topk: the query batch outgrew the threshold array shared with the peer GPUs; exchange it again "
                                  "(kv_index_thresholds_export / kv_index_thresholds_peers)");
   KV_CUDA(ix->d_gthr.ensure(n_q));
-  const int n_peers = (ix->n_peers > 0 && n_q <= ix->peer_cap) ? ix->n_peers : 0;
-  const int64_t parts_alloc = std::max(n_parts, n_ssplits_a);
+  b.n_peers = (ix->n_peers > 0 && n_q <= ix->peer_cap) ? ix->n_peers : 0;
+  const int64_t parts_alloc = std::max(b.n_parts, b.n_ssplits_a);
   KV_CUDA(ix->d_part_s.ensure(parts_alloc * n_q * k));
   KV_CUDA(ix->d_part_r.ensure(parts_alloc * n_q * k));
   KV_CUDA(ix->d_stats.ensure(8));
-  const int n_seed = (int)n_bsplits * B_SEEDS_PER_QUERY;
+  b.n_seed = (int)n_bsplits * B_SEEDS_PER_QUERY;
   const int64_t chunks_per_split = ((n_blocks + n_bsplits - 1) / n_bsplits + 1) * B_BN;
-  const int max_pages = (int)(chunks_per_split / PAGE_RECS + 2);
+  b.max_pages = (int)(chunks_per_split / PAGE_RECS + 2);
   if (prune) {
-    KV_CUDA(ix->d_seeds.ensure(n_q * n_seed));
-    KV_CUDA(ix->d_direct.ensure(n_groups * GROUP_Q * n_seed));
+    KV_CUDA(ix->d_seeds.ensure(n_q * b.n_seed));
+    KV_CUDA(ix->d_direct.ensure(n_groups * GROUP_Q * b.n_seed));
     // the bound kernel writes the lists of whole tiles (4 groups each), including the groups past the last query
     KV_CUDA(ix->d_list_count.ensure(n_groups + n_tiles * 4 * n_bsplits));
-    KV_CUDA(ix->d_list_pages.ensure(n_tiles * 4 * n_bsplits * max_pages));
-    const int64_t want_pages = std::min<int64_t>(n_lists * max_pages, 524288 + n_lists);  // up to 4 GiB of records
+    KV_CUDA(ix->d_list_pages.ensure(n_tiles * 4 * n_bsplits * b.max_pages));
+    const int64_t want_pages = std::min<int64_t>(n_lists * b.max_pages, 524288 + n_lists);  // up to 4 GiB of records
     if (want_pages > ix->pool_pages) {
       KV_CUDA(ix->d_pool.ensure(want_pages * PAGE_RECS));
       ix->pool_pages = want_pages;
@@ -994,24 +1167,23 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
   }
   // Second pass without recomputation: the first bound pass stores every bound as an 8-bit code (n_q x chunks bytes)
   // when that fits comfortably (KAKVEDA_B200_BOUND_CODES=0 forces the recomputing second pass).
-  bool use_codes = false;
+  b.use_codes = false;
   if (prune) {
     const char *ce = getenv("KAKVEDA_B200_BOUND_CODES");
     const int64_t want = n_q * ix->n_chunks_pad;
     if (phase == 2) {
-      use_codes = ix->last_used_codes != 0;
+      b.use_codes = ix->last_used_codes != 0;
     } else if (!(ce && ce[0] == '0')) {
-      use_codes = want <= ix->d_ubq.cap;
-      if (!use_codes) {
+      b.use_codes = want <= ix->d_ubq.cap;
+      if (!b.use_codes) {
         size_t free_b = 0, total_b = 0;
         cudaMemGetInfo(&free_b, &total_b);
-        use_codes = want <= (int64_t)std::min<size_t>((size_t)64 << 30, free_b / 2);
-        if (use_codes) KV_CUDA(ix->d_ubq.ensure(want));
+        b.use_codes = want <= (int64_t)std::min<size_t>((size_t)64 << 30, free_b / 2);
+        if (b.use_codes) KV_CUDA(ix->d_ubq.ensure(want));
       }
     }
   }
-  if (phase != 2) ix->last_used_codes = use_codes ? 1 : 0;
-  const bool do_p1 = phase != 2, do_p2 = phase != 1;
+  if (phase != 2) ix->last_used_codes = b.use_codes ? 1 : 0;
   static bool attr_set[64] = {false};
   if (!attr_set[ix->device & 63]) {
     KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scan_smem_bytes(32)));
@@ -1019,181 +1191,67 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
     KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
     attr_set[ix->device & 63] = true;
   }
-  if (prune && bound_smem_bytes(max_pages) > 232448)
-    return kv_fail(KV_ERR_INVALID, "kv_topk: index too large for one bound-kernel row range (max_pages %d)", max_pages);
+  if (prune && bound_smem_bytes(b.max_pages) > 232448)
+    return kv_fail(KV_ERR_INVALID, "kv_topk: index too large for one bound-kernel row range (max_pages %d)", b.max_pages);
 
-  int64_t launches = 0;
-  if (do_p1) {
+  if (phase != 2) {
     KV_CUDA(cudaEventRecord(ix->ev[1], s));
     for (auto &e : ix->evk) KV_CUDA(cudaEventRecord(e, s));
   }
-  if (ix->n_rows > 0) {
-    const float *qc = ix->d_qconst.p;
-    if (do_p1) {  // global lower bounds of the k-th score start at -inf
-      KV_CUDA(cudaMemsetAsync(ix->d_stats.p, 0, 8 * sizeof(unsigned long long), s));
-      fill_int_kernel<<<(unsigned)((n_q + 255) / 256), 256, 0, s>>>(ix->d_gthr.p, n_q, (int)0xFF800000);
-      KV_CUDA(cudaGetLastError());
-      launches++;
-    }
-    ScanParams SP;
-    SP.blk = ix->d_blk.p; SP.binfo = ix->d_binfo.p; SP.B32 = ix->d_B32.p; SP.perm = ix->d_perm.p;
-    SP.n_chunks = ix->n_chunks; SP.n_rows = ix->n_rows; SP.row_base = ix->row_base;
-    SP.ovf_keys = ix->d_ovf_keys.p; SP.ovf_vals = ix->d_ovf_vals.p; SP.n_ovf = ix->n_ovf;
-    SP.qtab = ix->d_qtab.p; SP.q_nq = qc; SP.q_dotU = qc + n_q; SP.q_corrU = qc + 2 * n_q;
-    SP.q_excl = ix->has_excl ? ix->d_excl_sorted.p : nullptr;
-    SP.gthr = ix->d_gthr.p;
-    for (int i = 0; i < 7; i++) SP.peer_gthr[i] = i < n_peers ? ix->peer_gthr[i] : nullptr;
-    SP.n_peers = n_peers;
-    SP.stats = ix->d_stats.p; SP.n_q = n_q; SP.k = k; SP.jaccard = ix->jaccard;
-    SP.part_scores = ix->d_part_s.p; SP.part_rows = ix->d_part_r.p;
-    SP.list_count = nullptr; SP.list_pages = nullptr; SP.max_pages = max_pages; SP.pool = nullptr; SP.direct = nullptr;
-    SP.direct_stride = 0;
-    const size_t s_smem = scan_smem_bytes(k);
-    if (prune) {
-      if (do_p1) KV_CUDA(cudaMemsetAsync(ix->d_pool_ctl.p, 0, 2 * sizeof(unsigned int), s));
-      BoundParams BP;
-      BP.blk = ix->d_blk.p; BP.binfo = ix->d_binfo.p; BP.chunk_minB = ix->d_cminB.p;
-      BP.ovf_keys = ix->d_ovf_keys.p; BP.ovf_vals = ix->d_ovf_vals.p; BP.n_ovf = ix->n_ovf;
-      BP.n_chunks = ix->n_chunks; BP.n_q = n_q; BP.q2list = ix->d_q2list.p; BP.q3list = ix->d_q3list.p; BP.ubt = ix->d_ubt.p;
-      BP.rbloom = ix->d_rbloom.p; BP.rt_keys = ix->d_rt_keys.p; BP.rt_masks = ix->d_rt_masks.p; BP.rt_off = ix->d_rt_off.p;
-      BP.rt_size = ix->d_rt_size.p; BP.tfmax = ix->d_tfmax.p;
-      BP.q_nq = qc; BP.q_dotS = qc + 3 * n_q; BP.q_corrS = qc + 4 * n_q; BP.q_dotX = qc + 5 * n_q;
-      BP.q_rscale = qc + 6 * n_q;
-      BP.gthr = ix->d_gthr.p; BP.n_bsplits = (int)n_bsplits; BP.jaccard = ix->jaccard;
-      BP.seeds = ix->d_seeds.p;
-      BP.list_count = ix->d_list_count.p + n_groups; BP.list_pages = ix->d_list_pages.p; BP.max_pages = max_pages;
-      BP.pool = ix->d_pool.p; BP.pool_next = ix->d_pool_ctl.p; BP.pool_pages = (unsigned int)ix->pool_pages;
-      BP.overflow = (int *)(ix->d_pool_ctl.p + 1); BP.stats = ix->d_stats.p;
-      BP.dbg_xs = ix->dbg_xs; BP.dbg_stride = ix->n_chunks_pad;
-      BP.ubq = use_codes ? ix->d_ubq.p : nullptr; BP.ubq_stride = ix->n_chunks_pad;
-      const size_t b_smem = bound_smem_bytes(max_pages);
-      const dim3 bgrid((unsigned)n_tiles, (unsigned)n_bsplits);
-      if (do_p1) {
-        // pass 0: seeds
-        KV_CUDA(cudaEventRecord(ix->evk[0], s));
-        BP.pass = 0;
-        // the headline configuration (bound codes kept, TF-IDF cosine, no test hook) runs the specialised instantiation
-        if (BP.ubq && !BP.jaccard && !BP.dbg_xs && !getenv("KAKVEDA_B200_GENERIC_BOUND"))
-          tfidf_bound_kernel<true><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_u, BP);
-        else
-          tfidf_bound_kernel<false><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_u, BP);
-        KV_CUDA(cudaGetLastError());
-        seeds_to_lists_kernel<<<(unsigned)((n_groups * GROUP_Q * n_seed + 255) / 256), 256, 0, s>>>(ix->d_seeds.p, n_q, n_seed,
-                                                                                                   ix->d_direct.p, ix->d_list_count.p);
-        KV_CUDA(cudaGetLastError());
-        KV_CUDA(cudaEventRecord(ix->evk[1], s));
-        // seed scan: gives every query a lower bound of its k-th score
-        SP.list_mode = 1; SP.list_count = ix->d_list_count.p; SP.direct = ix->d_direct.p; SP.direct_stride = GROUP_Q * n_seed;
-        SP.n_bsplits = 1; SP.n_ssplits = (int)n_ssplits_a;
-        tfidf_scan_kernel<<<dim3((unsigned)n_groups, (unsigned)n_ssplits_a), S_WARPS * 32, s_smem, s>>>(SP);
-        KV_CUDA(cudaGetLastError());
-        KV_CUDA(cudaEventRecord(ix->evk[2], s));
-        launches += 3;
-        if (phase == 1) {  // the seed top-k of this shard, by original query
-          merge_topk_kernel<<<(unsigned)((n_q * 32 + 255) / 256), 256, 0, s>>>(ix->d_part_s.p, ix->d_part_r.p, (int)n_ssplits_a,
-                                                                               n_q, k, n_q * k, n_q * k, ix->d_qperm.p, d_out_s, d_out_r);
-          KV_CUDA(cudaGetLastError());
-          launches++;
-        }
-      }
-      if (!do_p2) {
-        ix->last_launches = launches;
-        return KV_OK;
-      }
-      ix->two_phase = phase == 2;
-      if (phase == 2) KV_CUDA(cudaEventRecord(ix->evp2, s));  // the caller's threshold exchange sits between evk[2] and this point
-      // pass 1: candidate lists -- from the stored codes when they were kept, else by recomputing the bounds
-      if (use_codes) {
-        SelectParams LP;
-        LP.ubq = ix->d_ubq.p; LP.ubq_stride = ix->n_chunks_pad; LP.n_chunks = ix->n_chunks; LP.n_q = n_q;
-        LP.q_nq = qc; LP.gthr = ix->d_gthr.p; LP.n_bsplits = (int)n_bsplits;
-        LP.list_count = BP.list_count; LP.list_pages = BP.list_pages; LP.max_pages = max_pages;
-        LP.pool = BP.pool; LP.pool_next = BP.pool_next; LP.pool_pages = BP.pool_pages; LP.overflow = BP.overflow; LP.stats = BP.stats;
-        tfidf_select_kernel<<<dim3((unsigned)n_groups, (unsigned)n_bsplits), SEL_WARPS * 32, (size_t)max_pages * sizeof(int), s>>>(LP);
-      } else {
-        BP.pass = 1;
-        tfidf_bound_kernel<false><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_u, BP);
-      }
-      KV_CUDA(cudaGetLastError());
-      KV_CUDA(cudaEventRecord(ix->evk[3], s));
-      SP.list_mode = 0; SP.list_count = ix->d_list_count.p + n_groups; SP.list_pages = ix->d_list_pages.p;
-      SP.pool = ix->d_pool.p; SP.direct = nullptr;
-      launches += 1;
-    } else {
-      SP.list_mode = 2;
-      if (jdense && do_p2) {
-        const int64_t jsplits = std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>((4LL * ix->sm_count + n_groups - 1) / n_groups, 256),
-                                                                       std::max<int64_t>(1, ix->n_chunks / 64)));
-        KV_CUDA(ix->d_part_s.ensure(jsplits * J_WARPS * n_q * k));
-        KV_CUDA(ix->d_part_r.ensure(jsplits * J_WARPS * n_q * k));
-        JaccardParams JP;
-        JP.blk = ix->d_blk.p; JP.binfo = ix->d_binfo.p; JP.B32 = ix->d_B32.p; JP.perm = ix->d_perm.p;
-        JP.n_chunks = ix->n_chunks; JP.n_rows = ix->n_rows; JP.row_base = ix->row_base;
-        JP.qtab = ix->d_qtab.p; JP.q_nq = qc; JP.q_dotU = qc + n_q; JP.q_excl = SP.q_excl; JP.gthr = ix->d_gthr.p;
-        JP.n_q = n_q; JP.k = k; JP.n_splits = (int)jsplits; JP.part_scores = ix->d_part_s.p; JP.part_rows = ix->d_part_r.p;
-        JP.stats = ix->d_stats.p;
-        static bool jattr[64] = {false};
-        if (!jattr[ix->device & 63]) {
-          KV_CUDA(cudaFuncSetAttribute(jaccard_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jaccard_smem_bytes(32)));
-          jattr[ix->device & 63] = true;
-        }
-        jaccard_scan_kernel<<<dim3((unsigned)n_groups, (unsigned)jsplits), J_WARPS * 32, jaccard_smem_bytes(k), s>>>(JP);
-        KV_CUDA(cudaGetLastError());
-        KV_CUDA(cudaEventRecord(ix->evk[4], s));
-        KV_CUDA(cudaEventRecord(ix->ev[2], s));
-        merge_topk_kernel<<<(unsigned)((n_q * 32 + 255) / 256), 256, 0, s>>>(ix->d_part_s.p, ix->d_part_r.p, (int)(jsplits * J_WARPS),
-                                                                             n_q, k, n_q * k, n_q * k, ix->d_qperm.p, d_out_s, d_out_r);
-        KV_CUDA(cudaGetLastError());
-        KV_CUDA(cudaEventRecord(ix->evk[5], s));
-        launches += 2;
-        goto after_scan;
-      }
-      if (!do_p2) {  // exhaustive mode has no seed phase: empty seed lists
-        fill_int_kernel<<<(unsigned)((n_q * k + 255) / 256), 256, 0, s>>>((int *)d_out_s, n_q * k, (int)0xFF800000);
-        fill_ll_kernel<<<(unsigned)((n_q * k + 255) / 256), 256, 0, s>>>(d_out_r, n_q * k, -1LL);
-        KV_CUDA(cudaGetLastError());
-        ix->last_launches = launches + 2;
-        return KV_OK;
-      }
-    }
-    SP.n_bsplits = (int)n_bsplits; SP.n_ssplits = (int)n_ssplits;
-    tfidf_scan_kernel<<<dim3((unsigned)n_lists, (unsigned)n_ssplits), S_WARPS * 32, s_smem, s>>>(SP);
-    KV_CUDA(cudaGetLastError());
-    KV_CUDA(cudaEventRecord(ix->evk[4], s));
-    KV_CUDA(cudaEventRecord(ix->ev[2], s));
-    merge_topk_kernel<<<(unsigned)((n_q * 32 + 255) / 256), 256, 0, s>>>(ix->d_part_s.p, ix->d_part_r.p, (int)n_parts,
-                                                                         n_q, k, n_q * k, n_q * k, ix->d_qperm.p, d_out_s, d_out_r);
-    KV_CUDA(cudaGetLastError());
-    KV_CUDA(cudaEventRecord(ix->evk[5], s));
-    launches += 2;
-  after_scan:
-    if (ix->batch_null) {
-      fill_null_kernel<<<(unsigned)((ix->batch_null * k + 255) / 256), 256, 0, s>>>(ix->d_qperm.p + n_q, (int)ix->batch_null, k,
-                                                                                    ix->n_rows, ix->row_base,
-                                                                                    ix->has_excl ? ix->d_excl_orig.p : nullptr, d_out_s, d_out_r);
-      KV_CUDA(cudaGetLastError());
-      launches++;
-    }
-    for (size_t i = 0; i < ix->irr_q.size(); i++) {
-      const int64_t q = ix->irr_q[i], a = ix->irr_indptr[i], b = ix->irr_indptr[i + 1];
-      int rc = score_impl(ix, ix->irr_ids.data() + a, ix->irr_tf.data() + a, b - a, ix->irr_oov[i], nullptr);
-      if (rc != KV_OK) return rc;
-      select_topk_kernel<<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
-                                            ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, d_out_s + q * k, d_out_r + q * k);
-      KV_CUDA(cudaGetLastError());
-      launches += 2;
-    }
-    KV_CUDA(cudaMemcpyAsync(ix->last_stats, ix->d_stats.p, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-    if (prune) KV_CUDA(cudaMemcpyAsync(&ix->last_stats[6], ix->d_pool_ctl.p, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
-  } else {
+  const int64_t prior_launches = phase == 2 ? ix->last_launches : 0;
+  ix->two_phase = prune && phase == 2;
+  if (ix->n_rows == 0) {
     KV_CUDA(cudaEventRecord(ix->ev[2], s));
     std::vector<float> es((size_t)(n_q * k), -INFINITY);
     std::vector<long long> er((size_t)(n_q * k), -1);
     KV_CUDA(cudaMemcpyAsync(d_out_s, es.data(), es.size() * 4, cudaMemcpyHostToDevice, s));
     KV_CUDA(cudaMemcpyAsync(d_out_r, er.data(), er.size() * 8, cudaMemcpyHostToDevice, s));
     KV_CUDA(cudaStreamSynchronize(s));
+    ix->last_launches = prior_launches;
+    KV_CUDA(cudaEventRecord(ix->ev[3], s));
+    return KV_OK;
   }
-  ix->last_launches = (phase == 2 ? ix->last_launches : 0) + launches;
+  if (phase != 2) {  // global lower bounds of the k-th score start at -inf
+    KV_CUDA(cudaMemsetAsync(ix->d_stats.p, 0, 8 * sizeof(unsigned long long), s));
+    fill_int_kernel<<<(unsigned)((n_q + 255) / 256), 256, 0, s>>>(ix->d_gthr.p, n_q, (int)0xFF800000);
+    KV_CUDA(cudaGetLastError());
+    b.launches++;
+  }
+  if (phase == 1 && !prune) {  // the exhaustive and Jaccard paths have no seed phase: empty seed lists
+    fill_int_kernel<<<(unsigned)((n_q * k + 255) / 256), 256, 0, s>>>((int *)d_out_s, n_q * k, (int)0xFF800000);
+    fill_ll_kernel<<<(unsigned)((n_q * k + 255) / 256), 256, 0, s>>>(d_out_r, n_q * k, -1LL);
+    KV_CUDA(cudaGetLastError());
+    ix->last_launches = b.launches + 2;
+    return KV_OK;
+  }
+  int rc = prune ? run_pruned(ix, b) : ix->jaccard ? run_jaccard(ix, b) : run_exhaustive(ix, b);
+  if (rc != KV_OK) return rc;
+  if (phase == 1) { ix->last_launches = b.launches; return KV_OK; }
+  KV_CUDA(cudaEventRecord(ix->evk[4], s));
+  KV_CUDA(cudaEventRecord(ix->ev[2], s));
+  if ((rc = launch_merge(ix, b, b.n_parts)) != KV_OK) return rc;
+  KV_CUDA(cudaEventRecord(ix->evk[5], s));
+  b.launches++;
+  // queries no path scanned: null queries score 0 against every row, irregular ones take the float64 full scan
+  if (ix->batch_null) {
+    fill_null_kernel<<<(unsigned)((ix->batch_null * k + 255) / 256), 256, 0, s>>>(ix->d_qperm.p + n_q, (int)ix->batch_null, k,
+                                                                                  ix->n_rows, ix->row_base,
+                                                                                  ix->has_excl ? ix->d_excl_orig.p : nullptr, d_out_s, d_out_r);
+    KV_CUDA(cudaGetLastError());
+    b.launches++;
+  }
+  for (size_t i = 0; i < ix->irr_q.size(); i++) {
+    const int64_t q = ix->irr_q[i], a = ix->irr_indptr[i], e = ix->irr_indptr[i + 1];
+    rc = score_impl(ix, ix->irr_ids.data() + a, ix->irr_tf.data() + a, e - a, ix->irr_oov[i], nullptr);
+    if (rc != KV_OK) return rc;
+    select_topk_kernel<<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
+                                          ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, d_out_s + q * k, d_out_r + q * k);
+    KV_CUDA(cudaGetLastError());
+    b.launches += 2;
+  }
+  KV_CUDA(cudaMemcpyAsync(ix->last_stats, ix->d_stats.p, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+  if (prune) KV_CUDA(cudaMemcpyAsync(&ix->last_stats[6], ix->d_pool_ctl.p, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+  ix->last_launches = prior_launches + b.launches;
   KV_CUDA(cudaEventRecord(ix->ev[3], s));
   return KV_OK;
 }
@@ -1599,7 +1657,8 @@ int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[17]) {
   bytes[0] = ix->blk_words * 4;
   bytes[1] = ix->n_rows * 4;
   bytes[2] = ix->n_chunks_pad * (int64_t)sizeof(BlockInfo);
-  bytes[3] = ix->n_chunks_pad * (int64_t)(NF * sizeof(__half) + sizeof(float)) + ix->rare_table_bytes + (ix->n_chunks_pad / 64) * (int64_t)(NF2 * 16);
+  const int64_t rare_table_bytes = ix->n_rt_slots * 12 + (ix->n_chunks_pad / 64) * (RB_BITS / 8);
+  bytes[3] = ix->n_chunks_pad * (int64_t)(NF * sizeof(__half) + sizeof(float)) + rare_table_bytes + (ix->n_chunks_pad / 64) * (int64_t)(NF2 * 16);
   counts[0] = ix->n_entries; counts[1] = ix->n_univ; counts[2] = ix->n_rows;
   counts[3] = ix->last_ctas; counts[4] = ix->last_tiles; counts[5] = ix->last_splits;
   counts[6] = ix->batch_h2d_bytes; counts[7] = ix->n_ovf;
@@ -1647,22 +1706,10 @@ uint64_t csr_checksum(const kv_index *ix) {
   return h;
 }
 
-struct LayoutHeader {
-  uint64_t magic, checksum;
-  int64_t n_rows, nnz, V, n_chunks, n_chunks_pad, blk_words, n_entries, n_rare_entries, n_ovf, n_rt_slots, n_blocks, univ_len;
-  int32_t jaccard, corpus_fit, threads, reserved;
-};
-
 template <class T>
 bool put(FILE *f, const std::vector<T> &v) { return v.empty() || fwrite(v.data(), sizeof(T), v.size(), f) == v.size(); }
 template <class T>
 bool get(FILE *f, std::vector<T> &v, size_t n) { v.resize(n); return n == 0 || fread(v.data(), sizeof(T), n, f) == n; }
-template <class T>
-int pull(std::vector<T> &h, const T *d, size_t n) {
-  h.resize(n);
-  if (n) KV_CUDA(cudaMemcpy(h.data(), d, n * sizeof(T), cudaMemcpyDeviceToHost));
-  return KV_OK;
-}
 }  // namespace
 
 extern "C" int kv_index_layout_save(kv_index *ix, const char *path) {
@@ -1671,32 +1718,24 @@ extern "C" int kv_index_layout_save(kv_index *ix, const char *path) {
   if (!ix->finalized || !ix->layout_valid) return kv_fail(KV_ERR_STATE, "kv_index_layout_save: index has no built layout (finalize first)");
   KV_CUDA(cudaSetDevice(ix->device));
   KV_CUDA(cudaStreamSynchronize(ix->stream));
-  LayoutHeader H{};
+  ScanLayout SL;
+  LayoutHeader &H = SL.H;
   H.magic = LAYOUT_MAGIC; H.checksum = csr_checksum(ix);
   H.n_rows = ix->n_rows; H.nnz = ix->nnz; H.V = (int64_t)ix->h_fslot.size(); H.n_chunks = ix->n_chunks; H.n_chunks_pad = ix->n_chunks_pad;
   H.blk_words = ix->blk_words; H.n_entries = ix->n_entries; H.n_rare_entries = ix->n_rare_entries; H.n_ovf = ix->n_ovf;
-  H.n_blocks = ix->n_chunks_pad / 64; H.univ_len = (int64_t)ix->layout_univ.size();
+  H.n_rt_slots = ix->n_rt_slots; H.n_blocks = ix->n_chunks_pad / 64; H.univ_len = (int64_t)ix->layout_univ.size();
   H.jaccard = ix->jaccard; H.corpus_fit = ix->corpus_fit;
-  std::vector<uint32_t> rt_off, rt_size;
-  int rc;
-  if ((rc = pull(rt_off, ix->d_rt_off.p, (size_t)H.n_blocks)) != KV_OK || (rc = pull(rt_size, ix->d_rt_size.p, (size_t)H.n_blocks)) != KV_OK) return rc;
-  H.n_rt_slots = H.n_blocks ? (int64_t)rt_off.back() + rt_size.back() : 0;
-  std::vector<int> perm;
-  std::vector<uint32_t> blk, ubt, rbloom, rt_keys, ovf_vals;
-  std::vector<BlockInfo> binfo;
-  std::vector<__half> uf;
-  std::vector<unsigned long long> rt_masks, ovf_keys;
-  if ((rc = pull(perm, ix->d_perm.p, (size_t)H.n_rows)) != KV_OK || (rc = pull(blk, ix->d_blk.p, (size_t)H.blk_words)) != KV_OK ||
-      (rc = pull(binfo, ix->d_binfo.p, (size_t)H.n_chunks_pad)) != KV_OK || (rc = pull(uf, ix->d_Uf.p, (size_t)H.n_chunks_pad * NF)) != KV_OK ||
-      (rc = pull(ubt, ix->d_ubt.p, (size_t)H.n_blocks * NF2 * 4)) != KV_OK || (rc = pull(rbloom, ix->d_rbloom.p, (size_t)H.n_blocks * (RB_BITS / 32))) != KV_OK ||
-      (rc = pull(rt_keys, ix->d_rt_keys.p, (size_t)H.n_rt_slots)) != KV_OK || (rc = pull(rt_masks, ix->d_rt_masks.p, (size_t)H.n_rt_slots)) != KV_OK ||
-      (rc = pull(ovf_keys, ix->d_ovf_keys.p, (size_t)H.n_ovf)) != KV_OK || (rc = pull(ovf_vals, ix->d_ovf_vals.p, (size_t)H.n_ovf)) != KV_OK)
-    return rc;
+  cudaError_t err = cudaSuccess;
+  each_array(SL, ix, [&](auto &h, auto &d, size_t n) {
+    h.resize(n);
+    if (n) err = cudaMemcpy(h.data(), d.p, n * sizeof(h[0]), cudaMemcpyDeviceToHost);
+    return err == cudaSuccess;
+  });
+  KV_CUDA(err);
   FILE *f = fopen(path, "wb");
   if (!f) return kv_fail(KV_ERR_INVALID, "kv_index_layout_save: cannot open %s", path);
-  bool ok = fwrite(&H, sizeof(H), 1, f) == 1 && put(f, ix->layout_univ) && put(f, ix->h_fslot) && put(f, ix->h_fslot2) && put(f, perm) &&
-            put(f, binfo) && put(f, blk) && put(f, uf) && put(f, ubt) && put(f, rbloom) && put(f, rt_off) && put(f, rt_size) && put(f, rt_keys) &&
-            put(f, rt_masks) && put(f, ovf_keys) && put(f, ovf_vals);
+  bool ok = fwrite(&H, sizeof(H), 1, f) == 1 && put(f, ix->layout_univ) &&
+            each_array(SL, ix, [&](const auto &h, auto &, size_t) { return put(f, h); });
   ok = (fclose(f) == 0) && ok;
   if (!ok) return kv_fail(KV_ERR_INVALID, "kv_index_layout_save: short write to %s", path);
   return KV_OK;
@@ -1708,60 +1747,18 @@ extern "C" int kv_index_layout_load(kv_index *ix, const char *path) {
   KV_CUDA(cudaSetDevice(ix->device));
   FILE *f = fopen(path, "rb");
   if (!f) return kv_fail(KV_ERR_INVALID, "kv_index_layout_load: cannot open %s", path);
-  LayoutHeader H{};
-  std::vector<uint8_t> univ;
-  std::vector<short> fslot;
-  std::vector<unsigned short> fslot2;
-  std::vector<int> perm;
-  std::vector<uint32_t> blk, ubt, rbloom, rt_off, rt_size, rt_keys, ovf_vals;
-  std::vector<BlockInfo> binfo;
-  std::vector<__half> uf;
-  std::vector<unsigned long long> rt_masks, ovf_keys;
-  bool ok = fread(&H, sizeof(H), 1, f) == 1 && H.magic == LAYOUT_MAGIC;
+  ScanLayout SL;
+  const LayoutHeader &H = SL.H;
+  bool ok = fread(&SL.H, sizeof(SL.H), 1, f) == 1 && H.magic == LAYOUT_MAGIC;
   if (ok && (H.n_rows != ix->n_rows || H.nnz != ix->nnz || H.jaccard != ix->jaccard || H.corpus_fit != ix->corpus_fit || H.checksum != csr_checksum(ix))) {
     fclose(f);
     return kv_fail(KV_ERR_STATE, "kv_index_layout_load: %s was built for other rows (or another mode)", path);
   }
-  ok = ok && get(f, univ, (size_t)H.univ_len) && get(f, fslot, (size_t)H.V) && get(f, fslot2, (size_t)H.V) && get(f, perm, (size_t)H.n_rows) &&
-       get(f, binfo, (size_t)H.n_chunks_pad) && get(f, blk, (size_t)H.blk_words) && get(f, uf, (size_t)H.n_chunks_pad * NF) &&
-       get(f, ubt, (size_t)H.n_blocks * NF2 * 4) && get(f, rbloom, (size_t)H.n_blocks * (RB_BITS / 32)) && get(f, rt_off, (size_t)H.n_blocks) &&
-       get(f, rt_size, (size_t)H.n_blocks) && get(f, rt_keys, (size_t)H.n_rt_slots) && get(f, rt_masks, (size_t)H.n_rt_slots) &&
-       get(f, ovf_keys, (size_t)H.n_ovf) && get(f, ovf_vals, (size_t)H.n_ovf);
+  ok = ok && get(f, SL.univ, (size_t)H.univ_len) && each_array(SL, ix, [&](auto &h, auto &, size_t n) { return get(f, h, n); });
   fclose(f);
   if (!ok) return kv_fail(KV_ERR_INVALID, "kv_index_layout_load: %s is not a layout file of this version (or is truncated)", path);
-  cudaStream_t s = ix->stream;
-  const int64_t nz = std::max<int64_t>(H.n_rows, 1);
-  KV_CUDA(ix->d_perm.ensure(nz)); KV_CUDA(ix->d_invperm.ensure(nz)); KV_CUDA(ix->d_B64.ensure(nz)); KV_CUDA(ix->d_B32.ensure(nz));
-  KV_CUDA(ix->d_blk.ensure(H.blk_words + 64)); KV_CUDA(ix->d_binfo.ensure(H.n_chunks_pad)); KV_CUDA(ix->d_Uf.ensure(H.n_chunks_pad * NF));
-  KV_CUDA(ix->d_cminB.ensure(H.n_chunks_pad)); KV_CUDA(ix->d_fslot.ensure(std::max<int64_t>(H.V, 1))); KV_CUDA(ix->d_fslot2.ensure(std::max<int64_t>(H.V, 1)));
-  KV_CUDA(ix->d_ubt.ensure((int64_t)ubt.size())); KV_CUDA(ix->d_rbloom.ensure((int64_t)rbloom.size()));
-  KV_CUDA(ix->d_rt_off.ensure(std::max<int64_t>(H.n_blocks, 1))); KV_CUDA(ix->d_rt_size.ensure(std::max<int64_t>(H.n_blocks, 1)));
-  KV_CUDA(ix->d_rt_keys.ensure(std::max<int64_t>(H.n_rt_slots, 1))); KV_CUDA(ix->d_rt_masks.ensure(std::max<int64_t>(H.n_rt_slots, 1)));
-  KV_CUDA(ix->d_ovf_keys.ensure(std::max<int64_t>(H.n_ovf, 1))); KV_CUDA(ix->d_ovf_vals.ensure(std::max<int64_t>(H.n_ovf, 1)));
-  auto up = [&](void *d, const void *h, size_t bytes) { return bytes ? cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, s) : cudaSuccess; };
-  KV_CUDA(up(ix->d_perm.p, perm.data(), perm.size() * 4)); KV_CUDA(up(ix->d_blk.p, blk.data(), blk.size() * 4));
-  KV_CUDA(up(ix->d_binfo.p, binfo.data(), binfo.size() * sizeof(BlockInfo))); KV_CUDA(up(ix->d_Uf.p, uf.data(), uf.size() * sizeof(__half)));
-  KV_CUDA(up(ix->d_fslot.p, fslot.data(), fslot.size() * 2)); KV_CUDA(up(ix->d_fslot2.p, fslot2.data(), fslot2.size() * 2));
-  KV_CUDA(up(ix->d_ubt.p, ubt.data(), ubt.size() * 4)); KV_CUDA(up(ix->d_rbloom.p, rbloom.data(), rbloom.size() * 4));
-  KV_CUDA(up(ix->d_rt_off.p, rt_off.data(), rt_off.size() * 4)); KV_CUDA(up(ix->d_rt_size.p, rt_size.data(), rt_size.size() * 4));
-  KV_CUDA(up(ix->d_rt_keys.p, rt_keys.data(), rt_keys.size() * 4)); KV_CUDA(up(ix->d_rt_masks.p, rt_masks.data(), rt_masks.size() * 8));
-  KV_CUDA(up(ix->d_ovf_keys.p, ovf_keys.data(), ovf_keys.size() * 8)); KV_CUDA(up(ix->d_ovf_vals.p, ovf_vals.data(), ovf_vals.size() * 4));
-  if (H.n_rows) {
-    invperm_kernel<<<(unsigned)((H.n_rows + 255) / 256), 256, 0, s>>>(ix->d_perm.p, H.n_rows, ix->d_invperm.p);
-    KV_CUDA(cudaGetLastError());
-  }
-  KV_CUDA(cudaStreamSynchronize(s));
-  {
-    int rc = make_map_f16_nf(&ix->map_u, ix->d_Uf.p, H.n_chunks_pad, B_BN);
-    if (rc != KV_OK) return rc;
-  }
-  ix->h_fslot = fslot; ix->h_fslot2 = fslot2;
-  ix->n_chunks = H.n_chunks; ix->n_chunks_pad = H.n_chunks_pad; ix->blk_words = H.blk_words; ix->n_entries = H.n_entries;
-  ix->n_rare_entries = H.n_rare_entries; ix->n_ovf = (int)H.n_ovf;
-  ix->rare_table_bytes = H.n_rt_slots * 12 + (int64_t)rbloom.size() * 4;
-  ix->layout_valid = H.n_rows > 0;
-  ix->layout_rows = H.n_rows;
-  ix->layout_univ = univ;
+  int rc = upload_layout(ix, SL);
+  if (rc != KV_OK) return rc;
   ix->finalized = false;
   return KV_OK;
 }

@@ -453,7 +453,7 @@ struct ScanParams {
   int n_bsplits, n_ssplits;
   unsigned long long *stats;    // [0] (query, chunk) pairs scored, [1] records
   int64_t n_q;
-  int k, jaccard;
+  int k;
   float *part_scores;  // [n_bsplits * n_ssplits][n_q][k]
   long long *part_rows;
 };
@@ -466,15 +466,6 @@ struct ScanHit {
   uint32_t m, c_lo, w_lo, w_hi;  // c fits 32 bits for tf <= 2 ... kept 64-bit via c_hi below
   uint32_t c_hi, pad0, pad1, pad2;
 };
-
-__device__ __forceinline__ float pair_score(int jaccard, float dot, float nq, float t) {
-  if (jaccard) {
-    const float den = nq + t - dot;
-    return den > 0.f ? __fdiv_rn(dot, den) : 0.f;
-  }
-  const float den = nq * t;
-  return den > 0.f ? __fdiv_rn(dot, __fsqrt_rn(den)) : 0.f;
-}
 
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(bar)), "r"(count));
@@ -720,14 +711,10 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
           float filt = __int_as_float(*(volatile int *)&P.gthr[q0 + qi]);
           if (*(volatile int *)&s_cnt[qi] == k) filt = fmaxf(filt, *(volatile float *)&s_lscore[qi * k + k - 1]);
           bool pass = true;
-          if (filt > 0.f) {
-            const float fq = P.jaccard ? filt * FILTER_SLACK : filt * filt * nq * FILTER_SLACK;
-            const float lhs = P.jaccard ? dot : dot * dot;
-            const float rhs = fq * (P.jaccard ? (nq + t - dot) : t);
-            pass = lhs >= rhs;
-          }
+          if (filt > 0.f) pass = dot * dot >= filt * filt * nq * FILTER_SLACK * t;
           if (pass) {
-            sc = pair_score(P.jaccard, dot, nq, t);
+            const float den = nq * t;
+            sc = den > 0.f ? __fdiv_rn(dot, __fsqrt_rn(den)) : 0.f;
             row = P.perm[pos0 + lane];
             cand = row != s_excl[qi] && sc >= filt;
           }

@@ -271,6 +271,17 @@ def test_pruned_scan_equals_exhaustive_scan(lib):
     # the tensor-core bounds leave only a small share of the (query, chunk) pairs to the exact scan
     assert 0 < lay["pairs_passed_bound"] < 0.2 * len(queries) * lay["chunks"], lay
     assert lay["pairs_scored"] >= lay["pairs_passed_bound"] and lay["records_written"] > 0
+    # without the stored bound codes, bound pass 1 recomputes the bounds to build the candidate lists: same results,
+    # and no pair passes that the codes (bounds rounded up to 1/250) would have dropped
+    os.environ["KAKVEDA_B200_BOUND_CODES"] = "0"
+    try:
+        s3, r3 = ix.topk(queries, k)
+        lay3 = ix.layout()
+    finally:
+        del os.environ["KAKVEDA_B200_BOUND_CODES"]
+    np.testing.assert_array_equal(r1, r3)
+    np.testing.assert_array_equal(s1, s3)
+    assert 0 < lay3["pairs_passed_bound"] <= lay["pairs_passed_bound"], (lay, lay3)
     os.environ["KAKVEDA_B200_NO_PRUNE"] = "1"
     try:
         s2, r2 = ix.topk(queries, k)
@@ -290,6 +301,46 @@ def test_pruned_scan_equals_exhaustive_scan(lib):
         np.testing.assert_allclose(s1[i], vals, rtol=RTOL32, atol=1e-7)
         for a, b in zip(order, r1[i].tolist()):
             assert a == b or full[a] == pytest.approx(full[b], rel=RTOL32)
+
+
+@pytest.mark.parametrize("bound_codes", ["1", "0"])
+def test_two_phase_batch_equals_one_phase_batch(lib, bound_codes):
+    """kv_topk_resident_seed + kv_index_raise_thresholds with the index's own k-th seed score + kv_topk_resident_finish
+    (the sharded step, on one index) returns bit for bit what kv_topk_resident does, with the bound codes kept and with
+    the recomputing bound pass 1."""
+    import os
+
+    import torch
+
+    from kakveda_b200 import GfkbIndex, synth
+
+    n, q, k = 300_000, 3000, 16
+    buf, off = synth.signatures_packed(synth.CORPUS_SEED, 0, n)
+    ix = GfkbIndex()
+    fb = ix.vocab.featurize_packed(buf, off, 0, grow=True)
+    ix.add_features(fb)
+    fb.close()
+    ix.finalize()
+    qfb = ix.vocab.featurize(synth.queries(q, n), grow=False)
+    ix.upload_queries(qfb)
+    qfb.close()
+    s1 = torch.empty((q, k), dtype=torch.float32, device="cuda")
+    r1 = torch.empty((q, k), dtype=torch.int64, device="cuda")
+    s2, r2 = torch.empty_like(s1), torch.empty_like(r1)
+    os.environ["KAKVEDA_B200_BOUND_CODES"] = bound_codes
+    try:
+        ix.topk_resident(k, s1.data_ptr(), r1.data_ptr())
+        ix.topk_resident_seed(k, s2.data_ptr(), r2.data_ptr())
+        kth = s2[:, k - 1].contiguous()
+        torch.cuda.synchronize()  # the index runs on its own stream
+        ix.raise_thresholds(kth.data_ptr(), q)
+        ix.topk_resident_finish(k, s2.data_ptr(), r2.data_ptr())
+    finally:
+        del os.environ["KAKVEDA_B200_BOUND_CODES"]
+    torch.cuda.synchronize()
+    assert torch.isfinite(kth).any()
+    np.testing.assert_array_equal(r1.cpu().numpy(), r2.cpu().numpy())
+    np.testing.assert_array_equal(s1.cpu().numpy(), s2.cpu().numpy())
 
 
 def test_query_batch_uploaded_as_slices_equals_whole_batch(lib):
