@@ -267,8 +267,10 @@ int kv_index_layout_load(kv_index *ix, const char *path);
  * the last query upload, [7] = tf-overflow entries, [8] = chunks (32 rows each), and for the last batch:
  * [9] = (query, chunk) pairs scored exactly (seed scan + candidate scan), [10] = candidate records scanned,
  * [11] = (query, chunk) pairs whose bound passed, [12] = candidate records written, [13] = kernels launched,
- * [14] = block entries of non-frequent features, [15] = candidate-pool pages used, [16] = pool pages allocated. */
-int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[17]);
+ * [14] = block entries of non-frequent features, [15] = candidate-pool pages used, [16] = pool pages allocated,
+ * [17] = second-class (query, feature) listings of the last query upload left out of their bound tile's dictionary
+ * (the bound kernel's epilogue adds those per block from the second-class bitmaps). */
+int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[18]);
 
 /* ------------------------------------------------------------------------------------
  * K2: dense-embedding cosine index (bf16 rows of `dim` elements, dim a multiple of 64) with the

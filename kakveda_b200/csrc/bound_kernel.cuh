@@ -15,8 +15,12 @@
 //     epilogue of block b -- this only computes BOUNDS; scores stay exact integer sums (K1b-S);
 //   * the next NF2 = 1024 features by chunk frequency ("second class": mid-frequency words and bigrams, each shared by
 //     many queries of a tile) are kept per 64-chunk block as two TRANSPOSED presence bitmaps Ubt[feature][tf >= 1,
-//     tf >= 2][64 chunk bits] (16 KB, one bulk-async copy per block, double buffered): a query thread reads ONE word per
-//     feature of its own list (<= Q2CAP) and has that feature's presence in its 16 chunk columns -- no atomics;
+//     tf >= 2][64 chunk bits].  A tile's queries list <= Q2CAP of them each; the KT2 = 256 most listed form the tile's
+//     dictionary (f2_dict_kernel) and are 256 more K of the same GEMM, into the same accumulators: A2 = the fp16
+//     weights (resident, TMA), B2 = 0 / 1 / T (T = largest tf rounded up to fp16) by the block's two bitmap rows of
+//     each column, built in shared memory by the MMA warpgroup after it has added the previous block into R.  A tile
+//     listing more than KT2 distinct ones leaves the least listed in the queries' lists: the epilogue adds those from
+//     the block's bitmap words in global memory (warps without such a feature skip that loop);
 //   * the remaining RARE features are joined the other way round: every 64-chunk block carries (built at finalize) a
 //     presence bitmap and an open-addressing table of its rare features (feature -> mask of the block's chunks holding
 //     it, largest tf); each query looks ITS OWN <= 32 rare features up -- one shared-memory bit test per (query,
@@ -43,6 +47,9 @@ namespace kvk {
 constexpr int B_BN = 64;                     // chunks per block = N of the MMA tile
 constexpr int B_BK = 64;                     // K slice: 64 fp16 = one 128-byte swizzle row
 constexpr int B_KSLICES = NF / B_BK;         // 4
+constexpr int B_KSLICES2 = KT2 / B_BK;       // 4: the second-class dictionary, one slice per warp of the MMA warpgroup
+// Wf2 [n_q_pad][KT2] goes through make_map_f16_nf, which maps rows of NF halves
+static_assert(KT2 == NF, "the dictionary's A operand shares the tensor-map shape of Wf");
 constexpr int B_STAGES = 2;
 constexpr int B_A_SLICE_BYTES = TILE_Q * B_BK * 2;  // 16 KiB: one K slice of the query operand
 constexpr int B_B_SLICE_BYTES = B_BN * B_BK * 2;    // 8 KiB: one K slice of the chunk operand
@@ -197,13 +204,14 @@ struct BoundParams {
   const uint32_t *ovf_vals;
   int n_ovf;
   int64_t n_chunks, n_q;
-  const uint2 *q3list;                                    // [n_tiles][Q3CAP][TILE_Q] rare (feature, fixed-point weight) lists
+  const uint32_t *q3id, *q3w;                             // [n_tiles][Q3CAP][TILE_Q] rare lists: feature, fixed-point weight
   const uint32_t *rbloom;                                 // [n_blocks][RB_BITS / 32]
   const uint32_t *rt_keys;                                // per-block rare tables: feature << 5 | largest tf (31: tfmax[])
   const unsigned long long *rt_masks;                     // ... chunks of the block holding the feature
   const uint32_t *rt_off, *rt_size;                       // [n_blocks]
   const uint32_t *tfmax;                                  // [V] largest tf of a feature (for entries whose 5-bit tf overflowed)
-  const uint2 *q2list;                                    // [n_tiles][Q2CAP][TILE_Q]
+  const uint32_t *d2col;                                  // [n_tiles][KT2] second-class dictionary (f2_dict_kernel)
+  const uint2 *q2list;                                    // [n_tiles][Q2CAP][TILE_Q] second-class features left out of it
   const uint32_t *ubt;                                    // [n_blocks][NF2][2][B_BN / 32]
   const float *q_nq, *q_dotS, *q_dotX, *q_corrS;          // [n_q] (sorted query order)
   const float *q_rscale;                                  // [n_q] 1 / s_q, a power of two: the unit of R's fixed point
@@ -221,14 +229,13 @@ struct BoundParams {
 
 struct __align__(1024) BoundSmem {
   unsigned char a[B_KSLICES][B_A_SLICE_BYTES];   // the tile's weight rows, resident
+  unsigned char a2[B_KSLICES2][B_A_SLICE_BYTES]; // the tile's weights of its second-class dictionary, resident
   unsigned char b[B_STAGES][B_B_SLICE_BYTES];    // chunk slices in flight
-  uint32_t ubt[2][NF2][2][B_BN / 32];            // second-class bitmaps (tf >= 1, tf >= 2) of the current / next block of chunks
-  uint32_t rbm[2][RB_BITS / 32];                 // rare-feature presence bitmap of the current / next block
-  uint32_t R[B_BN][TILE_Q];                      // frequent + rare part of the dot bound in units of 1 / s_q, [chunk][query]
-  uint2 q2[Q2CAP][TILE_Q];                       // the queries' second-class lists (bit row | (tfmax - 1) << 16, weight)
-  uint2 q3[Q3CAP][TILE_Q];                       // the queries' rare lists (feature id, fixed-point weight)
+  unsigned char b2[B_KSLICES2][B_B_SLICE_BYTES]; // the block's dictionary columns (0 / 1 / T), built by the MMA warpgroup
+  uint32_t rbm[RB_BITS / 32];                    // rare-feature presence bitmap of the block
+  uint32_t R[B_BN][TILE_Q];                      // the dot bound without the query constants, units of 1 / s_q, [chunk][query]
   float minB[2][B_BN];
-  uint64_t full_bar[B_STAGES], a_bar, blk_bar[2];
+  uint64_t full_bar[B_STAGES], a_bar, blk_bar;
   unsigned int lcount[4];
   int pages[1];  // [4][max_pages], sized at launch
 };
@@ -240,7 +247,8 @@ static inline size_t bound_smem_bytes(int max_pages) { return sizeof(BoundSmem) 
 // those three switches read from the parameters.
 template <bool FAST>
 __global__ void __launch_bounds__(B_THREADS, 1)
-tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_u, BoundParams P) {
+tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_w2,
+                   const __grid_constant__ CUtensorMap map_u, BoundParams P) {
   extern __shared__ unsigned char smem_raw[];
   const int pass = FAST ? 0 : P.pass;
   const bool has_codes = FAST ? true : (P.ubq != nullptr);
@@ -255,17 +263,10 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
   if (threadIdx.x == 0) {
     for (int i = 0; i < B_STAGES; i++) mbar_init(&S.full_bar[i], 1);
     mbar_init(&S.a_bar, 1);
-    mbar_init(&S.blk_bar[0], 1);
-    mbar_init(&S.blk_bar[1], 1);
+    mbar_init(&S.blk_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  {  // second-class and rare lists of the tile's queries, R = 0, list state
-    const uint4 *src2 = (const uint4 *)(P.q2list + (size_t)tile * Q2CAP * TILE_Q);
-    uint4 *dst2 = (uint4 *)&S.q2[0][0];
-    for (int i = threadIdx.x; i < Q2CAP * TILE_Q / 2; i += B_THREADS) dst2[i] = src2[i];
-    const uint4 *src3 = (const uint4 *)(P.q3list + (size_t)tile * Q3CAP * TILE_Q);
-    uint4 *dst3 = (uint4 *)&S.q3[0][0];
-    for (int i = threadIdx.x; i < Q3CAP * TILE_Q / 2; i += B_THREADS) dst3[i] = src3[i];
+  {  // R = 0, list state
     uint4 *r4 = (uint4 *)&S.R[0][0];
     for (int i = threadIdx.x; i < B_BN * TILE_Q / 4; i += B_THREADS) r4[i] = make_uint4(0u, 0u, 0u, 0u);
     for (int i = threadIdx.x; i < 4 * P.lists.max_pages; i += B_THREADS) S.pages[i] = -1;
@@ -274,25 +275,62 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
   __syncthreads();
 
   if (warp >= B_MMA_WARP) {
-    // ===== MMA warpgroup: frequent part of the block's bounds, added into R =====
+    // ===== MMA warpgroup: frequent and second-class part of the block's bounds, added into R =====
     // accumulator fragment of m64nNk16: warp w of the warpgroup holds rows 16 w + lane / 4 (+ 8) of each 64-query
     // half, register 4 j + e holds column 8 j + 2 (lane % 4) + (e & 1) of row + 8 (e >> 1)
     const int wq = warp - B_MMA_WARP;
     const bool producer = wq == 0 && lane == 0;
+    // 32-bit block and slice counters (fewer registers next to the 64 accumulators): the TMA coordinates are 32-bit
+    const int b0 = (int)blk_lo, n_blk = (int)(blk_hi - blk_lo);
     // chunk slices in global order g = (block - blk_lo) * B_KSLICES + slice; slice g goes to stage g % B_STAGES
-    const int64_t n_slices = (blk_hi - blk_lo) * B_KSLICES;
-    auto load_slice = [&](int64_t g) {
-      const int st = (int)(g % B_STAGES);
+    const int n_slices = n_blk * B_KSLICES;
+    auto load_slice = [&](int g) {
+      const int st = g % B_STAGES;
       mbar_expect_tx(&S.full_bar[st], B_B_SLICE_BYTES);
-      tma_load_2d(S.b[st], &map_u, &S.full_bar[st], (int)(g % B_KSLICES) * B_BK, (int)((blk_lo + g / B_KSLICES) * B_BN));
+      tma_load_2d(S.b[st], &map_u, &S.full_bar[st], (g % B_KSLICES) * B_BK, (b0 + g / B_KSLICES) * B_BN);
     };
     if (producer) {
-      mbar_expect_tx(&S.a_bar, B_KSLICES * B_A_SLICE_BYTES);
+      mbar_expect_tx(&S.a_bar, (B_KSLICES + B_KSLICES2) * B_A_SLICE_BYTES);
       for (int s = 0; s < B_KSLICES; s++) tma_load_2d(S.a[s], &map_w, &S.a_bar, s * B_BK, tile * TILE_Q);
-      for (int64_t g = 0; g < B_STAGES && g < n_slices; g++) load_slice(g);
+      for (int s = 0; s < B_KSLICES2; s++) tma_load_2d(S.a2[s], &map_w2, &S.a_bar, s * B_BK, tile * TILE_Q);
+      for (int g = 0; g < B_STAGES && g < n_slices; g++) load_slice(g);
+    }
+    // Second-class dictionary: thread t of the warpgroup owns columns 2 t, 2 t + 1 (warp wq: K slice wq).  Their
+    // 16-byte bitmap rows (tf >= 1, tf >= 2 over the block's 64 chunks) are loaded one block ahead into registers.
+    const uint32_t dc0 = P.d2col[(size_t)tile * KT2 + 2 * (wq * 32 + lane)];
+    const uint32_t dc1 = P.d2col[(size_t)tile * KT2 + 2 * (wq * 32 + lane) + 1];
+    uint4 u0 = make_uint4(0u, 0u, 0u, 0u), u1 = u0;
+    auto fetch_rows = [&](int i) {  // block blk_lo + i
+      const uint4 *src = reinterpret_cast<const uint4 *>(P.ubt) + (size_t)(b0 + i) * NF2;
+      if (dc0) u0 = __ldg(src + (dc0 & 0xFFFFu));  // dc == 0: unused column, stays 0
+      if (dc1) u1 = __ldg(src + (dc1 & 0xFFFFu));
+    };
+    // B2 (K-major like the chunk slices: chunk n's 128-byte row, 16-byte units swizzled by n % 8) = 0, 1 (fp16 0x3C00)
+    // or T: one 4-byte store per chunk, a warp's 32 stores fill one row (no bank conflicts)
+    auto build_b2 = [&]() {
+      unsigned char *dst = S.b2[wq] + (lane & 3) * 4;
+#pragma unroll
+      for (int n = 0; n < B_BN; n++) {
+        const uint32_t w1a = n < 32 ? u0.x : u0.y, w2a = n < 32 ? u0.z : u0.w;
+        const uint32_t w1b = n < 32 ? u1.x : u1.y, w2b = n < 32 ? u1.z : u1.w;
+        const uint32_t lo = (w2a >> (n & 31)) & 1u ? dc0 >> 16 : ((w1a >> (n & 31)) & 1u ? 0x3C00u : 0u);
+        const uint32_t hi = (w2b >> (n & 31)) & 1u ? dc1 >> 16 : ((w1b >> (n & 31)) & 1u ? 0x3C00u : 0u);
+        *reinterpret_cast<uint32_t *>(dst + n * 128 + ((((uint32_t)lane >> 2) ^ (uint32_t)(n & 7)) << 4)) = lo | hi << 16;
+      }
+    };
+    // generic-proxy stores of B2 -> visible to the wgmmas (async proxy) of every warp of the warpgroup
+    auto publish_b2 = [&]() {
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      asm volatile("bar.sync %0, 128;" ::"n"(B_BAR_MMA) : "memory");
+    };
+    if (n_blk > 0) {
+      fetch_rows(0);
+      build_b2();
+      if (n_blk > 1) fetch_rows(1);
+      publish_b2();
     }
     // refill the stage of slice g (read by every warp of the warpgroup: wgmma_wait done) with slice g + B_STAGES
-    auto release = [&](int64_t g) {
+    auto release = [&](int g) {
       asm volatile("bar.sync %0, 128;" ::"n"(B_BAR_MMA) : "memory");
       if (producer && g + B_STAGES < n_slices) load_slice(g + B_STAGES);
     };
@@ -309,13 +347,25 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
     mbar_wait_idle(&S.a_bar, 0);
     int stage = 0;
     uint32_t phase = 0;
-    int64_t it = 0, g = 0;
-    for (int64_t bk = blk_lo; bk < blk_hi; bk++, it++) {
+    int g = 0;
+    for (int it = 0; it < n_blk; it++) {
 #pragma unroll
       for (int h = 0; h < 2; h++)
 #pragma unroll
         for (int i = 0; i < 32; i++) wgmma_reg_fence(acc[h][i]);
       wgmma_fence();
+      // the second-class dictionary first: its operands are resident, so these issue while the chunk slices land
+#pragma unroll
+      for (int s = 0; s < B_KSLICES2; s++) {
+        const uint64_t db = wgmma_desc_sw128(S.b2[s]);
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          const uint64_t da = wgmma_desc_sw128(S.a2[s] + h * (B_A_SLICE_BYTES / 2));
+#pragma unroll
+          for (int kk = 0; kk < B_BK / 16; kk++)
+            wgmma_m64n64k16_f16(acc[h], da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), (uint32_t)((s | kk) != 0));
+        }
+      }
       for (int s = 0; s < B_KSLICES; s++, g++) {
         mbar_wait_idle(&S.full_bar[stage], phase);
         const uint64_t db = wgmma_desc_sw128(S.b[stage]);
@@ -324,7 +374,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
           const uint64_t da = wgmma_desc_sw128(S.a[s] + h * (B_A_SLICE_BYTES / 2));  // rows 64 h .. 64 h + 63
 #pragma unroll
           for (int kk = 0; kk < B_BK / 16; kk++)  // advance 32 bytes (2 x 16-byte units) per K=16 step inside the swizzle row
-            wgmma_m64n64k16_f16(acc[h], da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), (uint32_t)((s | kk) != 0));
+            wgmma_m64n64k16_f16(acc[h], da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), 1u);
         }
         wgmma_commit();
         if (s > 0) {  // the previous slice's group is done: its stage may be refilled
@@ -352,8 +402,14 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
         }
       }
       asm volatile("bar.arrive %0, %1;" ::"n"(B_BAR_RFULL), "n"(B_THREADS) : "memory");
+      // the GEMM of this block is done (wgmma_wait above): B2 takes the next block's columns
+      if (it + 1 < n_blk) {
+        build_b2();
+        if (it + 2 < n_blk) fetch_rows(it + 2);
+        publish_b2();
+      }
     }
-    if (it > 0) asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_RCLEAN), "n"(B_THREADS) : "memory");  // the last block's
+    if (n_blk > 0) asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_RCLEAN), "n"(B_THREADS) : "memory");  // the last block's
   } else {
     // ===== workers: join, then epilogue, per block =====
     const int qtr = warp & 3;   // quarter of the tile's queries = scan group of the tile
@@ -373,35 +429,41 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
 #pragma unroll
     for (int i = 0; i < B_SEEDS; i++) { sm[i] = -1.f; sc[i] = -1; }
     unsigned int n_pairs = 0, n_recs = 0;
-    // per-block side data (second-class bitmaps + rare presence bitmap): bulk-async copies, double buffered -- block
-    // b + 1 is fetched while block b is processed
-    auto fetch_block = [&](int64_t bk2, int buf) {
-      mbar_expect_tx(&S.blk_bar[buf], (uint32_t)(sizeof(S.ubt[0]) + sizeof(S.rbm[0])));
-      bulk_copy_g2s(&S.ubt[buf][0][0][0], P.ubt + (size_t)bk2 * (sizeof(S.ubt[0]) / 4), sizeof(S.ubt[0]), &S.blk_bar[buf]);
-      bulk_copy_g2s(&S.rbm[buf][0], P.rbloom + (size_t)bk2 * (RB_BITS / 32), sizeof(S.rbm[0]), &S.blk_bar[buf]);
+    // the rare join's thread = (query jq, quarter `part` of its rare list): the list's feature ids stay in registers
+    constexpr int NR = Q3CAP / 4;  // list entries of a thread
+    const int jq = threadIdx.x & (TILE_Q - 1), part = threadIdx.x >> 7;  // 512 worker threads = 128 queries x 4
+    const size_t q3o = (size_t)tile * Q3CAP * TILE_Q + (size_t)part * TILE_Q + jq;  // entry part + 4 k: + 4 k TILE_Q
+    uint32_t fid[NR];
+#pragma unroll
+    for (int k = 0; k < NR; k++) fid[k] = P.q3id[q3o + (size_t)k * 4 * TILE_Q];  // FID_NONE past the end of the list
+    // rare presence bitmap of the block: one bulk-async copy, issued for block b + 1 as soon as the join of block b has
+    // read the buffer (after the RFULL barrier); it lands while block b's epilogue runs
+    auto fetch_bitmap = [&](int64_t bk2) {
+      mbar_expect_tx(&S.blk_bar, (uint32_t)sizeof(S.rbm));
+      bulk_copy_g2s(&S.rbm[0], P.rbloom + (size_t)bk2 * (RB_BITS / 32), sizeof(S.rbm), &S.blk_bar);
     };
-    if (threadIdx.x == 0 && blk_lo < blk_hi) fetch_block(blk_lo, 0);
+    if (threadIdx.x == 0 && blk_lo < blk_hi) fetch_bitmap(blk_lo);
+    // second-class features of the warp's queries left out of the tile's dictionary (only tiles listing more than KT2
+    // distinct ones): added per block from the bitmaps in global memory; most warps have none and skip the loop
+    const uint2 *ql2 = P.q2list + (size_t)tile * Q2CAP * TILE_Q + qi;
+    const bool warp_left = __any_sync(FULL, q_ok && __uint_as_float(ql2[0].y) > 0.f);
     int64_t it = 0;
     for (int64_t bk = blk_lo; bk < blk_hi; bk++, it++) {
       const int as = (int)(it & 1);
-      const uint32_t aphase = (uint32_t)((it >> 1) & 1);
       const int64_t c0 = bk * B_BN;
-      if (threadIdx.x == 0 && bk + 1 < blk_hi) fetch_block(bk + 1, as ^ 1);  // its buffers were last read two barriers ago
-      mbar_wait(&S.blk_bar[as], aphase);
+      mbar_wait(&S.blk_bar, (uint32_t)(it & 1));
       // ---- rare join, inverted: thread (query, quarter of its rare list) tests each feature in the block's presence
       //      bitmap; on a hit it probes the block's table (L2) and adds weight x tf to R[chunk][query] for every chunk
       //      of the mask.  Rows are text-sorted, so one feature can sit in most chunks of a block: R is dense.
       //      Three phases, each issuing all of its loads before it consumes one (bitmap bits, first-slot keys of the
-      //      hits, masks of the found keys): one or two L2 latencies per thread and block rather than two per hit. ----
+      //      hits, masks and weights of the found keys): one or two L2 latencies per thread and block rather than two
+      //      per hit. ----
       {
-        constexpr int NR = Q3CAP / 4;  // list entries of a thread
-        const int jq = threadIdx.x & (TILE_Q - 1), part = threadIdx.x >> 7;  // 512 worker threads = 128 queries x 4
-        const uint32_t *bm = S.rbm[as];
+        const uint32_t *bm = S.rbm;
         const uint32_t tsize = P.rt_size[bk], toff = P.rt_off[bk];
-        uint32_t fid[NR], h[NR], key[NR];
+        uint32_t h[NR], key[NR];
 #pragma unroll
         for (int k = 0; k < NR; k++) {
-          fid[k] = S.q3[part + 4 * k][jq].x;  // FID_NONE past the end of the list (padding queries: all ones)
           const uint32_t bb = rb_bit(fid[k]);
           const bool hit = fid[k] < FID_NONE && ((bm[bb >> 5] >> (bb & 31u)) & 1u);
           h[k] = rt_slot(fid[k], tsize);
@@ -414,17 +476,18 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
             key[k] = __ldg(P.rt_keys + toff + h[k]);
           }
         unsigned long long cm[NR];
-        uint32_t tf[NR];
+        uint32_t tf[NR], w[NR];
 #pragma unroll
         for (int k = 0; k < NR; k++) {
           const bool found = key[k] != KEY_EMPTY;
           cm[k] = found ? __ldg(P.rt_masks + toff + h[k]) : 0ull;
+          w[k] = found ? __ldg(P.q3w + q3o + (size_t)k * 4 * TILE_Q) : 0u;
           tf[k] = key[k] & 31u;
           if (found && tf[k] == TF_OVF) tf[k] = __ldg(P.tfmax + fid[k]);
         }
 #pragma unroll
         for (int k = 0; k < NR; k++) {
-          const uint32_t x = S.q3[part + 4 * k][jq].y * tf[k];  // fixed point, <= 2^30 + tf (prep_queries_kernel)
+          const uint32_t x = w[k] * tf[k];  // fixed point, <= 2^30 + tf (prep_queries_kernel)
           for (unsigned long long m = cm[k]; m; m &= m - 1) atomicAdd(&S.R[__ffsll((long long)m) - 1][jq], x);
         }
       }
@@ -435,35 +498,39 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
         const float th = __int_as_float(__ldcg(&P.gthr[slot]));
         if (th > 0.f) tq = th * th * nq / (PRUNE_SLACK * PRUNE_SLACK);
       }
-      // R complete: the workers' rare join and the MMA warpgroup's frequent part of this block
+      // R complete: the workers' rare join and the MMA warpgroup's frequent + second-class part of this block
       asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_RFULL), "n"(B_THREADS) : "memory");
-      // ---- epilogue, thread = query, B_COLS chunk columns: rare + frequent part (R) + second-class part (bitmaps)
-      //      -> bound -> seed / candidate ----
+      if (threadIdx.x == 0 && bk + 1 < blk_hi) fetch_bitmap(bk + 1);  // every join has read this block's bitmap
+      // ---- epilogue, thread = query, B_COLS chunk columns: R + second-class features outside the dictionary -> bound
+      //      -> seed / candidate ----
       float x[B_COLS];
       {
         uint32_t *Rcol = &S.R[cs * B_COLS][qi];
 #pragma unroll
         for (int j = 0; j < B_COLS; j++) { x[j] = __uint2float_ru(Rcol[j * TILE_Q]) * rs; Rcol[j * TILE_Q] = 0u; }
       }
-      const uint32_t bsh = (uint32_t)((cs * B_COLS) & 31), bword = (uint32_t)((cs * B_COLS) >> 5);
-      constexpr uint32_t CMASK = B_COLS == 32 ? 0xFFFFFFFFu : ((1u << B_COLS) - 1u);
+      if (warp_left) {
+        const uint32_t bsh = (uint32_t)((cs * B_COLS) & 31), bword = (uint32_t)((cs * B_COLS) >> 5);
+        constexpr uint32_t CMASK = B_COLS == 32 ? 0xFFFFFFFFu : ((1u << B_COLS) - 1u);
+        const uint32_t *ub = P.ubt + (size_t)bk * NF2 * 4 + bword;  // [feature][tf >= 1, tf >= 2][2 words]
 #pragma unroll 1
-      for (int i = 0; i < Q2CAP; i++) {
-        const uint2 f2 = S.q2[i][qi];
-        const float w2 = q_ok ? __uint_as_float(f2.y) : 0.f;
-        if (!__any_sync(FULL, w2 > 0.f)) break;  // the lists are filled from the front
-        const uint32_t row2 = f2.x & 0xFFFFu, tm1 = f2.x >> 16;
-        const uint32_t m = w2 > 0.f ? ((S.ubt[as][row2][0][bword] >> bsh) & CMASK) : 0u;
-        if (m) {
-#pragma unroll
-          for (int j = 0; j < B_COLS; j++)
-            if ((m >> j) & 1u) x[j] += w2;
-          const uint32_t mm = tm1 ? ((S.ubt[as][row2][1][bword] >> bsh) & CMASK) : 0u;  // tf >= 2 there: up to tfmax - 1 more
-          if (mm) {
-            const float wex = __fmul_ru(w2, (float)tm1);
+        for (int i = 0; i < Q2CAP; i++) {
+          const uint2 f2 = __ldg(ql2 + (size_t)i * TILE_Q);
+          const float w2 = q_ok ? __uint_as_float(f2.y) : 0.f;
+          if (!__any_sync(FULL, w2 > 0.f)) break;  // the lists are filled from the front
+          const uint32_t row2 = f2.x & 0xFFFFu, tm1 = f2.x >> 16;
+          const uint32_t m = w2 > 0.f ? ((__ldg(ub + row2 * 4) >> bsh) & CMASK) : 0u;
+          if (m) {
 #pragma unroll
             for (int j = 0; j < B_COLS; j++)
-              if ((mm >> j) & 1u) x[j] += wex;
+              if ((m >> j) & 1u) x[j] += w2;
+            const uint32_t mm = tm1 ? ((__ldg(ub + row2 * 4 + 2) >> bsh) & CMASK) : 0u;  // tf >= 2: up to tfmax - 1 more
+            if (mm) {
+              const float wex = __fmul_ru(w2, (float)tm1);
+#pragma unroll
+              for (int j = 0; j < B_COLS; j++)
+                if ((mm >> j) & 1u) x[j] += wex;
+            }
           }
         }
       }
@@ -504,7 +571,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
         *reinterpret_cast<uint4 *>(P.ubq + (size_t)slot * P.ubq_stride + cbase) = make_uint4(codes[0], codes[1], codes[2], codes[3]);
       // four warps (one per chunk-column quarter) share the group's list
       if (pass == 1) list_append(P.lists, list, &S.lcount[qtr], my_pages, (uint32_t)(cbase + lane), mymask, n_pairs, n_recs);
-      // R is clean again (the MMA warpgroup may add the next block) and every reader of this block's side data is done
+      // R is clean again: the MMA warpgroup and, once all workers are here, the next block's join may add to it
       asm volatile("bar.arrive %0, %1;" ::"n"(B_BAR_RCLEAN), "n"(B_THREADS) : "memory");
       asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_WORKERS), "n"(B_WORKERS * 32) : "memory");
     }

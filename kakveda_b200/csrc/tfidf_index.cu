@@ -110,9 +110,11 @@ struct kv_index {
   DevBuf<uint8_t> d_flags;
   DevBuf<float> d_qconst;     // 7 * n_q: nq, dotU, corrU, dotS, corrS, dotX, 1 / s_q (fixed-point unit of the bound kernel's R)
   DevBuf<unsigned char> d_qtab;
-  DevBuf<uint2> d_q2list, d_q3list;
-  DevBuf<__half> d_Wf;
-  CUtensorMap map_w;
+  DevBuf<uint2> d_q2list;
+  DevBuf<uint32_t> d_q3id, d_q3w, d_d2col;  // rare lists (feature, weight); second-class dictionary of each tile
+  DevBuf<__half> d_Wf, d_Wf2;
+  DevBuf<unsigned long long> d_f2out;       // second-class listings left out of their tile's dictionary
+  CUtensorMap map_w, map_w2;
   DevBuf<int> d_gthr;
   // candidate lists of a batch
   DevBuf<int> d_seeds;
@@ -142,7 +144,7 @@ struct kv_index {
 
   // query batch currently resident on the device (kv_query_upload / first half of kv_topk)
   bool batch_valid = false;
-  int64_t batch_q = 0, batch_tiles = 0, batch_h2d_bytes = 0, batch_null = 0;
+  int64_t batch_q = 0, batch_tiles = 0, batch_h2d_bytes = 0, batch_null = 0, batch_f2_outside = 0;
   std::vector<int64_t> irr_q, irr_indptr;
   std::vector<uint32_t> irr_ids, irr_tf;
   std::vector<double> irr_oov;
@@ -332,14 +334,14 @@ void kv_index_destroy(kv_index *ix) {
   ix->d_B32.release(); ix->d_cminB.release(); ix->d_univ.release(); ix->d_perm.release(); ix->d_invperm.release();
   ix->d_blk.release(); ix->d_binfo.release(); ix->d_Uf.release(); ix->d_fslot.release(); ix->d_fslot2.release(); ix->d_ubt.release();
   ix->d_rbloom.release(); ix->d_rt_keys.release(); ix->d_rt_off.release(); ix->d_rt_size.release(); ix->d_rt_masks.release();
-  ix->d_q2list.release(); ix->d_q3list.release();
+  ix->d_q2list.release(); ix->d_q3id.release(); ix->d_q3w.release(); ix->d_d2col.release(); ix->d_f2out.release();
   ix->d_ovf_keys.release(); ix->d_ovf_vals.release();
   ix->d_rq_indptr.release(); ix->d_rq_ids.release(); ix->d_rq_tf.release(); ix->d_rq_const.release(); ix->d_rq_out.release();
   ix->d_rq_rows.release();
   ix->h_q_indptr.release(); ix->h_q_ids.release(); ix->h_q_tf.release(); ix->h_q_oov.release(); ix->h_qperm.release();
   ix->h_flags.release();
   ix->d_q_indptr.release(); ix->d_q_ids.release(); ix->d_q_tf.release(); ix->d_q_oov.release(); ix->d_qperm.release();
-  ix->d_flags.release(); ix->d_qconst.release(); ix->d_qtab.release(); ix->d_Wf.release();
+  ix->d_flags.release(); ix->d_qconst.release(); ix->d_qtab.release(); ix->d_Wf.release(); ix->d_Wf2.release();
   ix->d_gthr.release();
   ix->d_seeds.release(); ix->d_direct.release(); ix->d_pool.release(); ix->d_list_count.release(); ix->d_list_pages.release();
   ix->d_pool_ctl.release(); ix->d_ubq.release();
@@ -917,7 +919,11 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   KV_CUDA(ix->d_qtab.ensure(n_q * (int64_t)QTAB_BYTES));
   KV_CUDA(ix->d_Wf.ensure(n_q_pad * NF));
   KV_CUDA(ix->d_q2list.ensure(n_q_pad * Q2CAP));
-  KV_CUDA(ix->d_q3list.ensure(n_q_pad * Q3CAP));
+  KV_CUDA(ix->d_q3id.ensure(n_q_pad * Q3CAP));
+  KV_CUDA(ix->d_q3w.ensure(n_q_pad * Q3CAP));
+  KV_CUDA(ix->d_Wf2.ensure(n_q_pad * KT2));
+  KV_CUDA(ix->d_d2col.ensure(n_tiles * KT2));
+  KV_CUDA(ix->d_f2out.ensure(1));
   KV_CUDA(cudaEventRecord(ix->ev[0], s));
   KV_CUDA(cudaMemcpyAsync(ix->d_q_indptr.p, ix->h_q_indptr.p, (size_t)(n_q + 1) * 8, cudaMemcpyHostToDevice, s));
   if (nnz) {
@@ -930,9 +936,12 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   KV_CUDA(cudaEventRecord(ix->ev[1], s));
   // ---- device: per-query constants and tables, per-tile rare-feature tables ----
   KV_CUDA(cudaMemsetAsync(ix->d_Wf.p, 0, (size_t)n_q_pad * NF * sizeof(__half), s));
+  KV_CUDA(cudaMemsetAsync(ix->d_Wf2.p, 0, (size_t)n_q_pad * KT2 * sizeof(__half), s));
+  KV_CUDA(cudaMemsetAsync(ix->d_f2out.p, 0, sizeof(unsigned long long), s));
   // the lists of the padding queries of the last tile must be empty (weight 0 / no feature)
   KV_CUDA(cudaMemsetAsync(ix->d_q2list.p, 0, (size_t)n_q_pad * Q2CAP * sizeof(uint2), s));
-  KV_CUDA(cudaMemsetAsync(ix->d_q3list.p, 0xFF, (size_t)n_q_pad * Q3CAP * sizeof(uint2), s));
+  KV_CUDA(cudaMemsetAsync(ix->d_q3id.p, 0xFF, (size_t)n_q_pad * Q3CAP * sizeof(uint32_t), s));
+  KV_CUDA(cudaMemsetAsync(ix->d_q3w.p, 0, (size_t)n_q_pad * Q3CAP * sizeof(uint32_t), s));
   PrepParams P;
   P.q_indptr = ix->d_q_indptr.p; P.q_ids = ix->d_q_ids.p; P.q_tf = ix->d_q_tf.p; P.q_oov = ix->d_q_oov.p;
   P.qsrc = ix->d_qperm.p + 2 * n_q; P.flags = ix->d_flags.p;
@@ -943,14 +952,22 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   P.fslot = ix->d_fslot.p; P.fslot2 = ix->d_fslot2.p; P.q2list = ix->d_q2list.p; P.jaccard = ix->jaccard; P.corpus_fit = ix->corpus_fit;
   P.q_nq = ix->d_qconst.p; P.q_dotU = P.q_nq + n_q; P.q_corrU = P.q_nq + 2 * n_q; P.q_dotS = P.q_nq + 3 * n_q;
   P.q_corrS = P.q_nq + 4 * n_q; P.q_dotX = P.q_nq + 5 * n_q; P.q_rscale = P.q_nq + 6 * n_q;
-  P.qtab = ix->d_qtab.p; P.Wf = ix->d_Wf.p; P.q3list = ix->d_q3list.p;
+  P.qtab = ix->d_qtab.p; P.Wf = ix->d_Wf.p; P.q3id = ix->d_q3id.p; P.q3w = ix->d_q3w.p;
   prep_queries_kernel<<<(unsigned)((n_q + 127) / 128), 128, 0, s>>>(P);
+  KV_CUDA(cudaGetLastError());
+  DictParams DP;
+  DP.q2list = ix->d_q2list.p; DP.Wf2 = ix->d_Wf2.p; DP.d2col = ix->d_d2col.p; DP.n_outside = ix->d_f2out.p;
+  f2_dict_kernel<<<(unsigned)n_tiles, DICT_THREADS, 0, s>>>(DP);
   KV_CUDA(cudaGetLastError());
   {
     int rc = make_map_f16_nf(&ix->map_w, ix->d_Wf.p, n_q_pad, TILE_Q);
+    if (rc == KV_OK) rc = make_map_f16_nf(&ix->map_w2, ix->d_Wf2.p, n_q_pad, TILE_Q);  // KT2 == NF columns
     if (rc != KV_OK) return rc;
   }
+  unsigned long long f2_out = 0;
+  KV_CUDA(cudaMemcpyAsync(&f2_out, ix->d_f2out.p, sizeof(f2_out), cudaMemcpyDeviceToHost, s));
   KV_CUDA(cudaStreamSynchronize(s));  // the pinned staging buffers may be rewritten by the next call
+  ix->batch_f2_outside = (int64_t)f2_out;
   ix->batch_q = n_q;
   ix->batch_tiles = n_tiles;
   ix->batch_null = n_null;
@@ -1016,7 +1033,7 @@ static int run_pruned(kv_index *ix, Batch &b) {
   BoundParams BP;
   BP.blk = ix->d_blk.p; BP.binfo = ix->d_binfo.p; BP.chunk_minB = ix->d_cminB.p;
   BP.ovf_keys = ix->d_ovf_keys.p; BP.ovf_vals = ix->d_ovf_vals.p; BP.n_ovf = ix->n_ovf;
-  BP.n_chunks = ix->n_chunks; BP.n_q = n_q; BP.q2list = ix->d_q2list.p; BP.q3list = ix->d_q3list.p; BP.ubt = ix->d_ubt.p;
+  BP.n_chunks = ix->n_chunks; BP.n_q = n_q; BP.q3id = ix->d_q3id.p; BP.q3w = ix->d_q3w.p; BP.d2col = ix->d_d2col.p; BP.q2list = ix->d_q2list.p; BP.ubt = ix->d_ubt.p;
   BP.rbloom = ix->d_rbloom.p; BP.rt_keys = ix->d_rt_keys.p; BP.rt_masks = ix->d_rt_masks.p; BP.rt_off = ix->d_rt_off.p;
   BP.rt_size = ix->d_rt_size.p; BP.tfmax = ix->d_tfmax.p;
   BP.q_nq = qc; BP.q_dotS = qc + 3 * n_q; BP.q_corrS = qc + 4 * n_q; BP.q_dotX = qc + 5 * n_q; BP.q_rscale = qc + 6 * n_q;
@@ -1034,9 +1051,9 @@ static int run_pruned(kv_index *ix, Batch &b) {
     BP.pass = 0;
     // the headline configuration (bound codes kept, no test hook) runs the specialised instantiation
     if (BP.ubq && !BP.dbg_xs && !getenv("KAKVEDA_B200_GENERIC_BOUND"))
-      tfidf_bound_kernel<true><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_u, BP);
+      tfidf_bound_kernel<true><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_w2, ix->map_u, BP);
     else
-      tfidf_bound_kernel<false><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_u, BP);
+      tfidf_bound_kernel<false><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_w2, ix->map_u, BP);
     KV_CUDA(cudaGetLastError());
     seeds_to_lists_kernel<<<(unsigned)((b.n_groups * GROUP_Q * b.n_seed + 255) / 256), 256, 0, s>>>(
         ix->d_seeds.p, n_q, b.n_seed, ix->d_direct.p, ix->d_list_count.p);
@@ -1062,7 +1079,7 @@ static int run_pruned(kv_index *ix, Batch &b) {
     tfidf_select_kernel<<<dim3((unsigned)b.n_groups, (unsigned)b.n_bsplits), SEL_WARPS * 32, (size_t)b.max_pages * sizeof(int), s>>>(LP);
   } else {
     BP.pass = 1;
-    tfidf_bound_kernel<false><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_u, BP);
+    tfidf_bound_kernel<false><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_w2, ix->map_u, BP);
   }
   KV_CUDA(cudaGetLastError());
   KV_CUDA(cudaEventRecord(ix->evk[3], s));
@@ -1652,7 +1669,7 @@ int kv_index_last_score_ms(const kv_index *ix, float *ms) {
   return KV_OK;
 }
 
-int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[17]) {
+int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[18]) {
   if (!ix || !bytes || !counts) return kv_fail(KV_ERR_INVALID, "kv_index_layout: bad arguments");
   bytes[0] = ix->blk_words * 4;
   bytes[1] = ix->n_rows * 4;
@@ -1671,6 +1688,7 @@ int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[17]) {
   counts[14] = ix->n_rare_entries;
   counts[15] = (int64_t)(ix->last_stats[6] & 0xFFFFFFFFull);  // pool pages used
   counts[16] = ix->pool_pages;
+  counts[17] = ix->batch_f2_outside;  // second-class (query, feature) listings of the batch left out of their tile's dictionary
   return KV_OK;
 }
 

@@ -42,6 +42,7 @@ constexpr int CHUNK_ROWS = 32;
 constexpr int NF = 256;   // features evaluated densely (tensor cores) by the bound kernel
 constexpr int NF2 = 1024; // the next most frequent features: per 64-chunk block two transposed bitmaps [NF2][tf >= 1, tf >= 2][64 bits]
 constexpr int Q2CAP = 24; // features of that class a query keeps in its own list (further ones are treated as rare)
+constexpr int KT2 = 256;  // columns of a bound tile's second-class dictionary (extra K of the bound GEMM)
 constexpr uint32_t FID_BITS = 26;
 constexpr uint32_t FID_MASK = (1u << FID_BITS) - 1;
 constexpr uint32_t FID_NONE = FID_MASK;  // sentinel feature id (never in a table)
@@ -325,7 +326,7 @@ struct PrepParams {
   float *q_rscale;          // [n_q] 1 / s_q: fixed-point unit of the bound kernel's accumulator R (see below)
   unsigned char *qtab;      // [n_q][QTAB_BYTES]
   __half *Wf;               // [n_q_pad][NF], zeroed by the caller
-  uint2 *q3list;            // [n_tiles][Q3CAP][TILE_Q] (rare feature id, weight ceil(tf_q a(t) s_q) as an integer)
+  uint32_t *q3id, *q3w;     // [n_tiles][Q3CAP][TILE_Q] rare feature id, weight ceil(tf_q a(t) s_q) as an integer
   uint2 *q2list;            // [n_tiles][Q2CAP][TILE_Q] (bit row | (tfmax(t) - 1) << 16, weight tf_q a(t) as float bits)
 };
 
@@ -343,11 +344,13 @@ __global__ void prep_queries_kernel(PrepParams P) {
   const bool regular = P.flags[i] == 0;
   uint2 *q2 = P.q2list + ((size_t)(i / TILE_Q) * Q2CAP) * TILE_Q + (i % TILE_Q);
   for (int j = 0; j < Q2CAP; j++) q2[(size_t)j * TILE_Q] = make_uint2(0u, 0u);
-  uint2 *q3 = P.q3list + ((size_t)(i / TILE_Q) * Q3CAP) * TILE_Q + (i % TILE_Q);
-  for (int j = 0; j < Q3CAP; j++) q3[(size_t)j * TILE_Q] = make_uint2(FID_NONE, 0u);
+  const size_t q3o = ((size_t)(i / TILE_Q) * Q3CAP) * TILE_Q + (i % TILE_Q);
+  uint32_t *q3id = P.q3id + q3o, *q3w = P.q3w + q3o;
+  for (int j = 0; j < Q3CAP; j++) { q3id[(size_t)j * TILE_Q] = FID_NONE; q3w[(size_t)j * TILE_Q] = 0u; }
   int c3 = 0;
   float dotX = 0.f;
-  double xmax = 0.0;  // upper bound of what the bound kernel sums into R for this query: frequent and listed rare terms
+  double xmax = 0.0;  // upper bound of what the bound kernel sums into R for this query: frequent, listed second-class
+                      // and listed rare terms
   for (int64_t p = P.q_indptr[q]; p < P.q_indptr[q + 1]; p++) {
     const uint32_t t = P.q_ids[p];
     const double f = (double)P.q_tf[p];
@@ -377,11 +380,17 @@ __global__ void prep_queries_kernel(PrepParams P) {
         xmax += (double)__half2float(wf) * tm;
       } else if (P.fslot2[t] != 0xFFFFu && c2 < P.q2cap) {
         const uint32_t tm1 = min(P.tfmax[t] - 1u, 65535u);  // weight of the 'tf >= 2' plane: (largest tf - 1) more times
-        q2[(size_t)c2 * TILE_Q] = make_uint2((uint32_t)P.fslot2[t] | (tm1 << 16), __float_as_uint(__double2float_ru(f * a * (1.0 + 1e-6))));
+        const float w2 = __double2float_ru(f * a * (1.0 + 1e-6));
+        q2[(size_t)c2 * TILE_Q] = make_uint2((uint32_t)P.fslot2[t] | (tm1 << 16), __float_as_uint(w2));
+        // what a column of the tile's dictionary adds to R (f2_dict_kernel): fp16 weight x fp16 largest tf, both rounded
+        // up (a largest tf beyond the fp16 range never takes a column)
+        const float th = __half2float(__float2half_ru((float)(tm1 + 1u)));
+        if (isfinite(th)) xmax += (double)__half2float(__float2half_ru(w2)) * (double)th;
         c2++;
       } else if (P.fslot2[t] == 0xFFFFu && c3 < Q3CAP) {  // rare: looked up per block of chunks by the bound kernel
         const float w3 = __double2float_ru(f * a * (1.0 + 1e-6));
-        q3[(size_t)c3 * TILE_Q] = make_uint2(t, __float_as_uint(w3));  // scaled to an integer below, once s_q is known
+        q3id[(size_t)c3 * TILE_Q] = t;
+        q3w[(size_t)c3 * TILE_Q] = __float_as_uint(w3);  // scaled to an integer below, once s_q is known
         xmax += (double)w3 * tm;
         c3++;
       } else {  // no list slot left: assumed present in every chunk with its largest tf (a valid, loose bound)
@@ -389,19 +398,23 @@ __global__ void prep_queries_kernel(PrepParams P) {
       }
     }
   }
-  // Fixed-point scale of R (the bound kernel's frequent + rare part, summed with integer shared atomics): s_q = 2^(30 - e)
-  // with xmax < 2^e, so xmax s_q <= 2^30, and a power of two, so scaling is exact.  No wrap: R[chunk][query] is one
-  // MMA term ceil(acc s_q) plus at most Q3CAP rare terms w3 tf with w3 = ceil(weight s_q) <= weight s_q + 1.  The
-  // accumulator acc is the fp32 tensor-core sum of fp16 weights times the chunk's largest tf (fp16, within 2^-11 of
-  // it), and every tf is at most tfmax(t) <= 65535, so R <= 1.001 xmax s_q + 1 + Q3CAP 65535 < 2^31.  A wrapped sum
-  // would LOWER a bound and pruning would drop rows.  xmax < 2^31 for a regular query (classify_queries) and 0 for the
-  // others, so s_q and 1 / s_q are normal floats.
+  // Fixed-point scale of R (the bound kernel's frequent + second-class + rare part, summed with integer shared atomics):
+  // s_q = 2^(30 - e) with xmax < 2^e, so xmax s_q <= 2^30, and a power of two, so scaling is exact.  No wrap:
+  // R[chunk][query] is one MMA term ceil(acc s_q) plus at most Q3CAP rare terms w3 tf with w3 = ceil(weight s_q) <=
+  // weight s_q + 1.  The accumulator acc is the fp32 tensor-core sum of fp16 weights times fp16 B values: the chunk's
+  // largest tf (frequent features, within 2^-11 of it) or 0 / 1 / the feature's largest tf rounded up to fp16 (the
+  // tile's second-class dictionary), each product counted in xmax above with both factors as the GEMM sees them.  A
+  // query lists only a subset of its second-class features in the dictionary, so acc <= 1.001 xmax; every tf is at
+  // most tfmax(t) <= 65535, so R <= 1.001 xmax s_q + 1 + Q3CAP 65535 < 2^31.  A wrapped sum would LOWER a bound and
+  // pruning would drop rows.  xmax < 2^31 for a regular query (classify_queries bounds the sum over every non-universal
+  // feature, s_dot amax < 2^30, and fp16 rounding adds at most 2^-10 to each product) and 0 for the others, so s_q
+  // and 1 / s_q are normal floats.
   int e = 0;
   frexp(xmax, &e);
   const double s_q = ldexp(1.0, 30 - e);
   for (int j = 0; j < c3; j++) {
-    uint2 &r = q3[(size_t)j * TILE_Q];
-    r.y = (uint32_t)ceil((double)__uint_as_float(r.y) * s_q);  // <= xmax s_q: fits
+    uint32_t &w = q3w[(size_t)j * TILE_Q];
+    w = (uint32_t)ceil((double)__uint_as_float(w) * s_q);  // <= xmax s_q: fits
   }
   P.q_rscale[i] = (float)ldexp(1.0, e - 30);
   P.q_nq[i] = regular ? (float)nq : 0.f;  // nq == 0 switches the query off in the kernels
@@ -410,6 +423,84 @@ __global__ void prep_queries_kernel(PrepParams P) {
   P.q_dotS[i] = __double2float_ru(dotU * (1.0 + 1e-6));  // bounds may only err upwards
   P.q_corrS[i] = __double2float_rd(corrU + corrS);       // ... and their denominators downwards
   P.q_dotX[i] = dotX;
+}
+
+// ----------------------------------------------------------------------------------------
+// second-class dictionary of a bound tile (after prep_queries_kernel): the KT2 bit rows most listed by the tile's 128
+// queries (count descending, lower row first: deterministic) become extra K columns of the bound GEMM.  Per column the
+// bit row and T = the feature's largest tf rounded up to fp16 (the bound kernel's B value is 0, 1 or T by the block's
+// tf >= 1 / tf >= 2 bitmaps); per query its fp16 weight, rounded up, in the A operand Wf2.  The listed features left
+// out (only tiles with more than KT2 distinct ones) stay in the query's list, moved to its front: the bound kernel's
+// epilogue adds them from the block's bitmaps, as exactly as a dictionary column would.
+// ----------------------------------------------------------------------------------------
+struct DictParams {
+  uint2 *q2list;                  // [n_tiles][Q2CAP][TILE_Q]; on return only the features left out of the dictionary
+  __half *Wf2;                    // [n_q_pad][KT2], zeroed by the caller
+  uint32_t *d2col;                // [n_tiles][KT2] bit row | fp16 bits of T << 16; 0: unused column
+  unsigned long long *n_outside;  // listed (query, feature) incidences left out of their tile's dictionary
+};
+
+constexpr int DICT_THREADS = 256;
+
+__global__ void __launch_bounds__(DICT_THREADS) f2_dict_kernel(DictParams P) {
+  __shared__ uint32_t cnt[NF2];     // listings of each bit row in the tile
+  __shared__ uint16_t th[NF2];      // fp16 bits of T of each listed row
+  __shared__ int16_t col_of[NF2];   // column of a row, -1: none
+  __shared__ uint32_t keys[NF2];    // listed rows, count << 10 | (NF2 - 1 - row): a larger key ranks first
+  __shared__ uint32_t colw[KT2];
+  __shared__ uint32_t n_keys;
+  __shared__ unsigned int n_out;
+  static_assert(NF2 == 1024 && Q2CAP * TILE_Q < (1 << 22), "dictionary key packing");
+  const int tile = blockIdx.x;
+  for (int r = threadIdx.x; r < NF2; r += DICT_THREADS) { cnt[r] = 0; col_of[r] = -1; }
+  for (int c = threadIdx.x; c < KT2; c += DICT_THREADS) colw[c] = 0;
+  if (threadIdx.x == 0) { n_keys = 0; n_out = 0; }
+  __syncthreads();
+  uint2 *q2 = P.q2list + (size_t)tile * Q2CAP * TILE_Q;
+  for (int e = threadIdx.x; e < Q2CAP * TILE_Q; e += DICT_THREADS) {
+    const uint2 f = q2[e];
+    if (!(__uint_as_float(f.y) > 0.f)) continue;
+    const __half T = __float2half_ru((float)((f.x >> 16) + 1u));
+    if (!__hisinf(T)) {  // a B value of inf would turn the product with a zero weight into NaN
+      atomicAdd(&cnt[f.x & 0xFFFFu], 1u);
+      th[f.x & 0xFFFFu] = __half_as_ushort(T);  // the same value from every listing of the row
+    }
+  }
+  __syncthreads();
+  for (int r = threadIdx.x; r < NF2; r += DICT_THREADS)
+    if (cnt[r]) keys[atomicAdd(&n_keys, 1u)] = cnt[r] << 10 | (uint32_t)(NF2 - 1 - r);
+  __syncthreads();
+  const int nk = (int)n_keys;
+  for (int i = threadIdx.x; i < nk; i += DICT_THREADS) {
+    const uint32_t k = keys[i];
+    int rank = 0;
+    for (int j = 0; j < nk; j++) rank += keys[j] > k;
+    if (rank < KT2) {
+      const int r = NF2 - 1 - (int)(k & (NF2 - 1));
+      col_of[r] = (int16_t)rank;
+      colw[rank] = (uint32_t)r | (uint32_t)th[r] << 16;
+    }
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < KT2; c += DICT_THREADS) P.d2col[(size_t)tile * KT2 + c] = colw[c];
+  if (threadIdx.x < TILE_Q) {
+    const int64_t slot = (int64_t)tile * TILE_Q + threadIdx.x;
+    __half *wrow = P.Wf2 + (size_t)slot * KT2;
+    uint2 *ql = q2 + threadIdx.x;
+    int used = 0, out = 0;
+    for (; used < Q2CAP; used++) {  // the lists are filled from the front; padding queries have none
+      const uint2 f = ql[(size_t)used * TILE_Q];
+      const float w2 = __uint_as_float(f.y);
+      if (!(w2 > 0.f)) break;
+      const int c = col_of[f.x & 0xFFFFu];
+      if (c >= 0) wrow[c] = __float2half_ru(__fadd_ru(__half2float(wrow[c]), w2));
+      else ql[(size_t)(out++) * TILE_Q] = f;  // out <= used: never overwrites an entry still to be read
+    }
+    for (int j = out; j < used; j++) ql[(size_t)j * TILE_Q] = make_uint2(0u, 0u);
+    if (out) atomicAdd(&n_out, (unsigned int)out);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && n_out) atomicAdd(P.n_outside, (unsigned long long)n_out);
 }
 
 __host__ __device__ __forceinline__ uint32_t rb_bit(uint32_t fid) { return (fid * 0x85EBCA6Bu) >> 16; }  // 16 bits: RB_BITS

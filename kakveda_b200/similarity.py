@@ -408,14 +408,14 @@ class GfkbIndex:
 
     def layout(self) -> dict:
         b = (C.c_int64 * 4)()
-        c = (C.c_int64 * 17)()
+        c = (C.c_int64 * 18)()
         _capi.check(_capi.load().kv_index_layout(self._h, b, c))
         return {"block_bytes": b[0], "norm_bytes": b[1], "directory_bytes": b[2], "dense_bytes": b[3],
                 "entries": c[0], "universal_features": c[1], "rows": c[2], "last_ctas": c[3], "last_tiles": c[4],
                 "last_splits": c[5], "last_upload_bytes": c[6], "tf_overflow_entries": c[7], "chunks": c[8],
                 "pairs_scored": c[9], "records_scanned": c[10], "pairs_passed_bound": c[11],
                 "records_written": c[12], "kernel_launches": c[13], "rare_entries": c[14],
-                "pool_pages_used": c[15], "pool_pages": c[16]}
+                "pool_pages_used": c[15], "pool_pages": c[16], "f2_outside_dictionary": c[17]}
 
     def save_layout(self, path) -> None:
         """Persist the built scan layout (row order, column blocks, bound structures) of a finalized index."""
