@@ -40,16 +40,13 @@
 #pragma once
 #include "tfidf_kernels.cuh"
 
-#include <cuda.h>
-
 namespace kvk {
 
 constexpr int B_BN = 64;                     // chunks per block = N of the MMA tile
 constexpr int B_BK = 64;                     // K slice: 64 fp16 = one 128-byte swizzle row
 constexpr int B_KSLICES = NF / B_BK;         // 4
 constexpr int B_KSLICES2 = KT2 / B_BK;       // 4: the second-class dictionary, one slice per warp of the MMA warpgroup
-// Wf2 [n_q_pad][KT2] goes through make_map_f16_nf, which maps rows of NF halves
-static_assert(KT2 == NF, "the dictionary's A operand shares the tensor-map shape of Wf");
+static_assert(KT2 == 2 * 128, "each thread of the MMA warpgroup builds two columns of the dictionary's B operand");
 constexpr int B_STAGES = 2;
 constexpr int B_A_SLICE_BYTES = TILE_Q * B_BK * 2;  // 16 KiB: one K slice of the query operand
 constexpr int B_B_SLICE_BYTES = B_BN * B_BK * 2;    // 8 KiB: one K slice of the chunk operand
@@ -64,33 +61,6 @@ constexpr int B_COLS = B_BN / 4;             // chunk columns per epilogue threa
 constexpr int B_SEEDS = 4;                   // seeds per worker thread
 constexpr int B_SEEDS_PER_QUERY = 4 * B_SEEDS;
 constexpr float UBQ_SCALE = 250.f;           // 8-bit bound code = ceil(bound * 250), saturating at 255 (bounds reach ~1.001)
-
-__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-          smem_addr(dst)),
-      "l"((uint64_t)map), "r"(smem_addr(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-
-// wgmma shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups 1024 bytes apart (the operand tile
-// starts on a 1024-byte boundary, so the base offset is 0).  Advancing the start address by 32 bytes selects the next
-// K = 16 step inside the swizzled 128-byte row.
-__device__ __forceinline__ uint64_t wgmma_desc_sw128(const void *smem) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr(smem) & 0x3FFFF) >> 4);  // start address
-  d |= (uint64_t)1 << 16;                              // leading byte offset (unused for swizzled K-major)
-  d |= (uint64_t)(1024 >> 4) << 32;                    // stride byte offset
-  d |= (uint64_t)1 << 62;                              // SWIZZLE_128B
-  return d;
-}
-
-__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
-// keeps the compiler from moving accesses of an accumulator register across an asynchronous wgmma
-__device__ __forceinline__ void wgmma_reg_fence(float &r) { asm volatile("" : "+f"(r)::"memory"); }
 
 // D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, fp16 in, fp32 accumulators in registers (both operands K-major)
 __device__ __forceinline__ void wgmma_m64n64k16_f16(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
@@ -252,9 +222,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
   extern __shared__ unsigned char smem_raw[];
   const int pass = FAST ? 0 : P.pass;
   const bool has_codes = FAST ? true : (P.ubq != nullptr);
-  // 1024-byte alignment by an OFFSET into the shared array (not by rounding a generic pointer): the compiler keeps
-  // the shared address space, so every access below is LDS/STS/ATOMS instead of a generic load / store / atomic
-  BoundSmem &S = *reinterpret_cast<BoundSmem *>(smem_raw + ((1024u - (smem_addr(smem_raw) & 1023u)) & 1023u));
+  BoundSmem &S = *reinterpret_cast<BoundSmem *>(smem_raw + smem_align1024(smem_raw));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = blockIdx.x, bsplit = blockIdx.y;
   const int64_t n_blocks = (P.n_chunks + B_BN - 1) / B_BN;
@@ -642,31 +610,6 @@ __global__ void __launch_bounds__(SEL_WARPS * 32) tfidf_select_kernel(SelectPara
   __syncthreads();
   if (threadIdx.x == 0) P.lists.count[list] = s_count;
   flush_list_stats(P.stats, n_pairs, n_recs);
-}
-
-typedef CUresult (*PFN_encodeTiled_kv)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                       const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                       CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-// tensor map of a row-major fp16 matrix [rows][NF], box = 64 columns x box_rows rows, 128-byte swizzle
-static int make_map_f16_nf(CUtensorMap *map, const void *base, int64_t rows, int box_rows) {
-  static PFN_encodeTiled_kv fn = nullptr;
-  if (!fn) {
-    void *p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess || !p)
-      return kv_fail(KV_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-    fn = (PFN_encodeTiled_kv)p;
-  }
-  cuuint64_t gdim[2] = {(cuuint64_t)NF, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)NF * 2};
-  cuuint32_t box[2] = {(cuuint32_t)B_BK, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void *>(base), gdim, gstride, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return kv_fail(KV_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)r);
-  return KV_OK;
 }
 
 }  // namespace kvk

@@ -22,12 +22,13 @@
 // Each (query tile, split, column half) writes one partial list; K5 (kv_merge_topk_device) merges them.  CTAs
 // working on the same queries exchange k-th-score lower bounds through global memory (gthr).
 #include "kv_cuda.cuh"
+#include "sm90.cuh"
 
-#include <cuda.h>
 #include <cuda_bf16.h>
 
 #include <algorithm>
 #include <cstdlib>
+#include <memory>
 #include <mutex>
 #include <vector>
 
@@ -44,53 +45,6 @@ constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
 constexpr int MAXK = 32;       // per-query list slots: 2 x 32 x 128 x 8 B = 64 KiB beside the 3 x 48 KiB ring (k <= 32)
 constexpr int EPI_THREADS = 256;  // the two consumer warpgroups
 constexpr int N_THREADS = EPI_THREADS + 32;  // + the TMA producer warp
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_LOOP:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra WAIT_DONE;\n"
-      "bra WAIT_LOOP;\n"
-      "WAIT_DONE:\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-
-__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-          smem_u32(dst)),
-      "l"((uint64_t)map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-
-// wgmma shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups 1024 bytes apart (every operand
-// tile starts on a 1024-byte boundary: base offset 0).  +32 bytes of start address = the next K = 16 step of the row.
-__device__ __forceinline__ uint64_t wgmma_desc(const void *smem) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_u32(smem) & 0x3FFFF) >> 4);  // start address
-  d |= (uint64_t)1 << 16;                             // leading byte offset (unused for swizzled K-major)
-  d |= (uint64_t)(1024 >> 4) << 32;                   // stride byte offset
-  d |= (uint64_t)1 << 62;                             // SWIZZLE_128B
-  return d;
-}
-
-// keeps the compiler from moving accesses of an accumulator register across an asynchronous wgmma
-__device__ __forceinline__ void reg_fence(float &r) { asm volatile("" : "+f"(r)::"memory"); }
 
 // D[64 x 256] (+)= A[64 x 16] * B[256 x 16]^T, bf16 in, fp32 accumulators in registers (both operands K-major)
 __device__ __forceinline__ void wgmma_m64n256k16_bf16(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
@@ -161,9 +115,7 @@ struct __align__(1024) DenseSmem {
 __global__ void __launch_bounds__(N_THREADS, 1)
 dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c, DenseParams P) {
   extern __shared__ unsigned char smem_raw[];
-  // aligned by an OFFSET into the shared array (not by rounding a generic pointer): the compiler keeps the shared
-  // address space, so list and norm accesses are LDS/STS instead of generic loads / stores
-  DenseSmem &S = *reinterpret_cast<DenseSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
+  DenseSmem &S = *reinterpret_cast<DenseSmem *>(smem_raw + smem_align1024(smem_raw));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // work item = (query tile, row split); consecutive CTAs take consecutive query tiles of the same split, so the
   // CTAs resident at one time stream the same corpus rows (B tiles are shared through L2)
@@ -243,19 +195,19 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
       // ---- MMA over the K slices; a slice's ring slot is released once the next slice's MMAs are issued and the
       //      slice's own have completed ----
 #pragma unroll
-      for (int i = 0; i < 128; i++) reg_fence(acc[i]);
-      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+      for (int i = 0; i < 128; i++) wgmma_reg_fence(acc[i]);
+      wgmma_fence();
       int prev = -1;
       for (int kb = 0; kb < n_kb; kb++) {
         mbar_wait(&S.full_bar[stage], phase);
-        const uint64_t da = wgmma_desc(S.stage[stage] + wg * (A_BYTES / 2));  // rows 64 wg .. 64 wg + 63 of the tile
-        const uint64_t db = wgmma_desc(S.stage[stage] + A_BYTES);
+        const uint64_t da = wgmma_desc_sw128(S.stage[stage] + wg * (A_BYTES / 2));  // rows 64 wg .. 64 wg + 63 of the tile
+        const uint64_t db = wgmma_desc_sw128(S.stage[stage] + A_BYTES);
 #pragma unroll
         for (int kk = 0; kk < BK / UMMA_K; kk++)  // advance 32 bytes (2 x 16-byte units) per K=16 step inside the swizzle row
           wgmma_m64n256k16_bf16(acc, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), (uint32_t)((kb | kk) != 0));
-        asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+        wgmma_commit();
         if (prev >= 0) {
-          asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+          wgmma_wait<1>();
           __syncwarp();
           if (lane == 0) mbar_arrive(&S.empty_bar[prev]);
         }
@@ -290,9 +242,9 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
         }
       }
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+      wgmma_wait<0>();
 #pragma unroll
-      for (int i = 0; i < 128; i++) reg_fence(acc[i]);
+      for (int i = 0; i < 128; i++) wgmma_reg_fence(acc[i]);
       __syncwarp();
       if (lane == 0) mbar_arrive(&S.empty_bar[prev]);
       if (P.dbg == 1) continue;
@@ -365,37 +317,13 @@ __global__ void inv_norm_kernel(const __nv_bfloat16 *__restrict__ x, int64_t n, 
   if (lane == 0) out[r] = s > 0.0 ? (float)(1.0 / sqrt(s)) : 0.f;
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                    const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-int make_map(CUtensorMap *map, const void *base, int64_t rows, int dim, int box_rows) {
-  static PFN_encodeTiled fn = nullptr;
-  if (!fn) {
-    void *p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess || !p)
-      return kv_fail(KV_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-    fn = (PFN_encodeTiled)p;
-  }
-  cuuint64_t gdim[2] = {(cuuint64_t)dim, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)dim * 2};
-  cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(base), gdim, gstride, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return kv_fail(KV_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)r);
-  return KV_OK;
-}
-
 }  // namespace
 
 struct kv_dense_index {
   int device = 0, dim = 0;
   int64_t row_base = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
+  CudaStream stream;
+  CudaEvent ev[2];
   std::mutex mu;
   int sm_count = 132;
   DevVec<__nv_bfloat16> rows;
@@ -414,24 +342,18 @@ extern "C" {
 int kv_dense_create(int device, int dim, int64_t row_base, kv_dense_index **out) {
   if (!out) return kv_fail(KV_ERR_INVALID, "kv_dense_create: out is NULL");
   if (dim < BK || dim % BK != 0 || dim > 8192) return kv_fail(KV_ERR_INVALID, "kv_dense_create: dim must be a multiple of 64 (64..8192)");
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-    cudaGetLastError();
-    return kv_fail(KV_ERR_CUDA, "kv_dense_create: no CUDA device visible (this library has no CPU path)");
-  }
-  if (device < 0 || device >= n) return kv_fail(KV_ERR_INVALID, "kv_dense_create: device %d out of range", device);
-  KV_CUDA(cudaSetDevice(device));
-  kv_dense_index *dx = new kv_dense_index();
+  int sm_count = 0;
+  int rc = open_device(device, "kv_dense_create", &sm_count);
+  if (rc != KV_OK) return rc;
+  std::unique_ptr<kv_dense_index> dx(new kv_dense_index());
   dx->device = device;
   dx->dim = dim;
   dx->row_base = row_base;
-  cudaDeviceProp prop;
-  KV_CUDA(cudaGetDeviceProperties(&prop, device));
-  dx->sm_count = prop.multiProcessorCount;
-  KV_CUDA(cudaStreamCreateWithFlags(&dx->stream, cudaStreamNonBlocking));
-  for (auto &e : dx->ev) KV_CUDA(cudaEventCreate(&e));
+  dx->sm_count = sm_count;
+  KV_CUDA(dx->stream.create());
+  for (auto &e : dx->ev) KV_CUDA(e.create());
   KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
-  *out = dx;
+  *out = dx.release();
   return KV_OK;
 }
 
@@ -439,10 +361,6 @@ void kv_dense_destroy(kv_dense_index *dx) {
   if (!dx) return;
   cudaSetDevice(dx->device);
   cudaStreamSynchronize(dx->stream);
-  dx->rows.release(); dx->d_inv_c.release(); dx->d_inv_q.release(); dx->d_part_s.release(); dx->d_out_s.release();
-  dx->d_part_r.release(); dx->d_out_r.release(); dx->d_q.release(); dx->d_gthr.release();
-  for (auto &e : dx->ev) if (e) cudaEventDestroy(e);
-  if (dx->stream) cudaStreamDestroy(dx->stream);
   delete dx;
 }
 
@@ -493,9 +411,9 @@ static int dense_run(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, 
   inv_norm_kernel<<<(unsigned)((n_q * 32 + 255) / 256), 256, 0, s>>>(d_q, n_q, dx->dim, dx->d_inv_q.p);
   KV_CUDA(cudaGetLastError());
   CUtensorMap map_q, map_c;
-  int rc = make_map(&map_q, d_q, n_q, dx->dim, BM);
+  int rc = make_map_2d(&map_q, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, d_q, n_q, dx->dim, BM);
   if (rc != KV_OK) return rc;
-  rc = make_map(&map_c, dx->rows.p, dx->n_rows, dx->dim, BN);
+  rc = make_map_2d(&map_c, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, dx->rows.p, dx->n_rows, dx->dim, BN);
   if (rc != KV_OK) return rc;
   const int64_t q_tiles = (n_q + BM - 1) / BM, r_tiles = (dx->n_rows + BN - 1) / BN;
   // row splits: as few as possible (long row ranges keep the k-th-score thresholds high) while the CTA count

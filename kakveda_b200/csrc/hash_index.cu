@@ -10,6 +10,7 @@
 #include "kv_cuda.cuh"
 
 #include <algorithm>
+#include <memory>
 #include <mutex>
 #include <vector>
 
@@ -98,8 +99,8 @@ __global__ void __launch_bounds__(1024) hash_scan_kernel(const ulonglong2 *__res
 struct kv_hash_index {
   int device = 0;
   int64_t row_base = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
+  CudaStream stream;
+  CudaEvent ev[2];
   std::mutex mu;
   int sm_count = 132;
   DevVec<unsigned long long> rows;
@@ -116,23 +117,17 @@ extern "C" {
 
 int kv_hash_create(int device, int64_t row_base, kv_hash_index **out) {
   if (!out) return kv_fail(KV_ERR_INVALID, "kv_hash_create: out is NULL");
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-    cudaGetLastError();
-    return kv_fail(KV_ERR_CUDA, "kv_hash_create: no CUDA device visible (this library has no CPU path)");
-  }
-  if (device < 0 || device >= n) return kv_fail(KV_ERR_INVALID, "kv_hash_create: device %d out of range", device);
-  KV_CUDA(cudaSetDevice(device));
-  kv_hash_index *hx = new kv_hash_index();
+  int sm_count = 0;
+  int rc = open_device(device, "kv_hash_create", &sm_count);
+  if (rc != KV_OK) return rc;
+  std::unique_ptr<kv_hash_index> hx(new kv_hash_index());
   hx->device = device;
   hx->row_base = row_base;
-  cudaDeviceProp prop;
-  KV_CUDA(cudaGetDeviceProperties(&prop, device));
-  hx->sm_count = prop.multiProcessorCount;
-  KV_CUDA(cudaStreamCreateWithFlags(&hx->stream, cudaStreamNonBlocking));
-  for (auto &e : hx->ev) KV_CUDA(cudaEventCreate(&e));
+  hx->sm_count = sm_count;
+  KV_CUDA(hx->stream.create());
+  for (auto &e : hx->ev) KV_CUDA(e.create());
   KV_CUDA(cudaFuncSetAttribute(hash_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HQ_SLOTS * 12 + 2 * HQ_BIT_WORDS * 4));
-  *out = hx;
+  *out = hx.release();
   return KV_OK;
 }
 
@@ -140,9 +135,6 @@ void kv_hash_destroy(kv_hash_index *hx) {
   if (!hx) return;
   cudaSetDevice(hx->device);
   cudaStreamSynchronize(hx->stream);
-  hx->rows.release(); hx->d_keys.release(); hx->d_pairs.release(); hx->d_qidx.release(); hx->d_bits.release(); hx->d_count.release();
-  for (auto &e : hx->ev) if (e) cudaEventDestroy(e);
-  if (hx->stream) cudaStreamDestroy(hx->stream);
   delete hx;
 }
 

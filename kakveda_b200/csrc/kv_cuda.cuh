@@ -4,6 +4,8 @@
 
 #include <cuda_runtime.h>
 
+#include <utility>
+
 #define KV_CUDA(expr)                                                                         \
   do {                                                                                        \
     cudaError_t _e = (expr);                                                                  \
@@ -12,11 +14,22 @@
                      __FILE__, __LINE__);                                                     \
   } while (0)
 
+// Checks that `device` exists, makes it current and reads its SM count: the first step of every create function
+// (`fn` names it in the error message).  No visible device is KV_ERR_CUDA ("no CUDA device visible").
+int open_device(int device, const char *fn, int *sm_count);
+
+// The buffers and handles below own what they hold: it is freed when they are destroyed, and they are move-only, so a
+// copy (two owners) does not compile.  Destroy them with their device current.
+
 // Growable device array (amortised doubling) -- the raw CSR of an append-only index.
 template <typename T>
 struct DevVec {
   T *p = nullptr;
   int64_t n = 0, cap = 0;
+  DevVec() = default;
+  DevVec(DevVec &&o) noexcept : p(std::exchange(o.p, nullptr)), n(std::exchange(o.n, 0)), cap(std::exchange(o.cap, 0)) {}
+  DevVec(const DevVec &) = delete;
+  ~DevVec() { cudaFree(p); }
   cudaError_t reserve(int64_t want, cudaStream_t s) {
     if (want <= cap) return cudaSuccess;
     int64_t nc = cap ? cap : 1024;
@@ -35,7 +48,6 @@ struct DevVec {
     cap = nc;
     return cudaSuccess;
   }
-  void release() { cudaFree(p); p = nullptr; n = cap = 0; }
 };
 
 // Fixed-size device buffer re-allocated only when it must grow (scratch reused across calls).
@@ -43,6 +55,10 @@ template <typename T>
 struct DevBuf {
   T *p = nullptr;
   int64_t cap = 0;
+  DevBuf() = default;
+  DevBuf(DevBuf &&o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+  DevBuf(const DevBuf &) = delete;
+  ~DevBuf() { cudaFree(p); }
   cudaError_t ensure(int64_t want) {
     if (want <= cap) return cudaSuccess;
     cudaFree(p);
@@ -52,13 +68,16 @@ struct DevBuf {
     if (e == cudaSuccess) cap = want;
     return e;
   }
-  void release() { cudaFree(p); p = nullptr; cap = 0; }
 };
 
 template <typename T>
 struct PinnedBuf {
   T *p = nullptr;
   int64_t cap = 0;
+  PinnedBuf() = default;
+  PinnedBuf(PinnedBuf &&o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+  PinnedBuf(const PinnedBuf &) = delete;
+  ~PinnedBuf() { cudaFreeHost(p); }
   cudaError_t ensure(int64_t want) {
     if (want <= cap) return cudaSuccess;
     cudaFreeHost(p);
@@ -68,5 +87,26 @@ struct PinnedBuf {
     if (e == cudaSuccess) cap = want;
     return e;
   }
-  void release() { cudaFreeHost(p); p = nullptr; cap = 0; }
+};
+
+// Non-blocking stream; converts to cudaStream_t.
+struct CudaStream {
+  cudaStream_t s = nullptr;
+  CudaStream() = default;
+  CudaStream(CudaStream &&o) noexcept : s(std::exchange(o.s, nullptr)) {}
+  CudaStream(const CudaStream &) = delete;
+  ~CudaStream() { if (s) cudaStreamDestroy(s); }
+  cudaError_t create() { return cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking); }
+  operator cudaStream_t() const { return s; }
+};
+
+// Event with timing; converts to cudaEvent_t.
+struct CudaEvent {
+  cudaEvent_t e = nullptr;
+  CudaEvent() = default;
+  CudaEvent(CudaEvent &&o) noexcept : e(std::exchange(o.e, nullptr)) {}
+  CudaEvent(const CudaEvent &) = delete;
+  ~CudaEvent() { if (e) cudaEventDestroy(e); }
+  cudaError_t create() { return cudaEventCreate(&e); }
+  operator cudaEvent_t() const { return e; }
 };

@@ -37,10 +37,10 @@ int host_threads() {
 struct kv_index {
   int device = 0;
   int64_t row_base = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  cudaEvent_t evk[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // bound/scan kernel boundaries of a batch
-  cudaEvent_t evp2 = nullptr;  // start of phase 2 of a two-phase batch
+  CudaStream stream;
+  CudaEvent ev[5];
+  CudaEvent evk[6];  // bound/scan kernel boundaries of a batch
+  CudaEvent evp2;    // start of phase 2 of a two-phase batch
   bool two_phase = false;
   std::mutex mu;
   int sm_count = 132;
@@ -288,7 +288,7 @@ int upload_layout(kv_index *ix, const ScanLayout &L) {
     KV_CUDA(cudaGetLastError());
   }
   KV_CUDA(cudaStreamSynchronize(s));  // the caller's staging vectors may go out of scope
-  int rc = make_map_f16_nf(&ix->map_u, ix->d_Uf.p, H.n_chunks_pad, B_BN);
+  int rc = make_map_2d(&ix->map_u, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ix->d_Uf.p, H.n_chunks_pad, NF, B_BN);
   if (rc != KV_OK) return rc;
   ix->h_fslot = L.fslot; ix->h_fslot2 = L.fslot2;
   ix->n_chunks = H.n_chunks; ix->n_chunks_pad = H.n_chunks_pad; ix->blk_words = H.blk_words; ix->n_entries = H.n_entries;
@@ -303,24 +303,24 @@ extern "C" {
 
 int kv_index_create(int device, int64_t row_base, kv_index **out) {
   if (!out) return kv_fail(KV_ERR_INVALID, "kv_index_create: out is NULL");
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-    cudaGetLastError();
-    return kv_fail(KV_ERR_CUDA, "kv_index_create: no CUDA device visible (this library has no CPU path)");
-  }
-  if (device < 0 || device >= n) return kv_fail(KV_ERR_INVALID, "kv_index_create: device %d out of range", device);
-  KV_CUDA(cudaSetDevice(device));
-  kv_index *ix = new kv_index();
+  int sm_count = 0;
+  int rc = open_device(device, "kv_index_create", &sm_count);
+  if (rc != KV_OK) return rc;
+  std::unique_ptr<kv_index> ix(new kv_index());
   ix->device = device;
   ix->row_base = row_base;
-  cudaDeviceProp prop;
-  KV_CUDA(cudaGetDeviceProperties(&prop, device));
-  ix->sm_count = prop.multiProcessorCount;
-  KV_CUDA(cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking));
-  for (auto &e : ix->ev) KV_CUDA(cudaEventCreate(&e));
-  for (auto &e : ix->evk) KV_CUDA(cudaEventCreate(&e));
-  KV_CUDA(cudaEventCreate(&ix->evp2));
-  *out = ix;
+  ix->sm_count = sm_count;
+  KV_CUDA(ix->stream.create());
+  for (auto &e : ix->ev) KV_CUDA(e.create());
+  for (auto &e : ix->evk) KV_CUDA(e.create());
+  KV_CUDA(ix->evp2.create());
+  constexpr auto smem_limit = cudaFuncAttributeMaxDynamicSharedMemorySize;
+  KV_CUDA(cudaFuncSetAttribute(tfidf_score_kernel, smem_limit, 200 * 1024));
+  KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel, smem_limit, (int)scan_smem_bytes(32)));
+  KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<true>, smem_limit, 232448));
+  KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<false>, smem_limit, 232448));
+  KV_CUDA(cudaFuncSetAttribute(jaccard_scan_kernel, smem_limit, (int)jaccard_smem_bytes(32)));
+  *out = ix.release();
   return KV_OK;
 }
 
@@ -328,33 +328,7 @@ void kv_index_destroy(kv_index *ix) {
   if (!ix) return;
   cudaSetDevice(ix->device);
   cudaStreamSynchronize(ix->stream);
-  ix->indptr.release(); ix->ids.release(); ix->tf.release();
-  ix->d_df.release(); ix->d_cnt.release(); ix->d_tfmin.release(); ix->d_tfmax.release(); ix->d_utf.release();
-  ix->d_a64.release(); ix->d_d64.release(); ix->d_bb64.release(); ix->d_B64.release();
-  ix->d_B32.release(); ix->d_cminB.release(); ix->d_univ.release(); ix->d_perm.release(); ix->d_invperm.release();
-  ix->d_blk.release(); ix->d_binfo.release(); ix->d_Uf.release(); ix->d_fslot.release(); ix->d_fslot2.release(); ix->d_ubt.release();
-  ix->d_rbloom.release(); ix->d_rt_keys.release(); ix->d_rt_off.release(); ix->d_rt_size.release(); ix->d_rt_masks.release();
-  ix->d_q2list.release(); ix->d_q3id.release(); ix->d_q3w.release(); ix->d_d2col.release(); ix->d_f2out.release();
-  ix->d_ovf_keys.release(); ix->d_ovf_vals.release();
-  ix->d_rq_indptr.release(); ix->d_rq_ids.release(); ix->d_rq_tf.release(); ix->d_rq_const.release(); ix->d_rq_out.release();
-  ix->d_rq_rows.release();
-  ix->h_q_indptr.release(); ix->h_q_ids.release(); ix->h_q_tf.release(); ix->h_q_oov.release(); ix->h_qperm.release();
-  ix->h_flags.release();
-  ix->d_q_indptr.release(); ix->d_q_ids.release(); ix->d_q_tf.release(); ix->d_q_oov.release(); ix->d_qperm.release();
-  ix->d_flags.release(); ix->d_qconst.release(); ix->d_qtab.release(); ix->d_Wf.release(); ix->d_Wf2.release();
-  ix->d_gthr.release();
-  ix->d_seeds.release(); ix->d_direct.release(); ix->d_pool.release(); ix->d_list_count.release(); ix->d_list_pages.release();
-  ix->d_pool_ctl.release(); ix->d_ubq.release();
-  close_peers(ix);
-  ix->d_excl_sorted.release(); ix->d_excl_orig.release();
-  ix->d_stats.release();
-  ix->d_part_s.release(); ix->d_out_s.release(); ix->d_part_r.release(); ix->d_out_r.release();
-  ix->h_out_s.release(); ix->h_out_r.release();
-  ix->h_qtab.release(); ix->d_qtab1.release(); ix->d_scores.release();
-  for (auto &e : ix->ev) if (e) cudaEventDestroy(e);
-  for (auto &e : ix->evk) if (e) cudaEventDestroy(e);
-  if (ix->evp2) cudaEventDestroy(ix->evp2);
-  if (ix->stream) cudaStreamDestroy(ix->stream);
+  close_peers(ix);  // the peers' mapped threshold arrays: not memory this handle allocated
   delete ix;
 }
 
@@ -701,11 +675,6 @@ static int score_impl(kv_index *ix, const uint32_t *q_ids, const uint32_t *q_tf,
   P.w_unscale = std::ldexp(1.0, -e_w); P.c_unscale = std::ldexp(1.0, -e_c);
   P.nq = nq; P.dotU = dotU; P.corrU = corrU; P.jaccard = ix->jaccard; P.out = ix->d_scores.p;
   const size_t smem = tab_bytes + 8 * 32 * 24;
-  static bool attr_set[64] = {false};
-  if (!attr_set[ix->device & 63]) {
-    KV_CUDA(cudaFuncSetAttribute(tfidf_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr_set[ix->device & 63] = true;
-  }
   int blocks = (int)std::min<int64_t>((ix->n_chunks + 7) / 8, (int64_t)ix->sm_count * 8);
   if (blocks < 1) blocks = 1;
   KV_CUDA(cudaEventRecord(ix->ev[1], s));
@@ -947,8 +916,6 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   P.qsrc = ix->d_qperm.p + 2 * n_q; P.flags = ix->d_flags.p;
   P.n_q = n_q; P.V = ix->V; P.n_total = ix->n_total;
   P.a64 = ix->d_a64.p; P.d64 = ix->d_d64.p; P.univ = ix->d_univ.p; P.utf = ix->d_utf.p; P.tfmax = ix->d_tfmax.p;
-  P.q2cap = Q2CAP;
-  if (const char *e = getenv("KAKVEDA_B200_Q2CAP")) P.q2cap = std::max(0, std::min(Q2CAP, atoi(e)));
   P.fslot = ix->d_fslot.p; P.fslot2 = ix->d_fslot2.p; P.q2list = ix->d_q2list.p; P.jaccard = ix->jaccard; P.corpus_fit = ix->corpus_fit;
   P.q_nq = ix->d_qconst.p; P.q_dotU = P.q_nq + n_q; P.q_corrU = P.q_nq + 2 * n_q; P.q_dotS = P.q_nq + 3 * n_q;
   P.q_corrS = P.q_nq + 4 * n_q; P.q_dotX = P.q_nq + 5 * n_q; P.q_rscale = P.q_nq + 6 * n_q;
@@ -960,8 +927,8 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   f2_dict_kernel<<<(unsigned)n_tiles, DICT_THREADS, 0, s>>>(DP);
   KV_CUDA(cudaGetLastError());
   {
-    int rc = make_map_f16_nf(&ix->map_w, ix->d_Wf.p, n_q_pad, TILE_Q);
-    if (rc == KV_OK) rc = make_map_f16_nf(&ix->map_w2, ix->d_Wf2.p, n_q_pad, TILE_Q);  // KT2 == NF columns
+    int rc = make_map_2d(&ix->map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ix->d_Wf.p, n_q_pad, NF, TILE_Q);
+    if (rc == KV_OK) rc = make_map_2d(&ix->map_w2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ix->d_Wf2.p, n_q_pad, KT2, TILE_Q);
     if (rc != KV_OK) return rc;
   }
   unsigned long long f2_out = 0;
@@ -1118,11 +1085,6 @@ static int run_jaccard(kv_index *ix, Batch &b) {
   JP.qtab = ix->d_qtab.p; JP.q_nq = qc; JP.q_dotU = qc + n_q; JP.q_excl = ix->has_excl ? ix->d_excl_sorted.p : nullptr;
   JP.gthr = ix->d_gthr.p; JP.stats = ix->d_stats.p;
   JP.n_q = n_q; JP.k = b.k; JP.n_splits = (int)jsplits; JP.part_scores = ix->d_part_s.p; JP.part_rows = ix->d_part_r.p;
-  static bool jattr[64] = {false};
-  if (!jattr[ix->device & 63]) {
-    KV_CUDA(cudaFuncSetAttribute(jaccard_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jaccard_smem_bytes(32)));
-    jattr[ix->device & 63] = true;
-  }
   jaccard_scan_kernel<<<dim3((unsigned)n_groups, (unsigned)jsplits), J_WARPS * 32, jaccard_smem_bytes(b.k), ix->stream>>>(JP);
   KV_CUDA(cudaGetLastError());
   b.launches++;
@@ -1201,13 +1163,6 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
     }
   }
   if (phase != 2) ix->last_used_codes = b.use_codes ? 1 : 0;
-  static bool attr_set[64] = {false};
-  if (!attr_set[ix->device & 63]) {
-    KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scan_smem_bytes(32)));
-    KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-    KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-    attr_set[ix->device & 63] = true;
-  }
   if (prune && bound_smem_bytes(b.max_pages) > 232448)
     return kv_fail(KV_ERR_INVALID, "kv_topk: index too large for one bound-kernel row range (max_pages %d)", b.max_pages);
 
@@ -1647,7 +1602,6 @@ int kv_debug_bound_numerators(kv_index *ix, int k, float *out, int32_t *slot_que
       slot_query[i] = ix->h_qperm.p[i];
     }
   }
-  xs.release();
   return rc;
 }
 

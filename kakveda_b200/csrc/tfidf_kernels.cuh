@@ -33,6 +33,7 @@
 // are exact integer sums of tf_c w(t) and tf_c^2 c(t).  Relative resolution 2^-32 per term (float32 has 2^-24).
 #pragma once
 #include "kv_cuda.cuh"
+#include "sm90.cuh"
 
 #include <cuda_fp16.h>
 
@@ -193,8 +194,6 @@ __device__ __forceinline__ uint32_t lanemask_lt() {
   return v;
 }
 
-__device__ __forceinline__ uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
 // ----------------------------------------------------------------------------------------
 // K1a: one query against every row, float64 (the drop-in SimilarityEngine.score path).  One warp per chunk: the
 // lanes probe the block's entries in the query table, every hit adds its fixed-point weight to the rows of its
@@ -321,7 +320,6 @@ struct PrepParams {
   const short *fslot;       // feature -> column of the dense matrices, -1: not a frequent feature
   const unsigned short *fslot2;  // feature -> bit row of the block bitmaps (second class), 0xFFFF: none
   int jaccard, corpus_fit;
-  int q2cap;                // second-class features a query lists itself (<= Q2CAP)
   float *q_nq, *q_dotU, *q_corrU, *q_dotS, *q_corrS, *q_dotX;  // [n_q] by sorted slot
   float *q_rscale;          // [n_q] 1 / s_q: fixed-point unit of the bound kernel's accumulator R (see below)
   unsigned char *qtab;      // [n_q][QTAB_BYTES]
@@ -378,7 +376,7 @@ __global__ void prep_queries_kernel(PrepParams P) {
         const __half wf = __float2half_ru(__double2float_ru(f * a));
         P.Wf[(size_t)i * NF + fs] = wf;
         xmax += (double)__half2float(wf) * tm;
-      } else if (P.fslot2[t] != 0xFFFFu && c2 < P.q2cap) {
+      } else if (P.fslot2[t] != 0xFFFFu && c2 < Q2CAP) {
         const uint32_t tm1 = min(P.tfmax[t] - 1u, 65535u);  // weight of the 'tf >= 2' plane: (largest tf - 1) more times
         const float w2 = __double2float_ru(f * a * (1.0 + 1e-6));
         q2[(size_t)c2 * TILE_Q] = make_uint2((uint32_t)P.fslot2[t] | (tm1 << 16), __float_as_uint(w2));
@@ -558,28 +556,6 @@ struct ScanHit {
   uint32_t c_hi, pad0, pad1, pad2;
 };
 
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_LOOP:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra WAIT_DONE;\n"
-      "bra WAIT_LOOP;\n"
-      "WAIT_DONE:\n"
-      "}\n" ::"r"(smem_addr(bar)),
-      "r"(parity)
-      : "memory");
-}
 // 1-D bulk asynchronous copy global -> shared (TMA engine), completion counted in bytes on an mbarrier
 __device__ __forceinline__ void bulk_copy_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_addr(dst)),
