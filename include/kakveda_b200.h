@@ -202,6 +202,23 @@ int kv_query_set_exclusions(kv_index *ix, const int64_t *exclude_rows, int64_t n
  * excluding itself (follow with kv_topk_resident / kv_topk_resident_host). */
 int kv_selfjoin_upload(kv_index *ix, int64_t q_begin, int64_t q_end);
 
+/* Threshold search over the resident batch (kv_query_upload / kv_selfjoin_upload; exclusions honoured): every
+ * (query, row) pair whose score -- the float32 value kv_topk reports for that pair -- is >= threshold,
+ * 0 < threshold <= 1.  *n_pairs receives the count; the pairs stay in the handle until kv_range_fetch, the next
+ * upload, finalize or range call.  Extension for threshold consumers (services/warning_policy/app.py:22,52 compares
+ * with failure_matching.similarity_threshold; kv_cluster_csr links on the exact threshold graph).  It runs bound pass 1
+ * on the fixed threshold and the candidate scan with an emitting epilogue (the exhaustive scan on small indexes), then
+ * the float64 full scan of irregular queries; the resident batch, its exclusions and the top-k thresholds are left as
+ * they were, so a later kv_topk_resident* returns what it would have without it.  kv_index_last_kernel_ms: [0] = [1] =
+ * 0, [2] = bound pass 1, [3] = the scan (including a re-run after the pair buffer grew), [4] = irregular-query
+ * fallbacks; kv_index_layout counters [9]-[13] describe the run.  threshold NaN, <= 0 or > 1: KV_ERR_INVALID.
+ * KV_ERR_NOMEM when the candidate pool is exhausted or the pairs do not fit in device memory (the message gives their
+ * count).  Jaccard indexes: KV_ERR_INVALID (K3 has no emitting form). */
+int kv_range_resident(kv_index *ix, float threshold, int64_t *n_pairs);
+/* The last range result: indptr[n_q+1] by original query, rows[n_pairs] (global), scores[n_pairs]; per query
+ * ordered by (score desc, row asc).  KV_ERR_STATE when there is none. */
+int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores);
+
 /* K6: float64 scores of selected (query, row) pairs: rows[n_q*k] are GLOBAL row ids (e.g. what kv_topk returned;
  * -1 = unused slot), out_scores[n_q*k] (host) receives the float64 cosine of SimilarityEngine.score
  * (similarity.py:14-20) for that row, -inf for unused slots and rows that live on another shard.  Summation follows
@@ -242,7 +259,8 @@ int kv_merge_topk_device_on(int device, const void *d_scores_in, const void *d_r
  * ms[0] = H2D of the query batch, ms[1] = bound + scan kernels, ms[2] = merge (+ fallbacks), ms[3] = D2H. */
 int kv_index_last_timing(const kv_index *ix, float ms[4]);
 /* ... and of its kernels: ms[0] = bound pass 0 (seeds; wgmma GEMM + rare-feature join), ms[1] = seed scan,
- * ms[2] = bound pass 1 (candidate lists), ms[3] = candidate scan, ms[4] = merge.  Exhaustive mode: only [3], [4]. */
+ * ms[2] = bound pass 1 (candidate lists), ms[3] = candidate scan, ms[4] = merge.  Exhaustive mode: only [3], [4].
+ * After kv_range_resident: see there. */
 int kv_index_last_kernel_ms(const kv_index *ix, float ms[5]);
 /* Test hook: runs the resident batch once and returns the numerators (dot-product upper bounds) the bound kernel formed
  * for every (query slot, chunk): out[n_q][chunks] floats, slot_query[i] = original query of sorted slot i.  Needs an
@@ -328,6 +346,11 @@ int kv_hash_last_timing(const kv_hash_index *hx, float *scan_ms, int *passes);
  * ---------------------------------------------------------------------------------- */
 int kv_cluster_topk(int64_t n, int k, const int64_t *rows, const float *scores, float threshold, int64_t *labels,
                     int64_t *n_clusters);
+/* Connected components of the graph whose edges are i -- rows[j] for j in [indptr[i], indptr[i+1]) (rows < 0
+ * skipped, rows >= n rejected): labels[i] = smallest row of i's component (union-find of kv_cluster_topk).  With the
+ * result of kv_selfjoin_upload + kv_range_resident these are the components of the exact threshold graph, which a
+ * top-k list cannot give when a text is stored more than k times. */
+int kv_cluster_csr(int64_t n, const int64_t *indptr, const int64_t *rows, int64_t *labels, int64_t *n_clusters);
 
 /* ------------------------------------------------------------------------------------
  * Synthetic failures.jsonl-shaped signature_text generator (test / bench support; the

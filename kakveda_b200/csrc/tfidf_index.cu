@@ -132,6 +132,14 @@ struct kv_index {
   DevBuf<int> d_excl_sorted, d_excl_orig;  // self-join exclusions of the resident batch (by sorted slot / by original query)
   std::vector<int> h_excl_orig;
   bool has_excl = false;
+  // threshold search over the resident batch (kv_range_resident): its own threshold array (not d_gthr, which peers push
+  // into and a top-k raises), the pair buffer, the pair count, and the result until it is fetched
+  DevBuf<int> d_rthr;
+  DevBuf<RangePair> d_range;
+  DevBuf<unsigned long long> d_range_count;
+  PinnedBuf<RangePair> h_range;
+  bool range_valid = false;
+  int64_t range_q = 0, range_pairs = 0;
   DevBuf<unsigned long long> d_stats;
   DevBuf<float> d_part_s, d_out_s;
   DevBuf<long long> d_part_r, d_out_r;
@@ -316,7 +324,8 @@ int kv_index_create(int device, int64_t row_base, kv_index **out) {
   KV_CUDA(ix->evp2.create());
   constexpr auto smem_limit = cudaFuncAttributeMaxDynamicSharedMemorySize;
   KV_CUDA(cudaFuncSetAttribute(tfidf_score_kernel, smem_limit, 200 * 1024));
-  KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel, smem_limit, (int)scan_smem_bytes(32)));
+  KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<false>, smem_limit, (int)scan_smem_bytes(32)));
+  KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<true>, smem_limit, (int)scan_smem_bytes(0)));
   KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<true>, smem_limit, 232448));
   KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<false>, smem_limit, 232448));
   KV_CUDA(cudaFuncSetAttribute(jaccard_scan_kernel, smem_limit, (int)jaccard_smem_bytes(32)));
@@ -563,7 +572,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
       KV_CUDA(cudaStreamSynchronize(s));
       ix->V = V;
       ix->finalized = true;
-      ix->batch_valid = false;
+      ix->batch_valid = ix->range_valid = false;
       ix->last_finalize_kind = 2;
       return KV_OK;
     }
@@ -604,7 +613,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
   KV_CUDA(cudaStreamSynchronize(s));
   ix->V = V;
   ix->finalized = true;
-  ix->batch_valid = false;
+  ix->batch_valid = ix->range_valid = false;
   ix->last_finalize_kind = 1;
   return KV_OK;
 }
@@ -770,7 +779,7 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   if (n_q >= (1LL << 31) - TILE_Q) return kv_fail(KV_ERR_INVALID, "kv_topk: too many queries in one call");
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
-  ix->batch_valid = false;
+  ix->batch_valid = ix->range_valid = false;
   ix->has_excl = false;
   ix->irr_q.clear(); ix->irr_indptr.assign(1, 0); ix->irr_ids.clear(); ix->irr_tf.clear(); ix->irr_oov.clear();
   const int T = host_threads();
@@ -957,13 +966,15 @@ static int prepare_batch(kv_index *ix, const int64_t *q_indptr, const uint32_t *
 // lower bound of the final k-th score; a row-sharded GFKB exchanges it between the GPUs).  phase 2: the rest.
 // Three device paths: pruned (bound pass 0 -> seed scan -> candidate selection -> scan of the candidates), exhaustive
 // (small indexes, KAKVEDA_B200_NO_PRUNE=1: every chunk is a candidate of every query) and Jaccard (K3).
+// A threshold search (kv_range_resident, range = true, k = 0) runs the second phase of the pruned path -- bound pass 1
+// on the fixed threshold, then the scan -- or the exhaustive scan, with K1b-R as the scan.
 struct Batch {
   int k, phase;
   float *out_s;  // the outputs, [n_q][k] by original query
   long long *out_r;
   int64_t n_q, n_tiles, n_groups, n_bsplits, n_ssplits, n_ssplits_a, n_parts;
   int max_pages, n_seed, n_peers;
-  bool use_codes;
+  bool prune, use_codes, range = false;
   int64_t launches = 0;
 };
 
@@ -983,11 +994,30 @@ static ScanParams scan_params(const kv_index *ix, const Batch &b) {
   SP.n_chunks = ix->n_chunks; SP.n_rows = ix->n_rows; SP.row_base = ix->row_base;
   SP.ovf_keys = ix->d_ovf_keys.p; SP.ovf_vals = ix->d_ovf_vals.p; SP.n_ovf = ix->n_ovf;
   SP.qtab = ix->d_qtab.p; SP.q_nq = qc; SP.q_dotU = qc + b.n_q; SP.q_corrU = qc + 2 * b.n_q;
-  SP.q_excl = ix->has_excl ? ix->d_excl_sorted.p : nullptr; SP.gthr = ix->d_gthr.p;
+  SP.q_excl = ix->has_excl ? ix->d_excl_sorted.p : nullptr; SP.gthr = b.range ? ix->d_rthr.p : ix->d_gthr.p;
   for (int i = 0; i < 7; i++) SP.peer_gthr[i] = i < b.n_peers ? ix->peer_gthr[i] : nullptr;
   SP.n_peers = b.n_peers; SP.stats = ix->d_stats.p; SP.n_q = b.n_q; SP.k = b.k;
   SP.part_scores = ix->d_part_s.p; SP.part_rows = ix->d_part_r.p; SP.max_pages = b.max_pages;
+  SP.qperm = ix->d_qperm.p; SP.range_out = ix->d_range.p; SP.range_count = ix->d_range_count.p;
+  SP.range_cap = (unsigned long long)ix->d_range.cap;
   return SP;
+}
+
+// K1b-S, or K1b-R for a threshold search, over a grid of candidate lists
+static int launch_scan(kv_index *ix, const Batch &b, const ScanParams &SP, dim3 grid) {
+  if (b.range) tfidf_scan_kernel<true><<<grid, S_WARPS * 32, scan_smem_bytes(0), ix->stream>>>(SP);
+  else tfidf_scan_kernel<false><<<grid, S_WARPS * 32, scan_smem_bytes(b.k), ix->stream>>>(SP);
+  KV_CUDA(cudaGetLastError());
+  return KV_OK;
+}
+
+// The scan of the candidate lists bound pass 1 or the selection kernel built
+static int scan_candidates(kv_index *ix, Batch &b) {
+  ScanParams SP = scan_params(ix, b);
+  SP.list_mode = 0; SP.list_count = ix->d_list_count.p + b.n_groups; SP.list_pages = ix->d_list_pages.p; SP.pool = ix->d_pool.p;
+  SP.n_bsplits = (int)b.n_bsplits; SP.n_ssplits = (int)b.n_ssplits;
+  b.launches++;
+  return launch_scan(ix, b, SP, dim3((unsigned)(b.n_groups * b.n_bsplits), (unsigned)b.n_ssplits));
 }
 
 // Pruned path.  Phase 0 / 1: bound pass 0 (seeds and bound codes) -> seed scan; phase 1 ends with the seed top-k.
@@ -1004,7 +1034,7 @@ static int run_pruned(kv_index *ix, Batch &b) {
   BP.rbloom = ix->d_rbloom.p; BP.rt_keys = ix->d_rt_keys.p; BP.rt_masks = ix->d_rt_masks.p; BP.rt_off = ix->d_rt_off.p;
   BP.rt_size = ix->d_rt_size.p; BP.tfmax = ix->d_tfmax.p;
   BP.q_nq = qc; BP.q_dotS = qc + 3 * n_q; BP.q_corrS = qc + 4 * n_q; BP.q_dotX = qc + 5 * n_q; BP.q_rscale = qc + 6 * n_q;
-  BP.gthr = ix->d_gthr.p; BP.n_bsplits = (int)b.n_bsplits; BP.seeds = ix->d_seeds.p;
+  BP.gthr = b.range ? ix->d_rthr.p : ix->d_gthr.p; BP.n_bsplits = (int)b.n_bsplits; BP.seeds = ix->d_seeds.p;
   BP.lists.count = ix->d_list_count.p + b.n_groups; BP.lists.pages = ix->d_list_pages.p; BP.lists.max_pages = b.max_pages;
   BP.lists.pool = ix->d_pool.p; BP.lists.pool_next = ix->d_pool_ctl.p; BP.lists.pool_pages = (unsigned int)ix->pool_pages;
   BP.lists.overflow = (int *)(ix->d_pool_ctl.p + 1); BP.stats = ix->d_stats.p;
@@ -1029,7 +1059,7 @@ static int run_pruned(kv_index *ix, Batch &b) {
     // seed scan: gives every query a lower bound of its k-th score
     SP.list_mode = 1; SP.list_count = ix->d_list_count.p; SP.direct = ix->d_direct.p; SP.direct_stride = GROUP_Q * b.n_seed;
     SP.n_bsplits = 1; SP.n_ssplits = (int)b.n_ssplits_a;
-    tfidf_scan_kernel<<<dim3((unsigned)b.n_groups, (unsigned)b.n_ssplits_a), S_WARPS * 32, scan_smem_bytes(b.k), s>>>(SP);
+    tfidf_scan_kernel<false><<<dim3((unsigned)b.n_groups, (unsigned)b.n_ssplits_a), S_WARPS * 32, scan_smem_bytes(b.k), s>>>(SP);
     KV_CUDA(cudaGetLastError());
     KV_CUDA(cudaEventRecord(ix->evk[2], s));
     b.launches += 3;
@@ -1050,23 +1080,16 @@ static int run_pruned(kv_index *ix, Batch &b) {
   }
   KV_CUDA(cudaGetLastError());
   KV_CUDA(cudaEventRecord(ix->evk[3], s));
-  SP.list_mode = 0; SP.list_count = BP.lists.count; SP.list_pages = ix->d_list_pages.p; SP.pool = ix->d_pool.p;
-  SP.n_bsplits = (int)b.n_bsplits; SP.n_ssplits = (int)b.n_ssplits;
-  tfidf_scan_kernel<<<dim3((unsigned)(b.n_groups * b.n_bsplits), (unsigned)b.n_ssplits), S_WARPS * 32, scan_smem_bytes(b.k), s>>>(SP);
-  KV_CUDA(cudaGetLastError());
-  b.launches += 2;
-  return KV_OK;
+  b.launches++;
+  return scan_candidates(ix, b);
 }
 
 // Exhaustive path: every chunk of a list's chunk range x every query of the group
 static int run_exhaustive(kv_index *ix, Batch &b) {
   ScanParams SP = scan_params(ix, b);
   SP.list_mode = 2; SP.n_bsplits = (int)b.n_bsplits; SP.n_ssplits = (int)b.n_ssplits;
-  tfidf_scan_kernel<<<dim3((unsigned)(b.n_groups * b.n_bsplits), (unsigned)b.n_ssplits), S_WARPS * 32, scan_smem_bytes(b.k),
-                      ix->stream>>>(SP);
-  KV_CUDA(cudaGetLastError());
   b.launches++;
-  return KV_OK;
+  return launch_scan(ix, b, SP, dim3((unsigned)(b.n_groups * b.n_bsplits), (unsigned)b.n_ssplits));
 }
 
 // Jaccard path: token sets have no text structure to prune on -- the dense-regime kernel K3 scores every chunk for a
@@ -1091,18 +1114,14 @@ static int run_jaccard(kv_index *ix, Batch &b) {
   return KV_OK;
 }
 
-static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, int phase = 0) {
-  if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_topk_resident: no query batch uploaded");
-  if (k < 1 || k > 32) return kv_fail(KV_ERR_INVALID, "kv_topk: k must be 1..32");
-  KV_CUDA(cudaSetDevice(ix->device));
-  cudaStream_t s = ix->stream;
-  Batch b;
-  b.k = k; b.phase = phase; b.out_s = d_out_s; b.out_r = d_out_r;
+// Splits of the resident batch, pruned or exhaustive path, and the buffers of the candidate lists: sets b's sizes,
+// b.prune and the last_* launch counts.  Shared by the top-k batch and the threshold search.
+static int size_batch(kv_index *ix, Batch &b) {
   const int64_t n_q = b.n_q = ix->batch_q, n_tiles = b.n_tiles = ix->batch_tiles;
   const int64_t n_groups = b.n_groups = (n_q + GROUP_Q - 1) / GROUP_Q;
   const int64_t n_blocks = (ix->n_chunks + B_BN - 1) / B_BN;
   const char *env = getenv("KAKVEDA_B200_NO_PRUNE");
-  const bool prune = !(env && env[0] == '1') && !ix->jaccard && ix->n_chunks >= 512;
+  const bool prune = b.prune = !(env && env[0] == '1') && !ix->jaccard && ix->n_chunks >= 512;
   int64_t &n_bsplits = b.n_bsplits, &n_ssplits = b.n_ssplits;
   if (prune) {
     n_bsplits = std::max<int64_t>(1, std::min<int64_t>((ix->sm_count + n_tiles - 1) / n_tiles, n_blocks));
@@ -1119,14 +1138,6 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
   b.n_parts = n_bsplits * n_ssplits;
   b.n_ssplits_a = std::max<int64_t>(1, std::min<int64_t>((4LL * ix->sm_count + n_groups - 1) / n_groups, 8));
   ix->last_tiles = n_tiles; ix->last_splits = b.n_parts; ix->last_ctas = n_lists * n_ssplits;
-  if (n_q > ix->d_gthr.cap && (ix->gthr_exported || ix->n_peers))
-    return kv_fail(KV_ERR_STATE, "kv_topk: the query batch outgrew the threshold array shared with the peer GPUs; exchange it again "
-                                 "(kv_index_thresholds_export / kv_index_thresholds_peers)");
-  KV_CUDA(ix->d_gthr.ensure(n_q));
-  b.n_peers = (ix->n_peers > 0 && n_q <= ix->peer_cap) ? ix->n_peers : 0;
-  const int64_t parts_alloc = std::max(b.n_parts, b.n_ssplits_a);
-  KV_CUDA(ix->d_part_s.ensure(parts_alloc * n_q * k));
-  KV_CUDA(ix->d_part_r.ensure(parts_alloc * n_q * k));
   KV_CUDA(ix->d_stats.ensure(8));
   b.n_seed = (int)n_bsplits * B_SEEDS_PER_QUERY;
   const int64_t chunks_per_split = ((n_blocks + n_bsplits - 1) / n_bsplits + 1) * B_BN;
@@ -1144,6 +1155,30 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
     }
     KV_CUDA(ix->d_pool_ctl.ensure(2));
   }
+  if (prune && bound_smem_bytes(b.max_pages) > 232448)
+    return kv_fail(KV_ERR_INVALID, "kv_topk: index too large for one bound-kernel row range (max_pages %d)", b.max_pages);
+  return KV_OK;
+}
+
+static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, int phase = 0) {
+  if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_topk_resident: no query batch uploaded");
+  if (k < 1 || k > 32) return kv_fail(KV_ERR_INVALID, "kv_topk: k must be 1..32");
+  KV_CUDA(cudaSetDevice(ix->device));
+  cudaStream_t s = ix->stream;
+  Batch b;
+  b.k = k; b.phase = phase; b.out_s = d_out_s; b.out_r = d_out_r;
+  int rc = size_batch(ix, b);
+  if (rc != KV_OK) return rc;
+  const int64_t n_q = b.n_q;
+  const bool prune = b.prune;
+  if (n_q > ix->d_gthr.cap && (ix->gthr_exported || ix->n_peers))
+    return kv_fail(KV_ERR_STATE, "kv_topk: the query batch outgrew the threshold array shared with the peer GPUs; exchange it again "
+                                 "(kv_index_thresholds_export / kv_index_thresholds_peers)");
+  KV_CUDA(ix->d_gthr.ensure(n_q));
+  b.n_peers = (ix->n_peers > 0 && n_q <= ix->peer_cap) ? ix->n_peers : 0;
+  const int64_t parts_alloc = std::max(b.n_parts, b.n_ssplits_a);
+  KV_CUDA(ix->d_part_s.ensure(parts_alloc * n_q * k));
+  KV_CUDA(ix->d_part_r.ensure(parts_alloc * n_q * k));
   // Second pass without recomputation: the first bound pass stores every bound as an 8-bit code (n_q x chunks bytes)
   // when that fits comfortably (KAKVEDA_B200_BOUND_CODES=0 forces the recomputing second pass).
   b.use_codes = false;
@@ -1163,8 +1198,6 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
     }
   }
   if (phase != 2) ix->last_used_codes = b.use_codes ? 1 : 0;
-  if (prune && bound_smem_bytes(b.max_pages) > 232448)
-    return kv_fail(KV_ERR_INVALID, "kv_topk: index too large for one bound-kernel row range (max_pages %d)", b.max_pages);
 
   if (phase != 2) {
     KV_CUDA(cudaEventRecord(ix->ev[1], s));
@@ -1196,7 +1229,7 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
     ix->last_launches = b.launches + 2;
     return KV_OK;
   }
-  int rc = prune ? run_pruned(ix, b) : ix->jaccard ? run_jaccard(ix, b) : run_exhaustive(ix, b);
+  rc = prune ? run_pruned(ix, b) : ix->jaccard ? run_jaccard(ix, b) : run_exhaustive(ix, b);
   if (rc != KV_OK) return rc;
   if (phase == 1) { ix->last_launches = b.launches; return KV_OK; }
   KV_CUDA(cudaEventRecord(ix->evk[4], s));
@@ -1228,17 +1261,109 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
   return KV_OK;
 }
 
-// after the stream is synchronised: timings of the batch and the candidate-pool check
-static int finish_batch(kv_index *ix) {
-  for (int i = 1; i < 4; i++) cudaEventElapsedTime(&ix->last_ms[i], ix->ev[i], ix->ev[i + 1]);
-  for (int i = 0; i < 5; i++) cudaEventElapsedTime(&ix->last_kernel_ms[i], ix->evk[i], ix->evk[i + 1]);
-  if (ix->two_phase) cudaEventElapsedTime(&ix->last_kernel_ms[2], ix->evp2, ix->evk[3]);
+// after the stream is synchronised: whether the last run's bound pass ran out of candidate-pool pages
+static int check_pool(kv_index *ix) {
   const unsigned int *ctl = (const unsigned int *)&ix->last_stats[6];
   if (ix->n_rows > 0 && ctl[1] != 0) {
     ix->last_stats[6] = 0;
     return kv_fail(KV_ERR_NOMEM, "kv_topk: the candidate pool (%lld pages) is exhausted; split the query batch",
                    (long long)ix->pool_pages);
   }
+  return KV_OK;
+}
+
+// after the stream is synchronised: timings of the batch and the candidate-pool check
+static int finish_batch(kv_index *ix) {
+  for (int i = 1; i < 4; i++) cudaEventElapsedTime(&ix->last_ms[i], ix->ev[i], ix->ev[i + 1]);
+  for (int i = 0; i < 5; i++) cudaEventElapsedTime(&ix->last_kernel_ms[i], ix->evk[i], ix->evk[i + 1]);
+  if (ix->two_phase) cudaEventElapsedTime(&ix->last_kernel_ms[2], ix->evp2, ix->evk[3]);
+  return check_pool(ix);
+}
+
+// Threshold search over the resident batch: every pair with score >= thr lands in d_range, *n_pairs = their count.
+// When they do not fit, d_range grows to the exact count and only the scan and the fallbacks run again (the candidate
+// lists depend on the threshold alone).  Events: evk[2] -> evk[3] bound pass 1, evk[3] -> evk[4] scan, evk[4] -> evk[5]
+// irregular-query fallbacks.  Caller holds ix->mu.
+static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
+  ix->range_valid = false;
+  if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_range_resident: no query batch uploaded");
+  if (ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_range_resident: Jaccard indexes have no threshold search");
+  KV_CUDA(cudaSetDevice(ix->device));
+  cudaStream_t s = ix->stream;
+  Batch b;
+  b.k = 0; b.phase = 2; b.out_s = nullptr; b.out_r = nullptr; b.range = true; b.use_codes = false; b.n_peers = 0;
+  int rc = size_batch(ix, b);
+  if (rc != KV_OK) return rc;
+  const int64_t n_q = b.n_q;
+  KV_CUDA(ix->d_rthr.ensure(n_q));
+  KV_CUDA(ix->d_range.ensure(65536));
+  KV_CUDA(ix->d_range_count.ensure(1));
+  for (auto &e : ix->evk) KV_CUDA(cudaEventRecord(e, s));
+  KV_CUDA(cudaMemsetAsync(ix->d_stats.p, 0, 8 * sizeof(unsigned long long), s));
+  KV_CUDA(cudaMemsetAsync(ix->d_range_count.p, 0, sizeof(unsigned long long), s));
+  float ms[5] = {0, 0, 0, 0, 0};
+  unsigned long long count = 0;
+  if (ix->n_rows > 0) {
+    int thr_bits;
+    memcpy(&thr_bits, &thr, sizeof(thr_bits));
+    fill_int_kernel<<<(unsigned)((n_q + 255) / 256), 256, 0, s>>>(ix->d_rthr.p, n_q, thr_bits);
+    KV_CUDA(cudaGetLastError());
+    b.launches++;
+    for (int run = 0;; run++) {
+      if (run == 0 && b.prune) {
+        KV_CUDA(cudaMemsetAsync(ix->d_pool_ctl.p, 0, 2 * sizeof(unsigned int), s));
+        KV_CUDA(cudaEventRecord(ix->evk[2], s));
+        rc = run_pruned(ix, b);  // bound pass 1 (ends with evk[3]), then the scan
+      } else {
+        KV_CUDA(cudaEventRecord(ix->evk[3], s));
+        rc = b.prune ? scan_candidates(ix, b) : run_exhaustive(ix, b);
+      }
+      if (rc != KV_OK) return rc;
+      KV_CUDA(cudaEventRecord(ix->evk[4], s));
+      for (size_t i = 0; i < ix->irr_q.size(); i++) {
+        const int64_t q = ix->irr_q[i], a = ix->irr_indptr[i], e = ix->irr_indptr[i + 1];
+        rc = score_impl(ix, ix->irr_ids.data() + a, ix->irr_tf.data() + a, e - a, ix->irr_oov[i], nullptr);
+        if (rc != KV_OK) return rc;
+        const unsigned grid = (unsigned)std::min<int64_t>((ix->n_rows + 255) / 256, 8LL * ix->sm_count);
+        select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, thr,
+                                                 ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, (int)q, ix->d_range.p,
+                                                 ix->d_range_count.p, (unsigned long long)ix->d_range.cap);
+        KV_CUDA(cudaGetLastError());
+        b.launches += 2;
+      }
+      KV_CUDA(cudaEventRecord(ix->evk[5], s));
+      KV_CUDA(cudaMemcpyAsync(&count, ix->d_range_count.p, sizeof(count), cudaMemcpyDeviceToHost, s));
+      KV_CUDA(cudaMemcpyAsync(ix->last_stats, ix->d_stats.p, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+      if (b.prune) KV_CUDA(cudaMemcpyAsync(&ix->last_stats[6], ix->d_pool_ctl.p, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+      KV_CUDA(cudaStreamSynchronize(s));
+      if (run == 0 && b.prune) {
+        cudaEventElapsedTime(&ms[2], ix->evk[2], ix->evk[3]);
+        if ((rc = check_pool(ix)) != KV_OK) return rc;
+      }
+      float t_scan = 0, t_fallback = 0;
+      cudaEventElapsedTime(&t_scan, ix->evk[3], ix->evk[4]);
+      cudaEventElapsedTime(&t_fallback, ix->evk[4], ix->evk[5]);
+      ms[3] += t_scan;
+      ms[4] += t_fallback;
+      if (count <= (unsigned long long)ix->d_range.cap) break;
+      if (ix->d_range.ensure((int64_t)count) != cudaSuccess) {
+        cudaGetLastError();
+        return kv_fail(KV_ERR_NOMEM, "kv_range_resident: %llu pairs reach the threshold; their buffer does not fit in device memory "
+                                     "(raise the threshold or split the query batch)", count);
+      }
+      // the counters describe one run: the bound pass's stay, the scan's start again
+      KV_CUDA(cudaMemsetAsync(ix->d_stats.p, 0, 2 * sizeof(unsigned long long), s));
+      KV_CUDA(cudaMemsetAsync(ix->d_range_count.p, 0, sizeof(unsigned long long), s));
+    }
+  } else {
+    for (auto &st : ix->last_stats) st = 0;
+  }
+  for (int i = 0; i < 5; i++) ix->last_kernel_ms[i] = ms[i];
+  ix->last_launches = b.launches;
+  ix->range_q = n_q;
+  ix->range_pairs = (int64_t)count;
+  ix->range_valid = true;
+  *n_pairs = (int64_t)count;
   return KV_OK;
 }
 
@@ -1452,6 +1577,54 @@ int kv_topk_resident_host(kv_index *ix, int k, float *out_scores, int64_t *out_r
   KV_CUDA(cudaEventRecord(ix->ev[4], ix->stream));
   KV_CUDA(cudaStreamSynchronize(ix->stream));
   return finish_batch(ix);
+}
+
+int kv_range_resident(kv_index *ix, float threshold, int64_t *n_pairs) {
+  if (!ix || !n_pairs) return kv_fail(KV_ERR_INVALID, "kv_range_resident: bad arguments");
+  if (!(threshold > 0.f && threshold <= 1.f)) return kv_fail(KV_ERR_INVALID, "kv_range_resident: threshold must be in (0, 1]");
+  std::lock_guard<std::mutex> g(ix->mu);
+  return run_range(ix, threshold, n_pairs);
+}
+
+// The pairs come back in emit order, which the scan does not fix; scores are exact integer sums rounded once, so
+// (score desc, row asc) is a total order of each query's pairs and the result is deterministic.
+int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores) {
+  if (!ix || !indptr) return kv_fail(KV_ERR_INVALID, "kv_range_fetch: bad arguments");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (!ix->range_valid) return kv_fail(KV_ERR_STATE, "kv_range_fetch: no threshold search result (kv_range_resident first)");
+  const int64_t n_q = ix->range_q, n = ix->range_pairs;
+  if (n > 0 && (!rows || !scores)) return kv_fail(KV_ERR_INVALID, "kv_range_fetch: bad arguments");
+  KV_CUDA(cudaSetDevice(ix->device));
+  KV_CUDA(ix->h_range.ensure(std::max<int64_t>(n, 1)));
+  if (n) {
+    KV_CUDA(cudaMemcpyAsync(ix->h_range.p, ix->d_range.p, (size_t)n * sizeof(RangePair), cudaMemcpyDeviceToHost, ix->stream));
+    KV_CUDA(cudaStreamSynchronize(ix->stream));
+  }
+  // counting sort by query, then each query's segment by (score desc, row asc)
+  const RangePair *rec = ix->h_range.p;
+  std::vector<RangePair> by_q;
+  try {
+    by_q.resize((size_t)n);
+  } catch (const std::bad_alloc &) {
+    return kv_fail(KV_ERR_NOMEM, "kv_range_fetch: out of host memory");
+  }
+  for (int64_t q = 0; q <= n_q; q++) indptr[q] = 0;
+  for (int64_t i = 0; i < n; i++) indptr[rec[i].q + 1]++;
+  for (int64_t q = 0; q < n_q; q++) indptr[q + 1] += indptr[q];
+  std::vector<int64_t> next(indptr, indptr + n_q);
+  for (int64_t i = 0; i < n; i++) by_q[(size_t)next[(size_t)rec[i].q]++] = rec[i];
+  parallel_for(n_q, n >= 65536 ? host_threads() : 1, [&](int, int64_t a, int64_t b) {
+    for (int64_t q = a; q < b; q++) {
+      RangePair *lo = by_q.data() + indptr[q], *hi = by_q.data() + indptr[q + 1];
+      std::sort(lo, hi, [](const RangePair &x, const RangePair &y) { return x.score != y.score ? x.score > y.score : x.row < y.row; });
+      for (RangePair *p = lo; p < hi; p++) {
+        rows[p - by_q.data()] = p->row;
+        scores[p - by_q.data()] = p->score;
+      }
+    }
+  });
+  ix->range_valid = false;
+  return KV_OK;
 }
 
 int kv_index_thresholds_export(kv_index *ix, int64_t capacity, void *handle_out) {

@@ -514,7 +514,16 @@ __host__ __device__ __forceinline__ uint32_t rt_slot(uint32_t fid, uint32_t size
 // completion; double buffered, so the next block lands while this one is scored) and scores it for each query of the
 // mask: lanes probe 32 block entries at a time in the query's table, hits add their fixed-point weights to the rows
 // of their masks, lane = row.  Survivors of the division-free pre-test enter the query's sorted list under a lock.
+// K1b-R (RANGE = true) is the same scan for a threshold search: the filter is the query's fixed threshold and every
+// row that reaches it is appended to a global pair buffer instead of a top-k list.
 // ----------------------------------------------------------------------------------------
+// One match of a threshold search (16 bytes)
+struct RangePair {
+  int32_t q;    // original query index
+  float score;  // the float32 score the top-k path reports for the pair
+  int64_t row;  // global row
+};
+
 struct ScanParams {
   const uint32_t *blk;
   const BlockInfo *binfo;
@@ -545,7 +554,26 @@ struct ScanParams {
   int k;
   float *part_scores;  // [n_bsplits * n_ssplits][n_q][k]
   long long *part_rows;
+  // threshold search (tfidf_scan_kernel<true>): gthr holds the fixed threshold, k is 0, matches are appended here
+  const int *qperm;                  // [n_q] sorted slot -> original query
+  RangePair *range_out;              // [range_cap]
+  unsigned long long *range_count;   // matches found (may exceed range_cap: those past it are not written)
+  unsigned long long range_cap;
 };
+
+// Appends the pairs (*q, score, row) of the lanes with `hit` set: one reservation per warp
+__device__ __forceinline__ void range_emit(RangePair *out, unsigned long long *count, unsigned long long cap, bool hit,
+                                           const int *q, float score, int64_t row) {
+  const uint32_t hm = __ballot_sync(FULL, hit);
+  if (hm == 0) return;
+  unsigned long long base = 0;
+  if ((threadIdx.x & 31) == 0) base = atomicAdd(count, (unsigned long long)__popc(hm));
+  base = __shfl_sync(FULL, base, 0);
+  if (hit) {
+    const unsigned long long o = base + (unsigned long long)__popc(hm & lanemask_lt());
+    if (o < cap) out[o] = RangePair{*q, score, row};
+  }
+}
 
 constexpr int S_WARPS = 8;
 constexpr int S_BUF_ENTRIES = 256;  // a staged block holds up to this many entries (larger blocks are read in place)
@@ -563,6 +591,7 @@ __device__ __forceinline__ void bulk_copy_g2s(void *dst, const void *src, uint32
                : "memory");
 }
 
+template <bool RANGE>
 __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams P) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int k = P.k;
@@ -772,11 +801,16 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
           const float dot = s_dotU[qi] + __ull2float_rn(acc_w) * (1.f / 4294967296.f);
           const float corr = s_corrU[qi] - __ull2float_rn(acc_c) * (1.f / 16777216.f);
           const float t = Bc + corr;
-          // optimistic filter (read without the lock): the list's k-th SCORE once it is full, and the global lower bound
-          // of the k-th score.  Scores only ever rise, so a stale value merely lets a few more rows through; rows tying
-          // with it are let through as well -- the exact (score desc, row asc) comparison happens under the lock.
-          float filt = __int_as_float(*(volatile int *)&P.gthr[q0 + qi]);
-          if (*(volatile int *)&s_cnt[qi] == k) filt = fmaxf(filt, *(volatile float *)&s_lscore[qi * k + k - 1]);
+          float filt;
+          if constexpr (RANGE) {
+            filt = __int_as_float(P.gthr[q0 + qi]);  // the search threshold: fixed for the whole scan
+          } else {
+            // optimistic filter (read without the lock): the list's k-th SCORE once it is full, and the global lower
+            // bound of the k-th score.  Scores only ever rise, so a stale value merely lets a few more rows through; rows
+            // tying with it are let through as well -- the exact (score desc, row asc) comparison happens under the lock.
+            filt = __int_as_float(*(volatile int *)&P.gthr[q0 + qi]);
+            if (*(volatile int *)&s_cnt[qi] == k) filt = fmaxf(filt, *(volatile float *)&s_lscore[qi * k + k - 1]);
+          }
           bool pass = true;
           if (filt > 0.f) pass = dot * dot >= filt * filt * nq * FILTER_SLACK * t;
           if (pass) {
@@ -785,6 +819,10 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
             row = P.perm[pos0 + lane];
             cand = row != s_excl[qi] && sc >= filt;
           }
+        }
+        if constexpr (RANGE) {
+          range_emit(P.range_out, P.range_count, P.range_cap, cand, P.qperm + q0 + qi, sc, P.row_base + row);
+          continue;
         }
         const uint32_t cm = __ballot_sync(FULL, cand);
         if (cm) {
@@ -836,14 +874,15 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
     atomicAdd(&s_stat[1], recs_done);
   }
   __syncthreads();
-  // publish this CTA's partial lists (already ordered)
-  const int part = bsplit * P.n_ssplits + ssplit;
-  for (int i = threadIdx.x; i < q_count * k; i += blockDim.x) {
-    const int qi = i / k, j = i - qi * k;
-    const size_t o = ((size_t)part * P.n_q + (q0 + qi)) * k + j;
-    const bool used = j < s_cnt[qi];
-    P.part_scores[o] = used ? s_lscore[i] : -INFINITY;
-    P.part_rows[o] = used ? (long long)(P.row_base + s_lrow[i]) : -1LL;
+  if constexpr (!RANGE) {  // publish this CTA's partial lists (already ordered)
+    const int part = bsplit * P.n_ssplits + ssplit;
+    for (int i = threadIdx.x; i < q_count * k; i += blockDim.x) {
+      const int qi = i / k, j = i - qi * k;
+      const size_t o = ((size_t)part * P.n_q + (q0 + qi)) * k + j;
+      const bool used = j < s_cnt[qi];
+      P.part_scores[o] = used ? s_lscore[i] : -INFINITY;
+      P.part_rows[o] = used ? (long long)(P.row_base + s_lrow[i]) : -1LL;
+    }
   }
   if (threadIdx.x == 0 && P.stats) {
     atomicAdd(&P.stats[0], (unsigned long long)s_stat[0]);
@@ -1225,6 +1264,20 @@ __global__ void select_topk_kernel(const double *__restrict__ scores, int64_t n,
       }
     }
     __syncthreads();
+  }
+}
+
+// Fallback of a threshold search for one (irregular) query: every row whose float64 score, rounded to the float32
+// select_topk_kernel reports, reaches the threshold is appended to the pair buffer.
+__global__ void select_range_kernel(const double *__restrict__ scores, int64_t n, int64_t row_base, float thr, int64_t excl,
+                                    int q, RangePair *out, unsigned long long *count, unsigned long long cap) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int qv = q;
+  // whole warps step together (blockDim is a multiple of 32): range_emit needs every lane
+  for (int64_t r0 = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) & ~31LL; r0 < n; r0 += stride) {
+    const int64_t r = r0 + (threadIdx.x & 31);
+    const float s = r < n ? (float)scores[r] : -INFINITY;
+    range_emit(out, count, cap, r < n && r != excl && s >= thr, &qv, s, row_base + r);
   }
 }
 

@@ -4,8 +4,8 @@ The reference's pattern detector (services/pattern_detector/app.py:28-60) pulls 
 those whose ``failure_type`` equals the event's, and upserts ONE named pattern when they span >= 2 apps.  This module
 keeps that contract (``pattern_payload`` builds the same ``/patterns/upsert`` body: sorted unique failure_ids and
 affected_apps, app.py:41-43,50-56) but can split a failure type into several patterns by similarity: every row's k
-nearest other rows come from the device self-join, rows whose similarity reaches the threshold are linked, connected
-components are the candidate patterns.  The grouping by similarity is an extension (the reference has none); its oracle
+nearest other rows (or, with ``k=None``, every other row above the threshold) come from the device self-join, rows
+whose similarity reaches the threshold are linked, connected components are the candidate patterns.  The grouping by similarity is an extension (the reference has none); its oracle
 is a Python union-find over the float64 all-pairs matrix (tests).
 """
 from __future__ import annotations
@@ -31,6 +31,19 @@ def cluster_topk(rows: np.ndarray, scores: np.ndarray, threshold: float) -> Tupl
     return labels, int(count.value)
 
 
+def cluster_csr(indptr: np.ndarray, rows: np.ndarray) -> Tuple[np.ndarray, int]:
+    """labels[i] = smallest row id of i's component in the graph {i ~ rows[j] : indptr[i] <= j < indptr[i+1], rows[j] >= 0}."""
+    indptr = np.ascontiguousarray(indptr, dtype=np.int64)
+    rows = np.ascontiguousarray(rows, dtype=np.int64)
+    n = len(indptr) - 1
+    labels = np.empty(n, dtype=np.int64)
+    count = C.c_int64(0)
+    _capi.check(_capi.load().kv_cluster_csr(n, indptr.ctypes.data_as(C.POINTER(C.c_int64)),
+                                            rows.ctypes.data_as(C.POINTER(C.c_int64)),
+                                            labels.ctypes.data_as(C.POINTER(C.c_int64)), C.byref(count)))
+    return labels, int(count.value)
+
+
 def pattern_payload(name: str, records: Sequence[Mapping[str, Any]], description: Optional[str] = None) -> Dict[str, Any]:
     """The ``/patterns/upsert`` body the reference builds from a group of failures (app.py:41-43,50-56)."""
     affected = sorted(set(sum([list(r.get("affected_apps", [])) for r in records], [])))
@@ -38,23 +51,35 @@ def pattern_payload(name: str, records: Sequence[Mapping[str, Any]], description
     return {"name": name, "failure_ids": failure_ids, "affected_apps": affected, "description": description}
 
 
-def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: float = 0.8, k: int = 32,
+def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: float = 0.8, k: Optional[int] = 32,
                     min_apps: int = 2, failure_type: Optional[str] = None) -> List[Dict[str, Any]]:
     """Similarity-split version of pattern_detector.on_failure.
 
     ``index``: a finalized ``GfkbIndex`` whose row i is ``records[i]['signature_text']`` (corpus-fit mode gives a
     symmetric measure; the default mode works too).  Returns one payload per connected component that, restricted
     to ``failure_type`` (if given), spans at least ``min_apps`` apps (app.py:45-46) -- ordered by smallest row id.
+    ``k``: rows are linked only through every row's k nearest other rows, so when a text is stored more than k times
+    its copies fill the lists and pairs of similar texts are never seen.  ``k=None`` links on the exact threshold
+    graph (``selfjoin_range``).
     """
-    scores, rows = index.selfjoin_topk(k)
-    keep = np.ones(len(records), dtype=bool)
+    n = len(records)
+    keep = np.ones(n, dtype=bool)
     if failure_type is not None:
-        keep = np.fromiter((r.get("failure_type") == failure_type for r in records), dtype=bool, count=len(records))
-        # rows of other failure types neither join nor bridge components
-        bad = ~keep[np.clip(rows, 0, len(records) - 1)] | (rows < 0)
-        scores = np.where(bad, -np.inf, scores).astype(np.float32)
-        scores[~keep] = -np.inf
-    labels, _ = cluster_topk(rows, scores, threshold)
+        keep = np.fromiter((r.get("failure_type") == failure_type for r in records), dtype=bool, count=n)
+    if k is None:
+        indptr, rows, _ = index.selfjoin_range(threshold)
+        if failure_type is not None:  # rows of other failure types neither join nor bridge components
+            src = np.repeat(np.arange(n), np.diff(indptr))
+            rows = np.where(keep[src] & keep[rows], rows, -1)
+        labels, _ = cluster_csr(indptr, rows)
+    else:
+        scores, rows = index.selfjoin_topk(k)
+        if failure_type is not None:
+            # rows of other failure types neither join nor bridge components
+            bad = ~keep[np.clip(rows, 0, n - 1)] | (rows < 0)
+            scores = np.where(bad, -np.inf, scores).astype(np.float32)
+            scores[~keep] = -np.inf
+        labels, _ = cluster_topk(rows, scores, threshold)
     groups: Dict[int, List[int]] = {}
     for i, lab in enumerate(labels.tolist()):
         if keep[i]:

@@ -355,6 +355,42 @@ class GfkbIndex:
         _capi.check(_capi.load().kv_selfjoin_upload(self._h, lo, hi))
         return self.topk_resident_host(hi - lo, k)
 
+    def _range_resident(self, n_q: int, threshold: float) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        lib = _capi.load()
+        n = C.c_int64(0)
+        _capi.check(lib.kv_range_resident(self._h, np.float32(threshold), C.byref(n)))
+        indptr = np.empty(n_q + 1, dtype=np.int64)
+        rows = np.empty(n.value, dtype=np.int64)
+        scores = np.empty(n.value, dtype=np.float32)
+        _capi.check(lib.kv_range_fetch(self._h, _ptr(indptr, C.c_int64), _ptr(rows, C.c_int64), _ptr(scores, C.c_float)))
+        return indptr, rows, scores
+
+    def range_features(self, fb: FeatureBatch, threshold: float) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """Threshold search: every (query, row) pair whose float32 score (the value ``topk`` reports) is >= ``threshold``,
+        0 < threshold <= 1.  Returns ``(indptr int64[n_q+1], rows int64[P], scores float32[P])``: query q's pairs are
+        ``[indptr[q], indptr[q+1])``, ordered by (score desc, row asc); rows are global."""
+        if fb.n == 0:
+            return np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32)
+        self.upload_queries(fb)
+        return self._range_resident(fb.n, threshold)
+
+    def range(self, queries: Sequence[str], threshold: float) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """``range_features`` of texts."""
+        fb = self.vocab.featurize(queries, grow=False)
+        try:
+            return self.range_features(fb, threshold)
+        finally:
+            fb.close()
+
+    def selfjoin_range(self, threshold: float, lo: int = 0, hi: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """All-pairs threshold search: for local rows [lo, hi) every OTHER row scoring >= ``threshold`` (CSR as in
+        ``range_features``, query i = row lo + i)."""
+        hi = self.n_rows if hi is None else hi
+        if hi <= lo:
+            return np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32)
+        _capi.check(_capi.load().kv_selfjoin_upload(self._h, lo, hi))
+        return self._range_resident(hi - lo, threshold)
+
     def rescore(self, fb: FeatureBatch, rows: np.ndarray) -> np.ndarray:
         """K6: float64 scores of the pairs (query q, GLOBAL row rows[q, j]); identical rows tie exactly on every shard."""
         rows = np.ascontiguousarray(rows, dtype=np.int64)
