@@ -316,7 +316,24 @@ int kv_dense_topk_device(kv_dense_index *dx, const void *d_q_bf16, int64_t n_q, 
 /* All-pairs on one shard without copying: local rows [q_begin, q_end) are the queries, each row's own entry is
  * excluded, results (device) as above. */
 int kv_dense_selfjoin_device(kv_dense_index *dx, int64_t q_begin, int64_t q_end, int k, void *d_scores, void *d_rows);
-/* CUDA-event milliseconds of the GEMM+top-k kernel of the last kv_dense_topk and its row splits. */
+/* Threshold search (K2-R, the same GEMM with an emitting epilogue): every (query, row) pair whose cosine -- the float32
+ * value kv_dense_topk reports for that pair, bit for bit -- is >= threshold, 0 < threshold <= 1.  Rows are global
+ * (row_base applied); q is the query's index within the call (row - q_begin for the self-join, which excludes each
+ * row's own entry; exclude_base as in kv_dense_topk_device).  *n_pairs receives the count; the pairs stay in the handle
+ * until kv_dense_range_fetch or the next range, top-k, append or finalize call.  The pair buffer starts at 65,536
+ * records and keeps its capacity; when a search finds more pairs it grows to the exact count and the whole kernel,
+ * GEMM included, runs again.  threshold NaN, <= 0 or > 1, n_q >= 2^31, or device queries not 16-byte aligned:
+ * KV_ERR_INVALID.  Index not finalized: KV_ERR_STATE.  KV_ERR_NOMEM when the pairs do not fit in device memory (the
+ * message gives their count). */
+int kv_dense_range(kv_dense_index *dx, const uint16_t *q_bf16, int64_t n_q, float threshold, int64_t *n_pairs);
+int kv_dense_range_device(kv_dense_index *dx, const void *d_q_bf16, int64_t n_q, float threshold,
+                          int64_t exclude_base, int64_t *n_pairs);
+int kv_dense_selfjoin_range(kv_dense_index *dx, int64_t q_begin, int64_t q_end, float threshold, int64_t *n_pairs);
+/* The last dense range result (host outputs): indptr[n_q+1] by query, rows[n_pairs], scores[n_pairs]; per query ordered
+ * by (score desc, row asc).  KV_ERR_STATE when there is none. */
+int kv_dense_range_fetch(kv_dense_index *dx, int64_t *indptr, int64_t *rows, float *scores);
+/* CUDA-event milliseconds of the GEMM kernel of the last kv_dense_topk* / kv_dense_selfjoin_device or range call (a
+ * range re-run after the pair buffer grew included) and its row splits. */
 int kv_dense_last_timing(const kv_dense_index *dx, float *gemm_ms, int64_t *splits);
 
 /* ------------------------------------------------------------------------------------

@@ -94,6 +94,10 @@ SIGNATURES = {
     "kv_dense_append_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64]),
     "kv_dense_topk_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p]),
     "kv_dense_selfjoin_device": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
+    "kv_dense_range": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint16), C.c_int64, C.c_float, c_i64p]),
+    "kv_dense_range_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_int64, c_i64p]),
+    "kv_dense_selfjoin_range": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_float, c_i64p]),
+    "kv_dense_range_fetch": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f32p]),
     "kv_dense_last_timing": (C.c_int, [C.c_void_p, c_f32p, c_i64p]),
     "kv_hash_create": (C.c_int, [C.c_int, C.c_int64, C.POINTER(C.c_void_p)]),
     "kv_hash_destroy": (None, [C.c_void_p]),

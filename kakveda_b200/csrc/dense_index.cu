@@ -21,6 +21,9 @@
 // While the consumers run a tile's epilogue, the producer already fills the ring with the next tile's first slices.
 // Each (query tile, split, column half) writes one partial list; K5 (kv_merge_topk_device) merges them.  CTAs
 // working on the same queries exchange k-th-score lower bounds through global memory (gthr).
+// K2-R (dense_topk_kernel<true>) is the same kernel for a threshold search: producer, ring, MMAs and register exchange
+// are unchanged; the epilogue keeps no lists and appends every pair whose score (the same float32 expression) reaches
+// the threshold to a global pair buffer, one reservation per warp and 16-column group (dense_emit).
 #include "kv_cuda.cuh"
 #include "sm90.cuh"
 
@@ -95,6 +98,16 @@ struct DenseParams {
   long long *part_rows;
 };
 
+// Output of the threshold search (dense_topk_kernel<true>, which leaves k, gthr and the partial lists of DenseParams
+// unused; the top-k form ignores this argument).  A kernel argument of its own: added to DenseParams it changes the
+// top-k form's register allocation.
+struct DenseRangeOut {
+  float thr;                  // every pair whose score is >= thr is appended
+  RangePair *out;             // [cap]
+  unsigned long long *count;  // pairs found (may exceed cap: those past it are not written)
+  unsigned long long cap;
+};
+
 // order-preserving float <-> unsigned key (cosines may be negative)
 __device__ __forceinline__ unsigned int fkey(float f) {
   unsigned int b = __float_as_uint(f);
@@ -112,8 +125,42 @@ struct __align__(1024) DenseSmem {
   int lrow[2][MAXK][BM];
 };
 
+// K2-R: appends this thread's pairs of one 16-column group (columns c0 + {0, 1, 4, 5, 8, 9, 12, 13} of the tile at
+// row0): (q, tv[e] * inv_q, global row) for each element whose score reaches R.thr, whose row exists and is not the
+// excluded one.  All 32 lanes call it; the warp reserves its records with one atomic (none when no lane has a hit).
+__device__ __forceinline__ void dense_emit(const DenseParams &P, const DenseRangeOut &R, const float (&tv)[8], float inv_q, int q,
+                                           int64_t row0, int c0, int excl) {
+  const int lane = threadIdx.x & 31;
+  uint32_t hits = 0;
+#pragma unroll
+  for (int e = 0; e < 8; e++) {
+    const int64_t r = row0 + c0 + 8 * (e >> 2) + 4 * ((e >> 1) & 1) + (e & 1);
+    if (tv[e] * inv_q >= R.thr && r < P.n_rows && (int)r != excl) hits |= 1u << e;
+  }
+  const int nh = __popc(hits);
+  int incl = nh;  // inclusive prefix sum of the warp's hit counts: lane 31 holds the total
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+    if (lane >= o) incl += v;
+  }
+  unsigned long long base = 0;
+  if (lane == 31 && incl > 0) base = atomicAdd(R.count, (unsigned long long)incl);
+  unsigned long long o = __shfl_sync(0xFFFFFFFFu, base, 31) + (unsigned long long)(incl - nh);
+#pragma unroll
+  for (int e = 0; e < 8; e++) {
+    if (hits & (1u << e)) {
+      const int64_t r = row0 + c0 + 8 * (e >> 2) + 4 * ((e >> 1) & 1) + (e & 1);
+      if (o < R.cap) R.out[o] = RangePair{q, tv[e] * inv_q, P.row_base + r};
+      o++;
+    }
+  }
+}
+
+template <bool RANGE>
 __global__ void __launch_bounds__(N_THREADS, 1)
-dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c, DenseParams P) {
+dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c, DenseParams P,
+                  DenseRangeOut R) {
   extern __shared__ unsigned char smem_raw[];
   DenseSmem &S = *reinterpret_cast<DenseSmem *>(smem_raw + smem_align1024(smem_raw));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -215,7 +262,7 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
       if (qtile != cur_qtile) {  // (CTA-uniform) next query tile: publish and restart the lists
-        flush();
+        if constexpr (!RANGE) flush();
         cur_qtile = qtile;
         q = (int64_t)qtile * BM + qi;
         q_ok = q < P.n_q;
@@ -224,21 +271,25 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
           const int64_t e = P.excl_base >= 0 ? P.excl_base + q - P.row_base : -1;
           excl = (e >= 0 && e < P.n_rows) ? (int)e : -1;
         }
-        cnt = 0;
-        thr = gth = gth_pred = -INFINITY;
-        lo = q_ok ? -INFINITY : INFINITY;
-        for (int j = 0; j < k; j++) { ls[j * BM] = -INFINITY; lr[j * BM] = 0x7fffffff; }
+        if constexpr (!RANGE) {
+          cnt = 0;
+          thr = gth = gth_pred = -INFINITY;
+          lo = q_ok ? -INFINITY : INFINITY;
+          for (int j = 0; j < k; j++) { ls[j * BM] = -INFINITY; lr[j * BM] = 0x7fffffff; }
+        }
       }
       const int as = (int)(it & 1);
       // inverse norms of this tile's rows (0 past the end; such rows are rejected by index below)
       const int64_t row0 = t * BN;
       for (int c = et; c < BN; c += EPI_THREADS) S.inv_c[as][c] = (row0 + c < P.n_rows) ? P.inv_norm_c[row0 + c] : -INFINITY;  // 0 * -inf = NaN: never a candidate
-      if (q_ok) {
-        const unsigned int gk = *(volatile unsigned int *)&P.gthr[q];
-        if (gk > fkey(-INFINITY) && fkey_inv(gk) > gth) {
-          gth = fkey_inv(gk);
-          gth_pred = fkey_inv(gk - 1);  // the order-preserving key makes "previous float" a decrement
-          lo = fmaxf(thr, gth_pred);
+      if constexpr (!RANGE) {
+        if (q_ok) {
+          const unsigned int gk = *(volatile unsigned int *)&P.gthr[q];
+          if (gk > fkey(-INFINITY) && fkey_inv(gk) > gth) {
+            gth = fkey_inv(gk);
+            gth_pred = fkey_inv(gk - 1);  // the order-preserving key makes "previous float" a decrement
+            lo = fmaxf(thr, gth_pred);
+          }
         }
       }
       asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -278,28 +329,36 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
         const float m01 = fmaxf(tv[0], tv[1]), m23 = fmaxf(tv[2], tv[3]);
         const float m45 = fmaxf(tv[4], tv[5]), m67 = fmaxf(tv[6], tv[7]);
         const float best = fmaxf(fmaxf(m01, m23), fmaxf(m45, m67)) * inv_q;
-        if (best > lo) {
+        if constexpr (RANGE) {
+          // inv_q > 0 and rounding is monotone, so no score of the group reaches thr unless best does (zero and
+          // padded queries have inv_q = 0: best is 0 or NaN)
+          if (__any_sync(FULL_MASK, best >= R.thr)) dense_emit(P, R, tv, inv_q, (int)q, row0, 16 * sb + cofs, excl);
+        } else {
+          if (best > lo) {
 #pragma unroll  // static indices keep tv[] in registers
-          for (int e = 0; e < 8; e++) {
-            const float sc = tv[e] * inv_q;
-            const int col = 8 * (2 * sb + (e >> 2)) + cofs + (e & 1) + 4 * ((e >> 1) & 1);
-            if (sc > lo && (int)(row0 + col) != excl) {
-              int pos = cnt < k ? cnt++ : k - 1;
-              while (pos > 0 && ls[(pos - 1) * BM] < sc) {
-                ls[pos * BM] = ls[(pos - 1) * BM];
-                lr[pos * BM] = lr[(pos - 1) * BM];
-                pos--;
+            for (int e = 0; e < 8; e++) {
+              const float sc = tv[e] * inv_q;
+              const int col = 8 * (2 * sb + (e >> 2)) + cofs + (e & 1) + 4 * ((e >> 1) & 1);
+              if (sc > lo && (int)(row0 + col) != excl) {
+                int pos = cnt < k ? cnt++ : k - 1;
+                while (pos > 0 && ls[(pos - 1) * BM] < sc) {
+                  ls[pos * BM] = ls[(pos - 1) * BM];
+                  lr[pos * BM] = lr[(pos - 1) * BM];
+                  pos--;
+                }
+                ls[pos * BM] = sc;
+                lr[pos * BM] = (int)(row0 + col);
+                if (cnt == k) { thr = ls[(k - 1) * BM]; lo = fmaxf(thr, gth_pred); }
               }
-              ls[pos * BM] = sc;
-              lr[pos * BM] = (int)(row0 + col);
-              if (cnt == k) { thr = ls[(k - 1) * BM]; lo = fmaxf(thr, gth_pred); }
             }
           }
         }
       }
-      if (q_ok && cnt == k && thr > gth) atomicMax(&P.gthr[q], fkey(thr));
+      if constexpr (!RANGE) {
+        if (q_ok && cnt == k && thr > gth) atomicMax(&P.gthr[q], fkey(thr));
+      }
     }
-    flush();
+    if constexpr (!RANGE) flush();
   }
 }
 
@@ -332,6 +391,12 @@ struct kv_dense_index {
   DevBuf<long long> d_part_r, d_out_r;
   DevBuf<__nv_bfloat16> d_q;
   DevBuf<unsigned int> d_gthr;
+  // last threshold search: pairs in emit order, kept until fetched or until the next range, top-k, append or finalize
+  DevBuf<RangePair> d_range;
+  DevBuf<unsigned long long> d_range_count;
+  PinnedBuf<RangePair> h_range;
+  bool range_valid = false;
+  int64_t range_q = 0, range_pairs = 0;
   bool finalized = false;
   float last_ms = 0;
   int64_t last_splits = 0;
@@ -352,7 +417,8 @@ int kv_dense_create(int device, int dim, int64_t row_base, kv_dense_index **out)
   dx->sm_count = sm_count;
   KV_CUDA(dx->stream.create());
   for (auto &e : dx->ev) KV_CUDA(e.create());
-  KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
+  KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
+  KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
   *out = dx.release();
   return KV_OK;
 }
@@ -371,6 +437,7 @@ int kv_dense_append(kv_dense_index *dx, const uint16_t *rows_bf16, int64_t n) {
   if (!dx || n < 0 || (n > 0 && !rows_bf16)) return kv_fail(KV_ERR_INVALID, "kv_dense_append: bad arguments");
   if (n == 0) return KV_OK;
   std::lock_guard<std::mutex> g(dx->mu);
+  dx->range_valid = false;
   KV_CUDA(cudaSetDevice(dx->device));
   if (dx->n_rows + n >= (1LL << 31) - BN) return kv_fail(KV_ERR_INVALID, "kv_dense_append: more than 2^31 rows in one shard");
   KV_CUDA(dx->rows.reserve((dx->n_rows + n) * dx->dim, dx->stream));
@@ -385,6 +452,7 @@ int kv_dense_append(kv_dense_index *dx, const uint16_t *rows_bf16, int64_t n) {
 int kv_dense_finalize(kv_dense_index *dx) {
   if (!dx) return kv_fail(KV_ERR_INVALID, "kv_dense_finalize: NULL handle");
   std::lock_guard<std::mutex> g(dx->mu);
+  dx->range_valid = false;
   KV_CUDA(cudaSetDevice(dx->device));
   KV_CUDA(dx->d_inv_c.ensure(std::max<int64_t>(dx->n_rows, 1)));
   if (dx->n_rows) {
@@ -396,24 +464,18 @@ int kv_dense_finalize(kv_dense_index *dx) {
   return KV_OK;
 }
 
-// scan + merge of n_q queries already on the device (d_q: bf16 [n_q, dim], 16-byte aligned) into device buffers
-static int dense_run(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, int k, int64_t excl_base, float *d_out_s,
-                     long long *d_out_r) {
+// What the top-k and the range scan of n_q queries already on the device (d_q: bf16 [n_q, dim], 16-byte aligned)
+// share: the queries' inverse norms, both tensor maps, the row splits (dx->last_splits) and every DenseParams field but
+// the epilogue's.  Needs n_rows > 0.
+static int dense_setup(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, int64_t excl_base, CUtensorMap *map_q,
+                       CUtensorMap *map_c, DenseParams &P) {
   cudaStream_t s = dx->stream;
-  if (dx->n_rows == 0) {
-    KV_CUDA(cudaMemsetAsync(d_out_r, 0xFF, (size_t)n_q * k * 8, s));  // row -1
-    std::vector<float> neg((size_t)(n_q * k), -INFINITY);
-    KV_CUDA(cudaMemcpyAsync(d_out_s, neg.data(), neg.size() * 4, cudaMemcpyHostToDevice, s));
-    KV_CUDA(cudaStreamSynchronize(s));
-    return KV_OK;
-  }
   KV_CUDA(dx->d_inv_q.ensure(n_q));
   inv_norm_kernel<<<(unsigned)((n_q * 32 + 255) / 256), 256, 0, s>>>(d_q, n_q, dx->dim, dx->d_inv_q.p);
   KV_CUDA(cudaGetLastError());
-  CUtensorMap map_q, map_c;
-  int rc = make_map_2d(&map_q, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, d_q, n_q, dx->dim, BM);
+  int rc = make_map_2d(map_q, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, d_q, n_q, dx->dim, BM);
   if (rc != KV_OK) return rc;
-  rc = make_map_2d(&map_c, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, dx->rows.p, dx->n_rows, dx->dim, BN);
+  rc = make_map_2d(map_c, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, dx->rows.p, dx->n_rows, dx->dim, BN);
   if (rc != KV_OK) return rc;
   const int64_t q_tiles = (n_q + BM - 1) / BM, r_tiles = (dx->n_rows + BN - 1) / BN;
   // row splits: as few as possible (long row ranges keep the k-th-score thresholds high) while the CTA count
@@ -430,28 +492,99 @@ static int dense_run(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, 
     n_lists = std::max<int64_t>(1, std::min<int64_t>(n_lists, r_tiles));
   }
   dx->last_splits = n_lists;
-  const int64_t n_part = n_lists * 2;  // two epilogue threads (column halves) per query and CTA
+  P = DenseParams{};
+  P.n_rows = dx->n_rows; P.row_base = dx->row_base; P.n_q = n_q; P.dim = dx->dim; P.n_lists = (int)n_lists;
+  P.excl_base = excl_base;
+  P.r_tiles = r_tiles; P.q_tiles = q_tiles;
+  P.dbg = getenv("KAKVEDA_B200_DENSE_DBG") ? atoi(getenv("KAKVEDA_B200_DENSE_DBG")) : 0;
+  P.inv_norm_c = dx->d_inv_c.p; P.inv_norm_q = dx->d_inv_q.p;
+  return KV_OK;
+}
+
+// scan + merge of n_q queries already on the device (d_q: bf16 [n_q, dim], 16-byte aligned) into device buffers
+static int dense_run(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, int k, int64_t excl_base, float *d_out_s,
+                     long long *d_out_r) {
+  cudaStream_t s = dx->stream;
+  if (dx->n_rows == 0) {
+    KV_CUDA(cudaMemsetAsync(d_out_r, 0xFF, (size_t)n_q * k * 8, s));  // row -1
+    std::vector<float> neg((size_t)(n_q * k), -INFINITY);
+    KV_CUDA(cudaMemcpyAsync(d_out_s, neg.data(), neg.size() * 4, cudaMemcpyHostToDevice, s));
+    KV_CUDA(cudaStreamSynchronize(s));
+    return KV_OK;
+  }
+  CUtensorMap map_q, map_c;
+  DenseParams P;
+  int rc = dense_setup(dx, d_q, n_q, excl_base, &map_q, &map_c, P);
+  if (rc != KV_OK) return rc;
+  const int64_t n_part = (int64_t)P.n_lists * 2;  // two epilogue threads (column halves) per query and CTA
   KV_CUDA(dx->d_part_s.ensure(n_part * n_q * k)); KV_CUDA(dx->d_part_r.ensure(n_part * n_q * k));
   KV_CUDA(dx->d_gthr.ensure(n_q));
   KV_CUDA(cudaMemsetAsync(dx->d_gthr.p, 0, (size_t)n_q * 4, s));
   // unused (query tile, slot) pairs stay "empty": row -1 (the merge ignores their scores)
   KV_CUDA(cudaMemsetAsync(dx->d_part_r.p, 0xFF, (size_t)n_part * n_q * k * 8, s));
   KV_CUDA(cudaMemsetAsync(dx->d_part_s.p, 0xFF, (size_t)n_part * n_q * k * 4, s));
-  DenseParams P;
-  P.n_rows = dx->n_rows; P.row_base = dx->row_base; P.n_q = n_q; P.dim = dx->dim; P.k = k; P.n_lists = (int)n_lists;
-  P.excl_base = excl_base;
-  P.r_tiles = r_tiles; P.q_tiles = q_tiles;
-  P.dbg = getenv("KAKVEDA_B200_DENSE_DBG") ? atoi(getenv("KAKVEDA_B200_DENSE_DBG")) : 0;
-  P.inv_norm_c = dx->d_inv_c.p; P.inv_norm_q = dx->d_inv_q.p; P.gthr = dx->d_gthr.p;
+  P.k = k;
+  P.gthr = dx->d_gthr.p;
   P.part_scores = dx->d_part_s.p; P.part_rows = dx->d_part_r.p;
-  const int64_t grid = q_tiles * n_lists;
+  const int64_t grid = P.q_tiles * P.n_lists;
   KV_CUDA(cudaEventRecord(dx->ev[0], s));
-  dense_topk_kernel<<<(unsigned)grid, N_THREADS, sizeof(DenseSmem) + 1024, s>>>(map_q, map_c, P);
+  dense_topk_kernel<false><<<(unsigned)grid, N_THREADS, sizeof(DenseSmem) + 1024, s>>>(map_q, map_c, P, DenseRangeOut{});
   KV_CUDA(cudaGetLastError());
   KV_CUDA(cudaEventRecord(dx->ev[1], s));
   KV_CUDA(cudaStreamSynchronize(s));
   cudaEventElapsedTime(&dx->last_ms, dx->ev[0], dx->ev[1]);
   return kv_merge_topk_device(dx->device, dx->d_part_s.p, dx->d_part_r.p, (int)n_part, n_q, k, d_out_s, d_out_r);
+}
+
+// Threshold search of n_q queries already on the device (as dense_run): every pair whose score reaches thr lands in
+// d_range, in emit order; the handle records the result for kv_dense_range_fetch.  The pair buffer starts at 65,536
+// records and keeps its capacity across calls.  When a search finds more pairs, the buffer grows to the exact count
+// and the kernel runs once more -- the whole GEMM again, since the pairs are only known in its epilogue.  last_ms sums
+// both runs.  Caller holds dx->mu.
+static int dense_range(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, float thr, int64_t excl_base,
+                       int64_t *n_pairs) {
+  cudaStream_t s = dx->stream;
+  unsigned long long count = 0;
+  float total_ms = 0.f;
+  dx->last_splits = 0;
+  if (dx->n_rows > 0 && n_q > 0) {
+    CUtensorMap map_q, map_c;
+    DenseParams P;
+    int rc = dense_setup(dx, d_q, n_q, excl_base, &map_q, &map_c, P);
+    if (rc != KV_OK) return rc;
+    KV_CUDA(dx->d_range.ensure(65536));
+    KV_CUDA(dx->d_range_count.ensure(1));
+    DenseRangeOut R;
+    R.thr = thr;
+    R.count = dx->d_range_count.p;
+    const int64_t grid = P.q_tiles * P.n_lists;
+    for (;;) {
+      R.out = dx->d_range.p;
+      R.cap = (unsigned long long)dx->d_range.cap;
+      KV_CUDA(cudaMemsetAsync(dx->d_range_count.p, 0, sizeof(unsigned long long), s));
+      KV_CUDA(cudaEventRecord(dx->ev[0], s));
+      dense_topk_kernel<true><<<(unsigned)grid, N_THREADS, sizeof(DenseSmem) + 1024, s>>>(map_q, map_c, P, R);
+      KV_CUDA(cudaGetLastError());
+      KV_CUDA(cudaEventRecord(dx->ev[1], s));
+      KV_CUDA(cudaMemcpyAsync(&count, dx->d_range_count.p, sizeof(count), cudaMemcpyDeviceToHost, s));
+      KV_CUDA(cudaStreamSynchronize(s));
+      float ms = 0.f;
+      cudaEventElapsedTime(&ms, dx->ev[0], dx->ev[1]);
+      total_ms += ms;
+      if (count <= R.cap) break;
+      if (dx->d_range.ensure((int64_t)count) != cudaSuccess) {
+        cudaGetLastError();
+        return kv_fail(KV_ERR_NOMEM, "kv_dense_range: %llu pairs reach the threshold; their buffer does not fit in device memory "
+                                     "(raise the threshold or split the query batch)", count);
+      }
+    }
+  }
+  dx->last_ms = total_ms;
+  dx->range_q = n_q;
+  dx->range_pairs = (int64_t)count;
+  dx->range_valid = true;
+  *n_pairs = (int64_t)count;
+  return KV_OK;
 }
 
 // q: n_q x dim bfloat16 bit patterns (host).  Outputs (host): scores float32[n_q*k], rows int64[n_q*k],
@@ -460,6 +593,7 @@ int kv_dense_topk(kv_dense_index *dx, const uint16_t *q_bf16, int64_t n_q, int k
   if (!dx || n_q < 0 || k < 1 || k > MAXK || (n_q > 0 && (!q_bf16 || !out_scores || !out_rows)))
     return kv_fail(KV_ERR_INVALID, "kv_dense_topk: bad arguments (k must be 1..32)");
   std::lock_guard<std::mutex> g(dx->mu);
+  dx->range_valid = false;
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_topk: index not finalized");
   if (n_q == 0) return KV_OK;
   KV_CUDA(cudaSetDevice(dx->device));
@@ -480,6 +614,7 @@ int kv_dense_topk_device(kv_dense_index *dx, const void *d_q_bf16, int64_t n_q, 
     return kv_fail(KV_ERR_INVALID, "kv_dense_topk_device: bad arguments (k must be 1..32)");
   if (((uintptr_t)d_q_bf16 & 15) != 0) return kv_fail(KV_ERR_INVALID, "kv_dense_topk_device: queries must be 16-byte aligned");
   std::lock_guard<std::mutex> g(dx->mu);
+  dx->range_valid = false;
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_topk_device: index not finalized");
   if (n_q == 0) return KV_OK;
   KV_CUDA(cudaSetDevice(dx->device));
@@ -491,6 +626,7 @@ int kv_dense_append_device(kv_dense_index *dx, const void *d_rows_bf16, int64_t 
   if (!dx || n < 0 || (n > 0 && !d_rows_bf16)) return kv_fail(KV_ERR_INVALID, "kv_dense_append_device: bad arguments");
   if (n == 0) return KV_OK;
   std::lock_guard<std::mutex> g(dx->mu);
+  dx->range_valid = false;
   KV_CUDA(cudaSetDevice(dx->device));
   if (dx->n_rows + n >= (1LL << 31) - BN) return kv_fail(KV_ERR_INVALID, "kv_dense_append_device: more than 2^31 rows in one shard");
   KV_CUDA(dx->rows.reserve((dx->n_rows + n) * dx->dim, dx->stream));
@@ -508,12 +644,75 @@ int kv_dense_selfjoin_device(kv_dense_index *dx, int64_t q_begin, int64_t q_end,
   if (!dx || q_begin < 0 || q_end < q_begin || k < 1 || k > MAXK || !d_scores || !d_rows)
     return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_device: bad arguments (k must be 1..32)");
   std::lock_guard<std::mutex> g(dx->mu);
+  dx->range_valid = false;
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_selfjoin_device: index not finalized");
   if (q_end > dx->n_rows) return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_device: row range outside the index");
   if (q_end == q_begin) return KV_OK;
   KV_CUDA(cudaSetDevice(dx->device));
   return dense_run(dx, dx->rows.p + q_begin * dx->dim, q_end - q_begin, k, dx->row_base + q_begin, (float *)d_scores,
                    (long long *)d_rows);
+}
+
+static bool valid_threshold(float thr) { return thr > 0.f && thr <= 1.f; }  // false for NaN
+
+int kv_dense_range(kv_dense_index *dx, const uint16_t *q_bf16, int64_t n_q, float threshold, int64_t *n_pairs) {
+  if (!dx || !n_pairs || n_q < 0 || n_q >= (1LL << 31) || (n_q > 0 && !q_bf16))
+    return kv_fail(KV_ERR_INVALID, "kv_dense_range: bad arguments (n_q must be below 2^31)");
+  if (!valid_threshold(threshold)) return kv_fail(KV_ERR_INVALID, "kv_dense_range: threshold must be in (0, 1]");
+  std::lock_guard<std::mutex> g(dx->mu);
+  dx->range_valid = false;
+  if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_range: index not finalized");
+  KV_CUDA(cudaSetDevice(dx->device));
+  if (n_q > 0 && dx->n_rows > 0) {
+    KV_CUDA(dx->d_q.ensure(n_q * dx->dim));
+    KV_CUDA(cudaMemcpyAsync(dx->d_q.p, q_bf16, (size_t)n_q * dx->dim * 2, cudaMemcpyHostToDevice, dx->stream));
+  }
+  return dense_range(dx, dx->d_q.p, n_q, threshold, -1, n_pairs);
+}
+
+int kv_dense_range_device(kv_dense_index *dx, const void *d_q_bf16, int64_t n_q, float threshold, int64_t exclude_base,
+                          int64_t *n_pairs) {
+  if (!dx || !n_pairs || n_q < 0 || n_q >= (1LL << 31) || (n_q > 0 && !d_q_bf16))
+    return kv_fail(KV_ERR_INVALID, "kv_dense_range_device: bad arguments (n_q must be below 2^31)");
+  if (((uintptr_t)d_q_bf16 & 15) != 0) return kv_fail(KV_ERR_INVALID, "kv_dense_range_device: queries must be 16-byte aligned");
+  if (!valid_threshold(threshold)) return kv_fail(KV_ERR_INVALID, "kv_dense_range_device: threshold must be in (0, 1]");
+  std::lock_guard<std::mutex> g(dx->mu);
+  dx->range_valid = false;
+  if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_range_device: index not finalized");
+  KV_CUDA(cudaSetDevice(dx->device));
+  return dense_range(dx, (const __nv_bfloat16 *)d_q_bf16, n_q, threshold, exclude_base, n_pairs);
+}
+
+int kv_dense_selfjoin_range(kv_dense_index *dx, int64_t q_begin, int64_t q_end, float threshold, int64_t *n_pairs) {
+  if (!dx || !n_pairs || q_begin < 0 || q_end < q_begin || q_end - q_begin >= (1LL << 31))
+    return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_range: bad arguments");
+  if (!valid_threshold(threshold)) return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_range: threshold must be in (0, 1]");
+  std::lock_guard<std::mutex> g(dx->mu);
+  dx->range_valid = false;
+  if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_selfjoin_range: index not finalized");
+  if (q_end > dx->n_rows) return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_range: row range outside the index");
+  KV_CUDA(cudaSetDevice(dx->device));
+  return dense_range(dx, dx->rows.p + q_begin * dx->dim, q_end - q_begin, threshold, dx->row_base + q_begin, n_pairs);
+}
+
+// The pairs come back in emit order, which the kernel does not fix; (score desc, row asc) is a total order of each
+// query's pairs, so the result is deterministic.
+int kv_dense_range_fetch(kv_dense_index *dx, int64_t *indptr, int64_t *rows, float *scores) {
+  if (!dx || !indptr) return kv_fail(KV_ERR_INVALID, "kv_dense_range_fetch: bad arguments");
+  std::lock_guard<std::mutex> g(dx->mu);
+  if (!dx->range_valid) return kv_fail(KV_ERR_STATE, "kv_dense_range_fetch: no threshold search result (kv_dense_range* first)");
+  const int64_t n_q = dx->range_q, n = dx->range_pairs;
+  if (n > 0 && (!rows || !scores)) return kv_fail(KV_ERR_INVALID, "kv_dense_range_fetch: bad arguments");
+  KV_CUDA(cudaSetDevice(dx->device));
+  KV_CUDA(dx->h_range.ensure(std::max<int64_t>(n, 1)));
+  if (n) {
+    KV_CUDA(cudaMemcpyAsync(dx->h_range.p, dx->d_range.p, (size_t)n * sizeof(RangePair), cudaMemcpyDeviceToHost, dx->stream));
+    KV_CUDA(cudaStreamSynchronize(dx->stream));
+  }
+  const int rc = range_order(dx->h_range.p, n, n_q, indptr, rows, scores, "kv_dense_range_fetch");
+  if (rc != KV_OK) return rc;
+  dx->range_valid = false;
+  return KV_OK;
 }
 
 int kv_dense_last_timing(const kv_dense_index *dx, float *gemm_ms, int64_t *splits) {

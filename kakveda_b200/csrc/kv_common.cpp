@@ -3,7 +3,12 @@
 #include "kv_cuda.cuh"
 #include "sm90.cuh"
 
+#include <algorithm>
+#include <cstdlib>
 #include <cstring>
+#include <new>
+#include <thread>
+#include <vector>
 
 namespace {
 thread_local char g_err[512] = "";
@@ -18,6 +23,43 @@ int kv_fail(int code, const char *fmt, ...) {
 }
 
 void kv_clear_error() { g_err[0] = 0; }
+
+int host_threads() {
+  int t = (int)std::thread::hardware_concurrency();
+  if (const char *e = getenv("KAKVEDA_B200_THREADS")) t = atoi(e);
+  return std::max(1, std::min(t, 64));
+}
+
+int range_order(const RangePair *rec, int64_t n, int64_t n_q, int64_t *indptr, int64_t *rows, float *scores, const char *fn) {
+  std::vector<RangePair> by_q;
+  try {
+    by_q.resize((size_t)n);
+  } catch (const std::bad_alloc &) {
+    return kv_fail(KV_ERR_NOMEM, "%s: out of host memory", fn);
+  }
+  for (int64_t q = 0; q <= n_q; q++) indptr[q] = 0;
+  for (int64_t i = 0; i < n; i++) indptr[rec[i].q + 1]++;
+  for (int64_t q = 0; q < n_q; q++) indptr[q + 1] += indptr[q];
+  std::vector<int64_t> next(indptr, indptr + n_q);
+  for (int64_t i = 0; i < n; i++) by_q[(size_t)next[(size_t)rec[i].q]++] = rec[i];
+  // thread t orders queries [n_q t / T, n_q (t + 1) / T)
+  const int T = (int)std::max<int64_t>(1, std::min<int64_t>(n >= 65536 ? host_threads() : 1, n_q));
+  auto body = [&](int t) {
+    for (int64_t q = n_q * t / T; q < n_q * (t + 1) / T; q++) {
+      RangePair *lo = by_q.data() + indptr[q], *hi = by_q.data() + indptr[q + 1];
+      std::sort(lo, hi, [](const RangePair &x, const RangePair &y) { return x.score != y.score ? x.score > y.score : x.row < y.row; });
+      for (RangePair *p = lo; p < hi; p++) {
+        rows[p - by_q.data()] = p->row;
+        scores[p - by_q.data()] = p->score;
+      }
+    }
+  };
+  std::vector<std::thread> th;
+  for (int t = 1; t < T; t++) th.emplace_back(body, t);
+  body(0);
+  for (auto &x : th) x.join();
+  return KV_OK;
+}
 
 int open_device(int device, const char *fn, int *sm_count) {
   int n = 0;

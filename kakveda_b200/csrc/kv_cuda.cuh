@@ -89,6 +89,18 @@ struct PinnedBuf {
   }
 };
 
+// One match of a threshold search (16 bytes): what the emitting scans (K1b-R, K2-R) append to their pair buffer
+struct RangePair {
+  int32_t q;    // query index within the search
+  float score;  // the float32 score the top-k path reports for the pair
+  int64_t row;  // global row
+};
+
+// Orders the n pairs of a threshold search over n_q queries (emit order, as the device left them) into
+// indptr[n_q+1] / rows[n] / scores[n]: a counting sort by query, then each query's segment by (score desc, row asc) on
+// the host threads.  `fn` names the caller in error messages.
+int range_order(const RangePair *rec, int64_t n, int64_t n_q, int64_t *indptr, int64_t *rows, float *scores, const char *fn);
+
 // Non-blocking stream; converts to cudaStream_t.
 struct CudaStream {
   cudaStream_t s = nullptr;

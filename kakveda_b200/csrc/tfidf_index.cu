@@ -23,14 +23,6 @@
 using namespace kvk;
 using namespace kvh;  // parallel_for, stable_sort_indices, idf_host, build_blocks (block_builder.cuh)
 
-namespace {
-int host_threads() {
-  int t = (int)std::thread::hardware_concurrency();
-  if (const char *e = getenv("KAKVEDA_B200_THREADS")) t = atoi(e);
-  return std::max(1, std::min(t, 64));
-}
-}  // namespace
-
 // ----------------------------------------------------------------------------------------
 // handle
 // ----------------------------------------------------------------------------------------
@@ -1600,29 +1592,8 @@ int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores) 
     KV_CUDA(cudaMemcpyAsync(ix->h_range.p, ix->d_range.p, (size_t)n * sizeof(RangePair), cudaMemcpyDeviceToHost, ix->stream));
     KV_CUDA(cudaStreamSynchronize(ix->stream));
   }
-  // counting sort by query, then each query's segment by (score desc, row asc)
-  const RangePair *rec = ix->h_range.p;
-  std::vector<RangePair> by_q;
-  try {
-    by_q.resize((size_t)n);
-  } catch (const std::bad_alloc &) {
-    return kv_fail(KV_ERR_NOMEM, "kv_range_fetch: out of host memory");
-  }
-  for (int64_t q = 0; q <= n_q; q++) indptr[q] = 0;
-  for (int64_t i = 0; i < n; i++) indptr[rec[i].q + 1]++;
-  for (int64_t q = 0; q < n_q; q++) indptr[q + 1] += indptr[q];
-  std::vector<int64_t> next(indptr, indptr + n_q);
-  for (int64_t i = 0; i < n; i++) by_q[(size_t)next[(size_t)rec[i].q]++] = rec[i];
-  parallel_for(n_q, n >= 65536 ? host_threads() : 1, [&](int, int64_t a, int64_t b) {
-    for (int64_t q = a; q < b; q++) {
-      RangePair *lo = by_q.data() + indptr[q], *hi = by_q.data() + indptr[q + 1];
-      std::sort(lo, hi, [](const RangePair &x, const RangePair &y) { return x.score != y.score ? x.score > y.score : x.row < y.row; });
-      for (RangePair *p = lo; p < hi; p++) {
-        rows[p - by_q.data()] = p->row;
-        scores[p - by_q.data()] = p->score;
-      }
-    }
-  });
+  const int rc = range_order(ix->h_range.p, n, n_q, indptr, rows, scores, "kv_range_fetch");
+  if (rc != KV_OK) return rc;
   ix->range_valid = false;
   return KV_OK;
 }

@@ -517,13 +517,6 @@ __host__ __device__ __forceinline__ uint32_t rt_slot(uint32_t fid, uint32_t size
 // K1b-R (RANGE = true) is the same scan for a threshold search: the filter is the query's fixed threshold and every
 // row that reaches it is appended to a global pair buffer instead of a top-k list.
 // ----------------------------------------------------------------------------------------
-// One match of a threshold search (16 bytes)
-struct RangePair {
-  int32_t q;    // original query index
-  float score;  // the float32 score the top-k path reports for the pair
-  int64_t row;  // global row
-};
-
 struct ScanParams {
   const uint32_t *blk;
   const BlockInfo *binfo;

@@ -56,7 +56,8 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
     """Similarity-split version of pattern_detector.on_failure.
 
     ``index``: a finalized ``GfkbIndex`` whose row i is ``records[i]['signature_text']`` (corpus-fit mode gives a
-    symmetric measure; the default mode works too).  Returns one payload per connected component that, restricted
+    symmetric measure; the default mode works too), or a finalized ``DenseIndex`` whose row i is record i's embedding
+    (cosine).  Returns one payload per connected component that, restricted
     to ``failure_type`` (if given), spans at least ``min_apps`` apps (app.py:45-46) -- ordered by smallest row id.
     ``k``: rows are linked only through every row's k nearest other rows, so when a text is stored more than k times
     its copies fill the lists and pairs of similar texts are never seen.  ``k=None`` links on the exact threshold
