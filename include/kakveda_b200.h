@@ -213,11 +213,25 @@ int kv_selfjoin_upload(kv_index *ix, int64_t q_begin, int64_t q_end);
  * 0, [2] = bound pass 1, [3] = the scan (including a re-run after the pair buffer grew), [4] = irregular-query
  * fallbacks; kv_index_layout counters [9]-[13] describe the run.  threshold NaN, <= 0 or > 1: KV_ERR_INVALID.
  * KV_ERR_NOMEM when the candidate pool is exhausted or the pairs do not fit in device memory (the message gives their
- * count).  Jaccard indexes: KV_ERR_INVALID (K3 has no emitting form). */
+ * count).  Jaccard indexes: KV_ERR_INVALID (they search with kv_jaccard_range_resident). */
 int kv_range_resident(kv_index *ix, float threshold, int64_t *n_pairs);
 /* The last range result: indptr[n_q+1] by original query, rows[n_pairs] (global), scores[n_pairs]; per query
- * ordered by (score desc, row asc).  KV_ERR_STATE when there is none. */
+ * ordered by (score desc, row asc).  KV_ERR_STATE when there is none (always on a Jaccard index). */
 int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores);
+/* The threshold search of a Jaccard index (KV_MODE_JACCARD), over the batch uploaded by kv_query_upload or
+ * kv_selfjoin_upload (exclusions honoured): every (query, row) pair whose float32 score -- the value kv_topk reports,
+ * |q ∩ row| / |q ∪ row| rounded once -- is >= threshold, 0 < threshold <= 1 (else KV_ERR_INVALID).  K3-R scores every
+ * chunk like the top-k scan and appends each match with its exact counts; queries of more than 64 tokens take the
+ * float64 full scan, whose exact ratio gives the counts back.  The pair buffer starts at 65,536 records and grows to
+ * the exact count when a search finds more (the scan then runs again; KV_ERR_NOMEM with the count when the pairs do
+ * not fit in device memory).  The result stays until kv_jaccard_range_fetch or the next upload, top-k, range, append
+ * or finalize call.  kv_index_last_kernel_ms: [3] = the scan (re-run included), [4] = irregular-query fallbacks.
+ * Both functions return KV_ERR_INVALID on a TF-IDF index. */
+int kv_jaccard_range_resident(kv_index *ix, float threshold, int64_t *n_pairs);
+/* The last Jaccard range result: indptr[n_q+1] by original query, rows[n_pairs] (global), scores[n_pairs] (float32),
+ * inter[n_pairs] = |q ∩ row| and uni[n_pairs] = |q ∪ row|; per query ordered by (score desc, row asc), as
+ * kv_range_fetch.  scores[i] is the float32 quotient inter[i] / uni[i].  KV_ERR_STATE when there is none. */
+int kv_jaccard_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores, int32_t *inter, int32_t *uni);
 
 /* K6: float64 scores of selected (query, row) pairs: rows[n_q*k] are GLOBAL row ids (e.g. what kv_topk returned;
  * -1 = unused slot), out_scores[n_q*k] (host) receives the float64 cosine of SimilarityEngine.score

@@ -709,7 +709,7 @@ int kv_dense_range_fetch(kv_dense_index *dx, int64_t *indptr, int64_t *rows, flo
     KV_CUDA(cudaMemcpyAsync(dx->h_range.p, dx->d_range.p, (size_t)n * sizeof(RangePair), cudaMemcpyDeviceToHost, dx->stream));
     KV_CUDA(cudaStreamSynchronize(dx->stream));
   }
-  const int rc = range_order(dx->h_range.p, n, n_q, indptr, rows, scores, "kv_dense_range_fetch");
+  const int rc = range_order(dx->h_range.p, n, n_q, 0, indptr, rows, scores, nullptr, nullptr, "kv_dense_range_fetch");
   if (rc != KV_OK) return rc;
   dx->range_valid = false;
   return KV_OK;

@@ -8,6 +8,7 @@
 #include <cstring>
 #include <new>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 namespace {
@@ -30,8 +31,18 @@ int host_threads() {
   return std::max(1, std::min(t, 64));
 }
 
-int range_order(const RangePair *rec, int64_t n, int64_t n_q, int64_t *indptr, int64_t *rows, float *scores, const char *fn) {
-  std::vector<RangePair> by_q;
+namespace {
+// score and row of a record in the order range_order sorts by
+inline float pair_score(const RangePair &p) { return p.score; }
+inline int64_t pair_row(const RangePair &p) { return p.row; }
+inline float pair_score(const JaccardPair &p) { return (float)p.inter / (float)p.uni; }
+inline int64_t pair_row(const JaccardPair &p) { return p.row; }
+}  // namespace
+
+template <class Rec>
+int range_order(const Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
+                int32_t *inter, int32_t *uni, const char *fn) {
+  std::vector<Rec> by_q;
   try {
     by_q.resize((size_t)n);
   } catch (const std::bad_alloc &) {
@@ -46,11 +57,19 @@ int range_order(const RangePair *rec, int64_t n, int64_t n_q, int64_t *indptr, i
   const int T = (int)std::max<int64_t>(1, std::min<int64_t>(n >= 65536 ? host_threads() : 1, n_q));
   auto body = [&](int t) {
     for (int64_t q = n_q * t / T; q < n_q * (t + 1) / T; q++) {
-      RangePair *lo = by_q.data() + indptr[q], *hi = by_q.data() + indptr[q + 1];
-      std::sort(lo, hi, [](const RangePair &x, const RangePair &y) { return x.score != y.score ? x.score > y.score : x.row < y.row; });
-      for (RangePair *p = lo; p < hi; p++) {
-        rows[p - by_q.data()] = p->row;
-        scores[p - by_q.data()] = p->score;
+      Rec *lo = by_q.data() + indptr[q], *hi = by_q.data() + indptr[q + 1];
+      std::sort(lo, hi, [](const Rec &x, const Rec &y) {
+        const float sx = pair_score(x), sy = pair_score(y);
+        return sx != sy ? sx > sy : pair_row(x) < pair_row(y);
+      });
+      for (Rec *p = lo; p < hi; p++) {
+        const size_t i = (size_t)(p - by_q.data());
+        rows[i] = row_base + pair_row(*p);
+        scores[i] = pair_score(*p);
+        if constexpr (std::is_same_v<Rec, JaccardPair>) {
+          inter[i] = p->inter;
+          uni[i] = p->uni;
+        }
       }
     }
   };
@@ -60,6 +79,11 @@ int range_order(const RangePair *rec, int64_t n, int64_t n_q, int64_t *indptr, i
   for (auto &x : th) x.join();
   return KV_OK;
 }
+
+template int range_order<RangePair>(const RangePair *, int64_t, int64_t, int64_t, int64_t *, int64_t *, float *, int32_t *,
+                                    int32_t *, const char *);
+template int range_order<JaccardPair>(const JaccardPair *, int64_t, int64_t, int64_t, int64_t *, int64_t *, float *,
+                                      int32_t *, int32_t *, const char *);
 
 int open_device(int device, const char *fn, int *sm_count) {
   int n = 0;

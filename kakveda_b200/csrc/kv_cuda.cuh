@@ -96,10 +96,23 @@ struct RangePair {
   int64_t row;  // global row
 };
 
+// One match of a Jaccard threshold search (16 bytes, what K3-R and its irregular-query fallback append).  The exact
+// counts travel with the pair and the float32 score is their quotient, formed where the pairs are ordered: inter and
+// union are integer-valued floats on the device, so the host's IEEE division gives the bits of the device's __fdiv_rn.
+struct JaccardPair {
+  int32_t q;      // original query
+  int32_t row;    // local original row (below 2^31: the row permutation is int)
+  int32_t inter;  // |q ∩ row|
+  int32_t uni;    // |q ∪ row|
+};
+
 // Orders the n pairs of a threshold search over n_q queries (emit order, as the device left them) into
-// indptr[n_q+1] / rows[n] / scores[n]: a counting sort by query, then each query's segment by (score desc, row asc) on
-// the host threads.  `fn` names the caller in error messages.
-int range_order(const RangePair *rec, int64_t n, int64_t n_q, int64_t *indptr, int64_t *rows, float *scores, const char *fn);
+// indptr[n_q+1] / rows[n] / scores[n] (and, for JaccardPair records, inter[n] / uni[n]): a counting sort by query, then
+// each query's segment by (score desc, row asc) on the host threads.  row_base is added to JaccardPair rows (RangePair
+// rows are global already).  `fn` names the caller in error messages.  Defined for Rec = RangePair and JaccardPair.
+template <class Rec>
+int range_order(const Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
+                int32_t *inter, int32_t *uni, const char *fn);
 
 // Non-blocking stream; converts to cudaStream_t.
 struct CudaStream {

@@ -131,6 +131,11 @@ struct kv_index {
   DevBuf<unsigned long long> d_range_count;
   PinnedBuf<RangePair> h_range;
   bool range_valid = false;
+  // the same on a Jaccard index (K3-R, kv_jaccard_range_resident): the records carry the exact counts and have a
+  // result flag of their own, so kv_range_fetch never reads them
+  DevBuf<JaccardPair> d_jrange;
+  PinnedBuf<JaccardPair> h_jrange;
+  bool jrange_valid = false;
   int64_t range_q = 0, range_pairs = 0;
   DevBuf<unsigned long long> d_stats;
   DevBuf<float> d_part_s, d_out_s;
@@ -320,7 +325,8 @@ int kv_index_create(int device, int64_t row_base, kv_index **out) {
   KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<true>, smem_limit, (int)scan_smem_bytes(0)));
   KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<true>, smem_limit, 232448));
   KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<false>, smem_limit, 232448));
-  KV_CUDA(cudaFuncSetAttribute(jaccard_scan_kernel, smem_limit, (int)jaccard_smem_bytes(32)));
+  KV_CUDA(cudaFuncSetAttribute(jaccard_scan_kernel<false>, smem_limit, (int)jaccard_smem_bytes(32)));
+  KV_CUDA(cudaFuncSetAttribute(jaccard_scan_kernel<true>, smem_limit, (int)jaccard_smem_bytes(0)));
   *out = ix.release();
   return KV_OK;
 }
@@ -377,6 +383,7 @@ int kv_index_append(kv_index *ix, const int64_t *indptr, const uint32_t *ids, co
   ix->ids.n = ix->nnz;
   ix->tf.n = ix->nnz;
   ix->finalized = false;
+  ix->jrange_valid = false;
   return KV_OK;
 }
 
@@ -564,7 +571,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
       KV_CUDA(cudaStreamSynchronize(s));
       ix->V = V;
       ix->finalized = true;
-      ix->batch_valid = ix->range_valid = false;
+      ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
       ix->last_finalize_kind = 2;
       return KV_OK;
     }
@@ -605,7 +612,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
   KV_CUDA(cudaStreamSynchronize(s));
   ix->V = V;
   ix->finalized = true;
-  ix->batch_valid = ix->range_valid = false;
+  ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
   ix->last_finalize_kind = 1;
   return KV_OK;
 }
@@ -771,7 +778,7 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   if (n_q >= (1LL << 31) - TILE_Q) return kv_fail(KV_ERR_INVALID, "kv_topk: too many queries in one call");
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
-  ix->batch_valid = ix->range_valid = false;
+  ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
   ix->has_excl = false;
   ix->irr_q.clear(); ix->irr_indptr.assign(1, 0); ix->irr_ids.clear(); ix->irr_tf.clear(); ix->irr_oov.clear();
   const int T = host_threads();
@@ -1085,22 +1092,30 @@ static int run_exhaustive(kv_index *ix, Batch &b) {
 }
 
 // Jaccard path: token sets have no text structure to prune on -- the dense-regime kernel K3 scores every chunk for a
-// whole scan group at once
+// whole scan group at once.  A threshold search runs K3-R, which appends to d_jrange instead of filling lists.
 static int run_jaccard(kv_index *ix, Batch &b) {
   const int64_t n_q = b.n_q, n_groups = b.n_groups;
   const int64_t jsplits = std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>((4LL * ix->sm_count + n_groups - 1) / n_groups, 256),
                                                                  std::max<int64_t>(1, ix->n_chunks / 64)));
   b.n_parts = jsplits * J_WARPS;
-  KV_CUDA(ix->d_part_s.ensure(b.n_parts * n_q * b.k));
-  KV_CUDA(ix->d_part_r.ensure(b.n_parts * n_q * b.k));
+  if (!b.range) {
+    KV_CUDA(ix->d_part_s.ensure(b.n_parts * n_q * b.k));
+    KV_CUDA(ix->d_part_r.ensure(b.n_parts * n_q * b.k));
+  }
   const float *qc = ix->d_qconst.p;
   JaccardParams JP;
   JP.blk = ix->d_blk.p; JP.binfo = ix->d_binfo.p; JP.B32 = ix->d_B32.p; JP.perm = ix->d_perm.p;
   JP.n_chunks = ix->n_chunks; JP.n_rows = ix->n_rows; JP.row_base = ix->row_base;
   JP.qtab = ix->d_qtab.p; JP.q_nq = qc; JP.q_dotU = qc + n_q; JP.q_excl = ix->has_excl ? ix->d_excl_sorted.p : nullptr;
-  JP.gthr = ix->d_gthr.p; JP.stats = ix->d_stats.p;
+  JP.gthr = b.range ? ix->d_rthr.p : ix->d_gthr.p; JP.stats = ix->d_stats.p;
   JP.n_q = n_q; JP.k = b.k; JP.n_splits = (int)jsplits; JP.part_scores = ix->d_part_s.p; JP.part_rows = ix->d_part_r.p;
-  jaccard_scan_kernel<<<dim3((unsigned)n_groups, (unsigned)jsplits), J_WARPS * 32, jaccard_smem_bytes(b.k), ix->stream>>>(JP);
+  const dim3 grid((unsigned)n_groups, (unsigned)jsplits);
+  if (b.range) {
+    const JaccardRangeOut R{ix->d_qperm.p, ix->d_jrange.p, ix->d_range_count.p, (unsigned long long)ix->d_jrange.cap};
+    jaccard_scan_kernel<true><<<grid, J_WARPS * 32, jaccard_smem_bytes(0), ix->stream>>>(JP, R);
+  } else {
+    jaccard_scan_kernel<false><<<grid, J_WARPS * 32, jaccard_smem_bytes(b.k), ix->stream>>>(JP, JaccardRangeOut{});
+  }
   KV_CUDA(cudaGetLastError());
   b.launches++;
   return KV_OK;
@@ -1155,6 +1170,7 @@ static int size_batch(kv_index *ix, Batch &b) {
 static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, int phase = 0) {
   if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_topk_resident: no query batch uploaded");
   if (k < 1 || k > 32) return kv_fail(KV_ERR_INVALID, "kv_topk: k must be 1..32");
+  ix->jrange_valid = false;
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
   Batch b;
@@ -1272,23 +1288,26 @@ static int finish_batch(kv_index *ix) {
   return check_pool(ix);
 }
 
-// Threshold search over the resident batch: every pair with score >= thr lands in d_range, *n_pairs = their count.
-// When they do not fit, d_range grows to the exact count and only the scan and the fallbacks run again (the candidate
-// lists depend on the threshold alone).  Events: evk[2] -> evk[3] bound pass 1, evk[3] -> evk[4] scan, evk[4] -> evk[5]
-// irregular-query fallbacks.  Caller holds ix->mu.
-static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
-  ix->range_valid = false;
-  if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_range_resident: no query batch uploaded");
-  if (ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_range_resident: Jaccard indexes have no threshold search");
+// Threshold search over the resident batch: every pair with score >= thr lands in d_range (d_jrange on a Jaccard
+// index), *n_pairs = their count.  When they do not fit, the buffer grows to the exact count and only the scan and the
+// fallbacks run again (the candidate lists depend on the threshold alone).  Events: evk[2] -> evk[3] bound pass 1,
+// evk[3] -> evk[4] scan, evk[4] -> evk[5] irregular-query fallbacks.  `fn` names the caller in error messages.
+// Caller holds ix->mu.
+static int run_range(kv_index *ix, float thr, int64_t *n_pairs, const char *fn) {
+  ix->range_valid = ix->jrange_valid = false;
+  if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "%s: no query batch uploaded", fn);
+  const bool jac = ix->jaccard != 0;
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
   Batch b;
   b.k = 0; b.phase = 2; b.out_s = nullptr; b.out_r = nullptr; b.range = true; b.use_codes = false; b.n_peers = 0;
-  int rc = size_batch(ix, b);
+  int rc = size_batch(ix, b);  // a Jaccard index never prunes
   if (rc != KV_OK) return rc;
   const int64_t n_q = b.n_q;
   KV_CUDA(ix->d_rthr.ensure(n_q));
-  KV_CUDA(ix->d_range.ensure(65536));
+  if (jac) KV_CUDA(ix->d_jrange.ensure(65536));
+  else KV_CUDA(ix->d_range.ensure(65536));
+  auto range_cap = [&] { return (unsigned long long)(jac ? ix->d_jrange.cap : ix->d_range.cap); };
   KV_CUDA(ix->d_range_count.ensure(1));
   for (auto &e : ix->evk) KV_CUDA(cudaEventRecord(e, s));
   KV_CUDA(cudaMemsetAsync(ix->d_stats.p, 0, 8 * sizeof(unsigned long long), s));
@@ -1308,7 +1327,7 @@ static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
         rc = run_pruned(ix, b);  // bound pass 1 (ends with evk[3]), then the scan
       } else {
         KV_CUDA(cudaEventRecord(ix->evk[3], s));
-        rc = b.prune ? scan_candidates(ix, b) : run_exhaustive(ix, b);
+        rc = jac ? run_jaccard(ix, b) : b.prune ? scan_candidates(ix, b) : run_exhaustive(ix, b);
       }
       if (rc != KV_OK) return rc;
       KV_CUDA(cudaEventRecord(ix->evk[4], s));
@@ -1317,9 +1336,15 @@ static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
         rc = score_impl(ix, ix->irr_ids.data() + a, ix->irr_tf.data() + a, e - a, ix->irr_oov[i], nullptr);
         if (rc != KV_OK) return rc;
         const unsigned grid = (unsigned)std::min<int64_t>((ix->n_rows + 255) / 256, 8LL * ix->sm_count);
-        select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, thr,
-                                                 ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, (int)q, ix->d_range.p,
-                                                 ix->d_range_count.p, (unsigned long long)ix->d_range.cap);
+        const int64_t excl = ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1;
+        if (jac) {
+          const double nq = host_query_norm(ix, ix->irr_ids.data() + a, ix->irr_tf.data() + a, e - a, ix->irr_oov[i]);  // |q|
+          jaccard_select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->d_B64.p, ix->d_invperm.p, ix->n_rows, nq, thr, excl,
+                                                           (int)q, ix->d_jrange.p, ix->d_range_count.p, range_cap());
+        } else {
+          select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, thr, excl, (int)q, ix->d_range.p,
+                                                   ix->d_range_count.p, range_cap());
+        }
         KV_CUDA(cudaGetLastError());
         b.launches += 2;
       }
@@ -1337,11 +1362,11 @@ static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
       cudaEventElapsedTime(&t_fallback, ix->evk[4], ix->evk[5]);
       ms[3] += t_scan;
       ms[4] += t_fallback;
-      if (count <= (unsigned long long)ix->d_range.cap) break;
-      if (ix->d_range.ensure((int64_t)count) != cudaSuccess) {
+      if (count <= range_cap()) break;
+      if ((jac ? ix->d_jrange.ensure((int64_t)count) : ix->d_range.ensure((int64_t)count)) != cudaSuccess) {
         cudaGetLastError();
-        return kv_fail(KV_ERR_NOMEM, "kv_range_resident: %llu pairs reach the threshold; their buffer does not fit in device memory "
-                                     "(raise the threshold or split the query batch)", count);
+        return kv_fail(KV_ERR_NOMEM, "%s: %llu pairs reach the threshold; their buffer does not fit in device memory "
+                                     "(raise the threshold or split the query batch)", fn, count);
       }
       // the counters describe one run: the bound pass's stay, the scan's start again
       KV_CUDA(cudaMemsetAsync(ix->d_stats.p, 0, 2 * sizeof(unsigned long long), s));
@@ -1354,7 +1379,7 @@ static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
   ix->last_launches = b.launches;
   ix->range_q = n_q;
   ix->range_pairs = (int64_t)count;
-  ix->range_valid = true;
+  (jac ? ix->jrange_valid : ix->range_valid) = true;
   *n_pairs = (int64_t)count;
   return KV_OK;
 }
@@ -1575,7 +1600,17 @@ int kv_range_resident(kv_index *ix, float threshold, int64_t *n_pairs) {
   if (!ix || !n_pairs) return kv_fail(KV_ERR_INVALID, "kv_range_resident: bad arguments");
   if (!(threshold > 0.f && threshold <= 1.f)) return kv_fail(KV_ERR_INVALID, "kv_range_resident: threshold must be in (0, 1]");
   std::lock_guard<std::mutex> g(ix->mu);
-  return run_range(ix, threshold, n_pairs);
+  if (ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_range_resident: a Jaccard index searches with kv_jaccard_range_resident");
+  return run_range(ix, threshold, n_pairs, "kv_range_resident");
+}
+
+int kv_jaccard_range_resident(kv_index *ix, float threshold, int64_t *n_pairs) {
+  if (!ix || !n_pairs) return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_resident: bad arguments");
+  if (!(threshold > 0.f && threshold <= 1.f))
+    return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_resident: threshold must be in (0, 1]");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (!ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_resident: not a Jaccard index (kv_range_resident)");
+  return run_range(ix, threshold, n_pairs, "kv_jaccard_range_resident");
 }
 
 // The pairs come back in emit order, which the scan does not fix; scores are exact integer sums rounded once, so
@@ -1592,9 +1627,30 @@ int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores) 
     KV_CUDA(cudaMemcpyAsync(ix->h_range.p, ix->d_range.p, (size_t)n * sizeof(RangePair), cudaMemcpyDeviceToHost, ix->stream));
     KV_CUDA(cudaStreamSynchronize(ix->stream));
   }
-  const int rc = range_order(ix->h_range.p, n, n_q, indptr, rows, scores, "kv_range_fetch");
+  const int rc = range_order(ix->h_range.p, n, n_q, 0, indptr, rows, scores, nullptr, nullptr, "kv_range_fetch");
   if (rc != KV_OK) return rc;
   ix->range_valid = false;
+  return KV_OK;
+}
+
+// Same order as kv_range_fetch: the score is inter / union rounded to float32, and equal scores order by row.
+int kv_jaccard_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores, int32_t *inter, int32_t *uni) {
+  if (!ix || !indptr) return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_fetch: bad arguments");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (!ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_fetch: not a Jaccard index (kv_range_fetch)");
+  if (!ix->jrange_valid)
+    return kv_fail(KV_ERR_STATE, "kv_jaccard_range_fetch: no threshold search result (kv_jaccard_range_resident first)");
+  const int64_t n_q = ix->range_q, n = ix->range_pairs;
+  if (n > 0 && (!rows || !scores || !inter || !uni)) return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_fetch: bad arguments");
+  KV_CUDA(cudaSetDevice(ix->device));
+  KV_CUDA(ix->h_jrange.ensure(std::max<int64_t>(n, 1)));
+  if (n) {
+    KV_CUDA(cudaMemcpyAsync(ix->h_jrange.p, ix->d_jrange.p, (size_t)n * sizeof(JaccardPair), cudaMemcpyDeviceToHost, ix->stream));
+    KV_CUDA(cudaStreamSynchronize(ix->stream));
+  }
+  const int rc = range_order(ix->h_jrange.p, n, n_q, ix->row_base, indptr, rows, scores, inter, uni, "kv_jaccard_range_fetch");
+  if (rc != KV_OK) return rc;
+  ix->jrange_valid = false;
   return KV_OK;
 }
 

@@ -896,6 +896,8 @@ static inline size_t scan_smem_bytes(int k) {
 // 8-bit counters (lane-parallel) and added by the lanes whose query holds the token -- after the chunk a lane holds
 // |q ∩ row| for all 32 rows as bytes.  Exact integers; score = |∩| / (|q| + |row| - |∩|); per-warp private top-k lists
 // (no locks), merged by K5.  Queries are limited to 64 tokens like everywhere (more: float64 full-scan path).
+// K3-R (RANGE = true) is the same scan for a threshold search: no lists; P.gthr holds the fixed threshold, and every
+// (query, row) pair whose score reaches it is appended to R.out with its exact counts.
 // ----------------------------------------------------------------------------------------
 struct JaccardParams {
   const uint32_t *blk;
@@ -919,7 +921,18 @@ constexpr int J_SLOTS = 4096;  // union table of a group: <= 32 x 64 tokens
 
 static inline size_t jaccard_smem_bytes(int k) { return (size_t)J_SLOTS * 8 + (size_t)J_WARPS * 32 * 36 + (size_t)J_WARPS * k * 32 * 8; }
 
-__global__ void __launch_bounds__(J_WARPS * 32, 2) jaccard_scan_kernel(JaccardParams P) {
+// Output of the threshold search (jaccard_scan_kernel<true>, which leaves k and the partial lists of JaccardParams
+// unused; the top-k form ignores this argument).  A kernel argument of its own, so that the top-k form's parameter
+// block stays as it was.
+struct JaccardRangeOut {
+  const int *qperm;           // [n_q] sorted slot -> original query
+  JaccardPair *out;           // [cap]
+  unsigned long long *count;  // pairs found (may exceed cap: those past it are not written)
+  unsigned long long cap;
+};
+
+template <bool RANGE>
+__global__ void __launch_bounds__(J_WARPS * 32, 2) jaccard_scan_kernel(JaccardParams P, JaccardRangeOut R) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint32_t *s_keys = (uint32_t *)smem_raw;                 // [J_SLOTS]
   uint32_t *s_qm = s_keys + J_SLOTS;                       // [J_SLOTS] queries of the group holding the token
@@ -952,9 +965,13 @@ __global__ void __launch_bounds__(J_WARPS * 32, 2) jaccard_scan_kernel(JaccardPa
   const float nq = valid ? P.q_nq[q0 + lane] : 0.f;
   const float dotU = valid ? P.q_dotU[q0 + lane] : 0.f;
   const int excl = (valid && P.q_excl) ? P.q_excl[q0 + lane] : -1;
+  // threshold search: this lane's fixed threshold and original query
+  const float rthr = (RANGE && valid) ? __int_as_float(P.gthr[q0 + lane]) : 0.f;
+  const int rq = (RANGE && valid) ? R.qperm[q0 + lane] : 0;
   float *ls = s_ls + (size_t)warp * k * 32 + lane;  // element j at ls[j * 32]
   int *lr = s_lr + (size_t)warp * k * 32 + lane;
-  for (int j = 0; j < k; j++) { ls[j * 32] = -INFINITY; lr[j * 32] = 0x7fffffff; }
+  if constexpr (!RANGE)
+    for (int j = 0; j < k; j++) { ls[j * 32] = -INFINITY; lr[j * 32] = 0x7fffffff; }
   int cnt = 0;
   float kth = -INFINITY;
   int kth_row = 0x7fffffff;
@@ -1009,6 +1026,44 @@ __global__ void __launch_bounds__(J_WARPS * 32, 2) jaccard_scan_kernel(JaccardPa
       __syncwarp();
     }
     done++;
+    if constexpr (RANGE) {
+      // this lane's hits among the chunk's 32 rows (the score is the top-k epilogue's expression), then one
+      // reservation for the warp's hits from an inclusive prefix sum of the lanes' counts
+      uint32_t hits = 0;
+#pragma unroll
+      for (int r = 0; r < 32; r++) {
+        const float t = __shfl_sync(FULL, myB, r);
+        const int row = __shfl_sync(FULL, myrow, r);
+        if (r >= rows || !valid || row == excl) continue;
+        const float inter = dotU + (float)((cw[r >> 2] >> ((r & 3) * 8)) & 0xFFu);
+        const float uni = nq + t - inter;
+        if (!(inter >= rthr * uni * FILTER_SLACK)) continue;  // pre-test without division, looser than the test below
+        if (uni > 0.f && __fdiv_rn(inter, uni) >= rthr) hits |= 1u << r;
+      }
+      const int nh = __popc(hits);
+      int incl = nh;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(FULL, incl, o);
+        if (lane >= o) incl += v;
+      }
+      const int total = __shfl_sync(FULL, incl, 31);
+      if (total == 0) continue;
+      unsigned long long base = 0;
+      if (lane == 31) base = atomicAdd(R.count, (unsigned long long)total);
+      unsigned long long o = __shfl_sync(FULL, base, 31) + (unsigned long long)(incl - nh);
+#pragma unroll
+      for (int r = 0; r < 32; r++) {
+        const float t = __shfl_sync(FULL, myB, r);
+        const int row = __shfl_sync(FULL, myrow, r);
+        if ((hits >> r) & 1u) {
+          const float inter = dotU + (float)((cw[r >> 2] >> ((r & 3) * 8)) & 0xFFu);
+          if (o < R.cap) R.out[o] = JaccardPair{rq, row, (int)inter, (int)(nq + t - inter)};
+          o++;
+        }
+      }
+      continue;
+    }
     // 32 rows of the chunk for this lane's query
     float filt = kth;
     if (valid) filt = fmaxf(filt, __int_as_float(__ldcg(&P.gthr[q0 + lane])));
@@ -1041,7 +1096,7 @@ __global__ void __launch_bounds__(J_WARPS * 32, 2) jaccard_scan_kernel(JaccardPa
   }
   // publish this warp's partial lists
   const int part = split * J_WARPS + warp;
-  if (lane < q_count) {
+  if (!RANGE && lane < q_count) {
     for (int j = 0; j < k; j++) {
       const size_t o = ((size_t)part * P.n_q + (q0 + lane)) * k + j;
       const bool used = j < cnt;
@@ -1271,6 +1326,32 @@ __global__ void select_range_kernel(const double *__restrict__ scores, int64_t n
     const int64_t r = r0 + (threadIdx.x & 31);
     const float s = r < n ? (float)scores[r] : -INFINITY;
     range_emit(out, count, cap, r < n && r != excl && s >= thr, &qv, s, row_base + r);
+  }
+}
+
+// The same fallback for a Jaccard threshold search: the test is the float32 rounding of K1a's float64 ratio, and each
+// pair carries its exact counts.  K1a forms s = I / (T - I) from exact integers (T = |q| + |row|) with one rounding,
+// so I = rint(s T / (1 + s)) recovers |q ∩ row|: the expression is off by a few ulps of I, far below 1/2.
+__global__ void jaccard_select_range_kernel(const double *__restrict__ scores, const double *__restrict__ B64,
+                                            const int *__restrict__ invperm, int64_t n, double nq, float thr, int64_t excl,
+                                            int q, JaccardPair *out, unsigned long long *count, unsigned long long cap) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int lane = threadIdx.x & 31;
+  // whole warps step together (blockDim is a multiple of 32): one reservation per warp and 32 rows
+  for (int64_t r0 = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) & ~31LL; r0 < n; r0 += stride) {
+    const int64_t r = r0 + lane;
+    const double s = r < n ? scores[r] : 0.0;
+    const bool hit = r < n && r != excl && (float)s >= thr;
+    const uint32_t hm = __ballot_sync(FULL, hit);
+    if (hm == 0) continue;
+    unsigned long long base = 0;
+    if (lane == 0) base = atomicAdd(count, (unsigned long long)__popc(hm));
+    base = __shfl_sync(FULL, base, 0);
+    if (hit) {
+      const double T = nq + B64[invperm[r]], I = rint(s * T / (1.0 + s));
+      const unsigned long long o = base + (unsigned long long)__popc(hm & lanemask_lt());
+      if (o < cap) out[o] = JaccardPair{q, (int)r, (int)I, (int)(T - I)};
+    }
   }
 }
 

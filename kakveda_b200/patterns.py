@@ -56,8 +56,9 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
     """Similarity-split version of pattern_detector.on_failure.
 
     ``index``: a finalized ``GfkbIndex`` whose row i is ``records[i]['signature_text']`` (corpus-fit mode gives a
-    symmetric measure; the default mode works too), or a finalized ``DenseIndex`` whose row i is record i's embedding
-    (cosine).  Returns one payload per connected component that, restricted
+    symmetric measure; the default mode works too), a finalized ``DenseIndex`` whose row i is record i's embedding
+    (cosine), or a finalized ``JaccardIndex`` whose row i is record i's token set.  Returns one payload per connected
+    component that, restricted
     to ``failure_type`` (if given), spans at least ``min_apps`` apps (app.py:45-46) -- ordered by smallest row id.
     ``k``: rows are linked only through every row's k nearest other rows, so when a text is stored more than k times
     its copies fill the lists and pairs of similar texts are never seen.  ``k=None`` links on the exact threshold
@@ -67,14 +68,15 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
     keep = np.ones(n, dtype=bool)
     if failure_type is not None:
         keep = np.fromiter((r.get("failure_type") == failure_type for r in records), dtype=bool, count=n)
+    # a JaccardIndex returns the exact counts after these arrays: only the leading ones are used
     if k is None:
-        indptr, rows, _ = index.selfjoin_range(threshold)
+        indptr, rows = index.selfjoin_range(threshold)[:2]
         if failure_type is not None:  # rows of other failure types neither join nor bridge components
             src = np.repeat(np.arange(n), np.diff(indptr))
             rows = np.where(keep[src] & keep[rows], rows, -1)
         labels, _ = cluster_csr(indptr, rows)
     else:
-        scores, rows = index.selfjoin_topk(k)
+        scores, rows = index.selfjoin_topk(k)[:2]
         if failure_type is not None:
             # rows of other failure types neither join nor bridge components
             bad = ~keep[np.clip(rows, 0, n - 1)] | (rows < 0)
