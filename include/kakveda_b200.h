@@ -232,6 +232,18 @@ int kv_jaccard_range_resident(kv_index *ix, float threshold, int64_t *n_pairs);
  * inter[n_pairs] = |q ∩ row| and uni[n_pairs] = |q ∪ row|; per query ordered by (score desc, row asc), as
  * kv_range_fetch.  scores[i] is the float32 quotient inter[i] / uni[i].  KV_ERR_STATE when there is none. */
 int kv_jaccard_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores, int32_t *inter, int32_t *uni);
+/* Both fetches order the pairs on the device (an LSD radix sort of the records on (query, score desc, row)) and copy
+ * the ordered arrays back; when pairs plus queries number below 8192 they copy the records back and order them on one
+ * host core, which is faster there (the same bits either way).  The _device forms write the same arrays, bit for bit, to caller-owned device memory (e.g.
+ * torch tensors) on the index's device: d_indptr int64[n_q+1], d_rows int64[n_pairs], d_scores float32[n_pairs], and
+ * for Jaccard d_inter / d_uni int32[n_pairs].  They consume the result like the host fetch and return once the work on
+ * the handle's stream is complete.  KV_ERR_STATE when there is no result (none computed, fetched already, or dropped by
+ * a later upload); KV_ERR_INVALID on the other index kind, or when a pointer is not device memory of the index's device
+ * aligned to its element size (the arrays of n_pairs elements are not looked at when n_pairs == 0).  KV_ERR_NOMEM (with
+ * the pair count) when the ordering's scratch -- about the pair buffer's size again -- does not fit; the result then
+ * stays for another try. */
+int kv_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores);
+int kv_jaccard_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores, void *d_inter, void *d_uni);
 
 /* K6: float64 scores of selected (query, row) pairs: rows[n_q*k] are GLOBAL row ids (e.g. what kv_topk returned;
  * -1 = unused slot), out_scores[n_q*k] (host) receives the float64 cosine of SimilarityEngine.score
@@ -280,6 +292,14 @@ int kv_index_last_kernel_ms(const kv_index *ix, float ms[5]);
  * for every (query slot, chunk): out[n_q][chunks] floats, slot_query[i] = original query of sorted slot i.  Needs an
  * index large enough for the pruned path (>= 512 chunks of 32 rows); tests/test_gpu_parity.py compares with NumPy. */
 int kv_debug_bound_numerators(kv_index *ix, int k, float *out, int32_t *slot_query);
+/* Test hook: orders n caller-built range records (host memory, 16 bytes each, the layout the range scans emit) on
+ * `device` with the code the fetch functions use, so that inputs a real search cannot cheaply produce can be checked.
+ * jaccard = 0: records {int32 q, float32 score, int64 row} (rows global, row_base ignored); jaccard != 0: {int32 q,
+ * int32 local row, int32 inter, int32 uni}, rows + row_base, scores inter / uni in float32.  Outputs as
+ * kv_jaccard_range_fetch (host); inter / uni are only written for Jaccard records.  Records with a query outside
+ * 0..n_q-1, a NaN score or counts outside 0 <= inter <= uni, uni >= 1: KV_ERR_INVALID. */
+int kv_debug_range_order(int device, int jaccard, const void *records, int64_t n, int64_t n_q, int64_t row_base,
+                         int64_t *indptr, int64_t *rows, float *scores, int32_t *inter, int32_t *uni);
 /* CUDA-event milliseconds of the scan kernel of the last kv_score call (K1a). */
 int kv_index_last_score_ms(const kv_index *ix, float *ms);
 
@@ -346,6 +366,8 @@ int kv_dense_selfjoin_range(kv_dense_index *dx, int64_t q_begin, int64_t q_end, 
 /* The last dense range result (host outputs): indptr[n_q+1] by query, rows[n_pairs], scores[n_pairs]; per query ordered
  * by (score desc, row asc).  KV_ERR_STATE when there is none. */
 int kv_dense_range_fetch(kv_dense_index *dx, int64_t *indptr, int64_t *rows, float *scores);
+/* The same arrays in caller-owned device memory, as kv_range_fetch_device (the host fetch orders on the device too). */
+int kv_dense_range_fetch_device(kv_dense_index *dx, void *d_indptr, void *d_rows, void *d_scores);
 /* CUDA-event milliseconds of the GEMM kernel of the last kv_dense_topk* / kv_dense_selfjoin_device or range call (a
  * range re-run after the pair buffer grew included) and its row splits. */
 int kv_dense_last_timing(const kv_dense_index *dx, float *gemm_ms, int64_t *splits);
@@ -382,6 +404,14 @@ int kv_cluster_topk(int64_t n, int k, const int64_t *rows, const float *scores, 
  * result of kv_selfjoin_upload + kv_range_resident these are the components of the exact threshold graph, which a
  * top-k list cannot give when a text is stored more than k times. */
 int kv_cluster_csr(int64_t n, const int64_t *indptr, const int64_t *rows, int64_t *labels, int64_t *n_clusters);
+/* kv_cluster_csr on the device: d_indptr int64[n+1], d_rows int64 (indexed absolutely by indptr, so indptr[0] may be
+ * nonzero) and d_labels int64[n] are device memory of `device` (e.g. the output of kv_range_fetch_device); the same
+ * labels, bit for bit.  A lock-free union-find (roots hooked under smaller roots with compare-and-swap), so labels do
+ * not depend on thread timing.  Validation passes run before any hooking: indptr not monotone or indptr[0] < 0, or a
+ * row >= n: KV_ERR_INVALID.  Pointers that are not device memory of `device` aligned to 8 bytes: KV_ERR_INVALID.
+ * Runs on a stream of its own and returns when the labels are written; n_clusters (host, may be NULL). */
+int kv_cluster_csr_device(int device, int64_t n, const void *d_indptr, const void *d_rows, void *d_labels,
+                          int64_t *n_clusters);
 
 /* ------------------------------------------------------------------------------------
  * Synthetic failures.jsonl-shaped signature_text generator (test / bench support; the

@@ -72,8 +72,13 @@ SIGNATURES = {
     "kv_range_fetch": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f32p]),
     "kv_jaccard_range_resident": (C.c_int, [C.c_void_p, C.c_float, c_i64p]),
     "kv_jaccard_range_fetch": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f32p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "kv_range_fetch_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kv_jaccard_range_fetch_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kv_cluster_topk": (C.c_int, [C.c_int64, C.c_int, c_i64p, c_f32p, C.c_float, c_i64p, c_i64p]),
     "kv_cluster_csr": (C.c_int, [C.c_int64, c_i64p, c_i64p, c_i64p, c_i64p]),
+    "kv_cluster_csr_device": (C.c_int, [C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, c_i64p]),
+    "kv_debug_range_order": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, c_i64p, c_i64p, c_f32p,
+                                       C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "kv_index_thresholds_export": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p]),
     "kv_index_thresholds_peers": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64]),
     "kv_merge_topk_device": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_void_p,
@@ -100,6 +105,7 @@ SIGNATURES = {
     "kv_dense_range_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_int64, c_i64p]),
     "kv_dense_selfjoin_range": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_float, c_i64p]),
     "kv_dense_range_fetch": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f32p]),
+    "kv_dense_range_fetch_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kv_dense_last_timing": (C.c_int, [C.c_void_p, c_f32p, c_i64p]),
     "kv_hash_create": (C.c_int, [C.c_int, C.c_int64, C.POINTER(C.c_void_p)]),
     "kv_hash_destroy": (None, [C.c_void_p]),

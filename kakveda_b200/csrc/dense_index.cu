@@ -394,9 +394,9 @@ struct kv_dense_index {
   // last threshold search: pairs in emit order, kept until fetched or until the next range, top-k, append or finalize
   DevBuf<RangePair> d_range;
   DevBuf<unsigned long long> d_range_count;
-  PinnedBuf<RangePair> h_range;
   bool range_valid = false;
   int64_t range_q = 0, range_pairs = 0;
+  RangeOrderScratch rsort;  // the fetches order the pairs on the device (range_order.cu)
   bool finalized = false;
   float last_ms = 0;
   int64_t last_splits = 0;
@@ -704,14 +704,30 @@ int kv_dense_range_fetch(kv_dense_index *dx, int64_t *indptr, int64_t *rows, flo
   const int64_t n_q = dx->range_q, n = dx->range_pairs;
   if (n > 0 && (!rows || !scores)) return kv_fail(KV_ERR_INVALID, "kv_dense_range_fetch: bad arguments");
   KV_CUDA(cudaSetDevice(dx->device));
-  KV_CUDA(dx->h_range.ensure(std::max<int64_t>(n, 1)));
-  if (n) {
-    KV_CUDA(cudaMemcpyAsync(dx->h_range.p, dx->d_range.p, (size_t)n * sizeof(RangePair), cudaMemcpyDeviceToHost, dx->stream));
-    KV_CUDA(cudaStreamSynchronize(dx->stream));
-  }
-  const int rc = range_order(dx->h_range.p, n, n_q, 0, indptr, rows, scores, nullptr, nullptr, "kv_dense_range_fetch");
+  // ordered on the device in the pair buffer itself (range_order.cu); a failed scratch allocation keeps the result
+  const int rc = range_order_to_host(dx->d_range.p, n, n_q, 0, indptr, rows, scores, nullptr, nullptr, dx->rsort, dx->stream,
+                                     "kv_dense_range_fetch");
+  if (rc != KV_ERR_NOMEM) dx->range_valid = false;
+  return rc;
+}
+
+// Device outputs: the same arrays, written to caller-owned device memory of the index's device.
+int kv_dense_range_fetch_device(kv_dense_index *dx, void *d_indptr, void *d_rows, void *d_scores) {
+  const char *fn = "kv_dense_range_fetch_device";
+  if (!dx) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
+  std::lock_guard<std::mutex> g(dx->mu);
+  if (!dx->range_valid) return kv_fail(KV_ERR_STATE, "%s: no threshold search result (kv_dense_range* first)", fn);
+  const int64_t n_q = dx->range_q, n = dx->range_pairs;
+  int rc = check_device_ptr(d_indptr, dx->device, 8, "indptr", fn);
+  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_rows, dx->device, 8, "rows", fn);
+  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_scores, dx->device, 4, "scores", fn);
   if (rc != KV_OK) return rc;
-  dx->range_valid = false;
+  KV_CUDA(cudaSetDevice(dx->device));
+  rc = range_order_device(dx->d_range.p, n, n_q, 0, (int64_t *)d_indptr, (int64_t *)d_rows, (float *)d_scores, nullptr, nullptr,
+                          dx->rsort, dx->stream, fn);
+  if (rc != KV_ERR_NOMEM) dx->range_valid = false;
+  if (rc != KV_OK) return rc;
+  KV_CUDA(cudaStreamSynchronize(dx->stream));
   return KV_OK;
 }
 

@@ -6,10 +6,7 @@
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
-#include <new>
 #include <thread>
-#include <type_traits>
-#include <vector>
 
 namespace {
 thread_local char g_err[512] = "";
@@ -30,60 +27,6 @@ int host_threads() {
   if (const char *e = getenv("KAKVEDA_B200_THREADS")) t = atoi(e);
   return std::max(1, std::min(t, 64));
 }
-
-namespace {
-// score and row of a record in the order range_order sorts by
-inline float pair_score(const RangePair &p) { return p.score; }
-inline int64_t pair_row(const RangePair &p) { return p.row; }
-inline float pair_score(const JaccardPair &p) { return (float)p.inter / (float)p.uni; }
-inline int64_t pair_row(const JaccardPair &p) { return p.row; }
-}  // namespace
-
-template <class Rec>
-int range_order(const Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
-                int32_t *inter, int32_t *uni, const char *fn) {
-  std::vector<Rec> by_q;
-  try {
-    by_q.resize((size_t)n);
-  } catch (const std::bad_alloc &) {
-    return kv_fail(KV_ERR_NOMEM, "%s: out of host memory", fn);
-  }
-  for (int64_t q = 0; q <= n_q; q++) indptr[q] = 0;
-  for (int64_t i = 0; i < n; i++) indptr[rec[i].q + 1]++;
-  for (int64_t q = 0; q < n_q; q++) indptr[q + 1] += indptr[q];
-  std::vector<int64_t> next(indptr, indptr + n_q);
-  for (int64_t i = 0; i < n; i++) by_q[(size_t)next[(size_t)rec[i].q]++] = rec[i];
-  // thread t orders queries [n_q t / T, n_q (t + 1) / T)
-  const int T = (int)std::max<int64_t>(1, std::min<int64_t>(n >= 65536 ? host_threads() : 1, n_q));
-  auto body = [&](int t) {
-    for (int64_t q = n_q * t / T; q < n_q * (t + 1) / T; q++) {
-      Rec *lo = by_q.data() + indptr[q], *hi = by_q.data() + indptr[q + 1];
-      std::sort(lo, hi, [](const Rec &x, const Rec &y) {
-        const float sx = pair_score(x), sy = pair_score(y);
-        return sx != sy ? sx > sy : pair_row(x) < pair_row(y);
-      });
-      for (Rec *p = lo; p < hi; p++) {
-        const size_t i = (size_t)(p - by_q.data());
-        rows[i] = row_base + pair_row(*p);
-        scores[i] = pair_score(*p);
-        if constexpr (std::is_same_v<Rec, JaccardPair>) {
-          inter[i] = p->inter;
-          uni[i] = p->uni;
-        }
-      }
-    }
-  };
-  std::vector<std::thread> th;
-  for (int t = 1; t < T; t++) th.emplace_back(body, t);
-  body(0);
-  for (auto &x : th) x.join();
-  return KV_OK;
-}
-
-template int range_order<RangePair>(const RangePair *, int64_t, int64_t, int64_t, int64_t *, int64_t *, float *, int32_t *,
-                                    int32_t *, const char *);
-template int range_order<JaccardPair>(const JaccardPair *, int64_t, int64_t, int64_t, int64_t *, int64_t *, float *,
-                                      int32_t *, int32_t *, const char *);
 
 int open_device(int device, const char *fn, int *sm_count) {
   int n = 0;

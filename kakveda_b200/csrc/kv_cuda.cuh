@@ -4,6 +4,7 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <utility>
 
 #define KV_CUDA(expr)                                                                         \
@@ -106,13 +107,37 @@ struct JaccardPair {
   int32_t uni;    // |q ∪ row|
 };
 
-// Orders the n pairs of a threshold search over n_q queries (emit order, as the device left them) into
-// indptr[n_q+1] / rows[n] / scores[n] (and, for JaccardPair records, inter[n] / uni[n]): a counting sort by query, then
-// each query's segment by (score desc, row asc) on the host threads.  row_base is added to JaccardPair rows (RangePair
-// rows are global already).  `fn` names the caller in error messages.  Defined for Rec = RangePair and JaccardPair.
+// Scratch of the device ordering of range records (range_order.cu), owned by an index handle: the buffers keep their
+// capacity across calls, like the pair buffer itself.
+struct RangeOrderScratch {
+  DevBuf<int4> alt;                       // the records' second home during the radix passes
+  DevBuf<unsigned int> counts, partials;  // per-tile digit counts (digit-major) and the sums of their scan tiles
+  DevBuf<unsigned long long> stats;       // min / max of each key field
+  DevBuf<unsigned char> out;              // the ordered arrays on their way to the host (host fetch only)
+  PinnedBuf<int4> staged;                 // the records of a small result, ordered on the host (host fetch only)
+};
+
+// Host fetches whose pairs plus queries number fewer than this order them on one host core (range_order_to_host); the
+// device fetches, and the host fetches of larger results, order on the device.  Measured in DESIGN §6.
+constexpr int64_t RANGE_HOST_ORDER_MAX = 8192;
+
+// Orders the n pairs of a threshold search over n_q queries (emit order, as the device left them; rec is reordered in
+// place) into device arrays indptr[n_q+1] / rows[n] / scores[n] (and, for JaccardPair records, inter[n] / uni[n]) on
+// stream s: per query by (score desc, row asc).  row_base is added to JaccardPair rows (RangePair rows are global
+// already).  Returns once the work is enqueued.  KV_ERR_NOMEM (with the pair count) when the scratch does not fit.
+// `fn` names the caller in error messages.  Defined for Rec = RangePair and JaccardPair.
 template <class Rec>
-int range_order(const Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
-                int32_t *inter, int32_t *uni, const char *fn);
+int range_order_device(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
+                       int32_t *inter, int32_t *uni, RangeOrderScratch &sc, cudaStream_t s, const char *fn);
+// The same into host arrays, stream synchronised: ordered on the device into sc.out and copied back, or below
+// RANGE_HOST_ORDER_MAX pairs plus queries copied back as records and ordered on the host (the same bits).
+template <class Rec>
+int range_order_to_host(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
+                        int32_t *inter, int32_t *uni, RangeOrderScratch &sc, cudaStream_t s, const char *fn);
+
+// KV_OK when p is device memory of `device` aligned to `align` bytes, else KV_ERR_INVALID naming `what` (a host pointer
+// passed by mistake is an error, never a fault).
+int check_device_ptr(const void *p, int device, size_t align, const char *what, const char *fn);
 
 // Non-blocking stream; converts to cudaStream_t.
 struct CudaStream {

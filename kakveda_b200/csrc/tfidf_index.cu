@@ -129,14 +129,13 @@ struct kv_index {
   DevBuf<int> d_rthr;
   DevBuf<RangePair> d_range;
   DevBuf<unsigned long long> d_range_count;
-  PinnedBuf<RangePair> h_range;
   bool range_valid = false;
   // the same on a Jaccard index (K3-R, kv_jaccard_range_resident): the records carry the exact counts and have a
   // result flag of their own, so kv_range_fetch never reads them
   DevBuf<JaccardPair> d_jrange;
-  PinnedBuf<JaccardPair> h_jrange;
   bool jrange_valid = false;
   int64_t range_q = 0, range_pairs = 0;
+  RangeOrderScratch rsort;  // the fetches order the pairs on the device (range_order.cu)
   DevBuf<unsigned long long> d_stats;
   DevBuf<float> d_part_s, d_out_s;
   DevBuf<long long> d_part_r, d_out_r;
@@ -1614,7 +1613,10 @@ int kv_jaccard_range_resident(kv_index *ix, float threshold, int64_t *n_pairs) {
 }
 
 // The pairs come back in emit order, which the scan does not fix; scores are exact integer sums rounded once, so
-// (score desc, row asc) is a total order of each query's pairs and the result is deterministic.
+// (score desc, row asc) is a total order of each query's pairs and the result is deterministic.  Both fetches order the
+// pairs on the device (range_order.cu, in the pair buffer itself: the fetch consumes the result) and copy the ordered
+// arrays back.  Once ordering has started the result is gone whatever happens; a scratch allocation that fails first
+// (KV_ERR_NOMEM) leaves it for another try.
 int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores) {
   if (!ix || !indptr) return kv_fail(KV_ERR_INVALID, "kv_range_fetch: bad arguments");
   std::lock_guard<std::mutex> g(ix->mu);
@@ -1622,15 +1624,10 @@ int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores) 
   const int64_t n_q = ix->range_q, n = ix->range_pairs;
   if (n > 0 && (!rows || !scores)) return kv_fail(KV_ERR_INVALID, "kv_range_fetch: bad arguments");
   KV_CUDA(cudaSetDevice(ix->device));
-  KV_CUDA(ix->h_range.ensure(std::max<int64_t>(n, 1)));
-  if (n) {
-    KV_CUDA(cudaMemcpyAsync(ix->h_range.p, ix->d_range.p, (size_t)n * sizeof(RangePair), cudaMemcpyDeviceToHost, ix->stream));
-    KV_CUDA(cudaStreamSynchronize(ix->stream));
-  }
-  const int rc = range_order(ix->h_range.p, n, n_q, 0, indptr, rows, scores, nullptr, nullptr, "kv_range_fetch");
-  if (rc != KV_OK) return rc;
-  ix->range_valid = false;
-  return KV_OK;
+  const int rc = range_order_to_host(ix->d_range.p, n, n_q, 0, indptr, rows, scores, nullptr, nullptr, ix->rsort, ix->stream,
+                                     "kv_range_fetch");
+  if (rc != KV_ERR_NOMEM) ix->range_valid = false;
+  return rc;
 }
 
 // Same order as kv_range_fetch: the score is inter / union rounded to float32, and equal scores order by row.
@@ -1643,14 +1640,52 @@ int kv_jaccard_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *
   const int64_t n_q = ix->range_q, n = ix->range_pairs;
   if (n > 0 && (!rows || !scores || !inter || !uni)) return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_fetch: bad arguments");
   KV_CUDA(cudaSetDevice(ix->device));
-  KV_CUDA(ix->h_jrange.ensure(std::max<int64_t>(n, 1)));
-  if (n) {
-    KV_CUDA(cudaMemcpyAsync(ix->h_jrange.p, ix->d_jrange.p, (size_t)n * sizeof(JaccardPair), cudaMemcpyDeviceToHost, ix->stream));
-    KV_CUDA(cudaStreamSynchronize(ix->stream));
-  }
-  const int rc = range_order(ix->h_jrange.p, n, n_q, ix->row_base, indptr, rows, scores, inter, uni, "kv_jaccard_range_fetch");
+  const int rc = range_order_to_host(ix->d_jrange.p, n, n_q, ix->row_base, indptr, rows, scores, inter, uni, ix->rsort,
+                                     ix->stream, "kv_jaccard_range_fetch");
+  if (rc != KV_ERR_NOMEM) ix->jrange_valid = false;
+  return rc;
+}
+
+// Device outputs: the same arrays, written to caller-owned device memory of the index's device.
+int kv_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores) {
+  const char *fn = "kv_range_fetch_device";
+  if (!ix) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (ix->jaccard) return kv_fail(KV_ERR_INVALID, "%s: a Jaccard index fetches with kv_jaccard_range_fetch_device", fn);
+  if (!ix->range_valid) return kv_fail(KV_ERR_STATE, "%s: no threshold search result (kv_range_resident first)", fn);
+  const int64_t n_q = ix->range_q, n = ix->range_pairs;
+  int rc = check_device_ptr(d_indptr, ix->device, 8, "indptr", fn);
+  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_rows, ix->device, 8, "rows", fn);
+  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_scores, ix->device, 4, "scores", fn);
   if (rc != KV_OK) return rc;
-  ix->jrange_valid = false;
+  KV_CUDA(cudaSetDevice(ix->device));
+  rc = range_order_device(ix->d_range.p, n, n_q, 0, (int64_t *)d_indptr, (int64_t *)d_rows, (float *)d_scores, nullptr, nullptr,
+                          ix->rsort, ix->stream, fn);
+  if (rc != KV_ERR_NOMEM) ix->range_valid = false;
+  if (rc != KV_OK) return rc;
+  KV_CUDA(cudaStreamSynchronize(ix->stream));
+  return KV_OK;
+}
+
+int kv_jaccard_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores, void *d_inter, void *d_uni) {
+  const char *fn = "kv_jaccard_range_fetch_device";
+  if (!ix) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (!ix->jaccard) return kv_fail(KV_ERR_INVALID, "%s: not a Jaccard index (kv_range_fetch_device)", fn);
+  if (!ix->jrange_valid) return kv_fail(KV_ERR_STATE, "%s: no threshold search result (kv_jaccard_range_resident first)", fn);
+  const int64_t n_q = ix->range_q, n = ix->range_pairs;
+  int rc = check_device_ptr(d_indptr, ix->device, 8, "indptr", fn);
+  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_rows, ix->device, 8, "rows", fn);
+  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_scores, ix->device, 4, "scores", fn);
+  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_inter, ix->device, 4, "inter", fn);
+  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_uni, ix->device, 4, "uni", fn);
+  if (rc != KV_OK) return rc;
+  KV_CUDA(cudaSetDevice(ix->device));
+  rc = range_order_device(ix->d_jrange.p, n, n_q, ix->row_base, (int64_t *)d_indptr, (int64_t *)d_rows, (float *)d_scores,
+                          (int32_t *)d_inter, (int32_t *)d_uni, ix->rsort, ix->stream, fn);
+  if (rc != KV_ERR_NOMEM) ix->jrange_valid = false;
+  if (rc != KV_OK) return rc;
+  KV_CUDA(cudaStreamSynchronize(ix->stream));
   return KV_OK;
 }
 

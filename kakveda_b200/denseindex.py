@@ -11,7 +11,7 @@ from typing import Tuple
 
 import numpy as np
 
-from . import _capi
+from . import _capi, _devout
 
 
 def to_bf16_bits(x: np.ndarray) -> np.ndarray:
@@ -82,7 +82,11 @@ class DenseIndex:
                                                rows.ctypes.data_as(C.POINTER(C.c_int64))))
         return scores, rows
 
-    def _range_fetch(self, n_q: int, n_pairs: int) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    def _range_fetch(self, n_q: int, n_pairs: int, device_out: bool = False):
+        if device_out:
+            out = _devout.range_arrays(self.device, n_q, n_pairs)
+            _capi.check(_capi.load().kv_dense_range_fetch_device(self._h, *_devout.ptrs(out)))
+            return out
         indptr = np.empty(n_q + 1, dtype=np.int64)
         rows = np.empty(n_pairs, dtype=np.int64)
         scores = np.empty(n_pairs, dtype=np.float32)
@@ -91,20 +95,22 @@ class DenseIndex:
                                                       scores.ctypes.data_as(C.POINTER(C.c_float))))
         return indptr, rows, scores
 
-    def range(self, queries: np.ndarray, threshold: float) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    def range(self, queries: np.ndarray, threshold: float, device_out: bool = False):
         """Threshold search: every (query, row) pair whose cosine (the float32 value ``topk`` reports, bit for bit) is
         >= ``threshold``, 0 < threshold <= 1.  ``queries``: float rows or bf16 bit patterns (uint16), host memory.
         Returns ``(indptr int64[n_q+1], rows int64[P], scores float32[P])``: query q's pairs are
-        ``[indptr[q], indptr[q+1])``, ordered by (score desc, row asc); rows are global."""
+        ``[indptr[q], indptr[q+1])``, ordered by (score desc, row asc); rows are global.  ``device_out``: the same
+        arrays as torch tensors on the index's device."""
         bits = queries if queries.dtype == np.uint16 else to_bf16_bits(queries)
         bits = np.ascontiguousarray(bits).reshape(-1, self.dim)
         n = C.c_int64(0)
         _capi.check(_capi.load().kv_dense_range(self._h, bits.ctypes.data_as(C.POINTER(C.c_uint16)), bits.shape[0],
                                                 np.float32(threshold), C.byref(n)))
-        return self._range_fetch(bits.shape[0], n.value)
+        return self._range_fetch(bits.shape[0], n.value, device_out)
 
-    def range_device(self, queries, threshold: float, exclude_base: int = -1) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
-        """``range`` of queries on the device (a contiguous torch bfloat16 tensor [Q, dim]); results on the host.
+    def range_device(self, queries, threshold: float, exclude_base: int = -1, device_out: bool = False):
+        """``range`` of queries on the device (a contiguous torch bfloat16 tensor [Q, dim]); results on the host, or
+        with ``device_out`` as torch tensors on the index's device.
         ``exclude_base >= 0``: query q never matches GLOBAL row ``exclude_base + q``."""
         import torch
 
@@ -114,15 +120,15 @@ class DenseIndex:
         n = C.c_int64(0)
         _capi.check(_capi.load().kv_dense_range_device(self._h, C.c_void_p(queries.data_ptr()), n_q, np.float32(threshold),
                                                        exclude_base, C.byref(n)))
-        return self._range_fetch(n_q, n.value)
+        return self._range_fetch(n_q, n.value, device_out)
 
-    def selfjoin_range(self, threshold: float, lo: int = 0, hi: int | None = None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    def selfjoin_range(self, threshold: float, lo: int = 0, hi: int | None = None, device_out: bool = False):
         """All-pairs threshold search: for local rows [lo, hi) every OTHER row scoring >= ``threshold`` (CSR as in
         ``range``, query i = row lo + i)."""
         hi = self.n_rows if hi is None else hi
         n = C.c_int64(0)
         _capi.check(_capi.load().kv_dense_selfjoin_range(self._h, lo, hi, np.float32(threshold), C.byref(n)))
-        return self._range_fetch(hi - lo, n.value)
+        return self._range_fetch(hi - lo, n.value, device_out)
 
     def last_timing(self) -> Tuple[float, int]:
         ms, sp = C.c_float(), C.c_int64()

@@ -16,7 +16,7 @@ from typing import Optional, Sequence, Tuple
 
 import numpy as np
 
-from . import _capi
+from . import _capi, _devout
 
 
 def _csr(sets: Sequence[Sequence[int]]) -> Tuple[np.ndarray, np.ndarray]:
@@ -36,7 +36,7 @@ class JaccardIndex:
     def __init__(self, vocab_size: int, device: int = 0, row_base: int = 0):
         h = C.c_void_p()
         _capi.check(_capi.load().kv_index_create(device, row_base, C.byref(h)))
-        self._h, self.vocab_size = h, int(vocab_size)
+        self._h, self.vocab_size, self.device = h, int(vocab_size), device
         # the appended rows, for the counts of self-join pairs (the query of a self-join is a stored row)
         self._parts = []
         _capi.check(_capi.load().kv_index_set_mode(h, 1))
@@ -115,10 +115,14 @@ class JaccardIndex:
     def topk_sets(self, queries: Sequence[Sequence[int]], k: int = 16):
         return self.topk_csr(*_csr(queries), k=k)
 
-    def _range_resident(self, n_q: int, threshold: float):
+    def _range_resident(self, n_q: int, threshold: float, device_out: bool = False):
         lib = _capi.load()
         n = C.c_int64(0)
         _capi.check(lib.kv_jaccard_range_resident(self._h, np.float32(threshold), C.byref(n)))
+        if device_out:
+            out = _devout.range_arrays(self.device, n_q, n.value, jaccard=True)
+            _capi.check(lib.kv_jaccard_range_fetch_device(self._h, *_devout.ptrs(out)))
+            return out
         indptr = np.empty(n_q + 1, dtype=np.int64)
         rows = np.empty(n.value, dtype=np.int64)
         scores = np.empty(n.value, dtype=np.float32)
@@ -128,28 +132,30 @@ class JaccardIndex:
                                                _p(inter, C.c_int32), _p(union, C.c_int32)))
         return indptr, rows, scores, inter, union
 
-    @staticmethod
-    def _empty_range():
+    def _empty_range(self, device_out: bool = False):
+        if device_out:
+            return _devout.empty_range(self.device, jaccard=True)
         return (np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32), np.zeros(0, np.int32),
                 np.zeros(0, np.int32))
 
-    def range_csr(self, indptr: np.ndarray, ids: np.ndarray, threshold: float):
+    def range_csr(self, indptr: np.ndarray, ids: np.ndarray, threshold: float, device_out: bool = False):
         """Threshold search: every (query, row) pair whose float32 score (the value ``topk_csr`` reports) is
         >= ``threshold``, 0 < threshold <= 1.  Returns ``(indptr int64[Q+1], rows int64[P], scores float32[P],
         inter int32[P], union int32[P])``: query q's pairs are ``[indptr[q], indptr[q+1])``, ordered by (score desc,
-        row asc); rows are global; ``scores == float32(inter / union)`` with the exact counts."""
+        row asc); rows are global; ``scores == float32(inter / union)`` with the exact counts.  ``device_out``: the
+        same five arrays as torch tensors on the index's device."""
         indptr, ids, oov = self._strip_oov(indptr, ids)
         n = len(indptr) - 1
         if n == 0:
-            return self._empty_range()
+            return self._empty_range(device_out)
         tf = np.ones(len(ids), dtype=np.uint32)
         _capi.check(_capi.load().kv_query_upload(self._h, _p(indptr, C.c_int64), _p(ids, C.c_uint32), _p(tf, C.c_uint32),
                                                  _p(oov, C.c_double), n))
-        return self._range_resident(n, threshold)
+        return self._range_resident(n, threshold, device_out)
 
-    def range_sets(self, queries: Sequence[Sequence[int]], threshold: float):
+    def range_sets(self, queries: Sequence[Sequence[int]], threshold: float, device_out: bool = False):
         """``range_csr`` of token sets."""
-        return self.range_csr(*_csr(queries), threshold)
+        return self.range_csr(*_csr(queries), threshold, device_out)
 
     def selfjoin_topk(self, k: int, lo: int = 0, hi: Optional[int] = None):
         """All-pairs: for local rows [lo, hi) the k best OTHER rows (the row itself is excluded), as ``topk_csr``:
@@ -168,14 +174,14 @@ class JaccardIndex:
         inter, union = self._counts(indptr, ids, np.zeros(n, np.float64), rows)
         return scores, rows, inter, union
 
-    def selfjoin_range(self, threshold: float, lo: int = 0, hi: Optional[int] = None):
+    def selfjoin_range(self, threshold: float, lo: int = 0, hi: Optional[int] = None, device_out: bool = False):
         """All-pairs threshold search: for local rows [lo, hi) every OTHER row scoring >= ``threshold`` (the five
         arrays of ``range_csr``, query i = row lo + i)."""
         hi = self.n_rows if hi is None else hi
         if hi <= lo:
-            return self._empty_range()
+            return self._empty_range(device_out)
         _capi.check(_capi.load().kv_selfjoin_upload(self._h, lo, hi))
-        return self._range_resident(hi - lo, threshold)
+        return self._range_resident(hi - lo, threshold, device_out)
 
     def last_timing_ms(self):
         ms = (C.c_float * 4)()

@@ -31,8 +31,32 @@ def cluster_topk(rows: np.ndarray, scores: np.ndarray, threshold: float) -> Tupl
     return labels, int(count.value)
 
 
-def cluster_csr(indptr: np.ndarray, rows: np.ndarray) -> Tuple[np.ndarray, int]:
-    """labels[i] = smallest row id of i's component in the graph {i ~ rows[j] : indptr[i] <= j < indptr[i+1], rows[j] >= 0}."""
+def _cluster_csr_device(indptr, rows):
+    import torch
+
+    for name, t in (("indptr", indptr), ("rows", rows)):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.int64):
+            raise ValueError(f"cluster_csr: {name} must be an int64 CUDA tensor when the other one is on the device")
+    if indptr.device != rows.device or indptr.dim() != 1 or indptr.numel() < 1:
+        raise ValueError("cluster_csr: indptr and rows must be on one device, indptr 1-D with n + 1 entries")
+    indptr, rows = indptr.contiguous(), rows.contiguous()
+    n = indptr.numel() - 1
+    labels = torch.empty(n, dtype=torch.int64, device=indptr.device)
+    count = C.c_int64(0)
+    torch.cuda.current_stream(indptr.device).synchronize()  # the library reads the inputs on a stream of its own
+    _capi.check(_capi.load().kv_cluster_csr_device(indptr.device.index, n, C.c_void_p(indptr.data_ptr()),
+                                                   C.c_void_p(rows.data_ptr()), C.c_void_p(labels.data_ptr()),
+                                                   C.byref(count)))
+    return labels, int(count.value)
+
+
+def cluster_csr(indptr, rows) -> Tuple[Any, int]:
+    """labels[i] = smallest row id of i's component in the graph {i ~ rows[j] : indptr[i] <= j < indptr[i+1], rows[j] >= 0}.
+
+    NumPy inputs are clustered on the host; int64 CUDA tensors (e.g. ``selfjoin_range(..., device_out=True)``) on
+    their device, and the labels come back as a tensor there."""
+    if getattr(indptr, "is_cuda", False) or getattr(rows, "is_cuda", False):
+        return _cluster_csr_device(indptr, rows)
     indptr = np.ascontiguousarray(indptr, dtype=np.int64)
     rows = np.ascontiguousarray(rows, dtype=np.int64)
     n = len(indptr) - 1
@@ -70,11 +94,19 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
         keep = np.fromiter((r.get("failure_type") == failure_type for r in records), dtype=bool, count=n)
     # a JaccardIndex returns the exact counts after these arrays: only the leading ones are used
     if k is None:
-        indptr, rows = index.selfjoin_range(threshold)[:2]
+        # the threshold graph stays on the device: only the n labels come back
+        import torch
+
+        indptr, rows = index.selfjoin_range(threshold, device_out=True)[:2]
         if failure_type is not None:  # rows of other failure types neither join nor bridge components
-            src = np.repeat(np.arange(n), np.diff(indptr))
-            rows = np.where(keep[src] & keep[rows], rows, -1)
+            m = indptr.numel() - 1
+            if m > n or (rows.numel() and int(rows.max()) >= n):
+                raise IndexError(f"detect_patterns: the index holds rows beyond the {n} records")
+            keep_d = torch.from_numpy(keep).to(rows.device)
+            src = torch.repeat_interleave(torch.arange(m, device=rows.device), torch.diff(indptr))
+            rows = torch.where(keep_d[src] & keep_d[rows], rows, torch.full_like(rows, -1))
         labels, _ = cluster_csr(indptr, rows)
+        labels = labels.cpu().numpy()
     else:
         scores, rows = index.selfjoin_topk(k)[:2]
         if failure_type is not None:

@@ -20,7 +20,7 @@ from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from . import _capi
+from . import _capi, _devout
 
 _TOKEN = re.compile(r"(?u)\b\w\w+\b")  # sklearn text.py:1969; used only for non-ASCII documents
 
@@ -355,41 +355,51 @@ class GfkbIndex:
         _capi.check(_capi.load().kv_selfjoin_upload(self._h, lo, hi))
         return self.topk_resident_host(hi - lo, k)
 
-    def _range_resident(self, n_q: int, threshold: float) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    def _range_resident(self, n_q: int, threshold: float, device_out: bool = False):
         lib = _capi.load()
         n = C.c_int64(0)
         _capi.check(lib.kv_range_resident(self._h, np.float32(threshold), C.byref(n)))
+        if device_out:
+            out = _devout.range_arrays(self.device, n_q, n.value)
+            _capi.check(lib.kv_range_fetch_device(self._h, *_devout.ptrs(out)))
+            return out
         indptr = np.empty(n_q + 1, dtype=np.int64)
         rows = np.empty(n.value, dtype=np.int64)
         scores = np.empty(n.value, dtype=np.float32)
         _capi.check(lib.kv_range_fetch(self._h, _ptr(indptr, C.c_int64), _ptr(rows, C.c_int64), _ptr(scores, C.c_float)))
         return indptr, rows, scores
 
-    def range_features(self, fb: FeatureBatch, threshold: float) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    def _empty_range(self, device_out: bool):
+        if device_out:
+            return _devout.empty_range(self.device)
+        return np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32)
+
+    def range_features(self, fb: FeatureBatch, threshold: float, device_out: bool = False):
         """Threshold search: every (query, row) pair whose float32 score (the value ``topk`` reports) is >= ``threshold``,
         0 < threshold <= 1.  Returns ``(indptr int64[n_q+1], rows int64[P], scores float32[P])``: query q's pairs are
-        ``[indptr[q], indptr[q+1])``, ordered by (score desc, row asc); rows are global."""
+        ``[indptr[q], indptr[q+1])``, ordered by (score desc, row asc); rows are global.  ``device_out``: the same
+        arrays as torch tensors on the index's device (nothing is copied to the host)."""
         if fb.n == 0:
-            return np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32)
+            return self._empty_range(device_out)
         self.upload_queries(fb)
-        return self._range_resident(fb.n, threshold)
+        return self._range_resident(fb.n, threshold, device_out)
 
-    def range(self, queries: Sequence[str], threshold: float) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    def range(self, queries: Sequence[str], threshold: float, device_out: bool = False):
         """``range_features`` of texts."""
         fb = self.vocab.featurize(queries, grow=False)
         try:
-            return self.range_features(fb, threshold)
+            return self.range_features(fb, threshold, device_out)
         finally:
             fb.close()
 
-    def selfjoin_range(self, threshold: float, lo: int = 0, hi: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    def selfjoin_range(self, threshold: float, lo: int = 0, hi: Optional[int] = None, device_out: bool = False):
         """All-pairs threshold search: for local rows [lo, hi) every OTHER row scoring >= ``threshold`` (CSR as in
         ``range_features``, query i = row lo + i)."""
         hi = self.n_rows if hi is None else hi
         if hi <= lo:
-            return np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32)
+            return self._empty_range(device_out)
         _capi.check(_capi.load().kv_selfjoin_upload(self._h, lo, hi))
-        return self._range_resident(hi - lo, threshold)
+        return self._range_resident(hi - lo, threshold, device_out)
 
     def rescore(self, fb: FeatureBatch, rows: np.ndarray) -> np.ndarray:
         """K6: float64 scores of the pairs (query q, GLOBAL row rows[q, j]); identical rows tie exactly on every shard."""

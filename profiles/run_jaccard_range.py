@@ -8,9 +8,11 @@ swaps), so that theta in {0.5, 0.7, 0.9} returns a non-trivial number of pairs.
 Times, in one process and alternated per round after a warm-up round (which also grows the pair buffer): K3 top-16
 (`kv_topk_resident_host`, kernel = CUDA events around the scan) against K3-R (`kv_jaccard_range_resident`, kernel =
 `kv_index_last_kernel_ms()[3]`, irregular-query fallbacks [4]) on the same uploaded batch, the host clock around
-`kv_jaccard_range_fetch` (copy back, counting sort by query, per-query sort), and the self-join of the first
+`kv_jaccard_range_fetch` (ordering on the device, arrays copied back) and, for the same search run again, around
+`kv_jaccard_range_fetch_device` (arrays left in device memory; the digests must agree), and the self-join of the first
 `--selfjoin` (200k) sets as an index of their own: self-join top-16 against the self-join range at each theta."""
 import ctypes as C
+import hashlib
 import subprocess
 import sys
 import time
@@ -20,7 +22,7 @@ import numpy as np
 import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
-from kakveda_b200 import JaccardIndex, _capi
+from kakveda_b200 import JaccardIndex, _capi, _devout
 
 args = [a for i, a in enumerate(sys.argv[1:]) if not a.startswith("--") and not sys.argv[i].startswith("--")]
 n = int(args[0]) if args else 1_000_000
@@ -81,8 +83,13 @@ def kernel_ms(jx):
     return list(ms)
 
 
+def digest(arrays):
+    return hashlib.sha256(b"".join(a.tobytes() for a in arrays)).hexdigest()[:16]
+
+
 def range_timed(jx, n_q, theta):
-    """(pairs, K3-R ms, fallback ms, call ms, fetch + ordering ms) of one search over the resident batch."""
+    """(pairs, K3-R ms, fallback ms, call ms, host fetch ms, device fetch ms, digest): the search over the resident
+    batch twice, fetched to host memory (ordering on the device, arrays copied back) and then to device memory."""
     cnt = C.c_int64(0)
     t0 = time.perf_counter()
     _capi.check(lib.kv_jaccard_range_resident(jx._h, C.c_float(theta), C.byref(cnt)))
@@ -95,7 +102,15 @@ def range_timed(jx, n_q, theta):
     _capi.check(lib.kv_jaccard_range_fetch(jx._h, p(out[0], C.c_int64), p(out[1], C.c_int64), p(out[2], C.c_float),
                                            p(out[3], C.c_int32), p(out[4], C.c_int32)))
     t3 = time.perf_counter()
-    return m, ms[3], ms[4], 1e3 * (t1 - t0), 1e3 * (t3 - t2)
+    d_host = digest([out[0]] + [a[:m] for a in out[1:]])
+    _capi.check(lib.kv_jaccard_range_resident(jx._h, C.c_float(theta), C.byref(cnt)))
+    dout = _devout.range_arrays(0, n_q, cnt.value, jaccard=True)
+    torch.cuda.synchronize()
+    t4 = time.perf_counter()
+    _capi.check(lib.kv_jaccard_range_fetch_device(jx._h, *_devout.ptrs(dout)))
+    t5 = time.perf_counter()
+    assert digest([a.cpu().numpy() for a in dout]) == d_host
+    return m, ms[3], ms[4], 1e3 * (t1 - t0), 1e3 * (t3 - t2), 1e3 * (t5 - t4), d_host
 
 
 def topk_timed(jx, n_q, k):
@@ -111,10 +126,10 @@ def run(jx, label, n_q, upload, report):
     if report:
         print(f"{label} K3_top16 kernel_ms {ms:.2f}", flush=True)
     for theta in thetas:  # the range leaves the uploaded batch as it was
-        m, kms, fms, call, fetch = range_timed(jx, n_q, theta)
+        m, kms, fms, call, fetch, dfetch, dg = range_timed(jx, n_q, theta)
         if report:
             print(f"{label} K3R theta {theta} pairs {m} kernel_ms {kms:.2f} fallback_ms {fms:.2f} call_ms {call:.1f} "
-                  f"fetch_order_ms {fetch:.1f}", flush=True)
+                  f"host_fetch_ms {fetch:.1f} device_fetch_ms {dfetch:.1f} digest {dg}", flush=True)
 
 
 jx = JaccardIndex(V)
