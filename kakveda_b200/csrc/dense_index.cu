@@ -219,7 +219,7 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
     float inv_q = 0.f;
     float thr = -INFINITY;  // own k-th score: later rows must beat it strictly (rows ascend inside a CTA)
     float gth = -INFINITY;  // k-th score another CTA already secured for this query: ties may still win on row id
-    float gth_pred = -INFINITY;  // largest float below gth
+    float gth_pred = -INFINITY;  // largest float below gth (-0 is not below +0)
     float lo = INFINITY;         // a row enters the list iff its score > lo
     auto flush = [&]() {    // publish the list of (cur_qtile, this CTA)
       if (cur_qtile < 0 || !q_ok) return;
@@ -287,7 +287,9 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
           const unsigned int gk = *(volatile unsigned int *)&P.gthr[q];
           if (gk > fkey(-INFINITY) && fkey_inv(gk) > gth) {
             gth = fkey_inv(gk);
-            gth_pred = fkey_inv(gk - 1);  // the order-preserving key makes "previous float" a decrement
+            // the order-preserving key makes "previous float" a decrement, except below +0: the key before it is -0,
+            // which compares equal to +0 and would reject the rows scoring exactly 0 that tie with a k-th score of 0
+            gth_pred = fkey_inv(gk - (gk == fkey(0.f) ? 2u : 1u));
             lo = fmaxf(thr, gth_pred);
           }
         }
