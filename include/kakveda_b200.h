@@ -202,6 +202,20 @@ int kv_query_set_exclusions(kv_index *ix, const int64_t *exclude_rows, int64_t n
  * excluding itself (follow with kv_topk_resident / kv_topk_resident_host). */
 int kv_selfjoin_upload(kv_index *ix, int64_t q_begin, int64_t q_end);
 
+/* Label filter.  kv_index_set_row_labels gives every local row a label >= 0 (e.g. a failure-type id), labels[n] by
+ * local row, n == kv_index_rows (else KV_ERR_INVALID, as for a negative label).  Labels may be set before or after
+ * finalize and survive either kind of finalize and kv_index_layout_load; kv_index_append drops them.  NULL clears.
+ * kv_query_set_filter restricts each query of the resident batch (kv_query_upload / kv_selfjoin_upload) to the rows
+ * carrying labels[q] (by original query; -1: every row), with the lifetime of kv_query_set_exclusions; NULL clears.
+ * A filtered query's top-k is the top-k over its label's rows -- (score desc, row asc), the same float32 scores as
+ * unfiltered, the zero-score fill and null queries take the label's rows in ascending order, (-inf, -1) past its last
+ * row -- and its threshold search returns the unfiltered pairs of its label.  The index statistics do not change.
+ * KV_ERR_INVALID: wrong length, a label below -1, or a Jaccard index (mode 1).  KV_ERR_STATE: a filtered batch on an
+ * index whose labels are missing or stale (appended rows), here or at the search.  Not combinable with the threshold
+ * exchange of a row-sharded GFKB (kv_index_thresholds_*: KV_ERR_INVALID). */
+int kv_index_set_row_labels(kv_index *ix, const int32_t *labels, int64_t n);
+int kv_query_set_filter(kv_index *ix, const int32_t *labels, int64_t n_q);
+
 /* Threshold search over the resident batch (kv_query_upload / kv_selfjoin_upload; exclusions honoured): every
  * (query, row) pair whose score -- the float32 value kv_topk reports for that pair -- is >= threshold,
  * 0 < threshold <= 1.  *n_pairs receives the count; the pairs stay in the handle until kv_range_fetch, the next

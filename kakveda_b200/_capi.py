@@ -67,6 +67,8 @@ SIGNATURES = {
     "kv_topk_resident_finish": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "kv_query_set_exclusions": (C.c_int, [C.c_void_p, c_i64p, C.c_int64]),
     "kv_selfjoin_upload": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64]),
+    "kv_index_set_row_labels": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int64]),
+    "kv_query_set_filter": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int64]),
     "kv_rescore_pairs": (C.c_int, [C.c_void_p, c_i64p, c_u32p, c_u32p, c_f64p, C.c_int64, C.c_int, c_i64p, c_f64p]),
     "kv_range_resident": (C.c_int, [C.c_void_p, C.c_float, c_i64p]),
     "kv_range_fetch": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f32p]),

@@ -570,10 +570,15 @@ struct SelectParams {
   int n_bsplits;
   CandLists lists;
   unsigned long long *stats;
+  const int *q_label;                   // FILTER: [n_q] label filter by sorted slot, -1 = any (kv_query_set_filter)
+  const unsigned long long *chunk_sig;  // FILTER: [n_chunks_pad] chunk label signatures
 };
 
 constexpr int SEL_WARPS = 8;
 
+// FILTER: a chunk joins a filtered query's mask only when its label signature holds the query's label bit as well --
+// with few allowed rows among the seeds the threshold stays at 0 and the code test alone would pass every chunk
+template <bool FILTER>
 __global__ void __launch_bounds__(SEL_WARPS * 32) tfidf_select_kernel(SelectParams P) {
   extern __shared__ int s_pages[];  // [max_pages]
   __shared__ unsigned int s_count;
@@ -594,15 +599,27 @@ __global__ void __launch_bounds__(SEL_WARPS * 32) tfidf_select_kernel(SelectPara
   const int64_t n_blocks = (P.n_chunks + B_BN - 1) / B_BN;
   const int64_t c_lo = (n_blocks * bsplit / P.n_bsplits) * B_BN, c_hi = min(P.n_chunks, (n_blocks * (bsplit + 1) / P.n_bsplits) * B_BN);
   const unsigned char *row = P.ubq + (size_t)min(slot, P.n_q - 1) * P.ubq_stride;
+  unsigned long long qbit = 0;  // FILTER: the query's label bit, every bit when it is not filtered
+  if constexpr (FILTER) {
+    const int lb = q_ok ? P.q_label[slot] : -1;
+    qbit = lb < 0 ? ~0ull : 1ull << (lb & 63);
+  }
   unsigned int n_pairs = 0, n_recs = 0;
   for (int64_t c = c_lo + 32 * warp; c < c_hi; c += 32 * SEL_WARPS) {
     const uint4 a = __ldcs(reinterpret_cast<const uint4 *>(row + c)), b = __ldcs(reinterpret_cast<const uint4 *>(row + c + 16));
     const uint32_t wds[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    unsigned long long sig = 0;  // FILTER: signature of chunk c + lane
+    if constexpr (FILTER) sig = c + lane < c_hi ? P.chunk_sig[c + lane] : 0ull;
     uint32_t mymask = 0;
 #pragma unroll
     for (int j = 0; j < 32; j++) {
       const uint32_t code = (wds[j >> 2] >> ((j & 3) * 8)) & 0xFFu;
-      const uint32_t m = __ballot_sync(FULL, q_ok && code >= tcode && c + j < c_hi);
+      bool take = q_ok && code >= tcode && c + j < c_hi;
+      if constexpr (FILTER) {
+        const unsigned long long sig_j = __shfl_sync(FULL, sig, j);  // every lane: not under the condition above
+        take = take && (sig_j & qbit) != 0ull;
+      }
+      const uint32_t m = __ballot_sync(FULL, take);
       if (lane == j) mymask = m;
     }
     list_append(P.lists, list, &s_count, s_pages, (uint32_t)(c + lane), mymask, n_pairs, n_recs);

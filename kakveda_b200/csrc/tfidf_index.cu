@@ -124,6 +124,18 @@ struct kv_index {
   DevBuf<int> d_excl_sorted, d_excl_orig;  // self-join exclusions of the resident batch (by sorted slot / by original query)
   std::vector<int> h_excl_orig;
   bool has_excl = false;
+  // row labels (kv_index_set_row_labels), by local row; dropped by an append.  On the device (rebuilt by every finalize):
+  // by row, by scan position, the chunk label signatures and the first LAB_FIRST rows of every label
+  std::vector<int> h_labels;
+  bool has_labels = false, labels_on_device = false;
+  DevBuf<int> d_labels_row, d_label_pos, d_lab_keys, d_lab_rows;
+  DevBuf<unsigned long long> d_chunk_sig;
+  int n_lab = 0;
+  // label filter of the resident batch (kv_query_set_filter; by sorted slot / by original query), only while some
+  // query is filtered
+  DevBuf<int> d_filt_sorted, d_filt_orig;
+  std::vector<int> h_filt_orig;
+  bool has_filter = false;
   // threshold search over the resident batch (kv_range_resident): its own threshold array (not d_gthr, which peers push
   // into and a top-k raises), the pair buffer, the pair count, and the result until it is fetched
   DevBuf<int> d_rthr;
@@ -383,6 +395,9 @@ int kv_index_append(kv_index *ix, const int64_t *indptr, const uint32_t *ids, co
   ix->tf.n = ix->nnz;
   ix->finalized = false;
   ix->jrange_valid = false;
+  // labels describe the rows they were given for: a filtered query fails until the rows are labelled again
+  ix->h_labels.clear();
+  ix->has_labels = ix->labels_on_device = false;
   return KV_OK;
 }
 
@@ -470,6 +485,74 @@ static int upload_idf_tables(kv_index *ix, int64_t V) {
   KV_CUDA(cudaMemcpyAsync(ix->d_d64.p, hd.data(), (size_t)V * 8, cudaMemcpyHostToDevice, ix->stream));
   KV_CUDA(cudaStreamSynchronize(ix->stream));
   return KV_OK;
+}
+
+// The device copies of the row labels for the current layout: by row (fallbacks), by scan position and as chunk
+// signatures (scan and selection), and the first LAB_FIRST rows of every label (null queries).  Nothing to do until
+// the index is finalized; every finalize calls it again.
+static int upload_labels(kv_index *ix) {
+  ix->labels_on_device = false;
+  if (!ix->has_labels || !ix->finalized) return KV_OK;
+  cudaStream_t s = ix->stream;
+  const int64_t n = ix->n_rows, n_pos = ix->n_chunks_pad * CHUNK_ROWS;
+  std::vector<int> keys(ix->h_labels);
+  std::sort(keys.begin(), keys.end());
+  keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
+  std::vector<int> first(keys.size() * LAB_FIRST, -1), cnt(keys.size(), 0);
+  for (int64_t r = 0; r < n; r++) {
+    const size_t i = (size_t)(std::lower_bound(keys.begin(), keys.end(), ix->h_labels[(size_t)r]) - keys.begin());
+    if (cnt[i] < LAB_FIRST) first[i * LAB_FIRST + (size_t)cnt[i]++] = (int)r;
+  }
+  ix->n_lab = (int)keys.size();
+  KV_CUDA(ix->d_lab_keys.ensure(std::max<int64_t>((int64_t)keys.size(), 1)));
+  KV_CUDA(ix->d_lab_rows.ensure(std::max<int64_t>((int64_t)first.size(), 1)));
+  if (!keys.empty()) {
+    KV_CUDA(cudaMemcpyAsync(ix->d_lab_keys.p, keys.data(), keys.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    KV_CUDA(cudaMemcpyAsync(ix->d_lab_rows.p, first.data(), first.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  }
+  if (n > 0) {
+    KV_CUDA(ix->d_labels_row.ensure(n));
+    KV_CUDA(ix->d_label_pos.ensure(n_pos));
+    KV_CUDA(ix->d_chunk_sig.ensure(ix->n_chunks_pad));
+    KV_CUDA(cudaMemcpyAsync(ix->d_labels_row.p, ix->h_labels.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
+    label_pos_kernel<<<(unsigned)((n_pos + 255) / 256), 256, 0, s>>>(ix->d_perm.p, ix->d_labels_row.p, n, n_pos, ix->d_label_pos.p);
+    KV_CUDA(cudaGetLastError());
+    chunk_sig_kernel<<<(unsigned)((ix->n_chunks_pad + 255) / 256), 256, 0, s>>>(ix->d_label_pos.p, ix->n_chunks_pad, ix->d_chunk_sig.p);
+    KV_CUDA(cudaGetLastError());
+  }
+  KV_CUDA(cudaStreamSynchronize(s));  // the host staging vectors go out of scope
+  ix->labels_on_device = true;
+  return KV_OK;
+}
+
+static bool labels_ready(const kv_index *ix) {
+  return ix->has_labels && ix->labels_on_device && (int64_t)ix->h_labels.size() == ix->n_rows;
+}
+
+// A filtered batch never runs on labels that do not describe the current rows
+static int check_filter(const kv_index *ix, const char *fn) {
+  if (ix->has_filter && !labels_ready(ix))
+    return kv_fail(KV_ERR_STATE, "%s: the batch is filtered but the row labels are missing or stale (set them again after an append)", fn);
+  return KV_OK;
+}
+
+int kv_index_set_row_labels(kv_index *ix, const int32_t *labels, int64_t n) {
+  if (!ix) return kv_fail(KV_ERR_INVALID, "kv_index_set_row_labels: NULL handle");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (!labels) {
+    ix->h_labels.clear();
+    ix->has_labels = ix->labels_on_device = false;
+    return KV_OK;
+  }
+  if (n != ix->n_rows)
+    return kv_fail(KV_ERR_INVALID, "kv_index_set_row_labels: %lld labels for an index of %lld rows", (long long)n,
+                   (long long)ix->n_rows);
+  for (int64_t i = 0; i < n; i++)
+    if (labels[i] < 0) return kv_fail(KV_ERR_INVALID, "kv_index_set_row_labels: label %d of row %lld is negative", labels[i], (long long)i);
+  ix->h_labels.assign(labels, labels + n);
+  ix->has_labels = true;
+  KV_CUDA(cudaSetDevice(ix->device));
+  return upload_labels(ix);
 }
 
 int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
@@ -572,7 +655,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
       ix->finalized = true;
       ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
       ix->last_finalize_kind = 2;
-      return KV_OK;
+      return upload_labels(ix);
     }
   }
   ix->layout_valid = false;
@@ -613,7 +696,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
   ix->finalized = true;
   ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
   ix->last_finalize_kind = 1;
-  return KV_OK;
+  return upload_labels(ix);
 }
 
 int kv_index_last_finalize_kind(const kv_index *ix) { return ix ? ix->last_finalize_kind : 0; }
@@ -778,7 +861,7 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
   ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
-  ix->has_excl = false;
+  ix->has_excl = ix->has_filter = false;
   ix->irr_q.clear(); ix->irr_indptr.assign(1, 0); ix->irr_ids.clear(); ix->irr_tf.clear(); ix->irr_oov.clear();
   const int T = host_threads();
   const auto t_begin = std::chrono::steady_clock::now();
@@ -993,6 +1076,7 @@ static ScanParams scan_params(const kv_index *ix, const Batch &b) {
   SP.ovf_keys = ix->d_ovf_keys.p; SP.ovf_vals = ix->d_ovf_vals.p; SP.n_ovf = ix->n_ovf;
   SP.qtab = ix->d_qtab.p; SP.q_nq = qc; SP.q_dotU = qc + b.n_q; SP.q_corrU = qc + 2 * b.n_q;
   SP.q_excl = ix->has_excl ? ix->d_excl_sorted.p : nullptr; SP.gthr = b.range ? ix->d_rthr.p : ix->d_gthr.p;
+  if (ix->has_filter) { SP.q_label = ix->d_filt_sorted.p; SP.label_pos = ix->d_label_pos.p; SP.chunk_sig = ix->d_chunk_sig.p; }
   for (int i = 0; i < 7; i++) SP.peer_gthr[i] = i < b.n_peers ? ix->peer_gthr[i] : nullptr;
   SP.n_peers = b.n_peers; SP.stats = ix->d_stats.p; SP.n_q = b.n_q; SP.k = b.k;
   SP.part_scores = ix->d_part_s.p; SP.part_rows = ix->d_part_r.p; SP.max_pages = b.max_pages;
@@ -1071,7 +1155,11 @@ static int run_pruned(kv_index *ix, Batch &b) {
     SelectParams LP;
     LP.ubq = ix->d_ubq.p; LP.ubq_stride = ix->n_chunks_pad; LP.n_chunks = ix->n_chunks; LP.n_q = n_q;
     LP.q_nq = qc; LP.gthr = ix->d_gthr.p; LP.n_bsplits = (int)b.n_bsplits; LP.lists = BP.lists; LP.stats = BP.stats;
-    tfidf_select_kernel<<<dim3((unsigned)b.n_groups, (unsigned)b.n_bsplits), SEL_WARPS * 32, (size_t)b.max_pages * sizeof(int), s>>>(LP);
+    LP.q_label = ix->d_filt_sorted.p; LP.chunk_sig = ix->d_chunk_sig.p;
+    const dim3 sgrid((unsigned)b.n_groups, (unsigned)b.n_bsplits);
+    const size_t s_smem = (size_t)b.max_pages * sizeof(int);
+    if (ix->has_filter) tfidf_select_kernel<true><<<sgrid, SEL_WARPS * 32, s_smem, s>>>(LP);
+    else tfidf_select_kernel<false><<<sgrid, SEL_WARPS * 32, s_smem, s>>>(LP);
   } else {
     BP.pass = 1;
     tfidf_bound_kernel<false><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_w2, ix->map_u, BP);
@@ -1169,12 +1257,17 @@ static int size_batch(kv_index *ix, Batch &b) {
 static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, int phase = 0) {
   if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_topk_resident: no query batch uploaded");
   if (k < 1 || k > 32) return kv_fail(KV_ERR_INVALID, "kv_topk: k must be 1..32");
+  int rc = check_filter(ix, "kv_topk");
+  if (rc != KV_OK) return rc;
+  // the thresholds peers push are those of unfiltered queries: not a bound of a filtered query's k-th score
+  if (ix->has_filter && (ix->gthr_exported || ix->n_peers))
+    return kv_fail(KV_ERR_INVALID, "kv_topk: a label filter cannot be combined with the threshold exchange of a row-sharded GFKB");
   ix->jrange_valid = false;
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
   Batch b;
   b.k = k; b.phase = phase; b.out_s = d_out_s; b.out_r = d_out_r;
-  int rc = size_batch(ix, b);
+  rc = size_batch(ix, b);
   if (rc != KV_OK) return rc;
   const int64_t n_q = b.n_q;
   const bool prune = b.prune;
@@ -1246,9 +1339,12 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
   b.launches++;
   // queries no path scanned: null queries score 0 against every row, irregular ones take the float64 full scan
   if (ix->batch_null) {
+    const LabelFirstRows L{ix->d_lab_keys.p, ix->d_lab_rows.p, ix->n_lab};
     fill_null_kernel<<<(unsigned)((ix->batch_null * k + 255) / 256), 256, 0, s>>>(ix->d_qperm.p + n_q, (int)ix->batch_null, k,
                                                                                   ix->n_rows, ix->row_base,
-                                                                                  ix->has_excl ? ix->d_excl_orig.p : nullptr, d_out_s, d_out_r);
+                                                                                  ix->has_excl ? ix->d_excl_orig.p : nullptr,
+                                                                                  ix->has_filter ? ix->d_filt_orig.p : nullptr, L,
+                                                                                  d_out_s, d_out_r);
     KV_CUDA(cudaGetLastError());
     b.launches++;
   }
@@ -1257,7 +1353,8 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
     rc = score_impl(ix, ix->irr_ids.data() + a, ix->irr_tf.data() + a, e - a, ix->irr_oov[i], nullptr);
     if (rc != KV_OK) return rc;
     select_topk_kernel<<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
-                                          ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, d_out_s + q * k, d_out_r + q * k);
+                                          ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->d_labels_row.p,
+                                          ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, d_out_s + q * k, d_out_r + q * k);
     KV_CUDA(cudaGetLastError());
     b.launches += 2;
   }
@@ -1295,12 +1392,14 @@ static int finish_batch(kv_index *ix) {
 static int run_range(kv_index *ix, float thr, int64_t *n_pairs, const char *fn) {
   ix->range_valid = ix->jrange_valid = false;
   if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "%s: no query batch uploaded", fn);
+  int rc = check_filter(ix, fn);
+  if (rc != KV_OK) return rc;
   const bool jac = ix->jaccard != 0;
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
   Batch b;
   b.k = 0; b.phase = 2; b.out_s = nullptr; b.out_r = nullptr; b.range = true; b.use_codes = false; b.n_peers = 0;
-  int rc = size_batch(ix, b);  // a Jaccard index never prunes
+  rc = size_batch(ix, b);  // a Jaccard index never prunes
   if (rc != KV_OK) return rc;
   const int64_t n_q = b.n_q;
   KV_CUDA(ix->d_rthr.ensure(n_q));
@@ -1341,7 +1440,8 @@ static int run_range(kv_index *ix, float thr, int64_t *n_pairs, const char *fn) 
           jaccard_select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->d_B64.p, ix->d_invperm.p, ix->n_rows, nq, thr, excl,
                                                            (int)q, ix->d_jrange.p, ix->d_range_count.p, range_cap());
         } else {
-          select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, thr, excl, (int)q, ix->d_range.p,
+          select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, thr, excl, ix->d_labels_row.p,
+                                                   ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, (int)q, ix->d_range.p,
                                                    ix->d_range_count.p, range_cap());
         }
         KV_CUDA(cudaGetLastError());
@@ -1575,6 +1675,35 @@ static int set_exclusions_locked(kv_index *ix, const int64_t *exclude_rows, int6
   KV_CUDA(cudaMemcpyAsync(ix->d_excl_orig.p, ix->h_excl_orig.data(), (size_t)n_q * sizeof(int), cudaMemcpyHostToDevice, ix->stream));
   KV_CUDA(cudaStreamSynchronize(ix->stream));
   ix->has_excl = true;
+  return KV_OK;
+}
+
+int kv_query_set_filter(kv_index *ix, const int32_t *labels, int64_t n_q) {
+  if (!ix) return kv_fail(KV_ERR_INVALID, "kv_query_set_filter: NULL handle");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (labels && ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_query_set_filter: a Jaccard index (mode 1) has no label filter");
+  if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_query_set_filter: no query batch uploaded");
+  if (!labels) { ix->has_filter = false; return KV_OK; }
+  if (n_q != ix->batch_q) return kv_fail(KV_ERR_INVALID, "kv_query_set_filter: %lld labels for a batch of %lld queries",
+                                         (long long)n_q, (long long)ix->batch_q);
+  bool any = false;
+  for (int64_t q = 0; q < n_q; q++) {
+    if (labels[q] < -1) return kv_fail(KV_ERR_INVALID, "kv_query_set_filter: label %d of query %lld is below -1", labels[q], (long long)q);
+    any = any || labels[q] >= 0;
+  }
+  ix->has_filter = false;
+  if (!any) return KV_OK;  // every query unfiltered: the unfiltered batch
+  if (!labels_ready(ix))
+    return kv_fail(KV_ERR_STATE, "kv_query_set_filter: the index has no row labels for its current rows (kv_index_set_row_labels)");
+  KV_CUDA(cudaSetDevice(ix->device));
+  ix->h_filt_orig.assign(labels, labels + n_q);
+  std::vector<int> sorted((size_t)n_q);
+  for (int64_t i = 0; i < n_q; i++) sorted[(size_t)i] = ix->h_filt_orig[(size_t)ix->h_qperm.p[i]];
+  KV_CUDA(ix->d_filt_sorted.ensure(n_q)); KV_CUDA(ix->d_filt_orig.ensure(n_q));
+  KV_CUDA(cudaMemcpyAsync(ix->d_filt_sorted.p, sorted.data(), (size_t)n_q * sizeof(int), cudaMemcpyHostToDevice, ix->stream));
+  KV_CUDA(cudaMemcpyAsync(ix->d_filt_orig.p, ix->h_filt_orig.data(), (size_t)n_q * sizeof(int), cudaMemcpyHostToDevice, ix->stream));
+  KV_CUDA(cudaStreamSynchronize(ix->stream));
+  ix->has_filter = true;
   return KV_OK;
 }
 
@@ -1967,5 +2096,6 @@ extern "C" int kv_index_layout_load(kv_index *ix, const char *path) {
   int rc = upload_layout(ix, SL);
   if (rc != KV_OK) return rc;
   ix->finalized = false;
+  ix->labels_on_device = false;  // positions changed: the finalize that follows rebuilds them
   return KV_OK;
 }

@@ -169,6 +169,27 @@ __global__ void invperm_kernel(const int *__restrict__ perm, int64_t n, int *inv
   if (pos < n) invperm[perm[pos]] = (int)pos;
 }
 
+// Row labels in scan order (kv_index_set_row_labels): label_pos[pos] = label of the row at position pos, -1 past the
+// last row (label_pos holds n_chunks_pad * 32 entries)
+__global__ void label_pos_kernel(const int *__restrict__ perm, const int *__restrict__ labels, int64_t n_rows, int64_t n_pos,
+                                 int *label_pos) {
+  const int64_t pos = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (pos < n_pos) label_pos[pos] = pos < n_rows ? labels[perm[pos]] : -1;
+}
+
+// chunk label signature: bit (label & 63) of every label a row of the chunk carries.  No false negatives, so a chunk
+// whose signature lacks a query's bit holds no row of that query's label.
+__global__ void chunk_sig_kernel(const int *__restrict__ label_pos, int64_t n_chunks_pad, unsigned long long *sig) {
+  const int64_t c = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (c >= n_chunks_pad) return;
+  unsigned long long m = 0;
+  for (int i = 0; i < CHUNK_ROWS; i++) {
+    const int l = label_pos[c * CHUNK_ROWS + i];
+    if (l >= 0) m |= 1ull << (l & 63);
+  }
+  sig[c] = m;
+}
+
 // ----------------------------------------------------------------------------------------
 // device helpers
 // ----------------------------------------------------------------------------------------
@@ -529,6 +550,10 @@ struct ScanParams {
   const unsigned char *qtab;              // [n_q][QTAB_BYTES]
   const float *q_nq, *q_dotU, *q_corrU;   // [n_q] (sorted query order)
   const int *q_excl;                      // [n_q] or NULL: local ORIGINAL row a query must not match (self-join), -1 = none
+  // label filter (kv_query_set_filter); q_label NULL: the batch has none and the other two are not read
+  const int *q_label;                     // [n_q] label a query's rows must carry, -1 = any
+  const int *label_pos;                   // [n_chunks_pad * 32] row label by scan position
+  const unsigned long long *chunk_sig;    // [n_chunks_pad] chunk label signatures
   int *gthr;                              // [n_q] float bits: lower bound of the global k-th score
   int *peer_gthr[7];                      // the same array on the other GPUs of a row-sharded GFKB (peer memory over
   int n_peers;                            //   NVLink): a raised bound is pushed to every shard, so all of them prune with it
@@ -600,7 +625,8 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   float *s_nq = (float *)(s_lock + GROUP_Q);                                // [GROUP_Q] per-query constants
   float *s_dotU = s_nq + GROUP_Q, *s_corrU = s_dotU + GROUP_Q;
   int *s_excl = (int *)(s_corrU + GROUP_Q);
-  unsigned int *s_next = (unsigned int *)(s_excl + GROUP_Q);                // [1] next record of this CTA's range
+  int *s_qlab = s_excl + GROUP_Q;                                           // [GROUP_Q] label filter, -1 = any
+  unsigned int *s_next = (unsigned int *)(s_qlab + GROUP_Q);                // [1] next record of this CTA's range
   unsigned int *s_stat = s_next + 1;                                        // [2]
 
   const int list = blockIdx.x, ssplit = blockIdx.y;
@@ -644,6 +670,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
       s_dotU[qi] = ok ? P.q_dotU[q0 + qi] : 0.f;
       s_corrU[qi] = ok ? P.q_corrU[q0 + qi] : 0.f;
       s_excl[qi] = (ok && P.q_excl) ? P.q_excl[q0 + qi] : -1;
+      s_qlab[qi] = (ok && P.q_label) ? P.q_label[q0 + qi] : -1;
     }
     if (threadIdx.x == 0) { *s_next = r_lo; s_stat[0] = s_stat[1] = 0; }
     if (lane == 0) {
@@ -678,6 +705,11 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
       else rec = P.pool[(size_t)P.list_pages[(size_t)list * P.max_pages + (r / PAGE_RECS)] * PAGE_RECS + (r % PAGE_RECS)];
       chunk = rec.x;
       mask = rec.y;
+    }
+    if (P.q_label) {  // drop the filtered queries whose label no row of the chunk carries: an emptied record is never staged
+      const unsigned long long sig = P.chunk_sig[chunk];
+      const int lb = s_qlab[lane];
+      mask &= __ballot_sync(FULL, lb < 0 || ((sig >> (lb & 63)) & 1ull));
     }
   };
   auto grab = [&]() -> uint32_t {
@@ -735,11 +767,14 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
       const int rows = (int)min((int64_t)CHUNK_ROWS, P.n_rows - pos0);
       const uint32_t valid = rows == 32 ? FULL : ((1u << rows) - 1u);
       const float Bc = lane < rows ? P.B32[pos0 + lane] : 0.f;
+      const int lpos = P.q_label ? P.label_pos[pos0 + lane] : -1;  // one 128-byte line per record
       recs_done++;
       for (uint32_t qm = mask_cur; qm; qm &= qm - 1) {
         const int qi = __ffs(qm) - 1;
         const float nq = s_nq[qi];
         if (!(nq > 0.f)) continue;  // null / irregular query: answered elsewhere
+        const int ql = s_qlab[qi];
+        if (ql >= 0 && __ballot_sync(FULL, lpos == ql) == 0) continue;  // signature collision: no row of the label here
         pairs_done++;
         const uint32_t *keys = s_keys + qi * QKEYS;
         const QFeat *feats = s_feats + qi * QFEATS;
@@ -810,7 +845,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
             const float den = nq * t;
             sc = den > 0.f ? __fdiv_rn(dot, __fsqrt_rn(den)) : 0.f;
             row = P.perm[pos0 + lane];
-            cand = row != s_excl[qi] && sc >= filt;
+            cand = row != s_excl[qi] && sc >= filt && (ql < 0 || lpos == ql);
           }
         }
         if constexpr (RANGE) {
@@ -885,7 +920,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
 
 static inline size_t scan_smem_bytes(int k) {
   return (size_t)GROUP_Q * QTAB_BYTES + (size_t)S_WARPS * 2 * S_BUF_BYTES + (size_t)S_WARPS * 32 * sizeof(ScanHit) +
-         (size_t)S_WARPS * 2 * 8 + (size_t)GROUP_Q * k * 8 + (size_t)GROUP_Q * 4 * 6 + 16;
+         (size_t)S_WARPS * 2 * 8 + (size_t)GROUP_Q * k * 8 + (size_t)GROUP_Q * 4 * 7 + 16;
 }
 
 // ----------------------------------------------------------------------------------------
@@ -1256,22 +1291,53 @@ __global__ void merge_topk_kernel(const float *__restrict__ in_s, const long lon
   }
 }
 
+constexpr int LAB_FIRST = 33;  // smallest rows kept per label: k <= 32 of them plus one a self-join excludes
+
+// The rows of each label in ascending order, first LAB_FIRST of them (kv_index_set_row_labels): keys[n_lab] sorted,
+// rows[n_lab][LAB_FIRST] local rows, -1 past the label's last row
+struct LabelFirstRows {
+  const int *keys, *rows;
+  int n_lab;
+};
+
 // Null queries (no feature in common with any row: every score is 0): the stable sort keeps the
-// first k rows.  One thread per (query, slot).
+// first k rows -- of the query's label when it is filtered (label_by_query: by ORIGINAL query, NULL: no filter).
+// One thread per (query, slot).
 __global__ void fill_null_kernel(const int *__restrict__ null_q, int n_null, int k, int64_t n_rows, int64_t row_base,
-                                 const int *__restrict__ excl_by_query, float *out_s, long long *out_r) {
+                                 const int *__restrict__ excl_by_query, const int *__restrict__ label_by_query,
+                                 LabelFirstRows L, float *out_s, long long *out_r) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_null * k) return;
   int q = null_q[i / k], j = i % k;
   const int ex = excl_by_query ? excl_by_query[q] : -1;  // by ORIGINAL query index
+  const int lb = label_by_query ? label_by_query[q] : -1;
+  if (lb >= 0) {
+    int lo = 0, hi = L.n_lab - 1, idx = -1;
+    while (lo <= hi) {
+      const int mid = (lo + hi) >> 1;
+      if (L.keys[mid] == lb) { idx = mid; break; }
+      if (L.keys[mid] < lb) lo = mid + 1; else hi = mid - 1;
+    }
+    int r = -1;
+    for (int t = 0, seen = 0; idx >= 0 && t < LAB_FIRST; t++) {  // the j-th row of the label once the excluded one is skipped
+      const int x = L.rows[(size_t)idx * LAB_FIRST + t];
+      if (x < 0) break;
+      if (x == ex) continue;
+      if (seen++ == j) { r = x; break; }
+    }
+    out_s[(size_t)q * k + j] = r >= 0 ? 0.f : -INFINITY;
+    out_r[(size_t)q * k + j] = r >= 0 ? row_base + r : -1LL;
+    return;
+  }
   const int64_t r = (ex >= 0 && j >= ex) ? j + 1 : j;     // the j-th row once the excluded one is skipped
   out_s[(size_t)q * k + j] = r < n_rows ? 0.f : -INFINITY;
   out_r[(size_t)q * k + j] = r < n_rows ? row_base + r : -1LL;
 }
 
-// Fallback selection for one (irregular) query: k passes of block-wide arg-best over float64 scores.
+// Fallback selection for one (irregular) query: k passes of block-wide arg-best over float64 scores.  lab >= 0: only
+// rows with labels[row] == lab (by original row) compete.
 __global__ void select_topk_kernel(const double *__restrict__ scores, int64_t n, int64_t row_base, int k, int64_t excl,
-                                   float *out_s, long long *out_r) {
+                                   const int *__restrict__ labels, int lab, float *out_s, long long *out_r) {
   __shared__ float s_s[32];
   __shared__ long long s_r[32];
   __shared__ float prev_s;
@@ -1284,7 +1350,7 @@ __global__ void select_topk_kernel(const double *__restrict__ scores, int64_t n,
     const float ps = prev_s;
     const long long pr = prev_r;
     for (int64_t r = threadIdx.x; r < n; r += blockDim.x) {
-      if (r == excl) continue;
+      if (r == excl || (lab >= 0 && labels[r] != lab)) continue;
       float s = (float)scores[r];
       bool after = (s < ps) || (s == ps && r > pr);  // strictly after the previously selected pair
       if (after && (br < 0 || s > bs || (s == bs && r < br))) { bs = s; br = r; }
@@ -1316,16 +1382,17 @@ __global__ void select_topk_kernel(const double *__restrict__ scores, int64_t n,
 }
 
 // Fallback of a threshold search for one (irregular) query: every row whose float64 score, rounded to the float32
-// select_topk_kernel reports, reaches the threshold is appended to the pair buffer.
+// select_topk_kernel reports, reaches the threshold is appended to the pair buffer (lab >= 0: rows of that label only).
 __global__ void select_range_kernel(const double *__restrict__ scores, int64_t n, int64_t row_base, float thr, int64_t excl,
-                                    int q, RangePair *out, unsigned long long *count, unsigned long long cap) {
+                                    const int *__restrict__ labels, int lab, int q, RangePair *out, unsigned long long *count,
+                                    unsigned long long cap) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   const int qv = q;
   // whole warps step together (blockDim is a multiple of 32): range_emit needs every lane
   for (int64_t r0 = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) & ~31LL; r0 < n; r0 += stride) {
     const int64_t r = r0 + (threadIdx.x & 31);
     const float s = r < n ? (float)scores[r] : -INFINITY;
-    range_emit(out, count, cap, r < n && r != excl && s >= thr, &qv, s, row_base + r);
+    range_emit(out, count, cap, r < n && r != excl && (lab < 0 || labels[r] == lab) && s >= thr, &qv, s, row_base + r);
   }
 }
 

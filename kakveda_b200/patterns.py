@@ -76,7 +76,8 @@ def pattern_payload(name: str, records: Sequence[Mapping[str, Any]], description
 
 
 def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: float = 0.8, k: Optional[int] = 32,
-                    min_apps: int = 2, failure_type: Optional[str] = None) -> List[Dict[str, Any]]:
+                    min_apps: int = 2, failure_type: Optional[str] = None,
+                    filter_first: bool = False) -> List[Dict[str, Any]]:
     """Similarity-split version of pattern_detector.on_failure.
 
     ``index``: a finalized ``GfkbIndex`` whose row i is ``records[i]['signature_text']`` (corpus-fit mode gives a
@@ -87,13 +88,31 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
     ``k``: rows are linked only through every row's k nearest other rows, so when a text is stored more than k times
     its copies fill the lists and pairs of similar texts are never seen.  ``k=None`` links on the exact threshold
     graph (``selfjoin_range``).
+    ``filter_first`` (with ``failure_type``, ``GfkbIndex`` only): the index's row labels are set to the records' failure
+    types and the self-join searches every row among the rows of its own type, so with an integer ``k`` other types
+    cannot fill a row's list and hide its same-type neighbours.  With ``k=None`` the components are the default's.
     """
     n = len(records)
     keep = np.ones(n, dtype=bool)
     if failure_type is not None:
         keep = np.fromiter((r.get("failure_type") == failure_type for r in records), dtype=bool, count=n)
+    if filter_first and failure_type is not None:
+        from .similarity import GfkbIndex
+
+        if not isinstance(index, GfkbIndex):
+            raise NotImplementedError("detect_patterns(filter_first=True) searches by label on a GfkbIndex only")
+        types: Dict[Any, int] = {}
+        index.set_row_labels(np.fromiter((types.setdefault(r.get("failure_type"), len(types)) for r in records),
+                                         dtype=np.int32, count=n))
+        if k is None:
+            indptr, rows = index.selfjoin_range(threshold, device_out=True, same_label=True)[:2]
+            labels, _ = cluster_csr(indptr, rows)
+            labels = labels.cpu().numpy()
+        else:
+            scores, rows = index.selfjoin_topk(k, same_label=True)
+            labels, _ = cluster_topk(rows, scores, threshold)
     # a JaccardIndex returns the exact counts after these arrays: only the leading ones are used
-    if k is None:
+    elif k is None:
         # the threshold graph stays on the device: only the n labels come back
         import torch
 

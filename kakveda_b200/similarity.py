@@ -205,6 +205,7 @@ class GfkbIndex:
         self._h = h
         self.device = device
         self.row_base = row_base
+        self._row_labels: Optional[np.ndarray] = None  # what set_row_labels gave, until the next append
 
     # -- build ---------------------------------------------------------------------------
     def add_features(self, fb: FeatureBatch, lo: int = 0, hi: Optional[int] = None) -> None:
@@ -214,6 +215,19 @@ class GfkbIndex:
         ip = np.ascontiguousarray(fb.indptr[lo:hi + 1])
         _capi.check(_capi.load().kv_index_append(self._h, _ptr(ip, C.c_int64), _ptr(fb.ids, C.c_uint32),
                                                  _ptr(fb.tf, C.c_uint32), hi - lo))
+        self._row_labels = None  # the library drops the labels on an append
+
+    def set_row_labels(self, labels: Optional[np.ndarray]) -> None:
+        """One label >= 0 per local row (e.g. a failure-type id), for the ``labels`` / ``same_label`` filters of the
+        query methods; ``None`` clears.  Survives finalize; an append drops the labels (a filtered query then raises
+        until they are set again)."""
+        if labels is None:
+            _capi.check(_capi.load().kv_index_set_row_labels(self._h, None, 0))
+            self._row_labels = None
+            return
+        labels = np.ascontiguousarray(labels, dtype=np.int32)
+        _capi.check(_capi.load().kv_index_set_row_labels(self._h, _ptr(labels, C.c_int32), len(labels)))
+        self._row_labels = labels.copy()
 
     def add_texts(self, texts: Sequence[str]) -> None:
         fb = self.vocab.featurize(texts, grow=True)
@@ -266,7 +280,14 @@ class GfkbIndex:
         finally:
             fb.close()
 
-    def topk_features(self, fb: FeatureBatch, k: int) -> Tuple[np.ndarray, np.ndarray]:
+    def topk_features(self, fb: FeatureBatch, k: int, labels: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """``labels``: per query the row label its results must carry (-1: any row), see ``set_filter``."""
+        if labels is not None:
+            if fb.n == 0:
+                return np.zeros((0, k), np.float32), np.zeros((0, k), np.int64)
+            self.upload_queries(fb)
+            self.set_filter(labels)
+            return self.topk_resident_host(fb.n, k)
         scores = np.empty((fb.n, k), dtype=np.float32)
         rows = np.empty((fb.n, k), dtype=np.int64)
         _capi.check(_capi.load().kv_topk(self._h, _ptr(fb.indptr, C.c_int64), _ptr(fb.ids, C.c_uint32),
@@ -340,6 +361,16 @@ class GfkbIndex:
         rows = np.ascontiguousarray(rows, dtype=np.int64)
         _capi.check(_capi.load().kv_query_set_exclusions(self._h, _ptr(rows, C.c_int64), len(rows)))
 
+    def set_filter(self, labels: Optional[np.ndarray]) -> None:
+        """Query q of the resident batch only matches rows labelled ``labels[q]`` (-1 = any row; ``set_row_labels``);
+        ``None`` clears, and so does the next upload.  The index statistics are not changed: the scores are the
+        unfiltered ones."""
+        if labels is None:
+            _capi.check(_capi.load().kv_query_set_filter(self._h, None, 0))
+            return
+        labels = np.ascontiguousarray(labels, dtype=np.int32)
+        _capi.check(_capi.load().kv_query_set_filter(self._h, _ptr(labels, C.c_int32), len(labels)))
+
     def topk_resident_host(self, n_q: int, k: int) -> Tuple[np.ndarray, np.ndarray]:
         """Scan + merge of the resident batch of ``n_q`` queries, results copied to the host."""
         scores = np.empty((n_q, k), dtype=np.float32)
@@ -347,12 +378,21 @@ class GfkbIndex:
         _capi.check(_capi.load().kv_topk_resident_host(self._h, k, _ptr(scores, C.c_float), _ptr(rows, C.c_int64)))
         return scores, rows
 
-    def selfjoin_topk(self, k: int, lo: int = 0, hi: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray]:
-        """All-pairs: for local rows [lo, hi) the k best OTHER rows (the row itself is excluded)."""
+    def _selfjoin_upload(self, lo: int, hi: int, same_label: bool) -> None:
+        _capi.check(_capi.load().kv_selfjoin_upload(self._h, lo, hi))
+        if same_label:
+            if self._row_labels is None or len(self._row_labels) != self.n_rows:
+                raise RuntimeError("same_label: the index has no row labels for its current rows (set_row_labels)")
+            self.set_filter(self._row_labels[lo:hi])
+
+    def selfjoin_topk(self, k: int, lo: int = 0, hi: Optional[int] = None,
+                      same_label: bool = False) -> Tuple[np.ndarray, np.ndarray]:
+        """All-pairs: for local rows [lo, hi) the k best OTHER rows (the row itself is excluded).  ``same_label``:
+        row i's list holds only rows with row i's label."""
         hi = self.n_rows if hi is None else hi
         if hi <= lo:
             return np.zeros((0, k), np.float32), np.zeros((0, k), np.int64)
-        _capi.check(_capi.load().kv_selfjoin_upload(self._h, lo, hi))
+        self._selfjoin_upload(lo, hi, same_label)
         return self.topk_resident_host(hi - lo, k)
 
     def _range_resident(self, n_q: int, threshold: float, device_out: bool = False):
@@ -374,31 +414,37 @@ class GfkbIndex:
             return _devout.empty_range(self.device)
         return np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32)
 
-    def range_features(self, fb: FeatureBatch, threshold: float, device_out: bool = False):
+    def range_features(self, fb: FeatureBatch, threshold: float, device_out: bool = False,
+                       labels: Optional[np.ndarray] = None):
         """Threshold search: every (query, row) pair whose float32 score (the value ``topk`` reports) is >= ``threshold``,
         0 < threshold <= 1.  Returns ``(indptr int64[n_q+1], rows int64[P], scores float32[P])``: query q's pairs are
         ``[indptr[q], indptr[q+1])``, ordered by (score desc, row asc); rows are global.  ``device_out``: the same
-        arrays as torch tensors on the index's device (nothing is copied to the host)."""
+        arrays as torch tensors on the index's device (nothing is copied to the host).  ``labels``: per query the row
+        label its pairs must carry (-1: any row), see ``set_filter``."""
         if fb.n == 0:
             return self._empty_range(device_out)
         self.upload_queries(fb)
+        if labels is not None:
+            self.set_filter(labels)
         return self._range_resident(fb.n, threshold, device_out)
 
-    def range(self, queries: Sequence[str], threshold: float, device_out: bool = False):
+    def range(self, queries: Sequence[str], threshold: float, device_out: bool = False,
+              labels: Optional[np.ndarray] = None):
         """``range_features`` of texts."""
         fb = self.vocab.featurize(queries, grow=False)
         try:
-            return self.range_features(fb, threshold, device_out)
+            return self.range_features(fb, threshold, device_out, labels)
         finally:
             fb.close()
 
-    def selfjoin_range(self, threshold: float, lo: int = 0, hi: Optional[int] = None, device_out: bool = False):
+    def selfjoin_range(self, threshold: float, lo: int = 0, hi: Optional[int] = None, device_out: bool = False,
+                       same_label: bool = False):
         """All-pairs threshold search: for local rows [lo, hi) every OTHER row scoring >= ``threshold`` (CSR as in
-        ``range_features``, query i = row lo + i)."""
+        ``range_features``, query i = row lo + i).  ``same_label``: only rows with row i's label."""
         hi = self.n_rows if hi is None else hi
         if hi <= lo:
             return self._empty_range(device_out)
-        _capi.check(_capi.load().kv_selfjoin_upload(self._h, lo, hi))
+        self._selfjoin_upload(lo, hi, same_label)
         return self._range_resident(hi - lo, threshold, device_out)
 
     def rescore(self, fb: FeatureBatch, rows: np.ndarray) -> np.ndarray:
@@ -427,11 +473,12 @@ class GfkbIndex:
         """Phase 2 of a sharded step: candidate selection + scan + merge of the resident batch."""
         _capi.check(_capi.load().kv_topk_resident_finish(self._h, k, C.c_void_p(d_scores_ptr), C.c_void_p(d_rows_ptr)))
 
-    def topk(self, queries: Sequence[str], k: int) -> Tuple[np.ndarray, np.ndarray]:
-        """(scores float32 [Q,k], rows int64 [Q,k]) ordered by (score desc, row asc) (K1b+K5)."""
+    def topk(self, queries: Sequence[str], k: int, labels: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """(scores float32 [Q,k], rows int64 [Q,k]) ordered by (score desc, row asc) (K1b+K5).  ``labels``: per query
+        the row label its results must carry (-1: any row)."""
         fb = self.vocab.featurize(queries, grow=False)
         try:
-            return self.topk_features(fb, k)
+            return self.topk_features(fb, k, labels)
         finally:
             fb.close()
 

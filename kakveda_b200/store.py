@@ -118,6 +118,9 @@ class GfkbStore:
         self._n_indexed = 0       # records[:_n_indexed] are on the device (main + tail)
         self._main_df: Optional[np.ndarray] = None
         self._dirty = False
+        # failure_type -> row label of the device index, numbered in order of first appearance; label of each record
+        self._type_ids: Dict[str, int] = {}
+        self._labels: List[int] = []
         self.stats = {"full_rebuilds": 0, "stat_refreshes": 0, "compactions": 0, "quarantined": 0}
         self.quarantined: List[int] = []  # indices of loaded records that cannot be indexed (they keep their row, with no features)
         if self.path is not None and self.path.exists():
@@ -147,7 +150,14 @@ class GfkbStore:
         self._latest = {}
         for i, r in enumerate(self.records):
             self._latest[(r["failure_type"], r["signature_text"])] = i
+        self._type_ids, self._labels = {}, []
         self._rebuild_main()
+
+    def _row_labels(self, lo: int, hi: int) -> np.ndarray:
+        """int32 row labels of records[lo:hi]: their failure types, numbered in order of first appearance."""
+        for r in self.records[len(self._labels):hi]:
+            self._labels.append(self._type_ids.setdefault(r["failure_type"], len(self._type_ids)))
+        return np.asarray(self._labels[lo:hi], dtype=np.int32)
 
     def _rebuild_main(self) -> None:
         for ix in (self._main, self._tail):
@@ -195,6 +205,7 @@ class GfkbStore:
                 self.stats["layout_restored"] = self.stats.get("layout_restored", 0) + 1
             elif lay_path is not None:
                 self._main.save_layout(lay_path)
+            self._main.set_row_labels(self._row_labels(0, n))
             self.stats["full_rebuilds"] += 1
         self._n_main = self._n_indexed = n
         self._dirty = False
@@ -213,6 +224,7 @@ class GfkbStore:
             self._tail = GfkbIndex(device=self.device, row_base=self._n_main, vocab=self.vocab)
         if pending:
             self._tail.add_texts(pending)
+        self._tail.set_row_labels(self._row_labels(self._n_main, len(self.records)))  # an append dropped them
         self._n_indexed = len(self.records)
         # global statistics = main + tail (the df all-reduce of a sharded GFKB, done in-process)
         v = len(self.vocab)
@@ -276,15 +288,18 @@ class GfkbStore:
             return {"ok": True, "created": created, "failure": rec}
 
     # -- match (services/gfkb/app.py:79-102) -------------------------------------------------------------------
-    def _candidates(self, fb: FeatureBatch, k: int, limit: int = MATCH_LIMIT) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    def _candidates(self, fb: FeatureBatch, k: int, limit: int = MATCH_LIMIT,
+                    labels: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
         """Per query: candidate rows from both segments with their float64 scores, ordered (score desc, row asc), and
-        whether the candidate stage may have missed a top-``limit`` row (``ambiguous_candidates``)."""
+        whether the candidate stage may have missed a top-``limit`` row (``ambiguous_candidates``).  ``labels``: per
+        query the failure-type label its candidates must carry (-1: any)."""
         rows_all, f64_all = [], []
         amb = np.zeros(fb.n, dtype=bool)
         for ix in (self._main, self._tail):
             if ix is None or ix.n_rows == 0:
                 continue
-            s32, rows = ix.topk_features(fb, min(k, MAX_LIMIT))
+            kk = min(k, MAX_LIMIT)
+            s32, rows = ix.topk_features(fb, kk) if labels is None else ix.topk_features(fb, kk, labels)
             amb |= ambiguous_candidates(s32, rows, limit)
             rows_all.append(rows)
             f64_all.append(ix.rescore(fb, rows))
@@ -294,22 +309,54 @@ class GfkbStore:
         order = np.lexsort((big, -f64), axis=1)  # last key is primary: score descending, then row ascending
         return np.take_along_axis(rows, order, axis=1), np.take_along_axis(f64, order, axis=1), amb
 
-    def _exact_top(self, signature_text: str, limit: int) -> Tuple[List[int], List[float]]:
+    def _exact_top(self, signature_text: str, limit: int, label: int = -1) -> Tuple[List[int], List[float]]:
         """Rows and float64 scores of the reference's ``sorted(..., reverse=True)[:limit]`` on the full score vector
-        (K1a on both segments): no candidate stage at all."""
+        (K1a on both segments): no candidate stage at all.  ``label`` >= 0: over the rows of that failure-type label."""
         parts = [ix.score(signature_text) for ix in (self._main, self._tail) if ix is not None and ix.n_rows]
         scores = np.concatenate(parts)
-        order = stable_top(scores, limit)
+        if label >= 0:
+            idx = np.flatnonzero(self._row_labels(0, len(scores)) == label)  # ascending: the stable order is kept
+            order = idx[stable_top(scores[idx], limit)].tolist()
+        else:
+            order = stable_top(scores, limit)
         return order, [float(scores[i]) for i in order]
 
+    def _match_filter_first(self, signature_texts: Sequence[str], failure_types: Sequence[Optional[str]],
+                            limit: int) -> List[List[dict]]:
+        """The best ``limit`` rows OF each query's failure type (all rows for a query without one)."""
+        self._row_labels(0, len(self.records))  # number every stored type
+        labels = np.array([-1 if not ft else self._type_ids.get(ft, -2) for ft in failure_types], dtype=np.int32)
+        out: List[List[dict]] = [[] for _ in signature_texts]
+        scan = np.flatnonzero(labels != -2)  # a type no stored row has: no match, and nothing to scan
+        if len(scan) == 0:
+            return out
+        fb = self.vocab.featurize([signature_texts[i] for i in scan], grow=False)
+        try:
+            rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit, labels[scan])
+        finally:
+            fb.close()
+        for j, i in enumerate(scan.tolist()):
+            if amb[j]:
+                top_r, top_s = self._exact_top(signature_texts[i], limit, int(labels[i]))
+                self.stats["exact_fallbacks"] = self.stats.get("exact_fallbacks", 0) + 1
+            else:
+                top_r, top_s = rows[j, :limit].tolist(), f64[j, :limit].tolist()
+            out[i] = [_to_match(self.records[r], s) for r, s in zip(top_r, top_s) if r >= 0]
+        return out
+
     def match_batch(self, signature_texts: Sequence[str], failure_types: Optional[Sequence[Optional[str]]] = None,
-                    limit: int = MATCH_LIMIT) -> List[List[dict]]:
+                    limit: int = MATCH_LIMIT, filter_first: bool = False) -> List[List[dict]]:
+        """``filter_first=False`` (default): the reference's handler -- the best ``limit`` rows, THEN the failure_type
+        filter, so rows of other types can leave fewer than ``limit`` (or no) matches.  ``filter_first=True``: the best
+        ``limit`` rows of the query's failure_type, searched on the device among that type's rows only."""
         if limit > MAX_LIMIT:
             raise ValueError(f"limit {limit} exceeds the {MAX_LIMIT} rows the fused top-k holds per query")
         with self._lock:
             if not self.records:
                 return [[] for _ in signature_texts]  # app.py:82-83
             self._sync()
+            if filter_first and failure_types is not None and any(failure_types):
+                return self._match_filter_first(signature_texts, failure_types, limit)
             fb = self.vocab.featurize(list(signature_texts), grow=False)
             try:
                 rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit)
@@ -334,8 +381,8 @@ class GfkbStore:
                 out.append(matches)
             return out
 
-    def match(self, signature_text: str, failure_type: Optional[str] = None) -> List[dict]:
-        return self.match_batch([signature_text], [failure_type])[0]
+    def match(self, signature_text: str, failure_type: Optional[str] = None, filter_first: bool = False) -> List[dict]:
+        return self.match_batch([signature_text], [failure_type], filter_first=filter_first)[0]
 
     def match_exact(self, signature_text: str, failure_type: Optional[str] = None, limit: int = MATCH_LIMIT) -> List[dict]:
         """The handler on the full float64 score vector (K1a on both segments): no candidate stage at all."""
