@@ -216,6 +216,32 @@ int kv_selfjoin_upload(kv_index *ix, int64_t q_begin, int64_t q_end);
 int kv_index_set_row_labels(kv_index *ix, const int32_t *labels, int64_t n);
 int kv_query_set_filter(kv_index *ix, const int32_t *labels, int64_t n_q);
 
+/* Row deletion (tombstones).  rows[n]: local rows, any order; duplicates and rows already deleted are allowed (a call
+ * that deletes no new row changes nothing).  A deleted row keeps its row id and its place in the scan layout but is
+ * never returned again by any search on the handle: top-k (seed, candidate and exhaustive scans), threshold search,
+ * self-joins, the float64 fallbacks of irregular queries and the null-query fill (a null query gets the first k LIVE
+ * rows, a filtered one the first k live rows of its label).
+ *   - Like an append, a deletion needs kv_index_finalize before the next search (until then: KV_ERR_STATE); the
+ *     resident batch and any range result are dropped.  A finalize whose only change since the last full rebuild is
+ *     deletions is a statistics-only refresh (kv_index_last_finalize_kind 2); after an append the full rebuild keeps
+ *     the deleted rows deleted.
+ *   - Statistics: N (without kv_index_set_global_df) and df count live rows, and so does kv_index_local_df, so the df
+ *     all-reduce of a row-sharded or segmented GFKB stays right.  Universal-feature folding and the tf extremes stay
+ *     properties of the layout rows, deleted ones included (a folded feature is still in every layout row).  A feature
+ *     of the vocabulary that no live row holds (df 0) scores like an out-of-vocabulary feature: idf ln((N+2)/2)+1 in
+ *     the query-inclusive mode, ignored in KV_MODE_TFIDF_CORPUS_FIT.
+ *   - Outputs: kv_score writes -inf for a deleted row, kv_rescore_pairs -inf (as for a row of another shard); the
+ *     kv_selfjoin_upload query of a deleted row has an empty list, (-inf, -1), and no threshold pairs -- it stays a
+ *     singleton in kv_cluster_*.
+ *   - Labels (kv_index_set_row_labels) survive deletions.  kv_index_layout_save / _load do not carry deletions (state
+ *     of the handle, not of the file); a layout load keeps the handle's deletions.
+ *   - KV_ERR_INVALID: a row outside 0..kv_index_rows-1, rows == NULL with n > 0, or a Jaccard index (mode 1).
+ * kv_index_live_rows: kv_index_rows minus the deleted rows.  kv_index_deleted_rows: out[n] = 1 for a deleted local
+ * row, 0 for a live one; n == kv_index_rows (else KV_ERR_INVALID). */
+int kv_index_delete_rows(kv_index *ix, const int64_t *rows, int64_t n);
+int64_t kv_index_live_rows(const kv_index *ix);
+int kv_index_deleted_rows(kv_index *ix, uint8_t *out, int64_t n);
+
 /* Threshold search over the resident batch (kv_query_upload / kv_selfjoin_upload; exclusions honoured): every
  * (query, row) pair whose score -- the float32 value kv_topk reports for that pair -- is >= threshold,
  * 0 < threshold <= 1.  *n_pairs receives the count; the pairs stay in the handle until kv_range_fetch, the next

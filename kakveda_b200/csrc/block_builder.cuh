@@ -32,6 +32,7 @@ inline void idf_host(int64_t n_total, uint32_t df, double &a, double &d, int jac
   double num = (double)(n_total + (corpus_fit ? 1 : 2));
   double ib = std::log(num / ((double)df + 1.0)) + 1.0;
   double iq = corpus_fit ? ib : std::log(num / ((double)df + 2.0)) + 1.0;
+  if (corpus_fit && df == 0) { a = d = 0.0; return; }  // in no live row: ignored like an out-of-vocabulary feature
   a = iq * iq;
   d = a - ib * ib;
 }

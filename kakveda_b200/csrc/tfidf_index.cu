@@ -136,6 +136,14 @@ struct kv_index {
   DevBuf<int> d_filt_sorted, d_filt_orig;
   std::vector<int> h_filt_orig;
   bool has_filter = false;
+  // deleted rows (kv_index_delete_rows), by local row (empty until the first deletion; an append extends it).  They
+  // keep their place in the scan layout.  On the device while any row is deleted, rebuilt by every finalize: by row,
+  // the live word of every chunk (by scan position) and the first LAB_FIRST live rows (null queries)
+  std::vector<uint8_t> h_dead;
+  int64_t n_dead = 0;
+  DevBuf<uint8_t> d_dead;
+  DevBuf<uint32_t> d_alive, d_dcnt;
+  DevBuf<int> d_dead_list, d_first_live;
   // threshold search over the resident batch (kv_range_resident): its own threshold array (not d_gthr, which peers push
   // into and a top-k raises), the pair buffer, the pair count, and the result until it is fetched
   DevBuf<int> d_rthr;
@@ -398,6 +406,7 @@ int kv_index_append(kv_index *ix, const int64_t *indptr, const uint32_t *ids, co
   // labels describe the rows they were given for: a filtered query fails until the rows are labelled again
   ix->h_labels.clear();
   ix->has_labels = ix->labels_on_device = false;
+  if (ix->n_dead) ix->h_dead.resize((size_t)ix->n_rows, 0);  // appended rows are live
   return KV_OK;
 }
 
@@ -405,6 +414,8 @@ int kv_index_set_mode(kv_index *ix, int mode) {
   if (!ix || (mode != KV_MODE_TFIDF_COSINE && mode != KV_MODE_JACCARD && mode != KV_MODE_TFIDF_CORPUS_FIT))
     return kv_fail(KV_ERR_INVALID, "kv_index_set_mode: mode must be KV_MODE_TFIDF_COSINE, KV_MODE_JACCARD or KV_MODE_TFIDF_CORPUS_FIT");
   std::lock_guard<std::mutex> g(ix->mu);
+  if (mode == KV_MODE_JACCARD && ix->n_dead)
+    return kv_fail(KV_ERR_INVALID, "kv_index_set_mode: a Jaccard index (mode 1) has no row deletion, and rows are deleted");
   if (mode == KV_MODE_JACCARD)
     for (uint16_t f : ix->h_tf)
       if (f != 1) return kv_fail(KV_ERR_INVALID, "kv_index_set_mode: Jaccard rows are token SETS (every tf must be 1)");
@@ -455,6 +466,30 @@ int kv_index_set_global_df(kv_index *ix, const uint32_t *df, int64_t vocab_size,
   return KV_OK;
 }
 
+// Document frequencies of the live rows: d_cnt (every row of the layout, already histogrammed) minus the entries of the
+// deleted rows, in d_dcnt; *out = d_cnt itself when nothing is deleted.  Caller holds ix->mu.
+static int live_counts(kv_index *ix, int64_t Vz, const uint32_t **out) {
+  *out = ix->d_cnt.p;
+  if (!ix->n_dead) return KV_OK;
+  cudaStream_t s = ix->stream;
+  std::vector<int> list;
+  list.reserve((size_t)ix->n_dead);
+  for (int64_t r = 0; r < ix->n_rows; r++)
+    if (ix->h_dead[(size_t)r]) list.push_back((int)r);
+  KV_CUDA(ix->d_dead_list.ensure((int64_t)list.size()));
+  KV_CUDA(ix->d_dcnt.ensure(Vz));
+  KV_CUDA(cudaMemcpyAsync(ix->d_dead_list.p, list.data(), list.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  KV_CUDA(cudaMemsetAsync(ix->d_dcnt.p, 0, (size_t)Vz * sizeof(uint32_t), s));
+  hist_rows_kernel<<<(unsigned)(((int64_t)list.size() * 32 + 255) / 256), 256, 0, s>>>(ix->indptr.p, ix->ids.p, ix->d_dead_list.p,
+                                                                                       (int64_t)list.size(), ix->d_dcnt.p);
+  KV_CUDA(cudaGetLastError());
+  sub_count_kernel<<<(unsigned)((Vz + 255) / 256), 256, 0, s>>>(ix->d_cnt.p, ix->d_dcnt.p, Vz, ix->d_dcnt.p);
+  KV_CUDA(cudaGetLastError());
+  KV_CUDA(cudaStreamSynchronize(s));  // the host list goes out of scope
+  *out = ix->d_dcnt.p;
+  return KV_OK;
+}
+
 int kv_index_local_df(kv_index *ix, uint32_t *df_out, int64_t vocab_size) {
   if (!ix || !df_out || vocab_size < 0) return kv_fail(KV_ERR_INVALID, "kv_index_local_df: bad arguments");
   std::lock_guard<std::mutex> g(ix->mu);
@@ -467,8 +502,11 @@ int kv_index_local_df(kv_index *ix, uint32_t *df_out, int64_t vocab_size) {
     hist_kernel<<<ix->sm_count * 8, 256, 0, ix->stream>>>(ix->ids.p, ix->tf.p, ix->nnz, ix->d_cnt.p, nullptr, nullptr);
     KV_CUDA(cudaGetLastError());
   }
+  const uint32_t *live = nullptr;
+  int rc = live_counts(ix, std::max<int64_t>(vocab_size, 1), &live);  // deleted rows do not count
+  if (rc != KV_OK) return rc;
   if (vocab_size)
-    KV_CUDA(cudaMemcpyAsync(df_out, ix->d_cnt.p, (size_t)vocab_size * sizeof(uint32_t), cudaMemcpyDeviceToHost, ix->stream));
+    KV_CUDA(cudaMemcpyAsync(df_out, live, (size_t)vocab_size * sizeof(uint32_t), cudaMemcpyDeviceToHost, ix->stream));
   KV_CUDA(cudaStreamSynchronize(ix->stream));
   return KV_OK;
 }
@@ -500,6 +538,7 @@ static int upload_labels(kv_index *ix) {
   keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
   std::vector<int> first(keys.size() * LAB_FIRST, -1), cnt(keys.size(), 0);
   for (int64_t r = 0; r < n; r++) {
+    if (ix->n_dead && ix->h_dead[(size_t)r]) continue;  // null queries get live rows only
     const size_t i = (size_t)(std::lower_bound(keys.begin(), keys.end(), ix->h_labels[(size_t)r]) - keys.begin());
     if (cnt[i] < LAB_FIRST) first[i * LAB_FIRST + (size_t)cnt[i]++] = (int)r;
   }
@@ -555,6 +594,63 @@ int kv_index_set_row_labels(kv_index *ix, const int32_t *labels, int64_t n) {
   return upload_labels(ix);
 }
 
+// The device copies of the deletions for the current layout (d_perm must hold it): deleted flags by row, the live word
+// of every chunk and the first LAB_FIRST live rows.  Nothing while no row is deleted: the kernels then get NULL.
+static int upload_dead(kv_index *ix) {
+  if (!ix->n_dead || ix->n_rows == 0) return KV_OK;
+  cudaStream_t s = ix->stream;
+  const int64_t n = ix->n_rows;
+  std::vector<int> first(LAB_FIRST, -1);
+  for (int64_t r = 0, c = 0; r < n && c < LAB_FIRST; r++)
+    if (!ix->h_dead[(size_t)r]) first[(size_t)c++] = (int)r;
+  KV_CUDA(ix->d_dead.ensure(n));
+  KV_CUDA(ix->d_alive.ensure(ix->n_chunks_pad));
+  KV_CUDA(ix->d_first_live.ensure(LAB_FIRST));
+  KV_CUDA(cudaMemcpyAsync(ix->d_dead.p, ix->h_dead.data(), (size_t)n, cudaMemcpyHostToDevice, s));
+  KV_CUDA(cudaMemcpyAsync(ix->d_first_live.p, first.data(), first.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  alive_kernel<<<(unsigned)((ix->n_chunks_pad + 255) / 256), 256, 0, s>>>(ix->d_perm.p, ix->d_dead.p, n, ix->n_chunks_pad, ix->d_alive.p);
+  KV_CUDA(cudaGetLastError());
+  KV_CUDA(cudaStreamSynchronize(s));  // the host list goes out of scope
+  return KV_OK;
+}
+
+// NULL while no row is deleted: the kernels' per-row and per-chunk tests are then skipped
+static const uint8_t *dead_rows(const kv_index *ix) { return ix->n_dead ? ix->d_dead.p : nullptr; }
+static const uint32_t *alive_words(const kv_index *ix) { return ix->n_dead ? ix->d_alive.p : nullptr; }
+
+int kv_index_delete_rows(kv_index *ix, const int64_t *rows, int64_t n) {
+  if (!ix || n < 0 || (n > 0 && !rows)) return kv_fail(KV_ERR_INVALID, "kv_index_delete_rows: bad arguments");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_index_delete_rows: a Jaccard index (mode 1) has no row deletion");
+  for (int64_t i = 0; i < n; i++)
+    if (rows[i] < 0 || rows[i] >= ix->n_rows)
+      return kv_fail(KV_ERR_INVALID, "kv_index_delete_rows: row %lld outside 0..%lld", (long long)rows[i], (long long)ix->n_rows - 1);
+  int64_t added = 0;
+  for (int64_t i = 0; i < n; i++) {
+    if (ix->h_dead.empty()) ix->h_dead.assign((size_t)ix->n_rows, 0);
+    uint8_t &d = ix->h_dead[(size_t)rows[i]];
+    if (!d) { d = 1; added++; }
+  }
+  if (!added) return KV_OK;  // duplicates and rows deleted before: nothing changes
+  ix->n_dead += added;
+  // like an append: statistics and the device copies are stale until the next finalize
+  ix->finalized = false;
+  ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
+  return KV_OK;
+}
+
+int64_t kv_index_live_rows(const kv_index *ix) { return ix ? ix->n_rows - ix->n_dead : 0; }
+
+int kv_index_deleted_rows(kv_index *ix, uint8_t *out, int64_t n) {
+  if (!ix || n < 0 || (n > 0 && !out)) return kv_fail(KV_ERR_INVALID, "kv_index_deleted_rows: bad arguments");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (n != ix->n_rows)
+    return kv_fail(KV_ERR_INVALID, "kv_index_deleted_rows: %lld flags for an index of %lld rows", (long long)n, (long long)ix->n_rows);
+  if (ix->n_dead) memcpy(out, ix->h_dead.data(), (size_t)n);
+  else if (n) memset(out, 0, (size_t)n);
+  return KV_OK;
+}
+
 int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
   if (!ix || vocab_size < 0) return kv_fail(KV_ERR_INVALID, "kv_index_finalize: bad arguments");
   std::lock_guard<std::mutex> g(ix->mu);
@@ -590,8 +686,13 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
     if (V) KV_CUDA(cudaMemcpyAsync(ix->d_df.p, ix->h_gdf.data(), (size_t)V * 4, cudaMemcpyHostToDevice, s));
     ix->n_total = ix->n_global;
   } else {
-    if (V) KV_CUDA(cudaMemcpyAsync(ix->d_df.p, ix->d_cnt.p, (size_t)V * 4, cudaMemcpyDeviceToDevice, s));
-    ix->n_total = n;
+    // N and df count live rows; d_cnt keeps counting every row of the layout, which is what decides a universal
+    // feature (folded into per-query constants): a deletion alone therefore never changes the layout
+    const uint32_t *live = nullptr;
+    int rc = live_counts(ix, Vz, &live);
+    if (rc != KV_OK) return rc;
+    if (V) KV_CUDA(cudaMemcpyAsync(ix->d_df.p, live, (size_t)V * 4, cudaMemcpyDeviceToDevice, s));
+    ix->n_total = n - ix->n_dead;
   }
   if (V) {
     IdfTables T{ix->d_a64.p, ix->d_d64.p, ix->d_bb64.p, ix->d_univ.p, ix->d_utf.p};
@@ -647,8 +748,10 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
       rownorm_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(ix->indptr.p, ix->ids.p, ix->tf.p, ix->d_perm.p, n,
                                                                       ix->d_bb64.p, ix->d_B64.p, ix->d_B32.p);
       KV_CUDA(cudaGetLastError());
+      int rc = upload_dead(ix);
+      if (rc != KV_OK) return rc;
       chunk_meta_kernel<<<(unsigned)((ix->n_chunks_pad + 255) / 256), 256, 0, s>>>(ix->d_B32.p, n, ix->n_chunks, ix->n_chunks_pad,
-                                                                                    ix->d_cminB.p);
+                                                                                    alive_words(ix), ix->d_cminB.p);
       KV_CUDA(cudaGetLastError());
       KV_CUDA(cudaStreamSynchronize(s));
       ix->V = V;
@@ -682,6 +785,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
     for (const auto &o : L.ovf) { SL.ovf_keys.push_back(o.first); SL.ovf_vals.push_back(o.second); }
   }
   int rc = upload_layout(ix, SL);
+  if (rc == KV_OK) rc = upload_dead(ix);
   if (rc != KV_OK) return rc;
   if (n) {
     rownorm_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(ix->indptr.p, ix->ids.p, ix->tf.p, ix->d_perm.p, n,
@@ -689,7 +793,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
     KV_CUDA(cudaGetLastError());
   }
   chunk_meta_kernel<<<(unsigned)((ix->n_chunks_pad + 255) / 256), 256, 0, s>>>(ix->d_B32.p, n, ix->n_chunks, ix->n_chunks_pad,
-                                                                                ix->d_cminB.p);
+                                                                                alive_words(ix), ix->d_cminB.p);
   KV_CUDA(cudaGetLastError());
   KV_CUDA(cudaStreamSynchronize(s));
   ix->V = V;
@@ -763,7 +867,7 @@ static int score_impl(kv_index *ix, const uint32_t *q_ids, const uint32_t *q_tf,
   P.qw = (const unsigned long long *)ix->d_qtab1.p; P.qc = P.qw + H; P.qkeys = (const uint32_t *)(P.qc + H);
   P.log_h = log_h;
   P.w_unscale = std::ldexp(1.0, -e_w); P.c_unscale = std::ldexp(1.0, -e_c);
-  P.nq = nq; P.dotU = dotU; P.corrU = corrU; P.jaccard = ix->jaccard; P.out = ix->d_scores.p;
+  P.nq = nq; P.dotU = dotU; P.corrU = corrU; P.jaccard = ix->jaccard; P.dead = dead_rows(ix); P.out = ix->d_scores.p;
   const size_t smem = tab_bytes + 8 * 32 * 24;
   int blocks = (int)std::min<int64_t>((ix->n_chunks + 7) / 8, (int64_t)ix->sm_count * 8);
   if (blocks < 1) blocks = 1;
@@ -798,7 +902,7 @@ struct QueryRun {
   // optional (kv_query_prepare_slice): the run's rows are stored SORTED by feature-id sequence (ties by original
   // index) and order[p] = original index, inside the run, of the query in row p -- merging then walks memory in order
   const int32_t *order = nullptr;
-  const uint8_t *flags = nullptr;   // optional, by row: 0 regular, 1 null, 2 irregular
+  const uint8_t *flags = nullptr;   // optional, by row: 0 regular, 1 null, 2 irregular, 3 off (a deleted row's self-join)
   int64_t n_q = 0;
 };
 
@@ -816,6 +920,7 @@ static void classify_queries(const kv_index *ix, const int64_t *q_indptr, const 
       for (int64_t p = q_indptr[q]; p < q_indptr[q + 1]; p++) {
         const uint32_t t = q_ids[p];
         if ((int64_t)t >= ix->V) continue;
+        if (ix->corpus_fit && ix->h_df[t] == 0) continue;  // in no live row: ignored like an out-of-vocabulary feature
         known = true;
         if (ix->h_univ[t]) continue;
         feats++;
@@ -1077,6 +1182,7 @@ static ScanParams scan_params(const kv_index *ix, const Batch &b) {
   SP.qtab = ix->d_qtab.p; SP.q_nq = qc; SP.q_dotU = qc + b.n_q; SP.q_corrU = qc + 2 * b.n_q;
   SP.q_excl = ix->has_excl ? ix->d_excl_sorted.p : nullptr; SP.gthr = b.range ? ix->d_rthr.p : ix->d_gthr.p;
   if (ix->has_filter) { SP.q_label = ix->d_filt_sorted.p; SP.label_pos = ix->d_label_pos.p; SP.chunk_sig = ix->d_chunk_sig.p; }
+  SP.alive = alive_words(ix);
   for (int i = 0; i < 7; i++) SP.peer_gthr[i] = i < b.n_peers ? ix->peer_gthr[i] : nullptr;
   SP.n_peers = b.n_peers; SP.stats = ix->d_stats.p; SP.n_q = b.n_q; SP.k = b.k;
   SP.part_scores = ix->d_part_s.p; SP.part_rows = ix->d_part_r.p; SP.max_pages = b.max_pages;
@@ -1344,7 +1450,7 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
                                                                                   ix->n_rows, ix->row_base,
                                                                                   ix->has_excl ? ix->d_excl_orig.p : nullptr,
                                                                                   ix->has_filter ? ix->d_filt_orig.p : nullptr, L,
-                                                                                  d_out_s, d_out_r);
+                                                                                  ix->n_dead ? ix->d_first_live.p : nullptr, d_out_s, d_out_r);
     KV_CUDA(cudaGetLastError());
     b.launches++;
   }
@@ -1354,7 +1460,8 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
     if (rc != KV_OK) return rc;
     select_topk_kernel<<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
                                           ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->d_labels_row.p,
-                                          ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, d_out_s + q * k, d_out_r + q * k);
+                                          ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix), d_out_s + q * k,
+                                          d_out_r + q * k);
     KV_CUDA(cudaGetLastError());
     b.launches += 2;
   }
@@ -1441,7 +1548,7 @@ static int run_range(kv_index *ix, float thr, int64_t *n_pairs, const char *fn) 
                                                            (int)q, ix->d_jrange.p, ix->d_range_count.p, range_cap());
         } else {
           select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, thr, excl, ix->d_labels_row.p,
-                                                   ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, (int)q, ix->d_range.p,
+                                                   ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix), (int)q, ix->d_range.p,
                                                    ix->d_range_count.p, range_cap());
         }
         KV_CUDA(cudaGetLastError());
@@ -1603,7 +1710,17 @@ int kv_selfjoin_upload(kv_index *ix, int64_t q_begin, int64_t q_end) {
   for (int64_t i = 0; i <= n; i++) ip[(size_t)i] = ix->h_indptr[(size_t)(q_begin + i)] - base;
   std::vector<uint32_t> tf32((size_t)ip[(size_t)n]);
   for (size_t i = 0; i < tf32.size(); i++) tf32[i] = ix->h_tf[(size_t)base + i];
-  int rc = prepare_batch(ix, ip.data(), ix->h_ids.data() + base, tf32.data(), nullptr, n);
+  QueryRun R;
+  R.indptr = ip.data(); R.ids = ix->h_ids.data() + base; R.tf = tf32.data(); R.n_q = n;
+  std::vector<uint8_t> flags;
+  if (ix->n_dead) {  // a deleted row's query is switched off (flag 3): no path answers it, its list stays (-inf, -1)
+    flags.resize((size_t)n);
+    classify_queries(ix, ip.data(), R.ids, R.tf, n, flags.data(), host_threads());
+    for (int64_t i = 0; i < n; i++)
+      if (ix->h_dead[(size_t)(q_begin + i)]) flags[(size_t)i] = 3;
+    R.flags = flags.data();
+  }
+  int rc = prepare_batch_runs(ix, &R, 1);
   if (rc != KV_OK) return rc;
   for (int64_t i = 0; i < n; i++) ex[(size_t)i] = ix->row_base + q_begin + i;
   return set_exclusions_locked(ix, ex.data(), n);
@@ -1648,7 +1765,7 @@ int kv_rescore_pairs(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_id
   P.q_indptr = ix->d_rq_indptr.p; P.q_ids = ix->d_rq_ids.p; P.q_tf = ix->d_rq_tf.p;
   P.q_nq = ix->d_rq_const.p;
   P.rows = ix->d_rq_rows.p; P.n_q = n_q; P.n_rows = ix->n_rows; P.row_base = ix->row_base; P.V = ix->V;
-  P.k = k; P.jaccard = ix->jaccard; P.out = ix->d_rq_out.p;
+  P.k = k; P.jaccard = ix->jaccard; P.dead = dead_rows(ix); P.out = ix->d_rq_out.p;
   rescore_kernel<<<(unsigned)((n_q * k * 32 + 255) / 256), 256, 0, s>>>(P);
   KV_CUDA(cudaGetLastError());
   KV_CUDA(cudaMemcpyAsync(out_scores, ix->d_rq_out.p, (size_t)n_q * k * 8, cudaMemcpyDeviceToHost, s));

@@ -102,10 +102,41 @@ __global__ void idf_kernel(const uint32_t *__restrict__ df, const uint32_t *__re
   double ib = jaccard ? 1.0 : log(num / ((double)df[t] + 1.0)) + 1.0;  // Jaccard: every token weighs 1
   double iq = jaccard ? 1.0 : (corpus_fit ? ib : log(num / ((double)df[t] + 2.0)) + 1.0);
   double a = iq * iq, bb = ib * ib;
-  T.a64[t] = a; T.d64[t] = a - bb; T.bb64[t] = bb;
+  // corpus_fit: a feature no live row holds (all its rows deleted) is outside the vocabulary a fit on the corpus
+  // would learn, so the query ignores it like an out-of-vocabulary feature (idf_host does the same)
+  if (corpus_fit && !jaccard && df[t] == 0) a = bb = 0.0;
+  T.a64[t] = a; T.d64[t] = a - bb; T.bb64[t] = ib * ib;
   bool u = n_local > 0 && (int64_t)cnt[t] == n_local && tfmin[t] == tfmax[t];
   T.univ[t] = u ? 1 : 0;
   T.utf[t] = u ? tfmin[t] : 0;
+}
+
+// Row deletion (kv_index_delete_rows): cnt[t] += entries of feature t in the listed rows -- one warp per listed row.
+// cnt minus this histogram is the live document frequency.
+__global__ void hist_rows_kernel(const int64_t *__restrict__ indptr, const uint32_t *__restrict__ ids,
+                                 const int *__restrict__ rows, int64_t n, uint32_t *cnt) {
+  const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  if (i >= n) return;
+  const int r = rows[i];
+  for (int64_t p = indptr[r] + (threadIdx.x & 31); p < indptr[r + 1]; p += 32) atomicAdd(&cnt[ids[p]], 1u);
+}
+
+__global__ void sub_count_kernel(const uint32_t *__restrict__ a, const uint32_t *__restrict__ b, int64_t n, uint32_t *out) {
+  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (t < n) out[t] = a[t] - b[t];
+}
+
+// Live word of every chunk: bit i set when the row at position 32c + i exists and is not deleted (dead: by row)
+__global__ void alive_kernel(const int *__restrict__ perm, const uint8_t *__restrict__ dead, int64_t n_rows,
+                             int64_t n_chunks_pad, uint32_t *alive) {
+  const int64_t c = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (c >= n_chunks_pad) return;
+  uint32_t m = 0;
+  for (int i = 0; i < CHUNK_ROWS; i++) {
+    const int64_t pos = c * CHUNK_ROWS + i;
+    if (pos < n_rows && !dead[perm[pos]]) m |= 1u << i;
+  }
+  alive[c] = m;
 }
 
 // one warp per position: B_c
@@ -132,16 +163,18 @@ __global__ void rownorm_kernel(const int64_t *__restrict__ indptr, const uint32_
 }
 
 // chunk_minB[c] for c < n_chunks; +inf for the padding chunks up to n_pad (and for chunks without a positive norm:
-// rows without features always score 0, they do not loosen a bound)
+// rows without features always score 0, they do not loosen a bound).  alive (NULL: no row deleted): deleted rows are
+// never returned, so they do not loosen a bound either -- an all-deleted chunk's bound is 0.
 __global__ void chunk_meta_kernel(const float *__restrict__ B32, int64_t n_rows, int64_t n_chunks, int64_t n_pad,
-                                  float *chunk_minB) {
+                                  const uint32_t *__restrict__ alive, float *chunk_minB) {
   int64_t c = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (c >= n_pad) return;
   float m = INFINITY;
   if (c < n_chunks) {
     const int64_t r = c * CHUNK_ROWS;
+    const uint32_t live = alive ? alive[c] : FULL;
     for (int64_t i = r; i < r + CHUNK_ROWS && i < n_rows; i++)
-      if (B32[i] > 0.f) m = fminf(m, B32[i]);
+      if (B32[i] > 0.f && ((live >> (i - r)) & 1u)) m = fminf(m, B32[i]);
   }
   chunk_minB[c] = m;
 }
@@ -236,6 +269,7 @@ struct ScoreParams {
   double w_unscale, c_unscale;  // 2^-e, 2^-e2
   double nq, dotU, corrU;
   int jaccard;
+  const uint8_t *dead;  // by ORIGINAL row, NULL: no row deleted (a deleted row scores -inf)
   double *out;  // by ORIGINAL row
 };
 
@@ -313,7 +347,8 @@ __global__ void __launch_bounds__(256) tfidf_score_kernel(ScoreParams P) {
         const double den = P.nq * (B + corr);
         sc = (den > 0.0 && dot != 0.0) ? dot / sqrt(den) : 0.0;
       }
-      P.out[P.perm[pos0 + lane]] = sc;
+      const int row = P.perm[pos0 + lane];
+      P.out[row] = (P.dead && P.dead[row]) ? -INFINITY : sc;
     }
   }
 }
@@ -333,7 +368,8 @@ struct PrepParams {
   const uint32_t *q_ids, *q_tf;
   const double *q_oov;      // [n_q] or NULL
   const int *qsrc;          // sorted slot -> row of the uploaded CSR
-  const uint8_t *flags;     // by sorted slot: 0 regular, 1 null (every score is 0), 2 irregular (float64 full-scan path)
+  const uint8_t *flags;     // by sorted slot: 0 regular, 1 null (every score is 0), 2 irregular (float64 full-scan path),
+                            // 3 off (a deleted row's self-join query: answered by no path)
   int64_t n_q, V, n_total;
   const double *a64, *d64;
   const uint8_t *univ;
@@ -554,6 +590,7 @@ struct ScanParams {
   const int *q_label;                     // [n_q] label a query's rows must carry, -1 = any
   const int *label_pos;                   // [n_chunks_pad * 32] row label by scan position
   const unsigned long long *chunk_sig;    // [n_chunks_pad] chunk label signatures
+  const uint32_t *alive;                  // [n_chunks_pad] live word per chunk (kv_index_delete_rows), NULL: none deleted
   int *gthr;                              // [n_q] float bits: lower bound of the global k-th score
   int *peer_gthr[7];                      // the same array on the other GPUs of a row-sharded GFKB (peer memory over
   int n_peers;                            //   NVLink): a raised bound is pushed to every shard, so all of them prune with it
@@ -711,6 +748,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
       const int lb = s_qlab[lane];
       mask &= __ballot_sync(FULL, lb < 0 || ((sig >> (lb & 63)) & 1ull));
     }
+    if (P.alive && P.alive[chunk] == 0u) mask = 0;  // every row of the chunk deleted: never staged
   };
   auto grab = [&]() -> uint32_t {
     uint32_t r = 0;
@@ -768,6 +806,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
       const uint32_t valid = rows == 32 ? FULL : ((1u << rows) - 1u);
       const float Bc = lane < rows ? P.B32[pos0 + lane] : 0.f;
       const int lpos = P.q_label ? P.label_pos[pos0 + lane] : -1;  // one 128-byte line per record
+      const bool live = P.alive ? ((P.alive[chunk_cur] >> lane) & 1u) != 0u : true;
       recs_done++;
       for (uint32_t qm = mask_cur; qm; qm &= qm - 1) {
         const int qi = __ffs(qm) - 1;
@@ -845,7 +884,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
             const float den = nq * t;
             sc = den > 0.f ? __fdiv_rn(dot, __fsqrt_rn(den)) : 0.f;
             row = P.perm[pos0 + lane];
-            cand = row != s_excl[qi] && sc >= filt && (ql < 0 || lpos == ql);
+            cand = row != s_excl[qi] && sc >= filt && (ql < 0 || lpos == ql) && live;
           }
         }
         if constexpr (RANGE) {
@@ -1182,7 +1221,8 @@ struct RescoreParams {
   const long long *rows;    // [n_q * k] global row ids (-1: unused slot)
   int64_t n_q, n_rows, row_base, V;
   int k, jaccard;
-  double *out;              // [n_q * k]; -inf for unused slots and rows of other shards
+  const uint8_t *dead;      // by local row, NULL: no row deleted
+  double *out;              // [n_q * k]; -inf for unused slots, rows of other shards and deleted rows
 };
 
 __global__ void __launch_bounds__(256) rescore_kernel(RescoreParams P) {
@@ -1192,7 +1232,7 @@ __global__ void __launch_bounds__(256) rescore_kernel(RescoreParams P) {
   const int64_t q = pair / P.k;
   const long long gr = P.rows[pair];
   const int64_t r = gr - P.row_base;
-  if (gr < 0 || r < 0 || r >= P.n_rows) {
+  if (gr < 0 || r < 0 || r >= P.n_rows || (P.dead && P.dead[r])) {
     if (lane == 0) P.out[pair] = -INFINITY;
     return;
   }
@@ -1301,26 +1341,32 @@ struct LabelFirstRows {
 };
 
 // Null queries (no feature in common with any row: every score is 0): the stable sort keeps the
-// first k rows -- of the query's label when it is filtered (label_by_query: by ORIGINAL query, NULL: no filter).
+// first k live rows -- of the query's label when it is filtered (label_by_query: by ORIGINAL query, NULL: no filter).
+// first_live: the first LAB_FIRST live rows, -1 past the last (NULL: no row deleted, rows 0, 1, ...).
 // One thread per (query, slot).
 __global__ void fill_null_kernel(const int *__restrict__ null_q, int n_null, int k, int64_t n_rows, int64_t row_base,
                                  const int *__restrict__ excl_by_query, const int *__restrict__ label_by_query,
-                                 LabelFirstRows L, float *out_s, long long *out_r) {
+                                 LabelFirstRows L, const int *__restrict__ first_live, float *out_s, long long *out_r) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_null * k) return;
   int q = null_q[i / k], j = i % k;
   const int ex = excl_by_query ? excl_by_query[q] : -1;  // by ORIGINAL query index
   const int lb = label_by_query ? label_by_query[q] : -1;
-  if (lb >= 0) {
-    int lo = 0, hi = L.n_lab - 1, idx = -1;
-    while (lo <= hi) {
-      const int mid = (lo + hi) >> 1;
-      if (L.keys[mid] == lb) { idx = mid; break; }
-      if (L.keys[mid] < lb) lo = mid + 1; else hi = mid - 1;
+  if (lb >= 0 || first_live) {
+    int idx = -1;
+    const int *list = first_live;
+    if (lb >= 0) {
+      int lo = 0, hi = L.n_lab - 1;
+      while (lo <= hi) {
+        const int mid = (lo + hi) >> 1;
+        if (L.keys[mid] == lb) { idx = mid; break; }
+        if (L.keys[mid] < lb) lo = mid + 1; else hi = mid - 1;
+      }
+      list = idx >= 0 ? L.rows + (size_t)idx * LAB_FIRST : nullptr;
     }
     int r = -1;
-    for (int t = 0, seen = 0; idx >= 0 && t < LAB_FIRST; t++) {  // the j-th row of the label once the excluded one is skipped
-      const int x = L.rows[(size_t)idx * LAB_FIRST + t];
+    for (int t = 0, seen = 0; list && t < LAB_FIRST; t++) {  // the j-th listed row once the excluded one is skipped
+      const int x = list[t];
       if (x < 0) break;
       if (x == ex) continue;
       if (seen++ == j) { r = x; break; }
@@ -1335,9 +1381,10 @@ __global__ void fill_null_kernel(const int *__restrict__ null_q, int n_null, int
 }
 
 // Fallback selection for one (irregular) query: k passes of block-wide arg-best over float64 scores.  lab >= 0: only
-// rows with labels[row] == lab (by original row) compete.
+// rows with labels[row] == lab (by original row) compete; dead (NULL: none) marks deleted rows, which never do.
 __global__ void select_topk_kernel(const double *__restrict__ scores, int64_t n, int64_t row_base, int k, int64_t excl,
-                                   const int *__restrict__ labels, int lab, float *out_s, long long *out_r) {
+                                   const int *__restrict__ labels, int lab, const uint8_t *__restrict__ dead,
+                                   float *out_s, long long *out_r) {
   __shared__ float s_s[32];
   __shared__ long long s_r[32];
   __shared__ float prev_s;
@@ -1350,7 +1397,7 @@ __global__ void select_topk_kernel(const double *__restrict__ scores, int64_t n,
     const float ps = prev_s;
     const long long pr = prev_r;
     for (int64_t r = threadIdx.x; r < n; r += blockDim.x) {
-      if (r == excl || (lab >= 0 && labels[r] != lab)) continue;
+      if (r == excl || (lab >= 0 && labels[r] != lab) || (dead && dead[r])) continue;
       float s = (float)scores[r];
       bool after = (s < ps) || (s == ps && r > pr);  // strictly after the previously selected pair
       if (after && (br < 0 || s > bs || (s == bs && r < br))) { bs = s; br = r; }
@@ -1382,17 +1429,19 @@ __global__ void select_topk_kernel(const double *__restrict__ scores, int64_t n,
 }
 
 // Fallback of a threshold search for one (irregular) query: every row whose float64 score, rounded to the float32
-// select_topk_kernel reports, reaches the threshold is appended to the pair buffer (lab >= 0: rows of that label only).
+// select_topk_kernel reports, reaches the threshold is appended to the pair buffer (lab >= 0: rows of that label only;
+// deleted rows never).
 __global__ void select_range_kernel(const double *__restrict__ scores, int64_t n, int64_t row_base, float thr, int64_t excl,
-                                    const int *__restrict__ labels, int lab, int q, RangePair *out, unsigned long long *count,
-                                    unsigned long long cap) {
+                                    const int *__restrict__ labels, int lab, const uint8_t *__restrict__ dead, int q,
+                                    RangePair *out, unsigned long long *count, unsigned long long cap) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   const int qv = q;
   // whole warps step together (blockDim is a multiple of 32): range_emit needs every lane
   for (int64_t r0 = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) & ~31LL; r0 < n; r0 += stride) {
     const int64_t r = r0 + (threadIdx.x & 31);
     const float s = r < n ? (float)scores[r] : -INFINITY;
-    range_emit(out, count, cap, r < n && r != excl && (lab < 0 || labels[r] == lab) && s >= thr, &qv, s, row_base + r);
+    range_emit(out, count, cap, r < n && r != excl && (lab < 0 || labels[r] == lab) && !(dead && dead[r]) && s >= thr, &qv, s,
+               row_base + r);
   }
 }
 

@@ -96,6 +96,11 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
     keep = np.ones(n, dtype=bool)
     if failure_type is not None:
         keep = np.fromiter((r.get("failure_type") == failure_type for r in records), dtype=bool, count=n)
+    if hasattr(index, "deleted_mask"):
+        # deleted rows (GfkbIndex.delete_rows) join no pattern: the self-join never returns them and their own lists
+        # are empty, so each is a singleton -- and a singleton record spanning two apps must not become a pattern
+        dead = index.deleted_mask()[:n]
+        keep[: len(dead)] &= ~dead
     if filter_first and failure_type is not None:
         from .similarity import GfkbIndex
 

@@ -67,3 +67,23 @@ def load(path: Path, signature_texts: Sequence[str]) -> Optional[Tuple[Vocabular
             return Vocabulary.from_keys(keys), ArrayBatch(indptr, ids, tf.astype(np.uint32)), n
     except Exception:  # unreadable / truncated / foreign file: the sidecar is only a cache
         return None
+
+
+def load_arrays(path: Path) -> Optional[Tuple[ArrayBatch, int]]:
+    """(CSR of the rows, n) as the file holds them, without the digest check of ``load`` -- for a writer that knows
+    which rows it saved (``GfkbStore`` rewriting its own sidecar after a purge); None if missing or unreadable."""
+    path = Path(path)
+    if not path.exists():
+        return None
+    try:
+        with np.load(path) as z:
+            meta = z["meta"]
+            if int(meta[0]) != FORMAT_VERSION:
+                return None
+            n, nnz = int(meta[1]), int(meta[2])
+            indptr, ids, tf = z["indptr"], z["ids"], z["tf"]
+            if len(indptr) != n + 1 or len(ids) != nnz or len(tf) != nnz:
+                return None
+            return ArrayBatch(indptr, ids, tf.astype(np.uint32)), n
+    except Exception:  # unreadable / truncated / foreign file: the sidecar is only a cache
+        return None

@@ -263,6 +263,26 @@ class GfkbIndex:
     def n_rows(self) -> int:
         return int(_capi.load().kv_index_rows(self._h))
 
+    def delete_rows(self, rows) -> None:
+        """Delete local ``rows`` (any order; duplicates and rows deleted before are allowed).  A deleted row keeps its
+        row id but no search returns it again and ``score`` gives it -inf; N and df count the live rows.  Like an
+        append, the deletion takes effect at the next ``finalize`` (a statistics-only refresh when nothing was
+        appended) and searches raise until then.  Not on a Jaccard index (mode 1)."""
+        rows = np.ascontiguousarray(rows, dtype=np.int64).reshape(-1)
+        _capi.check(_capi.load().kv_index_delete_rows(self._h, _ptr(rows, C.c_int64), len(rows)))
+
+    def deleted_mask(self) -> np.ndarray:
+        """bool [n_rows]: which local rows are deleted (the handle's own flags)."""
+        n = self.n_rows
+        out = np.zeros(n, dtype=np.uint8)
+        _capi.check(_capi.load().kv_index_deleted_rows(self._h, _ptr(out, C.c_uint8), n))
+        return out.astype(bool)
+
+    @property
+    def n_live_rows(self) -> int:
+        """``n_rows`` minus the deleted rows."""
+        return int(_capi.load().kv_index_live_rows(self._h))
+
     # -- query ---------------------------------------------------------------------------
     def score_features(self, ids: np.ndarray, tf: np.ndarray, oov_tf2: float) -> np.ndarray:
         out = np.empty(self.n_rows, dtype=np.float64)
@@ -273,7 +293,7 @@ class GfkbIndex:
         return out
 
     def score(self, query: str) -> np.ndarray:
-        """float64 cosine of ``query`` against every local row (K1a)."""
+        """float64 cosine of ``query`` against every local row (K1a); -inf for a deleted row."""
         fb = self.vocab.featurize([query], grow=False)
         try:
             return self.score_features(fb.ids, fb.tf, float(fb.oov[0]))

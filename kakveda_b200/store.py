@@ -11,6 +11,9 @@ the records and their device index resident and reproduces the three handlers th
   failure_type filter, mapped to FailureMatch fields.
 * ``warn_batch`` -- services/warning_policy/app.py:19-72: signature_text of the request, best match against the
   threshold, the reference's message strings.
+* ``purge_apps`` -- services/dashboard/app.py:330-375 on failures.jsonl: the purged app ids leave every record's
+  ``affected_apps``, records left with none are dropped, the file is rewritten.  The emptied records' device rows are
+  deleted in place (``GfkbIndex.delete_rows`` + a statistics-only finalize) instead of rebuilding the index.
 
 Index layout: a large MAIN segment (text-sorted scan layout, expensive to rebuild) plus a small TAIL segment that
 receives upserts.  TF-IDF statistics are global (every append changes N and df of every row), so after an append
@@ -23,6 +26,7 @@ feature order, so identical rows tie exactly in both segments) and ordered like 
 from __future__ import annotations
 
 import json
+import shutil
 import threading
 from datetime import datetime, timezone
 from pathlib import Path
@@ -114,8 +118,15 @@ class GfkbStore:
         self.vocab = Vocabulary()
         self._main: Optional[GfkbIndex] = None
         self._tail: Optional[GfkbIndex] = None
-        self._n_main = 0          # records[:_n_main] live in the main segment
+        self._n_main = 0          # device rows of the main segment (records[:_n_main] while no row is deleted)
         self._n_indexed = 0       # records[:_n_indexed] are on the device (main + tail)
+        self._n_dev = 0           # device rows of main + tail, deleted ones included
+        # Device row -> record index, -1 for a deleted row; None: the identity (no deletion since the last rebuild).
+        # Deletion removes rows and appends go at the end, so device-row order is monotone in record order: the
+        # (score desc, device row asc) order of a search is exactly the reference's stable order over the records.
+        self._row2rec: Optional[np.ndarray] = None
+        self._n_deleted = 0       # device rows deleted since the last rebuild (past tail_limit the next _sync compacts)
+        self._sidecar_rows = 0    # the sidecar file holds the CSR of records[:_sidecar_rows]
         self._main_df: Optional[np.ndarray] = None
         self._dirty = False
         # failure_type -> row label of the device index, numbered in order of first appearance; label of each record
@@ -207,34 +218,60 @@ class GfkbStore:
                 self._main.save_layout(lay_path)
             self._main.set_row_labels(self._row_labels(0, n))
             self.stats["full_rebuilds"] += 1
-        self._n_main = self._n_indexed = n
+        self._n_main = self._n_indexed = self._n_dev = n
+        self._sidecar_rows = n if self.sidecar_path is not None else 0  # the sidecar holds the CSR of records[:n]
+        self._row2rec = None
+        self._n_deleted = 0
         self._dirty = False
+
+    def _dev_labels(self, n_dev: int) -> np.ndarray:
+        """int32 failure-type label of the first ``n_dev`` device rows (main + tail), -1 for a deleted row."""
+        if self._row2rec is None:
+            return self._row_labels(0, n_dev)
+        rec_labels = self._row_labels(0, self._n_indexed)
+        out = np.full(n_dev, -1, dtype=np.int32)
+        live = self._row2rec >= 0
+        out[live] = rec_labels[self._row2rec[live]]
+        return out
+
+    def _to_records(self, rows: np.ndarray) -> np.ndarray:
+        """Device rows -> record indices (-1 stays -1)."""
+        if self._row2rec is None:
+            return rows
+        return np.where(rows >= 0, self._row2rec[np.clip(rows, 0, None)], -1)
 
     def _sync(self) -> None:
         """Bring the device index up to date with ``records`` (called lazily before a query)."""
         if not self._dirty and self._n_indexed == len(self.records):
             return
         pending = [self._index_text(i) for i in range(self._n_indexed, len(self.records))]
-        n_tail = len(self.records) - self._n_main
-        if self._main is None or n_tail > max(self.tail_limit, 0):
+        n_tail = self._n_dev - self._n_main + len(pending)
+        if self._main is None or n_tail > max(self.tail_limit, 0) or self._n_deleted > max(self.tail_limit, 0):
             self.stats["compactions"] += self._main is not None
             self._rebuild_main()
             return
-        if self._tail is None:
+        if self._tail is None and pending:  # a deletion alone needs no tail segment
             self._tail = GfkbIndex(device=self.device, row_base=self._n_main, vocab=self.vocab)
         if pending:
             self._tail.add_texts(pending)
-        self._tail.set_row_labels(self._row_labels(self._n_main, len(self.records)))  # an append dropped them
+            if self._row2rec is not None:
+                self._row2rec = np.concatenate([self._row2rec, np.arange(self._n_indexed, len(self.records), dtype=np.int64)])
+        self._n_dev += len(pending)
         self._n_indexed = len(self.records)
+        segments = [ix for ix in (self._main, self._tail) if ix is not None]
+        if self._tail is not None:
+            tail_labels = self._dev_labels(self._n_dev)[self._n_main:]
+            self._tail.set_row_labels(np.maximum(tail_labels, 0))  # an append dropped them; a deleted row's label is moot
         # global statistics = main + tail (the df all-reduce of a sharded GFKB, done in-process)
         v = len(self.vocab)
         if self._main_df is None:
             self._main_df = self._main.local_df().astype(np.int64)
         df = np.zeros(v, dtype=np.int64)
         df[: len(self._main_df)] = self._main_df
-        df += self._tail.local_df().astype(np.int64)
+        if self._tail is not None:
+            df += self._tail.local_df().astype(np.int64)
         df32 = df.astype(np.uint32)
-        for ix in (self._main, self._tail):
+        for ix in segments:
             ix.set_global_df(df32, len(self.records))
             ix.finalize()
         if self._main.last_finalize_kind == 2:
@@ -287,6 +324,109 @@ class GfkbStore:
             self._dirty = True
             return {"ok": True, "created": created, "failure": rec}
 
+    # -- purge (services/dashboard/app.py:322-375, failures.jsonl only) -----------------------------------------
+    def purge_apps(self, app_ids, backup: bool = True) -> Dict[str, int]:
+        """Remove ``app_ids`` from every record's ``affected_apps`` and drop the records left with none, like the
+        reference's ``_purge_jsonl_apps`` on failures.jsonl: a record counts as "updated" when its list changed and as
+        "removed" when it became empty (both at once is possible), every other record as "kept".  The file is
+        rewritten (after a ``failures.jsonl.bak-<UTC timestamp>`` copy when ``backup``).  The dropped records' device
+        rows are deleted in place; the next query runs a statistics-only finalize, or compacts the main segment once
+        more than ``tail_limit`` rows were deleted since the last rebuild."""
+        purge = set(app_ids)
+        with self._lock:
+            kept = removed = updated = 0
+            keep_idx: List[int] = []
+            for i, rec in enumerate(self.records):
+                apps = rec.get("affected_apps")
+                if "affected_apps" in rec and isinstance(apps, list):
+                    after = [a for a in apps if a not in purge]
+                    if after != apps:
+                        rec["affected_apps"] = after
+                        updated += 1
+                    if not after:
+                        removed += 1
+                        continue
+                keep_idx.append(i)
+                kept += 1
+            if self.path is not None and self.path.exists():
+                if backup:
+                    stamp = self._now().astimezone(timezone.utc).strftime("%Y%m%dT%H%M%SZ")
+                    shutil.copy2(self.path, self.path.with_name(f"{self.path.name}.bak-{stamp}"))
+                lines = [json.dumps(self.records[i], ensure_ascii=False) for i in keep_idx]
+                self.path.write_text("\n".join(lines) + ("\n" if lines else ""), encoding="utf-8")
+            if removed:
+                self._drop_records(keep_idx)
+            return {"kept": kept, "removed": removed, "updated": updated}
+
+    def _drop_records(self, keep_idx: List[int]) -> None:
+        """records := records[keep_idx] (ascending); the dropped records' device rows are deleted."""
+        n_old = len(self.records)
+        keep = np.zeros(n_old, dtype=bool)
+        keep[keep_idx] = True
+        old_texts = [self._index_text(i) for i in range(n_old)] if self.sidecar_path is not None else None
+        # device rows of the indexed records, in record order (monotone), and the new record index of every survivor
+        live_rows = np.flatnonzero(self._row2rec >= 0) if self._row2rec is not None else np.arange(self._n_indexed)
+        new_idx = np.cumsum(keep) - 1
+        gone = live_rows[~keep[: self._n_indexed]]
+        self.records = [self.records[i] for i in keep_idx]
+        self._labels = [lab for i, lab in enumerate(self._labels) if keep[i]]
+        self.quarantined = [int(new_idx[i]) for i in self.quarantined if keep[i]]
+        self._quarantine_set = set(self.quarantined)
+        self.stats["quarantined"] = len(self.quarantined)
+        self._latest = {}
+        for i, r in enumerate(self.records):  # the newest SURVIVING equal record (app.py:108-112)
+            self._latest[(r["failure_type"], r["signature_text"])] = i
+        n_idx_old = self._n_indexed
+        self._n_indexed = int(keep[:n_idx_old].sum())
+        if not self.records or self._main is None:
+            self._rebuild_main()
+        elif len(gone):
+            row2rec = np.full(self._n_dev, -1, dtype=np.int64) if self._row2rec is None else self._row2rec.copy()
+            row2rec[live_rows] = np.where(keep[:n_idx_old], new_idx[:n_idx_old], -1)
+            self._row2rec = row2rec
+            main_rows = gone[gone < self._n_main]
+            if len(main_rows):
+                self._main.delete_rows(main_rows)
+                self._main_df = None  # the main segment's live df changed
+            if self._tail is not None and len(gone) > len(main_rows):
+                self._tail.delete_rows(gone[gone >= self._n_main] - self._n_main)
+            self._n_deleted += len(gone)
+            self._dirty = True
+        if self.sidecar_path is not None:
+            self._rewrite_sidecar(old_texts, keep_idx)
+
+    def _rewrite_sidecar(self, old_texts: List[str], keep_idx: List[int]) -> None:
+        """The sidecar of the surviving records (the vocabulary as it is, their CSR gathered from the old sidecar, the
+        rows it did not hold featurised), so that a restart after a purge still skips the tokenisation; the persisted
+        layout describes the old rows and is removed (the next cold start rebuilds it once).  The store wrote the old
+        sidecar itself (records[:_sidecar_rows]), so it is read without checking its digest again; the cost is one read
+        and one write of the file, a row gather and the digest of the surviving texts, under the store lock."""
+        from .similarity import ArrayBatch, gather_rows
+
+        lay_path = Path(str(self.sidecar_path) + ".layout")
+        if lay_path.exists():
+            lay_path.unlink()
+        texts = [old_texts[i] for i in keep_idx]
+        held = _sidecar.load_arrays(self.sidecar_path)
+        n0 = held[1] if held is not None and held[1] == self._sidecar_rows else 0
+        parts = []
+        if n0:
+            parts.append(gather_rows(held[0], np.asarray([i for i in keep_idx if i < n0], dtype=np.int64)))
+        rest = [t for i, t in zip(keep_idx, texts) if i >= n0]
+        if rest:
+            fb = self.vocab.featurize(rest, grow=True)
+            try:
+                parts.append(ArrayBatch(np.array(fb.indptr), np.array(fb.ids), np.array(fb.tf)))
+            finally:
+                fb.close()
+        indptr = [np.zeros(1, dtype=np.int64)]
+        for p in parts:
+            indptr.append(p.indptr[1:] + indptr[-1][-1])
+        both = ArrayBatch(np.concatenate(indptr), np.concatenate([p.ids for p in parts] or [np.zeros(0, np.uint32)]),
+                          np.concatenate([p.tf for p in parts] or [np.zeros(0, np.uint32)]))
+        _sidecar.save(self.sidecar_path, self.vocab, both, texts)
+        self._sidecar_rows = len(texts)
+
     # -- match (services/gfkb/app.py:79-102) -------------------------------------------------------------------
     def _candidates(self, fb: FeatureBatch, k: int, limit: int = MATCH_LIMIT,
                     labels: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
@@ -307,19 +447,22 @@ class GfkbStore:
         f64 = np.concatenate(f64_all, axis=1)
         big = np.where(rows < 0, np.iinfo(np.int64).max, rows)
         order = np.lexsort((big, -f64), axis=1)  # last key is primary: score descending, then row ascending
-        return np.take_along_axis(rows, order, axis=1), np.take_along_axis(f64, order, axis=1), amb
+        return self._to_records(np.take_along_axis(rows, order, axis=1)), np.take_along_axis(f64, order, axis=1), amb
 
     def _exact_top(self, signature_text: str, limit: int, label: int = -1) -> Tuple[List[int], List[float]]:
         """Rows and float64 scores of the reference's ``sorted(..., reverse=True)[:limit]`` on the full score vector
         (K1a on both segments): no candidate stage at all.  ``label`` >= 0: over the rows of that failure-type label."""
         parts = [ix.score(signature_text) for ix in (self._main, self._tail) if ix is not None and ix.n_rows]
-        scores = np.concatenate(parts)
+        scores = np.concatenate(parts)  # by device row; -inf for a deleted row
         if label >= 0:
-            idx = np.flatnonzero(self._row_labels(0, len(scores)) == label)  # ascending: the stable order is kept
-            order = idx[stable_top(scores[idx], limit)].tolist()
+            idx = np.flatnonzero(self._dev_labels(len(scores)) == label)  # ascending: the stable order is kept
+            order = idx[stable_top(scores[idx], limit)]
+        elif self._row2rec is not None:
+            idx = np.flatnonzero(self._row2rec >= 0)
+            order = idx[stable_top(scores[idx], limit)]
         else:
-            order = stable_top(scores, limit)
-        return order, [float(scores[i]) for i in order]
+            order = np.asarray(stable_top(scores, limit), dtype=np.int64)
+        return self._to_records(order).tolist(), [float(scores[i]) for i in order]
 
     def _match_filter_first(self, signature_texts: Sequence[str], failure_types: Sequence[Optional[str]],
                             limit: int) -> List[List[dict]]:
