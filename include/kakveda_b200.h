@@ -325,7 +325,9 @@ int kv_merge_topk_device_on(int device, const void *d_scores_in, const void *d_r
  * ms[0] = H2D of the query batch, ms[1] = bound + scan kernels, ms[2] = merge (+ fallbacks), ms[3] = D2H. */
 int kv_index_last_timing(const kv_index *ix, float ms[4]);
 /* ... and of its kernels: ms[0] = bound pass 0 (seeds; wgmma GEMM + rare-feature join), ms[1] = seed scan,
- * ms[2] = bound pass 1 (candidate lists), ms[3] = candidate scan, ms[4] = merge.  Exhaustive mode: only [3], [4].
+ * ms[2] = bound pass 1 (candidate lists; when the bound codes of pass 0 were kept, only the snapshot of the
+ * threshold codes: the scan selects its candidates from the codes), ms[3] = candidate scan, ms[4] = merge.
+ * Exhaustive mode: only [3], [4].
  * After kv_range_resident: see there. */
 int kv_index_last_kernel_ms(const kv_index *ix, float ms[5]);
 /* Test hook: runs the resident batch once and returns the numerators (dot-product upper bounds) the bound kernel formed

@@ -32,7 +32,7 @@
 //   * epilogue (16 warps, four threads per query, 16 chunk columns of R each): bound vs the query's threshold.
 //     pass 0 keeps, per thread, the 4 best chunks by bound (16 seeds per query: K1b-S scores them first, which gives
 //     every query a close lower bound theta0 of its k-th best score) and stores every bound as an 8-bit code rounded up
-//     (the selection kernel below builds the candidate lists from the codes); pass 1 (only when the codes do not fit in
+//     (the candidate scan selects its candidates from the codes, against threshold_codes_kernel's snapshot); pass 1 (only when the codes do not fit in
 //     memory) recomputes the bounds and appends {chunk, mask of the group's surviving queries} to the scan group's
 //     candidate list (paged pool) for every chunk with ub >= theta0.
 // One CTA = one 128-query tile x one range of 64-chunk blocks; 20 warps: 16 workers (join + epilogue) and the MMA +
@@ -557,76 +557,21 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
 }
 
 // ----------------------------------------------------------------------------------------
-// K1b-B2: candidate lists from the stored 8-bit bound codes (second pass without recomputing the bounds).  One CTA =
-// one scan group (32 queries = the lanes) x one chunk range; a warp reads, per query, 32 codes (one 32-byte sector) and
-// compares them with the query's threshold code; ballots give the group's query mask per chunk; non-empty masks are
-// appended to the group's paged candidate list by the same list_append as K1b-B's pass 1.  HBM-bound: n_q x chunks bytes read once.
+// K1b-B2: threshold codes of the candidate scan's codes mode (second pass without recomputing the bounds).  A chunk is
+// a candidate of a query when its stored bound code reaches floor(UBQ_SCALE x the query's threshold) -- the threshold
+// as it stands after the seed scan (and the threshold exchange of a two-phase batch), snapshotted here because the scan
+// raises gthr while it selects: every CTA of a group then selects the same candidates, run after run.  256: the query
+// takes no candidate (null or irregular: answered elsewhere).
 // ----------------------------------------------------------------------------------------
-struct SelectParams {
-  const unsigned char *ubq;
-  int64_t ubq_stride, n_chunks, n_q;
-  const float *q_nq;
-  const int *gthr;
-  int n_bsplits;
-  CandLists lists;
-  unsigned long long *stats;
-  const int *q_label;                   // FILTER: [n_q] label filter by sorted slot, -1 = any (kv_query_set_filter)
-  const unsigned long long *chunk_sig;  // FILTER: [n_chunks_pad] chunk label signatures
-};
-
-constexpr int SEL_WARPS = 8;
-
-// FILTER: a chunk joins a filtered query's mask only when its label signature holds the query's label bit as well --
-// with few allowed rows among the seeds the threshold stays at 0 and the code test alone would pass every chunk
-template <bool FILTER>
-__global__ void __launch_bounds__(SEL_WARPS * 32) tfidf_select_kernel(SelectParams P) {
-  extern __shared__ int s_pages[];  // [max_pages]
-  __shared__ unsigned int s_count;
-  const int group = blockIdx.x, bsplit = blockIdx.y;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int list = group * P.n_bsplits + bsplit;
-  for (int i = threadIdx.x; i < P.lists.max_pages; i += blockDim.x) s_pages[i] = -1;
-  if (threadIdx.x == 0) s_count = 0;
-  __syncthreads();
-  const int64_t slot = (int64_t)group * GROUP_Q + lane;
-  const bool q_ok = slot < P.n_q && P.q_nq[slot] > 0.f;
-  uint32_t tcode = 256;  // never reached: the query takes no candidates
-  if (q_ok) {
-    const float th = __int_as_float(P.gthr[slot]);
-    tcode = th > 0.f ? (uint32_t)fminf(255.f, floorf(th * UBQ_SCALE)) : 0u;
+__global__ void threshold_codes_kernel(const float *__restrict__ q_nq, const int *__restrict__ gthr, int64_t n_q, int *tcode) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n_q) return;
+  uint32_t t = 256;
+  if (q_nq[i] > 0.f) {
+    const float th = __int_as_float(gthr[i]);
+    t = th > 0.f ? (uint32_t)fminf(255.f, floorf(th * UBQ_SCALE)) : 0u;
   }
-  // the chunk range of this split, in units of 32 chunks, interleaved over the warps
-  const int64_t n_blocks = (P.n_chunks + B_BN - 1) / B_BN;
-  const int64_t c_lo = (n_blocks * bsplit / P.n_bsplits) * B_BN, c_hi = min(P.n_chunks, (n_blocks * (bsplit + 1) / P.n_bsplits) * B_BN);
-  const unsigned char *row = P.ubq + (size_t)min(slot, P.n_q - 1) * P.ubq_stride;
-  unsigned long long qbit = 0;  // FILTER: the query's label bit, every bit when it is not filtered
-  if constexpr (FILTER) {
-    const int lb = q_ok ? P.q_label[slot] : -1;
-    qbit = lb < 0 ? ~0ull : 1ull << (lb & 63);
-  }
-  unsigned int n_pairs = 0, n_recs = 0;
-  for (int64_t c = c_lo + 32 * warp; c < c_hi; c += 32 * SEL_WARPS) {
-    const uint4 a = __ldcs(reinterpret_cast<const uint4 *>(row + c)), b = __ldcs(reinterpret_cast<const uint4 *>(row + c + 16));
-    const uint32_t wds[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-    unsigned long long sig = 0;  // FILTER: signature of chunk c + lane
-    if constexpr (FILTER) sig = c + lane < c_hi ? P.chunk_sig[c + lane] : 0ull;
-    uint32_t mymask = 0;
-#pragma unroll
-    for (int j = 0; j < 32; j++) {
-      const uint32_t code = (wds[j >> 2] >> ((j & 3) * 8)) & 0xFFu;
-      bool take = q_ok && code >= tcode && c + j < c_hi;
-      if constexpr (FILTER) {
-        const unsigned long long sig_j = __shfl_sync(FULL, sig, j);  // every lane: not under the condition above
-        take = take && (sig_j & qbit) != 0ull;
-      }
-      const uint32_t m = __ballot_sync(FULL, take);
-      if (lane == j) mymask = m;
-    }
-    list_append(P.lists, list, &s_count, s_pages, (uint32_t)(c + lane), mymask, n_pairs, n_recs);
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) P.lists.count[list] = s_count;
-  flush_list_stats(P.stats, n_pairs, n_recs);
+  tcode[i] = (int)t;
 }
 
 }  // namespace kvk

@@ -114,6 +114,7 @@ struct kv_index {
   DevBuf<uint32_t> d_list_count, d_list_pages;
   DevBuf<unsigned int> d_pool_ctl;  // [0] pages handed out, [1] overflow flag
   DevBuf<unsigned char> d_ubq;      // 8-bit bound codes of a batch, [n_q][n_chunks_pad] (when they fit)
+  DevBuf<int> d_tcode;              // threshold code per query of the scan of the codes (threshold_codes_kernel)
   int last_used_codes = 0;
   int64_t pool_pages = 0;
   // cross-GPU threshold exchange (row-sharded GFKB): d_gthr is exported over CUDA IPC, the peers' arrays are mapped here
@@ -1158,7 +1159,7 @@ struct Batch {
   int k, phase;
   float *out_s;  // the outputs, [n_q][k] by original query
   long long *out_r;
-  int64_t n_q, n_tiles, n_groups, n_bsplits, n_ssplits, n_ssplits_a, n_parts;
+  int64_t n_q, n_tiles, n_groups, n_bsplits, n_ssplits, n_ssplits_a, n_csplits, n_parts;
   int max_pages, n_seed, n_peers;
   bool prune, use_codes, range = false;
   int64_t launches = 0;
@@ -1199,18 +1200,24 @@ static int launch_scan(kv_index *ix, const Batch &b, const ScanParams &SP, dim3 
   return KV_OK;
 }
 
-// The scan of the candidate lists bound pass 1 or the selection kernel built
+// The scan of the candidates: of the lists bound pass 1 built, or, when the bound codes were kept, of the chunks whose
+// codes reach the threshold codes (selected in the scan kernel, n_csplits CTAs per group)
 static int scan_candidates(kv_index *ix, Batch &b) {
   ScanParams SP = scan_params(ix, b);
+  b.launches++;
+  if (b.use_codes) {
+    SP.list_mode = 3; SP.ubq = ix->d_ubq.p; SP.ubq_stride = ix->n_chunks_pad; SP.tcode = ix->d_tcode.p;
+    SP.n_bsplits = 1; SP.n_ssplits = (int)b.n_csplits;
+    return launch_scan(ix, b, SP, dim3((unsigned)b.n_groups, (unsigned)b.n_csplits));
+  }
   SP.list_mode = 0; SP.list_count = ix->d_list_count.p + b.n_groups; SP.list_pages = ix->d_list_pages.p; SP.pool = ix->d_pool.p;
   SP.n_bsplits = (int)b.n_bsplits; SP.n_ssplits = (int)b.n_ssplits;
-  b.launches++;
   return launch_scan(ix, b, SP, dim3((unsigned)(b.n_groups * b.n_bsplits), (unsigned)b.n_ssplits));
 }
 
 // Pruned path.  Phase 0 / 1: bound pass 0 (seeds and bound codes) -> seed scan; phase 1 ends with the seed top-k.
-// Phase 0 / 2: candidate lists -- from the stored codes when they were kept, else by recomputing the bounds (pass 1) --
-// then the scan of the candidates into b.n_parts partial lists.
+// Phase 0 / 2: the scan of the candidates into b.n_parts partial lists -- selected from the stored codes by the scan
+// itself when they were kept (after a snapshot of the threshold codes), else listed by recomputing the bounds (pass 1).
 static int run_pruned(kv_index *ix, Batch &b) {
   cudaStream_t s = ix->stream;
   const float *qc = ix->d_qconst.p; const int64_t n_q = b.n_q;
@@ -1258,14 +1265,7 @@ static int run_pruned(kv_index *ix, Batch &b) {
   }
   if (b.phase == 2) KV_CUDA(cudaEventRecord(ix->evp2, s));  // the caller's threshold exchange sits between evk[2] and this point
   if (b.use_codes) {
-    SelectParams LP;
-    LP.ubq = ix->d_ubq.p; LP.ubq_stride = ix->n_chunks_pad; LP.n_chunks = ix->n_chunks; LP.n_q = n_q;
-    LP.q_nq = qc; LP.gthr = ix->d_gthr.p; LP.n_bsplits = (int)b.n_bsplits; LP.lists = BP.lists; LP.stats = BP.stats;
-    LP.q_label = ix->d_filt_sorted.p; LP.chunk_sig = ix->d_chunk_sig.p;
-    const dim3 sgrid((unsigned)b.n_groups, (unsigned)b.n_bsplits);
-    const size_t s_smem = (size_t)b.max_pages * sizeof(int);
-    if (ix->has_filter) tfidf_select_kernel<true><<<sgrid, SEL_WARPS * 32, s_smem, s>>>(LP);
-    else tfidf_select_kernel<false><<<sgrid, SEL_WARPS * 32, s_smem, s>>>(LP);
+    threshold_codes_kernel<<<(unsigned)((n_q + 255) / 256), 256, 0, s>>>(qc, ix->d_gthr.p, n_q, ix->d_tcode.p);
   } else {
     BP.pass = 1;
     tfidf_bound_kernel<false><<<bgrid, B_THREADS, b_smem, s>>>(ix->map_w, ix->map_w2, ix->map_u, BP);
@@ -1314,6 +1314,8 @@ static int run_jaccard(kv_index *ix, Batch &b) {
   return KV_OK;
 }
 
+constexpr int64_t CODE_SPLIT_CTAS = 64;  // scan of the stored codes: aim for this many CTAs per SM (32 waves at 2 CTAs/SM)
+
 // Splits of the resident batch, pruned or exhaustive path, and the buffers of the candidate lists: sets b's sizes,
 // b.prune and the last_* launch counts.  Shared by the top-k batch and the threshold search.
 static int size_batch(kv_index *ix, Batch &b) {
@@ -1336,6 +1338,11 @@ static int size_batch(kv_index *ix, Batch &b) {
   }
   const int64_t n_lists = n_groups * n_bsplits;
   b.n_parts = n_bsplits * n_ssplits;
+  // scan of the stored codes (run_batch decides whether they are kept): CTAs per group over the group's windows of
+  // chunks, so that the grid spans many waves and the groups with the most candidates do not form the tail
+  const int64_t n_windows = (ix->n_chunks + S_WIN - 1) / S_WIN;
+  b.n_csplits = std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>((CODE_SPLIT_CTAS * ix->sm_count + n_groups - 1) / n_groups, 8), n_windows));
+  if (const char *e = getenv("KAKVEDA_B200_CODE_SPLITS")) b.n_csplits = std::max(1, atoi(e));  // tests: a forced split count
   b.n_ssplits_a = std::max<int64_t>(1, std::min<int64_t>((4LL * ix->sm_count + n_groups - 1) / n_groups, 8));
   ix->last_tiles = n_tiles; ix->last_splits = b.n_parts; ix->last_ctas = n_lists * n_ssplits;
   KV_CUDA(ix->d_stats.ensure(8));
@@ -1343,6 +1350,7 @@ static int size_batch(kv_index *ix, Batch &b) {
   const int64_t chunks_per_split = ((n_blocks + n_bsplits - 1) / n_bsplits + 1) * B_BN;
   b.max_pages = (int)(chunks_per_split / PAGE_RECS + 2);
   if (prune) {
+    KV_CUDA(ix->d_tcode.ensure(n_q));
     KV_CUDA(ix->d_seeds.ensure(n_q * b.n_seed));
     KV_CUDA(ix->d_direct.ensure(n_groups * GROUP_Q * b.n_seed));
     // the bound kernel writes the lists of whole tiles (4 groups each), including the groups past the last query
@@ -1382,7 +1390,7 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
                                  "(kv_index_thresholds_export / kv_index_thresholds_peers)");
   KV_CUDA(ix->d_gthr.ensure(n_q));
   b.n_peers = (ix->n_peers > 0 && n_q <= ix->peer_cap) ? ix->n_peers : 0;
-  const int64_t parts_alloc = std::max(b.n_parts, b.n_ssplits_a);
+  const int64_t parts_alloc = std::max({b.n_parts, b.n_ssplits_a, b.n_csplits});
   KV_CUDA(ix->d_part_s.ensure(parts_alloc * n_q * k));
   KV_CUDA(ix->d_part_r.ensure(parts_alloc * n_q * k));
   // Second pass without recomputation: the first bound pass stores every bound as an 8-bit code (n_q x chunks bytes)
@@ -1404,6 +1412,10 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
     }
   }
   if (phase != 2) ix->last_used_codes = b.use_codes ? 1 : 0;
+  if (b.use_codes) {
+    b.n_parts = b.n_csplits;
+    ix->last_splits = b.n_parts; ix->last_ctas = b.n_groups * b.n_csplits;
+  }
 
   if (phase != 2) {
     KV_CUDA(cudaEventRecord(ix->ev[1], s));

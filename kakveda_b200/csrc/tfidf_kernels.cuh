@@ -571,6 +571,10 @@ __host__ __device__ __forceinline__ uint32_t rt_slot(uint32_t fid, uint32_t size
 // completion; double buffered, so the next block lands while this one is scored) and scores it for each query of the
 // mask: lanes probe 32 block entries at a time in the query's table, hits add their fixed-point weights to the rows
 // of their masks, lane = row.  Survivors of the division-free pre-test enter the query's sorted list under a lock.
+// In the codes mode (list_mode 3) the records are not read from a list: a warp takes a window of S_WIN chunks, each
+// lane reads its query's S_WIN stored bound codes, and a ballot per chunk gives the chunk's query mask -- the warp
+// loads the codes of its next window before it scores the records of this one, so the n_q x chunks bytes of codes
+// stream in behind the scoring instead of in a separate selection pass that writes the lists to memory.
 // K1b-R (RANGE = true) is the same scan for a threshold search: the filter is the query's fixed threshold and every
 // row that reaches it is appended to a global pair buffer instead of a top-k list.
 // ----------------------------------------------------------------------------------------
@@ -595,8 +599,13 @@ struct ScanParams {
   int *peer_gthr[7];                      // the same array on the other GPUs of a row-sharded GFKB (peer memory over
   int n_peers;                            //   NVLink): a raised bound is pushed to every shard, so all of them prune with it
   // candidate lists: list l = group * n_bsplits + bsplit.  mode 0: paged pool, 1: fixed stride (seed lists),
-  // 2: every chunk of the list's chunk range x every query of the group (exhaustive)
+  // 2: every chunk of the list's chunk range x every query of the group (exhaustive), 3: built in the kernel from the
+  // stored bound codes (top-k scan only; n_bsplits 1, the CTAs of a group split its windows of S_WIN chunks)
   int list_mode;
+  const unsigned char *ubq;     // mode 3: [n_q][ubq_stride] 8-bit bound codes of bound pass 0
+  int64_t ubq_stride;
+  const int *tcode;             // mode 3: [n_q] code a chunk's bound needs for the query to take it, 256: none
+                                //   (threshold_codes_kernel: a snapshot, fixed while the scan raises gthr)
   const uint32_t *list_count;   // [n_lists]
   const uint32_t *list_pages;   // [n_lists][max_pages]
   int max_pages;
@@ -604,7 +613,8 @@ struct ScanParams {
   const uint2 *direct;          // mode 1: [n_lists][direct_stride]
   int direct_stride;
   int n_bsplits, n_ssplits;
-  unsigned long long *stats;    // [0] (query, chunk) pairs scored, [1] records
+  unsigned long long *stats;    // [0] (query, chunk) pairs scored, [1] records; mode 3 also [2] pairs and [3] records
+                                //   that passed the bound (as list_append counts them)
   int64_t n_q;
   int k;
   float *part_scores;  // [n_bsplits * n_ssplits][n_q][k]
@@ -633,6 +643,7 @@ __device__ __forceinline__ void range_emit(RangePair *out, unsigned long long *c
 constexpr int S_WARPS = 8;
 constexpr int S_BUF_ENTRIES = 256;  // a staged block holds up to this many entries (larger blocks are read in place)
 constexpr int S_BUF_BYTES = S_BUF_ENTRIES * 8;
+constexpr int S_WIN = 64;  // codes mode: chunks per window (a lane loads its query's S_WIN codes as four 16-byte loads)
 
 struct ScanHit {
   uint32_t m, c_lo, w_lo, w_hi;  // c fits 32 bits for tf <= 2 ... kept 64-bit via c_hi below
@@ -664,7 +675,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   int *s_excl = (int *)(s_corrU + GROUP_Q);
   int *s_qlab = s_excl + GROUP_Q;                                           // [GROUP_Q] label filter, -1 = any
   unsigned int *s_next = (unsigned int *)(s_qlab + GROUP_Q);                // [1] next record of this CTA's range
-  unsigned int *s_stat = s_next + 1;                                        // [2]
+  unsigned int *s_stat = s_next + 1;                                        // [4]
 
   const int list = blockIdx.x, ssplit = blockIdx.y;
   const int group = list / P.n_bsplits, bsplit = list - group * P.n_bsplits;
@@ -672,11 +683,15 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   const int q_count = (int)min((int64_t)GROUP_Q, P.n_q - q0);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const uint32_t lt = lanemask_lt();
+  bool codes = false;  // list_mode 3
+  if constexpr (!RANGE) codes = P.list_mode == 3;
 
-  // record range of this CTA
+  // record range of this CTA (codes mode: a range of windows)
   uint32_t n_rec;
   int64_t c_lo = 0;
-  if (P.list_mode == 2) {
+  if (codes) {
+    n_rec = (uint32_t)((P.n_chunks + S_WIN - 1) / S_WIN);
+  } else if (P.list_mode == 2) {
     c_lo = P.n_chunks * bsplit / P.n_bsplits;
     n_rec = (uint32_t)(P.n_chunks * (bsplit + 1) / P.n_bsplits - c_lo);
   } else {
@@ -709,7 +724,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
       s_excl[qi] = (ok && P.q_excl) ? P.q_excl[q0 + qi] : -1;
       s_qlab[qi] = (ok && P.q_label) ? P.q_label[q0 + qi] : -1;
     }
-    if (threadIdx.x == 0) { *s_next = r_lo; s_stat[0] = s_stat[1] = 0; }
+    if (threadIdx.x == 0) { *s_next = r_lo; s_stat[0] = s_stat[1] = s_stat[2] = s_stat[3] = 0; }
     if (lane == 0) {
       mbar_init(&s_bar[warp * 2], 1);
       mbar_init(&s_bar[warp * 2 + 1], 1);
@@ -773,22 +788,113 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
     return true;
   };
 
+  // Codes mode: the warp's window state.  A lane reads the codes of query q0 + lane (lanes past the group read the
+  // last query's row and take nothing); tq = 256 takes nothing.
+  uint32_t tq = 256;
+  unsigned long long qbit = ~0ull;  // the query's label bit (label filter), every bit when it is not filtered
+  const unsigned char *crow = nullptr;
+  uint4 wraw[S_WIN / 16];            // codes of window w_nxt (in flight while the current window's records are scored)
+  uint32_t w_nxt = 0;
+  int64_t wbase = 0;                 // first chunk of the current window
+  uint32_t wm[S_WIN / 32] = {};      // lane j: query mask of chunk wbase + 32 i + j
+  unsigned long long pend = 0;       // chunks of the current window with a record not yet taken
+  unsigned int sel_pairs = 0, sel_recs = 0;
+  auto load_window = [&](uint32_t w) {
+#pragma unroll
+    for (int i = 0; i < S_WIN / 16; i++) wraw[i] = __ldcs(reinterpret_cast<const uint4 *>(crow + (size_t)w * S_WIN) + i);
+  };
+  if (codes) {
+    if (lane < q_count) tq = (uint32_t)P.tcode[q0 + lane];
+    crow = P.ubq + (size_t)(q0 + min(lane, q_count - 1)) * P.ubq_stride;
+    if (P.q_label && s_qlab[lane] >= 0) qbit = 1ull << (s_qlab[lane] & 63);
+    w_nxt = grab();
+    if (w_nxt < r_hi) load_window(w_nxt);
+  }
+  // Next record of a codes-mode warp.  When the current window is used up, window w_nxt becomes current: its codes are
+  // compared with the threshold codes (the same test, in the same order, as bound pass 1's survivors: code >= tq, chunk
+  // in range, label signature), the next window's loads are issued, and a ballot per chunk transposes the comparisons
+  // into query masks.  Pairs and records are counted before the live-word test, as list_append counts them.
+  auto next_code_record = [&](int64_t &chunk, uint32_t &mask) -> bool {
+    while (pend == 0) {
+      if (w_nxt >= r_hi) return false;
+      wbase = (int64_t)w_nxt * S_WIN;
+      const uint32_t t4 = tq < 256 ? tq * 0x01010101u : 0u;
+      uint32_t ge[S_WIN / 4];  // byte i of ge[j]: 0xFF when the code of chunk wbase + 4 j + i reaches tq
+      bool any = false;
+#pragma unroll
+      for (int i = 0; i < S_WIN / 16; i++) {
+        const uint32_t v[4] = {wraw[i].x, wraw[i].y, wraw[i].z, wraw[i].w};
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+          ge[4 * i + j] = tq < 256 ? __vcmpgeu4(v[j], t4) : 0u;
+          any |= ge[4 * i + j] != 0u;
+        }
+      }
+      w_nxt = grab();
+      if (w_nxt < r_hi) load_window(w_nxt);
+#pragma unroll
+      for (int i = 0; i < S_WIN / 32; i++) wm[i] = 0;
+      if (!__any_sync(FULL, any)) continue;
+      if (P.q_label) {
+#pragma unroll
+        for (int i = 0; i < S_WIN / 32; i++) {
+          const unsigned long long sig = P.chunk_sig[wbase + 32 * i + lane];
+#pragma unroll
+          for (int j = 0; j < 32; j++) {
+            const unsigned long long sig_j = __shfl_sync(FULL, sig, j);
+            const bool take = ((ge[8 * i + (j >> 2)] >> ((j & 3) * 8)) & 1u) && (sig_j & qbit) != 0ull;
+            const uint32_t m = __ballot_sync(FULL, take);
+            if (lane == j) wm[i] = m;
+          }
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < S_WIN / 32; i++)
+#pragma unroll
+          for (int j = 0; j < 32; j++) {
+            const uint32_t m = __ballot_sync(FULL, (ge[8 * i + (j >> 2)] >> ((j & 3) * 8)) & 1u);
+            if (lane == j) wm[i] = m;
+          }
+      }
+      pend = 0;
+#pragma unroll
+      for (int i = 0; i < S_WIN / 32; i++) {
+        const int64_t c = wbase + 32 * i + lane;
+        if (c >= P.n_chunks) wm[i] = 0;
+        sel_pairs += (unsigned int)__popc(wm[i]);
+        sel_recs += wm[i] != 0u;
+        if (P.alive && P.alive[c] == 0u) wm[i] = 0;  // every row of the chunk deleted: never staged
+        pend |= (unsigned long long)__ballot_sync(FULL, wm[i] != 0u) << (32 * i);
+      }
+    }
+    const int i = __ffsll((long long)pend) - 1;
+    pend &= pend - 1;
+    chunk = wbase + i;
+    uint32_t m = wm[0];
+#pragma unroll
+    for (int j = 1; j < S_WIN / 32; j++)
+      if ((i >> 5) == j) m = wm[j];
+    mask = __shfl_sync(FULL, m, i & 31);
+    return true;
+  };
+  auto next_record = [&](int64_t &chunk, uint32_t &mask) -> bool {
+    if (codes) return next_code_record(chunk, mask);
+    const uint32_t r = grab();
+    if (r >= r_hi) return false;
+    fetch(r, chunk, mask);
+    return true;
+  };
+
   unsigned int pairs_done = 0, recs_done = 0;
-  uint32_t r_cur = grab();
   int64_t chunk_cur = 0, chunk_nxt = 0;
   uint32_t mask_cur = 0, mask_nxt = 0;
   bool staged_cur = false, staged_nxt = false;
   int b = 0;
-  if (r_cur < r_hi) {
-    fetch(r_cur, chunk_cur, mask_cur);
-    staged_cur = mask_cur ? issue(chunk_cur, b) : false;
-  }
-  while (r_cur < r_hi) {
-    const uint32_t r_nxt = grab();
-    if (r_nxt < r_hi) {
-      fetch(r_nxt, chunk_nxt, mask_nxt);
-      staged_nxt = mask_nxt ? issue(chunk_nxt, b ^ 1) : false;
-    }
+  bool have_cur = next_record(chunk_cur, mask_cur);
+  if (have_cur) staged_cur = mask_cur ? issue(chunk_cur, b) : false;
+  while (have_cur) {
+    const bool have_nxt = next_record(chunk_nxt, mask_nxt);
+    if (have_nxt) staged_nxt = mask_nxt ? issue(chunk_nxt, b ^ 1) : false;
     if (mask_cur) {
       const BlockInfo bi = P.binfo[chunk_cur];
       const int E = bi.n_entries, E4 = (E + 3) & ~3;
@@ -930,7 +1036,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
       }
     }
     __syncwarp();  // every lane is done with buffer b before a later copy may overwrite it
-    r_cur = r_nxt;
+    have_cur = have_nxt;
     chunk_cur = chunk_nxt;
     mask_cur = mask_nxt;
     staged_cur = staged_nxt;
@@ -939,6 +1045,10 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   if (lane == 0) {
     atomicAdd(&s_stat[0], pairs_done);
     atomicAdd(&s_stat[1], recs_done);
+  }
+  if (sel_recs) {
+    atomicAdd(&s_stat[2], sel_pairs);
+    atomicAdd(&s_stat[3], sel_recs);
   }
   __syncthreads();
   if constexpr (!RANGE) {  // publish this CTA's partial lists (already ordered)
@@ -954,12 +1064,16 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   if (threadIdx.x == 0 && P.stats) {
     atomicAdd(&P.stats[0], (unsigned long long)s_stat[0]);
     atomicAdd(&P.stats[1], (unsigned long long)s_stat[1]);
+    if (codes) {
+      atomicAdd(&P.stats[2], (unsigned long long)s_stat[2]);
+      atomicAdd(&P.stats[3], (unsigned long long)s_stat[3]);
+    }
   }
 }
 
 static inline size_t scan_smem_bytes(int k) {
   return (size_t)GROUP_Q * QTAB_BYTES + (size_t)S_WARPS * 2 * S_BUF_BYTES + (size_t)S_WARPS * 32 * sizeof(ScanHit) +
-         (size_t)S_WARPS * 2 * 8 + (size_t)GROUP_Q * k * 8 + (size_t)GROUP_Q * 4 * 7 + 16;
+         (size_t)S_WARPS * 2 * 8 + (size_t)GROUP_Q * k * 8 + (size_t)GROUP_Q * 4 * 7 + 32;
 }
 
 // ----------------------------------------------------------------------------------------
