@@ -334,6 +334,19 @@ int kv_index_last_kernel_ms(const kv_index *ix, float ms[5]);
  * for every (query slot, chunk): out[n_q][chunks] floats, slot_query[i] = original query of sorted slot i.  Needs an
  * index large enough for the pruned path (>= 512 chunks of 32 rows); tests/test_gpu_parity.py compares with NumPy. */
 int kv_debug_bound_numerators(kv_index *ix, int k, float *out, int32_t *slot_query);
+/* Test hook: runs the resident batch once, as kv_topk_resident does (same bound-kernel instantiation: the specialised
+ * one, or the generic one under KAKVEDA_B200_GENERIC_BOUND=1), and returns what bound pass 0 produced, by sorted query
+ * slot i (original query slot_query[i]):
+ *   codes[n_q][chunks]    the 8-bit bound codes the candidate scan selected from;
+ *   tcode[n_q]            the threshold codes it compared them with (256: the query takes no candidate);
+ *   q_terms[n_q][4]       the query constants of the bound: |q|^2, dotS, dotX, corrS;
+ *   chunk_minB[chunks]    the smallest positive live row norm per chunk (+inf: none);
+ *   row_at_pos[n_rows]    the local row at each scan position (chunk c = positions 32c .. 32c + 31).
+ * codes and slot_query are required, the other outputs may be NULL.  kv_index_layout describes this run afterwards.
+ * KV_ERR_STATE when no batch is uploaded or the run kept no codes (exhaustive path below 512 chunks,
+ * KAKVEDA_B200_BOUND_CODES=0, codes too large for the device, Jaccard mode). */
+int kv_debug_bound_codes(kv_index *ix, int k, uint8_t *codes, int32_t *slot_query, int32_t *tcode, float *q_terms,
+                         float *chunk_minB, int32_t *row_at_pos);
 /* Test hook: orders n caller-built range records (host memory, 16 bytes each, the layout the range scans emit) on
  * `device` with the code the fetch functions use, so that inputs a real search cannot cheaply produce can be checked.
  * jaccard = 0: records {int32 q, float32 score, int64 row} (rows global, row_base ignored); jaccard != 0: {int32 q,

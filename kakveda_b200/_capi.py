@@ -94,6 +94,8 @@ SIGNATURES = {
     "kv_index_last_kernel_ms": (C.c_int, [C.c_void_p, c_f32p]),
     "kv_index_last_score_ms": (C.c_int, [C.c_void_p, c_f32p]),
     "kv_debug_bound_numerators": (C.c_int, [C.c_void_p, C.c_int, c_f32p, C.POINTER(C.c_int32)]),
+    "kv_debug_bound_codes": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_uint8), C.POINTER(C.c_int32),
+                                       C.POINTER(C.c_int32), c_f32p, c_f32p, C.POINTER(C.c_int32)]),
     "kv_index_layout": (C.c_int, [C.c_void_p, c_i64p, c_i64p]),
     "kv_index_layout_save": (C.c_int, [C.c_void_p, C.c_char_p]),
     "kv_index_layout_load": (C.c_int, [C.c_void_p, C.c_char_p]),

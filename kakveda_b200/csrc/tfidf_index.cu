@@ -2098,6 +2098,49 @@ int kv_debug_bound_numerators(kv_index *ix, int k, float *out, int32_t *slot_que
   return rc;
 }
 
+// Test hook: what bound pass 0 of the resident batch produced on the headline path (no dbg_xs, so the instantiation is
+// the one kv_topk_resident picks): the 8-bit codes and threshold codes the candidate scan compared, the query constants
+// and chunk minima the bounds were formed from, and the scan layout's row order.
+int kv_debug_bound_codes(kv_index *ix, int k, uint8_t *codes, int32_t *slot_query, int32_t *tcode, float *q_terms,
+                         float *chunk_minB, int32_t *row_at_pos) {
+  if (!ix || !codes || !slot_query) return kv_fail(KV_ERR_INVALID, "kv_debug_bound_codes: bad arguments");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_debug_bound_codes: no query batch uploaded");
+  KV_CUDA(cudaSetDevice(ix->device));
+  const int64_t n_q = ix->batch_q;
+  KV_CUDA(ix->d_out_s.ensure(n_q * k)); KV_CUDA(ix->d_out_r.ensure(n_q * k));
+  int rc = run_batch(ix, k, ix->d_out_s.p, ix->d_out_r.p);
+  if (rc != KV_OK) return rc;
+  KV_CUDA(cudaEventRecord(ix->ev[4], ix->stream));
+  KV_CUDA(cudaStreamSynchronize(ix->stream));
+  if ((rc = finish_batch(ix)) != KV_OK) return rc;
+  if (!ix->last_used_codes) {
+    const char *np = getenv("KAKVEDA_B200_NO_PRUNE"), *ce = getenv("KAKVEDA_B200_BOUND_CODES");
+    const char *why = ix->jaccard ? "a Jaccard index has no bound pass"
+                      : (np && np[0] == '1') || ix->n_chunks < 512 ? "the exhaustive path ran (fewer than 512 chunks or KAKVEDA_B200_NO_PRUNE=1)"
+                      : (ce && ce[0] == '0') ? "KAKVEDA_B200_BOUND_CODES=0: bound pass 1 recomputed the bounds"
+                                             : "the codes did not fit in device memory";
+    return kv_fail(KV_ERR_STATE, "kv_debug_bound_codes: the run kept no bound codes (%s)", why);
+  }
+  const int64_t nch = ix->n_chunks;
+  KV_CUDA(cudaMemcpy2D(codes, (size_t)nch, ix->d_ubq.p, (size_t)ix->n_chunks_pad, (size_t)nch, (size_t)n_q, cudaMemcpyDeviceToHost));
+  for (int64_t i = 0; i < n_q; i++) slot_query[i] = ix->h_qperm.p[i];
+  if (tcode) KV_CUDA(cudaMemcpy(tcode, ix->d_tcode.p, (size_t)n_q * sizeof(int), cudaMemcpyDeviceToHost));
+  if (q_terms) {
+    std::vector<float> qc((size_t)(7 * n_q));
+    KV_CUDA(cudaMemcpy(qc.data(), ix->d_qconst.p, qc.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    for (int64_t i = 0; i < n_q; i++) {  // d_qconst: nq, dotU, corrU, dotS, corrS, dotX, 1 / s_q
+      q_terms[4 * i] = qc[(size_t)i];
+      q_terms[4 * i + 1] = qc[(size_t)(3 * n_q + i)];
+      q_terms[4 * i + 2] = qc[(size_t)(5 * n_q + i)];
+      q_terms[4 * i + 3] = qc[(size_t)(4 * n_q + i)];
+    }
+  }
+  if (chunk_minB) KV_CUDA(cudaMemcpy(chunk_minB, ix->d_cminB.p, (size_t)nch * sizeof(float), cudaMemcpyDeviceToHost));
+  if (row_at_pos && ix->n_rows) KV_CUDA(cudaMemcpy(row_at_pos, ix->d_perm.p, (size_t)ix->n_rows * sizeof(int), cudaMemcpyDeviceToHost));
+  return KV_OK;
+}
+
 int kv_index_last_timing(const kv_index *ix, float ms[4]) {
   if (!ix || !ms) return kv_fail(KV_ERR_INVALID, "kv_index_last_timing: bad arguments");
   for (int i = 0; i < 4; i++) ms[i] = ix->last_ms[i];

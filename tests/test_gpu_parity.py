@@ -578,18 +578,17 @@ def test_bound_kernel_numerators_vs_numpy(lib):
     _capi.check(lib.kv_debug_bound_numerators(ix._h, 16, got.ctypes.data_as(C.POINTER(C.c_float)),
                                               slot_query.ctypes.data_as(C.POINTER(C.c_int32))))
     qfb.close()
-    # NumPy: the scan layout's row order ((norm class, token order), 32 rows per chunk), chunk unions with the max tf
+    # NumPy: chunk unions (32 rows per chunk of the scan layout) with the max tf
     rowof = np.repeat(np.arange(n), np.diff(ip))
     df = np.bincount(ids, minlength=V).astype(np.float64)
     a = (np.log((n + 2) / (df + 2)) + 1) ** 2
-    B32 = np.bincount(rowof, weights=(tf * (np.log((n + 2) / (df + 1)) + 1)[ids]) ** 2, minlength=n).astype(np.float32)
-    L = int(np.diff(ip).max())
-    pad = np.zeros((n, L), dtype=np.int64)
-    pad[rowof, np.arange(len(ids)) - np.repeat(ip[:-1], np.diff(ip))] = ids + 1
-    cls = np.where(B32 > 0, np.floor(np.log2(np.maximum(B32, 1e-30).astype(np.float64)) * 2), -1000).astype(np.int64)
-    perm = np.lexsort([pad[:, j] for j in range(L - 1, -1, -1)] + [cls])
+    # the scan layout's row order, as the index built it (row_at_pos of kv_debug_bound_codes)
+    row_at_pos = np.zeros(n, dtype=np.int32)
+    _capi.check(lib.kv_debug_bound_codes(ix._h, 16, np.zeros((q, nch), dtype=np.uint8).ctypes.data_as(C.POINTER(C.c_uint8)),
+                                         np.zeros(q, dtype=np.int32).ctypes.data_as(C.POINTER(C.c_int32)), None, None,
+                                         None, row_at_pos.ctypes.data_as(C.POINTER(C.c_int32))))
     pos_of = np.empty(n, dtype=np.int64)
-    pos_of[perm] = np.arange(n)
+    pos_of[row_at_pos] = np.arange(n)
     key = (pos_of[rowof] // 32) * V + ids
     o = np.lexsort((tf, key))
     ks = key[o]
