@@ -216,6 +216,24 @@ int kv_selfjoin_upload(kv_index *ix, int64_t q_begin, int64_t q_end);
 int kv_index_set_row_labels(kv_index *ix, const int32_t *labels, int64_t n);
 int kv_query_set_filter(kv_index *ix, const int32_t *labels, int64_t n_q);
 
+/* Distinct top-k (field collapsing).  kv_index_set_row_groups gives every local row a group >= 0 (e.g. one id per
+ * distinct text), groups[n] by local row; validation and lifetime as kv_index_set_row_labels: n == kv_index_rows and
+ * every group >= 0 (else KV_ERR_INVALID), they survive either kind of finalize, kv_index_layout_load and deletions,
+ * kv_index_append drops them, NULL clears.  Setting groups changes no result by itself.
+ * kv_query_set_distinct(ix, 1) switches the resident batch (kv_query_upload / kv_selfjoin_upload) to distinct mode,
+ * 0 back; the next upload switches it off.  A distinct query's top-k, for kv_topk_resident and kv_topk_resident_host:
+ * of the rows it may match (live, not excluded, of its label when filtered) the best row of each group is the first in
+ * (score desc, row asc) order; the groups are ranked by their best rows in that order and the first k best rows are
+ * returned, (-inf, -1) past the last eligible group.  Scores are the float32 values of the non-distinct top-k, so
+ * singleton groups give its result bit for bit, and the zero-score fill and null queries take the first row of each
+ * new group in ascending row order.  kv_range_* ignores distinct mode: a threshold search already returns every pair.
+ * KV_ERR_INVALID: a Jaccard index (mode 1), here or at kv_index_set_row_groups; kv_topk_resident_seed / _finish or
+ * the threshold exchange of a row-sharded GFKB (kv_index_thresholds_*) in distinct mode -- a shard's seed scores are
+ * no lower bound of the global k-th group score, since one group can count on several shards.  KV_ERR_STATE: distinct
+ * mode on an index whose groups are missing or stale (appended rows), here or at the search. */
+int kv_index_set_row_groups(kv_index *ix, const int32_t *groups, int64_t n);
+int kv_query_set_distinct(kv_index *ix, int on);
+
 /* Row deletion (tombstones).  rows[n]: local rows, any order; duplicates and rows already deleted are allowed (a call
  * that deletes no new row changes nothing).  A deleted row keeps its row id and its place in the scan layout but is
  * never returned again by any search on the handle: top-k (seed, candidate and exhaustive scans), threshold search,

@@ -69,6 +69,8 @@ SIGNATURES = {
     "kv_selfjoin_upload": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64]),
     "kv_index_set_row_labels": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int64]),
     "kv_query_set_filter": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int64]),
+    "kv_index_set_row_groups": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int64]),
+    "kv_query_set_distinct": (C.c_int, [C.c_void_p, C.c_int]),
     "kv_index_delete_rows": (C.c_int, [C.c_void_p, c_i64p, C.c_int64]),
     "kv_index_live_rows": (C.c_int64, [C.c_void_p]),
     "kv_index_deleted_rows": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint8), C.c_int64]),
@@ -151,6 +153,12 @@ def load():
 
 def last_error() -> str:
     return load().kv_last_error().decode("utf-8", "replace")
+
+
+def no_distinct(distinct: bool, what: str) -> None:
+    """Distinct top-k (one row per group) is built for the TF-IDF ``GfkbIndex`` only."""
+    if distinct:
+        raise NotImplementedError(f"{what}: distinct top-k (kv_query_set_distinct) is only built for a single GfkbIndex")
 
 
 def check(rc: int) -> None:

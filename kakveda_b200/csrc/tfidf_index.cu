@@ -137,6 +137,12 @@ struct kv_index {
   DevBuf<int> d_filt_sorted, d_filt_orig;
   std::vector<int> h_filt_orig;
   bool has_filter = false;
+  // row groups (kv_index_set_row_groups), by local row; dropped by an append.  On the device (rebuilt by every
+  // finalize): by row (K5, fallbacks, null queries) and by scan position (scan).  Distinct mode of the resident batch
+  // (kv_query_set_distinct), cleared by the next upload.
+  std::vector<int> h_groups;
+  bool has_groups = false, groups_on_device = false, distinct = false;
+  DevBuf<int> d_groups_row, d_group_pos;
   // deleted rows (kv_index_delete_rows), by local row (empty until the first deletion; an append extends it).  They
   // keep their place in the scan layout.  On the device while any row is deleted, rebuilt by every finalize: by row,
   // the live word of every chunk (by scan position) and the first LAB_FIRST live rows (null queries)
@@ -341,8 +347,9 @@ int kv_index_create(int device, int64_t row_base, kv_index **out) {
   KV_CUDA(ix->evp2.create());
   constexpr auto smem_limit = cudaFuncAttributeMaxDynamicSharedMemorySize;
   KV_CUDA(cudaFuncSetAttribute(tfidf_score_kernel, smem_limit, 200 * 1024));
-  KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<false>, smem_limit, (int)scan_smem_bytes(32)));
-  KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<true>, smem_limit, (int)scan_smem_bytes(0)));
+  KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<false, false>, smem_limit, (int)scan_smem_bytes(32)));
+  KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<true, false>, smem_limit, (int)scan_smem_bytes(0)));
+  KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<false, true>, smem_limit, (int)scan_smem_bytes(32, true)));
   KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<true>, smem_limit, 232448));
   KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<false>, smem_limit, 232448));
   KV_CUDA(cudaFuncSetAttribute(jaccard_scan_kernel<false>, smem_limit, (int)jaccard_smem_bytes(32)));
@@ -407,6 +414,8 @@ int kv_index_append(kv_index *ix, const int64_t *indptr, const uint32_t *ids, co
   // labels describe the rows they were given for: a filtered query fails until the rows are labelled again
   ix->h_labels.clear();
   ix->has_labels = ix->labels_on_device = false;
+  ix->h_groups.clear();  // the same for groups: distinct mode fails until they are set again
+  ix->has_groups = ix->groups_on_device = false;
   if (ix->n_dead) ix->h_dead.resize((size_t)ix->n_rows, 0);  // appended rows are live
   return KV_OK;
 }
@@ -595,6 +604,55 @@ int kv_index_set_row_labels(kv_index *ix, const int32_t *labels, int64_t n) {
   return upload_labels(ix);
 }
 
+// The device copies of the row groups for the current layout: by row and by scan position.  Nothing to do until the
+// index is finalized; every finalize calls it again.
+static int upload_groups(kv_index *ix) {
+  ix->groups_on_device = false;
+  if (!ix->has_groups || !ix->finalized) return KV_OK;
+  cudaStream_t s = ix->stream;
+  const int64_t n = ix->n_rows, n_pos = ix->n_chunks_pad * CHUNK_ROWS;
+  if (n > 0) {
+    KV_CUDA(ix->d_groups_row.ensure(n));
+    KV_CUDA(ix->d_group_pos.ensure(n_pos));
+    KV_CUDA(cudaMemcpyAsync(ix->d_groups_row.p, ix->h_groups.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
+    label_pos_kernel<<<(unsigned)((n_pos + 255) / 256), 256, 0, s>>>(ix->d_perm.p, ix->d_groups_row.p, n, n_pos, ix->d_group_pos.p);
+    KV_CUDA(cudaGetLastError());
+    KV_CUDA(cudaStreamSynchronize(s));
+  }
+  ix->groups_on_device = true;
+  return KV_OK;
+}
+
+// the per-row sets a finalize rebuilds on the device: labels and groups
+static int upload_row_sets(kv_index *ix) {
+  const int rc = upload_labels(ix);
+  return rc != KV_OK ? rc : upload_groups(ix);
+}
+
+static bool groups_ready(const kv_index *ix) {
+  return ix->has_groups && ix->groups_on_device && (int64_t)ix->h_groups.size() == ix->n_rows;
+}
+
+int kv_index_set_row_groups(kv_index *ix, const int32_t *groups, int64_t n) {
+  if (!ix) return kv_fail(KV_ERR_INVALID, "kv_index_set_row_groups: NULL handle");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (!groups) {
+    ix->h_groups.clear();
+    ix->has_groups = ix->groups_on_device = false;
+    return KV_OK;
+  }
+  if (ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_index_set_row_groups: a Jaccard index (mode 1) has no distinct top-k");
+  if (n != ix->n_rows)
+    return kv_fail(KV_ERR_INVALID, "kv_index_set_row_groups: %lld groups for an index of %lld rows", (long long)n,
+                   (long long)ix->n_rows);
+  for (int64_t i = 0; i < n; i++)
+    if (groups[i] < 0) return kv_fail(KV_ERR_INVALID, "kv_index_set_row_groups: group %d of row %lld is negative", groups[i], (long long)i);
+  ix->h_groups.assign(groups, groups + n);
+  ix->has_groups = true;
+  KV_CUDA(cudaSetDevice(ix->device));
+  return upload_groups(ix);
+}
+
 // The device copies of the deletions for the current layout (d_perm must hold it): deleted flags by row, the live word
 // of every chunk and the first LAB_FIRST live rows.  Nothing while no row is deleted: the kernels then get NULL.
 static int upload_dead(kv_index *ix) {
@@ -759,7 +817,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
       ix->finalized = true;
       ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
       ix->last_finalize_kind = 2;
-      return upload_labels(ix);
+      return upload_row_sets(ix);
     }
   }
   ix->layout_valid = false;
@@ -801,7 +859,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
   ix->finalized = true;
   ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
   ix->last_finalize_kind = 1;
-  return upload_labels(ix);
+  return upload_row_sets(ix);
 }
 
 int kv_index_last_finalize_kind(const kv_index *ix) { return ix ? ix->last_finalize_kind : 0; }
@@ -967,7 +1025,7 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
   ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
-  ix->has_excl = ix->has_filter = false;
+  ix->has_excl = ix->has_filter = ix->distinct = false;
   ix->irr_q.clear(); ix->irr_indptr.assign(1, 0); ix->irr_ids.clear(); ix->irr_tf.clear(); ix->irr_oov.clear();
   const int T = host_threads();
   const auto t_begin = std::chrono::steady_clock::now();
@@ -1162,13 +1220,19 @@ struct Batch {
   int64_t n_q, n_tiles, n_groups, n_bsplits, n_ssplits, n_ssplits_a, n_csplits, n_parts;
   int max_pages, n_seed, n_peers;
   bool prune, use_codes, range = false;
+  bool distinct = false;  // kv_query_set_distinct: the scans keep one row per group, K5 skips taken groups
   int64_t launches = 0;
 };
 
 // K5: the first n_lists partial lists of the batch, per query -> the outputs, by original query
 static int launch_merge(kv_index *ix, const Batch &b, int64_t n_lists) {
-  merge_topk_kernel<<<(unsigned)((b.n_q * 32 + 255) / 256), 256, 0, ix->stream>>>(
-      ix->d_part_s.p, ix->d_part_r.p, (int)n_lists, b.n_q, b.k, b.n_q * b.k, b.n_q * b.k, ix->d_qperm.p, b.out_s, b.out_r);
+  if (b.distinct)
+    merge_topk_distinct_kernel<<<(unsigned)((b.n_q * 32 + 255) / 256), 256, 0, ix->stream>>>(
+        ix->d_part_s.p, ix->d_part_r.p, (int)n_lists, b.n_q, b.k, b.n_q * b.k, ix->d_qperm.p, ix->d_groups_row.p, ix->row_base,
+        b.out_s, b.out_r);
+  else
+    merge_topk_kernel<<<(unsigned)((b.n_q * 32 + 255) / 256), 256, 0, ix->stream>>>(
+        ix->d_part_s.p, ix->d_part_r.p, (int)n_lists, b.n_q, b.k, b.n_q * b.k, b.n_q * b.k, ix->d_qperm.p, b.out_s, b.out_r);
   KV_CUDA(cudaGetLastError());
   return KV_OK;
 }
@@ -1189,13 +1253,15 @@ static ScanParams scan_params(const kv_index *ix, const Batch &b) {
   SP.part_scores = ix->d_part_s.p; SP.part_rows = ix->d_part_r.p; SP.max_pages = b.max_pages;
   SP.qperm = ix->d_qperm.p; SP.range_out = ix->d_range.p; SP.range_count = ix->d_range_count.p;
   SP.range_cap = (unsigned long long)ix->d_range.cap;
+  SP.group_pos = b.distinct ? ix->d_group_pos.p : nullptr;
   return SP;
 }
 
-// K1b-S, or K1b-R for a threshold search, over a grid of candidate lists
+// K1b-S (distinct or not), or K1b-R for a threshold search, over a grid of candidate lists
 static int launch_scan(kv_index *ix, const Batch &b, const ScanParams &SP, dim3 grid) {
-  if (b.range) tfidf_scan_kernel<true><<<grid, S_WARPS * 32, scan_smem_bytes(0), ix->stream>>>(SP);
-  else tfidf_scan_kernel<false><<<grid, S_WARPS * 32, scan_smem_bytes(b.k), ix->stream>>>(SP);
+  if (b.range) tfidf_scan_kernel<true, false><<<grid, S_WARPS * 32, scan_smem_bytes(0), ix->stream>>>(SP);
+  else if (b.distinct) tfidf_scan_kernel<false, true><<<grid, S_WARPS * 32, scan_smem_bytes(b.k, true), ix->stream>>>(SP);
+  else tfidf_scan_kernel<false, false><<<grid, S_WARPS * 32, scan_smem_bytes(b.k), ix->stream>>>(SP);
   KV_CUDA(cudaGetLastError());
   return KV_OK;
 }
@@ -1254,8 +1320,8 @@ static int run_pruned(kv_index *ix, Batch &b) {
     // seed scan: gives every query a lower bound of its k-th score
     SP.list_mode = 1; SP.list_count = ix->d_list_count.p; SP.direct = ix->d_direct.p; SP.direct_stride = GROUP_Q * b.n_seed;
     SP.n_bsplits = 1; SP.n_ssplits = (int)b.n_ssplits_a;
-    tfidf_scan_kernel<false><<<dim3((unsigned)b.n_groups, (unsigned)b.n_ssplits_a), S_WARPS * 32, scan_smem_bytes(b.k), s>>>(SP);
-    KV_CUDA(cudaGetLastError());
+    const int rc = launch_scan(ix, b, SP, dim3((unsigned)b.n_groups, (unsigned)b.n_ssplits_a));
+    if (rc != KV_OK) return rc;
     KV_CUDA(cudaEventRecord(ix->evk[2], s));
     b.launches += 3;
     if (b.phase == 1) {  // the seed top-k of this shard, by original query
@@ -1376,11 +1442,18 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
   // the thresholds peers push are those of unfiltered queries: not a bound of a filtered query's k-th score
   if (ix->has_filter && (ix->gthr_exported || ix->n_peers))
     return kv_fail(KV_ERR_INVALID, "kv_topk: a label filter cannot be combined with the threshold exchange of a row-sharded GFKB");
+  if (ix->distinct) {
+    if (!groups_ready(ix))
+      return kv_fail(KV_ERR_STATE, "kv_topk: the batch is distinct but the row groups are missing or stale (set them again after an append)");
+    // a shard's seed k-th score is no lower bound of the global k-th GROUP score: one group can count on several shards
+    if (phase != 0 || ix->gthr_exported || ix->n_peers)
+      return kv_fail(KV_ERR_INVALID, "kv_topk: distinct mode cannot be combined with the two-phase top-k or the threshold exchange of a row-sharded GFKB");
+  }
   ix->jrange_valid = false;
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
   Batch b;
-  b.k = k; b.phase = phase; b.out_s = d_out_s; b.out_r = d_out_r;
+  b.k = k; b.phase = phase; b.out_s = d_out_s; b.out_r = d_out_r; b.distinct = ix->distinct;
   rc = size_batch(ix, b);
   if (rc != KV_OK) return rc;
   const int64_t n_q = b.n_q;
@@ -1456,7 +1529,13 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
   KV_CUDA(cudaEventRecord(ix->evk[5], s));
   b.launches++;
   // queries no path scanned: null queries score 0 against every row, irregular ones take the float64 full scan
-  if (ix->batch_null) {
+  if (ix->batch_null && b.distinct) {
+    fill_null_distinct_kernel<<<(unsigned)((ix->batch_null * 32 + 255) / 256), 256, 0, s>>>(
+        ix->d_qperm.p + n_q, (int)ix->batch_null, k, ix->n_rows, ix->row_base, ix->has_excl ? ix->d_excl_orig.p : nullptr,
+        ix->has_filter ? ix->d_filt_orig.p : nullptr, ix->d_labels_row.p, dead_rows(ix), ix->d_groups_row.p, d_out_s, d_out_r);
+    KV_CUDA(cudaGetLastError());
+    b.launches++;
+  } else if (ix->batch_null) {
     const LabelFirstRows L{ix->d_lab_keys.p, ix->d_lab_rows.p, ix->n_lab};
     fill_null_kernel<<<(unsigned)((ix->batch_null * k + 255) / 256), 256, 0, s>>>(ix->d_qperm.p + n_q, (int)ix->batch_null, k,
                                                                                   ix->n_rows, ix->row_base,
@@ -1470,10 +1549,16 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
     const int64_t q = ix->irr_q[i], a = ix->irr_indptr[i], e = ix->irr_indptr[i + 1];
     rc = score_impl(ix, ix->irr_ids.data() + a, ix->irr_tf.data() + a, e - a, ix->irr_oov[i], nullptr);
     if (rc != KV_OK) return rc;
-    select_topk_kernel<<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
-                                          ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->d_labels_row.p,
-                                          ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix), d_out_s + q * k,
-                                          d_out_r + q * k);
+    if (b.distinct)
+      select_topk_distinct_kernel<<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
+                                                     ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->d_labels_row.p,
+                                                     ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix),
+                                                     ix->d_groups_row.p, d_out_s + q * k, d_out_r + q * k);
+    else
+      select_topk_kernel<<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
+                                            ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->d_labels_row.p,
+                                            ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix), d_out_s + q * k,
+                                            d_out_r + q * k);
     KV_CUDA(cudaGetLastError());
     b.launches += 2;
   }
@@ -1833,6 +1918,19 @@ int kv_query_set_filter(kv_index *ix, const int32_t *labels, int64_t n_q) {
   KV_CUDA(cudaMemcpyAsync(ix->d_filt_orig.p, ix->h_filt_orig.data(), (size_t)n_q * sizeof(int), cudaMemcpyHostToDevice, ix->stream));
   KV_CUDA(cudaStreamSynchronize(ix->stream));
   ix->has_filter = true;
+  return KV_OK;
+}
+
+int kv_query_set_distinct(kv_index *ix, int on) {
+  if (!ix) return kv_fail(KV_ERR_INVALID, "kv_query_set_distinct: NULL handle");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (on && ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_query_set_distinct: a Jaccard index (mode 1) has no distinct top-k");
+  if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_query_set_distinct: no query batch uploaded");
+  ix->distinct = false;
+  if (!on) return KV_OK;
+  if (!groups_ready(ix))
+    return kv_fail(KV_ERR_STATE, "kv_query_set_distinct: the index has no row groups for its current rows (kv_index_set_row_groups)");
+  ix->distinct = true;
   return KV_OK;
 }
 
@@ -2268,6 +2366,6 @@ extern "C" int kv_index_layout_load(kv_index *ix, const char *path) {
   int rc = upload_layout(ix, SL);
   if (rc != KV_OK) return rc;
   ix->finalized = false;
-  ix->labels_on_device = false;  // positions changed: the finalize that follows rebuilds them
+  ix->labels_on_device = ix->groups_on_device = false;  // positions changed: the finalize that follows rebuilds them
   return KV_OK;
 }

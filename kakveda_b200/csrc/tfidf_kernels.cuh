@@ -624,6 +624,8 @@ struct ScanParams {
   RangePair *range_out;              // [range_cap]
   unsigned long long *range_count;   // matches found (may exceed range_cap: those past it are not written)
   unsigned long long range_cap;
+  // distinct top-k (tfidf_scan_kernel<false, true>, kv_query_set_distinct): row group by scan position
+  const int *group_pos;              // [n_chunks_pad * 32], -1 past the last row
 };
 
 // Appends the pairs (*q, score, row) of the lanes with `hit` set: one reservation per warp
@@ -657,7 +659,13 @@ __device__ __forceinline__ void bulk_copy_g2s(void *dst, const void *src, uint32
                : "memory");
 }
 
-template <bool RANGE>
+// DISTINCT (top-k only): every list entry also carries its row's group (s_lgrp) and a list holds at most one row per
+// group, the best one seen.  The warp first keeps the best survivor of each group of the chunk (__match_any_sync), so
+// runs of copies -- neighbours in text order -- reach the lock once; under the lock an entry of the new row's group is
+// found by a ballot and either kept (the new row is worse) or deleted before the new row is inserted.  A full list
+// then holds k distinct groups, so its k-th score stays a lower bound of the k-th group score: the threshold, the
+// codes snapshot and the bound passes are unchanged.
+template <bool RANGE, bool DISTINCT>
 __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams P) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int k = P.k;
@@ -676,6 +684,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   int *s_qlab = s_excl + GROUP_Q;                                           // [GROUP_Q] label filter, -1 = any
   unsigned int *s_next = (unsigned int *)(s_qlab + GROUP_Q);                // [1] next record of this CTA's range
   unsigned int *s_stat = s_next + 1;                                        // [4]
+  int *s_lgrp = (int *)(s_stat + 4);                                        // [GROUP_Q][k] (DISTINCT only)
 
   const int list = blockIdx.x, ssplit = blockIdx.y;
   const int group = list / P.n_bsplits, bsplit = list - group * P.n_bsplits;
@@ -712,6 +721,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
     for (int i = threadIdx.x; i < GROUP_Q * k; i += blockDim.x) {
       s_lscore[i] = -INFINITY;
       s_lrow[i] = 0x7fffffff;
+      if constexpr (DISTINCT) s_lgrp[i] = -1;
     }
     if (threadIdx.x < GROUP_Q) {
       const int qi = threadIdx.x;
@@ -913,6 +923,8 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
       const float Bc = lane < rows ? P.B32[pos0 + lane] : 0.f;
       const int lpos = P.q_label ? P.label_pos[pos0 + lane] : -1;  // one 128-byte line per record
       const bool live = P.alive ? ((P.alive[chunk_cur] >> lane) & 1u) != 0u : true;
+      int gpos = -1;
+      if constexpr (DISTINCT) gpos = P.group_pos[pos0 + lane];  // one 128-byte line per record
       recs_done++;
       for (uint32_t qm = mask_cur; qm; qm &= qm - 1) {
         const int qi = __ffs(qm) - 1;
@@ -997,7 +1009,19 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
           range_emit(P.range_out, P.range_count, P.range_cap, cand, P.qperm + q0 + qi, sc, P.row_base + row);
           continue;
         }
-        const uint32_t cm = __ballot_sync(FULL, cand);
+        uint32_t cm = __ballot_sync(FULL, cand);
+        if constexpr (DISTINCT) {
+          // the best survivor of each group of the chunk goes on (lanes without a survivor get keys of their own)
+          const uint32_t peers = __match_any_sync(FULL, cand ? gpos : -1 - lane);
+          bool keep = cand;
+          for (uint32_t m = __ballot_sync(FULL, cand && peers != (1u << lane)); m; m &= m - 1) {
+            const int j = __ffs(m) - 1;
+            const float s2 = __shfl_sync(FULL, sc, j);
+            const int r2 = __shfl_sync(FULL, row, j);
+            if (((peers >> j) & 1u) && (s2 > sc || (s2 == sc && r2 < row))) keep = false;
+          }
+          cm = __ballot_sync(FULL, keep);
+        }
         if (cm) {
           if (lane == 0) while (atomicCAS(&s_lock[qi], 0, 1) != 0) {}
           __syncwarp();
@@ -1005,25 +1029,48 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
           int cnt = *(volatile int *)&s_cnt[qi];
           float ls = lane < k ? *(volatile float *)&s_lscore[qi * k + lane] : -INFINITY;   // unused slots hold (-inf, INT_MAX)
           int lr = lane < k ? *(volatile int *)&s_lrow[qi * k + lane] : 0x7fffffff;
+          int lg = -1;                                                                      // ... and group -1
+          if constexpr (DISTINCT) lg = lane < k ? *(volatile int *)&s_lgrp[qi * k + lane] : -1;
           bool changed = false;
           for (uint32_t m = cm; m; m &= m - 1) {
             const int j = __ffs(m) - 1;
             const float ns = __shfl_sync(FULL, sc, j);
             const int nr = __shfl_sync(FULL, row, j);
+            int ng = -1;
+            if constexpr (DISTINCT) {
+              ng = __shfl_sync(FULL, gpos, j);
+              const uint32_t same = __ballot_sync(FULL, lane < k && lg == ng);  // at most one entry per group
+              if (same) {
+                const int p = __ffs(same) - 1;
+                const float ps = __shfl_sync(FULL, ls, p);
+                const int pr = __shfl_sync(FULL, lr, p);
+                if (!(ns > ps || (ns == ps && nr < pr))) continue;  // the group's entry is better: the row is dropped
+                // delete the group's entry: the entries after it move up by one, the last slot becomes unused
+                const float ds = __shfl_down_sync(FULL, ls, 1);
+                const int dr = __shfl_down_sync(FULL, lr, 1);
+                const int dg = __shfl_down_sync(FULL, lg, 1);
+                if (lane == k - 1) { ls = -INFINITY; lr = 0x7fffffff; lg = -1; }
+                else if (lane >= p && lane < k) { ls = ds; lr = dr; lg = dg; }
+                cnt--;
+              }
+            }
             // entries that stay ahead of the new one form a prefix of the sorted list
             const bool ahead = lane < k && (ls > ns || (ls == ns && lr < nr));
             const int pos = __popc(__ballot_sync(FULL, ahead));
             const float us = __shfl_up_sync(FULL, ls, 1);
             const int ur = __shfl_up_sync(FULL, lr, 1);
+            int ug = -1;
+            if constexpr (DISTINCT) ug = __shfl_up_sync(FULL, lg, 1);
             if (pos < k) {
-              if (lane > pos) { ls = us; lr = ur; }
-              else if (lane == pos) { ls = ns; lr = nr; }
+              if (lane > pos) { ls = us; lr = ur; if constexpr (DISTINCT) lg = ug; }
+              else if (lane == pos) { ls = ns; lr = nr; if constexpr (DISTINCT) lg = ng; }
               if (cnt < k) cnt++;
               changed = true;
             }
           }
           if (changed) {
             if (lane < k) { s_lscore[qi * k + lane] = ls; s_lrow[qi * k + lane] = lr; }
+            if constexpr (DISTINCT) if (lane < k) s_lgrp[qi * k + lane] = lg;
             if (lane == 0) s_cnt[qi] = cnt;
             const float ks = __shfl_sync(FULL, ls, k - 1);
             if (lane == 0 && cnt == k) publish_threshold(q0 + qi, ks);
@@ -1071,9 +1118,9 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   }
 }
 
-static inline size_t scan_smem_bytes(int k) {
+static inline size_t scan_smem_bytes(int k, bool distinct = false) {
   return (size_t)GROUP_Q * QTAB_BYTES + (size_t)S_WARPS * 2 * S_BUF_BYTES + (size_t)S_WARPS * 32 * sizeof(ScanHit) +
-         (size_t)S_WARPS * 2 * 8 + (size_t)GROUP_Q * k * 8 + (size_t)GROUP_Q * 4 * 7 + 32;
+         (size_t)S_WARPS * 2 * 8 + (size_t)GROUP_Q * k * 8 + (size_t)GROUP_Q * 4 * 7 + 32 + (distinct ? (size_t)GROUP_Q * k * 4 : 0);
 }
 
 // ----------------------------------------------------------------------------------------
@@ -1445,6 +1492,64 @@ __global__ void merge_topk_kernel(const float *__restrict__ in_s, const long lon
   }
 }
 
+// K5 of a distinct batch (kv_query_set_distinct).  Each partial list holds distinct groups; in the merged (score desc,
+// row asc) order a group's first entry is its best row, and every later entry of a taken group is skipped.  Exact: a
+// group of the global top-k is also in the top-k of the partial list that holds its best row.  groups: by local row
+// (global row - row_base).  One warp per query, as merge_topk_kernel; 256 threads per block.
+__global__ void merge_topk_distinct_kernel(const float *__restrict__ in_s, const long long *__restrict__ in_r, int n_lists,
+                                           int64_t n_q, int k, int64_t stride, const int *__restrict__ out_index,
+                                           const int *__restrict__ groups, int64_t row_base, float *out_s, long long *out_r) {
+  __shared__ int s_taken[8][32];  // per warp: the groups taken so far
+  const int64_t q = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (q >= n_q) return;
+  int *taken = s_taken[threadIdx.x >> 5];
+  const int64_t oq = out_index ? out_index[q] : q;
+  constexpr int MAXL = 64;
+  unsigned char head[MAXL];
+#pragma unroll
+  for (int i = 0; i < MAXL; i++) head[i] = 0;
+  for (int j = 0; j < k; j++) {
+    float bs = -INFINITY;
+    long long br = -1;
+    int bl = -1, bg = -1;
+    for (int i = 0; i < MAXL; i++) {
+      int l = lane + 32 * i;
+      if (l >= n_lists) break;
+      int h = head[i];
+      float s = -INFINITY;
+      long long r = -1;
+      int g = -1;
+      for (; h < k; h++) {  // skip the entries of taken groups
+        const size_t o = (size_t)l * stride + (size_t)q * k + h;
+        r = in_r[o];
+        if (r < 0) break;
+        g = groups[r - row_base];
+        bool seen = false;
+        for (int t = 0; t < j; t++) seen |= taken[t] == g;
+        if (!seen) { s = in_s[o]; break; }
+        r = -1;
+      }
+      head[i] = (unsigned char)h;
+      if (r >= 0 && (bl < 0 || better(s, r, bs, br))) { bs = s; br = r; bl = l; bg = g; }
+    }
+    for (int o = 16; o; o >>= 1) {
+      float s2 = __shfl_xor_sync(FULL, bs, o);
+      long long r2 = __shfl_xor_sync(FULL, br, o);
+      int l2 = __shfl_xor_sync(FULL, bl, o);
+      int g2 = __shfl_xor_sync(FULL, bg, o);
+      if (l2 >= 0 && (bl < 0 || better(s2, r2, bs, br))) { bs = s2; br = r2; bl = l2; bg = g2; }
+    }
+    if (bl >= 0 && (bl & 31) == lane) head[bl >> 5]++;
+    if (lane == 0) {
+      out_s[oq * k + j] = bl >= 0 ? bs : -INFINITY;
+      out_r[oq * k + j] = bl >= 0 ? br : -1LL;
+      taken[j] = bg;  // -1 once the lists are exhausted: no group is -1
+    }
+    __syncwarp();
+  }
+}
+
 constexpr int LAB_FIRST = 33;  // smallest rows kept per label: k <= 32 of them plus one a self-join excludes
 
 // The rows of each label in ascending order, first LAB_FIRST of them (kv_index_set_row_labels): keys[n_lab] sorted,
@@ -1539,6 +1644,101 @@ __global__ void select_topk_kernel(const double *__restrict__ scores, int64_t n,
       }
     }
     __syncthreads();
+  }
+}
+
+// select_topk_kernel of a distinct batch: each pass takes the next row in (score desc, row asc) order whose group
+// (groups: by local row) is not taken yet.  Every row before the previous pick is a pick or of a taken group, so
+// "strictly after the previous pick" stays the only order constraint.  The <= k taken groups sit in shared memory and
+// are only consulted for a row that would beat the thread's current best.
+__global__ void select_topk_distinct_kernel(const double *__restrict__ scores, int64_t n, int64_t row_base, int k, int64_t excl,
+                                            const int *__restrict__ labels, int lab, const uint8_t *__restrict__ dead,
+                                            const int *__restrict__ groups, float *out_s, long long *out_r) {
+  __shared__ float s_s[32];
+  __shared__ long long s_r[32];
+  __shared__ int s_taken[32];
+  __shared__ float prev_s;
+  __shared__ long long prev_r;
+  if (threadIdx.x == 0) { prev_s = INFINITY; prev_r = -1; }
+  __syncthreads();
+  for (int j = 0; j < k; j++) {
+    float bs = -INFINITY;
+    long long br = -1;
+    const float ps = prev_s;
+    const long long pr = prev_r;
+    for (int64_t r = threadIdx.x; r < n; r += blockDim.x) {
+      if (r == excl || (lab >= 0 && labels[r] != lab) || (dead && dead[r])) continue;
+      float s = (float)scores[r];
+      bool after = (s < ps) || (s == ps && r > pr);
+      if (after && (br < 0 || s > bs || (s == bs && r < br))) {
+        const int g = groups[r];
+        bool seen = false;
+        for (int t = 0; t < j; t++) seen |= s_taken[t] == g;
+        if (!seen) { bs = s; br = r; }
+      }
+    }
+    for (int o = 16; o; o >>= 1) {
+      float s2 = __shfl_xor_sync(FULL, bs, o);
+      long long r2 = __shfl_xor_sync(FULL, br, o);
+      if (r2 >= 0 && (br < 0 || s2 > bs || (s2 == bs && r2 < br))) { bs = s2; br = r2; }
+    }
+    if ((threadIdx.x & 31) == 0) { s_s[threadIdx.x >> 5] = bs; s_r[threadIdx.x >> 5] = br; }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+      int nw = blockDim.x >> 5;
+      bs = threadIdx.x < nw ? s_s[threadIdx.x] : -INFINITY;
+      br = threadIdx.x < nw ? s_r[threadIdx.x] : -1;
+      for (int o = 16; o; o >>= 1) {
+        float s2 = __shfl_xor_sync(FULL, bs, o);
+        long long r2 = __shfl_xor_sync(FULL, br, o);
+        if (r2 >= 0 && (br < 0 || s2 > bs || (s2 == bs && r2 < br))) { bs = s2; br = r2; }
+      }
+      if (threadIdx.x == 0) {
+        out_s[j] = br >= 0 ? bs : -INFINITY;
+        out_r[j] = br >= 0 ? row_base + br : -1LL;
+        s_taken[j] = br >= 0 ? groups[br] : -1;
+        if (br >= 0) { prev_s = bs; prev_r = br; } else { prev_s = -INFINITY; prev_r = (long long)n; }
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// fill_null_kernel of a distinct batch: one warp per null query walks the rows it may match (not excluded, of its
+// label when filtered -- labels by local row --, live) in ascending order and keeps the first row of each new group
+// until it has k.  A query whose eligible rows hold fewer than k groups walks the whole index.
+__global__ void fill_null_distinct_kernel(const int *__restrict__ null_q, int n_null, int k, int64_t n_rows, int64_t row_base,
+                                          const int *__restrict__ excl_by_query, const int *__restrict__ label_by_query,
+                                          const int *__restrict__ labels, const uint8_t *__restrict__ dead,
+                                          const int *__restrict__ groups, float *out_s, long long *out_r) {
+  const int w = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (w >= n_null) return;
+  const int q = null_q[w];
+  const int ex = excl_by_query ? excl_by_query[q] : -1;  // by ORIGINAL query index
+  const int lb = label_by_query ? label_by_query[q] : -1;
+  int tg = -1;  // lane t: group of the t-th row taken
+  int n = 0;
+  for (int64_t r0 = 0; r0 < n_rows && n < k; r0 += 32) {
+    const int64_t r = r0 + lane;
+    const bool elig = r < n_rows && r != ex && (lb < 0 || labels[r] == lb) && !(dead && dead[r]);
+    const int g = elig ? groups[r] : -1 - lane;
+    bool fresh = elig;
+    for (int t = 0; t < n; t++) fresh &= __shfl_sync(FULL, tg, t) != g;
+    const uint32_t peers = __match_any_sync(FULL, g);
+    fresh = fresh && __ffs(peers) - 1 == lane;  // the lowest row of its group among these 32
+    for (uint32_t fm = __ballot_sync(FULL, fresh); fm && n < k; fm &= fm - 1, n++) {
+      const int j = __ffs(fm) - 1;
+      const int gj = __shfl_sync(FULL, g, j);
+      if (lane == n) {
+        tg = gj;
+        out_s[(size_t)q * k + n] = 0.f;
+        out_r[(size_t)q * k + n] = row_base + r0 + j;
+      }
+    }
+  }
+  if (lane >= n && lane < k) {
+    out_s[(size_t)q * k + lane] = -INFINITY;
+    out_r[(size_t)q * k + lane] = -1LL;
   }
 }
 

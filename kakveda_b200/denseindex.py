@@ -12,6 +12,7 @@ from typing import Tuple
 import numpy as np
 
 from . import _capi, _devout
+from ._capi import no_distinct
 
 
 def to_bf16_bits(x: np.ndarray) -> np.ndarray:
@@ -42,9 +43,10 @@ class DenseIndex:
     def finalize(self) -> None:
         _capi.check(_capi.load().kv_dense_finalize(self._h))
 
-    def topk_device(self, queries, k: int = 16, exclude_base: int = -1):
+    def topk_device(self, queries, k: int = 16, exclude_base: int = -1, distinct: bool = False):
         """Queries and results on the device (torch): queries bfloat16 [Q, dim]; returns (float32 [Q,k], int64 [Q,k]).
         ``exclude_base >= 0``: query q never matches GLOBAL row ``exclude_base + q`` (self-join)."""
+        no_distinct(distinct, "DenseIndex.topk_device")
         import torch
 
         assert queries.is_cuda and queries.is_contiguous() and queries.element_size() == 2 and queries.shape[-1] == self.dim
@@ -56,8 +58,9 @@ class DenseIndex:
                                                       C.c_void_p(s.data_ptr()), C.c_void_p(r.data_ptr())))
         return s, r
 
-    def selfjoin_topk(self, k: int = 32, lo: int = 0, hi: int | None = None, device_out: bool = False):
+    def selfjoin_topk(self, k: int = 32, lo: int = 0, hi: int | None = None, device_out: bool = False, distinct: bool = False):
         """All-pairs (BASELINE configs[3]): for local rows [lo, hi) the k nearest OTHER rows."""
+        no_distinct(distinct, "DenseIndex.selfjoin_topk")
         import torch
 
         hi = self.n_rows if hi is None else hi
@@ -71,7 +74,8 @@ class DenseIndex:
     def n_rows(self) -> int:
         return int(_capi.load().kv_dense_rows(self._h))
 
-    def topk(self, queries: np.ndarray, k: int = 16) -> Tuple[np.ndarray, np.ndarray]:
+    def topk(self, queries: np.ndarray, k: int = 16, distinct: bool = False) -> Tuple[np.ndarray, np.ndarray]:
+        no_distinct(distinct, "DenseIndex.topk")
         bits = queries if queries.dtype == np.uint16 else to_bf16_bits(queries)
         bits = np.ascontiguousarray(bits).reshape(-1, self.dim)
         n = bits.shape[0]

@@ -25,6 +25,7 @@ from typing import Optional, Tuple
 import numpy as np
 
 from . import _capi
+from ._capi import no_distinct
 from .similarity import FeatureBatch, GfkbIndex, Vocabulary, gather_rows, text_order
 
 
@@ -223,8 +224,9 @@ class ShardedGfkb:
         self.index.upload_queries(qfb)
         self._exchange_thresholds(qfb.n)
 
-    def topk_resident(self, k: int):
+    def topk_resident(self, k: int, distinct: bool = False):
         """Device-only step on the uploaded batch: local scan+merge, all-gather, global merge."""
+        no_distinct(distinct, "ShardedGfkb.topk_resident")
         import torch
 
         q = self._resident_q
@@ -387,9 +389,10 @@ class ShardedGfkb:
         torch.cuda.current_stream().synchronize()
         return hs.numpy(), hr.numpy()
 
-    def topk_packed(self, data, offsets: np.ndarray, k: int, mode: int = 0):
+    def topk_packed(self, data, offsets: np.ndarray, k: int, mode: int = 0, distinct: bool = False):
         """End-to-end step from host text: featurise, upload, scan, exchange, merge, read back.  ``last_e2e_ms`` keeps
         the wall-clock split of the last call (featurise / upload incl. table kernels / device step / read-back)."""
+        no_distinct(distinct, "ShardedGfkb.topk_packed")
         import time
 
         t0 = time.perf_counter()
@@ -454,8 +457,9 @@ class ShardedDense:
         self.index.finalize()
         self._local = rows_local
 
-    def topk(self, queries, k: int = 16, exclude_base: int = -1):
+    def topk(self, queries, k: int = 16, exclude_base: int = -1, distinct: bool = False):
         """queries: torch bfloat16 CUDA [Q, dim], identical on every rank -> ([Q,k] float32, [Q,k] int64) on device."""
+        no_distinct(distinct, "ShardedDense.topk")
         s, r = self.index.topk_device(queries.contiguous(), k, exclude_base)
         if self.world == 1:
             return s, r
@@ -527,8 +531,9 @@ class ShardedJaccard:
         self.index.add_csr(np.ascontiguousarray(indptr, dtype=np.int64), np.ascontiguousarray(ids, dtype=np.uint32))
         self.index.finalize()
 
-    def topk_csr(self, indptr: np.ndarray, ids: np.ndarray, k: int = 16):
+    def topk_csr(self, indptr: np.ndarray, ids: np.ndarray, k: int = 16, distinct: bool = False):
         """(scores float32, rows int64, inter int32, union int32), each [Q,k], identical on every rank."""
+        no_distinct(distinct, "ShardedJaccard.topk_csr")
         import torch
         import torch.distributed as dist
 

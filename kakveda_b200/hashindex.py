@@ -13,6 +13,7 @@ from typing import Iterable, Sequence, Tuple
 import numpy as np
 
 from . import _capi
+from ._capi import no_distinct
 from .fingerprint import fingerprint_u64
 
 
@@ -33,8 +34,9 @@ class HashIndex:
     def n_rows(self) -> int:
         return int(_capi.load().kv_hash_rows(self._h))
 
-    def match_hashes(self, hashes: np.ndarray, k: int = 16) -> Tuple[np.ndarray, np.ndarray]:
+    def match_hashes(self, hashes: np.ndarray, k: int = 16, distinct: bool = False) -> Tuple[np.ndarray, np.ndarray]:
         """(rows int64 [Q,k] ascending, -1 padded; counts int64 [Q])."""
+        no_distinct(distinct, "HashIndex.match_hashes")
         hashes = np.ascontiguousarray(hashes, dtype=np.uint64)
         rows = np.empty((len(hashes), k), dtype=np.int64)
         counts = np.empty(len(hashes), dtype=np.int64)
@@ -43,7 +45,8 @@ class HashIndex:
                                                counts.ctypes.data_as(C.POINTER(C.c_int64))))
         return rows, counts
 
-    def match_signatures(self, signature_texts: Sequence[str], k: int = 16):
+    def match_signatures(self, signature_texts: Sequence[str], k: int = 16, distinct: bool = False):
+        no_distinct(distinct, "HashIndex.match_signatures")
         return self.match_hashes(np.fromiter((fingerprint_u64(s) for s in signature_texts), dtype=np.uint64), k)
 
     def last_timing(self) -> Tuple[float, int]:

@@ -17,6 +17,7 @@ from typing import Optional, Sequence, Tuple
 import numpy as np
 
 from . import _capi, _devout
+from ._capi import no_distinct
 
 
 def _csr(sets: Sequence[Sequence[int]]) -> Tuple[np.ndarray, np.ndarray]:
@@ -86,8 +87,9 @@ class JaccardIndex:
     def n_rows(self) -> int:
         return int(_capi.load().kv_index_rows(self._h))
 
-    def topk_csr(self, indptr: np.ndarray, ids: np.ndarray, k: int = 16):
+    def topk_csr(self, indptr: np.ndarray, ids: np.ndarray, k: int = 16, distinct: bool = False):
         """(scores float32 [Q,k], rows int64 [Q,k], inter int32 [Q,k], union int32 [Q,k])."""
+        no_distinct(distinct, "JaccardIndex.topk_csr")
         lib = _capi.load()
         indptr, ids, oov = self._strip_oov(indptr, ids)
         n = len(indptr) - 1
@@ -112,7 +114,8 @@ class JaccardIndex:
         indptr, ids, oov = self._strip_oov(indptr, ids)
         return self._counts(indptr, ids, oov, np.ascontiguousarray(rows, dtype=np.int64))
 
-    def topk_sets(self, queries: Sequence[Sequence[int]], k: int = 16):
+    def topk_sets(self, queries: Sequence[Sequence[int]], k: int = 16, distinct: bool = False):
+        no_distinct(distinct, "JaccardIndex.topk_sets")
         return self.topk_csr(*_csr(queries), k=k)
 
     def _range_resident(self, n_q: int, threshold: float, device_out: bool = False):
@@ -157,9 +160,10 @@ class JaccardIndex:
         """``range_csr`` of token sets."""
         return self.range_csr(*_csr(queries), threshold, device_out)
 
-    def selfjoin_topk(self, k: int, lo: int = 0, hi: Optional[int] = None):
+    def selfjoin_topk(self, k: int, lo: int = 0, hi: Optional[int] = None, distinct: bool = False):
         """All-pairs: for local rows [lo, hi) the k best OTHER rows (the row itself is excluded), as ``topk_csr``:
         ``(scores float32[n,k], rows int64[n,k], inter int32[n,k], union int32[n,k])``."""
+        no_distinct(distinct, "JaccardIndex.selfjoin_topk")
         hi = self.n_rows if hi is None else hi
         if hi <= lo:
             return (np.zeros((0, k), np.float32), np.zeros((0, k), np.int64), np.zeros((0, k), np.int32),

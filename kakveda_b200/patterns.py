@@ -77,7 +77,7 @@ def pattern_payload(name: str, records: Sequence[Mapping[str, Any]], description
 
 def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: float = 0.8, k: Optional[int] = 32,
                     min_apps: int = 2, failure_type: Optional[str] = None,
-                    filter_first: bool = False) -> List[Dict[str, Any]]:
+                    filter_first: bool = False, distinct: bool = False) -> List[Dict[str, Any]]:
     """Similarity-split version of pattern_detector.on_failure.
 
     ``index``: a finalized ``GfkbIndex`` whose row i is ``records[i]['signature_text']`` (corpus-fit mode gives a
@@ -91,6 +91,10 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
     ``filter_first`` (with ``failure_type``, ``GfkbIndex`` only): the index's row labels are set to the records' failure
     types and the self-join searches every row among the rows of its own type, so with an integer ``k`` other types
     cannot fill a row's list and hide its same-type neighbours.  With ``k=None`` the components are the default's.
+    ``distinct`` (integer ``k``, ``GfkbIndex`` only): the index's row groups are set to text identity -- the records'
+    (failure_type, signature_text) keys -- and every row's list holds at most one row per key, so copies link to
+    their key's lowest other copy and the other k - 1 slots go to other texts: a text stored more than k times no
+    longer hides its neighbours.  With ``k=None`` the components are the default's.
     """
     n = len(records)
     keep = np.ones(n, dtype=bool)
@@ -101,6 +105,14 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
         # are empty, so each is a singleton -- and a singleton record spanning two apps must not become a pattern
         dead = index.deleted_mask()[:n]
         keep[: len(dead)] &= ~dead
+    if distinct and k is not None:
+        from .similarity import GfkbIndex
+
+        if not isinstance(index, GfkbIndex):
+            raise NotImplementedError("detect_patterns(distinct=True) collapses copies on a GfkbIndex only")
+        keys: Dict[Any, int] = {}  # the (failure_type, signature_text) key an upsert versions: one text of one type
+        index.set_row_groups(np.fromiter((keys.setdefault((r.get("failure_type"), r.get("signature_text")), len(keys))
+                                          for r in records), dtype=np.int32, count=n))
     if filter_first and failure_type is not None:
         from .similarity import GfkbIndex
 
@@ -114,7 +126,7 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
             labels, _ = cluster_csr(indptr, rows)
             labels = labels.cpu().numpy()
         else:
-            scores, rows = index.selfjoin_topk(k, same_label=True)
+            scores, rows = index.selfjoin_topk(k, same_label=True, distinct=distinct)
             labels, _ = cluster_topk(rows, scores, threshold)
     # a JaccardIndex returns the exact counts after these arrays: only the leading ones are used
     elif k is None:
@@ -132,7 +144,7 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
         labels, _ = cluster_csr(indptr, rows)
         labels = labels.cpu().numpy()
     else:
-        scores, rows = index.selfjoin_topk(k)[:2]
+        scores, rows = index.selfjoin_topk(k, distinct=True)[:2] if distinct else index.selfjoin_topk(k)[:2]
         if failure_type is not None:
             # rows of other failure types neither join nor bridge components
             bad = ~keep[np.clip(rows, 0, n - 1)] | (rows < 0)

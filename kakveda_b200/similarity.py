@@ -206,6 +206,7 @@ class GfkbIndex:
         self.device = device
         self.row_base = row_base
         self._row_labels: Optional[np.ndarray] = None  # what set_row_labels gave, until the next append
+        self._group_rows: Optional[int] = None  # rows set_row_groups described, until the next append
 
     # -- build ---------------------------------------------------------------------------
     def add_features(self, fb: FeatureBatch, lo: int = 0, hi: Optional[int] = None) -> None:
@@ -215,7 +216,8 @@ class GfkbIndex:
         ip = np.ascontiguousarray(fb.indptr[lo:hi + 1])
         _capi.check(_capi.load().kv_index_append(self._h, _ptr(ip, C.c_int64), _ptr(fb.ids, C.c_uint32),
                                                  _ptr(fb.tf, C.c_uint32), hi - lo))
-        self._row_labels = None  # the library drops the labels on an append
+        self._row_labels = None  # the library drops the labels (and the groups) on an append
+        self._group_rows = None
 
     def set_row_labels(self, labels: Optional[np.ndarray]) -> None:
         """One label >= 0 per local row (e.g. a failure-type id), for the ``labels`` / ``same_label`` filters of the
@@ -228,6 +230,23 @@ class GfkbIndex:
         labels = np.ascontiguousarray(labels, dtype=np.int32)
         _capi.check(_capi.load().kv_index_set_row_labels(self._h, _ptr(labels, C.c_int32), len(labels)))
         self._row_labels = labels.copy()
+
+    def set_row_groups(self, groups: Optional[np.ndarray]) -> None:
+        """One group >= 0 per local row (e.g. one id per distinct text), for the ``distinct`` top-k of the query
+        methods; ``None`` clears.  Survives finalize, a layout load and deletions; an append drops the groups (a
+        distinct query then raises until they are set again).  Setting groups alone changes no result."""
+        if groups is None:
+            _capi.check(_capi.load().kv_index_set_row_groups(self._h, None, 0))
+            self._group_rows = None
+            return
+        groups = np.ascontiguousarray(groups, dtype=np.int32)
+        _capi.check(_capi.load().kv_index_set_row_groups(self._h, _ptr(groups, C.c_int32), len(groups)))
+        self._group_rows = len(groups)
+
+    @property
+    def has_row_groups(self) -> bool:
+        """Whether ``set_row_groups`` describes the current rows (an append drops the groups)."""
+        return self._group_rows is not None and self._group_rows == self.n_rows
 
     def add_texts(self, texts: Sequence[str]) -> None:
         fb = self.vocab.featurize(texts, grow=True)
@@ -300,13 +319,18 @@ class GfkbIndex:
         finally:
             fb.close()
 
-    def topk_features(self, fb: FeatureBatch, k: int, labels: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
-        """``labels``: per query the row label its results must carry (-1: any row), see ``set_filter``."""
-        if labels is not None:
+    def topk_features(self, fb: FeatureBatch, k: int, labels: Optional[np.ndarray] = None,
+                      distinct: bool = False) -> Tuple[np.ndarray, np.ndarray]:
+        """``labels``: per query the row label its results must carry (-1: any row), see ``set_filter``.  ``distinct``:
+        at most one row per group (``set_row_groups``), see ``set_distinct``."""
+        if labels is not None or distinct:
             if fb.n == 0:
                 return np.zeros((0, k), np.float32), np.zeros((0, k), np.int64)
             self.upload_queries(fb)
-            self.set_filter(labels)
+            if labels is not None:
+                self.set_filter(labels)
+            if distinct:
+                self.set_distinct(True)
             return self.topk_resident_host(fb.n, k)
         scores = np.empty((fb.n, k), dtype=np.float32)
         rows = np.empty((fb.n, k), dtype=np.int64)
@@ -391,6 +415,12 @@ class GfkbIndex:
         labels = np.ascontiguousarray(labels, dtype=np.int32)
         _capi.check(_capi.load().kv_query_set_filter(self._h, _ptr(labels, C.c_int32), len(labels)))
 
+    def set_distinct(self, on: bool) -> None:
+        """Distinct top-k for the resident batch (until the next upload): of the rows a query may match, the best row
+        of each group (``set_row_groups``) in (score desc, row asc) order, the groups ranked by it, and the first k
+        of them.  Scores are the non-distinct ones; threshold searches ignore the mode."""
+        _capi.check(_capi.load().kv_query_set_distinct(self._h, 1 if on else 0))
+
     def topk_resident_host(self, n_q: int, k: int) -> Tuple[np.ndarray, np.ndarray]:
         """Scan + merge of the resident batch of ``n_q`` queries, results copied to the host."""
         scores = np.empty((n_q, k), dtype=np.float32)
@@ -406,13 +436,16 @@ class GfkbIndex:
             self.set_filter(self._row_labels[lo:hi])
 
     def selfjoin_topk(self, k: int, lo: int = 0, hi: Optional[int] = None,
-                      same_label: bool = False) -> Tuple[np.ndarray, np.ndarray]:
+                      same_label: bool = False, distinct: bool = False) -> Tuple[np.ndarray, np.ndarray]:
         """All-pairs: for local rows [lo, hi) the k best OTHER rows (the row itself is excluded).  ``same_label``:
-        row i's list holds only rows with row i's label."""
+        row i's list holds only rows with row i's label.  ``distinct``: at most one row per group (``set_row_groups``);
+        row i's own group still counts, through its other rows."""
         hi = self.n_rows if hi is None else hi
         if hi <= lo:
             return np.zeros((0, k), np.float32), np.zeros((0, k), np.int64)
         self._selfjoin_upload(lo, hi, same_label)
+        if distinct:
+            self.set_distinct(True)
         return self.topk_resident_host(hi - lo, k)
 
     def _range_resident(self, n_q: int, threshold: float, device_out: bool = False):
@@ -493,12 +526,14 @@ class GfkbIndex:
         """Phase 2 of a sharded step: candidate selection + scan + merge of the resident batch."""
         _capi.check(_capi.load().kv_topk_resident_finish(self._h, k, C.c_void_p(d_scores_ptr), C.c_void_p(d_rows_ptr)))
 
-    def topk(self, queries: Sequence[str], k: int, labels: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
+    def topk(self, queries: Sequence[str], k: int, labels: Optional[np.ndarray] = None,
+             distinct: bool = False) -> Tuple[np.ndarray, np.ndarray]:
         """(scores float32 [Q,k], rows int64 [Q,k]) ordered by (score desc, row asc) (K1b+K5).  ``labels``: per query
-        the row label its results must carry (-1: any row)."""
+        the row label its results must carry (-1: any row).  ``distinct``: at most one row per group (the best one;
+        ``set_row_groups``)."""
         fb = self.vocab.featurize(queries, grow=False)
         try:
-            return self.topk_features(fb, k, labels)
+            return self.topk_features(fb, k, labels, distinct)
         finally:
             fb.close()
 

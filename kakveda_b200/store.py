@@ -132,6 +132,10 @@ class GfkbStore:
         # failure_type -> row label of the device index, numbered in order of first appearance; label of each record
         self._type_ids: Dict[str, int] = {}
         self._labels: List[int] = []
+        # (failure_type, signature_text) key -> row group of the device index (distinct match), numbered in order of
+        # first appearance; group of each record.  Set on the segments only when a distinct match needs them.
+        self._group_ids: Dict[Tuple[str, str], int] = {}
+        self._groups: List[int] = []
         self.stats = {"full_rebuilds": 0, "stat_refreshes": 0, "compactions": 0, "quarantined": 0}
         self.quarantined: List[int] = []  # indices of loaded records that cannot be indexed (they keep their row, with no features)
         if self.path is not None and self.path.exists():
@@ -162,6 +166,7 @@ class GfkbStore:
         for i, r in enumerate(self.records):
             self._latest[(r["failure_type"], r["signature_text"])] = i
         self._type_ids, self._labels = {}, []
+        self._group_ids, self._groups = {}, []
         self._rebuild_main()
 
     def _row_labels(self, lo: int, hi: int) -> np.ndarray:
@@ -233,6 +238,32 @@ class GfkbStore:
         live = self._row2rec >= 0
         out[live] = rec_labels[self._row2rec[live]]
         return out
+
+    def _rec_groups(self, hi: int) -> np.ndarray:
+        """int32 group of records[:hi]: their (failure_type, signature_text) keys, numbered in order of first appearance.
+        All rows of a group share their text, hence their score."""
+        for r in self.records[len(self._groups):hi]:
+            self._groups.append(self._group_ids.setdefault((r["failure_type"], r["signature_text"]), len(self._group_ids)))
+        return np.asarray(self._groups[:hi], dtype=np.int32)
+
+    def _dev_groups(self, n_dev: int) -> np.ndarray:
+        """int32 group of the first ``n_dev`` device rows (main + tail); a deleted row's group (0) is never read."""
+        rec_groups = self._rec_groups(self._n_indexed)
+        if self._row2rec is None:
+            return rec_groups[:n_dev]
+        out = np.zeros(n_dev, dtype=np.int32)
+        live = self._row2rec >= 0
+        out[live] = rec_groups[self._row2rec[live]]
+        return out
+
+    def _ensure_groups(self) -> None:
+        """Both segments carry the same group numbering (an append or a rebuild dropped it)."""
+        groups = None
+        for ix, lo in ((self._main, 0), (self._tail, self._n_main)):
+            if ix is not None and ix.n_rows and not ix.has_row_groups:
+                if groups is None:
+                    groups = self._dev_groups(self._n_dev)
+                ix.set_row_groups(groups[lo:lo + ix.n_rows])
 
     def _to_records(self, rows: np.ndarray) -> np.ndarray:
         """Device rows -> record indices (-1 stays -1)."""
@@ -370,6 +401,7 @@ class GfkbStore:
         gone = live_rows[~keep[: self._n_indexed]]
         self.records = [self.records[i] for i in keep_idx]
         self._labels = [lab for i, lab in enumerate(self._labels) if keep[i]]
+        self._groups = [g for i, g in enumerate(self._groups) if keep[i]]  # survivors keep their group ids
         self.quarantined = [int(new_idx[i]) for i in self.quarantined if keep[i]]
         self._quarantine_set = set(self.quarantined)
         self.stats["quarantined"] = len(self.quarantined)
@@ -428,18 +460,24 @@ class GfkbStore:
         self._sidecar_rows = len(texts)
 
     # -- match (services/gfkb/app.py:79-102) -------------------------------------------------------------------
-    def _candidates(self, fb: FeatureBatch, k: int, limit: int = MATCH_LIMIT,
-                    labels: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    def _candidates(self, fb: FeatureBatch, k: int, limit: int = MATCH_LIMIT, labels: Optional[np.ndarray] = None,
+                    distinct: bool = False) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
         """Per query: candidate rows from both segments with their float64 scores, ordered (score desc, row asc), and
         whether the candidate stage may have missed a top-``limit`` row (``ambiguous_candidates``).  ``labels``: per
-        query the failure-type label its candidates must carry (-1: any)."""
+        query the failure-type label its candidates must carry (-1: any).  ``distinct``: each segment returns one row
+        per (failure_type, signature_text) group, and the merge keeps the first row of each group."""
+        if distinct:
+            self._ensure_groups()
         rows_all, f64_all = [], []
         amb = np.zeros(fb.n, dtype=bool)
         for ix in (self._main, self._tail):
             if ix is None or ix.n_rows == 0:
                 continue
             kk = min(k, MAX_LIMIT)
-            s32, rows = ix.topk_features(fb, kk) if labels is None else ix.topk_features(fb, kk, labels)
+            if distinct:
+                s32, rows = ix.topk_features(fb, kk, labels, distinct=True)
+            else:
+                s32, rows = ix.topk_features(fb, kk) if labels is None else ix.topk_features(fb, kk, labels)
             amb |= ambiguous_candidates(s32, rows, limit)
             rows_all.append(rows)
             f64_all.append(ix.rescore(fb, rows))
@@ -447,14 +485,49 @@ class GfkbStore:
         f64 = np.concatenate(f64_all, axis=1)
         big = np.where(rows < 0, np.iinfo(np.int64).max, rows)
         order = np.lexsort((big, -f64), axis=1)  # last key is primary: score descending, then row ascending
-        return self._to_records(np.take_along_axis(rows, order, axis=1)), np.take_along_axis(f64, order, axis=1), amb
+        recs, f64 = self._to_records(np.take_along_axis(rows, order, axis=1)), np.take_along_axis(f64, order, axis=1)
+        if distinct:
+            recs, f64 = self._first_of_groups(recs, f64)
+        return recs, f64, amb
 
-    def _exact_top(self, signature_text: str, limit: int, label: int = -1) -> Tuple[List[int], List[float]]:
+    def _first_of_groups(self, recs: np.ndarray, f64: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
+        """Per query (rows ordered): the first record of each group, moved to the front; (-1, -inf) fill the rest."""
+        groups = self._rec_groups(self._n_indexed)
+        out_r = np.full_like(recs, -1)
+        out_s = np.full_like(f64, -np.inf)
+        for q in range(recs.shape[0]):
+            seen, j = set(), 0
+            for r, sc in zip(recs[q].tolist(), f64[q].tolist()):
+                if r < 0 or groups[r] in seen:
+                    continue
+                seen.add(groups[r])
+                out_r[q, j], out_s[q, j] = r, sc
+                j += 1
+        return out_r, out_s
+
+    def _distinct_match(self, rec: int, score: float) -> dict:
+        """A distinct result: its key's NEWEST record (the one the next upsert would version) with the key's score."""
+        r = self.records[rec]
+        return _to_match(self.records[self._latest[(r["failure_type"], r["signature_text"])]], score)
+
+    def _exact_top(self, signature_text: str, limit: int, label: int = -1,
+                   distinct: bool = False) -> Tuple[List[int], List[float]]:
         """Rows and float64 scores of the reference's ``sorted(..., reverse=True)[:limit]`` on the full score vector
-        (K1a on both segments): no candidate stage at all.  ``label`` >= 0: over the rows of that failure-type label."""
+        (K1a on both segments): no candidate stage at all.  ``label`` >= 0: over the rows of that failure-type label.
+        ``distinct``: over the first eligible row of each (failure_type, signature_text) group."""
         parts = [ix.score(signature_text) for ix in (self._main, self._tail) if ix is not None and ix.n_rows]
         scores = np.concatenate(parts)  # by device row; -inf for a deleted row
-        if label >= 0:
+        if distinct:
+            if label >= 0:
+                idx = np.flatnonzero(self._dev_labels(len(scores)) == label)
+            elif self._row2rec is not None:
+                idx = np.flatnonzero(self._row2rec >= 0)
+            else:
+                idx = np.arange(len(scores))
+            _, first = np.unique(self._dev_groups(len(scores))[idx], return_index=True)
+            idx = idx[np.sort(first)]  # ascending: the stable order is kept
+            order = idx[stable_top(scores[idx], limit)]
+        elif label >= 0:
             idx = np.flatnonzero(self._dev_labels(len(scores)) == label)  # ascending: the stable order is kept
             order = idx[stable_top(scores[idx], limit)]
         elif self._row2rec is not None:
@@ -465,7 +538,7 @@ class GfkbStore:
         return self._to_records(order).tolist(), [float(scores[i]) for i in order]
 
     def _match_filter_first(self, signature_texts: Sequence[str], failure_types: Sequence[Optional[str]],
-                            limit: int) -> List[List[dict]]:
+                            limit: int, distinct: bool = False) -> List[List[dict]]:
         """The best ``limit`` rows OF each query's failure type (all rows for a query without one)."""
         self._row_labels(0, len(self.records))  # number every stored type
         labels = np.array([-1 if not ft else self._type_ids.get(ft, -2) for ft in failure_types], dtype=np.int32)
@@ -475,23 +548,30 @@ class GfkbStore:
             return out
         fb = self.vocab.featurize([signature_texts[i] for i in scan], grow=False)
         try:
-            rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit, labels[scan])
+            if distinct:
+                rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit, labels[scan], True)
+            else:
+                rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit, labels[scan])
         finally:
             fb.close()
         for j, i in enumerate(scan.tolist()):
             if amb[j]:
-                top_r, top_s = self._exact_top(signature_texts[i], limit, int(labels[i]))
+                top_r, top_s = (self._exact_top(signature_texts[i], limit, int(labels[i]), True) if distinct
+                                else self._exact_top(signature_texts[i], limit, int(labels[i])))
                 self.stats["exact_fallbacks"] = self.stats.get("exact_fallbacks", 0) + 1
             else:
                 top_r, top_s = rows[j, :limit].tolist(), f64[j, :limit].tolist()
-            out[i] = [_to_match(self.records[r], s) for r, s in zip(top_r, top_s) if r >= 0]
+            to_match = self._distinct_match if distinct else (lambda r, s: _to_match(self.records[r], s))
+            out[i] = [to_match(r, s) for r, s in zip(top_r, top_s) if r >= 0]
         return out
 
     def match_batch(self, signature_texts: Sequence[str], failure_types: Optional[Sequence[Optional[str]]] = None,
-                    limit: int = MATCH_LIMIT, filter_first: bool = False) -> List[List[dict]]:
+                    limit: int = MATCH_LIMIT, filter_first: bool = False, distinct: bool = False) -> List[List[dict]]:
         """``filter_first=False`` (default): the reference's handler -- the best ``limit`` rows, THEN the failure_type
         filter, so rows of other types can leave fewer than ``limit`` (or no) matches.  ``filter_first=True``: the best
-        ``limit`` rows of the query's failure_type, searched on the device among that type's rows only."""
+        ``limit`` rows of the query's failure_type, searched on the device among that type's rows only.
+        ``distinct=True``: the best ``limit`` distinct failures, one per (failure_type, signature_text) key instead of
+        one per stored version, each reported with the fields of the key's newest record and the key's score."""
         if limit > MAX_LIMIT:
             raise ValueError(f"limit {limit} exceeds the {MAX_LIMIT} rows the fused top-k holds per query")
         with self._lock:
@@ -499,10 +579,13 @@ class GfkbStore:
                 return [[] for _ in signature_texts]  # app.py:82-83
             self._sync()
             if filter_first and failure_types is not None and any(failure_types):
-                return self._match_filter_first(signature_texts, failure_types, limit)
+                return self._match_filter_first(signature_texts, failure_types, limit, distinct)
             fb = self.vocab.featurize(list(signature_texts), grow=False)
             try:
-                rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit)
+                if distinct:
+                    rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit, distinct=True)
+                else:
+                    rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit)
             finally:
                 fb.close()
             out = []
@@ -510,7 +593,8 @@ class GfkbStore:
                 ft = failure_types[i] if failure_types is not None else None
                 matches = []
                 if amb[i]:  # float32 candidates cannot decide this query's top rows: full float64 scan
-                    top_r, top_s = self._exact_top(signature_texts[i], limit)
+                    top_r, top_s = (self._exact_top(signature_texts[i], limit, distinct=True) if distinct
+                                    else self._exact_top(signature_texts[i], limit))
                     self.stats["exact_fallbacks"] = self.stats.get("exact_fallbacks", 0) + 1
                 else:
                     top_r, top_s = rows[i, :limit].tolist(), f64[i, :limit].tolist()
@@ -520,12 +604,13 @@ class GfkbStore:
                     rec = self.records[r]
                     if ft and rec["failure_type"] != ft:
                         continue
-                    matches.append(_to_match(rec, s))
+                    matches.append(self._distinct_match(r, s) if distinct else _to_match(rec, s))
                 out.append(matches)
             return out
 
-    def match(self, signature_text: str, failure_type: Optional[str] = None, filter_first: bool = False) -> List[dict]:
-        return self.match_batch([signature_text], [failure_type], filter_first=filter_first)[0]
+    def match(self, signature_text: str, failure_type: Optional[str] = None, filter_first: bool = False,
+              distinct: bool = False) -> List[dict]:
+        return self.match_batch([signature_text], [failure_type], filter_first=filter_first, distinct=distinct)[0]
 
     def match_exact(self, signature_text: str, failure_type: Optional[str] = None, limit: int = MATCH_LIMIT) -> List[dict]:
         """The handler on the full float64 score vector (K1a on both segments): no candidate stage at all."""
