@@ -444,6 +444,38 @@ int kv_dense_range_fetch_device(kv_dense_index *dx, void *d_indptr, void *d_rows
 /* CUDA-event milliseconds of the GEMM kernel of the last kv_dense_topk* / kv_dense_selfjoin_device or range call (a
  * range re-run after the pair buffer grew included) and its row splits. */
 int kv_dense_last_timing(const kv_dense_index *dx, float *gemm_ms, int64_t *splits);
+/* Dense row deletion (tombstones), as kv_index_delete_rows.  rows[n]: local rows, any order; duplicates and rows already
+ * deleted are allowed (a call that deletes no new row changes nothing).  A deleted row keeps its row id and its position
+ * but no top-k, threshold search or self-join returns it again; a self-join query whose own row is deleted gets an empty
+ * list, (-inf, -1), and no threshold pairs.
+ *   - Like an append, a deletion needs kv_dense_finalize before the next search (until then: KV_ERR_STATE) and drops
+ *     any range result.  The finalize gives every deleted row a NaN inverse norm, which removes all its scores in the
+ *     epilogue: the kernels themselves do not change.
+ *   - The deleted set belongs to the handle: appends and finalizes keep it, appended rows are live.  Row labels
+ *     (kv_dense_set_row_labels) survive deletions.
+ *   - KV_ERR_INVALID: a row outside 0..kv_dense_rows-1, or rows == NULL with n > 0.
+ * kv_dense_live_rows: kv_dense_rows minus the deleted rows.  kv_dense_deleted_rows: out[n] = 1 for a deleted local row,
+ * 0 for a live one; n == kv_dense_rows (else KV_ERR_INVALID). */
+int kv_dense_delete_rows(kv_dense_index *dx, const int64_t *rows, int64_t n);
+int64_t kv_dense_live_rows(const kv_dense_index *dx);
+int kv_dense_deleted_rows(kv_dense_index *dx, uint8_t *out, int64_t n);
+/* Dense label filter.  kv_dense_set_row_labels gives every local row a label >= 0, labels[n] by local row, n ==
+ * kv_dense_rows (else KV_ERR_INVALID, as for a negative label); NULL clears.  Labels may be set before or after
+ * finalize; finalize and deletions keep them, an append drops them.
+ * kv_dense_set_query_filter restricts each query of THE NEXT SEARCH CALL on the handle (kv_dense_topk, _topk_device,
+ * _selfjoin_device, _range, _range_device or _selfjoin_range) to the rows carrying labels[q] (-1: every row); NULL
+ * clears.  That call must have exactly n_q queries (else KV_ERR_INVALID) and clears the filter whether it succeeds or
+ * fails; an append or a finalize clears it too.  A filtered query's top-k is the top-k over its label's live rows --
+ * (score desc, row asc), the same float32 scores as unfiltered, (-inf, -1) past its label's last candidate -- and its
+ * threshold search returns the unfiltered pairs of its label; a -1 query gets the unfiltered answer.  The kernel skips
+ * every (128-query tile, 256-row tile) item whose row tile holds no live row of a label of the query tile.
+ * KV_ERR_INVALID: a query label below -1 (here) or a query count that differs (at the search).  KV_ERR_STATE: a
+ * filtered search on an index whose labels are missing or stale (appended rows). */
+int kv_dense_set_row_labels(kv_dense_index *dx, const int32_t *labels, int64_t n);
+int kv_dense_set_query_filter(kv_dense_index *dx, const int32_t *labels, int64_t n_q);
+/* Measurement and test hook: the (query tile, row tile) items the last dense search's kernel skipped and its total
+ * items (q_tiles x r_tiles; skipped is 0 for an unfiltered search). */
+int kv_dense_last_skipped(const kv_dense_index *dx, int64_t *skipped, int64_t *items);
 
 /* ------------------------------------------------------------------------------------
  * K4: 64-bit fingerprint exact-match index.  One uint64 per row = the leading 64 bits of

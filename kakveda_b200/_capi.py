@@ -116,6 +116,12 @@ SIGNATURES = {
     "kv_dense_range_fetch": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f32p]),
     "kv_dense_range_fetch_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kv_dense_last_timing": (C.c_int, [C.c_void_p, c_f32p, c_i64p]),
+    "kv_dense_delete_rows": (C.c_int, [C.c_void_p, c_i64p, C.c_int64]),
+    "kv_dense_live_rows": (C.c_int64, [C.c_void_p]),
+    "kv_dense_deleted_rows": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint8), C.c_int64]),
+    "kv_dense_set_row_labels": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int64]),
+    "kv_dense_set_query_filter": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int64]),
+    "kv_dense_last_skipped": (C.c_int, [C.c_void_p, c_i64p, c_i64p]),
     "kv_hash_create": (C.c_int, [C.c_int, C.c_int64, C.POINTER(C.c_void_p)]),
     "kv_hash_destroy": (None, [C.c_void_p]),
     "kv_hash_append": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.c_int64]),

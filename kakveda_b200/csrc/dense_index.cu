@@ -31,6 +31,7 @@
 
 #include <algorithm>
 #include <cstdlib>
+#include <cstring>
 #include <memory>
 #include <mutex>
 #include <vector>
@@ -108,6 +109,18 @@ struct DenseRangeOut {
   unsigned long long cap;
 };
 
+// Label filter of one search (dense_topk_kernel<*, true>; the unfiltered forms ignore this argument).  The queries
+// are in kernel order: stable-sorted by label, so that a 128-query tile holds few labels.  Query p (kernel order) is
+// the call's query qperm[p]: its partial lists, its range records and its self-join exclusion use that index.
+struct DenseFilter {
+  const int *lab_c;                     // [n_rows] row labels (>= 0)
+  const int *lab_q;                     // [n_q] query labels, kernel order (-1: any row)
+  const int64_t *qperm;                 // [n_q] original query index of kernel query p
+  const unsigned long long *tile_sig;   // [r_tiles] OR of 1 << (label & 63) over the tile's live rows
+  const unsigned long long *qsig;       // [q_tiles] the same over the tile's queries (all ones: an unfiltered query)
+  unsigned long long *skipped;          // (query tile, row tile) items skipped, counted by the producers
+};
+
 // order-preserving float <-> unsigned key (cosines may be negative)
 __device__ __forceinline__ unsigned int fkey(float f) {
   unsigned int b = __float_as_uint(f);
@@ -123,6 +136,7 @@ struct __align__(1024) DenseSmem {
   __align__(16) float inv_c[2][BN];
   float lscore[2][MAXK][BM];  // [column half][slot][query]: the 32 lanes of a warp hit 32 different banks
   int lrow[2][MAXK][BM];
+  int lab_c[2][BN];  // FILTER: this tile's row labels (-1 past the end); last, so the other members keep their offsets
 };
 
 // K2-R: appends this thread's pairs of one 16-column group (columns c0 + {0, 1, 4, 5, 8, 9, 12, 13} of the tile at
@@ -157,10 +171,13 @@ __device__ __forceinline__ void dense_emit(const DenseParams &P, const DenseRang
   }
 }
 
-template <bool RANGE>
+// FILTER: query p only matches rows labelled F.lab_q[p] (-1: any row).  An item whose row tile holds no live row of
+// any label of its query tile (tile_sig & qsig == 0; a signature has no false negatives) is skipped by the producer
+// (no loads) and by the consumers (no MMAs, ring waits or epilogue) alike, so the ring's stage and phase stay in step.
+template <bool RANGE, bool FILTER>
 __global__ void __launch_bounds__(N_THREADS, 1)
 dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c, DenseParams P,
-                  DenseRangeOut R) {
+                  DenseRangeOut R, DenseFilter F) {
   extern __shared__ unsigned char smem_raw[];
   DenseSmem &S = *reinterpret_cast<DenseSmem *>(smem_raw + smem_align1024(smem_raw));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -184,9 +201,13 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
+      unsigned long long n_skip = 0;
       for (int64_t L = L0; L < L1; L++) {
         const int qtile = (int)(L / P.r_tiles);
         const int64_t t = L % P.r_tiles;
+        if constexpr (FILTER) {
+          if ((F.tile_sig[t] & F.qsig[qtile]) == 0) { n_skip++; continue; }
+        }
         for (int kb = 0; kb < n_kb; kb++) {
           mbar_wait(&S.empty_bar[stage], phase ^ 1);
           mbar_expect_tx(&S.full_bar[stage], STAGE_BYTES);
@@ -194,6 +215,9 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
           tma_load_2d(S.stage[stage] + A_BYTES, &map_c, &S.full_bar[stage], kb * BK, (int)(t * BN));
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
+      }
+      if constexpr (FILTER) {
+        if (n_skip) atomicAdd(F.skipped, n_skip);
       }
     }
   } else {
@@ -221,11 +245,13 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
     float gth = -INFINITY;  // k-th score another CTA already secured for this query: ties may still win on row id
     float gth_pred = -INFINITY;  // largest float below gth (-0 is not below +0)
     float lo = INFINITY;         // a row enters the list iff its score > lo
+    int qlab = -1;               // FILTER: this thread's query label (-1: any row)
+    int64_t qo = 0;              // FILTER: the call's index of this thread's query, qperm[q]
     auto flush = [&]() {    // publish the list of (cur_qtile, this CTA)
       if (cur_qtile < 0 || !q_ok) return;
       const int slot = (int)my_split * 2 + half;
       for (int j = 0; j < k; j++) {
-        const size_t o = ((size_t)slot * P.n_q + q) * k + j;
+        const size_t o = ((size_t)slot * P.n_q + (FILTER ? qo : q)) * k + j;
         P.part_scores[o] = j < cnt ? ls[j * BM] : -INFINITY;
         P.part_rows[o] = j < cnt ? (long long)(P.row_base + lr[j * BM]) : -1LL;
       }
@@ -239,36 +265,46 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
     for (int64_t L = L0; L < L1; L++, it++) {
       const int qtile = (int)(L / P.r_tiles);
       const int64_t t = L % P.r_tiles;
-      // ---- MMA over the K slices; a slice's ring slot is released once the next slice's MMAs are issued and the
-      //      slice's own have completed ----
-#pragma unroll
-      for (int i = 0; i < 128; i++) wgmma_reg_fence(acc[i]);
-      wgmma_fence();
+      bool skip = false;  // (CTA-uniform) the producer issued no loads for this item
+      if constexpr (FILTER) skip = (F.tile_sig[t] & F.qsig[qtile]) == 0;
       int prev = -1;
-      for (int kb = 0; kb < n_kb; kb++) {
-        mbar_wait(&S.full_bar[stage], phase);
-        const uint64_t da = wgmma_desc_sw128(S.stage[stage] + wg * (A_BYTES / 2));  // rows 64 wg .. 64 wg + 63 of the tile
-        const uint64_t db = wgmma_desc_sw128(S.stage[stage] + A_BYTES);
+      if (!skip) {
+        // ---- MMA over the K slices; a slice's ring slot is released once the next slice's MMAs are issued and the
+        //      slice's own have completed ----
 #pragma unroll
-        for (int kk = 0; kk < BK / UMMA_K; kk++)  // advance 32 bytes (2 x 16-byte units) per K=16 step inside the swizzle row
-          wgmma_m64n256k16_bf16(acc, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), (uint32_t)((kb | kk) != 0));
-        wgmma_commit();
-        if (prev >= 0) {
-          wgmma_wait<1>();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&S.empty_bar[prev]);
+        for (int i = 0; i < 128; i++) wgmma_reg_fence(acc[i]);
+        wgmma_fence();
+        for (int kb = 0; kb < n_kb; kb++) {
+          mbar_wait(&S.full_bar[stage], phase);
+          const uint64_t da = wgmma_desc_sw128(S.stage[stage] + wg * (A_BYTES / 2));  // rows 64 wg .. 64 wg + 63 of the tile
+          const uint64_t db = wgmma_desc_sw128(S.stage[stage] + A_BYTES);
+#pragma unroll
+          for (int kk = 0; kk < BK / UMMA_K; kk++)  // advance 32 bytes (2 x 16-byte units) per K=16 step inside the swizzle row
+            wgmma_m64n256k16_bf16(acc, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), (uint32_t)((kb | kk) != 0));
+          wgmma_commit();
+          if (prev >= 0) {
+            wgmma_wait<1>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&S.empty_bar[prev]);
+          }
+          prev = stage;
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        prev = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      // the query-tile switch runs for a skipped item too: a query tile whose first row tiles are all skipped must
+      // still publish the previous tile's lists and start its own
       if (qtile != cur_qtile) {  // (CTA-uniform) next query tile: publish and restart the lists
         if constexpr (!RANGE) flush();
         cur_qtile = qtile;
         q = (int64_t)qtile * BM + qi;
         q_ok = q < P.n_q;
         inv_q = q_ok ? P.inv_norm_q[q] : 0.f;
+        if constexpr (FILTER) {
+          qlab = q_ok ? F.lab_q[q] : -1;
+          qo = q_ok ? F.qperm[q] : q;
+        }
         {
-          const int64_t e = P.excl_base >= 0 ? P.excl_base + q - P.row_base : -1;
+          const int64_t e = P.excl_base >= 0 ? P.excl_base + (FILTER ? qo : q) - P.row_base : -1;
           excl = (e >= 0 && e < P.n_rows) ? (int)e : -1;
         }
         if constexpr (!RANGE) {
@@ -278,10 +314,18 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
           for (int j = 0; j < k; j++) { ls[j * BM] = -INFINITY; lr[j * BM] = 0x7fffffff; }
         }
       }
+      if constexpr (FILTER) {
+        // `it` counts the tiles whose inverse norms and labels were staged: the double buffer alternates between
+        // processed tiles only
+        if (skip) { it--; continue; }
+      }
       const int as = (int)(it & 1);
       // inverse norms of this tile's rows (0 past the end; such rows are rejected by index below)
       const int64_t row0 = t * BN;
       for (int c = et; c < BN; c += EPI_THREADS) S.inv_c[as][c] = (row0 + c < P.n_rows) ? P.inv_norm_c[row0 + c] : -INFINITY;  // 0 * -inf = NaN: never a candidate
+      if constexpr (FILTER) {
+        for (int c = et; c < BN; c += EPI_THREADS) S.lab_c[as][c] = (row0 + c < P.n_rows) ? F.lab_c[row0 + c] : -1;
+      }
       if constexpr (!RANGE) {
         if (q_ok) {
           const unsigned int gk = *(volatile unsigned int *)&P.gthr[q];
@@ -315,14 +359,29 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
       if (P.dbg == 2) { if (acc[0] == 1.2345678f && acc[127] == 9.87654321f) thr = 1.f; continue; }
       // per 8 values (16 columns): scale, max -> one branch; only groups where some query of the warp has a
       // candidate are walked element by element (`sc > lo` == `sc > thr && sc >= gth`, lo = max(thr, pred(gth)))
+      // A NaN scale removes an element: a deleted row's inverse norm is NaN (kv_dense_finalize), and so is the scale of
+      // a row outside a filtered query's label here, and a deleted self-join query's inv_q.  fmaxf drops NaN operands,
+      // and NaN fails every `> lo` and `>= thr` test, so such an element is never a candidate and never emitted.  Neither
+      // edge case turns NaN into a number: a zero query has inv_q = 0 and NaN * 0 is NaN; a padded row (past n_rows)
+      // is never deleted and has the -inf scale, whose products are -inf or NaN (0 * -inf) and fail the same tests.
 #pragma unroll
       for (int sb = 0; sb < 16; sb++) {
         float tv[8];
 #pragma unroll
         for (int jj = 0; jj < 2; jj++) {
           const int j = 2 * sb + jj;
-          const float2 icl = *reinterpret_cast<const float2 *>(&S.inv_c[as][8 * j + cofs]);
-          const float2 ich = *reinterpret_cast<const float2 *>(&S.inv_c[as][8 * j + 4 + cofs]);
+          float2 icl = *reinterpret_cast<const float2 *>(&S.inv_c[as][8 * j + cofs]);
+          float2 ich = *reinterpret_cast<const float2 *>(&S.inv_c[as][8 * j + 4 + cofs]);
+          if constexpr (FILTER) {
+            if (qlab >= 0) {
+              const int2 ll = *reinterpret_cast<const int2 *>(&S.lab_c[as][8 * j + cofs]);
+              const int2 lh = *reinterpret_cast<const int2 *>(&S.lab_c[as][8 * j + 4 + cofs]);
+              if (ll.x != qlab) icl.x = __int_as_float(0x7fc00000);
+              if (ll.y != qlab) icl.y = __int_as_float(0x7fc00000);
+              if (lh.x != qlab) ich.x = __int_as_float(0x7fc00000);
+              if (lh.y != qlab) ich.y = __int_as_float(0x7fc00000);
+            }
+          }
           tv[4 * jj + 0] = acc[4 * j + 0] * icl.x;
           tv[4 * jj + 1] = acc[4 * j + 1] * icl.y;
           tv[4 * jj + 2] = acc[4 * j + 2] * ich.x;
@@ -334,7 +393,7 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
         if constexpr (RANGE) {
           // inv_q > 0 and rounding is monotone, so no score of the group reaches thr unless best does (zero and
           // padded queries have inv_q = 0: best is 0 or NaN)
-          if (__any_sync(FULL_MASK, best >= R.thr)) dense_emit(P, R, tv, inv_q, (int)q, row0, 16 * sb + cofs, excl);
+          if (__any_sync(FULL_MASK, best >= R.thr)) dense_emit(P, R, tv, inv_q, (int)(FILTER ? qo : q), row0, 16 * sb + cofs, excl);
         } else {
           if (best > lo) {
 #pragma unroll  // static indices keep tv[] in registers
@@ -378,6 +437,35 @@ __global__ void inv_norm_kernel(const __nv_bfloat16 *__restrict__ x, int64_t n, 
   if (lane == 0) out[r] = s > 0.0 ? (float)(1.0 / sqrt(s)) : 0.f;
 }
 
+// tombstones: x[idx[i]] = NaN (a deleted row's inverse norm, or a deleted self-join query's)
+__global__ void nan_scatter_kernel(float *x, const int64_t *__restrict__ idx, int64_t n) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i < n) x[idx[i]] = __int_as_float(0x7fc00000);
+}
+
+// one block of BN threads per 256-row tile: OR of 1 << (label & 63) over the tile's live rows (a deleted row has a NaN
+// inverse norm); an all-deleted tile gets 0
+__global__ void tile_sig_kernel(const int *__restrict__ lab, const float *__restrict__ inv_c, int64_t n,
+                                unsigned long long *sig) {
+  __shared__ unsigned long long s;
+  if (threadIdx.x == 0) s = 0;
+  __syncthreads();
+  const int64_t r = blockIdx.x * (int64_t)BN + threadIdx.x;
+  if (r < n && !isnan(inv_c[r])) atomicOr(&s, 1ull << (lab[r] & 63));
+  __syncthreads();
+  if (threadIdx.x == 0) sig[blockIdx.x] = s;
+}
+
+// dst[p] = src[perm[p]], bf16 rows of dim elements (dim a multiple of 64: 16-byte vectors)
+__global__ void gather_rows_kernel(const uint4 *__restrict__ src, const int64_t *__restrict__ perm, int64_t n, int vec_per_row,
+                                   uint4 *dst) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n * vec_per_row) return;
+  const int64_t p = i / vec_per_row;
+  const int v = (int)(i % vec_per_row);
+  dst[i] = src[perm[p] * vec_per_row + v];
+}
+
 }  // namespace
 
 struct kv_dense_index {
@@ -402,7 +490,94 @@ struct kv_dense_index {
   bool finalized = false;
   float last_ms = 0;
   int64_t last_splits = 0;
+  // row deletion: flags by local row (empty until the first deletion), applied as NaN inverse norms at every finalize
+  std::vector<uint8_t> h_dead;
+  int64_t n_dead = 0;
+  DevBuf<int64_t> d_dead;  // the deleted rows (finalize) or deleted self-join query positions (a search)
+  // row labels: kept by finalize and deletions, dropped by an append; the device copy and the tile signatures are
+  // rebuilt at every finalize and label upload
+  std::vector<int> h_labels;
+  bool has_labels = false;
+  DevBuf<int> d_lab_c;
+  DevBuf<unsigned long long> d_tile_sig;
+  // query filter of the next search call (kv_dense_set_query_filter), and that call's device inputs
+  std::vector<int> h_qfilter;
+  bool has_qfilter = false;
+  DevBuf<int> d_lab_q;
+  DevBuf<int64_t> d_qperm;
+  DevBuf<unsigned long long> d_qsig, d_skipped;
+  DevBuf<__nv_bfloat16> d_qf;  // the filtered call's queries in kernel order (when that order is not the identity)
+  int64_t last_skipped = 0, last_items = 0;
 };
+
+namespace {
+
+// A search call's query filter, taken from the handle (which it leaves cleared) and then laid out in kernel order.
+struct CallFilter {
+  bool on = false;               // some query is filtered: the FILTER kernel runs
+  std::vector<int> lab;          // [n_q] by original query
+  std::vector<int64_t> perm;     // [n_q] kernel order -> original query (stable sort by label)
+  bool identity = true;
+};
+
+// Takes (and clears) the handle's query filter for a call of n_q queries.  Caller holds dx->mu.
+int take_filter(kv_dense_index *dx, int64_t n_q, const char *fn, CallFilter &cf) {
+  const bool had = dx->has_qfilter;
+  dx->has_qfilter = false;
+  cf = CallFilter{};
+  if (!had) return KV_OK;
+  cf.lab.swap(dx->h_qfilter);
+  if ((int64_t)cf.lab.size() != n_q)
+    return kv_fail(KV_ERR_INVALID, "%s: the query filter has %lld labels for a call of %lld queries", fn, (long long)cf.lab.size(),
+                   (long long)n_q);
+  for (int l : cf.lab) cf.on = cf.on || l >= 0;
+  if (!cf.on) return KV_OK;  // every query unfiltered: the unfiltered call
+  if (!dx->has_labels || (int64_t)dx->h_labels.size() != dx->n_rows)
+    return kv_fail(KV_ERR_STATE, "%s: the index has no row labels for its current rows (kv_dense_set_row_labels)", fn);
+  cf.perm.resize((size_t)n_q);
+  for (int64_t i = 0; i < n_q; i++) cf.perm[(size_t)i] = i;
+  std::stable_sort(cf.perm.begin(), cf.perm.end(), [&](int64_t a, int64_t b) { return cf.lab[(size_t)a] < cf.lab[(size_t)b]; });
+  for (int64_t i = 0; i < n_q && cf.identity; i++) cf.identity = cf.perm[(size_t)i] == i;
+  return KV_OK;
+}
+
+// What an append of n rows changes besides the rows: the index needs a finalize, the row labels and the query filter
+// are dropped, the deleted rows stay deleted and the new rows are live.
+void dense_rows_appended(kv_dense_index *dx, int64_t n) {
+  dx->n_rows += n;
+  dx->rows.n = dx->n_rows * dx->dim;
+  dx->finalized = false;
+  dx->has_labels = false;
+  dx->h_labels.clear();
+  dx->has_qfilter = false;
+  if (!dx->h_dead.empty()) dx->h_dead.resize((size_t)dx->n_rows, 0);
+}
+
+// Rebuilds the tile signatures from the device labels and the inverse norms (NaN = deleted).  Needs a finalized index
+// with labels on the device.
+int build_tile_sig(kv_dense_index *dx) {
+  const int64_t r_tiles = (dx->n_rows + BN - 1) / BN;
+  if (!r_tiles) return KV_OK;
+  KV_CUDA(dx->d_tile_sig.ensure(r_tiles));
+  tile_sig_kernel<<<(unsigned)r_tiles, BN, 0, dx->stream>>>(dx->d_lab_c.p, dx->d_inv_c.p, dx->n_rows, dx->d_tile_sig.p);
+  KV_CUDA(cudaGetLastError());
+  KV_CUDA(cudaStreamSynchronize(dx->stream));
+  return KV_OK;
+}
+
+// Writes NaN at x[idx[i]] for the host list idx (through dx->d_dead).
+int scatter_nan(kv_dense_index *dx, float *x, const std::vector<int64_t> &idx) {
+  if (idx.empty()) return KV_OK;
+  const int64_t n = (int64_t)idx.size();
+  KV_CUDA(dx->d_dead.ensure(n));
+  KV_CUDA(cudaMemcpyAsync(dx->d_dead.p, idx.data(), (size_t)n * 8, cudaMemcpyHostToDevice, dx->stream));
+  nan_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, dx->stream>>>(x, dx->d_dead.p, n);
+  KV_CUDA(cudaGetLastError());
+  KV_CUDA(cudaStreamSynchronize(dx->stream));  // idx may be freed once this returns
+  return KV_OK;
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -419,8 +594,10 @@ int kv_dense_create(int device, int dim, int64_t row_base, kv_dense_index **out)
   dx->sm_count = sm_count;
   KV_CUDA(dx->stream.create());
   for (auto &e : dx->ev) KV_CUDA(e.create());
-  KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
-  KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
+  KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
+  KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
+  KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
+  KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
   *out = dx.release();
   return KV_OK;
 }
@@ -445,9 +622,7 @@ int kv_dense_append(kv_dense_index *dx, const uint16_t *rows_bf16, int64_t n) {
   KV_CUDA(dx->rows.reserve((dx->n_rows + n) * dx->dim, dx->stream));
   KV_CUDA(cudaMemcpyAsync(dx->rows.p + dx->n_rows * dx->dim, rows_bf16, (size_t)n * dx->dim * 2, cudaMemcpyHostToDevice, dx->stream));
   KV_CUDA(cudaStreamSynchronize(dx->stream));
-  dx->n_rows += n;
-  dx->rows.n = dx->n_rows * dx->dim;
-  dx->finalized = false;
+  dense_rows_appended(dx, n);
   return KV_OK;
 }
 
@@ -455,6 +630,7 @@ int kv_dense_finalize(kv_dense_index *dx) {
   if (!dx) return kv_fail(KV_ERR_INVALID, "kv_dense_finalize: NULL handle");
   std::lock_guard<std::mutex> g(dx->mu);
   dx->range_valid = false;
+  dx->has_qfilter = false;
   KV_CUDA(cudaSetDevice(dx->device));
   KV_CUDA(dx->d_inv_c.ensure(std::max<int64_t>(dx->n_rows, 1)));
   if (dx->n_rows) {
@@ -462,19 +638,127 @@ int kv_dense_finalize(kv_dense_index *dx) {
     KV_CUDA(cudaGetLastError());
   }
   KV_CUDA(cudaStreamSynchronize(dx->stream));
+  // tombstones: a deleted row's inverse norm is NaN, which removes every score of the row in the epilogue
+  if (dx->n_dead) {
+    std::vector<int64_t> dead;
+    dead.reserve((size_t)dx->n_dead);
+    for (int64_t r = 0; r < dx->n_rows; r++)
+      if (dx->h_dead[(size_t)r]) dead.push_back(r);
+    const int rc = scatter_nan(dx, dx->d_inv_c.p, dead);
+    if (rc != KV_OK) return rc;
+  }
+  if (dx->has_labels) {
+    const int rc = build_tile_sig(dx);
+    if (rc != KV_OK) return rc;
+  }
   dx->finalized = true;
+  return KV_OK;
+}
+
+int kv_dense_delete_rows(kv_dense_index *dx, const int64_t *rows, int64_t n) {
+  if (!dx || n < 0 || (n > 0 && !rows)) return kv_fail(KV_ERR_INVALID, "kv_dense_delete_rows: bad arguments");
+  std::lock_guard<std::mutex> g(dx->mu);
+  for (int64_t i = 0; i < n; i++)
+    if (rows[i] < 0 || rows[i] >= dx->n_rows)
+      return kv_fail(KV_ERR_INVALID, "kv_dense_delete_rows: row %lld outside 0..%lld", (long long)rows[i], (long long)dx->n_rows - 1);
+  int64_t added = 0;
+  for (int64_t i = 0; i < n; i++) {
+    if (dx->h_dead.empty()) dx->h_dead.assign((size_t)dx->n_rows, 0);
+    uint8_t &d = dx->h_dead[(size_t)rows[i]];
+    if (!d) { d = 1; added++; }
+  }
+  if (!added) return KV_OK;  // duplicates and rows deleted before: nothing changes
+  dx->n_dead += added;
+  // like an append: the inverse norms and tile signatures are stale until the next finalize
+  dx->finalized = false;
+  dx->range_valid = false;
+  return KV_OK;
+}
+
+int64_t kv_dense_live_rows(const kv_dense_index *dx) { return dx ? dx->n_rows - dx->n_dead : 0; }
+
+int kv_dense_deleted_rows(kv_dense_index *dx, uint8_t *out, int64_t n) {
+  if (!dx || n < 0 || (n > 0 && !out)) return kv_fail(KV_ERR_INVALID, "kv_dense_deleted_rows: bad arguments");
+  std::lock_guard<std::mutex> g(dx->mu);
+  if (n != dx->n_rows)
+    return kv_fail(KV_ERR_INVALID, "kv_dense_deleted_rows: %lld flags for an index of %lld rows", (long long)n, (long long)dx->n_rows);
+  if (dx->n_dead) memcpy(out, dx->h_dead.data(), (size_t)n);
+  else if (n) memset(out, 0, (size_t)n);
+  return KV_OK;
+}
+
+int kv_dense_set_row_labels(kv_dense_index *dx, const int32_t *labels, int64_t n) {
+  if (!dx) return kv_fail(KV_ERR_INVALID, "kv_dense_set_row_labels: NULL handle");
+  std::lock_guard<std::mutex> g(dx->mu);
+  if (!labels) {
+    dx->h_labels.clear();
+    dx->has_labels = false;
+    return KV_OK;
+  }
+  if (n != dx->n_rows)
+    return kv_fail(KV_ERR_INVALID, "kv_dense_set_row_labels: %lld labels for an index of %lld rows", (long long)n, (long long)dx->n_rows);
+  for (int64_t i = 0; i < n; i++)
+    if (labels[i] < 0) return kv_fail(KV_ERR_INVALID, "kv_dense_set_row_labels: label %d of row %lld is negative", labels[i], (long long)i);
+  KV_CUDA(cudaSetDevice(dx->device));
+  dx->has_labels = false;
+  dx->h_labels.assign(labels, labels + n);
+  KV_CUDA(dx->d_lab_c.ensure(std::max<int64_t>(n, 1)));
+  KV_CUDA(cudaMemcpyAsync(dx->d_lab_c.p, labels, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, dx->stream));
+  KV_CUDA(cudaStreamSynchronize(dx->stream));
+  dx->has_labels = true;
+  return dx->finalized ? build_tile_sig(dx) : KV_OK;  // else the next finalize builds the signatures
+}
+
+int kv_dense_set_query_filter(kv_dense_index *dx, const int32_t *labels, int64_t n_q) {
+  if (!dx || n_q < 0) return kv_fail(KV_ERR_INVALID, "kv_dense_set_query_filter: bad arguments");
+  std::lock_guard<std::mutex> g(dx->mu);
+  dx->has_qfilter = false;
+  if (!labels) return KV_OK;
+  for (int64_t q = 0; q < n_q; q++)
+    if (labels[q] < -1)
+      return kv_fail(KV_ERR_INVALID, "kv_dense_set_query_filter: label %d of query %lld is below -1", labels[q], (long long)q);
+  dx->h_qfilter.assign(labels, labels + n_q);
+  dx->has_qfilter = true;
+  return KV_OK;
+}
+
+int kv_dense_last_skipped(const kv_dense_index *dx, int64_t *skipped, int64_t *items) {
+  if (!dx || !skipped || !items) return kv_fail(KV_ERR_INVALID, "kv_dense_last_skipped: bad arguments");
+  *skipped = dx->last_skipped;
+  *items = dx->last_items;
   return KV_OK;
 }
 
 // What the top-k and the range scan of n_q queries already on the device (d_q: bf16 [n_q, dim], 16-byte aligned)
 // share: the queries' inverse norms, both tensor maps, the row splits (dx->last_splits) and every DenseParams field but
-// the epilogue's.  Needs n_rows > 0.
-static int dense_setup(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, int64_t excl_base, CUtensorMap *map_q,
-                       CUtensorMap *map_c, DenseParams &P) {
+// the epilogue's.  A filtered call (cf.on) runs on its queries in kernel order: d_q gathered into dx->d_qf unless that
+// order is the identity, and F filled.  sj_begin >= 0: the queries are the local rows sj_begin.., and a deleted one
+// gets a NaN inverse norm (an empty list, no pairs).  Needs n_rows > 0.
+static int dense_setup(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, int64_t excl_base, int64_t sj_begin,
+                       const CallFilter &cf, CUtensorMap *map_q, CUtensorMap *map_c, DenseParams &P, DenseFilter &F) {
   cudaStream_t s = dx->stream;
+  if (cf.on) {
+    KV_CUDA(dx->d_qperm.ensure(n_q));
+    KV_CUDA(cudaMemcpyAsync(dx->d_qperm.p, cf.perm.data(), (size_t)n_q * 8, cudaMemcpyHostToDevice, s));
+    if (!cf.identity) {
+      const int vpr = dx->dim / 8;  // 16-byte vectors per row
+      KV_CUDA(dx->d_qf.ensure(n_q * dx->dim));
+      gather_rows_kernel<<<(unsigned)((n_q * vpr + 255) / 256), 256, 0, s>>>((const uint4 *)d_q, dx->d_qperm.p, n_q, vpr,
+                                                                                (uint4 *)dx->d_qf.p);
+      KV_CUDA(cudaGetLastError());
+      d_q = dx->d_qf.p;
+    }
+  }
   KV_CUDA(dx->d_inv_q.ensure(n_q));
   inv_norm_kernel<<<(unsigned)((n_q * 32 + 255) / 256), 256, 0, s>>>(d_q, n_q, dx->dim, dx->d_inv_q.p);
   KV_CUDA(cudaGetLastError());
+  if (sj_begin >= 0 && dx->n_dead) {
+    std::vector<int64_t> dead_q;  // kernel positions of the deleted query rows
+    for (int64_t p = 0; p < n_q; p++)
+      if (dx->h_dead[(size_t)(sj_begin + (cf.on ? cf.perm[(size_t)p] : p))]) dead_q.push_back(p);
+    const int rc = scatter_nan(dx, dx->d_inv_q.p, dead_q);
+    if (rc != KV_OK) return rc;
+  }
   int rc = make_map_2d(map_q, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, d_q, n_q, dx->dim, BM);
   if (rc != KV_OK) return rc;
   rc = make_map_2d(map_c, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, dx->rows.p, dx->n_rows, dx->dim, BN);
@@ -500,13 +784,51 @@ static int dense_setup(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q
   P.r_tiles = r_tiles; P.q_tiles = q_tiles;
   P.dbg = getenv("KAKVEDA_B200_DENSE_DBG") ? atoi(getenv("KAKVEDA_B200_DENSE_DBG")) : 0;
   P.inv_norm_c = dx->d_inv_c.p; P.inv_norm_q = dx->d_inv_q.p;
+  dx->last_items = q_tiles * r_tiles;
+  dx->last_skipped = 0;
+  F = DenseFilter{};
+  if (cf.on) {
+    std::vector<int> lab_q((size_t)n_q);
+    std::vector<unsigned long long> qsig((size_t)q_tiles, 0ull);
+    for (int64_t p = 0; p < n_q; p++) {
+      const int l = cf.lab[(size_t)cf.perm[(size_t)p]];
+      lab_q[(size_t)p] = l;
+      qsig[(size_t)(p / BM)] |= l < 0 ? ~0ull : 1ull << (l & 63);
+    }
+    KV_CUDA(dx->d_lab_q.ensure(n_q)); KV_CUDA(dx->d_qsig.ensure(q_tiles)); KV_CUDA(dx->d_skipped.ensure(1));
+    KV_CUDA(cudaMemcpyAsync(dx->d_lab_q.p, lab_q.data(), (size_t)n_q * sizeof(int), cudaMemcpyHostToDevice, s));
+    KV_CUDA(cudaMemcpyAsync(dx->d_qsig.p, qsig.data(), (size_t)q_tiles * 8, cudaMemcpyHostToDevice, s));
+    KV_CUDA(cudaMemsetAsync(dx->d_skipped.p, 0, 8, s));
+    F.lab_c = dx->d_lab_c.p; F.lab_q = dx->d_lab_q.p; F.qperm = dx->d_qperm.p;
+    F.tile_sig = dx->d_tile_sig.p; F.qsig = dx->d_qsig.p; F.skipped = dx->d_skipped.p;
+  }
+  return KV_OK;
+}
+
+// launches the top-k or the threshold (range) form of K2, filtered when F.qperm is set
+static void dense_launch(bool range, cudaStream_t s, int64_t grid, const CUtensorMap &map_q, const CUtensorMap &map_c,
+                         const DenseParams &P, const DenseRangeOut &R, const DenseFilter &F) {
+  const size_t smem = sizeof(DenseSmem) + 1024;
+  if (range && F.qperm) dense_topk_kernel<true, true><<<(unsigned)grid, N_THREADS, smem, s>>>(map_q, map_c, P, R, F);
+  else if (range) dense_topk_kernel<true, false><<<(unsigned)grid, N_THREADS, smem, s>>>(map_q, map_c, P, R, F);
+  else if (F.qperm) dense_topk_kernel<false, true><<<(unsigned)grid, N_THREADS, smem, s>>>(map_q, map_c, P, R, F);
+  else dense_topk_kernel<false, false><<<(unsigned)grid, N_THREADS, smem, s>>>(map_q, map_c, P, R, F);
+}
+
+// after a filtered kernel (stream synchronized): its skip count
+static int read_skipped(kv_dense_index *dx, const DenseFilter &F) {
+  if (!F.qperm) return KV_OK;
+  unsigned long long v = 0;
+  KV_CUDA(cudaMemcpy(&v, F.skipped, 8, cudaMemcpyDeviceToHost));
+  dx->last_skipped = (int64_t)v;
   return KV_OK;
 }
 
 // scan + merge of n_q queries already on the device (d_q: bf16 [n_q, dim], 16-byte aligned) into device buffers
-static int dense_run(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, int k, int64_t excl_base, float *d_out_s,
-                     long long *d_out_r) {
+static int dense_run(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, int k, int64_t excl_base, int64_t sj_begin,
+                     const CallFilter &cf, float *d_out_s, long long *d_out_r) {
   cudaStream_t s = dx->stream;
+  dx->last_items = dx->last_skipped = 0;
   if (dx->n_rows == 0) {
     KV_CUDA(cudaMemsetAsync(d_out_r, 0xFF, (size_t)n_q * k * 8, s));  // row -1
     std::vector<float> neg((size_t)(n_q * k), -INFINITY);
@@ -516,7 +838,8 @@ static int dense_run(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, 
   }
   CUtensorMap map_q, map_c;
   DenseParams P;
-  int rc = dense_setup(dx, d_q, n_q, excl_base, &map_q, &map_c, P);
+  DenseFilter F;
+  int rc = dense_setup(dx, d_q, n_q, excl_base, sj_begin, cf, &map_q, &map_c, P, F);
   if (rc != KV_OK) return rc;
   const int64_t n_part = (int64_t)P.n_lists * 2;  // two epilogue threads (column halves) per query and CTA
   KV_CUDA(dx->d_part_s.ensure(n_part * n_q * k)); KV_CUDA(dx->d_part_r.ensure(n_part * n_q * k));
@@ -530,11 +853,13 @@ static int dense_run(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, 
   P.part_scores = dx->d_part_s.p; P.part_rows = dx->d_part_r.p;
   const int64_t grid = P.q_tiles * P.n_lists;
   KV_CUDA(cudaEventRecord(dx->ev[0], s));
-  dense_topk_kernel<false><<<(unsigned)grid, N_THREADS, sizeof(DenseSmem) + 1024, s>>>(map_q, map_c, P, DenseRangeOut{});
+  dense_launch(false, s, grid, map_q, map_c, P, DenseRangeOut{}, F);
   KV_CUDA(cudaGetLastError());
   KV_CUDA(cudaEventRecord(dx->ev[1], s));
   KV_CUDA(cudaStreamSynchronize(s));
   cudaEventElapsedTime(&dx->last_ms, dx->ev[0], dx->ev[1]);
+  rc = read_skipped(dx, F);
+  if (rc != KV_OK) return rc;
   return kv_merge_topk_device(dx->device, dx->d_part_s.p, dx->d_part_r.p, (int)n_part, n_q, k, d_out_s, d_out_r);
 }
 
@@ -544,15 +869,17 @@ static int dense_run(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, 
 // and the kernel runs once more -- the whole GEMM again, since the pairs are only known in its epilogue.  last_ms sums
 // both runs.  Caller holds dx->mu.
 static int dense_range(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, float thr, int64_t excl_base,
-                       int64_t *n_pairs) {
+                       int64_t sj_begin, const CallFilter &cf, int64_t *n_pairs) {
   cudaStream_t s = dx->stream;
   unsigned long long count = 0;
   float total_ms = 0.f;
   dx->last_splits = 0;
+  dx->last_items = dx->last_skipped = 0;
   if (dx->n_rows > 0 && n_q > 0) {
     CUtensorMap map_q, map_c;
     DenseParams P;
-    int rc = dense_setup(dx, d_q, n_q, excl_base, &map_q, &map_c, P);
+    DenseFilter F;
+    int rc = dense_setup(dx, d_q, n_q, excl_base, sj_begin, cf, &map_q, &map_c, P, F);
     if (rc != KV_OK) return rc;
     KV_CUDA(dx->d_range.ensure(65536));
     KV_CUDA(dx->d_range_count.ensure(1));
@@ -564,8 +891,9 @@ static int dense_range(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q
       R.out = dx->d_range.p;
       R.cap = (unsigned long long)dx->d_range.cap;
       KV_CUDA(cudaMemsetAsync(dx->d_range_count.p, 0, sizeof(unsigned long long), s));
+      if (F.qperm) KV_CUDA(cudaMemsetAsync(F.skipped, 0, 8, s));
       KV_CUDA(cudaEventRecord(dx->ev[0], s));
-      dense_topk_kernel<true><<<(unsigned)grid, N_THREADS, sizeof(DenseSmem) + 1024, s>>>(map_q, map_c, P, R);
+      dense_launch(true, s, grid, map_q, map_c, P, R, F);
       KV_CUDA(cudaGetLastError());
       KV_CUDA(cudaEventRecord(dx->ev[1], s));
       KV_CUDA(cudaMemcpyAsync(&count, dx->d_range_count.p, sizeof(count), cudaMemcpyDeviceToHost, s));
@@ -573,6 +901,8 @@ static int dense_range(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q
       float ms = 0.f;
       cudaEventElapsedTime(&ms, dx->ev[0], dx->ev[1]);
       total_ms += ms;
+      rc = read_skipped(dx, F);
+      if (rc != KV_OK) return rc;
       if (count <= R.cap) break;
       if (dx->d_range.ensure((int64_t)count) != cudaSuccess) {
         cudaGetLastError();
@@ -589,21 +919,27 @@ static int dense_range(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q
   return KV_OK;
 }
 
+// The entry points below take the handle's query filter first and leave it cleared, whether they succeed or fail.
+
 // q: n_q x dim bfloat16 bit patterns (host).  Outputs (host): scores float32[n_q*k], rows int64[n_q*k],
 // ordered by (score desc, row asc); unused slots (-inf, -1).
 int kv_dense_topk(kv_dense_index *dx, const uint16_t *q_bf16, int64_t n_q, int k, float *out_scores, int64_t *out_rows) {
-  if (!dx || n_q < 0 || k < 1 || k > MAXK || (n_q > 0 && (!q_bf16 || !out_scores || !out_rows)))
-    return kv_fail(KV_ERR_INVALID, "kv_dense_topk: bad arguments (k must be 1..32)");
+  if (!dx) return kv_fail(KV_ERR_INVALID, "kv_dense_topk: bad arguments (k must be 1..32)");
   std::lock_guard<std::mutex> g(dx->mu);
+  CallFilter cf;
+  const int frc = take_filter(dx, n_q, "kv_dense_topk", cf);
+  if (n_q < 0 || k < 1 || k > MAXK || (n_q > 0 && (!q_bf16 || !out_scores || !out_rows)))
+    return kv_fail(KV_ERR_INVALID, "kv_dense_topk: bad arguments (k must be 1..32)");
   dx->range_valid = false;
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_topk: index not finalized");
+  if (frc != KV_OK) return frc;
   if (n_q == 0) return KV_OK;
   KV_CUDA(cudaSetDevice(dx->device));
   cudaStream_t s = dx->stream;
   KV_CUDA(dx->d_q.ensure(n_q * dx->dim));
   KV_CUDA(cudaMemcpyAsync(dx->d_q.p, q_bf16, (size_t)n_q * dx->dim * 2, cudaMemcpyHostToDevice, s));
   KV_CUDA(dx->d_out_s.ensure(n_q * k)); KV_CUDA(dx->d_out_r.ensure(n_q * k));
-  int rc = dense_run(dx, dx->d_q.p, n_q, k, -1, dx->d_out_s.p, dx->d_out_r.p);
+  int rc = dense_run(dx, dx->d_q.p, n_q, k, -1, -1, cf, dx->d_out_s.p, dx->d_out_r.p);
   if (rc != KV_OK) return rc;
   KV_CUDA(cudaMemcpy(out_scores, dx->d_out_s.p, (size_t)n_q * k * 4, cudaMemcpyDeviceToHost));
   KV_CUDA(cudaMemcpy(out_rows, dx->d_out_r.p, (size_t)n_q * k * 8, cudaMemcpyDeviceToHost));
@@ -612,15 +948,19 @@ int kv_dense_topk(kv_dense_index *dx, const uint16_t *q_bf16, int64_t n_q, int k
 
 int kv_dense_topk_device(kv_dense_index *dx, const void *d_q_bf16, int64_t n_q, int k, int64_t exclude_base, void *d_scores,
                          void *d_rows) {
-  if (!dx || n_q < 0 || k < 1 || k > MAXK || (n_q > 0 && (!d_q_bf16 || !d_scores || !d_rows)))
+  if (!dx) return kv_fail(KV_ERR_INVALID, "kv_dense_topk_device: bad arguments (k must be 1..32)");
+  std::lock_guard<std::mutex> g(dx->mu);
+  CallFilter cf;
+  const int frc = take_filter(dx, n_q, "kv_dense_topk_device", cf);
+  if (n_q < 0 || k < 1 || k > MAXK || (n_q > 0 && (!d_q_bf16 || !d_scores || !d_rows)))
     return kv_fail(KV_ERR_INVALID, "kv_dense_topk_device: bad arguments (k must be 1..32)");
   if (((uintptr_t)d_q_bf16 & 15) != 0) return kv_fail(KV_ERR_INVALID, "kv_dense_topk_device: queries must be 16-byte aligned");
-  std::lock_guard<std::mutex> g(dx->mu);
   dx->range_valid = false;
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_topk_device: index not finalized");
+  if (frc != KV_OK) return frc;
   if (n_q == 0) return KV_OK;
   KV_CUDA(cudaSetDevice(dx->device));
-  return dense_run(dx, (const __nv_bfloat16 *)d_q_bf16, n_q, k, exclude_base, (float *)d_scores, (long long *)d_rows);
+  return dense_run(dx, (const __nv_bfloat16 *)d_q_bf16, n_q, k, exclude_base, -1, cf, (float *)d_scores, (long long *)d_rows);
 }
 
 // rows already on the device (e.g. a torch tensor): device-to-device append
@@ -634,67 +974,82 @@ int kv_dense_append_device(kv_dense_index *dx, const void *d_rows_bf16, int64_t 
   KV_CUDA(dx->rows.reserve((dx->n_rows + n) * dx->dim, dx->stream));
   KV_CUDA(cudaMemcpyAsync(dx->rows.p + dx->n_rows * dx->dim, d_rows_bf16, (size_t)n * dx->dim * 2, cudaMemcpyDeviceToDevice, dx->stream));
   KV_CUDA(cudaStreamSynchronize(dx->stream));
-  dx->n_rows += n;
-  dx->rows.n = dx->n_rows * dx->dim;
-  dx->finalized = false;
+  dense_rows_appended(dx, n);
   return KV_OK;
 }
 
 // all-pairs (BASELINE configs[3]): local rows [q_begin, q_end) as queries against the whole shard, each row's own
 // entry excluded; outputs on the device
 int kv_dense_selfjoin_device(kv_dense_index *dx, int64_t q_begin, int64_t q_end, int k, void *d_scores, void *d_rows) {
-  if (!dx || q_begin < 0 || q_end < q_begin || k < 1 || k > MAXK || !d_scores || !d_rows)
-    return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_device: bad arguments (k must be 1..32)");
+  if (!dx) return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_device: bad arguments (k must be 1..32)");
   std::lock_guard<std::mutex> g(dx->mu);
+  CallFilter cf;
+  const int frc = take_filter(dx, q_end - q_begin, "kv_dense_selfjoin_device", cf);
+  if (q_begin < 0 || q_end < q_begin || k < 1 || k > MAXK || !d_scores || !d_rows)
+    return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_device: bad arguments (k must be 1..32)");
   dx->range_valid = false;
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_selfjoin_device: index not finalized");
   if (q_end > dx->n_rows) return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_device: row range outside the index");
+  if (frc != KV_OK) return frc;
   if (q_end == q_begin) return KV_OK;
   KV_CUDA(cudaSetDevice(dx->device));
-  return dense_run(dx, dx->rows.p + q_begin * dx->dim, q_end - q_begin, k, dx->row_base + q_begin, (float *)d_scores,
-                   (long long *)d_rows);
+  return dense_run(dx, dx->rows.p + q_begin * dx->dim, q_end - q_begin, k, dx->row_base + q_begin, q_begin, cf,
+                   (float *)d_scores, (long long *)d_rows);
 }
 
 static bool valid_threshold(float thr) { return thr > 0.f && thr <= 1.f; }  // false for NaN
 
 int kv_dense_range(kv_dense_index *dx, const uint16_t *q_bf16, int64_t n_q, float threshold, int64_t *n_pairs) {
-  if (!dx || !n_pairs || n_q < 0 || n_q >= (1LL << 31) || (n_q > 0 && !q_bf16))
+  if (!dx) return kv_fail(KV_ERR_INVALID, "kv_dense_range: bad arguments (n_q must be below 2^31)");
+  std::lock_guard<std::mutex> g(dx->mu);
+  CallFilter cf;
+  const int frc = take_filter(dx, n_q, "kv_dense_range", cf);
+  if (!n_pairs || n_q < 0 || n_q >= (1LL << 31) || (n_q > 0 && !q_bf16))
     return kv_fail(KV_ERR_INVALID, "kv_dense_range: bad arguments (n_q must be below 2^31)");
   if (!valid_threshold(threshold)) return kv_fail(KV_ERR_INVALID, "kv_dense_range: threshold must be in (0, 1]");
-  std::lock_guard<std::mutex> g(dx->mu);
   dx->range_valid = false;
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_range: index not finalized");
+  if (frc != KV_OK) return frc;
   KV_CUDA(cudaSetDevice(dx->device));
   if (n_q > 0 && dx->n_rows > 0) {
     KV_CUDA(dx->d_q.ensure(n_q * dx->dim));
     KV_CUDA(cudaMemcpyAsync(dx->d_q.p, q_bf16, (size_t)n_q * dx->dim * 2, cudaMemcpyHostToDevice, dx->stream));
   }
-  return dense_range(dx, dx->d_q.p, n_q, threshold, -1, n_pairs);
+  return dense_range(dx, dx->d_q.p, n_q, threshold, -1, -1, cf, n_pairs);
 }
 
 int kv_dense_range_device(kv_dense_index *dx, const void *d_q_bf16, int64_t n_q, float threshold, int64_t exclude_base,
                           int64_t *n_pairs) {
-  if (!dx || !n_pairs || n_q < 0 || n_q >= (1LL << 31) || (n_q > 0 && !d_q_bf16))
+  if (!dx) return kv_fail(KV_ERR_INVALID, "kv_dense_range_device: bad arguments (n_q must be below 2^31)");
+  std::lock_guard<std::mutex> g(dx->mu);
+  CallFilter cf;
+  const int frc = take_filter(dx, n_q, "kv_dense_range_device", cf);
+  if (!n_pairs || n_q < 0 || n_q >= (1LL << 31) || (n_q > 0 && !d_q_bf16))
     return kv_fail(KV_ERR_INVALID, "kv_dense_range_device: bad arguments (n_q must be below 2^31)");
   if (((uintptr_t)d_q_bf16 & 15) != 0) return kv_fail(KV_ERR_INVALID, "kv_dense_range_device: queries must be 16-byte aligned");
   if (!valid_threshold(threshold)) return kv_fail(KV_ERR_INVALID, "kv_dense_range_device: threshold must be in (0, 1]");
-  std::lock_guard<std::mutex> g(dx->mu);
   dx->range_valid = false;
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_range_device: index not finalized");
+  if (frc != KV_OK) return frc;
   KV_CUDA(cudaSetDevice(dx->device));
-  return dense_range(dx, (const __nv_bfloat16 *)d_q_bf16, n_q, threshold, exclude_base, n_pairs);
+  return dense_range(dx, (const __nv_bfloat16 *)d_q_bf16, n_q, threshold, exclude_base, -1, cf, n_pairs);
 }
 
 int kv_dense_selfjoin_range(kv_dense_index *dx, int64_t q_begin, int64_t q_end, float threshold, int64_t *n_pairs) {
-  if (!dx || !n_pairs || q_begin < 0 || q_end < q_begin || q_end - q_begin >= (1LL << 31))
+  if (!dx) return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_range: bad arguments");
+  std::lock_guard<std::mutex> g(dx->mu);
+  CallFilter cf;
+  const int frc = take_filter(dx, q_end - q_begin, "kv_dense_selfjoin_range", cf);
+  if (!n_pairs || q_begin < 0 || q_end < q_begin || q_end - q_begin >= (1LL << 31))
     return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_range: bad arguments");
   if (!valid_threshold(threshold)) return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_range: threshold must be in (0, 1]");
-  std::lock_guard<std::mutex> g(dx->mu);
   dx->range_valid = false;
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_selfjoin_range: index not finalized");
   if (q_end > dx->n_rows) return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_range: row range outside the index");
+  if (frc != KV_OK) return frc;
   KV_CUDA(cudaSetDevice(dx->device));
-  return dense_range(dx, dx->rows.p + q_begin * dx->dim, q_end - q_begin, threshold, dx->row_base + q_begin, n_pairs);
+  return dense_range(dx, dx->rows.p + q_begin * dx->dim, q_end - q_begin, threshold, dx->row_base + q_begin, q_begin, cf,
+                     n_pairs);
 }
 
 // The pairs come back in emit order, which the kernel does not fix; (score desc, row asc) is a total order of each

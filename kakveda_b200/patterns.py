@@ -96,6 +96,13 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
     their key's lowest other copy and the other k - 1 slots go to other texts: a text stored more than k times no
     longer hides its neighbours.  With ``k=None`` the components are the default's.
     """
+    from .similarity import GfkbIndex
+
+    # the index classes a mode is built for are checked before the index is touched
+    if distinct and k is not None and not isinstance(index, GfkbIndex):
+        raise NotImplementedError("detect_patterns(distinct=True) collapses copies on a GfkbIndex only")
+    if filter_first and failure_type is not None and not isinstance(index, GfkbIndex):
+        raise NotImplementedError("detect_patterns(filter_first=True) searches by label on a GfkbIndex only")
     n = len(records)
     keep = np.ones(n, dtype=bool)
     if failure_type is not None:
@@ -106,18 +113,10 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
         dead = index.deleted_mask()[:n]
         keep[: len(dead)] &= ~dead
     if distinct and k is not None:
-        from .similarity import GfkbIndex
-
-        if not isinstance(index, GfkbIndex):
-            raise NotImplementedError("detect_patterns(distinct=True) collapses copies on a GfkbIndex only")
         keys: Dict[Any, int] = {}  # the (failure_type, signature_text) key an upsert versions: one text of one type
         index.set_row_groups(np.fromiter((keys.setdefault((r.get("failure_type"), r.get("signature_text")), len(keys))
                                           for r in records), dtype=np.int32, count=n))
     if filter_first and failure_type is not None:
-        from .similarity import GfkbIndex
-
-        if not isinstance(index, GfkbIndex):
-            raise NotImplementedError("detect_patterns(filter_first=True) searches by label on a GfkbIndex only")
         types: Dict[Any, int] = {}
         index.set_row_labels(np.fromiter((types.setdefault(r.get("failure_type"), len(types)) for r in records),
                                          dtype=np.int32, count=n))
