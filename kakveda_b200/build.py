@@ -1,9 +1,11 @@
 """Build libkakveda_b200.so in-tree with nvcc for sm_90a (H100; no torch types cross the C ABI).
 
-    python -m kakveda_b200.build [--force] [--verbose]
+    python -m kakveda_b200.build [--force] [--verbose] [--scan-clocks]
 
 The shared object lands in ``kakveda_b200/lib/`` (git-ignored build product).  ``__graft_entry__.build()``
-calls :func:`build`.
+calls :func:`build`.  ``--scan-clocks`` builds the measuring variant of the candidate scan
+(``-DKV_SCAN_CLOCKS``) into ``libkakveda_b200_scanclocks.so`` next to the product library, which it leaves alone;
+``profiles/run_scan_split.py`` loads it through ``KAKVEDA_B200_LIB``.
 """
 from __future__ import annotations
 
@@ -35,28 +37,40 @@ def sources() -> list[Path]:
     return sorted(list(CSRC.glob("*.cu")) + list(CSRC.glob("*.cpp")))
 
 
-def _digest() -> str:
+SCAN_CLOCKS = dict(defines=("KV_SCAN_CLOCKS",), name="libkakveda_b200_scanclocks")
+
+
+def _digest(defines: tuple[str, ...] = ()) -> str:
     h = hashlib.sha256()
     for p in sources() + sorted(CSRC.glob("*.h")) + sorted(CSRC.glob("*.cuh")) + [PKG.parent / "include" / "kakveda_b200.h"]:
         h.update(p.name.encode())
         h.update(p.read_bytes())
-    h.update(" ".join(GENCODE + NVCC_FLAGS).encode())
+    h.update(" ".join(GENCODE + NVCC_FLAGS + [f"-D{d}" for d in defines]).encode())
     return h.hexdigest()
 
 
-def build(force: bool = False, verbose: bool = False) -> Path:
+def is_current(defines: tuple[str, ...] = (), name: str = LIB.stem) -> bool:
+    """Whether the library of that name was built from the present sources with these flags."""
+    lib, stamp = LIBDIR / f"{name}.so", LIBDIR / f"{name}.stamp"
+    return lib.exists() and stamp.exists() and stamp.read_text().strip() == _digest(defines)
+
+
+def build(force: bool = False, verbose: bool = False, defines: tuple[str, ...] = (), name: str = LIB.stem) -> Path:
+    """Compile the sources with ``-D<define>`` for each of `defines` into ``lib/<name>.so`` (objects under
+    ``lib/obj/<name>/``); a library whose stamp matches the sources and flags is kept."""
     LIBDIR.mkdir(exist_ok=True)
-    dig = _digest()
-    if not force and LIB.exists() and STAMP.exists() and STAMP.read_text().strip() == dig:
+    LIB, STAMP = LIBDIR / f"{name}.so", LIBDIR / f"{name}.stamp"
+    dig = _digest(defines)
+    if not force and is_current(defines, name):
         return LIB
     nvcc = _nvcc()
     objs = []
-    objdir = LIBDIR / "obj"
-    objdir.mkdir(exist_ok=True)
+    objdir = LIBDIR / "obj" / name
+    objdir.mkdir(parents=True, exist_ok=True)
     procs = []
     for src in sources():
         obj = objdir / (src.stem + ".o")
-        cmd = [nvcc, *GENCODE, *NVCC_FLAGS, "-x", "cu", "-c", str(src), "-o", str(obj)]
+        cmd = [nvcc, *GENCODE, *NVCC_FLAGS, *[f"-D{d}" for d in defines], "-x", "cu", "-c", str(src), "-o", str(obj)]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
             print(" ".join(cmd), flush=True)
@@ -80,4 +94,4 @@ def build(force: bool = False, verbose: bool = False) -> Path:
 
 
 if __name__ == "__main__":
-    print(build(force="--force" in sys.argv, verbose="--verbose" in sys.argv))
+    print(build(force="--force" in sys.argv, verbose="--verbose" in sys.argv, **(SCAN_CLOCKS if "--scan-clocks" in sys.argv else {})))

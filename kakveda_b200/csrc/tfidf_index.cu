@@ -1380,7 +1380,9 @@ static int run_jaccard(kv_index *ix, Batch &b) {
   return KV_OK;
 }
 
-constexpr int64_t CODE_SPLIT_CTAS = 64;  // scan of the stored codes: aim for this many CTAs per SM (32 waves at 2 CTAs/SM)
+// Scan of the stored codes: aim for this many CTAs per SM (32 waves at 2 CTAs/SM).  At the bench shape that is 3 CTAs
+// per group; 5 and 8 were measured slower (DESIGN section 6): every CTA of a group starts with empty lists.
+constexpr int64_t CODE_SPLIT_CTAS = 64;
 
 // Splits of the resident batch, pruned or exhaustive path, and the buffers of the candidate lists: sets b's sizes,
 // b.prune and the last_* launch counts.  Shared by the top-k batch and the threshold search.
@@ -2369,3 +2371,16 @@ extern "C" int kv_index_layout_load(kv_index *ix, const char *path) {
   ix->labels_on_device = ix->groups_on_device = false;  // positions changed: the finalize that follows rebuilds them
   return KV_OK;
 }
+
+#ifdef KV_SCAN_CLOCKS
+// Measuring build only (see KV_SCAN_CLOCKS in tfidf_kernels.cuh): copies the candidate scan's profile of the current
+// device to out[0..n) and clears it.  n must be the profile's slot count, so a caller with another layout fails.
+extern "C" int kv_debug_scan_profile(unsigned long long *out, int n) {
+  static unsigned long long zero[KVP_TOTAL];
+  if (!out || n != KVP_TOTAL) return kv_fail(KV_ERR_INVALID, "kv_debug_scan_profile: the profile has %d slots", (int)KVP_TOTAL);
+  KV_CUDA(cudaDeviceSynchronize());
+  KV_CUDA(cudaMemcpyFromSymbol(out, g_scan_prof, sizeof(zero)));
+  KV_CUDA(cudaMemcpyToSymbol(g_scan_prof, zero, sizeof(zero)));
+  return KV_OK;
+}
+#endif

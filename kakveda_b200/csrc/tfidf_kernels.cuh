@@ -642,15 +642,32 @@ __device__ __forceinline__ void range_emit(RangePair *out, unsigned long long *c
   }
 }
 
-constexpr int S_WARPS = 8;
+constexpr int S_WARPS = 12;
 constexpr int S_BUF_ENTRIES = 256;  // a staged block holds up to this many entries (larger blocks are read in place)
 constexpr int S_BUF_BYTES = S_BUF_ENTRIES * 8;
 constexpr int S_WIN = 64;  // codes mode: chunks per window (a lane loads its query's S_WIN codes as four 16-byte loads)
+constexpr unsigned long long KTH_NONE = 0xFF8000007FFFFFFFull;  // s_kth of a list that is not full: (-inf, INT_MAX)
 
-struct ScanHit {
-  uint32_t m, c_lo, w_lo, w_hi;  // c fits 32 bits for tf <= 2 ... kept 64-bit via c_hi below
-  uint32_t c_hi, pad0, pad1, pad2;
+// Measuring build of K1b-S (-DKV_SCAN_CLOCKS, profiles/run_scan_split.py): every warp of a codes-mode scan splits its
+// life into spans with clock(), counts what it meets, and adds both to g_scan_prof, which kv_debug_scan_profile reads.
+// The product build defines none of this and KV_SCAN_PROF(...) expands to nothing.
+#ifdef KV_SCAN_CLOCKS
+enum {
+  KVP_SELECT, KVP_WAIT, KVP_HEAD, KVP_PROBE, KVP_HITPROD, KVP_HITACC, KVP_EPI, KVP_LOCKWAIT, KVP_INSERT, KVP_TAIL,  // cycles
+  KVC_PAIRS, KVC_TRIPS, KVC_HITS, KVC_HITS_ALL, KVC_LOCKS, KVC_LOCKS_UNCHANGED, KVC_ROWS_PASSED, KVC_INPLACE, KVC_RECORDS,
+  KVC_WARPS, KVC_CTAS, KVC_CTA_PAIRS_MAX, KVP_N,
+  KVH_QUERIES = KVP_N,            // [33] records by queries in the mask
+  KVH_CTA_PAIRS = KVH_QUERIES + 33,  // [64] CTAs by pairs scored / 512 (last bucket: the rest)
+  KVP_TOTAL = KVH_CTA_PAIRS + 64
 };
+__device__ unsigned long long g_scan_prof[KVP_TOTAL];
+#define KV_SCAN_PROF(...) __VA_ARGS__
+// charges the cycles since the previous mark to a span (the warp is converged first, lane 0's clock is the warp's)
+#define KV_SCAN_MARK(slot) { __syncwarp(); const unsigned int kvp_n = clock(); kvp[slot] += kvp_n - kvp_t; kvp_t = kvp_n; }
+#else
+#define KV_SCAN_PROF(...)
+#define KV_SCAN_MARK(slot)
+#endif
 
 // 1-D bulk asynchronous copy global -> shared (TMA engine), completion counted in bytes on an mbarrier
 __device__ __forceinline__ void bulk_copy_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
@@ -672,9 +689,9 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   uint32_t *s_keys = (uint32_t *)smem_raw;                                  // [GROUP_Q][QKEYS]
   QFeat *s_feats = (QFeat *)(s_keys + GROUP_Q * QKEYS);                     // [GROUP_Q][QFEATS]
   unsigned char *s_buf = (unsigned char *)(s_feats + GROUP_Q * QFEATS);     // [S_WARPS][2][S_BUF_BYTES]
-  ScanHit *s_hits = (ScanHit *)(s_buf + S_WARPS * 2 * S_BUF_BYTES);         // [S_WARPS][32]
-  uint64_t *s_bar = (uint64_t *)(s_hits + S_WARPS * 32);                    // [S_WARPS][2]
-  float *s_lscore = (float *)(s_bar + S_WARPS * 2);                         // [GROUP_Q][k]
+  uint64_t *s_bar = (uint64_t *)(s_buf + S_WARPS * 2 * S_BUF_BYTES);        // [S_WARPS][2]
+  unsigned long long *s_kth = (unsigned long long *)(s_bar + S_WARPS * 2);  // [GROUP_Q] k-th entry of a full list
+  float *s_lscore = (float *)(s_kth + GROUP_Q);                             // [GROUP_Q][k]
   int *s_lrow = (int *)(s_lscore + GROUP_Q * k);                            // [GROUP_Q][k]
   int *s_cnt = s_lrow + GROUP_Q * k;                                        // [GROUP_Q]
   int *s_lock = s_cnt + GROUP_Q;                                            // [GROUP_Q]
@@ -697,11 +714,11 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
 
   // record range of this CTA (codes mode: a range of windows)
   uint32_t n_rec;
-  int64_t c_lo = 0;
+  uint32_t c_lo = 0;  // chunk indices are 32-bit in this kernel (a chunk is 32 rows)
   if (codes) {
     n_rec = (uint32_t)((P.n_chunks + S_WIN - 1) / S_WIN);
   } else if (P.list_mode == 2) {
-    c_lo = P.n_chunks * bsplit / P.n_bsplits;
+    c_lo = (uint32_t)(P.n_chunks * bsplit / P.n_bsplits);
     n_rec = (uint32_t)(P.n_chunks * (bsplit + 1) / P.n_bsplits - c_lo);
   } else {
     n_rec = P.list_count[list];
@@ -726,6 +743,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
     if (threadIdx.x < GROUP_Q) {
       const int qi = threadIdx.x;
       const bool ok = qi < q_count;
+      s_kth[qi] = KTH_NONE;
       s_cnt[qi] = 0;
       s_lock[qi] = 0;
       s_nq[qi] = ok ? P.q_nq[q0 + qi] : 0.f;
@@ -757,7 +775,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
     }
   };
 
-  auto fetch = [&](uint32_t r, int64_t &chunk, uint32_t &mask) {
+  auto fetch = [&](uint32_t r, uint32_t &chunk, uint32_t &mask) {
     if (P.list_mode == 2) {
       chunk = c_lo + r;
       mask = q_count == 32 ? FULL : ((1u << q_count) - 1u);
@@ -783,11 +801,10 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
 
   unsigned char *my_buf = s_buf + warp * 2 * S_BUF_BYTES;
   uint64_t *my_bar = s_bar + warp * 2;
-  ScanHit *my_hits = s_hits + warp * 32;
   uint32_t phases = 0;  // bit b: parity the next wait on buffer b expects
 
   // start the copy of a record's block (if it fits the staging buffer); returns whether it was staged
-  auto issue = [&](int64_t chunk, int b) -> bool {
+  auto issue = [&](uint32_t chunk, int b) -> bool {
     const BlockInfo bi = P.binfo[chunk];
     const int E4 = (bi.n_entries + 3) & ~3;
     if (E4 == 0 || E4 > S_BUF_ENTRIES) return false;
@@ -801,22 +818,18 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   // Codes mode: the warp's window state.  A lane reads the codes of query q0 + lane (lanes past the group read the
   // last query's row and take nothing); tq = 256 takes nothing.
   uint32_t tq = 256;
-  unsigned long long qbit = ~0ull;  // the query's label bit (label filter), every bit when it is not filtered
-  const unsigned char *crow = nullptr;
   uint4 wraw[S_WIN / 16];            // codes of window w_nxt (in flight while the current window's records are scored)
   uint32_t w_nxt = 0;
-  int64_t wbase = 0;                 // first chunk of the current window
+  uint32_t wbase = 0;                // first chunk of the current window
   uint32_t wm[S_WIN / 32] = {};      // lane j: query mask of chunk wbase + 32 i + j
   unsigned long long pend = 0;       // chunks of the current window with a record not yet taken
-  unsigned int sel_pairs = 0, sel_recs = 0;
   auto load_window = [&](uint32_t w) {
+    const unsigned char *crow = P.ubq + (size_t)(q0 + min(lane, q_count - 1)) * P.ubq_stride + (size_t)w * S_WIN;
 #pragma unroll
-    for (int i = 0; i < S_WIN / 16; i++) wraw[i] = __ldcs(reinterpret_cast<const uint4 *>(crow + (size_t)w * S_WIN) + i);
+    for (int i = 0; i < S_WIN / 16; i++) wraw[i] = __ldcs(reinterpret_cast<const uint4 *>(crow) + i);
   };
   if (codes) {
     if (lane < q_count) tq = (uint32_t)P.tcode[q0 + lane];
-    crow = P.ubq + (size_t)(q0 + min(lane, q_count - 1)) * P.ubq_stride;
-    if (P.q_label && s_qlab[lane] >= 0) qbit = 1ull << (s_qlab[lane] & 63);
     w_nxt = grab();
     if (w_nxt < r_hi) load_window(w_nxt);
   }
@@ -824,10 +837,10 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   // compared with the threshold codes (the same test, in the same order, as bound pass 1's survivors: code >= tq, chunk
   // in range, label signature), the next window's loads are issued, and a ballot per chunk transposes the comparisons
   // into query masks.  Pairs and records are counted before the live-word test, as list_append counts them.
-  auto next_code_record = [&](int64_t &chunk, uint32_t &mask) -> bool {
+  auto next_code_record = [&](uint32_t &chunk, uint32_t &mask) -> bool {
     while (pend == 0) {
       if (w_nxt >= r_hi) return false;
-      wbase = (int64_t)w_nxt * S_WIN;
+      wbase = w_nxt * S_WIN;
       const uint32_t t4 = tq < 256 ? tq * 0x01010101u : 0u;
       uint32_t ge[S_WIN / 4];  // byte i of ge[j]: 0xFF when the code of chunk wbase + 4 j + i reaches tq
       bool any = false;
@@ -846,6 +859,8 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
       for (int i = 0; i < S_WIN / 32; i++) wm[i] = 0;
       if (!__any_sync(FULL, any)) continue;
       if (P.q_label) {
+        const int lb = s_qlab[lane];
+        const unsigned long long qbit = lb >= 0 ? 1ull << (lb & 63) : ~0ull;  // the query's label bit, every bit when it is not filtered
 #pragma unroll
         for (int i = 0; i < S_WIN / 32; i++) {
           const unsigned long long sig = P.chunk_sig[wbase + 32 * i + lane];
@@ -867,14 +882,21 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
           }
       }
       pend = 0;
+      unsigned int sel_pairs = 0, sel_recs = 0;
 #pragma unroll
       for (int i = 0; i < S_WIN / 32; i++) {
-        const int64_t c = wbase + 32 * i + lane;
+        const uint32_t c = wbase + 32 * i + lane;
         if (c >= P.n_chunks) wm[i] = 0;
         sel_pairs += (unsigned int)__popc(wm[i]);
         sel_recs += wm[i] != 0u;
         if (P.alive && P.alive[c] == 0u) wm[i] = 0;  // every row of the chunk deleted: never staged
         pend |= (unsigned long long)__ballot_sync(FULL, wm[i] != 0u) << (32 * i);
+      }
+      sel_pairs = __reduce_add_sync(FULL, sel_pairs);
+      sel_recs = __reduce_add_sync(FULL, sel_recs);
+      if (lane == 0) {
+        atomicAdd(&s_stat[2], sel_pairs);
+        atomicAdd(&s_stat[3], sel_recs);
       }
     }
     const int i = __ffsll((long long)pend) - 1;
@@ -887,7 +909,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
     mask = __shfl_sync(FULL, m, i & 31);
     return true;
   };
-  auto next_record = [&](int64_t &chunk, uint32_t &mask) -> bool {
+  auto next_record = [&](uint32_t &chunk, uint32_t &mask) -> bool {
     if (codes) return next_code_record(chunk, mask);
     const uint32_t r = grab();
     if (r >= r_hi) return false;
@@ -896,7 +918,8 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   };
 
   unsigned int pairs_done = 0, recs_done = 0;
-  int64_t chunk_cur = 0, chunk_nxt = 0;
+  KV_SCAN_PROF(unsigned int kvp[KVP_N] = {}; unsigned int kvp_t = clock();)
+  uint32_t chunk_cur = 0, chunk_nxt = 0;
   uint32_t mask_cur = 0, mask_nxt = 0;
   bool staged_cur = false, staged_nxt = false;
   int b = 0;
@@ -905,6 +928,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   while (have_cur) {
     const bool have_nxt = next_record(chunk_nxt, mask_nxt);
     if (have_nxt) staged_nxt = mask_nxt ? issue(chunk_nxt, b ^ 1) : false;
+    KV_SCAN_MARK(KVP_SELECT)
     if (mask_cur) {
       const BlockInfo bi = P.binfo[chunk_cur];
       const int E = bi.n_entries, E4 = (E + 3) & ~3;
@@ -915,11 +939,13 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
         words = (const uint32_t *)(my_buf + b * S_BUF_BYTES);
       } else {
         words = P.blk + (size_t)bi.off4 * 4;
+        KV_SCAN_PROF(kvp[KVC_INPLACE]++;)
       }
+      KV_SCAN_MARK(KVP_WAIT)
+      KV_SCAN_PROF(kvp[KVC_RECORDS]++; if (codes && lane == 0) atomicAdd(&g_scan_prof[KVH_QUERIES + __popc(mask_cur)], 1ull);)
       masks = words + E4;
-      const int64_t pos0 = chunk_cur * CHUNK_ROWS;
+      const int64_t pos0 = (int64_t)chunk_cur * CHUNK_ROWS;
       const int rows = (int)min((int64_t)CHUNK_ROWS, P.n_rows - pos0);
-      const uint32_t valid = rows == 32 ? FULL : ((1u << rows) - 1u);
       const float Bc = lane < rows ? P.B32[pos0 + lane] : 0.f;
       const int lpos = P.q_label ? P.label_pos[pos0 + lane] : -1;  // one 128-byte line per record
       const bool live = P.alive ? ((P.alive[chunk_cur] >> lane) & 1u) != 0u : true;
@@ -935,7 +961,14 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
         pairs_done++;
         const uint32_t *keys = s_keys + qi * QKEYS;
         const QFeat *feats = s_feats + qi * QFEATS;
-        unsigned long long acc_w = 0, acc_c = 0;
+        // Hits reach the rows in two ways.  An entry held by every row of the chunk (W_ALL: the common case in a
+        // candidate chunk, whose rows are text neighbours) is summed by the lane that found it (lane = entry) and the
+        // warp adds those sums to every row once, after the last trip.  An entry held by some rows is handed to the
+        // row lanes by shuffle from the lane that found it.  64-bit integer sums: the order does not change a bit.
+        unsigned long long acc_w = 0, acc_c = 0;  // lane = row
+        unsigned long long all_w = 0, all_c = 0;  // lane = entry
+        KV_SCAN_PROF(kvp[KVC_PAIRS]++;)
+        KV_SCAN_MARK(KVP_HEAD)
         for (int e0 = 0; e0 < E; e0 += 32) {
           const int e = e0 + lane;
           const uint32_t w = e < E ? words[e] : PAD_WORD;
@@ -950,33 +983,37 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
               h = (h + 1) & (QKEYS - 1);
             }
           }
-          const uint32_t hm = __ballot_sync(FULL, idx >= 0);
-          if (hm == 0) continue;
+          KV_SCAN_PROF(kvp[KVC_TRIPS]++; kvp[KVC_HITS] += __popc(__ballot_sync(FULL, idx >= 0));
+                       kvp[KVC_HITS_ALL] += __popc(__ballot_sync(FULL, idx >= 0 && (w & W_ALL)));)
+          KV_SCAN_MARK(KVP_PROBE)
+          uint32_t hmask = 0;  // rows of a hit that is not W_ALL
+          unsigned long long ww = 0, cc = 0;
           if (idx >= 0) {
             uint32_t tf = w & 31u;
             if (tf == TF_OVF) tf = ovf_lookup(P.ovf_keys, P.ovf_vals, P.n_ovf, chunk_cur, (uint32_t)e);
             const QFeat f = feats[idx];
-            unsigned long long ww = ((unsigned long long)f.w_hi << 32) | f.w_lo, cc = (unsigned long long)f.cq;
+            ww = ((unsigned long long)f.w_hi << 32) | f.w_lo;
+            cc = (unsigned long long)f.cq;
             if (tf != 1u) { ww *= (unsigned long long)tf; cc *= (unsigned long long)tf * (unsigned long long)tf; }
-            ScanHit hrec;
-            hrec.m = (w & W_ALL) ? valid : masks[e];
-            hrec.w_lo = (uint32_t)ww; hrec.w_hi = (uint32_t)(ww >> 32);
-            hrec.c_lo = (uint32_t)cc; hrec.c_hi = (uint32_t)(cc >> 32);
-            hrec.pad0 = hrec.pad1 = hrec.pad2 = 0;
-            my_hits[__popc(hm & lt)] = hrec;
+            if (w & W_ALL) { all_w += ww; all_c += cc; }
+            else hmask = masks[e];
           }
-          __syncwarp();
-          const int nh = __popc(hm);
-          for (int i = 0; i < nh; i++) {
-            const uint4 h0 = *(const uint4 *)&my_hits[i];
-            const uint32_t chi = my_hits[i].c_hi;
-            if ((h0.x >> lane) & 1u) {
-              acc_w += ((unsigned long long)h0.w << 32) | h0.z;
-              acc_c += ((unsigned long long)chi << 32) | h0.y;
-            }
+          KV_SCAN_MARK(KVP_HITPROD)
+          for (uint32_t hm = __ballot_sync(FULL, hmask != 0u); hm; hm &= hm - 1) {
+            const int j = __ffs(hm) - 1;
+            const uint32_t m = __shfl_sync(FULL, hmask, j);
+            const unsigned long long hw = __shfl_sync(FULL, ww, j), hc = __shfl_sync(FULL, cc, j);
+            if ((m >> lane) & 1u) { acc_w += hw; acc_c += hc; }
           }
-          __syncwarp();
+          KV_SCAN_MARK(KVP_HITACC)
         }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+          all_w += __shfl_xor_sync(FULL, all_w, o);
+          all_c += __shfl_xor_sync(FULL, all_c, o);
+        }
+        acc_w += all_w;
+        acc_c += all_c;
         // fused epilogue: pre-test without division, exact score for survivors; the warp then takes the query's lock
         // ONCE and inserts all surviving rows of the chunk into the sorted list held one entry per lane (k <= 32)
         float sc = -INFINITY;
@@ -986,15 +1023,23 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
           const float dot = s_dotU[qi] + __ull2float_rn(acc_w) * (1.f / 4294967296.f);
           const float corr = s_corrU[qi] - __ull2float_rn(acc_c) * (1.f / 16777216.f);
           const float t = Bc + corr;
-          float filt;
+          float filt, ks = -INFINITY;
+          int kr = 0x7fffffff;
           if constexpr (RANGE) {
             filt = __int_as_float(P.gthr[q0 + qi]);  // the search threshold: fixed for the whole scan
           } else {
-            // optimistic filter (read without the lock): the list's k-th SCORE once it is full, and the global lower
-            // bound of the k-th score.  Scores only ever rise, so a stale value merely lets a few more rows through; rows
-            // tying with it are let through as well -- the exact (score desc, row asc) comparison happens under the lock.
+            // Filter read without the lock: the global lower bound of the k-th score (rows tying with it pass) and the
+            // list's k-th ENTRY once it is full, score and row in one 64-bit word, so the two always belong together.
+            // A row enters a full list only if it comes before that entry in (score desc, row asc) order, and the entry
+            // only ever improves: a stale word lets a few more rows through to the exact comparison under the lock and
+            // never keeps out a row that belongs.  DISTINCT has a second way in, replacing the entry of the row's own
+            // group; that entry is in the list, so it is no worse than the k-th one, and a row that does not come
+            // before the k-th entry does not come before its group's entry either.
             filt = __int_as_float(*(volatile int *)&P.gthr[q0 + qi]);
-            if (*(volatile int *)&s_cnt[qi] == k) filt = fmaxf(filt, *(volatile float *)&s_lscore[qi * k + k - 1]);
+            const unsigned long long kth = *(volatile unsigned long long *)&s_kth[qi];
+            ks = __int_as_float((int)(kth >> 32));
+            kr = (int)(uint32_t)kth;
+            filt = fmaxf(filt, ks);
           }
           bool pass = true;
           if (filt > 0.f) pass = dot * dot >= filt * filt * nq * FILTER_SLACK * t;
@@ -1002,7 +1047,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
             const float den = nq * t;
             sc = den > 0.f ? __fdiv_rn(dot, __fsqrt_rn(den)) : 0.f;
             row = P.perm[pos0 + lane];
-            cand = row != s_excl[qi] && sc >= filt && (ql < 0 || lpos == ql) && live;
+            cand = row != s_excl[qi] && sc >= filt && (sc > ks || row < kr) && (ql < 0 || lpos == ql) && live;
           }
         }
         if constexpr (RANGE) {
@@ -1010,6 +1055,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
           continue;
         }
         uint32_t cm = __ballot_sync(FULL, cand);
+        KV_SCAN_PROF(kvp[KVC_ROWS_PASSED] += __popc(cm);)
         if constexpr (DISTINCT) {
           // the best survivor of each group of the chunk goes on (lanes without a survivor get keys of their own)
           const uint32_t peers = __match_any_sync(FULL, cand ? gpos : -1 - lane);
@@ -1022,9 +1068,11 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
           }
           cm = __ballot_sync(FULL, keep);
         }
+        KV_SCAN_MARK(KVP_EPI)
         if (cm) {
           if (lane == 0) while (atomicCAS(&s_lock[qi], 0, 1) != 0) {}
           __syncwarp();
+          KV_SCAN_MARK(KVP_LOCKWAIT)
           __threadfence_block();
           int cnt = *(volatile int *)&s_cnt[qi];
           float ls = lane < k ? *(volatile float *)&s_lscore[qi * k + lane] : -INFINITY;   // unused slots hold (-inf, INT_MAX)
@@ -1072,12 +1120,16 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
             if (lane < k) { s_lscore[qi * k + lane] = ls; s_lrow[qi * k + lane] = lr; }
             if constexpr (DISTINCT) if (lane < k) s_lgrp[qi * k + lane] = lg;
             if (lane == 0) s_cnt[qi] = cnt;
+            if (lane == k - 1 && cnt == k)  // one 64-bit store: a reader never pairs a new score with an old row
+              s_kth[qi] = ((unsigned long long)(uint32_t)__float_as_int(ls) << 32) | (uint32_t)lr;
             const float ks = __shfl_sync(FULL, ls, k - 1);
             if (lane == 0 && cnt == k) publish_threshold(q0 + qi, ks);
           }
           __threadfence_block();
           __syncwarp();
           if (lane == 0) atomicExch(&s_lock[qi], 0);
+          KV_SCAN_PROF(kvp[KVC_LOCKS]++; kvp[KVC_LOCKS_UNCHANGED] += !changed;)
+          KV_SCAN_MARK(KVP_INSERT)
         }
         __syncwarp();
       }
@@ -1093,11 +1145,18 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
     atomicAdd(&s_stat[0], pairs_done);
     atomicAdd(&s_stat[1], recs_done);
   }
-  if (sel_recs) {
-    atomicAdd(&s_stat[2], sel_pairs);
-    atomicAdd(&s_stat[3], sel_recs);
-  }
+  KV_SCAN_MARK(KVP_SELECT)
   __syncthreads();
+  KV_SCAN_MARK(KVP_TAIL)
+  KV_SCAN_PROF(if (codes && lane == 0) {
+    kvp[KVC_WARPS] = 1;
+    for (int i = 0; i < KVC_CTAS; i++) atomicAdd(&g_scan_prof[i], (unsigned long long)kvp[i]);
+    if (warp == 0) {
+      atomicAdd(&g_scan_prof[KVC_CTAS], 1ull);
+      atomicMax(&g_scan_prof[KVC_CTA_PAIRS_MAX], (unsigned long long)s_stat[0]);
+      atomicAdd(&g_scan_prof[KVH_CTA_PAIRS + min(s_stat[0] / 512u, 63u)], 1ull);
+    }
+  })
   if constexpr (!RANGE) {  // publish this CTA's partial lists (already ordered)
     const int part = bsplit * P.n_ssplits + ssplit;
     for (int i = threadIdx.x; i < q_count * k; i += blockDim.x) {
@@ -1119,8 +1178,8 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
 }
 
 static inline size_t scan_smem_bytes(int k, bool distinct = false) {
-  return (size_t)GROUP_Q * QTAB_BYTES + (size_t)S_WARPS * 2 * S_BUF_BYTES + (size_t)S_WARPS * 32 * sizeof(ScanHit) +
-         (size_t)S_WARPS * 2 * 8 + (size_t)GROUP_Q * k * 8 + (size_t)GROUP_Q * 4 * 7 + 32 + (distinct ? (size_t)GROUP_Q * k * 4 : 0);
+  return (size_t)GROUP_Q * QTAB_BYTES + (size_t)S_WARPS * 2 * S_BUF_BYTES + (size_t)S_WARPS * 2 * 8 + (size_t)GROUP_Q * 8 +
+         (size_t)GROUP_Q * k * 8 + (size_t)GROUP_Q * 4 * 7 + 32 + (distinct ? (size_t)GROUP_Q * k * 4 : 0);
 }
 
 // ----------------------------------------------------------------------------------------
