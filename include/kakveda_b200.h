@@ -81,6 +81,21 @@ int kv_csr_view(const kv_csr *c, int64_t *n_docs, const int64_t **indptr, const 
                 const uint32_t **tf, const double **oov_tf2);
 void kv_csr_destroy(kv_csr *c);
 
+/* Device featuriser (featurize_device.cu).  A kv_vocab_mirror is an open-addressing table in the HBM of one device
+ * that maps the 128-bit key of every feature of a kv_vocab to its id (load factor <= 0.5, home slot k0 & (cap - 1),
+ * 40 bytes of HBM per feature at the largest load, 80 just after a growth).  kv_vocab_mirror_sync appends the ids
+ * [mirrored, kv_vocab_size(v)) and grows the table when needed; a vocabulary only grows, so the mirror is a prefix of it.
+ * A sync that meets a concurrent featurize(grow = 1) or import keeps the mirror as it was and returns KV_ERR_STATE (try
+ * again later).  *n_mirrored (optional) receives the features mirrored after the call.
+ * kv_featurize_device is kv_featurize(v, ..., grow = 0) computed on the device against the mirror (synced first), with
+ * the same result bit for bit and the same errors; it returns an ordinary host kv_csr. */
+typedef struct kv_vocab_mirror kv_vocab_mirror;
+int kv_vocab_mirror_create(int device, kv_vocab_mirror **out);
+void kv_vocab_mirror_destroy(kv_vocab_mirror *m);
+int kv_vocab_mirror_sync(kv_vocab_mirror *m, const kv_vocab *v, int64_t *n_mirrored);
+int kv_featurize_device(kv_vocab_mirror *m, const kv_vocab *v, const char *bytes, const int64_t *offsets, int64_t n_docs,
+                        int mode, kv_csr **out, int64_t *bad_doc);
+
 /* Host-only helpers for sharding a GFKB by TEXT RANGE (kakveda_b200/dist.py, order="text"; no device involved):
  * kv_text_order: perm_out[i] = the row at position i when the rows are sorted by their feature-id sequence (the
  * text order the scan layout uses; equal rows by row index).  kv_csr_gather_rows: copy the rows `rows[0..n_sel)` of a
@@ -182,8 +197,18 @@ int kv_query_prepare_slice(kv_index *ix, const int64_t *q_indptr, const uint32_t
 int kv_query_upload_runs(kv_index *ix, int n_runs, const int64_t *const *q_indptr, const uint32_t *const *q_ids,
                          const uint32_t *const *q_tf, const double *const *q_oov_tf2, const int32_t *const *order,
                          const uint8_t *const *flags, const int64_t *n_q);
-/* Host-side split of the last upload in ms: pinned staging, classification, text order, copies + table kernels. */
+/* kv_query_upload of the batch kv_featurize(v, bytes, offsets, n_q, mode, grow = 0) would give, built on the device:
+ * the text goes up, is featurised there against the mirror m (synced first; m must live on the index's device), and
+ * classification, text order and tables are computed there.  The resident batch is identical to the host path's.
+ * Errors: those of kv_featurize (*bad_doc on KV_ERR_NONASCII) and of kv_query_upload. */
+int kv_query_upload_text(kv_index *ix, kv_vocab_mirror *m, const kv_vocab *v, const char *bytes, const int64_t *offsets,
+                         int64_t n_q, int mode, int64_t *bad_doc);
+/* Host-side split of the last upload in ms: pinned staging, classification, text order, copies + table kernels.
+ * After kv_query_upload_text: text upload + featurisation, classification, text order, tables + copies back. */
 int kv_index_last_prepare_ms(const kv_index *ix, float ms[4]);
+/* Test hook: the resident batch's query order and flags (qperm[i] = original query at sorted slot i, flags[i] its
+ * class: 0 regular, 1 null, 2 irregular); n_q must be the batch size. */
+int kv_debug_query_order(kv_index *ix, int32_t *qperm, uint8_t *flags, int64_t n_q);
 int kv_topk_resident(kv_index *ix, int k, void *d_scores, void *d_rows);
 /* Same with host outputs (out_scores float32[n_q*k], out_rows int64[n_q*k]). */
 int kv_topk_resident_host(kv_index *ix, int k, float *out_scores, int64_t *out_rows);

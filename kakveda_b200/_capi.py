@@ -36,6 +36,11 @@ SIGNATURES = {
     "kv_csr_view": (C.c_int, [C.c_void_p, c_i64p, C.POINTER(c_i64p), C.POINTER(c_u32p), C.POINTER(c_u32p),
                               C.POINTER(c_f64p)]),
     "kv_csr_destroy": (None, [C.c_void_p]),
+    "kv_vocab_mirror_create": (C.c_int, [C.c_int, C.POINTER(C.c_void_p)]),
+    "kv_vocab_mirror_destroy": (None, [C.c_void_p]),
+    "kv_vocab_mirror_sync": (C.c_int, [C.c_void_p, C.c_void_p, c_i64p]),
+    "kv_featurize_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_char_p, c_i64p, C.c_int64, C.c_int, C.POINTER(C.c_void_p),
+                                      c_i64p]),
     "kv_text_order": (C.c_int, [c_i64p, c_u32p, C.c_int64, C.POINTER(C.c_int32), C.c_int]),
     "kv_csr_gather_rows": (C.c_int, [c_i64p, c_u32p, c_u32p, C.c_int64, c_i64p, C.c_int64, c_i64p, c_u32p, c_u32p, C.c_int]),
     "kv_index_create": (C.c_int, [C.c_int, C.c_int64, C.POINTER(C.c_void_p)]),
@@ -59,7 +64,9 @@ SIGNATURES = {
     "kv_query_upload_runs": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                        C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                        C.POINTER(C.c_void_p), c_i64p]),
+    "kv_query_upload_text": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p, c_i64p, C.c_int64, C.c_int, c_i64p]),
     "kv_index_last_prepare_ms": (C.c_int, [C.c_void_p, c_f32p]),
+    "kv_debug_query_order": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_uint8), C.c_int64]),
     "kv_topk_resident": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "kv_topk_resident_host": (C.c_int, [C.c_void_p, C.c_int, c_f32p, c_i64p]),
     "kv_topk_resident_seed": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),

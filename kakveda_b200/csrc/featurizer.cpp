@@ -146,11 +146,18 @@ struct kv_vocab {
   }
 };
 
-struct kv_csr {
-  std::vector<int64_t> indptr;
-  std::vector<uint32_t> ids, tf;
-  std::vector<double> oov;
-};
+int vocab_export_range(const kv_vocab *v, int64_t lo, int64_t hi, uint64_t *keys) {
+  int64_t found = 0;
+  for (uint64_t i = 0; i < v->cap; i++) {
+    const uint32_t id = v->slots[i].id.load(std::memory_order_acquire);
+    if (id >= SLOT_PENDING || (int64_t)id < lo || (int64_t)id >= hi) continue;  // empty, being created, or outside
+    keys[2 * (size_t)(id - lo)] = v->slots[i].k0;
+    keys[2 * (size_t)(id - lo) + 1] = v->slots[i].k1;
+    found++;
+  }
+  if (found != hi - lo) return kv_fail(KV_ERR_STATE, "vocabulary is being modified");
+  return KV_OK;
+}
 
 namespace {
 

@@ -135,6 +135,23 @@ template <class Rec>
 int range_order_to_host(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
                         int32_t *inter, int32_t *uni, RangeOrderScratch &sc, cudaStream_t s, const char *fn);
 
+// Exclusive scan of x[0, m) in place on stream s (range_order.cu); `part` is scratch.  The sums must stay below 2^32.
+int exclusive_scan_u32(unsigned *x, int64_t m, DevBuf<unsigned> &part, cudaStream_t s);
+
+// Device featuriser (featurize_device.cu): kv_featurize(grow = 0) of a packed text batch against the device mirror of
+// the vocabulary, into device CSR buffers (resized here: indptr n_docs + 1, ids / tf nnz, oov n_docs) on stream s, which
+// must belong to the mirror's device.  The caller holds the mirror's lock (mirror_lock) from before this call until the
+// stream has finished the work.  Returns with *nnz known and the last kernels enqueued.  KV_ERR_NONASCII sets *bad_doc.
+int featurize_device(kv_vocab_mirror *m, cudaStream_t s, const char *bytes, const int64_t *offsets, int64_t n_docs, int mode,
+                     DevBuf<int64_t> &indptr, DevBuf<uint32_t> &ids, DevBuf<uint32_t> &tf, DevBuf<double> &oov, int64_t *nnz,
+                     int64_t *bad_doc);
+// The mirror's device, and its lock (a std::mutex): featurize_device reads the table that kv_vocab_mirror_sync replaces.
+int mirror_device(const kv_vocab_mirror *m);
+// kv_vocab_mirror_sync with the mirror's lock held (makes the mirror's device current).
+int mirror_sync_locked(kv_vocab_mirror *m, const kv_vocab *v);
+void mirror_lock(kv_vocab_mirror *m);
+void mirror_unlock(kv_vocab_mirror *m);
+
 // KV_OK when p is device memory of `device` aligned to `align` bytes, else KV_ERR_INVALID naming `what` (a host pointer
 // passed by mistake is an error, never a fault).
 int check_device_ptr(const void *p, int device, size_t align, const char *what, const char *fn);

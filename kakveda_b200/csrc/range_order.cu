@@ -275,6 +275,17 @@ int check_device_ptr(const void *p, int device, size_t align, const char *what, 
   return KV_OK;
 }
 
+int exclusive_scan_u32(unsigned *x, int64_t m, DevBuf<unsigned> &part, cudaStream_t s) {
+  if (m <= 0) return KV_OK;
+  const int64_t n_part = (m + RO_TILE - 1) / RO_TILE;
+  KV_CUDA(part.ensure(n_part));
+  ro_scan_reduce_kernel<<<(unsigned)n_part, RO_THREADS, 0, s>>>(x, m, part.p);
+  ro_scan_partials_kernel<<<1, RO_THREADS, 0, s>>>(part.p, n_part);
+  ro_scan_down_kernel<<<(unsigned)n_part, RO_THREADS, 0, s>>>(x, m, part.p);
+  KV_CUDA(cudaGetLastError());
+  return KV_OK;
+}
+
 template <class Rec>
 int range_order_device(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
                        int32_t *inter, int32_t *uni, RangeOrderScratch &sc, cudaStream_t s, const char *fn) {

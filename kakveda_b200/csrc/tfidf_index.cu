@@ -33,6 +33,7 @@ struct kv_index {
   CudaEvent ev[5];
   CudaEvent evk[6];  // bound/scan kernel boundaries of a batch
   CudaEvent evp2;    // start of phase 2 of a two-phase batch
+  CudaEvent evq[4];  // stages of a text upload on the device (kv_query_upload_text)
   bool two_phase = false;
   std::mutex mu;
   int sm_count = 132;
@@ -95,6 +96,8 @@ struct kv_index {
   PinnedBuf<double> h_q_oov;
   PinnedBuf<int> h_qperm;     // 3 * n_q: sorted slot -> original query, null-query list, sorted slot -> row of the staged CSR
   PinnedBuf<uint8_t> h_flags;
+  DevBuf<uint8_t> d_qflag_row;  // a text upload's classification by row, and its text order (two halves: merge passes)
+  DevBuf<int> d_qorder;
   DevBuf<int64_t> d_q_indptr;
   DevBuf<uint32_t> d_q_ids, d_q_tf;
   DevBuf<double> d_q_oov;
@@ -344,6 +347,7 @@ int kv_index_create(int device, int64_t row_base, kv_index **out) {
   KV_CUDA(ix->stream.create());
   for (auto &e : ix->ev) KV_CUDA(e.create());
   for (auto &e : ix->evk) KV_CUDA(e.create());
+  for (auto &e : ix->evq) KV_CUDA(e.create());
   KV_CUDA(ix->evp2.create());
   constexpr auto smem_limit = cudaFuncAttributeMaxDynamicSharedMemorySize;
   KV_CUDA(cudaFuncSetAttribute(tfidf_score_kernel, smem_limit, 200 * 1024));
@@ -1002,6 +1006,8 @@ static bool csr_ok(const int64_t *q_indptr, const uint32_t *q_ids, const uint32_
   return true;
 }
 
+static int build_query_tables(kv_index *ix, int64_t n_q);
+
 static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   if (!ix->finalized) return kv_fail(KV_ERR_STATE, "kv_topk: index not finalized");
   int64_t n_q = 0, nnz = 0;
@@ -1131,22 +1137,13 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
     }
   }
 
-  const int64_t n_tiles = (n_q + TILE_Q - 1) / TILE_Q, n_q_pad = n_tiles * TILE_Q;
+  const int64_t n_tiles = (n_q + TILE_Q - 1) / TILE_Q;
   KV_CUDA(ix->d_q_indptr.ensure(n_q + 1));
   KV_CUDA(ix->d_q_ids.ensure(std::max<int64_t>(nnz, 1)));
   KV_CUDA(ix->d_q_tf.ensure(std::max<int64_t>(nnz, 1)));
   KV_CUDA(ix->d_q_oov.ensure(n_q));
   KV_CUDA(ix->d_qperm.ensure(3 * n_q));
   KV_CUDA(ix->d_flags.ensure(n_q));
-  KV_CUDA(ix->d_qconst.ensure(7 * n_q));
-  KV_CUDA(ix->d_qtab.ensure(n_q * (int64_t)QTAB_BYTES));
-  KV_CUDA(ix->d_Wf.ensure(n_q_pad * NF));
-  KV_CUDA(ix->d_q2list.ensure(n_q_pad * Q2CAP));
-  KV_CUDA(ix->d_q3id.ensure(n_q_pad * Q3CAP));
-  KV_CUDA(ix->d_q3w.ensure(n_q_pad * Q3CAP));
-  KV_CUDA(ix->d_Wf2.ensure(n_q_pad * KT2));
-  KV_CUDA(ix->d_d2col.ensure(n_tiles * KT2));
-  KV_CUDA(ix->d_f2out.ensure(1));
   KV_CUDA(cudaEventRecord(ix->ev[0], s));
   KV_CUDA(cudaMemcpyAsync(ix->d_q_indptr.p, ix->h_q_indptr.p, (size_t)(n_q + 1) * 8, cudaMemcpyHostToDevice, s));
   if (nnz) {
@@ -1157,6 +1154,38 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   KV_CUDA(cudaMemcpyAsync(ix->d_qperm.p, ix->h_qperm.p, (size_t)3 * n_q * sizeof(int), cudaMemcpyHostToDevice, s));
   KV_CUDA(cudaMemcpyAsync(ix->d_flags.p, ix->h_flags.p, (size_t)n_q, cudaMemcpyHostToDevice, s));
   KV_CUDA(cudaEventRecord(ix->ev[1], s));
+  {
+    const int rc = build_query_tables(ix, n_q);
+    if (rc != KV_OK) return rc;
+  }
+  unsigned long long f2_out = 0;
+  KV_CUDA(cudaMemcpyAsync(&f2_out, ix->d_f2out.p, sizeof(f2_out), cudaMemcpyDeviceToHost, s));
+  KV_CUDA(cudaStreamSynchronize(s));  // the pinned staging buffers may be rewritten by the next call
+  ix->batch_f2_outside = (int64_t)f2_out;
+  ix->batch_q = n_q;
+  ix->batch_tiles = n_tiles;
+  ix->batch_null = n_null;
+  ix->batch_h2d_bytes = (n_q + 1) * 8 + nnz * 8 + n_q * 8 + 3 * n_q * (int64_t)sizeof(int) + n_q;
+  ix->batch_valid = true;
+  cudaEventElapsedTime(&ix->last_ms[0], ix->ev[0], ix->ev[1]);
+  ix->last_prepare_ms[3] = ms_since(t_mark);
+  return KV_OK;
+}
+
+// The device half of an upload, shared by the host and the text path: with the query CSR (by row), d_qperm (qsrc) and
+// d_flags (by sorted slot) on the device, the per-query constants and tables and the per-tile rare-feature tables.
+static int build_query_tables(kv_index *ix, int64_t n_q) {
+  cudaStream_t s = ix->stream;
+  const int64_t n_tiles = (n_q + TILE_Q - 1) / TILE_Q, n_q_pad = n_tiles * TILE_Q;
+  KV_CUDA(ix->d_qconst.ensure(7 * n_q));
+  KV_CUDA(ix->d_qtab.ensure(n_q * (int64_t)QTAB_BYTES));
+  KV_CUDA(ix->d_Wf.ensure(n_q_pad * NF));
+  KV_CUDA(ix->d_q2list.ensure(n_q_pad * Q2CAP));
+  KV_CUDA(ix->d_q3id.ensure(n_q_pad * Q3CAP));
+  KV_CUDA(ix->d_q3w.ensure(n_q_pad * Q3CAP));
+  KV_CUDA(ix->d_Wf2.ensure(n_q_pad * KT2));
+  KV_CUDA(ix->d_d2col.ensure(n_tiles * KT2));
+  KV_CUDA(ix->d_f2out.ensure(1));
   // ---- device: per-query constants and tables, per-tile rare-feature tables ----
   KV_CUDA(cudaMemsetAsync(ix->d_Wf.p, 0, (size_t)n_q_pad * NF * sizeof(__half), s));
   KV_CUDA(cudaMemsetAsync(ix->d_Wf2.p, 0, (size_t)n_q_pad * KT2 * sizeof(__half), s));
@@ -1185,17 +1214,6 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
     if (rc == KV_OK) rc = make_map_2d(&ix->map_w2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ix->d_Wf2.p, n_q_pad, KT2, TILE_Q);
     if (rc != KV_OK) return rc;
   }
-  unsigned long long f2_out = 0;
-  KV_CUDA(cudaMemcpyAsync(&f2_out, ix->d_f2out.p, sizeof(f2_out), cudaMemcpyDeviceToHost, s));
-  KV_CUDA(cudaStreamSynchronize(s));  // the pinned staging buffers may be rewritten by the next call
-  ix->batch_f2_outside = (int64_t)f2_out;
-  ix->batch_q = n_q;
-  ix->batch_tiles = n_tiles;
-  ix->batch_null = n_null;
-  ix->batch_h2d_bytes = (n_q + 1) * 8 + nnz * 8 + n_q * 8 + 3 * n_q * (int64_t)sizeof(int) + n_q;
-  ix->batch_valid = true;
-  cudaEventElapsedTime(&ix->last_ms[0], ix->ev[0], ix->ev[1]);
-  ix->last_prepare_ms[3] = ms_since(t_mark);
   return KV_OK;
 }
 
@@ -1204,6 +1222,200 @@ static int prepare_batch(kv_index *ix, const int64_t *q_indptr, const uint32_t *
   QueryRun R;
   R.indptr = q_indptr; R.ids = q_ids; R.tf = q_tf; R.oov = q_oov; R.n_q = n_q;
   return prepare_batch_runs(ix, &R, 1);
+}
+
+// ---- the upload of a text batch featurised on the device (kv_query_upload_text) ----
+namespace {
+
+constexpr int TQ_THREADS = 256;
+
+inline unsigned tq_grid(int64_t n) { return (unsigned)std::max<int64_t>(1, (n + TQ_THREADS - 1) / TQ_THREADS); }
+
+// classify_queries on the device, one thread per query, the same float64 operations in the same order (no contraction)
+__global__ void __launch_bounds__(TQ_THREADS) classify_kernel(const int64_t *indptr, const uint32_t *ids, const uint32_t *tf,
+                                                              int64_t n_q, int64_t V, int corpus_fit, const uint32_t *df,
+                                                              const uint8_t *univ, const uint32_t *tfmax, double amax,
+                                                              uint8_t *flag) {
+  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= n_q) return;
+  bool known = false;
+  int feats = 0;
+  double s_dot = 0, s_corr = 0, wmax = 0;
+  for (int64_t p = indptr[q]; p < indptr[q + 1]; p++) {
+    const uint32_t t = ids[p];
+    if ((int64_t)t >= V) continue;
+    if (corpus_fit && df[t] == 0) continue;
+    known = true;
+    if (univ[t]) continue;
+    feats++;
+    const double tm = (double)tfmax[t], f = (double)tf[p];
+    s_dot = __dadd_rn(s_dot, __dmul_rn(f, tm));
+    s_corr = __dadd_rn(s_corr, __dmul_rn(tm, tm));
+    wmax = fmax(wmax, f);
+  }
+  uint8_t c = 0;
+  if (!known) c = 1;
+  else if (feats > QFEATS || __dmul_rn(s_dot, amax) >= 1073741824.0 || __dmul_rn(s_corr, 32.0) >= 1073741824.0 ||
+           __dmul_rn(wmax, amax) > 60000.0)
+    c = 2;
+  flag[q] = c;
+}
+
+// cmp_seq of queries a and b of the device CSR
+__device__ __forceinline__ int cmp_queries(const int64_t *indptr, const uint32_t *ids, int a, int b) {
+  const int64_t a0 = indptr[a], na = indptr[a + 1] - a0, b0 = indptr[b], nb = indptr[b + 1] - b0;
+  const int64_t n = na < nb ? na : nb;
+  for (int64_t i = 0; i < n; i++) {
+    const uint32_t x = ids[a0 + i], y = ids[b0 + i];
+    if (x != y) return x < y ? -1 : 1;
+  }
+  return na < nb ? -1 : (na > nb ? 1 : 0);
+}
+
+__global__ void __launch_bounds__(TQ_THREADS) iota_kernel(int *order, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) order[i] = (int)i;
+}
+
+// One pass of a stable bottom-up merge sort: the sorted runs [lo, lo + w) and [lo + w, lo + 2w) of `in` merge into
+// `out`.  Every element finds its place by a binary search in the other run: an element of the left run goes after the
+// right run's strictly smaller elements, one of the right run after the left run's smaller-or-equal elements, so equal
+// sequences keep their input order (== std::stable_sort with cmp_seq).
+__global__ void __launch_bounds__(TQ_THREADS) merge_pass_kernel(const int *in, int *out, int64_t n, int64_t w,
+                                                                const int64_t *indptr, const uint32_t *ids) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int64_t lo = i / (2 * w) * (2 * w), mid = min(lo + w, n), hi = min(lo + 2 * w, n);
+  const int x = in[i];
+  const bool left = i < mid;
+  int64_t a = left ? mid : lo, b = left ? hi : mid;  // search [a, b) for the first element placed after x
+  while (a < b) {
+    const int64_t m = (a + b) >> 1;
+    const int c = cmp_queries(indptr, ids, in[m], x);
+    if (left ? c < 0 : c <= 0) a = m + 1;
+    else b = m;
+  }
+  out[left ? i + (a - mid) : (i - mid) + a] = x;
+}
+
+// qperm / qsrc (the CSR rows are the original queries) and the flags by sorted slot
+__global__ void __launch_bounds__(TQ_THREADS) slot_order_kernel(const int *order, const uint8_t *flag_row, int64_t n,
+                                                                int *qperm, uint8_t *flags) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int row = order[i];
+  qperm[i] = row;
+  qperm[2 * n + i] = row;
+  flags[i] = flag_row[row];
+}
+
+}  // namespace
+
+static int prepare_batch_text(kv_index *ix, kv_vocab_mirror *m, const kv_vocab *v, const char *bytes,
+                              const int64_t *offsets, int64_t n_q, int mode, int64_t *bad_doc) {
+  if (!ix->finalized) return kv_fail(KV_ERR_STATE, "kv_topk: index not finalized");
+  if (n_q < 1) return kv_fail(KV_ERR_INVALID, "kv_topk: empty query batch");
+  if (n_q >= (1LL << 31) - TILE_Q) return kv_fail(KV_ERR_INVALID, "kv_topk: too many queries in one call");
+  if (mirror_device(m) != ix->device)
+    return kv_fail(KV_ERR_INVALID, "kv_query_upload_text: the vocabulary mirror is on device %d, the index on device %d",
+                   mirror_device(m), ix->device);
+  KV_CUDA(cudaSetDevice(ix->device));
+  cudaStream_t s = ix->stream;
+  ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
+  ix->has_excl = ix->has_filter = ix->distinct = false;
+  ix->irr_q.clear(); ix->irr_indptr.assign(1, 0); ix->irr_ids.clear(); ix->irr_tf.clear(); ix->irr_oov.clear();
+  const auto t_begin = std::chrono::steady_clock::now();
+
+  // ---- the text goes up and is featurised into the query CSR (by row) ----
+  int64_t nnz = 0;
+  {
+    mirror_lock(m);
+    int rc = mirror_sync_locked(m, v);
+    if (rc == KV_OK) rc = featurize_device(m, s, bytes, offsets, n_q, mode, ix->d_q_indptr, ix->d_q_ids, ix->d_q_tf,
+                                           ix->d_q_oov, &nnz, bad_doc);
+    if (rc == KV_OK && cudaStreamSynchronize(s) != cudaSuccess)  // the mirror's scratch is read until here
+      rc = kv_fail(KV_ERR_CUDA, "kv_query_upload_text: featurisation failed: %s", cudaGetErrorString(cudaGetLastError()));
+    mirror_unlock(m);
+    if (rc != KV_OK) return rc;
+  }
+  ix->last_prepare_ms[0] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+
+  // ---- classification and text order on the device ----
+  KV_CUDA(ix->d_qflag_row.ensure(n_q));
+  KV_CUDA(ix->d_qorder.ensure(2 * n_q));
+  KV_CUDA(ix->d_qperm.ensure(3 * n_q));
+  KV_CUDA(ix->d_flags.ensure(n_q));
+  KV_CUDA(ix->h_qperm.ensure(3 * n_q));
+  KV_CUDA(ix->h_flags.ensure(n_q));
+  const double amax = ix->jaccard ? 1.0 : std::pow(std::log((double)(ix->n_total + 2)) + 1.0, 2.0);
+  KV_CUDA(cudaEventRecord(ix->evq[0], s));
+  classify_kernel<<<tq_grid(n_q), TQ_THREADS, 0, s>>>(ix->d_q_indptr.p, ix->d_q_ids.p, ix->d_q_tf.p, n_q, ix->V, ix->corpus_fit,
+                                                     ix->d_df.p, ix->d_univ.p, ix->d_tfmax.p, amax, ix->d_qflag_row.p);
+  KV_CUDA(cudaGetLastError());
+  KV_CUDA(cudaEventRecord(ix->evq[1], s));
+  int *cur = ix->d_qorder.p, *other = cur + n_q;
+  iota_kernel<<<tq_grid(n_q), TQ_THREADS, 0, s>>>(cur, n_q);
+  for (int64_t w = 1; w < n_q; w *= 2) {
+    merge_pass_kernel<<<tq_grid(n_q), TQ_THREADS, 0, s>>>(cur, other, n_q, w, ix->d_q_indptr.p, ix->d_q_ids.p);
+    std::swap(cur, other);
+  }
+  KV_CUDA(cudaGetLastError());
+  KV_CUDA(cudaEventRecord(ix->evq[2], s));
+  slot_order_kernel<<<tq_grid(n_q), TQ_THREADS, 0, s>>>(cur, ix->d_qflag_row.p, n_q, ix->d_qperm.p, ix->d_flags.p);
+  KV_CUDA(cudaGetLastError());
+  {
+    const int rc = build_query_tables(ix, n_q);
+    if (rc != KV_OK) return rc;
+  }
+  // ---- back to the host: the order and flags (filters, exclusions and the test hooks read them), the null list ----
+  unsigned long long f2_out = 0;
+  KV_CUDA(cudaMemcpyAsync(ix->h_qperm.p, ix->d_qperm.p, (size_t)n_q * sizeof(int), cudaMemcpyDeviceToHost, s));
+  KV_CUDA(cudaMemcpyAsync(ix->h_flags.p, ix->d_flags.p, (size_t)n_q, cudaMemcpyDeviceToHost, s));
+  KV_CUDA(cudaMemcpyAsync(&f2_out, ix->d_f2out.p, sizeof(f2_out), cudaMemcpyDeviceToHost, s));
+  KV_CUDA(cudaEventRecord(ix->evq[3], s));
+  KV_CUDA(cudaStreamSynchronize(s));
+  int *qperm = ix->h_qperm.p, *null_list = qperm + n_q, *qsrc = qperm + 2 * n_q;
+  int64_t n_null = 0, n_irr = 0;
+  for (int64_t i = 0; i < n_q; i++) {
+    qsrc[i] = qperm[i];
+    if (ix->h_flags.p[i] == 1) null_list[n_null++] = qperm[i];
+    else if (ix->h_flags.p[i] == 2) n_irr++;
+  }
+  if (n_null) KV_CUDA(cudaMemcpyAsync(ix->d_qperm.p + n_q, null_list, (size_t)n_null * sizeof(int), cudaMemcpyHostToDevice, s));
+  // the irregular queries' CSR, for the float64 fallback (rare: one copy per query)
+  if (n_irr) {
+    KV_CUDA(ix->h_q_indptr.ensure(n_q + 1));
+    KV_CUDA(ix->h_q_oov.ensure(n_q));
+    KV_CUDA(cudaMemcpyAsync(ix->h_q_indptr.p, ix->d_q_indptr.p, (size_t)(n_q + 1) * 8, cudaMemcpyDeviceToHost, s));
+    KV_CUDA(cudaMemcpyAsync(ix->h_q_oov.p, ix->d_q_oov.p, (size_t)n_q * 8, cudaMemcpyDeviceToHost, s));
+    KV_CUDA(cudaStreamSynchronize(s));
+    for (int64_t i = 0; i < n_q; i++) {
+      if (ix->h_flags.p[i] != 2) continue;
+      const int64_t q = qperm[i], a = ix->h_q_indptr.p[q], b = ix->h_q_indptr.p[q + 1];
+      const size_t at = ix->irr_ids.size();
+      ix->irr_q.push_back(q);
+      ix->irr_ids.resize(at + (size_t)(b - a));
+      ix->irr_tf.resize(at + (size_t)(b - a));
+      if (b > a) {
+        KV_CUDA(cudaMemcpyAsync(ix->irr_ids.data() + at, ix->d_q_ids.p + a, (size_t)(b - a) * 4, cudaMemcpyDeviceToHost, s));
+        KV_CUDA(cudaMemcpyAsync(ix->irr_tf.data() + at, ix->d_q_tf.p + a, (size_t)(b - a) * 4, cudaMemcpyDeviceToHost, s));
+      }
+      ix->irr_indptr.push_back((int64_t)ix->irr_ids.size());
+      ix->irr_oov.push_back(ix->h_q_oov.p[q]);
+    }
+  }
+  KV_CUDA(cudaStreamSynchronize(s));
+  ix->batch_f2_outside = (int64_t)f2_out;
+  ix->batch_q = n_q;
+  ix->batch_tiles = (n_q + TILE_Q - 1) / TILE_Q;
+  ix->batch_null = n_null;
+  ix->batch_h2d_bytes = (offsets[n_q] - offsets[0]) + (n_q + 1) * 8 + n_null * (int64_t)sizeof(int);
+  ix->batch_valid = true;
+  cudaEventElapsedTime(&ix->last_prepare_ms[1], ix->evq[0], ix->evq[1]);
+  cudaEventElapsedTime(&ix->last_prepare_ms[2], ix->evq[1], ix->evq[2]);
+  cudaEventElapsedTime(&ix->last_prepare_ms[3], ix->evq[2], ix->evq[3]);
+  ix->last_ms[0] = 0;  // no CSR crossed the bus
+  return KV_OK;
 }
 
 // Device-only half: bounds + scans + merge (+ fallback scans for irregular queries) of the uploaded batch.
@@ -1727,6 +1939,23 @@ int kv_query_upload(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids
   if (!ix || n_q < 1 || !q_indptr) return kv_fail(KV_ERR_INVALID, "kv_query_upload: bad arguments");
   std::lock_guard<std::mutex> g(ix->mu);
   return prepare_batch(ix, q_indptr, q_ids, q_tf, q_oov_tf2, n_q);
+}
+
+int kv_query_upload_text(kv_index *ix, kv_vocab_mirror *m, const kv_vocab *v, const char *bytes, const int64_t *offsets,
+                         int64_t n_q, int mode, int64_t *bad_doc) {
+  if (!ix || !m || !v || n_q < 1 || !offsets || !bytes) return kv_fail(KV_ERR_INVALID, "kv_query_upload_text: bad arguments");
+  std::lock_guard<std::mutex> g(ix->mu);
+  return prepare_batch_text(ix, m, v, bytes, offsets, n_q, mode, bad_doc);
+}
+
+int kv_debug_query_order(kv_index *ix, int32_t *qperm, uint8_t *flags, int64_t n_q) {
+  if (!ix || !qperm || !flags) return kv_fail(KV_ERR_INVALID, "kv_debug_query_order: bad arguments");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_debug_query_order: no resident batch");
+  if (n_q != ix->batch_q) return kv_fail(KV_ERR_INVALID, "kv_debug_query_order: the batch has %lld queries", (long long)ix->batch_q);
+  memcpy(qperm, ix->h_qperm.p, (size_t)n_q * sizeof(int));
+  memcpy(flags, ix->h_flags.p, (size_t)n_q);
+  return KV_OK;
 }
 
 // A slice of a query batch prepared where it was featurised: the slice's CSR re-stored in text order (s_* outputs, row

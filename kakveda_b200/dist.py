@@ -26,7 +26,7 @@ import numpy as np
 
 from . import _capi
 from ._capi import no_distinct
-from .similarity import FeatureBatch, GfkbIndex, Vocabulary, gather_rows, text_order
+from .similarity import FeatureBatch, GfkbIndex, Vocabulary, _featurize_on_device, gather_rows, text_order
 
 
 def shard_bounds(n_rows: int, world: int, rank: int) -> Tuple[int, int]:
@@ -408,6 +408,22 @@ class ShardedGfkb:
             t4 = time.perf_counter()
             self.last_e2e_ms = {"prepare_sharded": 1e3 * (t2 - t0), "device_step": 1e3 * (t3 - t2), "read_back": 1e3 * (t4 - t3),
                                 "prepare_split": self.last_prepare_split_ms}
+            return out
+        n_q = len(offsets) - 1
+        if self.world == 1 and n_q and _featurize_on_device(n_q):
+            import torch
+
+            self.index.upload_text(data, offsets, mode)   # featurise, classify and order on the device
+            self._resident_q = n_q
+            t2 = time.perf_counter()
+            s, r = self.topk_resident(k)
+            torch.cuda.current_stream().synchronize()
+            t3 = time.perf_counter()
+            out = self._read_back(s, r)
+            t4 = time.perf_counter()
+            prep = self.index.last_prepare_ms()  # text upload + featurisation, classification, order, tables + copies
+            self.last_e2e_ms = {"featurize": prep[0], "upload": 1e3 * (t2 - t0) - prep[0], "device_step": 1e3 * (t3 - t2),
+                                "read_back": 1e3 * (t4 - t3), "upload_device_ms": prep}
             return out
         qfb = self.vocab.featurize_packed(data, offsets, mode, grow=False)
         try:

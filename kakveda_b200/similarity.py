@@ -13,6 +13,7 @@ back to scikit-learn or NumPy math: without the library or without a GPU the cal
 from __future__ import annotations
 
 import ctypes as C
+import os
 import re
 import threading
 from dataclasses import dataclass, field
@@ -23,6 +24,19 @@ import numpy as np
 from . import _capi, _devout
 
 _TOKEN = re.compile(r"(?u)\b\w\w+\b")  # sklearn text.py:1969; used only for non-ASCII documents
+
+# Query batches of at least this many texts are featurised, classified and text-ordered on the device
+# (kv_query_upload_text); smaller ones take the host featuriser and kv_query_upload.  Both give the same resident batch.
+# Measured in DESIGN §6 ("Device featuriser").
+DEVICE_FEATURIZE_MIN_QUERIES = 128
+
+
+def _featurize_on_device(n: int) -> bool:
+    """Which path a text batch of n queries takes.  KAKVEDA_B200_FEATURIZE=host|device forces one (tests)."""
+    force = os.environ.get("KAKVEDA_B200_FEATURIZE")
+    if force in ("host", "device"):
+        return force == "device"
+    return n >= DEVICE_FEATURIZE_MIN_QUERIES
 
 
 def _ptr(a: np.ndarray, ctype):
@@ -140,6 +154,7 @@ class Vocabulary:
         h = C.c_void_p()
         _capi.check(lib.kv_vocab_create(C.byref(h)))
         self._h = h
+        self._mirrors = {}  # device -> kv_vocab_mirror, created on first use
 
     def __len__(self) -> int:
         return int(_capi.load().kv_vocab_size(self._h))
@@ -177,7 +192,33 @@ class Vocabulary:
         data, offsets, mode = pack_texts(texts)
         return self.featurize_packed(data, offsets, mode, grow, n_threads)
 
+    def mirror(self, device: int) -> C.c_void_p:
+        """The device mirror of this vocabulary on ``device`` (created on first use), synced to the features it has
+        now.  Raises RuntimeError while a concurrent ``featurize(grow=True)`` keeps the vocabulary changing."""
+        lib = _capi.load()
+        m = self._mirrors.get(device)
+        if m is None:
+            m = C.c_void_p()
+            _capi.check(lib.kv_vocab_mirror_create(device, C.byref(m)))
+            self._mirrors[device] = m
+        _capi.check(lib.kv_vocab_mirror_sync(m, self._h, None))
+        return m
+
+    def featurize_packed_device(self, data, offsets: np.ndarray, mode: int, device: int = 0) -> FeatureBatch:
+        """``featurize_packed(..., grow=False)`` computed on ``device`` (same result bit for bit)."""
+        lib = _capi.load()
+        offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+        m = self.mirror(device)
+        out = C.c_void_p()
+        buf = data.ctypes.data_as(C.c_char_p) if isinstance(data, np.ndarray) else C.c_char_p(data)
+        _capi.check(lib.kv_featurize_device(m, self._h, buf, _ptr(offsets, C.c_int64), len(offsets) - 1, mode,
+                                            C.byref(out), None))
+        return FeatureBatch(out)
+
     def close(self) -> None:
+        for m in self._mirrors.values():
+            _capi.load().kv_vocab_mirror_destroy(m)
+        self._mirrors = {}
         if self._h is not None:
             _capi.load().kv_vocab_destroy(self._h)
             self._h = None
@@ -350,6 +391,25 @@ class GfkbIndex:
         _capi.check(_capi.load().kv_query_upload(self._h, _ptr(fb.indptr, C.c_int64), _ptr(fb.ids, C.c_uint32),
                                                  _ptr(fb.tf, C.c_uint32), _ptr(fb.oov, C.c_double), fb.n))
 
+    def upload_text(self, data, offsets: np.ndarray, mode: int) -> int:
+        """``upload_queries(vocab.featurize_packed(data, offsets, mode, grow=False))`` done on the device: the text goes
+        up and featurisation, classification and text order run there.  The resident batch is the same.  Returns the
+        number of queries."""
+        offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+        m = self.vocab.mirror(self.device)
+        buf = data.ctypes.data_as(C.c_char_p) if isinstance(data, np.ndarray) else C.c_char_p(data)
+        _capi.check(_capi.load().kv_query_upload_text(self._h, m, self.vocab._h, buf, _ptr(offsets, C.c_int64),
+                                                      len(offsets) - 1, mode, None))
+        return len(offsets) - 1
+
+    def query_order(self, n_q: int) -> Tuple[np.ndarray, np.ndarray]:
+        """Test hook: (qperm int32[n_q], flags uint8[n_q]) of the resident batch -- the original query at each sorted
+        slot and its class (0 regular, 1 null, 2 irregular)."""
+        qperm = np.empty(n_q, dtype=np.int32)
+        flags = np.empty(n_q, dtype=np.uint8)
+        _capi.check(_capi.load().kv_debug_query_order(self._h, _ptr(qperm, C.c_int32), _ptr(flags, C.c_uint8), n_q))
+        return qperm, flags
+
     def prepare_slice(self, fb, out=None):
         """A slice of a query batch re-stored in text order, as a run for ``upload_query_runs``: returns
         ``(indptr, ids, tf, oov, order, flags)`` where row p is the slice's p-th smallest query, ``order[p]`` its original
@@ -484,6 +544,11 @@ class GfkbIndex:
     def range(self, queries: Sequence[str], threshold: float, device_out: bool = False,
               labels: Optional[np.ndarray] = None):
         """``range_features`` of texts."""
+        if len(queries) and _featurize_on_device(len(queries)):
+            self.upload_text(*pack_texts(queries))
+            if labels is not None:
+                self.set_filter(labels)
+            return self._range_resident(len(queries), threshold, device_out)
         fb = self.vocab.featurize(queries, grow=False)
         try:
             return self.range_features(fb, threshold, device_out, labels)
@@ -531,6 +596,13 @@ class GfkbIndex:
         """(scores float32 [Q,k], rows int64 [Q,k]) ordered by (score desc, row asc) (K1b+K5).  ``labels``: per query
         the row label its results must carry (-1: any row).  ``distinct``: at most one row per group (the best one;
         ``set_row_groups``)."""
+        if len(queries) and _featurize_on_device(len(queries)):
+            self.upload_text(*pack_texts(queries))
+            if labels is not None:
+                self.set_filter(labels)
+            if distinct:
+                self.set_distinct(True)
+            return self.topk_resident_host(len(queries), k)
         fb = self.vocab.featurize(queries, grow=False)
         try:
             return self.topk_features(fb, k, labels, distinct)
