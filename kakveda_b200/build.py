@@ -1,11 +1,12 @@
 """Build libkakveda_b200.so in-tree with nvcc for sm_90a (H100; no torch types cross the C ABI).
 
-    python -m kakveda_b200.build [--force] [--verbose] [--scan-clocks]
+    python -m kakveda_b200.build [--force] [--verbose] [--scan-clocks | --bound-clocks]
 
 The shared object lands in ``kakveda_b200/lib/`` (git-ignored build product).  ``__graft_entry__.build()``
 calls :func:`build`.  ``--scan-clocks`` builds the measuring variant of the candidate scan
 (``-DKV_SCAN_CLOCKS``) into ``libkakveda_b200_scanclocks.so`` next to the product library, which it leaves alone;
-``profiles/run_scan_split.py`` loads it through ``KAKVEDA_B200_LIB``.
+``profiles/run_scan_split.py`` loads it through ``KAKVEDA_B200_LIB``.  ``--bound-clocks`` does the same for the bound
+kernel (``-DKV_BOUND_CLOCKS``, ``libkakveda_b200_boundclocks.so``, ``profiles/run_bound_split.py``).
 """
 from __future__ import annotations
 
@@ -38,6 +39,7 @@ def sources() -> list[Path]:
 
 
 SCAN_CLOCKS = dict(defines=("KV_SCAN_CLOCKS",), name="libkakveda_b200_scanclocks")
+BOUND_CLOCKS = dict(defines=("KV_BOUND_CLOCKS",), name="libkakveda_b200_boundclocks")
 
 
 def _digest(defines: tuple[str, ...] = ()) -> str:
@@ -94,4 +96,5 @@ def build(force: bool = False, verbose: bool = False, defines: tuple[str, ...] =
 
 
 if __name__ == "__main__":
-    print(build(force="--force" in sys.argv, verbose="--verbose" in sys.argv, **(SCAN_CLOCKS if "--scan-clocks" in sys.argv else {})))
+    variant = SCAN_CLOCKS if "--scan-clocks" in sys.argv else BOUND_CLOCKS if "--bound-clocks" in sys.argv else {}
+    print(build(force="--force" in sys.argv, verbose="--verbose" in sys.argv, **variant))

@@ -58,9 +58,50 @@ constexpr int B_THREADS = (B_WORKERS + 4) * 32;
 // the MMA warpgroup among itself (a chunk slice has been read by all four warps and may be refilled)
 constexpr int B_BAR_RFULL = 1, B_BAR_RCLEAN = 2, B_BAR_WORKERS = 3, B_BAR_MMA = 4;
 constexpr int B_COLS = B_BN / 4;             // chunk columns per epilogue thread (four threads serve a query)
+// Words per chunk row of R: the tile's queries and four of padding.  The MMA warpgroup's lanes add to chunks
+// 2 (lane % 4) + const and queries lane / 4 + const: with 128-word rows those are 8 banks, four lanes each at different
+// addresses; with 132-word rows the bank is 8 (lane % 4) + lane / 4 + const, 32 different ones.  The read-out (a warp =
+// 32 consecutive queries of one chunk row) is conflict-free with either.
+constexpr int B_RSTRIDE = TILE_Q + 4;
 constexpr int B_SEEDS = 4;                   // seeds per worker thread
 constexpr int B_SEEDS_PER_QUERY = 4 * B_SEEDS;
 constexpr float UBQ_SCALE = 250.f;           // 8-bit bound code = ceil(bound * 250), saturating at 255 (bounds reach ~1.001)
+
+// Measuring build of K1b-B (-DKV_BOUND_CLOCKS, profiles/run_bound_split.py): every warp splits each 64-chunk block of
+// its loop into clock() spans and counts what the rare join meets, every CTA notes its start and end on the global
+// timer, and all of it is added to g_bound_prof, which kv_debug_bound_profile reads.  The product build defines none
+// of this: KV_BOUND_PROF(...) and KV_BOUND_MARK(...) expand to nothing.
+#ifdef KV_BOUND_CLOCKS
+constexpr int KB_MAX_CTAS = 4096;  // CTAs whose start and end are kept (the bench shape launches 782)
+enum {
+  // cycles, per worker warp
+  KBW_BITMAP, KBW_JOIN1, KBW_JOIN2, KBW_JOIN3, KBW_FANOUT, KBW_RFULL, KBW_READOUT, KBW_F2LEFT, KBW_BOUND, KBW_STORE, KBW_BARRIER,
+  KBW_N,
+  // cycles, per warp of the MMA warpgroup
+  KBM_GEMM = KBW_N, KBM_RCLEAN, KBM_ADDS, KBM_B2, KB_NSPANS,
+  // counters: the join's bitmap hits, table hits, probe continuations and hit-mask bits (per thread, summed); fan-out
+  // iterations of a warp with one loop per list entry (sum over entries of the largest lane) and with one loop per
+  // thread (largest lane total); per block the slowest worker warp's join, and which side reached RFULL last
+  KBC_BIT_HITS = KB_NSPANS, KBC_TABLE_HITS, KBC_PROBE_CONT, KBC_MASK_BITS, KBC_FAN_PER_ENTRY, KBC_FAN_ONE_LOOP,
+  KBC_JOIN_SLOWEST, KBC_MMA_LAST, KBC_MMA_LAST_CYC, KBC_WORKERS_LAST_CYC, KBC_WORKER_WARP_BLOCKS, KBC_MMA_WARP_BLOCKS,
+  KBC_CTA_BLOCKS, KBC_CTAS, KB_NSLOTS,
+  KBT_START = KB_NSLOTS,               // [KB_MAX_CTAS] globaltimer ns, by blockIdx.y * gridDim.x + blockIdx.x
+  KBT_END = KBT_START + KB_MAX_CTAS,   // [KB_MAX_CTAS]
+  KB_TOTAL = KBT_END + KB_MAX_CTAS
+};
+__device__ unsigned long long g_bound_prof[KB_TOTAL];
+__device__ __forceinline__ unsigned long long kb_globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+#define KV_BOUND_PROF(...) __VA_ARGS__
+// charges the cycles since the previous mark to a span (the warp is converged first, lane 0's clock is the warp's)
+#define KV_BOUND_MARK(slot) { __syncwarp(); const unsigned int kbp_n = clock(); kbp[slot] += kbp_n - kbp_t; kbp_t = kbp_n; }
+#else
+#define KV_BOUND_PROF(...)
+#define KV_BOUND_MARK(slot)
+#endif
 
 // D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, fp16 in, fp32 accumulators in registers (both operands K-major)
 __device__ __forceinline__ void wgmma_m64n64k16_f16(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
@@ -105,6 +146,13 @@ __device__ __forceinline__ float rsqrt_approx(float x) {
   float y;
   asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
+}
+
+// ceil(v) clamped to 0 .. 255 as an integer, v any float (NaN: 255): the same value as (uint32_t)fminf(255.f, ceilf(v))
+// without the FRND and F2I of the conversion pipe.  At 2^23 one ulp of a float is 1, so adding 2^23 to a v in [0, 255]
+// rounding up leaves ceil(v) in the low mantissa bits.
+__device__ __forceinline__ uint32_t ceil_to_byte(float v) {
+  return __float_as_uint(__fadd_ru(fmaxf(fminf(v, 255.f), 0.f), 8388608.f)) & 0xFFu;
 }
 
 // The candidate lists of a batch: list l = group * n_bsplits + bsplit holds records {chunk, mask of the group's queries}
@@ -203,10 +251,13 @@ struct __align__(1024) BoundSmem {
   unsigned char b[B_STAGES][B_B_SLICE_BYTES];    // chunk slices in flight
   unsigned char b2[B_KSLICES2][B_B_SLICE_BYTES]; // the block's dictionary columns (0 / 1 / T), built by the MMA warpgroup
   uint32_t rbm[RB_BITS / 32];                    // rare-feature presence bitmap of the block
-  uint32_t R[B_BN][TILE_Q];                      // the dot bound without the query constants, units of 1 / s_q, [chunk][query]
+  uint32_t R[B_BN][B_RSTRIDE];                   // the dot bound without the query constants, units of 1 / s_q, [chunk][query]
   float minB[2][B_BN];
   uint64_t full_bar[B_STAGES], a_bar, blk_bar;
   unsigned int lcount[4];
+  // of the block in hand, clocks relative to prof_t0: the longest join of a worker warp, the last worker warp's and
+  // the MMA warpgroup's arrival at RFULL
+  KV_BOUND_PROF(unsigned int prof_t0, prof_join_max, prof_w_arrive, prof_m_arrive;)
   int pages[1];  // [4][max_pages], sized at launch
 };
 
@@ -233,10 +284,13 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
     mbar_init(&S.a_bar, 1);
     mbar_init(&S.blk_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    KV_BOUND_PROF(S.prof_t0 = clock(); S.prof_join_max = S.prof_w_arrive = S.prof_m_arrive = 0;
+                  const unsigned int cta = blockIdx.y * gridDim.x + blockIdx.x;
+                  if (cta < KB_MAX_CTAS) g_bound_prof[KBT_START + cta] = kb_globaltimer();)
   }
   {  // R = 0, list state
     uint4 *r4 = (uint4 *)&S.R[0][0];
-    for (int i = threadIdx.x; i < B_BN * TILE_Q / 4; i += B_THREADS) r4[i] = make_uint4(0u, 0u, 0u, 0u);
+    for (int i = threadIdx.x; i < B_BN * B_RSTRIDE / 4; i += B_THREADS) r4[i] = make_uint4(0u, 0u, 0u, 0u);
     for (int i = threadIdx.x; i < 4 * P.lists.max_pages; i += B_THREADS) S.pages[i] = -1;
     if (threadIdx.x < 4) S.lcount[threadIdx.x] = 0;
   }
@@ -316,6 +370,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
     int stage = 0;
     uint32_t phase = 0;
     int g = 0;
+    KV_BOUND_PROF(unsigned int kbp[KB_NSPANS] = {}; unsigned int kbp_t = clock(); const unsigned int kb_t0 = S.prof_t0;)
     for (int it = 0; it < n_blk; it++) {
 #pragma unroll
       for (int h = 0; h < 2; h++)
@@ -357,8 +412,10 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
 #pragma unroll
         for (int i = 0; i < 32; i++) wgmma_reg_fence(acc[h][i]);
       release(g - 1);
+      KV_BOUND_MARK(KBM_GEMM)
       // R holds the previous block's values until the workers' epilogue has read and cleared them
       if (it > 0) asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_RCLEAN), "n"(B_THREADS) : "memory");
+      KV_BOUND_MARK(KBM_RCLEAN)
 #pragma unroll
       for (int h = 0; h < 2; h++) {
         const int q0 = h * 64 + wq * 16 + (lane >> 2);
@@ -369,14 +426,22 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
           atomicAdd(&S.R[c][q0 + 8 * ((i >> 1) & 1)], __float2uint_ru(acc[h][i] * sq[h][(i >> 1) & 1]));
         }
       }
+      KV_BOUND_PROF(if (wq == 0 && lane == 0) S.prof_m_arrive = clock() - kb_t0;)
       asm volatile("bar.arrive %0, %1;" ::"n"(B_BAR_RFULL), "n"(B_THREADS) : "memory");
+      KV_BOUND_MARK(KBM_ADDS)
       // the GEMM of this block is done (wgmma_wait above): B2 takes the next block's columns
       if (it + 1 < n_blk) {
         build_b2();
         if (it + 2 < n_blk) fetch_rows(it + 2);
         publish_b2();
       }
+      KV_BOUND_MARK(KBM_B2)
     }
+    KV_BOUND_PROF(if (lane == 0) {
+      _Pragma("unroll")
+      for (int i = KBM_GEMM; i < KB_NSPANS; i++) atomicAdd(&g_bound_prof[i], (unsigned long long)kbp[i]);
+      atomicAdd(&g_bound_prof[KBC_MMA_WARP_BLOCKS], (unsigned long long)n_blk);
+    })
     if (n_blk > 0) asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_RCLEAN), "n"(B_THREADS) : "memory");  // the last block's
   } else {
     // ===== workers: join, then epilogue, per block =====
@@ -415,11 +480,20 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
     // distinct ones): added per block from the bitmaps in global memory; most warps have none and skip the loop
     const uint2 *ql2 = P.q2list + (size_t)tile * Q2CAP * TILE_Q + qi;
     const bool warp_left = __any_sync(FULL, q_ok && __uint_as_float(ql2[0].y) > 0.f);
+    // size and offset of the block's rare table, loaded one block ahead: the first-slot key loads need them at once,
+    // and loaded in the join they were a third dependent L2 round trip of every block
+    uint32_t tsize_n = 0, toff_n = 0;
+    if (blk_lo < blk_hi) { tsize_n = P.rt_size[blk_lo]; toff_n = P.rt_off[blk_lo]; }
     int64_t it = 0;
+    KV_BOUND_PROF(unsigned int kbp[KB_NSPANS] = {}; unsigned int kbp_t = clock(); const unsigned int kb_t0 = S.prof_t0;
+                  unsigned int kbc_bit = 0, kbc_tab = 0, kbc_cont = 0, kbc_bits = 0, kbc_fan_entry = 0, kbc_fan_one = 0;
+                  unsigned long long kbc_slowest = 0, kbc_mma_last = 0, kbc_mma_cyc = 0, kbc_w_cyc = 0;)
     for (int64_t bk = blk_lo; bk < blk_hi; bk++, it++) {
       const int as = (int)(it & 1);
       const int64_t c0 = bk * B_BN;
       mbar_wait(&S.blk_bar, (uint32_t)(it & 1));
+      KV_BOUND_MARK(KBW_BITMAP)
+      KV_BOUND_PROF(const unsigned int kb_join0 = kbp_t;)
       // ---- rare join, inverted: thread (query, quarter of its rare list) tests each feature in the block's presence
       //      bitmap; on a hit it probes the block's table (L2) and adds weight x tf to R[chunk][query] for every chunk
       //      of the mask.  Rows are text-sorted, so one feature can sit in most chunks of a block: R is dense.
@@ -428,7 +502,8 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
       //      per hit. ----
       {
         const uint32_t *bm = S.rbm;
-        const uint32_t tsize = P.rt_size[bk], toff = P.rt_off[bk];
+        const uint32_t tsize = tsize_n, toff = toff_n;
+        if (bk + 1 < blk_hi) { tsize_n = P.rt_size[bk + 1]; toff_n = P.rt_off[bk + 1]; }
         uint32_t h[NR], key[NR];
 #pragma unroll
         for (int k = 0; k < NR; k++) {
@@ -436,13 +511,17 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
           const bool hit = fid[k] < FID_NONE && ((bm[bb >> 5] >> (bb & 31u)) & 1u);
           h[k] = rt_slot(fid[k], tsize);
           key[k] = hit ? __ldg(P.rt_keys + toff + h[k]) : KEY_EMPTY;
+          KV_BOUND_PROF(kbc_bit += hit;)
         }
+        KV_BOUND_MARK(KBW_JOIN1)
 #pragma unroll
         for (int k = 0; k < NR; k++)  // first slot taken by another feature: continue the linear probe
           while (key[k] != KEY_EMPTY && (key[k] >> 5) != fid[k]) {
             h[k] = h[k] + 1 == tsize ? 0 : h[k] + 1;
             key[k] = __ldg(P.rt_keys + toff + h[k]);
+            KV_BOUND_PROF(kbc_cont++;)
           }
+        KV_BOUND_MARK(KBW_JOIN2)
         unsigned long long cm[NR];
         uint32_t tf[NR], w[NR];
 #pragma unroll
@@ -452,12 +531,27 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
           w[k] = found ? __ldg(P.q3w + q3o + (size_t)k * 4 * TILE_Q) : 0u;
           tf[k] = key[k] & 31u;
           if (found && tf[k] == TF_OVF) tf[k] = __ldg(P.tfmax + fid[k]);
+          KV_BOUND_PROF(kbc_tab += found;)
         }
+        KV_BOUND_MARK(KBW_JOIN3)
+        KV_BOUND_PROF({
+          unsigned int mine = 0;
+          _Pragma("unroll")
+          for (int k = 0; k < NR; k++) {
+            const unsigned int n = (unsigned int)__popcll(cm[k]);
+            mine += n;
+            kbc_fan_entry += __reduce_max_sync(FULL, n);
+          }
+          kbc_bits += mine;
+          kbc_fan_one += __reduce_max_sync(FULL, mine);
+        })
 #pragma unroll
         for (int k = 0; k < NR; k++) {
           const uint32_t x = w[k] * tf[k];  // fixed point, <= 2^30 + tf (prep_queries_kernel)
           for (unsigned long long m = cm[k]; m; m &= m - 1) atomicAdd(&S.R[__ffsll((long long)m) - 1][jq], x);
         }
+        KV_BOUND_MARK(KBW_FANOUT)
+        KV_BOUND_PROF(if (lane == 0) atomicMax(&S.prof_join_max, kbp_t - kb_join0);)
       }
       if (threadIdx.x < B_BN) S.minB[as][threadIdx.x] = P.chunk_minB[c0 + threadIdx.x];
       // this block's threshold of the query (pass 1: theta0 from the seed scan, possibly raised by peers meanwhile)
@@ -467,16 +561,25 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
         if (th > 0.f) tq = th * th * nq / (PRUNE_SLACK * PRUNE_SLACK);
       }
       // R complete: the workers' rare join and the MMA warpgroup's frequent + second-class part of this block
+      KV_BOUND_PROF(if (lane == 0) atomicMax(&S.prof_w_arrive, clock() - kb_t0);)
       asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_RFULL), "n"(B_THREADS) : "memory");
       if (threadIdx.x == 0 && bk + 1 < blk_hi) fetch_bitmap(bk + 1);  // every join has read this block's bitmap
+      KV_BOUND_MARK(KBW_RFULL)
+      KV_BOUND_PROF(if (threadIdx.x == 0) {  // the next block's values are written after this thread's RCLEAN / WORKERS arrival
+        const unsigned int ta = S.prof_w_arrive, tm = S.prof_m_arrive;
+        if ((int)(tm - ta) > 0) { kbc_mma_last++; kbc_mma_cyc += tm - ta; } else { kbc_w_cyc += ta - tm; }
+        kbc_slowest += S.prof_join_max;
+        S.prof_join_max = S.prof_w_arrive = 0;
+      })
       // ---- epilogue, thread = query, B_COLS chunk columns: R + second-class features outside the dictionary -> bound
       //      -> seed / candidate ----
       float x[B_COLS];
       {
         uint32_t *Rcol = &S.R[cs * B_COLS][qi];
 #pragma unroll
-        for (int j = 0; j < B_COLS; j++) { x[j] = __uint2float_ru(Rcol[j * TILE_Q]) * rs; Rcol[j * TILE_Q] = 0u; }
+        for (int j = 0; j < B_COLS; j++) { x[j] = __uint2float_ru(Rcol[j * B_RSTRIDE]) * rs; Rcol[j * B_RSTRIDE] = 0u; }
       }
+      KV_BOUND_MARK(KBW_READOUT)
       if (warp_left) {
         const uint32_t bsh = (uint32_t)((cs * B_COLS) & 31), bword = (uint32_t)((cs * B_COLS) >> 5);
         constexpr uint32_t CMASK = B_COLS == 32 ? 0xFFFFFFFFu : ((1u << B_COLS) - 1u);
@@ -502,6 +605,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
           }
         }
       }
+      KV_BOUND_MARK(KBW_F2LEFT)
       const float *mb = &S.minB[as][cs * B_COLS];
       const int64_t cbase = c0 + cs * B_COLS;
       uint32_t mymask = 0;
@@ -523,7 +627,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
         } else if (q_ok && c_ok) {
           // the bound itself (slack included): seeds are ranked by it, and it is stored as a code that only errs upwards
           float metric = den > 0.f ? xs * rsqrt_approx(nq * den) * (PRUNE_SLACK * 1.00001f) : INFINITY;
-          if (has_codes) codes[j >> 2] |= (uint32_t)fminf(255.f, ceilf(metric * UBQ_SCALE)) << ((j & 3) * 8);
+          if (has_codes) codes[j >> 2] |= ceil_to_byte(metric * UBQ_SCALE) << ((j & 3) * 8);
           if (metric > sm[B_SEEDS - 1]) {
             int cc = (int)(cbase + j);
 #pragma unroll
@@ -535,14 +639,42 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
           }
         }
       }
+      KV_BOUND_MARK(KBW_BOUND)
       if (pass == 0 && has_codes && q_in)
         *reinterpret_cast<uint4 *>(P.ubq + (size_t)slot * P.ubq_stride + cbase) = make_uint4(codes[0], codes[1], codes[2], codes[3]);
       // four warps (one per chunk-column quarter) share the group's list
       if (pass == 1) list_append(P.lists, list, &S.lcount[qtr], my_pages, (uint32_t)(cbase + lane), mymask, n_pairs, n_recs);
+      KV_BOUND_MARK(KBW_STORE)
       // R is clean again: the MMA warpgroup and, once all workers are here, the next block's join may add to it
       asm volatile("bar.arrive %0, %1;" ::"n"(B_BAR_RCLEAN), "n"(B_THREADS) : "memory");
       asm volatile("bar.sync %0, %1;" ::"n"(B_BAR_WORKERS), "n"(B_WORKERS * 32) : "memory");
+      KV_BOUND_MARK(KBW_BARRIER)
     }
+    KV_BOUND_PROF({
+      kbc_bit = __reduce_add_sync(FULL, kbc_bit); kbc_tab = __reduce_add_sync(FULL, kbc_tab);
+      kbc_cont = __reduce_add_sync(FULL, kbc_cont); kbc_bits = __reduce_add_sync(FULL, kbc_bits);
+      if (lane == 0) {
+        _Pragma("unroll")
+        for (int i = 0; i < KBW_N; i++) atomicAdd(&g_bound_prof[i], (unsigned long long)kbp[i]);
+        atomicAdd(&g_bound_prof[KBC_BIT_HITS], (unsigned long long)kbc_bit);
+        atomicAdd(&g_bound_prof[KBC_TABLE_HITS], (unsigned long long)kbc_tab);
+        atomicAdd(&g_bound_prof[KBC_PROBE_CONT], (unsigned long long)kbc_cont);
+        atomicAdd(&g_bound_prof[KBC_MASK_BITS], (unsigned long long)kbc_bits);
+        atomicAdd(&g_bound_prof[KBC_FAN_PER_ENTRY], (unsigned long long)kbc_fan_entry);
+        atomicAdd(&g_bound_prof[KBC_FAN_ONE_LOOP], (unsigned long long)kbc_fan_one);
+        atomicAdd(&g_bound_prof[KBC_WORKER_WARP_BLOCKS], (unsigned long long)it);
+      }
+      if (threadIdx.x == 0) {
+        atomicAdd(&g_bound_prof[KBC_JOIN_SLOWEST], kbc_slowest);
+        atomicAdd(&g_bound_prof[KBC_MMA_LAST], kbc_mma_last);
+        atomicAdd(&g_bound_prof[KBC_MMA_LAST_CYC], kbc_mma_cyc);
+        atomicAdd(&g_bound_prof[KBC_WORKERS_LAST_CYC], kbc_w_cyc);
+        atomicAdd(&g_bound_prof[KBC_CTA_BLOCKS], (unsigned long long)it);
+        atomicAdd(&g_bound_prof[KBC_CTAS], 1ull);
+        const unsigned int cta = blockIdx.y * gridDim.x + blockIdx.x;
+        if (cta < KB_MAX_CTAS) g_bound_prof[KBT_END + cta] = kb_globaltimer();
+      }
+    })
     if (pass == 0) {
       if (q_in) {
         int *o = P.seeds + ((size_t)slot * P.n_bsplits + bsplit) * B_SEEDS_PER_QUERY + cs * B_SEEDS;

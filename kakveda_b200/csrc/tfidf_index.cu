@@ -2613,3 +2613,17 @@ extern "C" int kv_debug_scan_profile(unsigned long long *out, int n) {
   return KV_OK;
 }
 #endif
+
+#ifdef KV_BOUND_CLOCKS
+// Measuring build only (see KV_BOUND_CLOCKS in bound_kernel.cuh): copies the bound kernel's profile of the current
+// device to out[0..n) and clears it.  n must be the profile's slot count, so a caller with another layout fails.
+extern "C" int kv_debug_bound_profile(unsigned long long *out, int n) {
+  if (!out || n != KB_TOTAL) return kv_fail(KV_ERR_INVALID, "kv_debug_bound_profile: the profile has %d slots", (int)KB_TOTAL);
+  KV_CUDA(cudaDeviceSynchronize());
+  KV_CUDA(cudaMemcpyFromSymbol(out, g_bound_prof, sizeof(g_bound_prof)));
+  void *p = nullptr;
+  KV_CUDA(cudaGetSymbolAddress(&p, g_bound_prof));
+  KV_CUDA(cudaMemset(p, 0, sizeof(g_bound_prof)));
+  return KV_OK;
+}
+#endif
