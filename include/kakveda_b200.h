@@ -419,8 +419,9 @@ int kv_index_layout_load(kv_index *ix, const char *path);
  * [11] = (query, chunk) pairs whose bound passed, [12] = candidate records written, [13] = kernels launched,
  * [14] = block entries of non-frequent features, [15] = candidate-pool pages used, [16] = pool pages allocated,
  * [17] = second-class (query, feature) listings of the last query upload left out of their bound tile's dictionary
- * (the bound kernel's epilogue adds those per block from the second-class bitmaps). */
-int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[18]);
+ * (the bound kernel's epilogue adds those per block from the second-class bitmaps), [18] = slots of the per-block rare
+ * tables (16 bytes each), [19] = rare tables the finalize enlarged past load 0.4 because cuckoo insertion failed. */
+int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[20]);
 
 /* ------------------------------------------------------------------------------------
  * K2: dense-embedding cosine index (bf16 rows of `dim` elements, dim a multiple of 64) with the

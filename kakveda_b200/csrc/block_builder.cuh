@@ -107,13 +107,45 @@ struct BlockLayout {
   std::vector<__half> Uf;                     // [n_chunks_pad][NF] largest tf of the frequent features per chunk
   std::vector<unsigned short> fslot2;         // [V] bit row of a second-class feature, 0xFFFF otherwise
   std::vector<uint32_t> Ubt;                  // [n_chunks_pad / 64][NF2][2][2]: bit c % 64 of plane 0 / 1 = present in chunk c with tf >= 1 / >= 2
-  // rare features per 64-chunk block (the bound kernel's inverted join): presence bitmap + open-addressing table
+  // rare features per 64-chunk block (the bound kernel's inverted join): presence bitmap + two-choice table
   std::vector<uint32_t> rbloom;               // [n_blocks][RB_BITS / 32]
-  std::vector<uint32_t> rt_keys;              // all tables: feature id << 5 | largest tf in the block (31: see tfmax), KEY_EMPTY
-  std::vector<unsigned long long> rt_masks;   // ... chunks of the block holding the feature
+  std::vector<uint4> rt_slots;                // all tables (slot layout: rt_slot2), a feature in slot rt_slot1 or rt_slot2 of its block's
   std::vector<uint32_t> rt_off, rt_size;      // [n_blocks] first slot / slots of a block's table
+  int64_t rt_enlarged = 0;                    // tables whose cuckoo insertion failed at the first size and were enlarged
+  // Only with build_blocks(..., linear_tables = true), for the host layout checks: the same entries placed by linear
+  // probing from rt_slot in tables of the same offsets and sizes, feature id << 5 | largest 5-bit tf (31: see tfmax) and
+  // the chunk mask in separate arrays (the rare-table format before the two-choice slots).  The index never builds them.
+  std::vector<uint32_t> rt_keys;
+  std::vector<unsigned long long> rt_masks;
   int64_t n_entries = 0, n_rare_entries = 0, n_f2_entries = 0;
 };
+
+// Places `n` entries (slots as in rt_slot2) in a two-choice table of *size slots (KEY_EMPTY-initialised by the caller) at tab:
+// cuckoo insertion in the given order with at most RT_MAX_KICKS evictions per entry.  Returns false when an entry found
+// no place; the caller then enlarges the table and starts over.  Deterministic: the same entries in the same order give
+// the same bytes.
+constexpr int RT_MAX_KICKS = 256;
+inline bool rt_cuckoo(const uint4 *entries, size_t n, uint4 *tab, uint32_t size) {
+  for (size_t i = 0; i < n; i++) {
+    uint4 e = entries[i];
+    uint32_t pos = rt_slot1(e.x, size);
+    if (tab[pos].x != KEY_EMPTY) {
+      const uint32_t p2 = rt_slot2(e.x, size);
+      if (tab[p2].x == KEY_EMPTY) pos = p2;
+    }
+    for (int kick = 0;; kick++) {
+      std::swap(e, tab[pos]);
+      if (e.x == KEY_EMPTY) break;
+      if (kick == RT_MAX_KICKS) return false;
+      const uint32_t a = rt_slot1(e.x, size);  // the evicted entry moves to its other slot
+      pos = pos == a ? rt_slot2(e.x, size) : a;
+    }
+  }
+  return true;
+}
+
+// Slots of a block's table for n entries: load factor <= 0.4, at least 4
+inline uint32_t rt_initial_size(size_t n) { return (uint32_t)std::max<size_t>(4, (n * 5 + 1) / 2); }
 
 // the sorted (feature, tf, row-in-chunk) keys of a chunk's non-universal entries
 inline void chunk_keys(const int64_t *indptr, const uint32_t *ids, const uint16_t *tf, const int *perm, int64_t n,
@@ -131,7 +163,8 @@ inline void chunk_keys(const int64_t *indptr, const uint32_t *ids, const uint16_
 }
 
 inline void build_blocks(const int64_t *indptr, const uint32_t *ids, const uint16_t *tf, const int *perm, int64_t n,
-                         int64_t V, const uint8_t *univ, const uint32_t *tfmaxg, int T, BlockLayout &L) {
+                         int64_t V, const uint8_t *univ, const uint32_t *tfmaxg, int T, BlockLayout &L,
+                         bool linear_tables = true) {
   L.n_chunks = (n + CHUNK_ROWS - 1) / CHUNK_ROWS;
   L.n_chunks_pad = std::max<int64_t>(128, (L.n_chunks + 127) / 128 * 128);
   T = (int)std::max<int64_t>(1, std::min<int64_t>(T, std::max<int64_t>(1, L.n_chunks)));
@@ -276,9 +309,11 @@ inline void build_blocks(const int64_t *indptr, const uint32_t *ids, const uint1
       size_t tt = (size_t)(std::upper_bound(L.part_off.begin(), L.part_off.end(), off_words) - L.part_off.begin()) - 1;
       return L.parts[tt].data() + (off_words - L.part_off[tt]);
     };
-    std::vector<std::vector<std::pair<uint32_t, unsigned long long>>> tabs((size_t)n_blocks);  // (key, mask) per block, grouped
-    parallel_for(n_blocks, T, [&](int, int64_t b0, int64_t b1) {
+    std::vector<std::vector<uint4>> tabs((size_t)n_blocks);  // the block's entries as slots, by feature
+    std::vector<int64_t> enlarged((size_t)T, 0);
+    parallel_for(n_blocks, T, [&](int t, int64_t b0, int64_t b1) {
       std::vector<unsigned long long> es;  // fid << 16 | tf5 << 8 | chunk in block
+      std::vector<uint4> scratch;
       for (int64_t b = b0; b < b1; b++) {
         es.clear();
         for (int64_t c = b * 64; c < std::min<int64_t>(L.n_chunks, b * 64 + 64); c++) {
@@ -294,29 +329,45 @@ inline void build_blocks(const int64_t *indptr, const uint32_t *ids, const uint1
           uint32_t tfm = 0;
           unsigned long long mask = 0;
           while (i < es.size() && (uint32_t)(es[i] >> 16) == f) { tfm = std::max<uint32_t>(tfm, (uint32_t)((es[i] >> 8) & 31u)); mask |= 1ULL << (es[i] & 63u); i++; }
-          tab.emplace_back((f << 5) | tfm, mask);
+          // the tf the bound kernel multiplies by: an overflowed 5-bit tf stands for the feature's global largest tf
+          tab.push_back(make_uint4(f, tfm == TF_OVF ? tfmaxg[f] : tfm, (uint32_t)mask, (uint32_t)(mask >> 32)));
           const uint32_t bb = rb_bit(f);
           L.rbloom[(size_t)b * (RB_BITS / 32) + (bb >> 5)] |= 1u << (bb & 31u);
         }
-        L.rt_size[(size_t)b] = (uint32_t)std::max<size_t>(4, tab.size() + tab.size() / 2 + 1);
+        // the size at which the cuckoo insertion succeeds: load <= 0.4, + 25 % per failure
+        uint32_t size = rt_initial_size(tab.size());
+        for (;;) {
+          scratch.assign(size, make_uint4(KEY_EMPTY, 0u, 0u, 0u));
+          if (rt_cuckoo(tab.data(), tab.size(), scratch.data(), size)) break;
+          size += size / 4;
+          enlarged[(size_t)t]++;
+        }
+        L.rt_size[(size_t)b] = size;
       }
     });
     int64_t total = 0;
     for (int64_t b = 0; b < n_blocks; b++) { L.rt_off[(size_t)b] = (uint32_t)total; total += L.rt_size[(size_t)b]; }
-    L.rt_keys.assign((size_t)total, KEY_EMPTY);
-    L.rt_masks.assign((size_t)total, 0ULL);
+    L.rt_slots.assign((size_t)total, make_uint4(KEY_EMPTY, 0u, 0u, 0u));
+    L.rt_enlarged = 0;
+    for (int64_t e : enlarged) L.rt_enlarged += e;
+    L.rt_keys.assign(linear_tables ? (size_t)total : 0, KEY_EMPTY);
+    L.rt_masks.assign(linear_tables ? (size_t)total : 0, 0ULL);
     parallel_for(n_blocks, T, [&](int, int64_t b0, int64_t b1) {
       for (int64_t b = b0; b < b1; b++) {
+        const auto &tab = tabs[(size_t)b];
         const uint32_t size = L.rt_size[(size_t)b];
-        uint32_t *keys = L.rt_keys.data() + L.rt_off[(size_t)b];
-        unsigned long long *masks = L.rt_masks.data() + L.rt_off[(size_t)b];
-        for (auto &e : tabs[(size_t)b]) {
-          uint32_t h = rt_slot(e.first >> 5, size);
-          while (keys[h] != KEY_EMPTY) h = h + 1 == size ? 0 : h + 1;
-          keys[h] = e.first;
-          masks[h] = e.second;
+        rt_cuckoo(tab.data(), tab.size(), L.rt_slots.data() + L.rt_off[(size_t)b], size);  // succeeds at this size
+        if (linear_tables) {
+          uint32_t *keys = L.rt_keys.data() + L.rt_off[(size_t)b];
+          unsigned long long *masks = L.rt_masks.data() + L.rt_off[(size_t)b];
+          for (const uint4 &e : tab) {
+            uint32_t h = rt_slot(e.x, size);
+            while (keys[h] != KEY_EMPTY) h = h + 1 == size ? 0 : h + 1;
+            keys[h] = (e.x << 5) | std::min<uint32_t>(e.y, TF_OVF);
+            masks[h] = (unsigned long long)e.z | ((unsigned long long)e.w << 32);
+          }
         }
-        std::vector<std::pair<uint32_t, unsigned long long>>().swap(tabs[(size_t)b]);
+        std::vector<uint4>().swap(tabs[(size_t)b]);
       }
     });
   }

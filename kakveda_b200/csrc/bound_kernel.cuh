@@ -22,10 +22,11 @@
 //     listing more than KT2 distinct ones leaves the least listed in the queries' lists: the epilogue adds those from
 //     the block's bitmap words in global memory (warps without such a feature skip that loop);
 //   * the remaining RARE features are joined the other way round: every 64-chunk block carries (built at finalize) a
-//     presence bitmap and an open-addressing table of its rare features (feature -> mask of the block's chunks holding
-//     it, largest tf); each query looks ITS OWN <= 32 rare features up -- one shared-memory bit test per (query,
-//     feature, block), and only on a hit a probe of the block's table in L2 -- and adds weight x tf into
-//     R[chunk][query] (shared memory).  1.8k bit tests per tile and block instead of 5.4k entry probes;
+//     presence bitmap and a two-choice table of its rare features (feature -> mask of the block's chunks holding it,
+//     largest tf, in one of two 16-byte slots); each query looks ITS OWN <= 32 rare features up -- one shared-memory bit
+//     test per (query, feature, block), and only on a hit a lookup of the block's table in L2, the warp's hits spread
+//     over its lanes -- and adds weight x tf into R[chunk][query] (shared memory).  1.8k bit tests per tile and block
+//     instead of 5.4k entry probes;
 //   * R is fixed point, uint32 in units of 1 / s_q per query (s_q: a power of two chosen by prep_queries_kernel so that
 //     R cannot wrap), every term rounded up into it: the MMA warpgroup's and the rare join's adds are native integer
 //     shared atomics (a float shared atomicAdd is a compare-and-swap loop on sm_90a);
@@ -75,15 +76,15 @@ constexpr float UBQ_SCALE = 250.f;           // 8-bit bound code = ceil(bound * 
 constexpr int KB_MAX_CTAS = 4096;  // CTAs whose start and end are kept (the bench shape launches 782)
 enum {
   // cycles, per worker warp
-  KBW_BITMAP, KBW_JOIN1, KBW_JOIN2, KBW_JOIN3, KBW_FANOUT, KBW_RFULL, KBW_READOUT, KBW_F2LEFT, KBW_BOUND, KBW_STORE, KBW_BARRIER,
-  KBW_N,
+  KBW_BITMAP, KBW_JOIN_BITS, KBW_JOIN_COMPACT, KBW_JOIN_SLOTS, KBW_FANOUT, KBW_RFULL, KBW_READOUT, KBW_F2LEFT, KBW_BOUND,
+  KBW_STORE, KBW_BARRIER, KBW_N,
   // cycles, per warp of the MMA warpgroup
   KBM_GEMM = KBW_N, KBM_RCLEAN, KBM_ADDS, KBM_B2, KB_NSPANS,
-  // counters: the join's bitmap hits, table hits, probe continuations and hit-mask bits (per thread, summed); fan-out
-  // iterations of a warp with one loop per list entry (sum over entries of the largest lane) and with one loop per
-  // thread (largest lane total); per block the slowest worker warp's join, and which side reached RFULL last
-  KBC_BIT_HITS = KB_NSPANS, KBC_TABLE_HITS, KBC_PROBE_CONT, KBC_MASK_BITS, KBC_FAN_PER_ENTRY, KBC_FAN_ONE_LOOP,
-  KBC_JOIN_SLOWEST, KBC_MMA_LAST, KBC_MMA_LAST_CYC, KBC_WORKERS_LAST_CYC, KBC_WORKER_WARP_BLOCKS, KBC_MMA_WARP_BLOCKS,
+  // counters: the join's bitmap hits (= lookups), lookup rounds of a warp, (warp, block)s needing a second round, table
+  // hits, hit-mask bits and fan-out iterations (largest lane per round); per block the slowest worker warp's join, and
+  // which side reached RFULL last
+  KBC_BIT_HITS = KB_NSPANS, KBC_ROUNDS, KBC_MULTI_ROUND, KBC_TABLE_HITS, KBC_MASK_BITS, KBC_FAN_ITERS, KBC_JOIN_SLOWEST,
+  KBC_MMA_LAST, KBC_MMA_LAST_CYC, KBC_WORKERS_LAST_CYC, KBC_WORKER_WARP_BLOCKS, KBC_MMA_WARP_BLOCKS,
   KBC_CTA_BLOCKS, KBC_CTAS, KB_NSLOTS,
   KBT_START = KB_NSLOTS,               // [KB_MAX_CTAS] globaltimer ns, by blockIdx.y * gridDim.x + blockIdx.x
   KBT_END = KBT_START + KB_MAX_CTAS,   // [KB_MAX_CTAS]
@@ -224,10 +225,8 @@ struct BoundParams {
   int64_t n_chunks, n_q;
   const uint32_t *q3id, *q3w;                             // [n_tiles][Q3CAP][TILE_Q] rare lists: feature, fixed-point weight
   const uint32_t *rbloom;                                 // [n_blocks][RB_BITS / 32]
-  const uint32_t *rt_keys;                                // per-block rare tables: feature << 5 | largest tf (31: tfmax[])
-  const unsigned long long *rt_masks;                     // ... chunks of the block holding the feature
+  const uint4 *rt_slots;                                  // per-block two-choice rare tables (slot layout: rt_slot2)
   const uint32_t *rt_off, *rt_size;                       // [n_blocks]
-  const uint32_t *tfmax;                                  // [V] largest tf of a feature (for entries whose 5-bit tf overflowed)
   const uint32_t *d2col;                                  // [n_tiles][KT2] second-class dictionary (f2_dict_kernel)
   const uint2 *q2list;                                    // [n_tiles][Q2CAP][TILE_Q] second-class features left out of it
   const uint32_t *ubt;                                    // [n_blocks][NF2][2][B_BN / 32]
@@ -486,7 +485,7 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
     if (blk_lo < blk_hi) { tsize_n = P.rt_size[blk_lo]; toff_n = P.rt_off[blk_lo]; }
     int64_t it = 0;
     KV_BOUND_PROF(unsigned int kbp[KB_NSPANS] = {}; unsigned int kbp_t = clock(); const unsigned int kb_t0 = S.prof_t0;
-                  unsigned int kbc_bit = 0, kbc_tab = 0, kbc_cont = 0, kbc_bits = 0, kbc_fan_entry = 0, kbc_fan_one = 0;
+                  unsigned int kbc_bit = 0, kbc_rounds = 0, kbc_multi = 0, kbc_tab = 0, kbc_bits = 0, kbc_fan = 0;
                   unsigned long long kbc_slowest = 0, kbc_mma_last = 0, kbc_mma_cyc = 0, kbc_w_cyc = 0;)
     for (int64_t bk = blk_lo; bk < blk_hi; bk++, it++) {
       const int as = (int)(it & 1);
@@ -495,62 +494,68 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
       KV_BOUND_MARK(KBW_BITMAP)
       KV_BOUND_PROF(const unsigned int kb_join0 = kbp_t;)
       // ---- rare join, inverted: thread (query, quarter of its rare list) tests each feature in the block's presence
-      //      bitmap; on a hit it probes the block's table (L2) and adds weight x tf to R[chunk][query] for every chunk
-      //      of the mask.  Rows are text-sorted, so one feature can sit in most chunks of a block: R is dense.
-      //      Three phases, each issuing all of its loads before it consumes one (bitmap bits, first-slot keys of the
-      //      hits, masks and weights of the found keys): one or two L2 latencies per thread and block rather than two
-      //      per hit. ----
+      //      bitmap; the warp's hits are then spread over its lanes, 32 per round, and each lane looks its hit up in the
+      //      block's two-choice table (both slots and the weight loaded together: one L2 round trip, hit or miss) and
+      //      adds weight x tf to R[chunk][query] for every chunk of the mask.  Rows are text-sorted, so one feature can
+      //      sit in most chunks of a block: R is dense. ----
       {
         const uint32_t *bm = S.rbm;
         const uint32_t tsize = tsize_n, toff = toff_n;
         if (bk + 1 < blk_hi) { tsize_n = P.rt_size[bk + 1]; toff_n = P.rt_off[bk + 1]; }
-        uint32_t h[NR], key[NR];
+        // the warp's hits, numbered entry-major: the hit of entry k at lane l is number pre_k + popc(ball[k] below l)
+        uint32_t ball[NR], n_hits = 0;
 #pragma unroll
         for (int k = 0; k < NR; k++) {
           const uint32_t bb = rb_bit(fid[k]);
-          const bool hit = fid[k] < FID_NONE && ((bm[bb >> 5] >> (bb & 31u)) & 1u);
-          h[k] = rt_slot(fid[k], tsize);
-          key[k] = hit ? __ldg(P.rt_keys + toff + h[k]) : KEY_EMPTY;
-          KV_BOUND_PROF(kbc_bit += hit;)
+          ball[k] = __ballot_sync(FULL, fid[k] < FID_NONE && ((bm[bb >> 5] >> (bb & 31u)) & 1u));
+          n_hits += __popc(ball[k]);
         }
-        KV_BOUND_MARK(KBW_JOIN1)
+        KV_BOUND_MARK(KBW_JOIN_BITS)
+        KV_BOUND_PROF(kbc_bit += n_hits; kbc_rounds += (n_hits + 31) / 32; kbc_multi += n_hits > 32;)
+        const uint4 *tab = P.rt_slots + toff;
+        for (uint32_t g = (uint32_t)lane; g - (uint32_t)lane < n_hits; g += 32) {  // round: hit g goes to lane g % 32
+          // entry k and source lane of hit g: the last k with pre_k <= g, then the (g - pre_k)-th set bit of ball[k]
+          uint32_t kk = 0, bk_bits = 0, rank = 0, pre = 0;
 #pragma unroll
-        for (int k = 0; k < NR; k++)  // first slot taken by another feature: continue the linear probe
-          while (key[k] != KEY_EMPTY && (key[k] >> 5) != fid[k]) {
-            h[k] = h[k] + 1 == tsize ? 0 : h[k] + 1;
-            key[k] = __ldg(P.rt_keys + toff + h[k]);
-            KV_BOUND_PROF(kbc_cont++;)
-          }
-        KV_BOUND_MARK(KBW_JOIN2)
-        unsigned long long cm[NR];
-        uint32_t tf[NR], w[NR];
-#pragma unroll
-        for (int k = 0; k < NR; k++) {
-          const bool found = key[k] != KEY_EMPTY;
-          cm[k] = found ? __ldg(P.rt_masks + toff + h[k]) : 0ull;
-          w[k] = found ? __ldg(P.q3w + q3o + (size_t)k * 4 * TILE_Q) : 0u;
-          tf[k] = key[k] & 31u;
-          if (found && tf[k] == TF_OVF) tf[k] = __ldg(P.tfmax + fid[k]);
-          KV_BOUND_PROF(kbc_tab += found;)
-        }
-        KV_BOUND_MARK(KBW_JOIN3)
-        KV_BOUND_PROF({
-          unsigned int mine = 0;
-          _Pragma("unroll")
           for (int k = 0; k < NR; k++) {
-            const unsigned int n = (unsigned int)__popcll(cm[k]);
-            mine += n;
-            kbc_fan_entry += __reduce_max_sync(FULL, n);
+            if (g >= pre) { kk = (uint32_t)k; bk_bits = ball[k]; rank = g - pre; }
+            pre += __popc(ball[k]);
           }
-          kbc_bits += mine;
-          kbc_fan_one += __reduce_max_sync(FULL, mine);
-        })
+          const bool has = g < n_hits;
+          uint32_t src = 0;  // binary search for the set bit with `rank` set bits below it (lane 0 for a lane without a hit)
 #pragma unroll
-        for (int k = 0; k < NR; k++) {
-          const uint32_t x = w[k] * tf[k];  // fixed point, <= 2^30 + tf (prep_queries_kernel)
-          for (unsigned long long m = cm[k]; m; m &= m - 1) atomicAdd(&S.R[__ffsll((long long)m) - 1][jq], x);
+          for (uint32_t s = 16; s; s >>= 1) {
+            const uint32_t c = (uint32_t)__popc((bk_bits >> src) & ((1u << s) - 1u));
+            if (rank >= c) { rank -= c; src += s; }
+          }
+          if (!has) src = 0;
+          uint32_t f = FID_NONE;
+#pragma unroll
+          for (int k = 0; k < NR; k++)
+            if (ball[k]) {
+              const uint32_t v = __shfl_sync(FULL, fid[k], src);
+              if (kk == (uint32_t)k) f = v;
+            }
+          const uint32_t jsrc = (uint32_t)(jq & (TILE_Q - 32)) | src;  // the source lane's query
+          KV_BOUND_MARK(KBW_JOIN_COMPACT)
+          uint4 s1 = make_uint4(KEY_EMPTY, 0u, 0u, 0u), s2 = s1;
+          uint32_t w = 0;
+          if (has) {
+            s1 = __ldg(tab + rt_slot1(f, tsize));
+            s2 = __ldg(tab + rt_slot2(f, tsize));
+            w = __ldg(P.q3w + (q3o - (size_t)jq + jsrc) + (size_t)kk * 4 * TILE_Q);
+          }
+          const uint4 s = s1.x == f ? s1 : s2;
+          unsigned long long m = has && s.x == f ? ((unsigned long long)s.w << 32 | s.z) : 0ull;
+          const uint32_t x = w * s.y;  // fixed point, <= 2^30 + tf (prep_queries_kernel)
+          KV_BOUND_MARK(KBW_JOIN_SLOTS)
+          KV_BOUND_PROF({
+            const unsigned int nb = (unsigned int)__popcll(m);
+            kbc_tab += m != 0; kbc_bits += nb; kbc_fan += __reduce_max_sync(FULL, nb);
+          })
+          for (; m; m &= m - 1) atomicAdd(&S.R[__ffsll((long long)m) - 1][jsrc], x);
+          KV_BOUND_MARK(KBW_FANOUT)
         }
-        KV_BOUND_MARK(KBW_FANOUT)
         KV_BOUND_PROF(if (lane == 0) atomicMax(&S.prof_join_max, kbp_t - kb_join0);)
       }
       if (threadIdx.x < B_BN) S.minB[as][threadIdx.x] = P.chunk_minB[c0 + threadIdx.x];
@@ -651,17 +656,18 @@ tfidf_bound_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_const
       KV_BOUND_MARK(KBW_BARRIER)
     }
     KV_BOUND_PROF({
-      kbc_bit = __reduce_add_sync(FULL, kbc_bit); kbc_tab = __reduce_add_sync(FULL, kbc_tab);
-      kbc_cont = __reduce_add_sync(FULL, kbc_cont); kbc_bits = __reduce_add_sync(FULL, kbc_bits);
+      // kbc_bit, kbc_rounds, kbc_multi and kbc_fan are the warp's (lane 0 adds them); the table hits and mask bits are
+      // per lane
+      kbc_tab = __reduce_add_sync(FULL, kbc_tab); kbc_bits = __reduce_add_sync(FULL, kbc_bits);
       if (lane == 0) {
         _Pragma("unroll")
         for (int i = 0; i < KBW_N; i++) atomicAdd(&g_bound_prof[i], (unsigned long long)kbp[i]);
         atomicAdd(&g_bound_prof[KBC_BIT_HITS], (unsigned long long)kbc_bit);
+        atomicAdd(&g_bound_prof[KBC_ROUNDS], (unsigned long long)kbc_rounds);
+        atomicAdd(&g_bound_prof[KBC_MULTI_ROUND], (unsigned long long)kbc_multi);
         atomicAdd(&g_bound_prof[KBC_TABLE_HITS], (unsigned long long)kbc_tab);
-        atomicAdd(&g_bound_prof[KBC_PROBE_CONT], (unsigned long long)kbc_cont);
         atomicAdd(&g_bound_prof[KBC_MASK_BITS], (unsigned long long)kbc_bits);
-        atomicAdd(&g_bound_prof[KBC_FAN_PER_ENTRY], (unsigned long long)kbc_fan_entry);
-        atomicAdd(&g_bound_prof[KBC_FAN_ONE_LOOP], (unsigned long long)kbc_fan_one);
+        atomicAdd(&g_bound_prof[KBC_FAN_ITERS], (unsigned long long)kbc_fan);
         atomicAdd(&g_bound_prof[KBC_WORKER_WARP_BLOCKS], (unsigned long long)it);
       }
       if (threadIdx.x == 0) {

@@ -70,13 +70,14 @@ struct kv_index {
   DevBuf<__half> d_Uf;
   DevBuf<short> d_fslot;
   DevBuf<unsigned short> d_fslot2;
-  DevBuf<uint32_t> d_ubt, d_rbloom, d_rt_keys, d_rt_off, d_rt_size;
-  DevBuf<unsigned long long> d_rt_masks;
+  DevBuf<uint32_t> d_ubt, d_rbloom, d_rt_off, d_rt_size;
+  DevBuf<uint4> d_rt_slots;
   CUtensorMap map_u;
   DevBuf<unsigned long long> d_ovf_keys;
   DevBuf<uint32_t> d_ovf_vals;
   int n_ovf = 0;
   int64_t n_rt_slots = 0;  // slots of all blocks' rare tables
+  int64_t rt_enlarged = 0;  // of those tables, the ones whose cuckoo insertion needed more than the initial size
   int64_t blk_words = 0, n_chunks = 0, n_chunks_pad = 0, n_entries = 0, n_rare_entries = 0;
   std::vector<uint32_t> h_df, h_tfmax;
   std::vector<short> h_fslot;
@@ -272,7 +273,7 @@ void sort_rows_by_text(const std::vector<int64_t> &indptr, const std::vector<uin
 struct LayoutHeader {
   uint64_t magic, checksum;
   int64_t n_rows, nnz, V, n_chunks, n_chunks_pad, blk_words, n_entries, n_rare_entries, n_ovf, n_rt_slots, n_blocks, univ_len;
-  int32_t jaccard, corpus_fit, threads, reserved;
+  int32_t jaccard, corpus_fit, threads, rt_enlarged;
 };
 
 struct ScanLayout {
@@ -284,8 +285,9 @@ struct ScanLayout {
   std::vector<BlockInfo> binfo;
   std::vector<uint32_t> blk;
   std::vector<__half> uf;
-  std::vector<uint32_t> ubt, rbloom, rt_off, rt_size, rt_keys;
-  std::vector<unsigned long long> rt_masks, ovf_keys;
+  std::vector<uint32_t> ubt, rbloom, rt_off, rt_size;
+  std::vector<uint4> rt_slots;
+  std::vector<unsigned long long> ovf_keys;
   std::vector<uint32_t> ovf_vals;
 };
 
@@ -298,7 +300,7 @@ bool each_array(SL &L, kv_index *ix, F &&f) {
   return f(L.fslot, ix->d_fslot, V) && f(L.fslot2, ix->d_fslot2, V) && f(L.perm, ix->d_perm, (size_t)H.n_rows) &&
          f(L.binfo, ix->d_binfo, pad) && f(L.blk, ix->d_blk, (size_t)H.blk_words) && f(L.uf, ix->d_Uf, pad * NF) &&
          f(L.ubt, ix->d_ubt, nb * NF2 * 4) && f(L.rbloom, ix->d_rbloom, nb * (RB_BITS / 32)) && f(L.rt_off, ix->d_rt_off, nb) &&
-         f(L.rt_size, ix->d_rt_size, nb) && f(L.rt_keys, ix->d_rt_keys, slots) && f(L.rt_masks, ix->d_rt_masks, slots) &&
+         f(L.rt_size, ix->d_rt_size, nb) && f(L.rt_slots, ix->d_rt_slots, slots) &&
          f(L.ovf_keys, ix->d_ovf_keys, n_ovf) && f(L.ovf_vals, ix->d_ovf_vals, n_ovf);
 }
 
@@ -327,6 +329,7 @@ int upload_layout(kv_index *ix, const ScanLayout &L) {
   ix->h_fslot = L.fslot; ix->h_fslot2 = L.fslot2;
   ix->n_chunks = H.n_chunks; ix->n_chunks_pad = H.n_chunks_pad; ix->blk_words = H.blk_words; ix->n_entries = H.n_entries;
   ix->n_rare_entries = H.n_rare_entries; ix->n_ovf = (int)H.n_ovf; ix->n_rt_slots = H.n_rt_slots;
+  ix->rt_enlarged = H.rt_enlarged;
   ix->layout_valid = H.n_rows > 0; ix->layout_rows = H.n_rows; ix->layout_univ = L.univ;
   return KV_OK;
 }
@@ -831,15 +834,15 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
   {
     BlockLayout L;
     build_blocks(ix->h_indptr.data(), ix->h_ids.data(), ix->h_tf.data(), SL.perm.data(), n, V, ix->h_univ.data(),
-                 ix->h_tfmax.data(), host_threads(), L);
+                 ix->h_tfmax.data(), host_threads(), L, /*linear_tables=*/false);
     LayoutHeader &H = SL.H;
     H.n_rows = n; H.V = Vz; H.n_chunks = L.n_chunks; H.n_chunks_pad = L.n_chunks_pad; H.n_blocks = L.n_chunks_pad / 64;
     H.blk_words = L.total_words; H.n_entries = L.n_entries; H.n_rare_entries = L.n_rare_entries;
-    H.n_rt_slots = (int64_t)L.rt_keys.size(); H.n_ovf = (int64_t)L.ovf.size(); H.univ_len = Vz;
+    H.n_rt_slots = (int64_t)L.rt_slots.size(); H.rt_enlarged = (int32_t)L.rt_enlarged; H.n_ovf = (int64_t)L.ovf.size(); H.univ_len = Vz;
     SL.univ = ix->h_univ;
     SL.fslot = std::move(L.fslot); SL.fslot2 = std::move(L.fslot2); SL.binfo = std::move(L.binfo); SL.uf = std::move(L.Uf);
     SL.ubt = std::move(L.Ubt); SL.rbloom = std::move(L.rbloom); SL.rt_off = std::move(L.rt_off); SL.rt_size = std::move(L.rt_size);
-    SL.rt_keys = std::move(L.rt_keys); SL.rt_masks = std::move(L.rt_masks);
+    SL.rt_slots = std::move(L.rt_slots);
     SL.blk.reserve((size_t)L.total_words);
     for (auto &part : L.parts) {  // the blocks of each build thread, back to back
       SL.blk.insert(SL.blk.end(), part.begin(), part.end());
@@ -1504,8 +1507,7 @@ static int run_pruned(kv_index *ix, Batch &b) {
   BP.blk = ix->d_blk.p; BP.binfo = ix->d_binfo.p; BP.chunk_minB = ix->d_cminB.p;
   BP.ovf_keys = ix->d_ovf_keys.p; BP.ovf_vals = ix->d_ovf_vals.p; BP.n_ovf = ix->n_ovf;
   BP.n_chunks = ix->n_chunks; BP.n_q = n_q; BP.q3id = ix->d_q3id.p; BP.q3w = ix->d_q3w.p; BP.d2col = ix->d_d2col.p; BP.q2list = ix->d_q2list.p; BP.ubt = ix->d_ubt.p;
-  BP.rbloom = ix->d_rbloom.p; BP.rt_keys = ix->d_rt_keys.p; BP.rt_masks = ix->d_rt_masks.p; BP.rt_off = ix->d_rt_off.p;
-  BP.rt_size = ix->d_rt_size.p; BP.tfmax = ix->d_tfmax.p;
+  BP.rbloom = ix->d_rbloom.p; BP.rt_slots = ix->d_rt_slots.p; BP.rt_off = ix->d_rt_off.p; BP.rt_size = ix->d_rt_size.p;
   BP.q_nq = qc; BP.q_dotS = qc + 3 * n_q; BP.q_corrS = qc + 4 * n_q; BP.q_dotX = qc + 5 * n_q; BP.q_rscale = qc + 6 * n_q;
   BP.gthr = b.range ? ix->d_rthr.p : ix->d_gthr.p; BP.n_bsplits = (int)b.n_bsplits; BP.seeds = ix->d_seeds.p;
   BP.lists.count = ix->d_list_count.p + b.n_groups; BP.lists.pages = ix->d_list_pages.p; BP.lists.max_pages = b.max_pages;
@@ -2488,12 +2490,12 @@ int kv_index_last_score_ms(const kv_index *ix, float *ms) {
   return KV_OK;
 }
 
-int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[18]) {
+int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[20]) {
   if (!ix || !bytes || !counts) return kv_fail(KV_ERR_INVALID, "kv_index_layout: bad arguments");
   bytes[0] = ix->blk_words * 4;
   bytes[1] = ix->n_rows * 4;
   bytes[2] = ix->n_chunks_pad * (int64_t)sizeof(BlockInfo);
-  const int64_t rare_table_bytes = ix->n_rt_slots * 12 + (ix->n_chunks_pad / 64) * (RB_BITS / 8);
+  const int64_t rare_table_bytes = ix->n_rt_slots * (int64_t)sizeof(uint4) + (ix->n_chunks_pad / 64) * (RB_BITS / 8);
   bytes[3] = ix->n_chunks_pad * (int64_t)(NF * sizeof(__half) + sizeof(float)) + rare_table_bytes + (ix->n_chunks_pad / 64) * (int64_t)(NF2 * 16);
   counts[0] = ix->n_entries; counts[1] = ix->n_univ; counts[2] = ix->n_rows;
   counts[3] = ix->last_ctas; counts[4] = ix->last_tiles; counts[5] = ix->last_splits;
@@ -2508,6 +2510,8 @@ int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[18]) {
   counts[15] = (int64_t)(ix->last_stats[6] & 0xFFFFFFFFull);  // pool pages used
   counts[16] = ix->pool_pages;
   counts[17] = ix->batch_f2_outside;  // second-class (query, feature) listings of the batch left out of their tile's dictionary
+  counts[18] = ix->n_rt_slots;
+  counts[19] = ix->rt_enlarged;
   return KV_OK;
 }
 
@@ -2522,7 +2526,7 @@ int kv_index_layout(const kv_index *ix, int64_t bytes[4], int64_t counts[18]) {
 // the statistics-only path (kv_index_last_finalize_kind == 2).
 // ----------------------------------------------------------------------------------------
 namespace {
-constexpr uint64_t LAYOUT_MAGIC = 0x32594C42564B4B41ULL;  // "AKKVBLY2"
+constexpr uint64_t LAYOUT_MAGIC = 0x33594C42564B4B41ULL;  // "AKKVBLY3"
 
 uint64_t csr_checksum(const kv_index *ix) {
   const int T = host_threads();
@@ -2560,7 +2564,7 @@ extern "C" int kv_index_layout_save(kv_index *ix, const char *path) {
   H.magic = LAYOUT_MAGIC; H.checksum = csr_checksum(ix);
   H.n_rows = ix->n_rows; H.nnz = ix->nnz; H.V = (int64_t)ix->h_fslot.size(); H.n_chunks = ix->n_chunks; H.n_chunks_pad = ix->n_chunks_pad;
   H.blk_words = ix->blk_words; H.n_entries = ix->n_entries; H.n_rare_entries = ix->n_rare_entries; H.n_ovf = ix->n_ovf;
-  H.n_rt_slots = ix->n_rt_slots; H.n_blocks = ix->n_chunks_pad / 64; H.univ_len = (int64_t)ix->layout_univ.size();
+  H.n_rt_slots = ix->n_rt_slots; H.rt_enlarged = (int32_t)ix->rt_enlarged; H.n_blocks = ix->n_chunks_pad / 64; H.univ_len = (int64_t)ix->layout_univ.size();
   H.jaccard = ix->jaccard; H.corpus_fit = ix->corpus_fit;
   cudaError_t err = cudaSuccess;
   each_array(SL, ix, [&](auto &h, auto &d, size_t n) {

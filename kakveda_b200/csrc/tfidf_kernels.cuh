@@ -559,9 +559,16 @@ __global__ void __launch_bounds__(DICT_THREADS) f2_dict_kernel(DictParams P) {
 }
 
 __host__ __device__ __forceinline__ uint32_t rb_bit(uint32_t fid) { return (fid * 0x85EBCA6Bu) >> 16; }  // 16 bits: RB_BITS
-// slot of a feature in a block's rare table of `size` slots (fast range reduction of a multiplicative hash)
+// slot of a feature in a table of `size` slots (fast range reduction of a multiplicative hash): the first slot of the
+// linear-probing tables build_blocks writes on request, and the first of a feature's two slots in a block's rare table
 __host__ __device__ __forceinline__ uint32_t rt_slot(uint32_t fid, uint32_t size) {
   return (uint32_t)(((unsigned long long)(fid * 0x9E3779B1u) * (unsigned long long)size) >> 32);
+}
+__host__ __device__ __forceinline__ uint32_t rt_slot1(uint32_t fid, uint32_t size) { return rt_slot(fid, size); }
+// the second slot: an independent multiplier.  A slot of a block's rare table is one uint4 {feature id (KEY_EMPTY: free),
+// tf, chunk mask low, high}: tf = the feature's largest tf in the block, or tfmax[feature] when that reaches TF_OVF.
+__host__ __device__ __forceinline__ uint32_t rt_slot2(uint32_t fid, uint32_t size) {
+  return (uint32_t)(((unsigned long long)(fid * 0xC2B2AE35u) * (unsigned long long)size) >> 32);
 }
 
 // ----------------------------------------------------------------------------------------

@@ -22,13 +22,12 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 
-WORKER_SPANS = ["wait for the block's rare bitmap", "join 1: bit tests, key loads issued", "join 2: keys arrive, probe continuations",
-                "join 3: masks, weights, tfmax", "join: fan-out into R", "wait for R complete (RFULL)", "R read-out",
+WORKER_SPANS = ["wait for the block's rare bitmap", "join: bit tests + ballots", "join: hit numbering + shuffles (per round)",
+                "join: slot + weight loads (per round)", "join: fan-out into R (per round)", "wait for R complete (RFULL)", "R read-out",
                 "second-class features left out of the dictionary", "bound, codes, seeds", "code store / list append",
                 "RCLEAN arrive + WORKERS barrier"]
 MMA_SPANS = ["chunk-slice waits + GEMM", "wait for R clean (RCLEAN)", "adds into R", "B2 build"]
-COUNTERS = ["bit_hits", "table_hits", "probe_continuations", "mask_bits", "fan_iters_loop_per_entry", "fan_iters_one_loop",
-            "join_slowest_warp_cycles", "mma_last_blocks", "mma_last_cycles", "workers_last_cycles", "worker_warp_blocks",
+COUNTERS = ["bit_hits", "rounds", "multi_round_warp_blocks", "table_hits", "mask_bits", "fan_iters", "join_slowest_warp_cycles", "mma_last_blocks", "mma_last_cycles", "workers_last_cycles", "worker_warp_blocks",
             "mma_warp_blocks", "cta_blocks", "ctas"]
 MAX_CTAS = 4096
 N_SLOTS = len(WORKER_SPANS) + len(MMA_SPANS) + len(COUNTERS) + 2 * MAX_CTAS
@@ -106,10 +105,9 @@ def child(variant: str, n: int, q: int, k: int) -> None:
     print(f"  MMA warpgroup: {'total':44s} {mspans.sum() / mb:8.0f}")
     tb = wb * 32  # (worker thread, block)
     print(f"[clocks] rare join per (thread, block), 8 list entries each: bitmap hits {c['bit_hits'] / tb:.3f}, table hits "
-          f"{c['table_hits'] / tb:.3f}, probe continuations {c['probe_continuations'] / tb:.3f}, hit-mask bits (adds into R) "
-          f"{c['mask_bits'] / tb:.3f}")
-    print(f"[clocks] fan-out iterations per (warp, block): one loop per list entry {c['fan_iters_loop_per_entry'] / wb:.2f}, "
-          f"one loop per thread {c['fan_iters_one_loop'] / wb:.2f}, the lanes' mean {c['mask_bits'] / tb:.2f}")
+          f"{c['table_hits'] / tb:.3f}, hit-mask bits (adds into R) {c['mask_bits'] / tb:.3f}")
+    print(f"[clocks] per (warp, block): lookups {c['bit_hits'] / wb:.2f}, rounds {c['rounds'] / wb:.3f}, share needing a second "
+          f"round {100 * c['multi_round_warp_blocks'] / wb:.2f} %, fan-out iterations {c['fan_iters'] / wb:.2f}")
     ml = c["mma_last_blocks"]
     print(f"[clocks] last at RFULL: the MMA warpgroup in {100 * ml / cb:.1f} % of the blocks (by {c['mma_last_cycles'] / max(ml, 1):.0f} "
           f"cycles), the slowest worker warp in the rest (by {c['workers_last_cycles'] / max(cb - ml, 1):.0f} cycles)")
