@@ -349,6 +349,9 @@ int kv_rescore_pairs(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_id
  * again after uploading a batch larger than `capacity` (kv_topk* returns KV_ERR_STATE otherwise). */
 int kv_index_thresholds_export(kv_index *ix, int64_t capacity, void *handle_out);
 int kv_index_thresholds_peers(kv_index *ix, const void *handles, int n_peers, int64_t capacity);
+/* Test hook: what kv_index_thresholds_peers does, for indexes of one process on one device (no CUDA IPC): ix pushes
+ * into the threshold arrays of `peers`, each exported before with at least `capacity` queries.  n_peers = 0 unlinks. */
+int kv_debug_thresholds_link(kv_index *ix, kv_index *const *peers, int n_peers, int64_t capacity);
 
 /* K5: merge n_lists partial top-k lists per query (device pointers; list l of query q at
  * [l*n_q*k + q*k], each sorted by (score desc,row asc)) into one [n_q*k] result with the

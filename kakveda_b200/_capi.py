@@ -95,6 +95,7 @@ SIGNATURES = {
                                        C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "kv_index_thresholds_export": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p]),
     "kv_index_thresholds_peers": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64]),
+    "kv_debug_thresholds_link": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int64]),
     "kv_merge_topk_device": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_void_p,
                                        C.c_void_p]),
     "kv_merge_topk_device_on": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int64,

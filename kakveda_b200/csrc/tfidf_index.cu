@@ -105,6 +105,7 @@ struct kv_index {
   DevBuf<int> d_qperm;
   DevBuf<uint8_t> d_flags;
   DevBuf<float> d_qconst;     // 7 * n_q: nq, dotU, corrU, dotS, corrS, dotX, 1 / s_q (fixed-point unit of the bound kernel's R)
+  DevBuf<unsigned long long> d_qfix;  // 2 * n_q: the universal features' fixed-point sums U_w, U_c (what the scan adds)
   DevBuf<unsigned char> d_qtab;
   DevBuf<uint2> d_q2list;
   DevBuf<uint32_t> d_q3id, d_q3w, d_d2col;  // rare lists (feature, weight); second-class dictionary of each tile
@@ -126,6 +127,7 @@ struct kv_index {
   int n_peers = 0;
   int *peer_gthr[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   int64_t peer_cap = 0;  // queries the exchanged arrays hold
+  bool peers_borrowed = false;  // peer_gthr points at other handles' arrays in this process (kv_debug_thresholds_link)
   DevBuf<int> d_excl_sorted, d_excl_orig;  // self-join exclusions of the resident batch (by sorted slot / by original query)
   std::vector<int> h_excl_orig;
   bool has_excl = false;
@@ -194,11 +196,13 @@ struct kv_index {
 };
 
 static void close_peers(kv_index *ix) {
-  for (int i = 0; i < ix->n_peers; i++)
-    if (ix->peer_gthr[i]) cudaIpcCloseMemHandle(ix->peer_gthr[i]);
+  if (!ix->peers_borrowed)
+    for (int i = 0; i < ix->n_peers; i++)
+      if (ix->peer_gthr[i]) cudaIpcCloseMemHandle(ix->peer_gthr[i]);
   for (auto &p : ix->peer_gthr) p = nullptr;
   ix->n_peers = 0;
   ix->peer_cap = 0;
+  ix->peers_borrowed = false;
 }
 
 namespace {
@@ -974,7 +978,11 @@ struct QueryRun {
 
 // null: no feature of the query is in the index (every score is 0).  irregular: more features than a query table
 // holds, or term frequencies so large that the 64-bit fixed-point sums or the fp16 bound weights could overflow --
-// such a query takes the float64 full-scan path (K1a + selection).
+// such a query takes the float64 full-scan path (K1a + selection).  The scan's sums, universal features included
+// (their common tf u stands in for tfmax; prep_queries_kernel folds them as the integers their entries would add):
+// a row's dot sum adds tf_c round(tf_q a 2^32) <= tfmax (tf_q a 2^32 + 1) per feature, below 2^32 amax s_dot + s_dot
+// < 2^62 + 2^30; its correction sum adds tf_c^2 round(-d 2^24) with -d = (idf_b - idf_q)(idf_b + idf_q) < ln 2 x
+// 2 sqrt(amax) < 32, below 2^29 s_corr + s_corr < 2^54.  Both fit 64 bits.
 static void classify_queries(const kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
                              int64_t n_q, uint8_t *flag, int T) {
   const double amax = ix->jaccard ? 1.0 : std::pow(std::log((double)(ix->n_total + 2)) + 1.0, 2.0);
@@ -988,7 +996,12 @@ static void classify_queries(const kv_index *ix, const int64_t *q_indptr, const 
         if ((int64_t)t >= ix->V) continue;
         if (ix->corpus_fit && ix->h_df[t] == 0) continue;  // in no live row: ignored like an out-of-vocabulary feature
         known = true;
-        if (ix->h_univ[t]) continue;
+        if (ix->h_univ[t]) {  // folded into the query's constants, but summed in fixed point like the other terms
+          const double u = (double)ix->h_utf[t], f = (double)q_tf[p];
+          s_dot += f * u;
+          s_corr += u * u;
+          continue;
+        }
         feats++;
         const double tm = (double)ix->h_tfmax[t], f = (double)q_tf[p];
         s_dot += f * tm;
@@ -1181,6 +1194,7 @@ static int build_query_tables(kv_index *ix, int64_t n_q) {
   cudaStream_t s = ix->stream;
   const int64_t n_tiles = (n_q + TILE_Q - 1) / TILE_Q, n_q_pad = n_tiles * TILE_Q;
   KV_CUDA(ix->d_qconst.ensure(7 * n_q));
+  KV_CUDA(ix->d_qfix.ensure(2 * n_q));
   KV_CUDA(ix->d_qtab.ensure(n_q * (int64_t)QTAB_BYTES));
   KV_CUDA(ix->d_Wf.ensure(n_q_pad * NF));
   KV_CUDA(ix->d_q2list.ensure(n_q_pad * Q2CAP));
@@ -1205,6 +1219,7 @@ static int build_query_tables(kv_index *ix, int64_t n_q) {
   P.fslot = ix->d_fslot.p; P.fslot2 = ix->d_fslot2.p; P.q2list = ix->d_q2list.p; P.jaccard = ix->jaccard; P.corpus_fit = ix->corpus_fit;
   P.q_nq = ix->d_qconst.p; P.q_dotU = P.q_nq + n_q; P.q_corrU = P.q_nq + 2 * n_q; P.q_dotS = P.q_nq + 3 * n_q;
   P.q_corrS = P.q_nq + 4 * n_q; P.q_dotX = P.q_nq + 5 * n_q; P.q_rscale = P.q_nq + 6 * n_q;
+  P.q_uw = ix->d_qfix.p; P.q_uc = ix->d_qfix.p + n_q;
   P.qtab = ix->d_qtab.p; P.Wf = ix->d_Wf.p; P.q3id = ix->d_q3id.p; P.q3w = ix->d_q3w.p;
   prep_queries_kernel<<<(unsigned)((n_q + 127) / 128), 128, 0, s>>>(P);
   KV_CUDA(cudaGetLastError());
@@ -1237,8 +1252,8 @@ inline unsigned tq_grid(int64_t n) { return (unsigned)std::max<int64_t>(1, (n + 
 // classify_queries on the device, one thread per query, the same float64 operations in the same order (no contraction)
 __global__ void __launch_bounds__(TQ_THREADS) classify_kernel(const int64_t *indptr, const uint32_t *ids, const uint32_t *tf,
                                                               int64_t n_q, int64_t V, int corpus_fit, const uint32_t *df,
-                                                              const uint8_t *univ, const uint32_t *tfmax, double amax,
-                                                              uint8_t *flag) {
+                                                              const uint8_t *univ, const uint32_t *utf, const uint32_t *tfmax,
+                                                              double amax, uint8_t *flag) {
   const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_q) return;
   bool known = false;
@@ -1249,7 +1264,12 @@ __global__ void __launch_bounds__(TQ_THREADS) classify_kernel(const int64_t *ind
     if ((int64_t)t >= V) continue;
     if (corpus_fit && df[t] == 0) continue;
     known = true;
-    if (univ[t]) continue;
+    if (univ[t]) {
+      const double u = (double)utf[t], f = (double)tf[p];
+      s_dot = __dadd_rn(s_dot, __dmul_rn(f, u));
+      s_corr = __dadd_rn(s_corr, __dmul_rn(u, u));
+      continue;
+    }
     feats++;
     const double tm = (double)tfmax[t], f = (double)tf[p];
     s_dot = __dadd_rn(s_dot, __dmul_rn(f, tm));
@@ -1353,7 +1373,7 @@ static int prepare_batch_text(kv_index *ix, kv_vocab_mirror *m, const kv_vocab *
   const double amax = ix->jaccard ? 1.0 : std::pow(std::log((double)(ix->n_total + 2)) + 1.0, 2.0);
   KV_CUDA(cudaEventRecord(ix->evq[0], s));
   classify_kernel<<<tq_grid(n_q), TQ_THREADS, 0, s>>>(ix->d_q_indptr.p, ix->d_q_ids.p, ix->d_q_tf.p, n_q, ix->V, ix->corpus_fit,
-                                                     ix->d_df.p, ix->d_univ.p, ix->d_tfmax.p, amax, ix->d_qflag_row.p);
+                                                     ix->d_df.p, ix->d_univ.p, ix->d_utf.p, ix->d_tfmax.p, amax, ix->d_qflag_row.p);
   KV_CUDA(cudaGetLastError());
   KV_CUDA(cudaEventRecord(ix->evq[1], s));
   int *cur = ix->d_qorder.p, *other = cur + n_q;
@@ -1459,7 +1479,7 @@ static ScanParams scan_params(const kv_index *ix, const Batch &b) {
   SP.blk = ix->d_blk.p; SP.binfo = ix->d_binfo.p; SP.B32 = ix->d_B32.p; SP.perm = ix->d_perm.p;
   SP.n_chunks = ix->n_chunks; SP.n_rows = ix->n_rows; SP.row_base = ix->row_base;
   SP.ovf_keys = ix->d_ovf_keys.p; SP.ovf_vals = ix->d_ovf_vals.p; SP.n_ovf = ix->n_ovf;
-  SP.qtab = ix->d_qtab.p; SP.q_nq = qc; SP.q_dotU = qc + b.n_q; SP.q_corrU = qc + 2 * b.n_q;
+  SP.qtab = ix->d_qtab.p; SP.q_nq = qc; SP.q_uw = ix->d_qfix.p; SP.q_uc = ix->d_qfix.p + b.n_q;
   SP.q_excl = ix->has_excl ? ix->d_excl_sorted.p : nullptr; SP.gthr = b.range ? ix->d_rthr.p : ix->d_gthr.p;
   if (ix->has_filter) { SP.q_label = ix->d_filt_sorted.p; SP.label_pos = ix->d_label_pos.p; SP.chunk_sig = ix->d_chunk_sig.p; }
   SP.alive = alive_words(ix);
@@ -2315,6 +2335,27 @@ int kv_index_thresholds_peers(kv_index *ix, const void *handles, int n_peers, in
   }
   ix->n_peers = n_peers;
   ix->peer_cap = capacity;
+  return KV_OK;
+}
+
+// Test hook: the peer threshold pushes of kv_index_thresholds_peers between indexes of ONE process on one device, without
+// CUDA IPC.  Every peer must already hold a threshold array of `capacity` queries (kv_index_thresholds_export); the
+// arrays are borrowed, so unmapping never closes an IPC mapping.  n_peers = 0 unlinks.
+int kv_debug_thresholds_link(kv_index *ix, kv_index *const *peers, int n_peers, int64_t capacity) {
+  if (!ix || n_peers < 0 || n_peers > 7 || (n_peers > 0 && (!peers || capacity < 1)))
+    return kv_fail(KV_ERR_INVALID, "kv_debug_thresholds_link: bad arguments (at most 7 peers)");
+  std::lock_guard<std::mutex> g(ix->mu);
+  KV_CUDA(cudaSetDevice(ix->device));
+  KV_CUDA(cudaStreamSynchronize(ix->stream));
+  close_peers(ix);
+  for (int i = 0; i < n_peers; i++) {
+    if (!peers[i] || peers[i] == ix || peers[i]->device != ix->device || peers[i]->d_gthr.cap < capacity)
+      return kv_fail(KV_ERR_INVALID, "kv_debug_thresholds_link: peer %d is not another exported index on this device", i);
+    ix->peer_gthr[i] = peers[i]->d_gthr.p;
+  }
+  ix->n_peers = n_peers;
+  ix->peer_cap = n_peers ? capacity : 0;
+  ix->peers_borrowed = n_peers > 0;
   return KV_OK;
 }
 

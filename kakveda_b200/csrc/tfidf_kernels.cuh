@@ -17,20 +17,23 @@
 //   * rows are sorted by (norm class, feature-id sequence = token order): rows with similar text are neighbours;
 //     perm[position] is the original row; a CHUNK is 32 consecutive positions (one row per lane);
 //   * features present in EVERY local row with one common tf ("universal": the field names of signature_text,
-//     fingerprint.py:60-65) are folded into per-query constants;
+//     fingerprint.py:60-65) are folded into per-query constants -- in fixed point, the exact integers the unfolded
+//     entries would add (see below);
 //   * per chunk one feature-major COLUMN BLOCK: the distinct (feature, tf) pairs of its rows, each with the 32-bit
 //     mask of the rows that hold it:  words[E] = [31] every valid row holds it  [30:5] feature id  [4:0] tf (31 =
 //     see overflow table), masks[E].  A query is scored against a chunk by probing the E words in its own hash table
 //     and adding each hit's weight to the rows of its mask -- a third of the entries a row-major stream needs, and
 //     the per-row sums are INTEGERS (fixed point, see below), so the order of the additions is irrelevant: rows
-//     with identical text get identical bits wherever they sit, and the (score desc, row asc) order of
-//     services/gfkb/app.py:89 is reproduced for duplicate rows;
+//     with identical text get identical bits wherever they sit -- in any row shard too, whichever features its index
+//     folds, since a folded feature adds the same integer as its entries would -- and the (score desc, row asc) order
+//     of services/gfkb/app.py:89 is reproduced for duplicate rows;
 //   * entries of the NF = 256 features found in most chunks ("frequent") come last in a block; for them a dense
 //     fp16 matrix Uf[chunk][256] holds the largest tf in the chunk -- the tensor-core part of the chunk bounds;
 //   * B32/B64: row norms B_c by position, chunk_minB: smallest positive norm of a chunk.
 //
 // Fixed point: a query's weights are w(t) = round(tf_q a(t) 2^32) (64-bit) and c(t) = round(-d(t) 2^24); a row's sums
-// are exact integer sums of tf_c w(t) and tf_c^2 c(t).  Relative resolution 2^-32 per term (float32 has 2^-24).
+// are exact integer sums of tf_c w(t) and tf_c^2 c(t), the universal features' u w(t) and u^2 c(t) included (u: their
+// common tf).  Relative resolution 2^-32 per term (float32 has 2^-24).
 #pragma once
 #include "kv_cuda.cuh"
 #include "sm90.cuh"
@@ -378,6 +381,7 @@ struct PrepParams {
   const unsigned short *fslot2;  // feature -> bit row of the block bitmaps (second class), 0xFFFF: none
   int jaccard, corpus_fit;
   float *q_nq, *q_dotU, *q_corrU, *q_dotS, *q_corrS, *q_dotX;  // [n_q] by sorted slot
+  unsigned long long *q_uw, *q_uc;  // [n_q] universal features in fixed point: sum u w(t), sum u^2 c(t) (the scan's constants)
   float *q_rscale;          // [n_q] 1 / s_q: fixed-point unit of the bound kernel's accumulator R (see below)
   unsigned char *qtab;      // [n_q][QTAB_BYTES]
   __half *Wf;               // [n_q_pad][NF], zeroed by the caller
@@ -395,6 +399,7 @@ __global__ void prep_queries_kernel(PrepParams P) {
   const double idf0 = P.jaccard ? 1.0 : (P.corpus_fit ? 0.0 : log((double)(P.n_total + 2) / 2.0) + 1.0);
   double nq = (P.q_oov ? P.q_oov[q] : 0.0) * idf0 * idf0;
   double dotU = 0.0, corrU = 0.0, corrS = 0.0;
+  unsigned long long uw = 0, uc = 0;
   int cnt = 0, c2 = 0;
   const bool regular = P.flags[i] == 0;
   uint2 *q2 = P.q2list + ((size_t)(i / TILE_Q) * Q2CAP) * TILE_Q + (i % TILE_Q);
@@ -416,6 +421,10 @@ __global__ void prep_queries_kernel(PrepParams P) {
       const double u = (double)P.utf[t];
       dotU += f * u * a;
       corrU += u * u * d;
+      // exactly what the feature's entries would add to the scan's integer sums (the weights are formed as below)
+      const unsigned long long ut = P.utf[t];
+      uw += (unsigned long long)__double2ll_rn(f * a * 4294967296.0) * ut;
+      uc += (unsigned long long)(uint32_t)__double2ll_rn(-d * 16777216.0) * ut * ut;
     } else if (regular && cnt < QFEATS) {
       const double tm = (double)P.tfmax[t];
       corrS += tm * tm * d;
@@ -475,6 +484,8 @@ __global__ void prep_queries_kernel(PrepParams P) {
   P.q_nq[i] = regular ? (float)nq : 0.f;  // nq == 0 switches the query off in the kernels
   P.q_dotU[i] = (float)dotU;
   P.q_corrU[i] = (float)corrU;
+  P.q_uw[i] = uw;
+  P.q_uc[i] = uc;
   P.q_dotS[i] = __double2float_ru(dotU * (1.0 + 1e-6));  // bounds may only err upwards
   P.q_corrS[i] = __double2float_rd(corrU + corrS);       // ... and their denominators downwards
   P.q_dotX[i] = dotX;
@@ -595,7 +606,8 @@ struct ScanParams {
   const uint32_t *ovf_vals;
   int n_ovf;
   const unsigned char *qtab;              // [n_q][QTAB_BYTES]
-  const float *q_nq, *q_dotU, *q_corrU;   // [n_q] (sorted query order)
+  const float *q_nq;                      // [n_q] (sorted query order)
+  const unsigned long long *q_uw, *q_uc;  // [n_q] universal features' fixed-point sums (prep_queries_kernel)
   const int *q_excl;                      // [n_q] or NULL: local ORIGINAL row a query must not match (self-join), -1 = none
   // label filter (kv_query_set_filter); q_label NULL: the batch has none and the other two are not read
   const int *q_label;                     // [n_q] label a query's rows must carry, -1 = any
@@ -698,13 +710,13 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   unsigned char *s_buf = (unsigned char *)(s_feats + GROUP_Q * QFEATS);     // [S_WARPS][2][S_BUF_BYTES]
   uint64_t *s_bar = (uint64_t *)(s_buf + S_WARPS * 2 * S_BUF_BYTES);        // [S_WARPS][2]
   unsigned long long *s_kth = (unsigned long long *)(s_bar + S_WARPS * 2);  // [GROUP_Q] k-th entry of a full list
-  float *s_lscore = (float *)(s_kth + GROUP_Q);                             // [GROUP_Q][k]
+  unsigned long long *s_uw = s_kth + GROUP_Q, *s_uc = s_uw + GROUP_Q;       // [GROUP_Q] per-query fixed-point constants
+  float *s_lscore = (float *)(s_uc + GROUP_Q);                              // [GROUP_Q][k]
   int *s_lrow = (int *)(s_lscore + GROUP_Q * k);                            // [GROUP_Q][k]
   int *s_cnt = s_lrow + GROUP_Q * k;                                        // [GROUP_Q]
   int *s_lock = s_cnt + GROUP_Q;                                            // [GROUP_Q]
   float *s_nq = (float *)(s_lock + GROUP_Q);                                // [GROUP_Q] per-query constants
-  float *s_dotU = s_nq + GROUP_Q, *s_corrU = s_dotU + GROUP_Q;
-  int *s_excl = (int *)(s_corrU + GROUP_Q);
+  int *s_excl = (int *)(s_nq + GROUP_Q);
   int *s_qlab = s_excl + GROUP_Q;                                           // [GROUP_Q] label filter, -1 = any
   unsigned int *s_next = (unsigned int *)(s_qlab + GROUP_Q);                // [1] next record of this CTA's range
   unsigned int *s_stat = s_next + 1;                                        // [4]
@@ -754,8 +766,8 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
       s_cnt[qi] = 0;
       s_lock[qi] = 0;
       s_nq[qi] = ok ? P.q_nq[q0 + qi] : 0.f;
-      s_dotU[qi] = ok ? P.q_dotU[q0 + qi] : 0.f;
-      s_corrU[qi] = ok ? P.q_corrU[q0 + qi] : 0.f;
+      s_uw[qi] = ok ? P.q_uw[q0 + qi] : 0ull;
+      s_uc[qi] = ok ? P.q_uc[q0 + qi] : 0ull;
       s_excl[qi] = (ok && P.q_excl) ? P.q_excl[q0 + qi] : -1;
       s_qlab[qi] = (ok && P.q_label) ? P.q_label[q0 + qi] : -1;
     }
@@ -1019,16 +1031,16 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
           all_w += __shfl_xor_sync(FULL, all_w, o);
           all_c += __shfl_xor_sync(FULL, all_c, o);
         }
-        acc_w += all_w;
-        acc_c += all_c;
+        acc_w += all_w + s_uw[qi];  // + the folded universal features: exact, so a row's bits do not depend on the fold
+        acc_c += all_c + s_uc[qi];
         // fused epilogue: pre-test without division, exact score for survivors; the warp then takes the query's lock
         // ONCE and inserts all surviving rows of the chunk into the sorted list held one entry per lane (k <= 32)
         float sc = -INFINITY;
         int row = 0x7fffffff;
         bool cand = false;
         if (lane < rows) {
-          const float dot = s_dotU[qi] + __ull2float_rn(acc_w) * (1.f / 4294967296.f);
-          const float corr = s_corrU[qi] - __ull2float_rn(acc_c) * (1.f / 16777216.f);
+          const float dot = __ull2float_rn(acc_w) * (1.f / 4294967296.f);
+          const float corr = -(__ull2float_rn(acc_c) * (1.f / 16777216.f));
           const float t = Bc + corr;
           float filt, ks = -INFINITY;
           int kr = 0x7fffffff;
@@ -1185,8 +1197,8 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
 }
 
 static inline size_t scan_smem_bytes(int k, bool distinct = false) {
-  return (size_t)GROUP_Q * QTAB_BYTES + (size_t)S_WARPS * 2 * S_BUF_BYTES + (size_t)S_WARPS * 2 * 8 + (size_t)GROUP_Q * 8 +
-         (size_t)GROUP_Q * k * 8 + (size_t)GROUP_Q * 4 * 7 + 32 + (distinct ? (size_t)GROUP_Q * k * 4 : 0);
+  return (size_t)GROUP_Q * QTAB_BYTES + (size_t)S_WARPS * 2 * S_BUF_BYTES + (size_t)S_WARPS * 2 * 8 + (size_t)GROUP_Q * 8 * 3 +
+         (size_t)GROUP_Q * k * 8 + (size_t)GROUP_Q * 4 * 5 + 32 + (distinct ? (size_t)GROUP_Q * k * 4 : 0);
 }
 
 // ----------------------------------------------------------------------------------------
