@@ -126,7 +126,7 @@ int kv_index_append(kv_index *ix, const int64_t *indptr, const uint32_t *ids, co
  * queries are then token-id SETS (every tf = 1; the id space is whatever the caller's vocabulary is),
  * score = |q ∩ row| / |q ∪ row| (0 for two empty sets).  The reference has no Jaccard path (its docs
  * list it as a possible measure, docs/failure-intelligence.md:43-46): parity UNPINNED, oracle = Python
- * sets.  kv_topk then ranks by float32 inter/union; kv_jaccard_counts returns the exact integers of the
+ * sets.  Top-k then ranks by float32 inter/union; kv_jaccard_counts returns the exact integers of the
  * selected pairs so that the caller can form the float64 ratio bit-exactly. */
 #define KV_MODE_TFIDF_COSINE 0
 #define KV_MODE_JACCARD 1
@@ -164,23 +164,12 @@ int64_t kv_index_rows(const kv_index *ix);
 int kv_score(kv_index *ix, const uint32_t *q_ids, const uint32_t *q_tf, int64_t q_nnz,
              double q_oov_tf2, double *out_scores);
 
-/* Batched scan with fused top-k (services/gfkb/app.py:88-89 generalised from 5 to k<=32):
- * for each query the k best rows ordered by (score desc, row asc) -- Python's stable
- * sort(reverse=True).  Outputs (host): out_scores[n_q*k] float32, out_rows[n_q*k] int64
- * (global row ids; unused tail slots: score -inf, row -1). */
-int kv_topk(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
-            const double *q_oov_tf2, int64_t n_q, int k, float *out_scores, int64_t *out_rows);
-
-/* Same, results left on the device (d_scores float32[n_q*k], d_rows int64[n_q*k], device
- * pointers owned by the caller, e.g. torch tensors feeding the NCCL all-gather); the call
- * returns after the work is enqueued AND completed on the handle's stream. */
-int kv_topk_device(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
-                   const double *q_oov_tf2, int64_t n_q, int k, void *d_scores, void *d_rows);
-
-/* The two halves of kv_topk_device, for callers that keep a query batch resident:
- * kv_query_upload does the host-side preparation and the host->device copies of a batch;
- * kv_topk_resident runs scan + merge for the uploaded batch (device work only) and returns
- * when it has completed.  The batch stays valid until the next upload or finalize. */
+/* Batched scan with fused top-k (services/gfkb/app.py:88-89 generalised from 5 to k<=32), in two steps:
+ * kv_query_upload (or _runs, _text, kv_selfjoin_upload) does the host-side preparation and the host->device copies of
+ * a query batch (n_q >= 1), which stays resident until the next upload or finalize; kv_topk_resident /
+ * kv_topk_resident_host run scan + merge for it, as often as wanted.  For each query the k best rows ordered by
+ * (score desc, row asc) -- Python's stable sort(reverse=True) -- as float32 scores[n_q*k] and int64 rows[n_q*k] by
+ * original query (global row ids; unused tail slots: score -inf, row -1). */
 int kv_query_upload(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
                     const double *q_oov_tf2, int64_t n_q);
 /* The same upload for a batch that arrives as n_runs consecutive slices (a row-sharded GFKB featurises one slice per
@@ -209,8 +198,10 @@ int kv_index_last_prepare_ms(const kv_index *ix, float ms[4]);
 /* Test hook: the resident batch's query order and flags (qperm[i] = original query at sorted slot i, flags[i] its
  * class: 0 regular, 1 null, 2 irregular); n_q must be the batch size. */
 int kv_debug_query_order(kv_index *ix, int32_t *qperm, uint8_t *flags, int64_t n_q);
+/* Top-k of the resident batch into caller-owned device memory (d_scores, d_rows; e.g. torch tensors feeding the NCCL
+ * all-gather); returns when the work on the handle's stream has completed.  k outside 1..32: KV_ERR_INVALID. */
 int kv_topk_resident(kv_index *ix, int k, void *d_scores, void *d_rows);
-/* Same with host outputs (out_scores float32[n_q*k], out_rows int64[n_q*k]). */
+/* Same with host outputs (out_scores, out_rows). */
 int kv_topk_resident_host(kv_index *ix, int k, float *out_scores, int64_t *out_rows);
 /* kv_topk_resident in two phases, for a row-sharded GFKB (kakveda_b200/dist.py): _seed = bound pass + seed scan, the
  * outputs receive this shard's seed top-k (device, [n_q*k], by original query); kv_index_raise_thresholds takes, per
@@ -286,9 +277,9 @@ int64_t kv_index_live_rows(const kv_index *ix);
 int kv_index_deleted_rows(kv_index *ix, uint8_t *out, int64_t n);
 
 /* Threshold search over the resident batch (kv_query_upload / kv_selfjoin_upload; exclusions honoured): every
- * (query, row) pair whose score -- the float32 value kv_topk reports for that pair -- is >= threshold,
+ * (query, row) pair whose score -- the float32 value the top-k reports for that pair -- is >= threshold,
  * 0 < threshold <= 1.  *n_pairs receives the count; the pairs stay in the handle until kv_range_fetch, the next
- * upload, finalize or range call.  Extension for threshold consumers (services/warning_policy/app.py:22,52 compares
+ * upload, range, append, deletion or finalize call.  Extension for threshold consumers (services/warning_policy/app.py:22,52 compares
  * with failure_matching.similarity_threshold; kv_cluster_csr links on the exact threshold graph).  It runs bound pass 1
  * on the fixed threshold and the candidate scan with an emitting epilogue (the exhaustive scan on small indexes), then
  * the float64 full scan of irregular queries; the resident batch, its exclusions and the top-k thresholds are left as
@@ -296,39 +287,32 @@ int kv_index_deleted_rows(kv_index *ix, uint8_t *out, int64_t n);
  * 0, [2] = bound pass 1, [3] = the scan (including a re-run after the pair buffer grew), [4] = irregular-query
  * fallbacks; kv_index_layout counters [9]-[13] describe the run.  threshold NaN, <= 0 or > 1: KV_ERR_INVALID.
  * KV_ERR_NOMEM when the candidate pool is exhausted or the pairs do not fit in device memory (the message gives their
- * count).  Jaccard indexes: KV_ERR_INVALID (they search with kv_jaccard_range_resident). */
+ * count).
+ * On a Jaccard index (KV_MODE_JACCARD) the score is |q ∩ row| / |q ∪ row| rounded once, and K3-R scores every chunk
+ * like the top-k scan and appends each match with its exact counts; queries of more than 64 tokens take the float64
+ * full scan, whose exact ratio gives the counts back.  Its pair buffer starts at 65,536 records and grows to the exact
+ * count when a search finds more (the scan then runs again).  kv_index_last_kernel_ms: [3] = the scan (re-run
+ * included), [4] = irregular-query fallbacks. */
 int kv_range_resident(kv_index *ix, float threshold, int64_t *n_pairs);
-/* The last range result: indptr[n_q+1] by original query, rows[n_pairs] (global), scores[n_pairs]; per query
- * ordered by (score desc, row asc).  KV_ERR_STATE when there is none (always on a Jaccard index). */
-int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores);
-/* The threshold search of a Jaccard index (KV_MODE_JACCARD), over the batch uploaded by kv_query_upload or
- * kv_selfjoin_upload (exclusions honoured): every (query, row) pair whose float32 score -- the value kv_topk reports,
- * |q ∩ row| / |q ∪ row| rounded once -- is >= threshold, 0 < threshold <= 1 (else KV_ERR_INVALID).  K3-R scores every
- * chunk like the top-k scan and appends each match with its exact counts; queries of more than 64 tokens take the
- * float64 full scan, whose exact ratio gives the counts back.  The pair buffer starts at 65,536 records and grows to
- * the exact count when a search finds more (the scan then runs again; KV_ERR_NOMEM with the count when the pairs do
- * not fit in device memory).  The result stays until kv_jaccard_range_fetch or the next upload, top-k, range, append
- * or finalize call.  kv_index_last_kernel_ms: [3] = the scan (re-run included), [4] = irregular-query fallbacks.
- * Both functions return KV_ERR_INVALID on a TF-IDF index. */
-int kv_jaccard_range_resident(kv_index *ix, float threshold, int64_t *n_pairs);
-/* The last Jaccard range result: indptr[n_q+1] by original query, rows[n_pairs] (global), scores[n_pairs] (float32),
- * inter[n_pairs] = |q ∩ row| and uni[n_pairs] = |q ∪ row|; per query ordered by (score desc, row asc), as
- * kv_range_fetch.  scores[i] is the float32 quotient inter[i] / uni[i].  KV_ERR_STATE when there is none. */
-int kv_jaccard_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores, int32_t *inter, int32_t *uni);
+/* The last range result: indptr[n_q+1] by original query, rows[n_pairs] (global), scores[n_pairs] (float32); per query
+ * ordered by (score desc, row asc).  On a Jaccard index also inter[n_pairs] = |q ∩ row| and uni[n_pairs] = |q ∪ row|,
+ * with scores[i] the float32 quotient inter[i] / uni[i]; a TF-IDF index has no counts.  inter and uni are required on
+ * a Jaccard index (like rows and scores: when there are pairs) and must be NULL on a TF-IDF index; anything else is
+ * KV_ERR_INVALID and leaves the result for a later fetch.  KV_ERR_STATE when there is no result. */
+int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores, int32_t *inter, int32_t *uni);
 /* Both fetches order the pairs on the device (an LSD radix sort of the records on (query, score desc, row)) and copy
  * the ordered arrays back; when pairs plus queries number below 8192 they copy the records back and order them on one
  * host core, which is faster there (the same bits either way).  The _device forms write the same arrays, bit for bit, to caller-owned device memory (e.g.
  * torch tensors) on the index's device: d_indptr int64[n_q+1], d_rows int64[n_pairs], d_scores float32[n_pairs], and
- * for Jaccard d_inter / d_uni int32[n_pairs].  They consume the result like the host fetch and return once the work on
- * the handle's stream is complete.  KV_ERR_STATE when there is no result (none computed, fetched already, or dropped by
- * a later upload); KV_ERR_INVALID on the other index kind, or when a pointer is not device memory of the index's device
- * aligned to its element size (the arrays of n_pairs elements are not looked at when n_pairs == 0).  KV_ERR_NOMEM (with
- * the pair count) when the ordering's scratch -- about the pair buffer's size again -- does not fit; the result then
- * stays for another try. */
-int kv_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores);
-int kv_jaccard_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores, void *d_inter, void *d_uni);
+ * for Jaccard d_inter / d_uni int32[n_pairs] (NULL on a TF-IDF index, as for the host fetch).  They consume the result
+ * like the host fetch and return once the work on the handle's stream is complete.  KV_ERR_STATE when there is no
+ * result (none computed, fetched already, or dropped by a later upload); KV_ERR_INVALID for count outputs that do not
+ * fit the index's mode, or when a pointer is not device memory of the index's device aligned to its element size (the
+ * arrays of n_pairs elements are not looked at when n_pairs == 0).  KV_ERR_NOMEM (with the pair count) when the
+ * ordering's scratch -- about the pair buffer's size again -- does not fit; the result then stays for another try. */
+int kv_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores, void *d_inter, void *d_uni);
 
-/* K6: float64 scores of selected (query, row) pairs: rows[n_q*k] are GLOBAL row ids (e.g. what kv_topk returned;
+/* K6: float64 scores of selected (query, row) pairs: rows[n_q*k] are GLOBAL row ids (e.g. what a top-k returned;
  * -1 = unused slot), out_scores[n_q*k] (host) receives the float64 cosine of SimilarityEngine.score
  * (similarity.py:14-20) for that row, -inf for unused slots and rows that live on another shard.  Summation follows
  * the row's stored feature order with nothing folded, so rows with identical text get identical bits on every shard /
@@ -346,7 +330,7 @@ int kv_rescore_pairs(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_id
  * shards prune with the best bound known anywhere (n_peers = 0 unmaps).  Results are unchanged -- a pushed value
  * always is a valid lower bound (k rows at least that good exist in some shard) -- only less is scanned.  Callers must
  * keep scans of different batches apart with a collective (the all-gather of partial top-k does that) and exchange
- * again after uploading a batch larger than `capacity` (kv_topk* returns KV_ERR_STATE otherwise). */
+ * again after uploading a batch larger than `capacity` (kv_topk_resident* returns KV_ERR_STATE otherwise). */
 int kv_index_thresholds_export(kv_index *ix, int64_t capacity, void *handle_out);
 int kv_index_thresholds_peers(kv_index *ix, const void *handles, int n_peers, int64_t capacity);
 /* Test hook: what kv_index_thresholds_peers does, for indexes of one process on one device (no CUDA IPC): ix pushes
@@ -366,9 +350,10 @@ int kv_merge_topk_device_on(int device, const void *d_scores_in, const void *d_r
                             int64_t n_q, int k, int64_t stride_s, int64_t stride_r, void *d_scores_out,
                             void *d_rows_out, void *stream, int sync);
 
-/* Timing of the last kv_topk / kv_topk_device call on this handle, CUDA-event
+/* Timing of the last query upload and top-k (kv_topk_resident, _host or _finish) on this handle, CUDA-event
  * milliseconds on its stream:
- * ms[0] = H2D of the query batch, ms[1] = bound + scan kernels, ms[2] = merge (+ fallbacks), ms[3] = D2H. */
+ * ms[0] = H2D of the query batch, ms[1] = bound + scan kernels, ms[2] = merge (+ fallbacks), ms[3] = D2H of host
+ * outputs. */
 int kv_index_last_timing(const kv_index *ix, float ms[4]);
 /* ... and of its kernels: ms[0] = bound pass 0 (seeds; wgmma GEMM + rare-feature join), ms[1] = seed scan,
  * ms[2] = bound pass 1 (candidate lists; when the bound codes of pass 0 were kept, only the snapshot of the
@@ -397,7 +382,7 @@ int kv_debug_bound_codes(kv_index *ix, int k, uint8_t *codes, int32_t *slot_quer
  * `device` with the code the fetch functions use, so that inputs a real search cannot cheaply produce can be checked.
  * jaccard = 0: records {int32 q, float32 score, int64 row} (rows global, row_base ignored); jaccard != 0: {int32 q,
  * int32 local row, int32 inter, int32 uni}, rows + row_base, scores inter / uni in float32.  Outputs as
- * kv_jaccard_range_fetch (host); inter / uni are only written for Jaccard records.  Records with a query outside
+ * kv_range_fetch (host); inter / uni are only written for Jaccard records.  Records with a query outside
  * 0..n_q-1, a NaN score or counts outside 0 <= inter <= uni, uni >= 1: KV_ERR_INVALID. */
 int kv_debug_range_order(int device, int jaccard, const void *records, int64_t n, int64_t n_q, int64_t row_base,
                          int64_t *indptr, int64_t *rows, float *scores, int32_t *inter, int32_t *uni);

@@ -55,9 +55,6 @@ SIGNATURES = {
     "kv_index_last_finalize_kind": (C.c_int, [C.c_void_p]),
     "kv_index_rows": (C.c_int64, [C.c_void_p]),
     "kv_score": (C.c_int, [C.c_void_p, c_u32p, c_u32p, C.c_int64, C.c_double, c_f64p]),
-    "kv_topk": (C.c_int, [C.c_void_p, c_i64p, c_u32p, c_u32p, c_f64p, C.c_int64, C.c_int, c_f32p, c_i64p]),
-    "kv_topk_device": (C.c_int, [C.c_void_p, c_i64p, c_u32p, c_u32p, c_f64p, C.c_int64, C.c_int, C.c_void_p,
-                                 C.c_void_p]),
     "kv_query_upload": (C.c_int, [C.c_void_p, c_i64p, c_u32p, c_u32p, c_f64p, C.c_int64]),
     "kv_query_prepare_slice": (C.c_int, [C.c_void_p, c_i64p, c_u32p, c_u32p, c_f64p, C.c_int64, c_i64p, c_u32p, c_u32p,
                                          c_f64p, C.POINTER(C.c_int32), C.POINTER(C.c_uint8)]),
@@ -83,11 +80,8 @@ SIGNATURES = {
     "kv_index_deleted_rows": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint8), C.c_int64]),
     "kv_rescore_pairs": (C.c_int, [C.c_void_p, c_i64p, c_u32p, c_u32p, c_f64p, C.c_int64, C.c_int, c_i64p, c_f64p]),
     "kv_range_resident": (C.c_int, [C.c_void_p, C.c_float, c_i64p]),
-    "kv_range_fetch": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f32p]),
-    "kv_jaccard_range_resident": (C.c_int, [C.c_void_p, C.c_float, c_i64p]),
-    "kv_jaccard_range_fetch": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f32p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
-    "kv_range_fetch_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "kv_jaccard_range_fetch_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kv_range_fetch": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f32p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "kv_range_fetch_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kv_cluster_topk": (C.c_int, [C.c_int64, C.c_int, c_i64p, c_f32p, C.c_float, c_i64p, c_i64p]),
     "kv_cluster_csr": (C.c_int, [C.c_int64, c_i64p, c_i64p, c_i64p, c_i64p]),
     "kv_cluster_csr_device": (C.c_int, [C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, c_i64p]),

@@ -162,24 +162,20 @@ struct kv_index {
   DevBuf<int> d_rthr;
   DevBuf<RangePair> d_range;
   DevBuf<unsigned long long> d_range_count;
-  bool range_valid = false;
-  // the same on a Jaccard index (K3-R, kv_jaccard_range_resident): the records carry the exact counts and have a
-  // result flag of their own, so kv_range_fetch never reads them
+  // on a Jaccard index (K3-R) the records carry the exact counts and local rows instead: d_jrange
   DevBuf<JaccardPair> d_jrange;
-  bool jrange_valid = false;
+  bool range_valid = false;
   int64_t range_q = 0, range_pairs = 0;
   RangeOrderScratch rsort;  // the fetches order the pairs on the device (range_order.cu)
   DevBuf<unsigned long long> d_stats;
   DevBuf<float> d_part_s, d_out_s;
   DevBuf<long long> d_part_r, d_out_r;
-  PinnedBuf<float> h_out_s;
-  PinnedBuf<long long> h_out_r;
   // single-query scratch
   PinnedBuf<unsigned char> h_qtab;
   DevBuf<unsigned char> d_qtab1;
   DevBuf<double> d_scores;
 
-  // query batch currently resident on the device (kv_query_upload / first half of kv_topk)
+  // query batch currently resident on the device (kv_query_upload and its variants)
   bool batch_valid = false;
   int64_t batch_q = 0, batch_tiles = 0, batch_h2d_bytes = 0, batch_null = 0, batch_f2_outside = 0;
   std::vector<int64_t> irr_q, irr_indptr;
@@ -421,7 +417,7 @@ int kv_index_append(kv_index *ix, const int64_t *indptr, const uint32_t *ids, co
   ix->ids.n = ix->nnz;
   ix->tf.n = ix->nnz;
   ix->finalized = false;
-  ix->jrange_valid = false;
+  ix->range_valid = false;
   // labels describe the rows they were given for: a filtered query fails until the rows are labelled again
   ix->h_labels.clear();
   ix->has_labels = ix->labels_on_device = false;
@@ -705,7 +701,7 @@ int kv_index_delete_rows(kv_index *ix, const int64_t *rows, int64_t n) {
   ix->n_dead += added;
   // like an append: statistics and the device copies are stale until the next finalize
   ix->finalized = false;
-  ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
+  ix->batch_valid = ix->range_valid = false;
   return KV_OK;
 }
 
@@ -826,7 +822,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
       KV_CUDA(cudaStreamSynchronize(s));
       ix->V = V;
       ix->finalized = true;
-      ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
+      ix->batch_valid = ix->range_valid = false;
       ix->last_finalize_kind = 2;
       return upload_row_sets(ix);
     }
@@ -868,7 +864,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
   KV_CUDA(cudaStreamSynchronize(s));
   ix->V = V;
   ix->finalized = true;
-  ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
+  ix->batch_valid = ix->range_valid = false;
   ix->last_finalize_kind = 1;
   return upload_row_sets(ix);
 }
@@ -1025,13 +1021,13 @@ static bool csr_ok(const int64_t *q_indptr, const uint32_t *q_ids, const uint32_
 static int build_query_tables(kv_index *ix, int64_t n_q);
 
 static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
-  if (!ix->finalized) return kv_fail(KV_ERR_STATE, "kv_topk: index not finalized");
+  if (!ix->finalized) return kv_fail(KV_ERR_STATE, "kv_query_upload: index not finalized");
   int64_t n_q = 0, nnz = 0;
   std::vector<int64_t> qb((size_t)n_runs + 1, 0), nb((size_t)n_runs + 1, 0);
   bool have_order = true, have_flags = true, any_order = false;
   for (int r = 0; r < n_runs; r++) {
     const QueryRun &R = runs[r];
-    if (R.n_q < 0 || !R.indptr || !csr_ok(R.indptr, R.ids, R.tf, R.n_q)) return kv_fail(KV_ERR_INVALID, "kv_topk: bad query CSR");
+    if (R.n_q < 0 || !R.indptr || !csr_ok(R.indptr, R.ids, R.tf, R.n_q)) return kv_fail(KV_ERR_INVALID, "kv_query_upload: bad query CSR");
     n_q += R.n_q;
     nnz += R.indptr[R.n_q] - R.indptr[0];
     qb[(size_t)r + 1] = n_q;
@@ -1042,11 +1038,11 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   }
   // a run with an order stores its rows sorted: without the orders of ALL runs the rows cannot be mapped back
   if (any_order && !have_order) return kv_fail(KV_ERR_INVALID, "kv_query_upload_runs: slice orders must be given for all runs or for none");
-  if (n_q < 1) return kv_fail(KV_ERR_INVALID, "kv_topk: empty query batch");
-  if (n_q >= (1LL << 31) - TILE_Q) return kv_fail(KV_ERR_INVALID, "kv_topk: too many queries in one call");
+  if (n_q < 1) return kv_fail(KV_ERR_INVALID, "kv_query_upload: empty query batch");
+  if (n_q >= (1LL << 31) - TILE_Q) return kv_fail(KV_ERR_INVALID, "kv_query_upload: too many queries in one call");
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
-  ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
+  ix->batch_valid = ix->range_valid = false;
   ix->has_excl = ix->has_filter = ix->distinct = false;
   ix->irr_q.clear(); ix->irr_indptr.assign(1, 0); ix->irr_ids.clear(); ix->irr_tf.clear(); ix->irr_oov.clear();
   const int T = host_threads();
@@ -1336,15 +1332,15 @@ __global__ void __launch_bounds__(TQ_THREADS) slot_order_kernel(const int *order
 
 static int prepare_batch_text(kv_index *ix, kv_vocab_mirror *m, const kv_vocab *v, const char *bytes,
                               const int64_t *offsets, int64_t n_q, int mode, int64_t *bad_doc) {
-  if (!ix->finalized) return kv_fail(KV_ERR_STATE, "kv_topk: index not finalized");
-  if (n_q < 1) return kv_fail(KV_ERR_INVALID, "kv_topk: empty query batch");
-  if (n_q >= (1LL << 31) - TILE_Q) return kv_fail(KV_ERR_INVALID, "kv_topk: too many queries in one call");
+  if (!ix->finalized) return kv_fail(KV_ERR_STATE, "kv_query_upload_text: index not finalized");
+  if (n_q < 1) return kv_fail(KV_ERR_INVALID, "kv_query_upload_text: empty query batch");
+  if (n_q >= (1LL << 31) - TILE_Q) return kv_fail(KV_ERR_INVALID, "kv_query_upload_text: too many queries in one call");
   if (mirror_device(m) != ix->device)
     return kv_fail(KV_ERR_INVALID, "kv_query_upload_text: the vocabulary mirror is on device %d, the index on device %d",
                    mirror_device(m), ix->device);
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
-  ix->batch_valid = ix->range_valid = ix->jrange_valid = false;
+  ix->batch_valid = ix->range_valid = false;
   ix->has_excl = ix->has_filter = ix->distinct = false;
   ix->irr_q.clear(); ix->irr_indptr.assign(1, 0); ix->irr_ids.clear(); ix->irr_tf.clear(); ix->irr_oov.clear();
   const auto t_begin = std::chrono::steady_clock::now();
@@ -1666,28 +1662,33 @@ static int size_batch(kv_index *ix, Batch &b) {
     KV_CUDA(ix->d_pool_ctl.ensure(2));
   }
   if (prune && bound_smem_bytes(b.max_pages) > 232448)
-    return kv_fail(KV_ERR_INVALID, "kv_topk: index too large for one bound-kernel row range (max_pages %d)", b.max_pages);
+    return kv_fail(KV_ERR_INVALID, "kv_topk_resident: index too large for one bound-kernel row range (max_pages %d)", b.max_pages);
   return KV_OK;
 }
 
+// d_out_s / d_out_r: device outputs [n_q*k] (NULL: ix->d_out_s / d_out_r).  phase 0 = the whole top-k, 1 = bound pass +
+// seed scan, 2 = the rest (kv_topk_resident_seed / _finish).
 static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, int phase = 0) {
   if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_topk_resident: no query batch uploaded");
-  if (k < 1 || k > 32) return kv_fail(KV_ERR_INVALID, "kv_topk: k must be 1..32");
-  int rc = check_filter(ix, "kv_topk");
+  if (k < 1 || k > 32) return kv_fail(KV_ERR_INVALID, "kv_topk_resident: k must be 1..32");
+  int rc = check_filter(ix, "kv_topk_resident");
   if (rc != KV_OK) return rc;
   // the thresholds peers push are those of unfiltered queries: not a bound of a filtered query's k-th score
   if (ix->has_filter && (ix->gthr_exported || ix->n_peers))
-    return kv_fail(KV_ERR_INVALID, "kv_topk: a label filter cannot be combined with the threshold exchange of a row-sharded GFKB");
+    return kv_fail(KV_ERR_INVALID, "kv_topk_resident: a label filter cannot be combined with the threshold exchange of a row-sharded GFKB");
   if (ix->distinct) {
     if (!groups_ready(ix))
-      return kv_fail(KV_ERR_STATE, "kv_topk: the batch is distinct but the row groups are missing or stale (set them again after an append)");
+      return kv_fail(KV_ERR_STATE, "kv_topk_resident: the batch is distinct but the row groups are missing or stale (set them again after an append)");
     // a shard's seed k-th score is no lower bound of the global k-th GROUP score: one group can count on several shards
     if (phase != 0 || ix->gthr_exported || ix->n_peers)
-      return kv_fail(KV_ERR_INVALID, "kv_topk: distinct mode cannot be combined with the two-phase top-k or the threshold exchange of a row-sharded GFKB");
+      return kv_fail(KV_ERR_INVALID, "kv_topk_resident: distinct mode cannot be combined with the two-phase top-k or the threshold exchange of a row-sharded GFKB");
   }
-  ix->jrange_valid = false;
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
+  if (!d_out_s) {  // results for a host read-back: the handle's own device outputs
+    KV_CUDA(ix->d_out_s.ensure(ix->batch_q * k)); KV_CUDA(ix->d_out_r.ensure(ix->batch_q * k));
+    d_out_s = ix->d_out_s.p; d_out_r = ix->d_out_r.p;
+  }
   Batch b;
   b.k = k; b.phase = phase; b.out_s = d_out_s; b.out_r = d_out_r; b.distinct = ix->distinct;
   rc = size_batch(ix, b);
@@ -1695,7 +1696,7 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
   const int64_t n_q = b.n_q;
   const bool prune = b.prune;
   if (n_q > ix->d_gthr.cap && (ix->gthr_exported || ix->n_peers))
-    return kv_fail(KV_ERR_STATE, "kv_topk: the query batch outgrew the threshold array shared with the peer GPUs; exchange it again "
+    return kv_fail(KV_ERR_STATE, "kv_topk_resident: the query batch outgrew the threshold array shared with the peer GPUs; exchange it again "
                                  "(kv_index_thresholds_export / kv_index_thresholds_peers)");
   KV_CUDA(ix->d_gthr.ensure(n_q));
   b.n_peers = (ix->n_peers > 0 && n_q <= ix->peer_cap) ? ix->n_peers : 0;
@@ -1810,7 +1811,7 @@ static int check_pool(kv_index *ix) {
   const unsigned int *ctl = (const unsigned int *)&ix->last_stats[6];
   if (ix->n_rows > 0 && ctl[1] != 0) {
     ix->last_stats[6] = 0;
-    return kv_fail(KV_ERR_NOMEM, "kv_topk: the candidate pool (%lld pages) is exhausted; split the query batch",
+    return kv_fail(KV_ERR_NOMEM, "kv_topk_resident: the candidate pool (%lld pages) is exhausted; split the query batch",
                    (long long)ix->pool_pages);
   }
   return KV_OK;
@@ -1827,10 +1828,10 @@ static int finish_batch(kv_index *ix) {
 // Threshold search over the resident batch: every pair with score >= thr lands in d_range (d_jrange on a Jaccard
 // index), *n_pairs = their count.  When they do not fit, the buffer grows to the exact count and only the scan and the
 // fallbacks run again (the candidate lists depend on the threshold alone).  Events: evk[2] -> evk[3] bound pass 1,
-// evk[3] -> evk[4] scan, evk[4] -> evk[5] irregular-query fallbacks.  `fn` names the caller in error messages.
-// Caller holds ix->mu.
-static int run_range(kv_index *ix, float thr, int64_t *n_pairs, const char *fn) {
-  ix->range_valid = ix->jrange_valid = false;
+// evk[3] -> evk[4] scan, evk[4] -> evk[5] irregular-query fallbacks.  Caller holds ix->mu.
+static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
+  const char *fn = "kv_range_resident";
+  ix->range_valid = false;
   if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "%s: no query batch uploaded", fn);
   int rc = check_filter(ix, fn);
   if (rc != KV_OK) return rc;
@@ -1918,41 +1919,24 @@ static int run_range(kv_index *ix, float thr, int64_t *n_pairs, const char *fn) 
   ix->last_launches = b.launches;
   ix->range_q = n_q;
   ix->range_pairs = (int64_t)count;
-  (jac ? ix->jrange_valid : ix->range_valid) = true;
+  ix->range_valid = true;
   *n_pairs = (int64_t)count;
   return KV_OK;
 }
 
-static int topk_impl(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
-                     const double *q_oov, int64_t n_q, int k, float *h_scores, int64_t *h_rows, void *d_scores_out,
-                     void *d_rows_out) {
-  if (!ix || n_q < 0 || k < 1 || k > 32 || (n_q > 0 && !q_indptr))
-    return kv_fail(KV_ERR_INVALID, "kv_topk: bad arguments (k must be 1..32)");
-  std::lock_guard<std::mutex> g(ix->mu);
-  if (!ix->finalized) return kv_fail(KV_ERR_STATE, "kv_topk: index not finalized");
-  if (n_q == 0) return KV_OK;
-  int rc = prepare_batch(ix, q_indptr, q_ids, q_tf, q_oov, n_q);
+// One top-k run of the resident batch into device outputs (NULL: the handle's own), copied to h_scores / h_rows when
+// given.  Returns once the stream is complete, with the batch's timings and the candidate-pool check.  Caller holds ix->mu.
+static int topk_run(kv_index *ix, int k, int phase, void *d_scores, void *d_rows, float *h_scores, int64_t *h_rows) {
+  int rc = run_batch(ix, k, (float *)d_scores, (long long *)d_rows, phase);
   if (rc != KV_OK) return rc;
   cudaStream_t s = ix->stream;
-  float *d_out_s = (float *)d_scores_out;
-  long long *d_out_r = (long long *)d_rows_out;
-  if (!d_out_s) {
-    KV_CUDA(ix->d_out_s.ensure(n_q * k)); KV_CUDA(ix->d_out_r.ensure(n_q * k));
-    d_out_s = ix->d_out_s.p; d_out_r = ix->d_out_r.p;
-  }
-  rc = run_batch(ix, k, d_out_s, d_out_r);
-  if (rc != KV_OK) return rc;
   if (h_scores) {
-    KV_CUDA(ix->h_out_s.ensure(n_q * k)); KV_CUDA(ix->h_out_r.ensure(n_q * k));
-    KV_CUDA(cudaMemcpyAsync(ix->h_out_s.p, d_out_s, (size_t)n_q * k * sizeof(float), cudaMemcpyDeviceToHost, s));
-    KV_CUDA(cudaMemcpyAsync(ix->h_out_r.p, d_out_r, (size_t)n_q * k * sizeof(long long), cudaMemcpyDeviceToHost, s));
+    const size_t n = (size_t)(ix->batch_q * k);
+    KV_CUDA(cudaMemcpyAsync(h_scores, ix->d_out_s.p, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+    KV_CUDA(cudaMemcpyAsync(h_rows, ix->d_out_r.p, n * sizeof(long long), cudaMemcpyDeviceToHost, s));
   }
   KV_CUDA(cudaEventRecord(ix->ev[4], s));
   KV_CUDA(cudaStreamSynchronize(s));
-  if (h_scores) {
-    memcpy(h_scores, ix->h_out_s.p, (size_t)n_q * k * sizeof(float));
-    memcpy(h_rows, ix->h_out_r.p, (size_t)n_q * k * sizeof(int64_t));
-  }
   return finish_batch(ix);
 }
 
@@ -2190,109 +2174,70 @@ int kv_query_set_distinct(kv_index *ix, int on) {
 int kv_topk_resident_host(kv_index *ix, int k, float *out_scores, int64_t *out_rows) {
   if (!ix || !out_scores || !out_rows) return kv_fail(KV_ERR_INVALID, "kv_topk_resident_host: bad arguments");
   std::lock_guard<std::mutex> g(ix->mu);
-  if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_topk_resident_host: no query batch uploaded");
-  if (k < 1 || k > 32) return kv_fail(KV_ERR_INVALID, "kv_topk: k must be 1..32");
-  const int64_t n_q = ix->batch_q;
-  KV_CUDA(cudaSetDevice(ix->device));
-  KV_CUDA(ix->d_out_s.ensure(n_q * k)); KV_CUDA(ix->d_out_r.ensure(n_q * k));
-  int rc = run_batch(ix, k, ix->d_out_s.p, ix->d_out_r.p);
-  if (rc != KV_OK) return rc;
-  KV_CUDA(cudaMemcpyAsync(out_scores, ix->d_out_s.p, (size_t)n_q * k * sizeof(float), cudaMemcpyDeviceToHost, ix->stream));
-  KV_CUDA(cudaMemcpyAsync(out_rows, ix->d_out_r.p, (size_t)n_q * k * sizeof(long long), cudaMemcpyDeviceToHost, ix->stream));
-  KV_CUDA(cudaEventRecord(ix->ev[4], ix->stream));
-  KV_CUDA(cudaStreamSynchronize(ix->stream));
-  return finish_batch(ix);
+  return topk_run(ix, k, 0, nullptr, nullptr, out_scores, out_rows);
 }
 
 int kv_range_resident(kv_index *ix, float threshold, int64_t *n_pairs) {
   if (!ix || !n_pairs) return kv_fail(KV_ERR_INVALID, "kv_range_resident: bad arguments");
   if (!(threshold > 0.f && threshold <= 1.f)) return kv_fail(KV_ERR_INVALID, "kv_range_resident: threshold must be in (0, 1]");
   std::lock_guard<std::mutex> g(ix->mu);
-  if (ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_range_resident: a Jaccard index searches with kv_jaccard_range_resident");
-  return run_range(ix, threshold, n_pairs, "kv_range_resident");
+  return run_range(ix, threshold, n_pairs);
 }
 
-int kv_jaccard_range_resident(kv_index *ix, float threshold, int64_t *n_pairs) {
-  if (!ix || !n_pairs) return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_resident: bad arguments");
-  if (!(threshold > 0.f && threshold <= 1.f))
-    return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_resident: threshold must be in (0, 1]");
-  std::lock_guard<std::mutex> g(ix->mu);
-  if (!ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_resident: not a Jaccard index (kv_range_resident)");
-  return run_range(ix, threshold, n_pairs, "kv_jaccard_range_resident");
+// The count outputs a fetch was given must fit the index's mode: required on a Jaccard index (like rows and scores, only
+// when there are pairs), NULL on a TF-IDF index.  Checked before anything is consumed.
+static int check_count_outputs(const kv_index *ix, const void *inter, const void *uni, const char *fn) {
+  if (!ix->jaccard && (inter || uni))
+    return kv_fail(KV_ERR_INVALID, "%s: a TF-IDF index has no count outputs (pass NULL for inter and uni)", fn);
+  if (ix->jaccard && ix->range_valid && ix->range_pairs > 0 && (!inter || !uni))
+    return kv_fail(KV_ERR_INVALID, "%s: a Jaccard index returns the exact counts (inter and uni are required)", fn);
+  return KV_OK;
 }
 
-// The pairs come back in emit order, which the scan does not fix; scores are exact integer sums rounded once, so
-// (score desc, row asc) is a total order of each query's pairs and the result is deterministic.  Both fetches order the
-// pairs on the device (range_order.cu, in the pair buffer itself: the fetch consumes the result) and copy the ordered
-// arrays back.  Once ordering has started the result is gone whatever happens; a scratch allocation that fails first
-// (KV_ERR_NOMEM) leaves it for another try.
-int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores) {
-  if (!ix || !indptr) return kv_fail(KV_ERR_INVALID, "kv_range_fetch: bad arguments");
+// The pairs come back in emit order, which the scan does not fix; scores are exact integer sums (Jaccard: the quotient
+// inter / union) rounded once, so (score desc, row asc) is a total order of each query's pairs and the result is
+// deterministic.  Both fetches order the pairs on the device (range_order.cu, in the pair buffer itself: the fetch
+// consumes the result) and copy the ordered arrays back.  Once ordering has started the result is gone whatever
+// happens; a scratch allocation that fails first (KV_ERR_NOMEM) leaves it for another try.  The records of a Jaccard
+// index hold local rows: the ordering adds row_base.
+int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores, int32_t *inter, int32_t *uni) {
+  const char *fn = "kv_range_fetch";
+  if (!ix || !indptr) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
   std::lock_guard<std::mutex> g(ix->mu);
-  if (!ix->range_valid) return kv_fail(KV_ERR_STATE, "kv_range_fetch: no threshold search result (kv_range_resident first)");
+  int rc = check_count_outputs(ix, inter, uni, fn);
+  if (rc != KV_OK) return rc;
+  if (!ix->range_valid) return kv_fail(KV_ERR_STATE, "%s: no threshold search result (kv_range_resident first)", fn);
   const int64_t n_q = ix->range_q, n = ix->range_pairs;
-  if (n > 0 && (!rows || !scores)) return kv_fail(KV_ERR_INVALID, "kv_range_fetch: bad arguments");
+  if (n > 0 && (!rows || !scores)) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
   KV_CUDA(cudaSetDevice(ix->device));
-  const int rc = range_order_to_host(ix->d_range.p, n, n_q, 0, indptr, rows, scores, nullptr, nullptr, ix->rsort, ix->stream,
-                                     "kv_range_fetch");
+  rc = ix->jaccard ? range_order_to_host(ix->d_jrange.p, n, n_q, ix->row_base, indptr, rows, scores, inter, uni, ix->rsort,
+                                         ix->stream, fn)
+                   : range_order_to_host(ix->d_range.p, n, n_q, 0, indptr, rows, scores, nullptr, nullptr, ix->rsort, ix->stream, fn);
   if (rc != KV_ERR_NOMEM) ix->range_valid = false;
-  return rc;
-}
-
-// Same order as kv_range_fetch: the score is inter / union rounded to float32, and equal scores order by row.
-int kv_jaccard_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores, int32_t *inter, int32_t *uni) {
-  if (!ix || !indptr) return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_fetch: bad arguments");
-  std::lock_guard<std::mutex> g(ix->mu);
-  if (!ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_fetch: not a Jaccard index (kv_range_fetch)");
-  if (!ix->jrange_valid)
-    return kv_fail(KV_ERR_STATE, "kv_jaccard_range_fetch: no threshold search result (kv_jaccard_range_resident first)");
-  const int64_t n_q = ix->range_q, n = ix->range_pairs;
-  if (n > 0 && (!rows || !scores || !inter || !uni)) return kv_fail(KV_ERR_INVALID, "kv_jaccard_range_fetch: bad arguments");
-  KV_CUDA(cudaSetDevice(ix->device));
-  const int rc = range_order_to_host(ix->d_jrange.p, n, n_q, ix->row_base, indptr, rows, scores, inter, uni, ix->rsort,
-                                     ix->stream, "kv_jaccard_range_fetch");
-  if (rc != KV_ERR_NOMEM) ix->jrange_valid = false;
   return rc;
 }
 
 // Device outputs: the same arrays, written to caller-owned device memory of the index's device.
-int kv_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores) {
+int kv_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores, void *d_inter, void *d_uni) {
   const char *fn = "kv_range_fetch_device";
   if (!ix) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
   std::lock_guard<std::mutex> g(ix->mu);
-  if (ix->jaccard) return kv_fail(KV_ERR_INVALID, "%s: a Jaccard index fetches with kv_jaccard_range_fetch_device", fn);
+  int rc = check_count_outputs(ix, d_inter, d_uni, fn);
+  if (rc != KV_OK) return rc;
   if (!ix->range_valid) return kv_fail(KV_ERR_STATE, "%s: no threshold search result (kv_range_resident first)", fn);
   const int64_t n_q = ix->range_q, n = ix->range_pairs;
-  int rc = check_device_ptr(d_indptr, ix->device, 8, "indptr", fn);
+  rc = check_device_ptr(d_indptr, ix->device, 8, "indptr", fn);
   if (rc == KV_OK && n > 0) rc = check_device_ptr(d_rows, ix->device, 8, "rows", fn);
   if (rc == KV_OK && n > 0) rc = check_device_ptr(d_scores, ix->device, 4, "scores", fn);
+  if (rc == KV_OK && n > 0 && ix->jaccard) rc = check_device_ptr(d_inter, ix->device, 4, "inter", fn);
+  if (rc == KV_OK && n > 0 && ix->jaccard) rc = check_device_ptr(d_uni, ix->device, 4, "uni", fn);
   if (rc != KV_OK) return rc;
   KV_CUDA(cudaSetDevice(ix->device));
-  rc = range_order_device(ix->d_range.p, n, n_q, 0, (int64_t *)d_indptr, (int64_t *)d_rows, (float *)d_scores, nullptr, nullptr,
-                          ix->rsort, ix->stream, fn);
+  rc = ix->jaccard ? range_order_device(ix->d_jrange.p, n, n_q, ix->row_base, (int64_t *)d_indptr, (int64_t *)d_rows,
+                                        (float *)d_scores, (int32_t *)d_inter, (int32_t *)d_uni, ix->rsort, ix->stream, fn)
+                   : range_order_device(ix->d_range.p, n, n_q, 0, (int64_t *)d_indptr, (int64_t *)d_rows, (float *)d_scores,
+                                        nullptr, nullptr, ix->rsort, ix->stream, fn);
   if (rc != KV_ERR_NOMEM) ix->range_valid = false;
-  if (rc != KV_OK) return rc;
-  KV_CUDA(cudaStreamSynchronize(ix->stream));
-  return KV_OK;
-}
-
-int kv_jaccard_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores, void *d_inter, void *d_uni) {
-  const char *fn = "kv_jaccard_range_fetch_device";
-  if (!ix) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
-  std::lock_guard<std::mutex> g(ix->mu);
-  if (!ix->jaccard) return kv_fail(KV_ERR_INVALID, "%s: not a Jaccard index (kv_range_fetch_device)", fn);
-  if (!ix->jrange_valid) return kv_fail(KV_ERR_STATE, "%s: no threshold search result (kv_jaccard_range_resident first)", fn);
-  const int64_t n_q = ix->range_q, n = ix->range_pairs;
-  int rc = check_device_ptr(d_indptr, ix->device, 8, "indptr", fn);
-  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_rows, ix->device, 8, "rows", fn);
-  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_scores, ix->device, 4, "scores", fn);
-  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_inter, ix->device, 4, "inter", fn);
-  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_uni, ix->device, 4, "uni", fn);
-  if (rc != KV_OK) return rc;
-  KV_CUDA(cudaSetDevice(ix->device));
-  rc = range_order_device(ix->d_jrange.p, n, n_q, ix->row_base, (int64_t *)d_indptr, (int64_t *)d_rows, (float *)d_scores,
-                          (int32_t *)d_inter, (int32_t *)d_uni, ix->rsort, ix->stream, fn);
-  if (rc != KV_ERR_NOMEM) ix->jrange_valid = false;
   if (rc != KV_OK) return rc;
   KV_CUDA(cudaStreamSynchronize(ix->stream));
   return KV_OK;
@@ -2362,11 +2307,7 @@ int kv_debug_thresholds_link(kv_index *ix, kv_index *const *peers, int n_peers, 
 int kv_topk_resident(kv_index *ix, int k, void *d_scores, void *d_rows) {
   if (!ix || !d_scores || !d_rows) return kv_fail(KV_ERR_INVALID, "kv_topk_resident: bad arguments");
   std::lock_guard<std::mutex> g(ix->mu);
-  int rc = run_batch(ix, k, (float *)d_scores, (long long *)d_rows);
-  if (rc != KV_OK) return rc;
-  KV_CUDA(cudaEventRecord(ix->ev[4], ix->stream));
-  KV_CUDA(cudaStreamSynchronize(ix->stream));
-  return finish_batch(ix);
+  return topk_run(ix, k, 0, d_scores, d_rows, nullptr, nullptr);
 }
 
 // Two-phase form for a row-sharded GFKB: _seed runs the bound pass and the seed scan of the resident batch and returns
@@ -2398,23 +2339,7 @@ int kv_index_raise_thresholds(kv_index *ix, const void *d_kth_scores, int64_t n_
 int kv_topk_resident_finish(kv_index *ix, int k, void *d_scores, void *d_rows) {
   if (!ix || !d_scores || !d_rows) return kv_fail(KV_ERR_INVALID, "kv_topk_resident_finish: bad arguments");
   std::lock_guard<std::mutex> g(ix->mu);
-  int rc = run_batch(ix, k, (float *)d_scores, (long long *)d_rows, 2);
-  if (rc != KV_OK) return rc;
-  KV_CUDA(cudaEventRecord(ix->ev[4], ix->stream));
-  KV_CUDA(cudaStreamSynchronize(ix->stream));
-  return finish_batch(ix);
-}
-
-int kv_topk(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
-            const double *q_oov_tf2, int64_t n_q, int k, float *out_scores, int64_t *out_rows) {
-  if (n_q > 0 && (!out_scores || !out_rows)) return kv_fail(KV_ERR_INVALID, "kv_topk: output buffers are NULL");
-  return topk_impl(ix, q_indptr, q_ids, q_tf, q_oov_tf2, n_q, k, out_scores, out_rows, nullptr, nullptr);
-}
-
-int kv_topk_device(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
-                   const double *q_oov_tf2, int64_t n_q, int k, void *d_scores, void *d_rows) {
-  if (n_q > 0 && (!d_scores || !d_rows)) return kv_fail(KV_ERR_INVALID, "kv_topk_device: output buffers are NULL");
-  return topk_impl(ix, q_indptr, q_ids, q_tf, q_oov_tf2, n_q, k, nullptr, nullptr, d_scores, d_rows);
+  return topk_run(ix, k, 2, d_scores, d_rows, nullptr, nullptr);
 }
 
 int kv_merge_topk_device(int device, const void *d_scores_in, const void *d_rows_in, int n_lists, int64_t n_q, int k,
@@ -2453,9 +2378,8 @@ int kv_debug_bound_numerators(kv_index *ix, int k, float *out, int32_t *slot_que
   DevBuf<float> xs;
   KV_CUDA(xs.ensure(n_q * stride));
   KV_CUDA(cudaMemset(xs.p, 0, (size_t)(n_q * stride) * 4));
-  KV_CUDA(ix->d_out_s.ensure(n_q * k)); KV_CUDA(ix->d_out_r.ensure(n_q * k));
   ix->dbg_xs = xs.p;
-  int rc = run_batch(ix, k, ix->d_out_s.p, ix->d_out_r.p);
+  int rc = run_batch(ix, k, nullptr, nullptr);
   ix->dbg_xs = nullptr;
   if (rc == KV_OK) {
     KV_CUDA(cudaEventRecord(ix->ev[4], ix->stream));
@@ -2480,12 +2404,8 @@ int kv_debug_bound_codes(kv_index *ix, int k, uint8_t *codes, int32_t *slot_quer
   if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_debug_bound_codes: no query batch uploaded");
   KV_CUDA(cudaSetDevice(ix->device));
   const int64_t n_q = ix->batch_q;
-  KV_CUDA(ix->d_out_s.ensure(n_q * k)); KV_CUDA(ix->d_out_r.ensure(n_q * k));
-  int rc = run_batch(ix, k, ix->d_out_s.p, ix->d_out_r.p);
+  int rc = topk_run(ix, k, 0, nullptr, nullptr, nullptr, nullptr);
   if (rc != KV_OK) return rc;
-  KV_CUDA(cudaEventRecord(ix->ev[4], ix->stream));
-  KV_CUDA(cudaStreamSynchronize(ix->stream));
-  if ((rc = finish_batch(ix)) != KV_OK) return rc;
   if (!ix->last_used_codes) {
     const char *np = getenv("KAKVEDA_B200_NO_PRUNE"), *ce = getenv("KAKVEDA_B200_BOUND_CODES");
     const char *why = ix->jaccard ? "a Jaccard index has no bound pass"

@@ -16,8 +16,9 @@ from typing import Optional, Sequence, Tuple
 
 import numpy as np
 
-from . import _capi, _devout
+from . import _capi
 from ._capi import no_distinct
+from .similarity import _KvIndex, _ptr
 
 
 def _csr(sets: Sequence[Sequence[int]]) -> Tuple[np.ndarray, np.ndarray]:
@@ -29,26 +30,23 @@ def _csr(sets: Sequence[Sequence[int]]) -> Tuple[np.ndarray, np.ndarray]:
     return indptr, ids
 
 
-def _p(a: np.ndarray, t):
-    return a.ctypes.data_as(C.POINTER(t))
+def _empty_topk(k: int):
+    return np.zeros((0, k), np.float32), np.zeros((0, k), np.int64), np.zeros((0, k), np.int32), np.zeros((0, k), np.int32)
 
 
-class JaccardIndex:
+class JaccardIndex(_KvIndex):
+    _jaccard = True
+
     def __init__(self, vocab_size: int, device: int = 0, row_base: int = 0):
-        h = C.c_void_p()
-        _capi.check(_capi.load().kv_index_create(device, row_base, C.byref(h)))
-        self._h, self.vocab_size, self.device = h, int(vocab_size), device
+        super().__init__(device, row_base)
+        self.vocab_size = int(vocab_size)
         # the appended rows, for the counts of self-join pairs (the query of a self-join is a stored row)
         self._parts = []
-        _capi.check(_capi.load().kv_index_set_mode(h, 1))
 
     def add_csr(self, indptr: np.ndarray, ids: np.ndarray) -> None:
         indptr = np.ascontiguousarray(indptr, dtype=np.int64)
         ids = np.ascontiguousarray(ids, dtype=np.uint32)
-        tf = np.ones(len(ids), dtype=np.uint32)
-        _capi.check(_capi.load().kv_index_append(self._h, indptr.ctypes.data_as(C.POINTER(C.c_int64)),
-                                                 ids.ctypes.data_as(C.POINTER(C.c_uint32)),
-                                                 tf.ctypes.data_as(C.POINTER(C.c_uint32)), len(indptr) - 1))
+        self._append(indptr, ids, np.ones(len(ids), dtype=np.uint32), len(indptr) - 1)
         if len(indptr) > 1:
             self._parts.append((np.diff(indptr), ids[indptr[0]:indptr[-1]].copy()))
 
@@ -81,23 +79,17 @@ class JaccardIndex:
         self.add_csr(*_csr(sets))
 
     def finalize(self) -> None:
-        _capi.check(_capi.load().kv_index_finalize(self._h, self.vocab_size))
-
-    @property
-    def n_rows(self) -> int:
-        return int(_capi.load().kv_index_rows(self._h))
+        self._finalize(self.vocab_size)
 
     def topk_csr(self, indptr: np.ndarray, ids: np.ndarray, k: int = 16, distinct: bool = False):
         """(scores float32 [Q,k], rows int64 [Q,k], inter int32 [Q,k], union int32 [Q,k])."""
         no_distinct(distinct, "JaccardIndex.topk_csr")
-        lib = _capi.load()
         indptr, ids, oov = self._strip_oov(indptr, ids)
         n = len(indptr) - 1
-        tf = np.ones(len(ids), dtype=np.uint32)
-        scores = np.empty((n, k), dtype=np.float32)
-        rows = np.empty((n, k), dtype=np.int64)
-        _capi.check(lib.kv_topk(self._h, _p(indptr, C.c_int64), _p(ids, C.c_uint32), _p(tf, C.c_uint32), _p(oov, C.c_double), n, k,
-                                _p(scores, C.c_float), _p(rows, C.c_int64)))
+        if n == 0:
+            return _empty_topk(k)
+        self._upload(indptr, ids, np.ones(len(ids), dtype=np.uint32), oov, n)
+        scores, rows = self.topk_resident_host(n, k)
         inter, union = self._counts(indptr, ids, oov, rows)
         return scores, rows, inter, union
 
@@ -105,8 +97,8 @@ class JaccardIndex:
         n, k = rows.shape
         inter = np.empty((n, k), dtype=np.int32)
         union = np.empty((n, k), dtype=np.int32)
-        _capi.check(_capi.load().kv_jaccard_counts(self._h, _p(indptr, C.c_int64), _p(ids, C.c_uint32), _p(oov, C.c_double), n, k,
-                                                   _p(rows, C.c_int64), _p(inter, C.c_int32), _p(union, C.c_int32)))
+        _capi.check(_capi.load().kv_jaccard_counts(self._h, _ptr(indptr, C.c_int64), _ptr(ids, C.c_uint32), _ptr(oov, C.c_double), n, k,
+                                                   _ptr(rows, C.c_int64), _ptr(inter, C.c_int32), _ptr(union, C.c_int32)))
         return inter, union
 
     def counts_csr(self, indptr: np.ndarray, ids: np.ndarray, rows: np.ndarray):
@@ -118,29 +110,6 @@ class JaccardIndex:
         no_distinct(distinct, "JaccardIndex.topk_sets")
         return self.topk_csr(*_csr(queries), k=k)
 
-    def _range_resident(self, n_q: int, threshold: float, device_out: bool = False):
-        lib = _capi.load()
-        n = C.c_int64(0)
-        _capi.check(lib.kv_jaccard_range_resident(self._h, np.float32(threshold), C.byref(n)))
-        if device_out:
-            out = _devout.range_arrays(self.device, n_q, n.value, jaccard=True)
-            _capi.check(lib.kv_jaccard_range_fetch_device(self._h, *_devout.ptrs(out)))
-            return out
-        indptr = np.empty(n_q + 1, dtype=np.int64)
-        rows = np.empty(n.value, dtype=np.int64)
-        scores = np.empty(n.value, dtype=np.float32)
-        inter = np.empty(n.value, dtype=np.int32)
-        union = np.empty(n.value, dtype=np.int32)
-        _capi.check(lib.kv_jaccard_range_fetch(self._h, _p(indptr, C.c_int64), _p(rows, C.c_int64), _p(scores, C.c_float),
-                                               _p(inter, C.c_int32), _p(union, C.c_int32)))
-        return indptr, rows, scores, inter, union
-
-    def _empty_range(self, device_out: bool = False):
-        if device_out:
-            return _devout.empty_range(self.device, jaccard=True)
-        return (np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32), np.zeros(0, np.int32),
-                np.zeros(0, np.int32))
-
     def range_csr(self, indptr: np.ndarray, ids: np.ndarray, threshold: float, device_out: bool = False):
         """Threshold search: every (query, row) pair whose float32 score (the value ``topk_csr`` reports) is
         >= ``threshold``, 0 < threshold <= 1.  Returns ``(indptr int64[Q+1], rows int64[P], scores float32[P],
@@ -151,9 +120,7 @@ class JaccardIndex:
         n = len(indptr) - 1
         if n == 0:
             return self._empty_range(device_out)
-        tf = np.ones(len(ids), dtype=np.uint32)
-        _capi.check(_capi.load().kv_query_upload(self._h, _p(indptr, C.c_int64), _p(ids, C.c_uint32), _p(tf, C.c_uint32),
-                                                 _p(oov, C.c_double), n))
+        self._upload(indptr, ids, np.ones(len(ids), dtype=np.uint32), oov, n)
         return self._range_resident(n, threshold, device_out)
 
     def range_sets(self, queries: Sequence[Sequence[int]], threshold: float, device_out: bool = False):
@@ -166,14 +133,10 @@ class JaccardIndex:
         no_distinct(distinct, "JaccardIndex.selfjoin_topk")
         hi = self.n_rows if hi is None else hi
         if hi <= lo:
-            return (np.zeros((0, k), np.float32), np.zeros((0, k), np.int64), np.zeros((0, k), np.int32),
-                    np.zeros((0, k), np.int32))
-        lib = _capi.load()
+            return _empty_topk(k)
         n = hi - lo
-        _capi.check(lib.kv_selfjoin_upload(self._h, lo, hi))
-        scores = np.empty((n, k), dtype=np.float32)
-        rows = np.empty((n, k), dtype=np.int64)
-        _capi.check(lib.kv_topk_resident_host(self._h, k, _p(scores, C.c_float), _p(rows, C.c_int64)))
+        self._selfjoin_upload(lo, hi)
+        scores, rows = self.topk_resident_host(n, k)
         indptr, ids = self._rows_csr(lo, hi)
         inter, union = self._counts(indptr, ids, np.zeros(n, np.float64), rows)
         return scores, rows, inter, union
@@ -184,21 +147,5 @@ class JaccardIndex:
         hi = self.n_rows if hi is None else hi
         if hi <= lo:
             return self._empty_range(device_out)
-        _capi.check(_capi.load().kv_selfjoin_upload(self._h, lo, hi))
+        self._selfjoin_upload(lo, hi)
         return self._range_resident(hi - lo, threshold, device_out)
-
-    def last_timing_ms(self):
-        ms = (C.c_float * 4)()
-        _capi.check(_capi.load().kv_index_last_timing(self._h, ms))
-        return tuple(ms)
-
-    def close(self) -> None:
-        if self._h is not None:
-            _capi.load().kv_index_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass

@@ -230,7 +230,91 @@ class Vocabulary:
             pass
 
 
-class GfkbIndex:
+class _KvIndex:
+    """One ``kv_index`` handle on one device, the plumbing shared by ``GfkbIndex`` (TF-IDF) and ``JaccardIndex`` (token
+    sets): create and destroy, append, finalize, the resident query batch, its top-k read back to the host and its
+    threshold search.  A subclass with ``_jaccard = True`` runs the handle in Jaccard mode, whose threshold search also
+    returns the exact counts of every pair."""
+
+    _jaccard = False
+    _h = None
+
+    def __init__(self, device: int, row_base: int):
+        lib = _capi.load()
+        h = C.c_void_p()
+        _capi.check(lib.kv_index_create(device, row_base, C.byref(h)))
+        self._h, self.device, self.row_base = h, device, row_base
+        if self._jaccard:
+            _capi.check(lib.kv_index_set_mode(h, 1))
+
+    def _append(self, indptr: np.ndarray, ids: np.ndarray, tf: np.ndarray, n: int) -> None:
+        _capi.check(_capi.load().kv_index_append(self._h, _ptr(indptr, C.c_int64), _ptr(ids, C.c_uint32),
+                                                 _ptr(tf, C.c_uint32), n))
+
+    def _finalize(self, vocab_size: int) -> None:
+        _capi.check(_capi.load().kv_index_finalize(self._h, vocab_size))
+
+    @property
+    def n_rows(self) -> int:
+        return int(_capi.load().kv_index_rows(self._h))
+
+    def _upload(self, indptr: np.ndarray, ids: np.ndarray, tf: np.ndarray, oov: np.ndarray, n: int) -> None:
+        """Make a query CSR of n >= 1 queries the resident batch (host prep + H2D)."""
+        _capi.check(_capi.load().kv_query_upload(self._h, _ptr(indptr, C.c_int64), _ptr(ids, C.c_uint32),
+                                                 _ptr(tf, C.c_uint32), _ptr(oov, C.c_double), n))
+
+    def _selfjoin_upload(self, lo: int, hi: int) -> None:
+        _capi.check(_capi.load().kv_selfjoin_upload(self._h, lo, hi))
+
+    def topk_resident_host(self, n_q: int, k: int) -> Tuple[np.ndarray, np.ndarray]:
+        """Scan + merge of the resident batch of ``n_q`` queries, results copied to the host."""
+        scores = np.empty((n_q, k), dtype=np.float32)
+        rows = np.empty((n_q, k), dtype=np.int64)
+        _capi.check(_capi.load().kv_topk_resident_host(self._h, k, _ptr(scores, C.c_float), _ptr(rows, C.c_int64)))
+        return scores, rows
+
+    def _range_resident(self, n_q: int, threshold: float, device_out: bool = False):
+        """Threshold search of the resident batch of ``n_q`` queries: ``(indptr, rows, scores)``, and on a Jaccard
+        index ``inter, union`` after them, as NumPy arrays or (``device_out``) torch tensors on the index's device."""
+        lib = _capi.load()
+        n = C.c_int64(0)
+        _capi.check(lib.kv_range_resident(self._h, np.float32(threshold), C.byref(n)))
+        if device_out:
+            out = _devout.range_arrays(self.device, n_q, n.value, jaccard=self._jaccard)
+            _capi.check(lib.kv_range_fetch_device(self._h, *_devout.ptrs(out), *[None] * (5 - len(out))))
+            return out
+        out = (np.empty(n_q + 1, dtype=np.int64), np.empty(n.value, dtype=np.int64), np.empty(n.value, dtype=np.float32))
+        counts = (np.empty(n.value, dtype=np.int32), np.empty(n.value, dtype=np.int32)) if self._jaccard else ()
+        _capi.check(lib.kv_range_fetch(self._h, _ptr(out[0], C.c_int64), _ptr(out[1], C.c_int64), _ptr(out[2], C.c_float),
+                                       *([_ptr(c, C.c_int32) for c in counts] or [None, None])))
+        return out + counts
+
+    def _empty_range(self, device_out: bool = False):
+        """The threshold search result of no queries."""
+        if device_out:
+            return _devout.empty_range(self.device, jaccard=self._jaccard)
+        out = (np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32))
+        return out + (np.zeros(0, np.int32), np.zeros(0, np.int32)) if self._jaccard else out
+
+    def last_timing_ms(self) -> Tuple[float, float, float, float]:
+        """CUDA-event ms of the last upload and top-k: H2D of the batch, bound + scan kernels, merge, D2H."""
+        ms = (C.c_float * 4)()
+        _capi.check(_capi.load().kv_index_last_timing(self._h, ms))
+        return tuple(ms)
+
+    def close(self) -> None:
+        if self._h is not None:
+            _capi.load().kv_index_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class GfkbIndex(_KvIndex):
     """Resident TF-IDF index of one row shard of the GFKB on one H100.
 
     ``row_base`` is the global index of the shard's first row; ``vocab`` may be shared between
@@ -239,13 +323,8 @@ class GfkbIndex:
     """
 
     def __init__(self, device: int = 0, row_base: int = 0, vocab: Optional[Vocabulary] = None):
-        lib = _capi.load()
         self.vocab = vocab if vocab is not None else Vocabulary()
-        h = C.c_void_p()
-        _capi.check(lib.kv_index_create(device, row_base, C.byref(h)))
-        self._h = h
-        self.device = device
-        self.row_base = row_base
+        super().__init__(device, row_base)
         self._row_labels: Optional[np.ndarray] = None  # what set_row_labels gave, until the next append
         self._group_rows: Optional[int] = None  # rows set_row_groups described, until the next append
 
@@ -254,9 +333,7 @@ class GfkbIndex:
         hi = fb.n if hi is None else hi
         if hi <= lo:
             return
-        ip = np.ascontiguousarray(fb.indptr[lo:hi + 1])
-        _capi.check(_capi.load().kv_index_append(self._h, _ptr(ip, C.c_int64), _ptr(fb.ids, C.c_uint32),
-                                                 _ptr(fb.tf, C.c_uint32), hi - lo))
+        self._append(np.ascontiguousarray(fb.indptr[lo:hi + 1]), fb.ids, fb.tf, hi - lo)
         self._row_labels = None  # the library drops the labels (and the groups) on an append
         self._group_rows = None
 
@@ -312,16 +389,12 @@ class GfkbIndex:
         _capi.check(_capi.load().kv_index_set_mode(self._h, int(mode)))
 
     def finalize(self) -> None:
-        _capi.check(_capi.load().kv_index_finalize(self._h, len(self.vocab)))
+        self._finalize(len(self.vocab))
 
     @property
     def last_finalize_kind(self) -> int:
         """1 = full rebuild, 2 = statistics-only refresh (rows unchanged, only global N / df moved)."""
         return int(_capi.load().kv_index_last_finalize_kind(self._h))
-
-    @property
-    def n_rows(self) -> int:
-        return int(_capi.load().kv_index_rows(self._h))
 
     def delete_rows(self, rows) -> None:
         """Delete local ``rows`` (any order; duplicates and rows deleted before are allowed).  A deleted row keeps its
@@ -364,32 +437,21 @@ class GfkbIndex:
                       distinct: bool = False) -> Tuple[np.ndarray, np.ndarray]:
         """``labels``: per query the row label its results must carry (-1: any row), see ``set_filter``.  ``distinct``:
         at most one row per group (``set_row_groups``), see ``set_distinct``."""
-        if labels is not None or distinct:
-            if fb.n == 0:
-                return np.zeros((0, k), np.float32), np.zeros((0, k), np.int64)
-            self.upload_queries(fb)
-            if labels is not None:
-                self.set_filter(labels)
-            if distinct:
-                self.set_distinct(True)
-            return self.topk_resident_host(fb.n, k)
-        scores = np.empty((fb.n, k), dtype=np.float32)
-        rows = np.empty((fb.n, k), dtype=np.int64)
-        _capi.check(_capi.load().kv_topk(self._h, _ptr(fb.indptr, C.c_int64), _ptr(fb.ids, C.c_uint32),
-                                         _ptr(fb.tf, C.c_uint32), _ptr(fb.oov, C.c_double), fb.n, k,
-                                         _ptr(scores, C.c_float), _ptr(rows, C.c_int64)))
-        return scores, rows
+        if fb.n == 0:
+            return np.zeros((0, k), np.float32), np.zeros((0, k), np.int64)
+        self.upload_queries(fb)
+        return self._topk_uploaded(fb.n, k, labels, distinct)
 
-    def topk_features_device(self, fb: FeatureBatch, k: int, d_scores_ptr: int, d_rows_ptr: int) -> None:
-        """Results stay on the device: float32[n,k] / int64[n,k] buffers owned by the caller."""
-        _capi.check(_capi.load().kv_topk_device(self._h, _ptr(fb.indptr, C.c_int64), _ptr(fb.ids, C.c_uint32),
-                                                _ptr(fb.tf, C.c_uint32), _ptr(fb.oov, C.c_double), fb.n, k,
-                                                C.c_void_p(d_scores_ptr), C.c_void_p(d_rows_ptr)))
+    def _topk_uploaded(self, n_q: int, k: int, labels: Optional[np.ndarray], distinct: bool):
+        if labels is not None:
+            self.set_filter(labels)
+        if distinct:
+            self.set_distinct(True)
+        return self.topk_resident_host(n_q, k)
 
     def upload_queries(self, fb: FeatureBatch) -> None:
         """Make a featurised batch resident on the device (host prep + H2D), for topk_resident."""
-        _capi.check(_capi.load().kv_query_upload(self._h, _ptr(fb.indptr, C.c_int64), _ptr(fb.ids, C.c_uint32),
-                                                 _ptr(fb.tf, C.c_uint32), _ptr(fb.oov, C.c_double), fb.n))
+        self._upload(fb.indptr, fb.ids, fb.tf, fb.oov, fb.n)
 
     def upload_text(self, data, offsets: np.ndarray, mode: int) -> int:
         """``upload_queries(vocab.featurize_packed(data, offsets, mode, grow=False))`` done on the device: the text goes
@@ -481,15 +543,8 @@ class GfkbIndex:
         of them.  Scores are the non-distinct ones; threshold searches ignore the mode."""
         _capi.check(_capi.load().kv_query_set_distinct(self._h, 1 if on else 0))
 
-    def topk_resident_host(self, n_q: int, k: int) -> Tuple[np.ndarray, np.ndarray]:
-        """Scan + merge of the resident batch of ``n_q`` queries, results copied to the host."""
-        scores = np.empty((n_q, k), dtype=np.float32)
-        rows = np.empty((n_q, k), dtype=np.int64)
-        _capi.check(_capi.load().kv_topk_resident_host(self._h, k, _ptr(scores, C.c_float), _ptr(rows, C.c_int64)))
-        return scores, rows
-
-    def _selfjoin_upload(self, lo: int, hi: int, same_label: bool) -> None:
-        _capi.check(_capi.load().kv_selfjoin_upload(self._h, lo, hi))
+    def _selfjoin_upload(self, lo: int, hi: int, same_label: bool = False) -> None:
+        super()._selfjoin_upload(lo, hi)
         if same_label:
             if self._row_labels is None or len(self._row_labels) != self.n_rows:
                 raise RuntimeError("same_label: the index has no row labels for its current rows (set_row_labels)")
@@ -508,25 +563,6 @@ class GfkbIndex:
             self.set_distinct(True)
         return self.topk_resident_host(hi - lo, k)
 
-    def _range_resident(self, n_q: int, threshold: float, device_out: bool = False):
-        lib = _capi.load()
-        n = C.c_int64(0)
-        _capi.check(lib.kv_range_resident(self._h, np.float32(threshold), C.byref(n)))
-        if device_out:
-            out = _devout.range_arrays(self.device, n_q, n.value)
-            _capi.check(lib.kv_range_fetch_device(self._h, *_devout.ptrs(out)))
-            return out
-        indptr = np.empty(n_q + 1, dtype=np.int64)
-        rows = np.empty(n.value, dtype=np.int64)
-        scores = np.empty(n.value, dtype=np.float32)
-        _capi.check(lib.kv_range_fetch(self._h, _ptr(indptr, C.c_int64), _ptr(rows, C.c_int64), _ptr(scores, C.c_float)))
-        return indptr, rows, scores
-
-    def _empty_range(self, device_out: bool):
-        if device_out:
-            return _devout.empty_range(self.device)
-        return np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32)
-
     def range_features(self, fb: FeatureBatch, threshold: float, device_out: bool = False,
                        labels: Optional[np.ndarray] = None):
         """Threshold search: every (query, row) pair whose float32 score (the value ``topk`` reports) is >= ``threshold``,
@@ -537,18 +573,18 @@ class GfkbIndex:
         if fb.n == 0:
             return self._empty_range(device_out)
         self.upload_queries(fb)
+        return self._range_uploaded(fb.n, threshold, device_out, labels)
+
+    def _range_uploaded(self, n_q: int, threshold: float, device_out: bool, labels: Optional[np.ndarray]):
         if labels is not None:
             self.set_filter(labels)
-        return self._range_resident(fb.n, threshold, device_out)
+        return self._range_resident(n_q, threshold, device_out)
 
     def range(self, queries: Sequence[str], threshold: float, device_out: bool = False,
               labels: Optional[np.ndarray] = None):
         """``range_features`` of texts."""
         if len(queries) and _featurize_on_device(len(queries)):
-            self.upload_text(*pack_texts(queries))
-            if labels is not None:
-                self.set_filter(labels)
-            return self._range_resident(len(queries), threshold, device_out)
+            return self._range_uploaded(self.upload_text(*pack_texts(queries)), threshold, device_out, labels)
         fb = self.vocab.featurize(queries, grow=False)
         try:
             return self.range_features(fb, threshold, device_out, labels)
@@ -597,22 +633,12 @@ class GfkbIndex:
         the row label its results must carry (-1: any row).  ``distinct``: at most one row per group (the best one;
         ``set_row_groups``)."""
         if len(queries) and _featurize_on_device(len(queries)):
-            self.upload_text(*pack_texts(queries))
-            if labels is not None:
-                self.set_filter(labels)
-            if distinct:
-                self.set_distinct(True)
-            return self.topk_resident_host(len(queries), k)
+            return self._topk_uploaded(self.upload_text(*pack_texts(queries)), k, labels, distinct)
         fb = self.vocab.featurize(queries, grow=False)
         try:
             return self.topk_features(fb, k, labels, distinct)
         finally:
             fb.close()
-
-    def last_timing_ms(self) -> Tuple[float, float, float, float]:
-        ms = (C.c_float * 4)()
-        _capi.check(_capi.load().kv_index_last_timing(self._h, ms))
-        return tuple(ms)
 
     def last_score_ms(self) -> float:
         ms = C.c_float()
@@ -654,17 +680,6 @@ class GfkbIndex:
             return False
         _capi.check(rc)
         return True
-
-    def close(self) -> None:
-        if self._h is not None:
-            _capi.load().kv_index_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 @dataclass

@@ -6,10 +6,10 @@ tokens swapped.  QUERIES (2048): half fresh sets of the same generator, half nea
 swaps), so that theta in {0.5, 0.7, 0.9} returns a non-trivial number of pairs.
 
 Times, in one process and alternated per round after a warm-up round (which also grows the pair buffer): K3 top-16
-(`kv_topk_resident_host`, kernel = CUDA events around the scan) against K3-R (`kv_jaccard_range_resident`, kernel =
+(`kv_topk_resident_host`, kernel = CUDA events around the scan) against K3-R (`kv_range_resident`, kernel =
 `kv_index_last_kernel_ms()[3]`, irregular-query fallbacks [4]) on the same uploaded batch, the host clock around
-`kv_jaccard_range_fetch` (ordering on the device, arrays copied back) and, for the same search run again, around
-`kv_jaccard_range_fetch_device` (arrays left in device memory; the digests must agree), and the self-join of the first
+`kv_range_fetch` (ordering on the device, arrays copied back) and, for the same search run again, around
+`kv_range_fetch_device` (arrays left in device memory; the digests must agree), and the self-join of the first
 `--selfjoin` (200k) sets as an index of their own: self-join top-16 against the self-join range at each theta."""
 import ctypes as C
 import hashlib
@@ -92,22 +92,22 @@ def range_timed(jx, n_q, theta):
     batch twice, fetched to host memory (ordering on the device, arrays copied back) and then to device memory."""
     cnt = C.c_int64(0)
     t0 = time.perf_counter()
-    _capi.check(lib.kv_jaccard_range_resident(jx._h, C.c_float(theta), C.byref(cnt)))
+    _capi.check(lib.kv_range_resident(jx._h, C.c_float(theta), C.byref(cnt)))
     t1 = time.perf_counter()
     ms = kernel_ms(jx)
     m = cnt.value
     out = [np.empty(n_q + 1, np.int64), np.empty(max(m, 1), np.int64), np.empty(max(m, 1), np.float32),
            np.empty(max(m, 1), np.int32), np.empty(max(m, 1), np.int32)]
     t2 = time.perf_counter()
-    _capi.check(lib.kv_jaccard_range_fetch(jx._h, p(out[0], C.c_int64), p(out[1], C.c_int64), p(out[2], C.c_float),
-                                           p(out[3], C.c_int32), p(out[4], C.c_int32)))
+    _capi.check(lib.kv_range_fetch(jx._h, p(out[0], C.c_int64), p(out[1], C.c_int64), p(out[2], C.c_float),
+                                   p(out[3], C.c_int32), p(out[4], C.c_int32)))
     t3 = time.perf_counter()
     d_host = digest([out[0]] + [a[:m] for a in out[1:]])
-    _capi.check(lib.kv_jaccard_range_resident(jx._h, C.c_float(theta), C.byref(cnt)))
+    _capi.check(lib.kv_range_resident(jx._h, C.c_float(theta), C.byref(cnt)))
     dout = _devout.range_arrays(0, n_q, cnt.value, jaccard=True)
     torch.cuda.synchronize()
     t4 = time.perf_counter()
-    _capi.check(lib.kv_jaccard_range_fetch_device(jx._h, *_devout.ptrs(dout)))
+    _capi.check(lib.kv_range_fetch_device(jx._h, *_devout.ptrs(dout)))
     t5 = time.perf_counter()
     assert digest([a.cpu().numpy() for a in dout]) == d_host
     return m, ms[3], ms[4], 1e3 * (t1 - t0), 1e3 * (t3 - t2), 1e3 * (t5 - t4), d_host

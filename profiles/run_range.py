@@ -69,7 +69,8 @@ def fetch_host(m):
     scores = np.empty(max(m, 1), np.float32)
     t0 = time.perf_counter()
     _capi.check(lib.kv_range_fetch(ix._h, indptr.ctypes.data_as(C.POINTER(C.c_int64)),
-                                   rows.ctypes.data_as(C.POINTER(C.c_int64)), scores.ctypes.data_as(C.POINTER(C.c_float))))
+                                   rows.ctypes.data_as(C.POINTER(C.c_int64)), scores.ctypes.data_as(C.POINTER(C.c_float)),
+                                   None, None))
     t1 = time.perf_counter()
     return digest(indptr, rows[:m], scores[:m]), t1 - t0
 
@@ -78,7 +79,7 @@ def fetch_device(m):
     out = _devout.range_arrays(0, q, m)
     torch.cuda.synchronize()
     t0 = time.perf_counter()
-    _capi.check(lib.kv_range_fetch_device(ix._h, *_devout.ptrs(out)))
+    _capi.check(lib.kv_range_fetch_device(ix._h, *_devout.ptrs(out), None, None))
     t1 = time.perf_counter()
     return digest(*(t.cpu().numpy() for t in out)), t1 - t0
 

@@ -1,4 +1,4 @@
-"""Jaccard threshold search (kv_jaccard_range_resident / kv_jaccard_range_fetch, JaccardIndex.range_* and
+"""Jaccard threshold search (kv_range_resident / kv_range_fetch on a Jaccard index, JaccardIndex.range_* and
 selfjoin_*) and pattern clustering of token sets on the exact threshold graph (detect_patterns(JaccardIndex, k=None)).
 
 The oracle is exact: (|q ∩ r|, |q ∪ r|) from ``oracle.tfidf_oracle.jaccard_sets`` (a scipy product of the binary
@@ -284,23 +284,21 @@ def test_jaccard_patterns_on_the_threshold_graph(lib):
     jx.close()
 
 
-def _fetch(lib, h, n_q, n, fn="kv_jaccard_range_fetch"):
+def _fetch(lib, h, n_q, n, counts=True):
+    """kv_range_fetch with the count outputs of a Jaccard index, or (counts=False) with NULL ones as on a TF-IDF index."""
     from kakveda_b200 import _capi
 
     indptr = np.empty(n_q + 1, np.int64)
     rows, scores = np.empty(max(n, 1), np.int64), np.empty(max(n, 1), np.float32)
     inter, union = np.empty(max(n, 1), np.int32), np.empty(max(n, 1), np.int32)
     p = lambda a, t: a.ctypes.data_as(C.POINTER(t))
-    if fn == "kv_range_fetch":
-        _capi.check(lib.kv_range_fetch(h, p(indptr, C.c_int64), p(rows, C.c_int64), p(scores, C.c_float)))
-    else:
-        _capi.check(lib.kv_jaccard_range_fetch(h, p(indptr, C.c_int64), p(rows, C.c_int64), p(scores, C.c_float),
-                                               p(inter, C.c_int32), p(union, C.c_int32)))
+    _capi.check(lib.kv_range_fetch(h, p(indptr, C.c_int64), p(rows, C.c_int64), p(scores, C.c_float),
+                                   p(inter, C.c_int32) if counts else None, p(union, C.c_int32) if counts else None))
     return indptr
 
 
 @pytest.mark.gpu
-def test_jaccard_range_state_and_errors(medium):
+def test_jaccard_range_fetch_counts_and_state(medium):
     from kakveda_b200 import GfkbIndex, JaccardIndex, _capi
     from kakveda_b200.jaccardindex import _csr
 
@@ -318,32 +316,36 @@ def test_jaccard_range_state_and_errors(medium):
     with pytest.raises(RuntimeError):
         _fetch(lib, jx._h, 8, 0)
     n = C.c_int64(0)
-    _capi.check(lib.kv_jaccard_range_resident(jx._h, C.c_float(0.5), C.byref(n)))
+    _capi.check(lib.kv_range_resident(jx._h, C.c_float(0.5), C.byref(n)))
     assert n.value > 0
-    with pytest.raises(RuntimeError):          # the TF-IDF fetch never reads a Jaccard result
-        _fetch(lib, jx._h, 8, n.value, fn="kv_range_fetch")
-    with pytest.raises(ValueError):            # nor does the TF-IDF search run on a Jaccard index
-        _capi.check(lib.kv_range_resident(jx._h, C.c_float(0.5), C.byref(n)))
-    _capi.check(lib.kv_jaccard_range_resident(jx._h, C.c_float(0.5), C.byref(n)))
+    with pytest.raises(ValueError):            # a Jaccard result is fetched with its counts
+        _fetch(lib, jx._h, 8, n.value, counts=False)
+    indptr = _fetch(lib, jx._h, 8, n.value)    # the rejected fetch left the result
+    assert indptr[-1] == n.value
+    _capi.check(lib.kv_range_resident(jx._h, C.c_float(0.5), C.byref(n)))
     upload()                                   # a new upload drops the result
     with pytest.raises(RuntimeError):
         _fetch(lib, jx._h, 8, n.value)
-    _capi.check(lib.kv_jaccard_range_resident(jx._h, C.c_float(0.5), C.byref(n)))
+    _capi.check(lib.kv_range_resident(jx._h, C.c_float(0.5), C.byref(n)))
     indptr = _fetch(lib, jx._h, 8, n.value)
     assert indptr[-1] == n.value
     with pytest.raises(RuntimeError):          # fetched once
         _fetch(lib, jx._h, 8, n.value)
-    # the Jaccard functions on a TF-IDF index
+    # count outputs on a TF-IDF index
     tx = GfkbIndex()
     tx.add_texts(["alpha beta gamma", "beta gamma delta", "epsilon zeta"])
     tx.finalize()
-    fb = tx.vocab.featurize(["alpha beta"], grow=False)
+    fb = tx.vocab.featurize(["alpha beta gamma"], grow=False)
     tx.upload_queries(fb)
     fb.close()
-    with pytest.raises(ValueError):
-        _capi.check(lib.kv_jaccard_range_resident(tx._h, C.c_float(0.5), C.byref(n)))
-    with pytest.raises(ValueError):
+    with pytest.raises(ValueError):            # no result yet, and the outputs do not fit the mode
         _fetch(lib, tx._h, 1, 0)
+    _capi.check(lib.kv_range_resident(tx._h, C.c_float(0.5), C.byref(n)))
+    assert n.value > 0
+    with pytest.raises(ValueError):
+        _fetch(lib, tx._h, 1, n.value)
+    indptr = _fetch(lib, tx._h, 1, n.value, counts=False)   # the rejected fetch left the result
+    assert indptr[-1] == n.value
     tx.close()
     # an empty index: empty CSR arrays
     empty = JaccardIndex(16)

@@ -207,7 +207,7 @@ def test_append_then_finalize_equals_fresh_build(lib):
     np.testing.assert_allclose(b, O.score_matrix_closed_form([q[2]], corpus[:100])[0], rtol=RTOL64, atol=1e-15)
 
 
-def test_sharded_equals_unsharded_on_one_gpu(lib):
+def test_sharded_resident_topk_equals_unsharded_on_one_gpu(lib):
     """Row shards with the global df + K5 merge reproduce the single-index result bit for bit."""
     import ctypes as C
 
@@ -239,7 +239,8 @@ def test_sharded_equals_unsharded_on_one_gpu(lib):
     for s, ix in enumerate(parts):
         ix.set_global_df(df.astype(np.uint32), n)
         ix.finalize()
-        ix.topk_features_device(qfb, k, ds[s].data_ptr(), dr[s].data_ptr())
+        ix.upload_queries(qfb)
+        ix.topk_resident(k, ds[s].data_ptr(), dr[s].data_ptr())
     out_s = torch.empty((q, k), dtype=torch.float32, device="cuda")
     out_r = torch.empty((q, k), dtype=torch.int64, device="cuda")
     _capi.check(_capi.load().kv_merge_topk_device(0, C.c_void_p(ds.data_ptr()), C.c_void_p(dr.data_ptr()), shards, q, k,

@@ -253,7 +253,7 @@ def test_range_leaves_the_batch_state_alone(medium):
 
 
 @pytest.mark.gpu
-def test_range_errors(medium):
+def test_range_errors_and_fetch_outputs(medium):
     from kakveda_b200 import GfkbIndex, _capi
 
     ix, corpus, queries, oracle = medium
@@ -285,7 +285,7 @@ def test_range_errors(medium):
     with pytest.raises(RuntimeError):
         _capi.check(_capi.load().kv_range_fetch(ix._h, indptr.ctypes.data_as(C.POINTER(C.c_int64)),
                                                 rows.ctypes.data_as(C.POINTER(C.c_int64)),
-                                                scores.ctypes.data_as(C.POINTER(C.c_float))))
+                                                scores.ctypes.data_as(C.POINTER(C.c_float)), None, None))
     empty = GfkbIndex()
     empty.finalize()
     indptr, rows, scores = empty.range(["alpha beta", "gamma"], 0.5)

@@ -369,7 +369,7 @@ def test_cluster_csr_device_edge_cases(lib):
 # ---- errors ---------------------------------------------------------------------------------------------------------
 
 @pytest.mark.gpu
-def test_device_entry_points_reject_bad_pointers(tfidf, lib):
+def test_device_fetch_rejects_bad_pointers_and_outputs(tfidf, lib):
     import torch
 
     from kakveda_b200 import DenseIndex, JaccardIndex, _capi
@@ -388,42 +388,49 @@ def test_device_entry_points_reject_bad_pointers(tfidf, lib):
         args = [vp(d) for d in dev]
         args[i] = vp(host[i])
         with pytest.raises(ValueError):
-            _capi.check(lib.kv_range_fetch_device(ix._h, *args))
+            _capi.check(lib.kv_range_fetch_device(ix._h, *args, None, None))
     spare = torch.empty(n.value + 1, dtype=torch.int64, device="cuda")
     with pytest.raises(ValueError):                        # misaligned rows
-        _capi.check(lib.kv_range_fetch_device(ix._h, vp(dev[0]), C.c_void_p(spare.data_ptr() + 4), vp(dev[2])))
-    with pytest.raises(ValueError):                        # the Jaccard fetch on a TF-IDF index
-        _capi.check(lib.kv_jaccard_range_fetch_device(ix._h, *[vp(d) for d in dev], vp(dev[2]), vp(dev[2])))
+        _capi.check(lib.kv_range_fetch_device(ix._h, vp(dev[0]), C.c_void_p(spare.data_ptr() + 4), vp(dev[2]), None, None))
+    with pytest.raises(ValueError):                        # count outputs on a TF-IDF index
+        _capi.check(lib.kv_range_fetch_device(ix._h, *[vp(d) for d in dev], vp(dev[2]), vp(dev[2])))
     # rejected calls leave the result: the fetch still works, once
-    _capi.check(lib.kv_range_fetch_device(ix._h, *[vp(d) for d in dev]))
+    _capi.check(lib.kv_range_fetch_device(ix._h, *[vp(d) for d in dev], None, None))
     assert int(dev[0][-1]) == n.value
     with pytest.raises(RuntimeError):
-        _capi.check(lib.kv_range_fetch_device(ix._h, *[vp(d) for d in dev]))
+        _capi.check(lib.kv_range_fetch_device(ix._h, *[vp(d) for d in dev], None, None))
     # a re-upload drops the result
     _capi.check(lib.kv_range_resident(ix._h, C.c_float(0.3), C.byref(n)))
     ix.upload_queries(fb)
     fb.close()
     with pytest.raises(RuntimeError):
-        _capi.check(lib.kv_range_fetch_device(ix._h, *[vp(d) for d in dev]))
+        _capi.check(lib.kv_range_fetch_device(ix._h, *[vp(d) for d in dev], None, None))
 
-    # Jaccard: the TF-IDF fetch on a Jaccard index, host pointers, a re-upload
+    # Jaccard: no count outputs, host pointers, a re-upload
     jx = JaccardIndex(64)
     jx.add_sets([[1, 2, 3], [1, 2, 3, 4], [5, 6]])
     jx.finalize()
     jx.range_sets([[1, 2, 3]], 0.5)
     _capi.check(lib.kv_selfjoin_upload(jx._h, 0, 3))
-    _capi.check(lib.kv_jaccard_range_resident(jx._h, C.c_float(0.5), C.byref(n)))
+    _capi.check(lib.kv_range_resident(jx._h, C.c_float(0.5), C.byref(n)))
     assert n.value == 2
     jd = [torch.empty(4, dtype=torch.int64, device="cuda"), torch.empty(2, dtype=torch.int64, device="cuda"),
           torch.empty(2, dtype=torch.float32, device="cuda"), torch.empty(2, dtype=torch.int32, device="cuda"),
           torch.empty(2, dtype=torch.int32, device="cuda")]
     with pytest.raises(ValueError):
-        _capi.check(lib.kv_range_fetch_device(jx._h, *[vp(d) for d in jd[:3]]))
+        _capi.check(lib.kv_range_fetch_device(jx._h, *[vp(d) for d in jd[:3]], None, None))
     with pytest.raises(ValueError):
-        _capi.check(lib.kv_jaccard_range_fetch_device(jx._h, *[vp(d) for d in jd[:4]], vp(np.empty(2, np.int32))))
+        _capi.check(lib.kv_range_fetch_device(jx._h, *[vp(d) for d in jd[:4]], vp(np.empty(2, np.int32))))
+    # rejected calls leave the result: the fetch still works, once
+    _capi.check(lib.kv_range_fetch_device(jx._h, *[vp(d) for d in jd]))
+    assert jd[0].tolist() == [0, 1, 2, 2] and jd[1].tolist() == [1, 0] and jd[3].tolist() == [3, 3] and jd[4].tolist() == [4, 4]
+    with pytest.raises(RuntimeError):
+        _capi.check(lib.kv_range_fetch_device(jx._h, *[vp(d) for d in jd]))
+    # a re-upload drops the result
+    _capi.check(lib.kv_range_resident(jx._h, C.c_float(0.5), C.byref(n)))
     _capi.check(lib.kv_selfjoin_upload(jx._h, 0, 3))
     with pytest.raises(RuntimeError):
-        _capi.check(lib.kv_jaccard_range_fetch_device(jx._h, *[vp(d) for d in jd]))
+        _capi.check(lib.kv_range_fetch_device(jx._h, *[vp(d) for d in jd]))
     jx.close()
 
     # dense: host pointers, and a top-k call drops the result
