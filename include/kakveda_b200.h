@@ -350,6 +350,23 @@ int kv_merge_topk_device_on(int device, const void *d_scores_in, const void *d_r
                             int64_t n_q, int k, int64_t stride_s, int64_t stride_r, void *d_scores_out,
                             void *d_rows_out, void *stream, int sync);
 
+/* Merge of n_runs (1..64) threshold-search results over disjoint rows -- e.g. the row shards' results after ONE
+ * all-gather -- into the single result over all the rows.  Run w is a CSR as kv_range_fetch_device writes it:
+ * indptr int64[n_q+1] at d_indptr + w*indptr_stride elements, with indptr[0] = 0 and indptr[n_q] = run_pairs[w] (host
+ * array); rows int64 / scores float32 (and, for Jaccard results, inter / uni int32: both set or both NULL) at their
+ * base + w*rec_stride_bytes bytes (a multiple of 8); each query's segment ordered by (score desc, row asc).  Writes
+ * d_indptr_out int64[n_q+1] (the summed counts) and the pairs of every query, the union of its segments in the same
+ * order, to d_rows_out / d_scores_out (/ d_inter_out / d_uni_out), all device memory of `device` (the record
+ * arrays are not looked at when no run holds a pair).  Runs on `stream`
+ * (a cudaStream_t, e.g. the all-gather's; NULL = legacy default stream) and returns once the outputs and their
+ * validity are known.  KV_ERR_INVALID, after the fact, for a decreasing indptr, a count that does not match run_pairs,
+ * a segment out of order or a (score, row) key present in two runs (the outputs are then undefined); for pointers
+ * that are not device memory of `device` aligned to their element size.  KV_ERR_NOMEM for 2^32 - 1 pairs or more. */
+int kv_merge_range_device_on(int device, int n_runs, int64_t n_q, const void *d_indptr, int64_t indptr_stride,
+                             const void *d_rows, const void *d_scores, const void *d_inter, const void *d_uni,
+                             int64_t rec_stride_bytes, const int64_t *run_pairs, void *d_indptr_out, void *d_rows_out,
+                             void *d_scores_out, void *d_inter_out, void *d_uni_out, void *stream);
+
 /* Timing of the last query upload and top-k (kv_topk_resident, _host or _finish) on this handle, CUDA-event
  * milliseconds on its stream:
  * ms[0] = H2D of the query batch, ms[1] = bound + scan kernels, ms[2] = merge (+ fallbacks), ms[3] = D2H of host

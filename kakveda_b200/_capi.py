@@ -94,6 +94,9 @@ SIGNATURES = {
                                        C.c_void_p]),
     "kv_merge_topk_device_on": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int64,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "kv_merge_range_device_on": (C.c_int, [C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_int64, c_i64p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p]),
     "kv_index_last_timing": (C.c_int, [C.c_void_p, c_f32p]),
     "kv_index_last_kernel_ms": (C.c_int, [C.c_void_p, c_f32p]),
     "kv_index_last_score_ms": (C.c_int, [C.c_void_p, c_f32p]),

@@ -8,7 +8,10 @@ only exchanges are
   TF-IDF's idf and row norms use GLOBAL df and N (``allreduce_df``);
 * once per query batch: ONE all-gather of the per-shard partial top-k (scores float32, rows int64),
   followed by a local merge ordered by (score desc, row asc) -- identical on every rank
-  (``gather_topk`` + ``kv_merge_topk_device``).
+  (``gather_topk`` + ``kv_merge_topk_device``);
+* once per threshold search: a 16-byte all-gather of the shards' pair counts, ONE all-gather of the per-shard CSR
+  results packed in equal slots, and the W-way merge of the ordered runs on the device (``gather_range_packed`` +
+  ``merge_range_on_device``, ``kv_merge_range_device_on``).  The threshold is fixed, so every shard searches alone.
 
 Every rank featurises the whole corpus text so that feature ids agree without exchanging the
 vocabulary (ids are deterministic, see csrc/featurizer.cpp); only its own rows go to its GPU.
@@ -24,7 +27,7 @@ from typing import Optional, Tuple
 
 import numpy as np
 
-from . import _capi
+from . import _capi, _devout
 from ._capi import no_distinct
 from .similarity import FeatureBatch, GfkbIndex, Vocabulary, _featurize_on_device, gather_rows, text_order
 
@@ -124,6 +127,105 @@ def merge_packed_on_device(device: int, gathered, q: int, k: int):
     return out_s, out_r
 
 
+# ---- threshold search: variable-sized results ------------------------------------------------------------------------
+
+def range_layout(n_q: int, p_max: int, jaccard: bool = False) -> Tuple[Tuple[int, int, int, int, int], int]:
+    """Byte offsets of one rank's packed threshold-search result and its slot size: indptr int64[n_q+1] | rows
+    int64[p_max] | scores float32[p_max] (| inter int32[p_max] | union int32[p_max]), each 16-byte aligned."""
+    al = lambda x: (x + 15) & ~15
+    o_r = al(8 * (n_q + 1))
+    o_s = al(o_r + 8 * p_max)
+    o_i = al(o_s + 4 * p_max)
+    o_u = al(o_i + 4 * p_max)
+    return (0, o_r, o_s, o_i, o_u), (al(o_u + 4 * p_max) if jaccard else o_i)
+
+
+def range_views(buf, n_q: int, n_pairs: int, p_max: int, jaccard: bool = False):
+    """``(indptr, rows, scores[, inter, union])`` views of a packed slot (uint8 torch tensor) holding ``n_pairs`` pairs:
+    what ``kv_range_fetch_device`` writes into."""
+    import torch
+
+    offs, _ = range_layout(n_q, p_max, jaccard)
+    out = [buf[: 8 * (n_q + 1)].view(torch.int64), buf[offs[1]:offs[1] + 8 * n_pairs].view(torch.int64),
+           buf[offs[2]:offs[2] + 4 * n_pairs].view(torch.float32)]
+    if jaccard:
+        out += [buf[offs[3]:offs[3] + 4 * n_pairs].view(torch.int32), buf[offs[4]:offs[4] + 4 * n_pairs].view(torch.int32)]
+    return out
+
+
+def gather_range_packed(device: int, n_q: int, n_pairs: int, fill, group=None, jaccard: bool = False):
+    """The exchange of a sharded threshold search.  A 16-byte all-gather of (pairs, free device bytes) fixes the slot
+    size from the largest shard's count; ``fill(views)`` then writes this rank's CSR result into ``range_views`` of its
+    slot (no extra copy), and ONE all-gather carries every slot.  Returns ``([W, slot] uint8, pairs per rank)``.
+    Every rank checks that the gathered slots plus the merged result fit the device with the least free memory, so
+    they all raise the same ``MemoryError`` (with the pair counts) or none does."""
+    import torch
+    import torch.distributed as dist
+
+    dev = torch.device("cuda", device)
+    world = dist.get_world_size(group)
+    free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+    sizes = torch.tensor([n_pairs, free], dtype=torch.int64).to(dev)
+    all_sizes = torch.empty((world, 2), dtype=torch.int64, device=dev)
+    dist.all_gather_into_tensor(all_sizes.view(-1), sizes, group=group)
+    all_sizes = all_sizes.cpu().numpy()
+    pairs = all_sizes[:, 0].astype(np.int64)
+    p_max, total = int(pairs.max()), int(pairs.sum())
+    _, slot = range_layout(n_q, p_max, jaccard)
+    need = (world + 1) * slot + 8 * (n_q + 1) + total * (20 if jaccard else 12)
+    if need > int(all_sizes[:, 1].min()):
+        raise MemoryError(f"sharded threshold search: {pairs.tolist()} pairs per shard ({total} in all) need "
+                          f"{need / 2**30:.2f} GiB for the exchange and the merged result, "
+                          f"{int(all_sizes[:, 1].min()) / 2**30:.2f} GiB are free (raise the threshold or split the query batch)")
+    buf = torch.empty(slot, dtype=torch.uint8, device=dev)
+    fill(range_views(buf, n_q, n_pairs, p_max, jaccard))
+    return gather_packed(buf, group), pairs
+
+
+def merge_range_on_device(device: int, gathered, n_q: int, pairs, jaccard: bool = False):
+    """``kv_merge_range_device_on`` directly on the gathered slots ([W, slot] uint8), on torch's current stream: the
+    single CSR result ``(indptr, rows, scores[, inter, union])`` as torch tensors on the device."""
+    import torch
+
+    pairs = np.ascontiguousarray(pairs, dtype=np.int64)
+    w = gathered.shape[0]
+    offs, slot = range_layout(n_q, int(pairs.max()), jaccard)
+    assert gathered.shape[1] == slot, (gathered.shape, slot)
+    out = _devout.range_arrays(device, n_q, int(pairs.sum()), jaccard)
+    base = gathered.data_ptr()
+    vp = lambda o: C.c_void_p(base + o)
+    stream = torch.cuda.current_stream(gathered.device).cuda_stream
+    _capi.check(_capi.load().kv_merge_range_device_on(device, w, n_q, vp(0), slot // 8, vp(offs[1]), vp(offs[2]),
+                                                      vp(offs[3]) if jaccard else None, vp(offs[4]) if jaccard else None,
+                                                      slot, pairs.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                      *_devout.ptrs(out), *([None, None] if not jaccard else []),
+                                                      C.c_void_p(stream)))
+    return out
+
+
+def _fetch_into(h, views) -> None:
+    """``kv_range_fetch_device`` of a kv_index handle's threshold-search result into ``views``."""
+    _capi.check(_capi.load().kv_range_fetch_device(h, *_devout.ptrs(views), *[None] * (5 - len(views))))
+
+
+def _concat_ranges(parts):
+    """Query blocks' CSR results (torch, on one device) -> one CSR over all the blocks."""
+    import torch
+
+    if len(parts) == 1:
+        return parts[0]
+    ips, off = [], 0
+    for p in parts:
+        ips.append(p[0][:-1] + off)
+        off += int(p[0][-1])
+    ips.append(torch.full((1,), off, dtype=torch.int64, device=parts[0][0].device))
+    return (torch.cat(ips),) + tuple(torch.cat([p[j] for p in parts]) for j in range(1, len(parts[0])))
+
+
+def _host(out, device_out: bool):
+    return out if device_out else tuple(t.cpu().numpy() for t in out)
+
+
 class ShardedGfkb:
     """This rank's share of a GFKB job spread over ``world`` GPUs.
 
@@ -151,10 +253,12 @@ class ShardedGfkb:
         self.vocab = Vocabulary()
         self.index: Optional[GfkbIndex] = None
         self.n_global = 0
+        self._corpus = None   # (data, offsets, mode) of the corpus text: the queries of selfjoin_range
 
     def build_packed(self, data, offsets: np.ndarray, mode: int = 0, n_threads: int = 0) -> None:
         import torch
 
+        self._corpus = (data, np.ascontiguousarray(offsets, dtype=np.int64), mode)
         fb = self.vocab.featurize_packed(data, offsets, mode, grow=True, n_threads=n_threads)
         self.n_global = fb.n
         lo, hi = shard_bounds(fb.n, self.world, self.rank) if self.mode == "rows" else (0, fb.n)
@@ -163,6 +267,7 @@ class ShardedGfkb:
             self.index = GfkbIndex(device=self.device, row_base=0, vocab=self.vocab)
             self.index.add_features(gather_rows(fb, sel, n_threads))
             self.row_map = torch.from_numpy(sel).to(f"cuda:{self.device}")
+            self._row_map_host = sel
         else:
             self.index = GfkbIndex(device=self.device, row_base=lo, vocab=self.vocab)
             self.index.add_features(fb, lo, hi)
@@ -444,6 +549,120 @@ class ShardedGfkb:
         finally:
             qfb.close()
 
+    # ---- threshold search ------------------------------------------------------------------------------------------
+    def set_row_labels(self, global_labels: Optional[np.ndarray]) -> None:
+        """One label >= 0 per GLOBAL row (e.g. a failure-type id): this shard keeps its rows' labels (by index range, or
+        through ``row_map`` for a text-order shard), for ``labels=`` of the threshold searches.  ``None`` clears."""
+        if global_labels is None:
+            self.index.set_row_labels(None)
+            return
+        lab = np.ascontiguousarray(global_labels, dtype=np.int32)
+        if len(lab) != self.n_global:
+            raise ValueError(f"set_row_labels: {len(lab)} labels for a corpus of {self.n_global} rows")
+        if self.row_map is not None:
+            lab = lab[self._row_map_host]
+        elif self.mode == "rows":
+            lo, hi = shard_bounds(self.n_global, self.world, self.rank)
+            lab = lab[lo:hi]
+        self.index.set_row_labels(lab)
+
+    def _set_resident_range(self, qfb: FeatureBatch) -> None:
+        """``set_resident`` that also takes a batch whose queries-mode slice on this rank is empty."""
+        if self.mode == "queries" and self.world > 1:
+            lo, hi = shard_bounds(qfb.n, self.world, self.rank)
+            self._qslice = (lo, hi)
+            self._resident_q = qfb.n
+            if hi > lo:
+                self.upload(qfb)
+            return
+        self.set_resident(qfb)
+
+    def _empty_range(self, device_out: bool):
+        if device_out:
+            return _devout.empty_range(self.device)
+        return np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32)
+
+    def range_resident(self, threshold: float, device_out: bool = False, labels: Optional[np.ndarray] = None):
+        """Threshold search of the resident batch over the whole sharded corpus: ``(indptr int64[n_q+1], rows int64[P],
+        scores float32[P])`` as ``GfkbIndex.range`` returns them (global rows, each query's pairs by (score desc, row
+        asc)), NumPy arrays or with ``device_out`` torch tensors on this rank's device; identical on every rank.
+        ``labels``: per query the row label its pairs must carry (-1: any row; ``set_row_labels``).  Every shard
+        searches its rows alone (the threshold is fixed); one all-gather of the results and the device merge follow."""
+        q = self._resident_q
+        lo, hi = self._qslice if self.mode == "queries" and self.world > 1 else (0, q)
+        if labels is not None and hi > lo:
+            self.index.set_filter(np.ascontiguousarray(labels, dtype=np.int32)[lo:hi])
+        if self.world == 1:
+            return self.index._range_resident(q, threshold, device_out)
+        n = C.c_int64(0)
+        if hi > lo:
+            _capi.check(_capi.load().kv_range_resident(self.index._h, np.float32(threshold), C.byref(n)))
+
+        def fill(views):
+            ip = views[0]
+            if hi == lo:
+                ip.zero_()
+                return
+            # queries mode: this rank's run holds empty segments outside its slice [lo, hi)
+            _fetch_into(self.index._h, [ip[lo:hi + 1]] + views[1:])
+            ip[:lo] = 0
+            ip[hi + 1:] = n.value
+            if self.row_map is not None:   # text-range shard: local -> global rows (ascending, so segments stay ordered)
+                views[1].copy_(self.row_map[views[1]])
+
+        gathered, pairs = gather_range_packed(self.device, q, n.value, fill, self.group)
+        return _host(merge_range_on_device(self.device, gathered, q, pairs), device_out)
+
+    def range_packed(self, data, offsets: np.ndarray, threshold: float, mode: int = 0, labels: Optional[np.ndarray] = None,
+                     device_out: bool = False):
+        """``range_resident`` of a batch of host text (packed as for ``topk_packed``).  Rows mode on several GPUs
+        prepares the batch with ``upload_text_sharded``."""
+        offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+        if len(offsets) <= 1:
+            return self._empty_range(device_out)
+        if self.world > 1 and self.mode == "rows":
+            self.upload_text_sharded(data, offsets, mode)
+        else:
+            qfb = self.vocab.featurize_packed(data, offsets, mode, grow=False)
+            try:
+                self._set_resident_range(qfb)
+            finally:
+                qfb.close()
+        return self.range_resident(threshold, device_out, labels)
+
+    def selfjoin_range(self, threshold: float, device_out: bool = False, block: int = 262144):
+        """All-pairs threshold search over the whole sharded corpus: for every global row every OTHER row scoring
+        >= ``threshold``, as ``GfkbIndex.selfjoin_range`` (query i = row i).  The queries are the corpus text that
+        ``build_packed`` keeps a reference to, in blocks of ``block`` rows; each block's merged result is appended."""
+        if self._corpus is None:
+            raise ValueError("selfjoin_range: build_packed first")
+        if self.world == 1:
+            return self.index.selfjoin_range(threshold, device_out=device_out)
+        data, off, mode = self._corpus
+        parts = []
+        for b0 in range(0, self.n_global, block):
+            b1 = min(self.n_global, b0 + block)
+            if self.mode == "rows":
+                self.upload_text_sharded(data, off[b0:b1 + 1], mode)
+                lo, hi = 0, b1 - b0
+            else:
+                qfb = self.vocab.featurize_packed(data, off[b0:b1 + 1], mode, grow=False)
+                try:
+                    self._set_resident_range(qfb)
+                finally:
+                    qfb.close()
+                lo, hi = self._qslice
+            if hi > lo:
+                excl = np.arange(b0 + lo, b0 + hi, dtype=np.int64)
+                if self.row_map is not None:   # global -> local row of this text-range shard (row_base 0), -1 elsewhere
+                    pos = np.minimum(np.searchsorted(self._row_map_host, excl), max(len(self._row_map_host) - 1, 0))
+                    excl = np.where(self._row_map_host[pos] == excl, pos, -1) if len(self._row_map_host) else np.full_like(excl, -1)
+                self.index.set_exclusions(excl)
+            parts.append(self.range_resident(threshold, device_out=True))
+        if not parts:
+            return self._empty_range(device_out)
+        return _host(_concat_ranges(parts), device_out)
+
 
 class ShardedDense:
     """Row-sharded dense-embedding GFKB (BASELINE configs[2] read as 768-d bf16 cosine, and configs[3] all-pairs).
@@ -513,6 +732,38 @@ class ShardedDense:
             out_r.append(r)
         return torch.cat(out_s), torch.cat(out_r)
 
+    def range(self, queries, threshold: float, device_out: bool = True, exclude_base: int = -1):
+        """Threshold search over the whole sharded GFKB: queries torch bfloat16 CUDA [Q, dim], identical on every rank
+        -> ``(indptr int64[Q+1], rows int64[P], scores float32[P])`` as ``DenseIndex.range_device`` returns them (torch
+        tensors on the device, or NumPy arrays without ``device_out``); identical on every rank.  ``exclude_base >= 0``:
+        query q never matches GLOBAL row ``exclude_base + q``."""
+        import torch
+
+        idx = self.index
+        queries = queries.contiguous()
+        if self.world == 1:
+            return idx.range_device(queries, threshold, exclude_base, device_out)
+        assert queries.is_cuda and queries.element_size() == 2 and queries.shape[-1] == self.dim
+        n_q = queries.shape[0]
+        torch.cuda.current_stream(queries.device).synchronize()  # the library reads the queries on its own stream
+        lib, n = _capi.load(), C.c_int64(0)
+        with idx._lock:
+            _capi.check(lib.kv_dense_range_device(idx._h, C.c_void_p(queries.data_ptr()), n_q, np.float32(threshold),
+                                                  exclude_base, C.byref(n)))
+            fill = lambda views: _capi.check(lib.kv_dense_range_fetch_device(idx._h, *_devout.ptrs(views)))
+            gathered, pairs = gather_range_packed(self.device, n_q, n.value, fill, self.group)
+        return _host(merge_range_on_device(self.device, gathered, n_q, pairs), device_out)
+
+    def selfjoin_range(self, threshold: float, block: int = 262144, device_out: bool = True):
+        """Every row's OTHER rows scoring >= ``threshold`` over the whole sharded GFKB (query i = global row i): the row
+        shards are all-gathered once (``gather_rows``), then blocks of ``block`` rows are searched as in ``range``."""
+        allrows = self.gather_rows()
+        parts = [self.range(allrows[b0:min(self.n_global, b0 + block)], threshold, True, exclude_base=b0)
+                 for b0 in range(0, self.n_global, block)]
+        if not parts:
+            return _host(_devout.empty_range(self.device), device_out)
+        return _host(_concat_ranges(parts), device_out)
+
 
 class ShardedJaccard:
     """Row-sharded token-set Jaccard GFKB (BASELINE configs[4]: 5M sets on 4 GPUs).  No global statistics exist for
@@ -527,11 +778,13 @@ class ShardedJaccard:
         self._cls = JaccardIndex
         self.index = None
         self.n_global = 0
+        self._csr = None   # the whole corpus (build_csr): the queries of selfjoin_range
 
     def build_csr(self, indptr: np.ndarray, ids: np.ndarray) -> None:
         """``indptr``/``ids``: the WHOLE corpus (every rank passes the same arrays); this rank keeps its row range."""
         n = len(indptr) - 1
         self.n_global = n
+        self._csr = (np.ascontiguousarray(indptr, dtype=np.int64), np.ascontiguousarray(ids, dtype=np.uint32))
         lo, hi = shard_bounds(n, self.world, self.rank)
         self.index = self._cls(self.vocab_size, device=self.device, row_base=lo)
         ip = np.ascontiguousarray(indptr[lo:hi + 1], dtype=np.int64)
@@ -543,6 +796,7 @@ class ShardedJaccard:
         lo, hi = shard_bounds(n_global, self.world, self.rank)
         assert len(indptr) - 1 == hi - lo
         self.n_global = n_global
+        self._csr = None
         self.index = self._cls(self.vocab_size, device=self.device, row_base=lo)
         self.index.add_csr(np.ascontiguousarray(indptr, dtype=np.int64), np.ascontiguousarray(ids, dtype=np.uint32))
         self.index.finalize()
@@ -565,3 +819,44 @@ class ShardedJaccard:
         dist.all_reduce(cnt, op=dist.ReduceOp.MAX, group=self.group)
         cnt = cnt.cpu().numpy()
         return ms.cpu().numpy(), rows, cnt[0], cnt[1]
+
+    def _range_csr(self, indptr: np.ndarray, ids: np.ndarray, threshold: float, exclude: Optional[np.ndarray], device_out: bool):
+        idx = self.index
+        ip, qids, oov = idx._strip_oov(indptr, ids)
+        n_q = len(ip) - 1
+        if n_q == 0:
+            return idx._empty_range(device_out)
+        lib, n = _capi.load(), C.c_int64(0)
+        idx._upload(ip, qids, np.ones(len(qids), dtype=np.uint32), oov, n_q)
+        if exclude is not None:   # global rows; the shard maps them to its own rows
+            exclude = np.ascontiguousarray(exclude, dtype=np.int64)
+            _capi.check(lib.kv_query_set_exclusions(idx._h, exclude.ctypes.data_as(C.POINTER(C.c_int64)), n_q))
+        _capi.check(lib.kv_range_resident(idx._h, np.float32(threshold), C.byref(n)))
+        gathered, pairs = gather_range_packed(self.device, n_q, n.value, lambda views: _fetch_into(idx._h, views), self.group,
+                                              jaccard=True)
+        return _host(merge_range_on_device(self.device, gathered, n_q, pairs, jaccard=True), device_out)
+
+    def range_csr(self, indptr: np.ndarray, ids: np.ndarray, threshold: float, device_out: bool = False):
+        """Threshold search over the whole sharded GFKB, as ``JaccardIndex.range_csr``: ``(indptr, rows, scores, inter,
+        union)``, identical on every rank.  The exact counts travel with the pairs (each shard counts its own rows)."""
+        if self.world == 1:
+            return self.index.range_csr(indptr, ids, threshold, device_out)
+        return self._range_csr(indptr, ids, threshold, None, device_out)
+
+    def selfjoin_range(self, threshold: float, device_out: bool = False, block: int = 262144):
+        """Every row's OTHER rows scoring >= ``threshold`` over the whole sharded GFKB (query i = global row i), as
+        ``JaccardIndex.selfjoin_range``; the queries are the corpus ``build_csr`` was given, in blocks of ``block`` rows.
+        After ``build_local_csr`` a shard lacks the other shards' rows: ValueError."""
+        if self._csr is None:
+            raise ValueError("selfjoin_range: needs the whole corpus (build_csr); build_local_csr keeps only this shard's rows")
+        if self.world == 1:
+            return self.index.selfjoin_range(threshold, device_out=device_out)
+        ip, ids = self._csr
+        parts = []
+        for b0 in range(0, self.n_global, block):
+            b1 = min(self.n_global, b0 + block)
+            parts.append(self._range_csr(ip[b0:b1 + 1] - ip[b0], ids[ip[b0]:ip[b1]], threshold,
+                                         np.arange(b0, b1, dtype=np.int64), True))
+        if not parts:
+            return self.index._empty_range(device_out)
+        return _host(_concat_ranges(parts), device_out)

@@ -82,7 +82,9 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
 
     ``index``: a finalized ``GfkbIndex`` whose row i is ``records[i]['signature_text']`` (corpus-fit mode gives a
     symmetric measure; the default mode works too), a finalized ``DenseIndex`` whose row i is record i's embedding
-    (cosine), or a finalized ``JaccardIndex`` whose row i is record i's token set.  Returns one payload per connected
+    (cosine), or a finalized ``JaccardIndex`` whose row i is record i's token set; with ``k=None`` also a row-sharded
+    ``ShardedGfkb`` / ``ShardedDense`` / ``ShardedJaccard`` (dist.py) over the records, whose replicated threshold
+    graph gives every rank the same payloads.  Returns one payload per connected
     component that, restricted
     to ``failure_type`` (if given), spans at least ``min_apps`` apps (app.py:45-46) -- ordered by smallest row id.
     ``k``: rows are linked only through every row's k nearest other rows, so when a text is stored more than k times
@@ -99,6 +101,9 @@ def detect_patterns(index, records: Sequence[Mapping[str, Any]], threshold: floa
     from .similarity import GfkbIndex
 
     # the index classes a mode is built for are checked before the index is touched
+    if k is not None and not hasattr(index, "selfjoin_topk"):
+        raise NotImplementedError(f"detect_patterns: {type(index).__name__} has no k-nearest self-join; "
+                                  "use k=None (the threshold graph, selfjoin_range)")
     if distinct and k is not None and not isinstance(index, GfkbIndex):
         raise NotImplementedError("detect_patterns(distinct=True) collapses copies on a GfkbIndex only")
     if filter_first and failure_type is not None and not isinstance(index, GfkbIndex):
