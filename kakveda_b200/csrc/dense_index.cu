@@ -24,6 +24,7 @@
 // K2-R (dense_topk_kernel<true>) is the same kernel for a threshold search: producer, ring, MMAs and register exchange
 // are unchanged; the epilogue keeps no lists and appends every pair whose score (the same float32 expression) reaches
 // the threshold to a global pair buffer, one reservation per warp and 16-column group (dense_emit).
+#include "index_state.cuh"
 #include "kv_cuda.cuh"
 #include "sm90.cuh"
 
@@ -481,18 +482,14 @@ struct kv_dense_index {
   DevBuf<long long> d_part_r, d_out_r;
   DevBuf<__nv_bfloat16> d_q;
   DevBuf<unsigned int> d_gthr;
-  // last threshold search: pairs in emit order, kept until fetched or until the next range, top-k, append or finalize
-  DevBuf<RangePair> d_range;
-  DevBuf<unsigned long long> d_range_count;
-  bool range_valid = false;
-  int64_t range_q = 0, range_pairs = 0;
+  // last threshold search, kept until fetched or until the next range, top-k, append, deletion or finalize
+  RangeResult<RangePair> range;
   RangeOrderScratch rsort;  // the fetches order the pairs on the device (range_order.cu)
   bool finalized = false;
   float last_ms = 0;
   int64_t last_splits = 0;
-  // row deletion: flags by local row (empty until the first deletion), applied as NaN inverse norms at every finalize
-  std::vector<uint8_t> h_dead;
-  int64_t n_dead = 0;
+  // row deletion, applied as NaN inverse norms at every finalize
+  Tombstones tomb;
   DevBuf<int64_t> d_dead;  // the deleted rows (finalize) or deleted self-join query positions (a search)
   // row labels: kept by finalize and deletions, dropped by an append; the device copy and the tile signatures are
   // rebuilt at every finalize and label upload
@@ -550,7 +547,7 @@ void dense_rows_appended(kv_dense_index *dx, int64_t n) {
   dx->has_labels = false;
   dx->h_labels.clear();
   dx->has_qfilter = false;
-  if (!dx->h_dead.empty()) dx->h_dead.resize((size_t)dx->n_rows, 0);
+  dx->tomb.extend(dx->n_rows);
 }
 
 // Rebuilds the tile signatures from the device labels and the inverse norms (NaN = deleted).  Needs a finalized index
@@ -616,7 +613,7 @@ int kv_dense_append(kv_dense_index *dx, const uint16_t *rows_bf16, int64_t n) {
   if (!dx || n < 0 || (n > 0 && !rows_bf16)) return kv_fail(KV_ERR_INVALID, "kv_dense_append: bad arguments");
   if (n == 0) return KV_OK;
   std::lock_guard<std::mutex> g(dx->mu);
-  dx->range_valid = false;
+  dx->range.drop();
   KV_CUDA(cudaSetDevice(dx->device));
   if (dx->n_rows + n >= (1LL << 31) - BN) return kv_fail(KV_ERR_INVALID, "kv_dense_append: more than 2^31 rows in one shard");
   KV_CUDA(dx->rows.reserve((dx->n_rows + n) * dx->dim, dx->stream));
@@ -629,7 +626,7 @@ int kv_dense_append(kv_dense_index *dx, const uint16_t *rows_bf16, int64_t n) {
 int kv_dense_finalize(kv_dense_index *dx) {
   if (!dx) return kv_fail(KV_ERR_INVALID, "kv_dense_finalize: NULL handle");
   std::lock_guard<std::mutex> g(dx->mu);
-  dx->range_valid = false;
+  dx->range.drop();
   dx->has_qfilter = false;
   KV_CUDA(cudaSetDevice(dx->device));
   KV_CUDA(dx->d_inv_c.ensure(std::max<int64_t>(dx->n_rows, 1)));
@@ -639,11 +636,11 @@ int kv_dense_finalize(kv_dense_index *dx) {
   }
   KV_CUDA(cudaStreamSynchronize(dx->stream));
   // tombstones: a deleted row's inverse norm is NaN, which removes every score of the row in the epilogue
-  if (dx->n_dead) {
+  if (dx->tomb.any()) {
     std::vector<int64_t> dead;
-    dead.reserve((size_t)dx->n_dead);
+    dead.reserve((size_t)dx->tomb.count);
     for (int64_t r = 0; r < dx->n_rows; r++)
-      if (dx->h_dead[(size_t)r]) dead.push_back(r);
+      if (dx->tomb.is_dead(r)) dead.push_back(r);
     const int rc = scatter_nan(dx, dx->d_inv_c.p, dead);
     if (rc != KV_OK) return rc;
   }
@@ -658,33 +655,21 @@ int kv_dense_finalize(kv_dense_index *dx) {
 int kv_dense_delete_rows(kv_dense_index *dx, const int64_t *rows, int64_t n) {
   if (!dx || n < 0 || (n > 0 && !rows)) return kv_fail(KV_ERR_INVALID, "kv_dense_delete_rows: bad arguments");
   std::lock_guard<std::mutex> g(dx->mu);
-  for (int64_t i = 0; i < n; i++)
-    if (rows[i] < 0 || rows[i] >= dx->n_rows)
-      return kv_fail(KV_ERR_INVALID, "kv_dense_delete_rows: row %lld outside 0..%lld", (long long)rows[i], (long long)dx->n_rows - 1);
   int64_t added = 0;
-  for (int64_t i = 0; i < n; i++) {
-    if (dx->h_dead.empty()) dx->h_dead.assign((size_t)dx->n_rows, 0);
-    uint8_t &d = dx->h_dead[(size_t)rows[i]];
-    if (!d) { d = 1; added++; }
-  }
-  if (!added) return KV_OK;  // duplicates and rows deleted before: nothing changes
-  dx->n_dead += added;
+  const int rc = dx->tomb.mark(rows, n, dx->n_rows, "kv_dense_delete_rows", &added);
+  if (rc != KV_OK || !added) return rc;  // duplicates and rows deleted before: nothing changes
   // like an append: the inverse norms and tile signatures are stale until the next finalize
   dx->finalized = false;
-  dx->range_valid = false;
+  dx->range.drop();
   return KV_OK;
 }
 
-int64_t kv_dense_live_rows(const kv_dense_index *dx) { return dx ? dx->n_rows - dx->n_dead : 0; }
+int64_t kv_dense_live_rows(const kv_dense_index *dx) { return dx ? dx->n_rows - dx->tomb.count : 0; }
 
 int kv_dense_deleted_rows(kv_dense_index *dx, uint8_t *out, int64_t n) {
   if (!dx || n < 0 || (n > 0 && !out)) return kv_fail(KV_ERR_INVALID, "kv_dense_deleted_rows: bad arguments");
   std::lock_guard<std::mutex> g(dx->mu);
-  if (n != dx->n_rows)
-    return kv_fail(KV_ERR_INVALID, "kv_dense_deleted_rows: %lld flags for an index of %lld rows", (long long)n, (long long)dx->n_rows);
-  if (dx->n_dead) memcpy(out, dx->h_dead.data(), (size_t)n);
-  else if (n) memset(out, 0, (size_t)n);
-  return KV_OK;
+  return dx->tomb.copy_out(out, n, dx->n_rows, "kv_dense_deleted_rows");
 }
 
 int kv_dense_set_row_labels(kv_dense_index *dx, const int32_t *labels, int64_t n) {
@@ -752,10 +737,10 @@ static int dense_setup(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q
   KV_CUDA(dx->d_inv_q.ensure(n_q));
   inv_norm_kernel<<<(unsigned)((n_q * 32 + 255) / 256), 256, 0, s>>>(d_q, n_q, dx->dim, dx->d_inv_q.p);
   KV_CUDA(cudaGetLastError());
-  if (sj_begin >= 0 && dx->n_dead) {
+  if (sj_begin >= 0 && dx->tomb.any()) {
     std::vector<int64_t> dead_q;  // kernel positions of the deleted query rows
     for (int64_t p = 0; p < n_q; p++)
-      if (dx->h_dead[(size_t)(sj_begin + (cf.on ? cf.perm[(size_t)p] : p))]) dead_q.push_back(p);
+      if (dx->tomb.is_dead(sj_begin + (cf.on ? cf.perm[(size_t)p] : p))) dead_q.push_back(p);
     const int rc = scatter_nan(dx, dx->d_inv_q.p, dead_q);
     if (rc != KV_OK) return rc;
   }
@@ -864,9 +849,8 @@ static int dense_run(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, 
 }
 
 // Threshold search of n_q queries already on the device (as dense_run): every pair whose score reaches thr lands in
-// d_range, in emit order; the handle records the result for kv_dense_range_fetch.  The pair buffer starts at 65,536
-// records and keeps its capacity across calls.  When a search finds more pairs, the buffer grows to the exact count
-// and the kernel runs once more -- the whole GEMM again, since the pairs are only known in its epilogue.  last_ms sums
+// dx->range, in emit order, for kv_dense_range_fetch.  When a search finds more pairs than the buffer holds, it grows to
+// the exact count and the kernel runs once more -- the whole GEMM again, since the pairs are only known in its epilogue.  last_ms sums
 // both runs.  Caller holds dx->mu.
 static int dense_range(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q, float thr, int64_t excl_base,
                        int64_t sj_begin, const CallFilter &cf, int64_t *n_pairs) {
@@ -881,22 +865,20 @@ static int dense_range(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q
     DenseFilter F;
     int rc = dense_setup(dx, d_q, n_q, excl_base, sj_begin, cf, &map_q, &map_c, P, F);
     if (rc != KV_OK) return rc;
-    KV_CUDA(dx->d_range.ensure(65536));
-    KV_CUDA(dx->d_range_count.ensure(1));
+    if ((rc = dx->range.prepare(s)) != KV_OK) return rc;
     DenseRangeOut R;
     R.thr = thr;
-    R.count = dx->d_range_count.p;
+    R.count = dx->range.d_count.p;
     const int64_t grid = P.q_tiles * P.n_lists;
     for (;;) {
-      R.out = dx->d_range.p;
-      R.cap = (unsigned long long)dx->d_range.cap;
-      KV_CUDA(cudaMemsetAsync(dx->d_range_count.p, 0, sizeof(unsigned long long), s));
+      R.out = dx->range.pairs.p;
+      R.cap = dx->range.capacity();
       if (F.qperm) KV_CUDA(cudaMemsetAsync(F.skipped, 0, 8, s));
       KV_CUDA(cudaEventRecord(dx->ev[0], s));
       dense_launch(true, s, grid, map_q, map_c, P, R, F);
       KV_CUDA(cudaGetLastError());
       KV_CUDA(cudaEventRecord(dx->ev[1], s));
-      KV_CUDA(cudaMemcpyAsync(&count, dx->d_range_count.p, sizeof(count), cudaMemcpyDeviceToHost, s));
+      KV_CUDA(cudaMemcpyAsync(&count, R.count, sizeof(count), cudaMemcpyDeviceToHost, s));
       KV_CUDA(cudaStreamSynchronize(s));
       float ms = 0.f;
       cudaEventElapsedTime(&ms, dx->ev[0], dx->ev[1]);
@@ -904,17 +886,11 @@ static int dense_range(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q
       rc = read_skipped(dx, F);
       if (rc != KV_OK) return rc;
       if (count <= R.cap) break;
-      if (dx->d_range.ensure((int64_t)count) != cudaSuccess) {
-        cudaGetLastError();
-        return kv_fail(KV_ERR_NOMEM, "kv_dense_range: %llu pairs reach the threshold; their buffer does not fit in device memory "
-                                     "(raise the threshold or split the query batch)", count);
-      }
+      if ((rc = dx->range.grow(count, s, "kv_dense_range")) != KV_OK) return rc;
     }
   }
   dx->last_ms = total_ms;
-  dx->range_q = n_q;
-  dx->range_pairs = (int64_t)count;
-  dx->range_valid = true;
+  dx->range.commit(n_q, (int64_t)count);
   *n_pairs = (int64_t)count;
   return KV_OK;
 }
@@ -930,7 +906,7 @@ int kv_dense_topk(kv_dense_index *dx, const uint16_t *q_bf16, int64_t n_q, int k
   const int frc = take_filter(dx, n_q, "kv_dense_topk", cf);
   if (n_q < 0 || k < 1 || k > MAXK || (n_q > 0 && (!q_bf16 || !out_scores || !out_rows)))
     return kv_fail(KV_ERR_INVALID, "kv_dense_topk: bad arguments (k must be 1..32)");
-  dx->range_valid = false;
+  dx->range.drop();
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_topk: index not finalized");
   if (frc != KV_OK) return frc;
   if (n_q == 0) return KV_OK;
@@ -955,7 +931,7 @@ int kv_dense_topk_device(kv_dense_index *dx, const void *d_q_bf16, int64_t n_q, 
   if (n_q < 0 || k < 1 || k > MAXK || (n_q > 0 && (!d_q_bf16 || !d_scores || !d_rows)))
     return kv_fail(KV_ERR_INVALID, "kv_dense_topk_device: bad arguments (k must be 1..32)");
   if (((uintptr_t)d_q_bf16 & 15) != 0) return kv_fail(KV_ERR_INVALID, "kv_dense_topk_device: queries must be 16-byte aligned");
-  dx->range_valid = false;
+  dx->range.drop();
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_topk_device: index not finalized");
   if (frc != KV_OK) return frc;
   if (n_q == 0) return KV_OK;
@@ -968,7 +944,7 @@ int kv_dense_append_device(kv_dense_index *dx, const void *d_rows_bf16, int64_t 
   if (!dx || n < 0 || (n > 0 && !d_rows_bf16)) return kv_fail(KV_ERR_INVALID, "kv_dense_append_device: bad arguments");
   if (n == 0) return KV_OK;
   std::lock_guard<std::mutex> g(dx->mu);
-  dx->range_valid = false;
+  dx->range.drop();
   KV_CUDA(cudaSetDevice(dx->device));
   if (dx->n_rows + n >= (1LL << 31) - BN) return kv_fail(KV_ERR_INVALID, "kv_dense_append_device: more than 2^31 rows in one shard");
   KV_CUDA(dx->rows.reserve((dx->n_rows + n) * dx->dim, dx->stream));
@@ -987,7 +963,7 @@ int kv_dense_selfjoin_device(kv_dense_index *dx, int64_t q_begin, int64_t q_end,
   const int frc = take_filter(dx, q_end - q_begin, "kv_dense_selfjoin_device", cf);
   if (q_begin < 0 || q_end < q_begin || k < 1 || k > MAXK || !d_scores || !d_rows)
     return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_device: bad arguments (k must be 1..32)");
-  dx->range_valid = false;
+  dx->range.drop();
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_selfjoin_device: index not finalized");
   if (q_end > dx->n_rows) return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_device: row range outside the index");
   if (frc != KV_OK) return frc;
@@ -1007,7 +983,7 @@ int kv_dense_range(kv_dense_index *dx, const uint16_t *q_bf16, int64_t n_q, floa
   if (!n_pairs || n_q < 0 || n_q >= (1LL << 31) || (n_q > 0 && !q_bf16))
     return kv_fail(KV_ERR_INVALID, "kv_dense_range: bad arguments (n_q must be below 2^31)");
   if (!valid_threshold(threshold)) return kv_fail(KV_ERR_INVALID, "kv_dense_range: threshold must be in (0, 1]");
-  dx->range_valid = false;
+  dx->range.drop();
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_range: index not finalized");
   if (frc != KV_OK) return frc;
   KV_CUDA(cudaSetDevice(dx->device));
@@ -1028,7 +1004,7 @@ int kv_dense_range_device(kv_dense_index *dx, const void *d_q_bf16, int64_t n_q,
     return kv_fail(KV_ERR_INVALID, "kv_dense_range_device: bad arguments (n_q must be below 2^31)");
   if (((uintptr_t)d_q_bf16 & 15) != 0) return kv_fail(KV_ERR_INVALID, "kv_dense_range_device: queries must be 16-byte aligned");
   if (!valid_threshold(threshold)) return kv_fail(KV_ERR_INVALID, "kv_dense_range_device: threshold must be in (0, 1]");
-  dx->range_valid = false;
+  dx->range.drop();
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_range_device: index not finalized");
   if (frc != KV_OK) return frc;
   KV_CUDA(cudaSetDevice(dx->device));
@@ -1043,7 +1019,7 @@ int kv_dense_selfjoin_range(kv_dense_index *dx, int64_t q_begin, int64_t q_end, 
   if (!n_pairs || q_begin < 0 || q_end < q_begin || q_end - q_begin >= (1LL << 31))
     return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_range: bad arguments");
   if (!valid_threshold(threshold)) return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_range: threshold must be in (0, 1]");
-  dx->range_valid = false;
+  dx->range.drop();
   if (!dx->finalized) return kv_fail(KV_ERR_STATE, "kv_dense_selfjoin_range: index not finalized");
   if (q_end > dx->n_rows) return kv_fail(KV_ERR_INVALID, "kv_dense_selfjoin_range: row range outside the index");
   if (frc != KV_OK) return frc;
@@ -1053,39 +1029,21 @@ int kv_dense_selfjoin_range(kv_dense_index *dx, int64_t q_begin, int64_t q_end, 
 }
 
 // The pairs come back in emit order, which the kernel does not fix; (score desc, row asc) is a total order of each
-// query's pairs, so the result is deterministic.
+// query's pairs, so the result is deterministic.  Both fetches order the pairs on the device and consume the result
+// (RangeResult).
 int kv_dense_range_fetch(kv_dense_index *dx, int64_t *indptr, int64_t *rows, float *scores) {
   if (!dx || !indptr) return kv_fail(KV_ERR_INVALID, "kv_dense_range_fetch: bad arguments");
   std::lock_guard<std::mutex> g(dx->mu);
-  if (!dx->range_valid) return kv_fail(KV_ERR_STATE, "kv_dense_range_fetch: no threshold search result (kv_dense_range* first)");
-  const int64_t n_q = dx->range_q, n = dx->range_pairs;
-  if (n > 0 && (!rows || !scores)) return kv_fail(KV_ERR_INVALID, "kv_dense_range_fetch: bad arguments");
-  KV_CUDA(cudaSetDevice(dx->device));
-  // ordered on the device in the pair buffer itself (range_order.cu); a failed scratch allocation keeps the result
-  const int rc = range_order_to_host(dx->d_range.p, n, n_q, 0, indptr, rows, scores, nullptr, nullptr, dx->rsort, dx->stream,
-                                     "kv_dense_range_fetch");
-  if (rc != KV_ERR_NOMEM) dx->range_valid = false;
-  return rc;
+  return dx->range.fetch_host("kv_dense_range_fetch", "kv_dense_range*", dx->device, dx->stream, dx->rsort, 0, indptr, rows,
+                              scores, nullptr, nullptr);
 }
 
 // Device outputs: the same arrays, written to caller-owned device memory of the index's device.
 int kv_dense_range_fetch_device(kv_dense_index *dx, void *d_indptr, void *d_rows, void *d_scores) {
-  const char *fn = "kv_dense_range_fetch_device";
-  if (!dx) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
+  if (!dx) return kv_fail(KV_ERR_INVALID, "kv_dense_range_fetch_device: bad arguments");
   std::lock_guard<std::mutex> g(dx->mu);
-  if (!dx->range_valid) return kv_fail(KV_ERR_STATE, "%s: no threshold search result (kv_dense_range* first)", fn);
-  const int64_t n_q = dx->range_q, n = dx->range_pairs;
-  int rc = check_device_ptr(d_indptr, dx->device, 8, "indptr", fn);
-  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_rows, dx->device, 8, "rows", fn);
-  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_scores, dx->device, 4, "scores", fn);
-  if (rc != KV_OK) return rc;
-  KV_CUDA(cudaSetDevice(dx->device));
-  rc = range_order_device(dx->d_range.p, n, n_q, 0, (int64_t *)d_indptr, (int64_t *)d_rows, (float *)d_scores, nullptr, nullptr,
-                          dx->rsort, dx->stream, fn);
-  if (rc != KV_ERR_NOMEM) dx->range_valid = false;
-  if (rc != KV_OK) return rc;
-  KV_CUDA(cudaStreamSynchronize(dx->stream));
-  return KV_OK;
+  return dx->range.fetch_device("kv_dense_range_fetch_device", "kv_dense_range*", dx->device, dx->stream, dx->rsort, 0, d_indptr,
+                                d_rows, d_scores, nullptr, nullptr);
 }
 
 int kv_dense_last_timing(const kv_dense_index *dx, float *gemm_ms, int64_t *splits) {

@@ -6,6 +6,7 @@
 // and kernel launches.
 #include "block_builder.cuh"
 #include "bound_kernel.cuh"
+#include "index_state.cuh"
 
 #include <algorithm>
 #include <atomic>
@@ -26,6 +27,61 @@ using namespace kvh;  // parallel_for, stable_sort_indices, idf_host, build_bloc
 // ----------------------------------------------------------------------------------------
 // handle
 // ----------------------------------------------------------------------------------------
+
+// One integer >= 0 per local row (row labels, row groups).  It describes the rows it was set for: an append drops it.
+// On the device, rebuilt by every finalize for the current scan layout: by row and by scan position.
+struct RowSet {
+  std::vector<int> h;
+  bool has = false, on_device = false;
+  DevBuf<int> d_row, d_pos;
+
+  // v[0, n) for an index of n_rows rows; `what` names one value in the errors ("label", "group")
+  int set(const int32_t *v, int64_t n, int64_t n_rows, const char *fn, const char *what) {
+    if (n != n_rows) return kv_fail(KV_ERR_INVALID, "%s: %lld %ss for an index of %lld rows", fn, (long long)n, what, (long long)n_rows);
+    for (int64_t i = 0; i < n; i++)
+      if (v[i] < 0) return kv_fail(KV_ERR_INVALID, "%s: %s %d of row %lld is negative", fn, what, v[i], (long long)i);
+    h.assign(v, v + n);
+    has = true;
+    return KV_OK;
+  }
+  void clear() {
+    h.clear();
+    has = on_device = false;
+  }
+  // set for the current n_rows rows and on the device for the current layout
+  bool ready(int64_t n_rows) const { return has && on_device && (int64_t)h.size() == n_rows; }
+  // The device copies for the layout whose scan position p holds row perm[p] (n_pos positions, n rows).
+  int upload(const int *perm, int64_t n, int64_t n_pos, cudaStream_t s) {
+    if (n == 0) return KV_OK;
+    KV_CUDA(d_row.ensure(n));
+    KV_CUDA(d_pos.ensure(n_pos));
+    KV_CUDA(cudaMemcpyAsync(d_row.p, h.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
+    label_pos_kernel<<<(unsigned)((n_pos + 255) / 256), 256, 0, s>>>(perm, d_row.p, n, n_pos, d_pos.p);
+    KV_CUDA(cudaGetLastError());
+    KV_CUDA(cudaStreamSynchronize(s));  // h may change once this returns
+    return KV_OK;
+  }
+};
+
+// The irregular queries of the resident batch (see classify_queries), in sorted-slot order: their original index and
+// CSR on the host, for the float64 full-scan fallback.
+struct IrregularQueries {
+  std::vector<int64_t> q, indptr{0};
+  std::vector<uint32_t> ids, tf;
+  std::vector<double> oov;
+
+  void clear() {
+    q.clear(); indptr.assign(1, 0); ids.clear(); tf.clear(); oov.clear();
+  }
+  void add(int64_t query, const uint32_t *q_ids, const uint32_t *q_tf, int64_t nnz, double q_oov) {
+    q.push_back(query);
+    ids.insert(ids.end(), q_ids, q_ids + nnz);
+    tf.insert(tf.end(), q_tf, q_tf + nnz);
+    indptr.push_back((int64_t)ids.size());
+    oov.push_back(q_oov);
+  }
+};
+
 struct kv_index {
   int device = 0;
   int64_t row_base = 0;
@@ -131,11 +187,10 @@ struct kv_index {
   DevBuf<int> d_excl_sorted, d_excl_orig;  // self-join exclusions of the resident batch (by sorted slot / by original query)
   std::vector<int> h_excl_orig;
   bool has_excl = false;
-  // row labels (kv_index_set_row_labels), by local row; dropped by an append.  On the device (rebuilt by every finalize):
-  // by row, by scan position, the chunk label signatures and the first LAB_FIRST rows of every label
-  std::vector<int> h_labels;
-  bool has_labels = false, labels_on_device = false;
-  DevBuf<int> d_labels_row, d_label_pos, d_lab_keys, d_lab_rows;
+  // row labels (kv_index_set_row_labels); besides the common device copies, the chunk label signatures and the first
+  // LAB_FIRST rows of every label
+  RowSet labels;
+  DevBuf<int> d_lab_keys, d_lab_rows;
   DevBuf<unsigned long long> d_chunk_sig;
   int n_lab = 0;
   // label filter of the resident batch (kv_query_set_filter; by sorted slot / by original query), only while some
@@ -143,29 +198,23 @@ struct kv_index {
   DevBuf<int> d_filt_sorted, d_filt_orig;
   std::vector<int> h_filt_orig;
   bool has_filter = false;
-  // row groups (kv_index_set_row_groups), by local row; dropped by an append.  On the device (rebuilt by every
-  // finalize): by row (K5, fallbacks, null queries) and by scan position (scan).  Distinct mode of the resident batch
-  // (kv_query_set_distinct), cleared by the next upload.
-  std::vector<int> h_groups;
-  bool has_groups = false, groups_on_device = false, distinct = false;
-  DevBuf<int> d_groups_row, d_group_pos;
-  // deleted rows (kv_index_delete_rows), by local row (empty until the first deletion; an append extends it).  They
-  // keep their place in the scan layout.  On the device while any row is deleted, rebuilt by every finalize: by row,
-  // the live word of every chunk (by scan position) and the first LAB_FIRST live rows (null queries)
-  std::vector<uint8_t> h_dead;
-  int64_t n_dead = 0;
+  // row groups (kv_index_set_row_groups): by row for K5, the fallbacks and null queries, by scan position for the
+  // scan.  Distinct mode of the resident batch (kv_query_set_distinct), cleared by the next upload.
+  RowSet groups;
+  bool distinct = false;
+  // deleted rows (kv_index_delete_rows).  They keep their place in the scan layout.  On the device while any row is
+  // deleted, rebuilt by every finalize: by row, the live word of every chunk (by scan position) and the first LAB_FIRST
+  // live rows (null queries)
+  Tombstones tomb;
   DevBuf<uint8_t> d_dead;
   DevBuf<uint32_t> d_alive, d_dcnt;
   DevBuf<int> d_dead_list, d_first_live;
   // threshold search over the resident batch (kv_range_resident): its own threshold array (not d_gthr, which peers push
-  // into and a top-k raises), the pair buffer, the pair count, and the result until it is fetched
+  // into and a top-k raises) and the result of the index's mode -- on a Jaccard index (K3-R) the records carry the
+  // exact counts and local rows.  Either result is dropped by the next upload, search, append, deletion or finalize.
   DevBuf<int> d_rthr;
-  DevBuf<RangePair> d_range;
-  DevBuf<unsigned long long> d_range_count;
-  // on a Jaccard index (K3-R) the records carry the exact counts and local rows instead: d_jrange
-  DevBuf<JaccardPair> d_jrange;
-  bool range_valid = false;
-  int64_t range_q = 0, range_pairs = 0;
+  RangeResult<RangePair> range;
+  RangeResult<JaccardPair> jrange;
   RangeOrderScratch rsort;  // the fetches order the pairs on the device (range_order.cu)
   DevBuf<unsigned long long> d_stats;
   DevBuf<float> d_part_s, d_out_s;
@@ -178,9 +227,7 @@ struct kv_index {
   // query batch currently resident on the device (kv_query_upload and its variants)
   bool batch_valid = false;
   int64_t batch_q = 0, batch_tiles = 0, batch_h2d_bytes = 0, batch_null = 0, batch_f2_outside = 0;
-  std::vector<int64_t> irr_q, irr_indptr;
-  std::vector<uint32_t> irr_ids, irr_tf;
-  std::vector<double> irr_oov;
+  IrregularQueries irr;
 
   float *dbg_xs = nullptr;  // test hook (kv_debug_bound_numerators)
   float last_ms[4] = {0, 0, 0, 0};
@@ -199,6 +246,11 @@ static void close_peers(kv_index *ix) {
   ix->n_peers = 0;
   ix->peer_cap = 0;
   ix->peers_borrowed = false;
+}
+
+static void drop_range(kv_index *ix) {
+  ix->range.drop();
+  ix->jrange.drop();
 }
 
 namespace {
@@ -417,13 +469,12 @@ int kv_index_append(kv_index *ix, const int64_t *indptr, const uint32_t *ids, co
   ix->ids.n = ix->nnz;
   ix->tf.n = ix->nnz;
   ix->finalized = false;
-  ix->range_valid = false;
-  // labels describe the rows they were given for: a filtered query fails until the rows are labelled again
-  ix->h_labels.clear();
-  ix->has_labels = ix->labels_on_device = false;
-  ix->h_groups.clear();  // the same for groups: distinct mode fails until they are set again
-  ix->has_groups = ix->groups_on_device = false;
-  if (ix->n_dead) ix->h_dead.resize((size_t)ix->n_rows, 0);  // appended rows are live
+  drop_range(ix);
+  // labels and groups describe the rows they were given for: a filtered or distinct query fails until they are set
+  // again.  Deleted rows stay deleted.
+  ix->labels.clear();
+  ix->groups.clear();
+  ix->tomb.extend(ix->n_rows);
   return KV_OK;
 }
 
@@ -431,7 +482,7 @@ int kv_index_set_mode(kv_index *ix, int mode) {
   if (!ix || (mode != KV_MODE_TFIDF_COSINE && mode != KV_MODE_JACCARD && mode != KV_MODE_TFIDF_CORPUS_FIT))
     return kv_fail(KV_ERR_INVALID, "kv_index_set_mode: mode must be KV_MODE_TFIDF_COSINE, KV_MODE_JACCARD or KV_MODE_TFIDF_CORPUS_FIT");
   std::lock_guard<std::mutex> g(ix->mu);
-  if (mode == KV_MODE_JACCARD && ix->n_dead)
+  if (mode == KV_MODE_JACCARD && ix->tomb.any())
     return kv_fail(KV_ERR_INVALID, "kv_index_set_mode: a Jaccard index (mode 1) has no row deletion, and rows are deleted");
   if (mode == KV_MODE_JACCARD)
     for (uint16_t f : ix->h_tf)
@@ -487,12 +538,12 @@ int kv_index_set_global_df(kv_index *ix, const uint32_t *df, int64_t vocab_size,
 // deleted rows, in d_dcnt; *out = d_cnt itself when nothing is deleted.  Caller holds ix->mu.
 static int live_counts(kv_index *ix, int64_t Vz, const uint32_t **out) {
   *out = ix->d_cnt.p;
-  if (!ix->n_dead) return KV_OK;
+  if (!ix->tomb.any()) return KV_OK;
   cudaStream_t s = ix->stream;
   std::vector<int> list;
-  list.reserve((size_t)ix->n_dead);
+  list.reserve((size_t)ix->tomb.count);
   for (int64_t r = 0; r < ix->n_rows; r++)
-    if (ix->h_dead[(size_t)r]) list.push_back((int)r);
+    if (ix->tomb.is_dead(r)) list.push_back((int)r);
   KV_CUDA(ix->d_dead_list.ensure((int64_t)list.size()));
   KV_CUDA(ix->d_dcnt.ensure(Vz));
   KV_CUDA(cudaMemcpyAsync(ix->d_dead_list.p, list.data(), list.size() * sizeof(int), cudaMemcpyHostToDevice, s));
@@ -542,52 +593,53 @@ static int upload_idf_tables(kv_index *ix, int64_t V) {
   return KV_OK;
 }
 
-// The device copies of the row labels for the current layout: by row (fallbacks), by scan position and as chunk
-// signatures (scan and selection), and the first LAB_FIRST rows of every label (null queries).  Nothing to do until
-// the index is finalized; every finalize calls it again.
-static int upload_labels(kv_index *ix) {
-  ix->labels_on_device = false;
-  if (!ix->has_labels || !ix->finalized) return KV_OK;
+// The device copies of one per-row set for the current layout (by row and by scan position); the labels add their
+// chunk signatures (scan and selection) and the first LAB_FIRST live rows of every label (null queries).  Nothing to
+// do until the index is finalized; every finalize calls it again.
+static int upload_row_set(kv_index *ix, RowSet &rs) {
+  rs.on_device = false;
+  if (!rs.has || !ix->finalized) return KV_OK;
   cudaStream_t s = ix->stream;
-  const int64_t n = ix->n_rows, n_pos = ix->n_chunks_pad * CHUNK_ROWS;
-  std::vector<int> keys(ix->h_labels);
-  std::sort(keys.begin(), keys.end());
-  keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
-  std::vector<int> first(keys.size() * LAB_FIRST, -1), cnt(keys.size(), 0);
-  for (int64_t r = 0; r < n; r++) {
-    if (ix->n_dead && ix->h_dead[(size_t)r]) continue;  // null queries get live rows only
-    const size_t i = (size_t)(std::lower_bound(keys.begin(), keys.end(), ix->h_labels[(size_t)r]) - keys.begin());
-    if (cnt[i] < LAB_FIRST) first[i * LAB_FIRST + (size_t)cnt[i]++] = (int)r;
+  const int64_t n = ix->n_rows;
+  int rc = rs.upload(ix->d_perm.p, n, ix->n_chunks_pad * CHUNK_ROWS, s);
+  if (rc != KV_OK) return rc;
+  if (&rs == &ix->labels) {
+    std::vector<int> keys(rs.h);
+    std::sort(keys.begin(), keys.end());
+    keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
+    std::vector<int> first(keys.size() * LAB_FIRST, -1), cnt(keys.size(), 0);
+    for (int64_t r = 0; r < n; r++) {
+      if (ix->tomb.is_dead(r)) continue;  // null queries get live rows only
+      const size_t i = (size_t)(std::lower_bound(keys.begin(), keys.end(), rs.h[(size_t)r]) - keys.begin());
+      if (cnt[i] < LAB_FIRST) first[i * LAB_FIRST + (size_t)cnt[i]++] = (int)r;
+    }
+    ix->n_lab = (int)keys.size();
+    KV_CUDA(ix->d_lab_keys.ensure(std::max<int64_t>((int64_t)keys.size(), 1)));
+    KV_CUDA(ix->d_lab_rows.ensure(std::max<int64_t>((int64_t)first.size(), 1)));
+    if (!keys.empty()) {
+      KV_CUDA(cudaMemcpyAsync(ix->d_lab_keys.p, keys.data(), keys.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+      KV_CUDA(cudaMemcpyAsync(ix->d_lab_rows.p, first.data(), first.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    }
+    if (n > 0) {
+      KV_CUDA(ix->d_chunk_sig.ensure(ix->n_chunks_pad));
+      chunk_sig_kernel<<<(unsigned)((ix->n_chunks_pad + 255) / 256), 256, 0, s>>>(rs.d_pos.p, ix->n_chunks_pad, ix->d_chunk_sig.p);
+      KV_CUDA(cudaGetLastError());
+    }
+    KV_CUDA(cudaStreamSynchronize(s));  // the host staging vectors go out of scope
   }
-  ix->n_lab = (int)keys.size();
-  KV_CUDA(ix->d_lab_keys.ensure(std::max<int64_t>((int64_t)keys.size(), 1)));
-  KV_CUDA(ix->d_lab_rows.ensure(std::max<int64_t>((int64_t)first.size(), 1)));
-  if (!keys.empty()) {
-    KV_CUDA(cudaMemcpyAsync(ix->d_lab_keys.p, keys.data(), keys.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-    KV_CUDA(cudaMemcpyAsync(ix->d_lab_rows.p, first.data(), first.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-  }
-  if (n > 0) {
-    KV_CUDA(ix->d_labels_row.ensure(n));
-    KV_CUDA(ix->d_label_pos.ensure(n_pos));
-    KV_CUDA(ix->d_chunk_sig.ensure(ix->n_chunks_pad));
-    KV_CUDA(cudaMemcpyAsync(ix->d_labels_row.p, ix->h_labels.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
-    label_pos_kernel<<<(unsigned)((n_pos + 255) / 256), 256, 0, s>>>(ix->d_perm.p, ix->d_labels_row.p, n, n_pos, ix->d_label_pos.p);
-    KV_CUDA(cudaGetLastError());
-    chunk_sig_kernel<<<(unsigned)((ix->n_chunks_pad + 255) / 256), 256, 0, s>>>(ix->d_label_pos.p, ix->n_chunks_pad, ix->d_chunk_sig.p);
-    KV_CUDA(cudaGetLastError());
-  }
-  KV_CUDA(cudaStreamSynchronize(s));  // the host staging vectors go out of scope
-  ix->labels_on_device = true;
+  rs.on_device = true;
   return KV_OK;
 }
 
-static bool labels_ready(const kv_index *ix) {
-  return ix->has_labels && ix->labels_on_device && (int64_t)ix->h_labels.size() == ix->n_rows;
+// the per-row sets a finalize rebuilds on the device: labels and groups
+static int upload_row_sets(kv_index *ix) {
+  const int rc = upload_row_set(ix, ix->labels);
+  return rc != KV_OK ? rc : upload_row_set(ix, ix->groups);
 }
 
 // A filtered batch never runs on labels that do not describe the current rows
 static int check_filter(const kv_index *ix, const char *fn) {
-  if (ix->has_filter && !labels_ready(ix))
+  if (ix->has_filter && !ix->labels.ready(ix->n_rows))
     return kv_fail(KV_ERR_STATE, "%s: the batch is filtered but the row labels are missing or stale (set them again after an append)", fn);
   return KV_OK;
 }
@@ -596,83 +648,42 @@ int kv_index_set_row_labels(kv_index *ix, const int32_t *labels, int64_t n) {
   if (!ix) return kv_fail(KV_ERR_INVALID, "kv_index_set_row_labels: NULL handle");
   std::lock_guard<std::mutex> g(ix->mu);
   if (!labels) {
-    ix->h_labels.clear();
-    ix->has_labels = ix->labels_on_device = false;
+    ix->labels.clear();
     return KV_OK;
   }
-  if (n != ix->n_rows)
-    return kv_fail(KV_ERR_INVALID, "kv_index_set_row_labels: %lld labels for an index of %lld rows", (long long)n,
-                   (long long)ix->n_rows);
-  for (int64_t i = 0; i < n; i++)
-    if (labels[i] < 0) return kv_fail(KV_ERR_INVALID, "kv_index_set_row_labels: label %d of row %lld is negative", labels[i], (long long)i);
-  ix->h_labels.assign(labels, labels + n);
-  ix->has_labels = true;
+  const int rc = ix->labels.set(labels, n, ix->n_rows, "kv_index_set_row_labels", "label");
+  if (rc != KV_OK) return rc;
   KV_CUDA(cudaSetDevice(ix->device));
-  return upload_labels(ix);
-}
-
-// The device copies of the row groups for the current layout: by row and by scan position.  Nothing to do until the
-// index is finalized; every finalize calls it again.
-static int upload_groups(kv_index *ix) {
-  ix->groups_on_device = false;
-  if (!ix->has_groups || !ix->finalized) return KV_OK;
-  cudaStream_t s = ix->stream;
-  const int64_t n = ix->n_rows, n_pos = ix->n_chunks_pad * CHUNK_ROWS;
-  if (n > 0) {
-    KV_CUDA(ix->d_groups_row.ensure(n));
-    KV_CUDA(ix->d_group_pos.ensure(n_pos));
-    KV_CUDA(cudaMemcpyAsync(ix->d_groups_row.p, ix->h_groups.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
-    label_pos_kernel<<<(unsigned)((n_pos + 255) / 256), 256, 0, s>>>(ix->d_perm.p, ix->d_groups_row.p, n, n_pos, ix->d_group_pos.p);
-    KV_CUDA(cudaGetLastError());
-    KV_CUDA(cudaStreamSynchronize(s));
-  }
-  ix->groups_on_device = true;
-  return KV_OK;
-}
-
-// the per-row sets a finalize rebuilds on the device: labels and groups
-static int upload_row_sets(kv_index *ix) {
-  const int rc = upload_labels(ix);
-  return rc != KV_OK ? rc : upload_groups(ix);
-}
-
-static bool groups_ready(const kv_index *ix) {
-  return ix->has_groups && ix->groups_on_device && (int64_t)ix->h_groups.size() == ix->n_rows;
+  return upload_row_set(ix, ix->labels);
 }
 
 int kv_index_set_row_groups(kv_index *ix, const int32_t *groups, int64_t n) {
   if (!ix) return kv_fail(KV_ERR_INVALID, "kv_index_set_row_groups: NULL handle");
   std::lock_guard<std::mutex> g(ix->mu);
   if (!groups) {
-    ix->h_groups.clear();
-    ix->has_groups = ix->groups_on_device = false;
+    ix->groups.clear();
     return KV_OK;
   }
   if (ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_index_set_row_groups: a Jaccard index (mode 1) has no distinct top-k");
-  if (n != ix->n_rows)
-    return kv_fail(KV_ERR_INVALID, "kv_index_set_row_groups: %lld groups for an index of %lld rows", (long long)n,
-                   (long long)ix->n_rows);
-  for (int64_t i = 0; i < n; i++)
-    if (groups[i] < 0) return kv_fail(KV_ERR_INVALID, "kv_index_set_row_groups: group %d of row %lld is negative", groups[i], (long long)i);
-  ix->h_groups.assign(groups, groups + n);
-  ix->has_groups = true;
+  const int rc = ix->groups.set(groups, n, ix->n_rows, "kv_index_set_row_groups", "group");
+  if (rc != KV_OK) return rc;
   KV_CUDA(cudaSetDevice(ix->device));
-  return upload_groups(ix);
+  return upload_row_set(ix, ix->groups);
 }
 
 // The device copies of the deletions for the current layout (d_perm must hold it): deleted flags by row, the live word
 // of every chunk and the first LAB_FIRST live rows.  Nothing while no row is deleted: the kernels then get NULL.
 static int upload_dead(kv_index *ix) {
-  if (!ix->n_dead || ix->n_rows == 0) return KV_OK;
+  if (!ix->tomb.any() || ix->n_rows == 0) return KV_OK;
   cudaStream_t s = ix->stream;
   const int64_t n = ix->n_rows;
   std::vector<int> first(LAB_FIRST, -1);
   for (int64_t r = 0, c = 0; r < n && c < LAB_FIRST; r++)
-    if (!ix->h_dead[(size_t)r]) first[(size_t)c++] = (int)r;
+    if (!ix->tomb.is_dead(r)) first[(size_t)c++] = (int)r;
   KV_CUDA(ix->d_dead.ensure(n));
   KV_CUDA(ix->d_alive.ensure(ix->n_chunks_pad));
   KV_CUDA(ix->d_first_live.ensure(LAB_FIRST));
-  KV_CUDA(cudaMemcpyAsync(ix->d_dead.p, ix->h_dead.data(), (size_t)n, cudaMemcpyHostToDevice, s));
+  KV_CUDA(cudaMemcpyAsync(ix->d_dead.p, ix->tomb.flags.data(), (size_t)n, cudaMemcpyHostToDevice, s));
   KV_CUDA(cudaMemcpyAsync(ix->d_first_live.p, first.data(), first.size() * sizeof(int), cudaMemcpyHostToDevice, s));
   alive_kernel<<<(unsigned)((ix->n_chunks_pad + 255) / 256), 256, 0, s>>>(ix->d_perm.p, ix->d_dead.p, n, ix->n_chunks_pad, ix->d_alive.p);
   KV_CUDA(cudaGetLastError());
@@ -681,40 +692,54 @@ static int upload_dead(kv_index *ix) {
 }
 
 // NULL while no row is deleted: the kernels' per-row and per-chunk tests are then skipped
-static const uint8_t *dead_rows(const kv_index *ix) { return ix->n_dead ? ix->d_dead.p : nullptr; }
-static const uint32_t *alive_words(const kv_index *ix) { return ix->n_dead ? ix->d_alive.p : nullptr; }
+static const uint8_t *dead_rows(const kv_index *ix) { return ix->tomb.any() ? ix->d_dead.p : nullptr; }
+static const uint32_t *alive_words(const kv_index *ix) { return ix->tomb.any() ? ix->d_alive.p : nullptr; }
 
 int kv_index_delete_rows(kv_index *ix, const int64_t *rows, int64_t n) {
   if (!ix || n < 0 || (n > 0 && !rows)) return kv_fail(KV_ERR_INVALID, "kv_index_delete_rows: bad arguments");
   std::lock_guard<std::mutex> g(ix->mu);
   if (ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_index_delete_rows: a Jaccard index (mode 1) has no row deletion");
-  for (int64_t i = 0; i < n; i++)
-    if (rows[i] < 0 || rows[i] >= ix->n_rows)
-      return kv_fail(KV_ERR_INVALID, "kv_index_delete_rows: row %lld outside 0..%lld", (long long)rows[i], (long long)ix->n_rows - 1);
   int64_t added = 0;
-  for (int64_t i = 0; i < n; i++) {
-    if (ix->h_dead.empty()) ix->h_dead.assign((size_t)ix->n_rows, 0);
-    uint8_t &d = ix->h_dead[(size_t)rows[i]];
-    if (!d) { d = 1; added++; }
-  }
-  if (!added) return KV_OK;  // duplicates and rows deleted before: nothing changes
-  ix->n_dead += added;
+  const int rc = ix->tomb.mark(rows, n, ix->n_rows, "kv_index_delete_rows", &added);
+  if (rc != KV_OK || !added) return rc;  // duplicates and rows deleted before: nothing changes
   // like an append: statistics and the device copies are stale until the next finalize
   ix->finalized = false;
-  ix->batch_valid = ix->range_valid = false;
+  ix->batch_valid = false;
+  drop_range(ix);
   return KV_OK;
 }
 
-int64_t kv_index_live_rows(const kv_index *ix) { return ix ? ix->n_rows - ix->n_dead : 0; }
+int64_t kv_index_live_rows(const kv_index *ix) { return ix ? ix->n_rows - ix->tomb.count : 0; }
 
 int kv_index_deleted_rows(kv_index *ix, uint8_t *out, int64_t n) {
   if (!ix || n < 0 || (n > 0 && !out)) return kv_fail(KV_ERR_INVALID, "kv_index_deleted_rows: bad arguments");
   std::lock_guard<std::mutex> g(ix->mu);
-  if (n != ix->n_rows)
-    return kv_fail(KV_ERR_INVALID, "kv_index_deleted_rows: %lld flags for an index of %lld rows", (long long)n, (long long)ix->n_rows);
-  if (ix->n_dead) memcpy(out, ix->h_dead.data(), (size_t)n);
-  else if (n) memset(out, 0, (size_t)n);
-  return KV_OK;
+  return ix->tomb.copy_out(out, n, ix->n_rows, "kv_index_deleted_rows");
+}
+
+// The end of both kinds of finalize (kind 1: full rebuild, 2: statistics-only refresh), once the scan layout is on the
+// device: row norms in scan order, the deletions and the chunk minima.  The index is then finalized for a vocabulary of V
+// features, the batch and the range result are dropped and the per-row sets are rebuilt for the layout.
+static int finish_finalize(kv_index *ix, int64_t V, int kind) {
+  cudaStream_t s = ix->stream;
+  const int64_t n = ix->n_rows;
+  if (n) {
+    rownorm_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(ix->indptr.p, ix->ids.p, ix->tf.p, ix->d_perm.p, n,
+                                                                    ix->d_bb64.p, ix->d_B64.p, ix->d_B32.p);
+    KV_CUDA(cudaGetLastError());
+  }
+  const int rc = upload_dead(ix);
+  if (rc != KV_OK) return rc;
+  chunk_meta_kernel<<<(unsigned)((ix->n_chunks_pad + 255) / 256), 256, 0, s>>>(ix->d_B32.p, n, ix->n_chunks, ix->n_chunks_pad,
+                                                                                alive_words(ix), ix->d_cminB.p);
+  KV_CUDA(cudaGetLastError());
+  KV_CUDA(cudaStreamSynchronize(s));
+  ix->V = V;
+  ix->finalized = true;
+  ix->batch_valid = false;
+  drop_range(ix);
+  ix->last_finalize_kind = kind;
+  return upload_row_sets(ix);
 }
 
 int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
@@ -758,7 +783,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
     int rc = live_counts(ix, Vz, &live);
     if (rc != KV_OK) return rc;
     if (V) KV_CUDA(cudaMemcpyAsync(ix->d_df.p, live, (size_t)V * 4, cudaMemcpyDeviceToDevice, s));
-    ix->n_total = n - ix->n_dead;
+    ix->n_total = n - ix->tomb.count;
   }
   if (V) {
     IdfTables T{ix->d_a64.p, ix->d_d64.p, ix->d_bb64.p, ix->d_univ.p, ix->d_utf.p};
@@ -811,20 +836,7 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
         KV_CUDA(cudaMemcpyAsync(ix->d_fslot.p, ix->h_fslot.data(), (size_t)Vz * sizeof(short), cudaMemcpyHostToDevice, s));
         KV_CUDA(cudaMemcpyAsync(ix->d_fslot2.p, ix->h_fslot2.data(), (size_t)Vz * sizeof(short), cudaMemcpyHostToDevice, s));
       }
-      rownorm_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(ix->indptr.p, ix->ids.p, ix->tf.p, ix->d_perm.p, n,
-                                                                      ix->d_bb64.p, ix->d_B64.p, ix->d_B32.p);
-      KV_CUDA(cudaGetLastError());
-      int rc = upload_dead(ix);
-      if (rc != KV_OK) return rc;
-      chunk_meta_kernel<<<(unsigned)((ix->n_chunks_pad + 255) / 256), 256, 0, s>>>(ix->d_B32.p, n, ix->n_chunks, ix->n_chunks_pad,
-                                                                                    alive_words(ix), ix->d_cminB.p);
-      KV_CUDA(cudaGetLastError());
-      KV_CUDA(cudaStreamSynchronize(s));
-      ix->V = V;
-      ix->finalized = true;
-      ix->batch_valid = ix->range_valid = false;
-      ix->last_finalize_kind = 2;
-      return upload_row_sets(ix);
+      return finish_finalize(ix, V, 2);
     }
   }
   ix->layout_valid = false;
@@ -850,23 +862,8 @@ int kv_index_finalize(kv_index *ix, int64_t vocab_size) {
     }
     for (const auto &o : L.ovf) { SL.ovf_keys.push_back(o.first); SL.ovf_vals.push_back(o.second); }
   }
-  int rc = upload_layout(ix, SL);
-  if (rc == KV_OK) rc = upload_dead(ix);
-  if (rc != KV_OK) return rc;
-  if (n) {
-    rownorm_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(ix->indptr.p, ix->ids.p, ix->tf.p, ix->d_perm.p, n,
-                                                                    ix->d_bb64.p, ix->d_B64.p, ix->d_B32.p);
-    KV_CUDA(cudaGetLastError());
-  }
-  chunk_meta_kernel<<<(unsigned)((ix->n_chunks_pad + 255) / 256), 256, 0, s>>>(ix->d_B32.p, n, ix->n_chunks, ix->n_chunks_pad,
-                                                                                alive_words(ix), ix->d_cminB.p);
-  KV_CUDA(cudaGetLastError());
-  KV_CUDA(cudaStreamSynchronize(s));
-  ix->V = V;
-  ix->finalized = true;
-  ix->batch_valid = ix->range_valid = false;
-  ix->last_finalize_kind = 1;
-  return upload_row_sets(ix);
+  const int rc = upload_layout(ix, SL);
+  return rc != KV_OK ? rc : finish_finalize(ix, V, 1);
 }
 
 int kv_index_last_finalize_kind(const kv_index *ix) { return ix ? ix->last_finalize_kind : 0; }
@@ -1020,6 +1017,25 @@ static bool csr_ok(const int64_t *q_indptr, const uint32_t *q_ids, const uint32_
 
 static int build_query_tables(kv_index *ix, int64_t n_q);
 
+// An upload replaces the resident batch: the old batch and the range result are dropped, and the exclusions, label
+// filter, distinct mode and irregular queries of the old batch go with it.
+static void start_batch(kv_index *ix) {
+  ix->batch_valid = false;
+  drop_range(ix);
+  ix->has_excl = ix->has_filter = ix->distinct = false;
+  ix->irr.clear();
+}
+
+// The new batch of n_q queries (n_null of them null) is resident: what the upload recorded, and the batch is valid.
+static void end_batch(kv_index *ix, int64_t n_q, int64_t n_null, int64_t h2d_bytes, unsigned long long f2_out) {
+  ix->batch_f2_outside = (int64_t)f2_out;
+  ix->batch_q = n_q;
+  ix->batch_tiles = (n_q + TILE_Q - 1) / TILE_Q;
+  ix->batch_null = n_null;
+  ix->batch_h2d_bytes = h2d_bytes;
+  ix->batch_valid = true;
+}
+
 static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   if (!ix->finalized) return kv_fail(KV_ERR_STATE, "kv_query_upload: index not finalized");
   int64_t n_q = 0, nnz = 0;
@@ -1042,9 +1058,7 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   if (n_q >= (1LL << 31) - TILE_Q) return kv_fail(KV_ERR_INVALID, "kv_query_upload: too many queries in one call");
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
-  ix->batch_valid = ix->range_valid = false;
-  ix->has_excl = ix->has_filter = ix->distinct = false;
-  ix->irr_q.clear(); ix->irr_indptr.assign(1, 0); ix->irr_ids.clear(); ix->irr_tf.clear(); ix->irr_oov.clear();
+  start_batch(ix);
   const int T = host_threads();
   const auto t_begin = std::chrono::steady_clock::now();
   auto ms_since = [](std::chrono::steady_clock::time_point t0) {
@@ -1140,16 +1154,11 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
     if (flag[(size_t)row] == 1) {
       null_list[n_null++] = (int)q;
     } else if (flag[(size_t)row] == 2) {
-      const int64_t a = q_indptr[row], b = q_indptr[row + 1];
-      ix->irr_q.push_back(q);
-      ix->irr_ids.insert(ix->irr_ids.end(), q_ids + a, q_ids + b);
-      ix->irr_tf.insert(ix->irr_tf.end(), q_tf + a, q_tf + b);
-      ix->irr_indptr.push_back((int64_t)ix->irr_ids.size());
-      ix->irr_oov.push_back(q_oov[row]);
+      const int64_t a = q_indptr[row];
+      ix->irr.add(q, q_ids + a, q_tf + a, q_indptr[row + 1] - a, q_oov[row]);
     }
   }
 
-  const int64_t n_tiles = (n_q + TILE_Q - 1) / TILE_Q;
   KV_CUDA(ix->d_q_indptr.ensure(n_q + 1));
   KV_CUDA(ix->d_q_ids.ensure(std::max<int64_t>(nnz, 1)));
   KV_CUDA(ix->d_q_tf.ensure(std::max<int64_t>(nnz, 1)));
@@ -1173,12 +1182,7 @@ static int prepare_batch_runs(kv_index *ix, const QueryRun *runs, int n_runs) {
   unsigned long long f2_out = 0;
   KV_CUDA(cudaMemcpyAsync(&f2_out, ix->d_f2out.p, sizeof(f2_out), cudaMemcpyDeviceToHost, s));
   KV_CUDA(cudaStreamSynchronize(s));  // the pinned staging buffers may be rewritten by the next call
-  ix->batch_f2_outside = (int64_t)f2_out;
-  ix->batch_q = n_q;
-  ix->batch_tiles = n_tiles;
-  ix->batch_null = n_null;
-  ix->batch_h2d_bytes = (n_q + 1) * 8 + nnz * 8 + n_q * 8 + 3 * n_q * (int64_t)sizeof(int) + n_q;
-  ix->batch_valid = true;
+  end_batch(ix, n_q, n_null, (n_q + 1) * 8 + nnz * 8 + n_q * 8 + 3 * n_q * (int64_t)sizeof(int) + n_q, f2_out);
   cudaEventElapsedTime(&ix->last_ms[0], ix->ev[0], ix->ev[1]);
   ix->last_prepare_ms[3] = ms_since(t_mark);
   return KV_OK;
@@ -1340,9 +1344,7 @@ static int prepare_batch_text(kv_index *ix, kv_vocab_mirror *m, const kv_vocab *
                    mirror_device(m), ix->device);
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
-  ix->batch_valid = ix->range_valid = false;
-  ix->has_excl = ix->has_filter = ix->distinct = false;
-  ix->irr_q.clear(); ix->irr_indptr.assign(1, 0); ix->irr_ids.clear(); ix->irr_tf.clear(); ix->irr_oov.clear();
+  start_batch(ix);
   const auto t_begin = std::chrono::steady_clock::now();
 
   // ---- the text goes up and is featurised into the query CSR (by row) ----
@@ -1408,28 +1410,22 @@ static int prepare_batch_text(kv_index *ix, kv_vocab_mirror *m, const kv_vocab *
     KV_CUDA(cudaMemcpyAsync(ix->h_q_indptr.p, ix->d_q_indptr.p, (size_t)(n_q + 1) * 8, cudaMemcpyDeviceToHost, s));
     KV_CUDA(cudaMemcpyAsync(ix->h_q_oov.p, ix->d_q_oov.p, (size_t)n_q * 8, cudaMemcpyDeviceToHost, s));
     KV_CUDA(cudaStreamSynchronize(s));
+    std::vector<uint32_t> ids, tf;
     for (int64_t i = 0; i < n_q; i++) {
       if (ix->h_flags.p[i] != 2) continue;
-      const int64_t q = qperm[i], a = ix->h_q_indptr.p[q], b = ix->h_q_indptr.p[q + 1];
-      const size_t at = ix->irr_ids.size();
-      ix->irr_q.push_back(q);
-      ix->irr_ids.resize(at + (size_t)(b - a));
-      ix->irr_tf.resize(at + (size_t)(b - a));
-      if (b > a) {
-        KV_CUDA(cudaMemcpyAsync(ix->irr_ids.data() + at, ix->d_q_ids.p + a, (size_t)(b - a) * 4, cudaMemcpyDeviceToHost, s));
-        KV_CUDA(cudaMemcpyAsync(ix->irr_tf.data() + at, ix->d_q_tf.p + a, (size_t)(b - a) * 4, cudaMemcpyDeviceToHost, s));
+      const int64_t q = qperm[i], a = ix->h_q_indptr.p[q], nnz_q = ix->h_q_indptr.p[q + 1] - a;
+      ids.resize((size_t)nnz_q);
+      tf.resize((size_t)nnz_q);
+      if (nnz_q) {
+        KV_CUDA(cudaMemcpyAsync(ids.data(), ix->d_q_ids.p + a, (size_t)nnz_q * 4, cudaMemcpyDeviceToHost, s));
+        KV_CUDA(cudaMemcpyAsync(tf.data(), ix->d_q_tf.p + a, (size_t)nnz_q * 4, cudaMemcpyDeviceToHost, s));
+        KV_CUDA(cudaStreamSynchronize(s));
       }
-      ix->irr_indptr.push_back((int64_t)ix->irr_ids.size());
-      ix->irr_oov.push_back(ix->h_q_oov.p[q]);
+      ix->irr.add(q, ids.data(), tf.data(), nnz_q, ix->h_q_oov.p[q]);
     }
   }
   KV_CUDA(cudaStreamSynchronize(s));
-  ix->batch_f2_outside = (int64_t)f2_out;
-  ix->batch_q = n_q;
-  ix->batch_tiles = (n_q + TILE_Q - 1) / TILE_Q;
-  ix->batch_null = n_null;
-  ix->batch_h2d_bytes = (offsets[n_q] - offsets[0]) + (n_q + 1) * 8 + n_null * (int64_t)sizeof(int);
-  ix->batch_valid = true;
+  end_batch(ix, n_q, n_null, (offsets[n_q] - offsets[0]) + (n_q + 1) * 8 + n_null * (int64_t)sizeof(int), f2_out);
   cudaEventElapsedTime(&ix->last_prepare_ms[1], ix->evq[0], ix->evq[1]);
   cudaEventElapsedTime(&ix->last_prepare_ms[2], ix->evq[1], ix->evq[2]);
   cudaEventElapsedTime(&ix->last_prepare_ms[3], ix->evq[2], ix->evq[3]);
@@ -1459,7 +1455,7 @@ struct Batch {
 static int launch_merge(kv_index *ix, const Batch &b, int64_t n_lists) {
   if (b.distinct)
     merge_topk_distinct_kernel<<<(unsigned)((b.n_q * 32 + 255) / 256), 256, 0, ix->stream>>>(
-        ix->d_part_s.p, ix->d_part_r.p, (int)n_lists, b.n_q, b.k, b.n_q * b.k, ix->d_qperm.p, ix->d_groups_row.p, ix->row_base,
+        ix->d_part_s.p, ix->d_part_r.p, (int)n_lists, b.n_q, b.k, b.n_q * b.k, ix->d_qperm.p, ix->groups.d_row.p, ix->row_base,
         b.out_s, b.out_r);
   else
     merge_topk_kernel<<<(unsigned)((b.n_q * 32 + 255) / 256), 256, 0, ix->stream>>>(
@@ -1477,14 +1473,14 @@ static ScanParams scan_params(const kv_index *ix, const Batch &b) {
   SP.ovf_keys = ix->d_ovf_keys.p; SP.ovf_vals = ix->d_ovf_vals.p; SP.n_ovf = ix->n_ovf;
   SP.qtab = ix->d_qtab.p; SP.q_nq = qc; SP.q_uw = ix->d_qfix.p; SP.q_uc = ix->d_qfix.p + b.n_q;
   SP.q_excl = ix->has_excl ? ix->d_excl_sorted.p : nullptr; SP.gthr = b.range ? ix->d_rthr.p : ix->d_gthr.p;
-  if (ix->has_filter) { SP.q_label = ix->d_filt_sorted.p; SP.label_pos = ix->d_label_pos.p; SP.chunk_sig = ix->d_chunk_sig.p; }
+  if (ix->has_filter) { SP.q_label = ix->d_filt_sorted.p; SP.label_pos = ix->labels.d_pos.p; SP.chunk_sig = ix->d_chunk_sig.p; }
   SP.alive = alive_words(ix);
   for (int i = 0; i < 7; i++) SP.peer_gthr[i] = i < b.n_peers ? ix->peer_gthr[i] : nullptr;
   SP.n_peers = b.n_peers; SP.stats = ix->d_stats.p; SP.n_q = b.n_q; SP.k = b.k;
   SP.part_scores = ix->d_part_s.p; SP.part_rows = ix->d_part_r.p; SP.max_pages = b.max_pages;
-  SP.qperm = ix->d_qperm.p; SP.range_out = ix->d_range.p; SP.range_count = ix->d_range_count.p;
-  SP.range_cap = (unsigned long long)ix->d_range.cap;
-  SP.group_pos = b.distinct ? ix->d_group_pos.p : nullptr;
+  SP.qperm = ix->d_qperm.p; SP.range_out = ix->range.pairs.p; SP.range_count = ix->range.d_count.p;
+  SP.range_cap = ix->range.capacity();
+  SP.group_pos = b.distinct ? ix->groups.d_pos.p : nullptr;
   return SP;
 }
 
@@ -1581,7 +1577,7 @@ static int run_exhaustive(kv_index *ix, Batch &b) {
 }
 
 // Jaccard path: token sets have no text structure to prune on -- the dense-regime kernel K3 scores every chunk for a
-// whole scan group at once.  A threshold search runs K3-R, which appends to d_jrange instead of filling lists.
+// whole scan group at once.  A threshold search runs K3-R, which appends to ix->jrange instead of filling lists.
 static int run_jaccard(kv_index *ix, Batch &b) {
   const int64_t n_q = b.n_q, n_groups = b.n_groups;
   const int64_t jsplits = std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>((4LL * ix->sm_count + n_groups - 1) / n_groups, 256),
@@ -1600,7 +1596,7 @@ static int run_jaccard(kv_index *ix, Batch &b) {
   JP.n_q = n_q; JP.k = b.k; JP.n_splits = (int)jsplits; JP.part_scores = ix->d_part_s.p; JP.part_rows = ix->d_part_r.p;
   const dim3 grid((unsigned)n_groups, (unsigned)jsplits);
   if (b.range) {
-    const JaccardRangeOut R{ix->d_qperm.p, ix->d_jrange.p, ix->d_range_count.p, (unsigned long long)ix->d_jrange.cap};
+    const JaccardRangeOut R{ix->d_qperm.p, ix->jrange.pairs.p, ix->jrange.d_count.p, ix->jrange.capacity()};
     jaccard_scan_kernel<true><<<grid, J_WARPS * 32, jaccard_smem_bytes(0), ix->stream>>>(JP, R);
   } else {
     jaccard_scan_kernel<false><<<grid, J_WARPS * 32, jaccard_smem_bytes(b.k), ix->stream>>>(JP, JaccardRangeOut{});
@@ -1677,7 +1673,7 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
   if (ix->has_filter && (ix->gthr_exported || ix->n_peers))
     return kv_fail(KV_ERR_INVALID, "kv_topk_resident: a label filter cannot be combined with the threshold exchange of a row-sharded GFKB");
   if (ix->distinct) {
-    if (!groups_ready(ix))
+    if (!ix->groups.ready(ix->n_rows))
       return kv_fail(KV_ERR_STATE, "kv_topk_resident: the batch is distinct but the row groups are missing or stale (set them again after an append)");
     // a shard's seed k-th score is no lower bound of the global k-th GROUP score: one group can count on several shards
     if (phase != 0 || ix->gthr_exported || ix->n_peers)
@@ -1769,7 +1765,7 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
   if (ix->batch_null && b.distinct) {
     fill_null_distinct_kernel<<<(unsigned)((ix->batch_null * 32 + 255) / 256), 256, 0, s>>>(
         ix->d_qperm.p + n_q, (int)ix->batch_null, k, ix->n_rows, ix->row_base, ix->has_excl ? ix->d_excl_orig.p : nullptr,
-        ix->has_filter ? ix->d_filt_orig.p : nullptr, ix->d_labels_row.p, dead_rows(ix), ix->d_groups_row.p, d_out_s, d_out_r);
+        ix->has_filter ? ix->d_filt_orig.p : nullptr, ix->labels.d_row.p, dead_rows(ix), ix->groups.d_row.p, d_out_s, d_out_r);
     KV_CUDA(cudaGetLastError());
     b.launches++;
   } else if (ix->batch_null) {
@@ -1778,22 +1774,23 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
                                                                                   ix->n_rows, ix->row_base,
                                                                                   ix->has_excl ? ix->d_excl_orig.p : nullptr,
                                                                                   ix->has_filter ? ix->d_filt_orig.p : nullptr, L,
-                                                                                  ix->n_dead ? ix->d_first_live.p : nullptr, d_out_s, d_out_r);
+                                                                                  ix->tomb.any() ? ix->d_first_live.p : nullptr, d_out_s, d_out_r);
     KV_CUDA(cudaGetLastError());
     b.launches++;
   }
-  for (size_t i = 0; i < ix->irr_q.size(); i++) {
-    const int64_t q = ix->irr_q[i], a = ix->irr_indptr[i], e = ix->irr_indptr[i + 1];
-    rc = score_impl(ix, ix->irr_ids.data() + a, ix->irr_tf.data() + a, e - a, ix->irr_oov[i], nullptr);
+  const IrregularQueries &irr = ix->irr;
+  for (size_t i = 0; i < irr.q.size(); i++) {
+    const int64_t q = irr.q[i], a = irr.indptr[i], e = irr.indptr[i + 1];
+    rc = score_impl(ix, irr.ids.data() + a, irr.tf.data() + a, e - a, irr.oov[i], nullptr);
     if (rc != KV_OK) return rc;
     if (b.distinct)
       select_topk_distinct_kernel<<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
-                                                     ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->d_labels_row.p,
+                                                     ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->labels.d_row.p,
                                                      ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix),
-                                                     ix->d_groups_row.p, d_out_s + q * k, d_out_r + q * k);
+                                                     ix->groups.d_row.p, d_out_s + q * k, d_out_r + q * k);
     else
       select_topk_kernel<<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
-                                            ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->d_labels_row.p,
+                                            ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->labels.d_row.p,
                                             ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix), d_out_s + q * k,
                                             d_out_r + q * k);
     KV_CUDA(cudaGetLastError());
@@ -1825,13 +1822,13 @@ static int finish_batch(kv_index *ix) {
   return check_pool(ix);
 }
 
-// Threshold search over the resident batch: every pair with score >= thr lands in d_range (d_jrange on a Jaccard
+// Threshold search over the resident batch: every pair with score >= thr lands in ix->range (ix->jrange on a Jaccard
 // index), *n_pairs = their count.  When they do not fit, the buffer grows to the exact count and only the scan and the
 // fallbacks run again (the candidate lists depend on the threshold alone).  Events: evk[2] -> evk[3] bound pass 1,
 // evk[3] -> evk[4] scan, evk[4] -> evk[5] irregular-query fallbacks.  Caller holds ix->mu.
 static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
   const char *fn = "kv_range_resident";
-  ix->range_valid = false;
+  drop_range(ix);
   if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "%s: no query batch uploaded", fn);
   int rc = check_filter(ix, fn);
   if (rc != KV_OK) return rc;
@@ -1844,13 +1841,12 @@ static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
   if (rc != KV_OK) return rc;
   const int64_t n_q = b.n_q;
   KV_CUDA(ix->d_rthr.ensure(n_q));
-  if (jac) KV_CUDA(ix->d_jrange.ensure(65536));
-  else KV_CUDA(ix->d_range.ensure(65536));
-  auto range_cap = [&] { return (unsigned long long)(jac ? ix->d_jrange.cap : ix->d_range.cap); };
-  KV_CUDA(ix->d_range_count.ensure(1));
+  rc = jac ? ix->jrange.prepare(s) : ix->range.prepare(s);
+  if (rc != KV_OK) return rc;
+  auto range_cap = [&] { return jac ? ix->jrange.capacity() : ix->range.capacity(); };
+  unsigned long long *d_count = jac ? ix->jrange.d_count.p : ix->range.d_count.p;
   for (auto &e : ix->evk) KV_CUDA(cudaEventRecord(e, s));
   KV_CUDA(cudaMemsetAsync(ix->d_stats.p, 0, 8 * sizeof(unsigned long long), s));
-  KV_CUDA(cudaMemsetAsync(ix->d_range_count.p, 0, sizeof(unsigned long long), s));
   float ms[5] = {0, 0, 0, 0, 0};
   unsigned long long count = 0;
   if (ix->n_rows > 0) {
@@ -1870,26 +1866,27 @@ static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
       }
       if (rc != KV_OK) return rc;
       KV_CUDA(cudaEventRecord(ix->evk[4], s));
-      for (size_t i = 0; i < ix->irr_q.size(); i++) {
-        const int64_t q = ix->irr_q[i], a = ix->irr_indptr[i], e = ix->irr_indptr[i + 1];
-        rc = score_impl(ix, ix->irr_ids.data() + a, ix->irr_tf.data() + a, e - a, ix->irr_oov[i], nullptr);
+      const IrregularQueries &irr = ix->irr;
+      for (size_t i = 0; i < irr.q.size(); i++) {
+        const int64_t q = irr.q[i], a = irr.indptr[i], e = irr.indptr[i + 1];
+        rc = score_impl(ix, irr.ids.data() + a, irr.tf.data() + a, e - a, irr.oov[i], nullptr);
         if (rc != KV_OK) return rc;
         const unsigned grid = (unsigned)std::min<int64_t>((ix->n_rows + 255) / 256, 8LL * ix->sm_count);
         const int64_t excl = ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1;
         if (jac) {
-          const double nq = host_query_norm(ix, ix->irr_ids.data() + a, ix->irr_tf.data() + a, e - a, ix->irr_oov[i]);  // |q|
+          const double nq = host_query_norm(ix, irr.ids.data() + a, irr.tf.data() + a, e - a, irr.oov[i]);  // |q|
           jaccard_select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->d_B64.p, ix->d_invperm.p, ix->n_rows, nq, thr, excl,
-                                                           (int)q, ix->d_jrange.p, ix->d_range_count.p, range_cap());
+                                                           (int)q, ix->jrange.pairs.p, d_count, range_cap());
         } else {
-          select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, thr, excl, ix->d_labels_row.p,
-                                                   ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix), (int)q, ix->d_range.p,
-                                                   ix->d_range_count.p, range_cap());
+          select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, thr, excl, ix->labels.d_row.p,
+                                                   ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix), (int)q, ix->range.pairs.p,
+                                                   d_count, range_cap());
         }
         KV_CUDA(cudaGetLastError());
         b.launches += 2;
       }
       KV_CUDA(cudaEventRecord(ix->evk[5], s));
-      KV_CUDA(cudaMemcpyAsync(&count, ix->d_range_count.p, sizeof(count), cudaMemcpyDeviceToHost, s));
+      KV_CUDA(cudaMemcpyAsync(&count, d_count, sizeof(count), cudaMemcpyDeviceToHost, s));
       KV_CUDA(cudaMemcpyAsync(ix->last_stats, ix->d_stats.p, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
       if (b.prune) KV_CUDA(cudaMemcpyAsync(&ix->last_stats[6], ix->d_pool_ctl.p, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
       KV_CUDA(cudaStreamSynchronize(s));
@@ -1903,23 +1900,17 @@ static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
       ms[3] += t_scan;
       ms[4] += t_fallback;
       if (count <= range_cap()) break;
-      if ((jac ? ix->d_jrange.ensure((int64_t)count) : ix->d_range.ensure((int64_t)count)) != cudaSuccess) {
-        cudaGetLastError();
-        return kv_fail(KV_ERR_NOMEM, "%s: %llu pairs reach the threshold; their buffer does not fit in device memory "
-                                     "(raise the threshold or split the query batch)", fn, count);
-      }
+      if ((rc = jac ? ix->jrange.grow(count, s, fn) : ix->range.grow(count, s, fn)) != KV_OK) return rc;
       // the counters describe one run: the bound pass's stay, the scan's start again
       KV_CUDA(cudaMemsetAsync(ix->d_stats.p, 0, 2 * sizeof(unsigned long long), s));
-      KV_CUDA(cudaMemsetAsync(ix->d_range_count.p, 0, sizeof(unsigned long long), s));
     }
   } else {
     for (auto &st : ix->last_stats) st = 0;
   }
   for (int i = 0; i < 5; i++) ix->last_kernel_ms[i] = ms[i];
   ix->last_launches = b.launches;
-  ix->range_q = n_q;
-  ix->range_pairs = (int64_t)count;
-  ix->range_valid = true;
+  if (jac) ix->jrange.commit(n_q, (int64_t)count);
+  else ix->range.commit(n_q, (int64_t)count);
   *n_pairs = (int64_t)count;
   return KV_OK;
 }
@@ -2047,11 +2038,11 @@ int kv_selfjoin_upload(kv_index *ix, int64_t q_begin, int64_t q_end) {
   QueryRun R;
   R.indptr = ip.data(); R.ids = ix->h_ids.data() + base; R.tf = tf32.data(); R.n_q = n;
   std::vector<uint8_t> flags;
-  if (ix->n_dead) {  // a deleted row's query is switched off (flag 3): no path answers it, its list stays (-inf, -1)
+  if (ix->tomb.any()) {  // a deleted row's query is switched off (flag 3): no path answers it, its list stays (-inf, -1)
     flags.resize((size_t)n);
     classify_queries(ix, ip.data(), R.ids, R.tf, n, flags.data(), host_threads());
     for (int64_t i = 0; i < n; i++)
-      if (ix->h_dead[(size_t)(q_begin + i)]) flags[(size_t)i] = 3;
+      if (ix->tomb.is_dead(q_begin + i)) flags[(size_t)i] = 3;
     R.flags = flags.data();
   }
   int rc = prepare_batch_runs(ix, &R, 1);
@@ -2144,7 +2135,7 @@ int kv_query_set_filter(kv_index *ix, const int32_t *labels, int64_t n_q) {
   }
   ix->has_filter = false;
   if (!any) return KV_OK;  // every query unfiltered: the unfiltered batch
-  if (!labels_ready(ix))
+  if (!ix->labels.ready(ix->n_rows))
     return kv_fail(KV_ERR_STATE, "kv_query_set_filter: the index has no row labels for its current rows (kv_index_set_row_labels)");
   KV_CUDA(cudaSetDevice(ix->device));
   ix->h_filt_orig.assign(labels, labels + n_q);
@@ -2165,7 +2156,7 @@ int kv_query_set_distinct(kv_index *ix, int on) {
   if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_query_set_distinct: no query batch uploaded");
   ix->distinct = false;
   if (!on) return KV_OK;
-  if (!groups_ready(ix))
+  if (!ix->groups.ready(ix->n_rows))
     return kv_fail(KV_ERR_STATE, "kv_query_set_distinct: the index has no row groups for its current rows (kv_index_set_row_groups)");
   ix->distinct = true;
   return KV_OK;
@@ -2189,58 +2180,35 @@ int kv_range_resident(kv_index *ix, float threshold, int64_t *n_pairs) {
 static int check_count_outputs(const kv_index *ix, const void *inter, const void *uni, const char *fn) {
   if (!ix->jaccard && (inter || uni))
     return kv_fail(KV_ERR_INVALID, "%s: a TF-IDF index has no count outputs (pass NULL for inter and uni)", fn);
-  if (ix->jaccard && ix->range_valid && ix->range_pairs > 0 && (!inter || !uni))
+  if (ix->jaccard && ix->jrange.valid && ix->jrange.n_pairs > 0 && (!inter || !uni))
     return kv_fail(KV_ERR_INVALID, "%s: a Jaccard index returns the exact counts (inter and uni are required)", fn);
   return KV_OK;
 }
 
 // The pairs come back in emit order, which the scan does not fix; scores are exact integer sums (Jaccard: the quotient
 // inter / union) rounded once, so (score desc, row asc) is a total order of each query's pairs and the result is
-// deterministic.  Both fetches order the pairs on the device (range_order.cu, in the pair buffer itself: the fetch
-// consumes the result) and copy the ordered arrays back.  Once ordering has started the result is gone whatever
-// happens; a scratch allocation that fails first (KV_ERR_NOMEM) leaves it for another try.  The records of a Jaccard
-// index hold local rows: the ordering adds row_base.
+// deterministic.  Both fetches order the pairs on the device and consume the result (RangeResult).
 int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores, int32_t *inter, int32_t *uni) {
-  const char *fn = "kv_range_fetch";
+  const char *fn = "kv_range_fetch", *search = "kv_range_resident";
   if (!ix || !indptr) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
   std::lock_guard<std::mutex> g(ix->mu);
-  int rc = check_count_outputs(ix, inter, uni, fn);
+  const int rc = check_count_outputs(ix, inter, uni, fn);
   if (rc != KV_OK) return rc;
-  if (!ix->range_valid) return kv_fail(KV_ERR_STATE, "%s: no threshold search result (kv_range_resident first)", fn);
-  const int64_t n_q = ix->range_q, n = ix->range_pairs;
-  if (n > 0 && (!rows || !scores)) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
-  KV_CUDA(cudaSetDevice(ix->device));
-  rc = ix->jaccard ? range_order_to_host(ix->d_jrange.p, n, n_q, ix->row_base, indptr, rows, scores, inter, uni, ix->rsort,
-                                         ix->stream, fn)
-                   : range_order_to_host(ix->d_range.p, n, n_q, 0, indptr, rows, scores, nullptr, nullptr, ix->rsort, ix->stream, fn);
-  if (rc != KV_ERR_NOMEM) ix->range_valid = false;
-  return rc;
+  return ix->jaccard ? ix->jrange.fetch_host(fn, search, ix->device, ix->stream, ix->rsort, ix->row_base, indptr, rows, scores, inter, uni)
+                     : ix->range.fetch_host(fn, search, ix->device, ix->stream, ix->rsort, ix->row_base, indptr, rows, scores, inter, uni);
 }
 
 // Device outputs: the same arrays, written to caller-owned device memory of the index's device.
 int kv_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores, void *d_inter, void *d_uni) {
-  const char *fn = "kv_range_fetch_device";
+  const char *fn = "kv_range_fetch_device", *search = "kv_range_resident";
   if (!ix) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
   std::lock_guard<std::mutex> g(ix->mu);
-  int rc = check_count_outputs(ix, d_inter, d_uni, fn);
+  const int rc = check_count_outputs(ix, d_inter, d_uni, fn);
   if (rc != KV_OK) return rc;
-  if (!ix->range_valid) return kv_fail(KV_ERR_STATE, "%s: no threshold search result (kv_range_resident first)", fn);
-  const int64_t n_q = ix->range_q, n = ix->range_pairs;
-  rc = check_device_ptr(d_indptr, ix->device, 8, "indptr", fn);
-  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_rows, ix->device, 8, "rows", fn);
-  if (rc == KV_OK && n > 0) rc = check_device_ptr(d_scores, ix->device, 4, "scores", fn);
-  if (rc == KV_OK && n > 0 && ix->jaccard) rc = check_device_ptr(d_inter, ix->device, 4, "inter", fn);
-  if (rc == KV_OK && n > 0 && ix->jaccard) rc = check_device_ptr(d_uni, ix->device, 4, "uni", fn);
-  if (rc != KV_OK) return rc;
-  KV_CUDA(cudaSetDevice(ix->device));
-  rc = ix->jaccard ? range_order_device(ix->d_jrange.p, n, n_q, ix->row_base, (int64_t *)d_indptr, (int64_t *)d_rows,
-                                        (float *)d_scores, (int32_t *)d_inter, (int32_t *)d_uni, ix->rsort, ix->stream, fn)
-                   : range_order_device(ix->d_range.p, n, n_q, 0, (int64_t *)d_indptr, (int64_t *)d_rows, (float *)d_scores,
-                                        nullptr, nullptr, ix->rsort, ix->stream, fn);
-  if (rc != KV_ERR_NOMEM) ix->range_valid = false;
-  if (rc != KV_OK) return rc;
-  KV_CUDA(cudaStreamSynchronize(ix->stream));
-  return KV_OK;
+  return ix->jaccard ? ix->jrange.fetch_device(fn, search, ix->device, ix->stream, ix->rsort, ix->row_base, d_indptr, d_rows,
+                                               d_scores, d_inter, d_uni)
+                     : ix->range.fetch_device(fn, search, ix->device, ix->stream, ix->rsort, ix->row_base, d_indptr, d_rows,
+                                              d_scores, d_inter, d_uni);
 }
 
 int kv_index_thresholds_export(kv_index *ix, int64_t capacity, void *handle_out) {
@@ -2562,7 +2530,7 @@ extern "C" int kv_index_layout_load(kv_index *ix, const char *path) {
   int rc = upload_layout(ix, SL);
   if (rc != KV_OK) return rc;
   ix->finalized = false;
-  ix->labels_on_device = ix->groups_on_device = false;  // positions changed: the finalize that follows rebuilds them
+  ix->labels.on_device = ix->groups.on_device = false;  // positions changed: the finalize that follows rebuilds them
   return KV_OK;
 }
 

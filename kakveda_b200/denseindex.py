@@ -14,16 +14,13 @@ import numpy as np
 
 from . import _capi, _devout
 from ._capi import no_distinct
+from .similarity import _ptr
 
 
 def to_bf16_bits(x: np.ndarray) -> np.ndarray:
     """float32 -> bfloat16 bit patterns (uint16), round-to-nearest-even."""
     u = np.ascontiguousarray(x, dtype=np.float32).view(np.uint32).astype(np.uint64)
     return (((u + 0x7FFF + ((u >> 16) & 1)) >> 16) & 0xFFFF).astype(np.uint16)
-
-
-def _ptr(a: np.ndarray, t):
-    return a.ctypes.data_as(C.POINTER(t))
 
 
 class DenseIndex:
@@ -169,18 +166,37 @@ class DenseIndex:
                                                    rows.ctypes.data_as(C.POINTER(C.c_int64))))
         return scores, rows
 
+    def _range_search_device(self, queries, threshold: float, exclude_base: int = -1,
+                             labels: Optional[np.ndarray] = None) -> int:
+        """Threshold search of queries on the device (a contiguous torch bfloat16 tensor [Q, dim]); returns the pair
+        count.  The result stays in the handle until ``_range_fetch_into``.  Caller holds ``_lock``."""
+        import torch
+
+        assert queries.is_cuda and queries.is_contiguous() and queries.element_size() == 2 and queries.shape[-1] == self.dim
+        torch.cuda.current_stream(queries.device).synchronize()  # the library reads the queries on its own stream
+        self._set_query_filter(labels, queries.shape[0])
+        n = C.c_int64(0)
+        _capi.check(_capi.load().kv_dense_range_device(self._h, C.c_void_p(queries.data_ptr()), queries.shape[0],
+                                                       np.float32(threshold), exclude_base, C.byref(n)))
+        return n.value
+
+    def _range_fetch_into(self, out, device_out: bool = True) -> None:
+        """Fetch the last search's result into ``out`` = ``(indptr, rows, scores)`` of its query and pair counts: torch
+        tensors or views on the index's device, or (not ``device_out``) NumPy arrays.  Caller holds ``_lock``."""
+        if device_out:
+            _capi.check(_capi.load().kv_dense_range_fetch_device(self._h, *_devout.ptrs(out)))
+        else:
+            _capi.check(_capi.load().kv_dense_range_fetch(self._h, _ptr(out[0], C.c_int64), _ptr(out[1], C.c_int64),
+                                                          _ptr(out[2], C.c_float)))
+
     def _range_fetch(self, n_q: int, n_pairs: int, device_out: bool = False):
+        """The last search's result, ``(indptr, rows, scores)``.  Caller holds ``_lock``."""
         if device_out:
             out = _devout.range_arrays(self.device, n_q, n_pairs)
-            _capi.check(_capi.load().kv_dense_range_fetch_device(self._h, *_devout.ptrs(out)))
-            return out
-        indptr = np.empty(n_q + 1, dtype=np.int64)
-        rows = np.empty(n_pairs, dtype=np.int64)
-        scores = np.empty(n_pairs, dtype=np.float32)
-        _capi.check(_capi.load().kv_dense_range_fetch(self._h, indptr.ctypes.data_as(C.POINTER(C.c_int64)),
-                                                      rows.ctypes.data_as(C.POINTER(C.c_int64)),
-                                                      scores.ctypes.data_as(C.POINTER(C.c_float))))
-        return indptr, rows, scores
+        else:
+            out = (np.empty(n_q + 1, np.int64), np.empty(n_pairs, np.int64), np.empty(n_pairs, np.float32))
+        self._range_fetch_into(out, device_out)
+        return out
 
     def range(self, queries: np.ndarray, threshold: float, device_out: bool = False, labels: Optional[np.ndarray] = None):
         """Threshold search: every (query, row) pair whose cosine (the float32 value ``topk`` reports, bit for bit) is
@@ -203,17 +219,9 @@ class DenseIndex:
         """``range`` of queries on the device (a contiguous torch bfloat16 tensor [Q, dim]); results on the host, or
         with ``device_out`` as torch tensors on the index's device.
         ``exclude_base >= 0``: query q never matches GLOBAL row ``exclude_base + q``.  ``labels`` as in ``range``."""
-        import torch
-
-        assert queries.is_cuda and queries.is_contiguous() and queries.element_size() == 2 and queries.shape[-1] == self.dim
-        n_q = queries.shape[0]
-        torch.cuda.current_stream(queries.device).synchronize()  # the library reads the queries on its own stream
-        n = C.c_int64(0)
         with self._lock:
-            self._set_query_filter(labels, n_q)
-            _capi.check(_capi.load().kv_dense_range_device(self._h, C.c_void_p(queries.data_ptr()), n_q,
-                                                           np.float32(threshold), exclude_base, C.byref(n)))
-            return self._range_fetch(n_q, n.value, device_out)
+            n = self._range_search_device(queries, threshold, exclude_base, labels)
+            return self._range_fetch(queries.shape[0], n, device_out)
 
     def selfjoin_range(self, threshold: float, lo: int = 0, hi: int | None = None, device_out: bool = False,
                        same_label: bool = False):

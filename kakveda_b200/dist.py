@@ -203,11 +203,6 @@ def merge_range_on_device(device: int, gathered, n_q: int, pairs, jaccard: bool 
     return out
 
 
-def _fetch_into(h, views) -> None:
-    """``kv_range_fetch_device`` of a kv_index handle's threshold-search result into ``views``."""
-    _capi.check(_capi.load().kv_range_fetch_device(h, *_devout.ptrs(views), *[None] * (5 - len(views))))
-
-
 def _concat_ranges(parts):
     """Query blocks' CSR results (torch, on one device) -> one CSR over all the blocks."""
     import torch
@@ -319,12 +314,8 @@ class ShardedGfkb:
             # this rank's slice of the batch: re-pack the CSR rows [lo, hi)
             lo, hi = shard_bounds(qfb.n, self.world, self.rank)
             self._qslice = (lo, hi)
-            ip = np.ascontiguousarray(qfb.indptr[lo:hi + 1])
-            _capi.check(_capi.load().kv_query_upload(self.index._h, ip.ctypes.data_as(C.POINTER(C.c_int64)),
-                                                     qfb.ids.ctypes.data_as(C.POINTER(C.c_uint32)),
-                                                     qfb.tf.ctypes.data_as(C.POINTER(C.c_uint32)),
-                                                     np.ascontiguousarray(qfb.oov[lo:hi]).ctypes.data_as(C.POINTER(C.c_double)),
-                                                     hi - lo))
+            self.index._upload(np.ascontiguousarray(qfb.indptr[lo:hi + 1]), qfb.ids, qfb.tf,
+                               np.ascontiguousarray(qfb.oov[lo:hi]), hi - lo)
             return
         self.index.upload_queries(qfb)
         self._exchange_thresholds(qfb.n)
@@ -578,9 +569,7 @@ class ShardedGfkb:
         self.set_resident(qfb)
 
     def _empty_range(self, device_out: bool):
-        if device_out:
-            return _devout.empty_range(self.device)
-        return np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32)
+        return self.index._empty_range(device_out)
 
     def range_resident(self, threshold: float, device_out: bool = False, labels: Optional[np.ndarray] = None):
         """Threshold search of the resident batch over the whole sharded corpus: ``(indptr int64[n_q+1], rows int64[P],
@@ -594,9 +583,7 @@ class ShardedGfkb:
             self.index.set_filter(np.ascontiguousarray(labels, dtype=np.int32)[lo:hi])
         if self.world == 1:
             return self.index._range_resident(q, threshold, device_out)
-        n = C.c_int64(0)
-        if hi > lo:
-            _capi.check(_capi.load().kv_range_resident(self.index._h, np.float32(threshold), C.byref(n)))
+        n = self.index._range_search(threshold) if hi > lo else 0
 
         def fill(views):
             ip = views[0]
@@ -604,13 +591,13 @@ class ShardedGfkb:
                 ip.zero_()
                 return
             # queries mode: this rank's run holds empty segments outside its slice [lo, hi)
-            _fetch_into(self.index._h, [ip[lo:hi + 1]] + views[1:])
+            self.index._range_fetch_into([ip[lo:hi + 1]] + views[1:])
             ip[:lo] = 0
-            ip[hi + 1:] = n.value
+            ip[hi + 1:] = n
             if self.row_map is not None:   # text-range shard: local -> global rows (ascending, so segments stay ordered)
                 views[1].copy_(self.row_map[views[1]])
 
-        gathered, pairs = gather_range_packed(self.device, q, n.value, fill, self.group)
+        gathered, pairs = gather_range_packed(self.device, q, n, fill, self.group)
         return _host(merge_range_on_device(self.device, gathered, q, pairs), device_out)
 
     def range_packed(self, data, offsets: np.ndarray, threshold: float, mode: int = 0, labels: Optional[np.ndarray] = None,
@@ -737,21 +724,14 @@ class ShardedDense:
         -> ``(indptr int64[Q+1], rows int64[P], scores float32[P])`` as ``DenseIndex.range_device`` returns them (torch
         tensors on the device, or NumPy arrays without ``device_out``); identical on every rank.  ``exclude_base >= 0``:
         query q never matches GLOBAL row ``exclude_base + q``."""
-        import torch
-
         idx = self.index
         queries = queries.contiguous()
         if self.world == 1:
             return idx.range_device(queries, threshold, exclude_base, device_out)
-        assert queries.is_cuda and queries.element_size() == 2 and queries.shape[-1] == self.dim
         n_q = queries.shape[0]
-        torch.cuda.current_stream(queries.device).synchronize()  # the library reads the queries on its own stream
-        lib, n = _capi.load(), C.c_int64(0)
         with idx._lock:
-            _capi.check(lib.kv_dense_range_device(idx._h, C.c_void_p(queries.data_ptr()), n_q, np.float32(threshold),
-                                                  exclude_base, C.byref(n)))
-            fill = lambda views: _capi.check(lib.kv_dense_range_fetch_device(idx._h, *_devout.ptrs(views)))
-            gathered, pairs = gather_range_packed(self.device, n_q, n.value, fill, self.group)
+            n = idx._range_search_device(queries, threshold, exclude_base)
+            gathered, pairs = gather_range_packed(self.device, n_q, n, idx._range_fetch_into, self.group)
         return _host(merge_range_on_device(self.device, gathered, n_q, pairs), device_out)
 
     def selfjoin_range(self, threshold: float, block: int = 262144, device_out: bool = True):
@@ -826,14 +806,11 @@ class ShardedJaccard:
         n_q = len(ip) - 1
         if n_q == 0:
             return idx._empty_range(device_out)
-        lib, n = _capi.load(), C.c_int64(0)
         idx._upload(ip, qids, np.ones(len(qids), dtype=np.uint32), oov, n_q)
         if exclude is not None:   # global rows; the shard maps them to its own rows
-            exclude = np.ascontiguousarray(exclude, dtype=np.int64)
-            _capi.check(lib.kv_query_set_exclusions(idx._h, exclude.ctypes.data_as(C.POINTER(C.c_int64)), n_q))
-        _capi.check(lib.kv_range_resident(idx._h, np.float32(threshold), C.byref(n)))
-        gathered, pairs = gather_range_packed(self.device, n_q, n.value, lambda views: _fetch_into(idx._h, views), self.group,
-                                              jaccard=True)
+            idx.set_exclusions(exclude)
+        gathered, pairs = gather_range_packed(self.device, n_q, idx._range_search(threshold),
+                                              idx._range_fetch_into, self.group, jaccard=True)
         return _host(merge_range_on_device(self.device, gathered, n_q, pairs, jaccard=True), device_out)
 
     def range_csr(self, indptr: np.ndarray, ids: np.ndarray, threshold: float, device_out: bool = False):

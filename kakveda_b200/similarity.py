@@ -273,28 +273,50 @@ class _KvIndex:
         _capi.check(_capi.load().kv_topk_resident_host(self._h, k, _ptr(scores, C.c_float), _ptr(rows, C.c_int64)))
         return scores, rows
 
+    def set_exclusions(self, rows: Optional[np.ndarray]) -> None:
+        """Query q of the resident batch must not match GLOBAL row ``rows[q]`` (-1 = none); ``None`` clears."""
+        if rows is None:
+            _capi.check(_capi.load().kv_query_set_exclusions(self._h, None, 0))
+            return
+        rows = np.ascontiguousarray(rows, dtype=np.int64)
+        _capi.check(_capi.load().kv_query_set_exclusions(self._h, _ptr(rows, C.c_int64), len(rows)))
+
+    def _range_search(self, threshold: float) -> int:
+        """Threshold search of the resident batch; returns the pair count.  The result stays in the handle until
+        ``_range_fetch_into`` (or the next upload, search, append, deletion or finalize)."""
+        n = C.c_int64(0)
+        _capi.check(_capi.load().kv_range_resident(self._h, np.float32(threshold), C.byref(n)))
+        return n.value
+
+    def _range_fetch_into(self, out, device_out: bool = True) -> None:
+        """Fetch the last search's result into ``out`` = ``(indptr, rows, scores[, inter, union])`` of the search's
+        query and pair counts: torch tensors or views on the index's device, or (not ``device_out``) NumPy arrays."""
+        lib = _capi.load()
+        if device_out:
+            _capi.check(lib.kv_range_fetch_device(self._h, *_devout.ptrs(out), *[None] * (5 - len(out))))
+            return
+        types = (C.c_int64, C.c_int64, C.c_float, C.c_int32, C.c_int32)
+        _capi.check(lib.kv_range_fetch(self._h, *[_ptr(a, t) for a, t in zip(out, types)], *[None] * (5 - len(out))))
+
+    def _range_arrays(self, n_q: int, n_pairs: int, device_out: bool):
+        """Uninitialised ``(indptr, rows, scores)``, and on a Jaccard index ``inter, union`` after them."""
+        if device_out:
+            return _devout.range_arrays(self.device, n_q, n_pairs, jaccard=self._jaccard)
+        out = (np.empty(n_q + 1, np.int64), np.empty(n_pairs, np.int64), np.empty(n_pairs, np.float32))
+        return out + (np.empty(n_pairs, np.int32), np.empty(n_pairs, np.int32)) if self._jaccard else out
+
     def _range_resident(self, n_q: int, threshold: float, device_out: bool = False):
         """Threshold search of the resident batch of ``n_q`` queries: ``(indptr, rows, scores)``, and on a Jaccard
         index ``inter, union`` after them, as NumPy arrays or (``device_out``) torch tensors on the index's device."""
-        lib = _capi.load()
-        n = C.c_int64(0)
-        _capi.check(lib.kv_range_resident(self._h, np.float32(threshold), C.byref(n)))
-        if device_out:
-            out = _devout.range_arrays(self.device, n_q, n.value, jaccard=self._jaccard)
-            _capi.check(lib.kv_range_fetch_device(self._h, *_devout.ptrs(out), *[None] * (5 - len(out))))
-            return out
-        out = (np.empty(n_q + 1, dtype=np.int64), np.empty(n.value, dtype=np.int64), np.empty(n.value, dtype=np.float32))
-        counts = (np.empty(n.value, dtype=np.int32), np.empty(n.value, dtype=np.int32)) if self._jaccard else ()
-        _capi.check(lib.kv_range_fetch(self._h, _ptr(out[0], C.c_int64), _ptr(out[1], C.c_int64), _ptr(out[2], C.c_float),
-                                       *([_ptr(c, C.c_int32) for c in counts] or [None, None])))
-        return out + counts
+        out = self._range_arrays(n_q, self._range_search(threshold), device_out)
+        self._range_fetch_into(out, device_out)
+        return out
 
     def _empty_range(self, device_out: bool = False):
         """The threshold search result of no queries."""
-        if device_out:
-            return _devout.empty_range(self.device, jaccard=self._jaccard)
-        out = (np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32))
-        return out + (np.zeros(0, np.int32), np.zeros(0, np.int32)) if self._jaccard else out
+        out = self._range_arrays(0, 0, device_out)
+        out[0][0] = 0
+        return out
 
     def last_timing_ms(self) -> Tuple[float, float, float, float]:
         """CUDA-event ms of the last upload and top-k: H2D of the batch, bound + scan kernels, merge, D2H."""
@@ -518,14 +540,6 @@ class GfkbIndex(_KvIndex):
         ms = (C.c_float * 4)()
         _capi.check(_capi.load().kv_index_last_prepare_ms(self._h, ms))
         return tuple(ms)
-
-    def set_exclusions(self, rows: Optional[np.ndarray]) -> None:
-        """Query q of the resident batch must not match GLOBAL row ``rows[q]`` (-1 = none); ``None`` clears."""
-        if rows is None:
-            _capi.check(_capi.load().kv_query_set_exclusions(self._h, None, 0))
-            return
-        rows = np.ascontiguousarray(rows, dtype=np.int64)
-        _capi.check(_capi.load().kv_query_set_exclusions(self._h, _ptr(rows, C.c_int64), len(rows)))
 
     def set_filter(self, labels: Optional[np.ndarray]) -> None:
         """Query q of the resident batch only matches rows labelled ``labels[q]`` (-1 = any row; ``set_row_labels``);
