@@ -206,7 +206,12 @@ int kv_topk_resident_host(kv_index *ix, int k, float *out_scores, int64_t *out_r
 /* kv_topk_resident in two phases, for a row-sharded GFKB (kakveda_b200/dist.py): _seed = bound pass + seed scan, the
  * outputs receive this shard's seed top-k (device, [n_q*k], by original query); kv_index_raise_thresholds takes, per
  * query, a lower bound of the GLOBAL k-th score (device float32[n_q]; the k-th of the merged seed lists of all shards)
- * and raises the pruning thresholds of the resident batch; _finish = candidate selection + scan + merge. */
+ * and raises the pruning thresholds of the resident batch; _finish = candidate selection + scan + merge.  The seed
+ * lists honour the batch's filter and distinct mode.  _seed writes the slots of regular queries only: null and
+ * irregular queries have no seed list, so a caller that merges the seed lists fills the outputs with (-inf, -1) first.
+ * For a distinct batch the k-th seed score must be taken over distinct groups -- one group can appear in several
+ * shards' seed lists: slot k-1 of kv_merge_topk_distinct_device_on over the gathered seed lists (global rows); the
+ * batch must be switched on with kv_query_set_distinct(ix, KV_DISTINCT_MERGED_SEEDS), else KV_ERR_INVALID. */
 int kv_topk_resident_seed(kv_index *ix, int k, void *d_scores, void *d_rows);
 int kv_index_raise_thresholds(kv_index *ix, const void *d_kth_scores, int64_t n_q);
 int kv_topk_resident_finish(kv_index *ix, int k, void *d_scores, void *d_rows);
@@ -227,8 +232,9 @@ int kv_selfjoin_upload(kv_index *ix, int64_t q_begin, int64_t q_end);
  * unfiltered, the zero-score fill and null queries take the label's rows in ascending order, (-inf, -1) past its last
  * row -- and its threshold search returns the unfiltered pairs of its label.  The index statistics do not change.
  * KV_ERR_INVALID: wrong length, a label below -1, or a Jaccard index (mode 1).  KV_ERR_STATE: a filtered batch on an
- * index whose labels are missing or stale (appended rows), here or at the search.  Not combinable with the threshold
- * exchange of a row-sharded GFKB (kv_index_thresholds_*: KV_ERR_INVALID). */
+ * index whose labels are missing or stale (appended rows), here or at the search.  A filtered batch may use
+ * kv_topk_resident_seed / _finish and the threshold exchange of a row-sharded GFKB (kv_index_thresholds_*) when every
+ * rank sets the same filter (see there). */
 int kv_index_set_row_labels(kv_index *ix, const int32_t *labels, int64_t n);
 int kv_query_set_filter(kv_index *ix, const int32_t *labels, int64_t n_q);
 
@@ -243,10 +249,16 @@ int kv_query_set_filter(kv_index *ix, const int32_t *labels, int64_t n_q);
  * returned, (-inf, -1) past the last eligible group.  Scores are the float32 values of the non-distinct top-k, so
  * singleton groups give its result bit for bit, and the zero-score fill and null queries take the first row of each
  * new group in ascending row order.  kv_range_* ignores distinct mode: a threshold search already returns every pair.
- * KV_ERR_INVALID: a Jaccard index (mode 1), here or at kv_index_set_row_groups; kv_topk_resident_seed / _finish or
- * the threshold exchange of a row-sharded GFKB (kv_index_thresholds_*) in distinct mode -- a shard's seed scores are
- * no lower bound of the global k-th group score, since one group can count on several shards.  KV_ERR_STATE: distinct
- * mode on an index whose groups are missing or stale (appended rows), here or at the search. */
+ * A row-sharded GFKB gives each shard the groups of its own rows (one group may span shards) and switches its batch on
+ * with on = KV_DISTINCT_MERGED_SEEDS: distinct mode, plus the caller's promise that it merges the shards' seed lists
+ * group-aware (kv_merge_topk_distinct_device_on) and raises the thresholds to slot k-1 of that merge.  Only then do
+ * kv_topk_resident_seed / _finish run a distinct batch; with on = 1 they refuse it (KV_ERR_INVALID), since the k-th of
+ * the shards' raw seed scores may count one group several times and is no lower bound of the global k-th group score.
+ * The threshold exchange (kv_index_thresholds_*) takes distinct batches in either form.  The final merge of the
+ * shards' lists is kv_merge_topk_distinct_device_on.
+ * KV_ERR_INVALID: a Jaccard index (mode 1), here or at kv_index_set_row_groups.  KV_ERR_STATE: distinct mode on an
+ * index whose groups are missing or stale (appended rows), here or at the search. */
+#define KV_DISTINCT_MERGED_SEEDS 2
 int kv_index_set_row_groups(kv_index *ix, const int32_t *groups, int64_t n);
 int kv_query_set_distinct(kv_index *ix, int on);
 
@@ -330,7 +342,11 @@ int kv_rescore_pairs(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_id
  * shards prune with the best bound known anywhere (n_peers = 0 unmaps).  Results are unchanged -- a pushed value
  * always is a valid lower bound (k rows at least that good exist in some shard) -- only less is scanned.  Callers must
  * keep scans of different batches apart with a collective (the all-gather of partial top-k does that) and exchange
- * again after uploading a batch larger than `capacity` (kv_topk_resident* returns KV_ERR_STATE otherwise). */
+ * again after uploading a batch larger than `capacity` (kv_topk_resident* returns KV_ERR_STATE otherwise).
+ * Contract: every rank holds the same resident batch WITH THE SAME FILTER AND DISTINCT MODE (kv_query_set_filter,
+ * kv_query_set_distinct).  Then a pushed value is the k-th score of a list of rows of the query's label -- of k distinct
+ * groups in distinct mode -- and bounds the query's global (filtered, distinct) k-th score.  For a distinct batch the
+ * seed k-th score given to kv_index_raise_thresholds is taken over distinct groups (kv_merge_topk_distinct_device_on). */
 int kv_index_thresholds_export(kv_index *ix, int64_t capacity, void *handle_out);
 int kv_index_thresholds_peers(kv_index *ix, const void *handles, int n_peers, int64_t capacity);
 /* Test hook: what kv_index_thresholds_peers does, for indexes of one process on one device (no CUDA IPC): ix pushes
@@ -349,6 +365,18 @@ int kv_merge_topk_device(int device, const void *d_scores_in, const void *d_rows
 int kv_merge_topk_device_on(int device, const void *d_scores_in, const void *d_rows_in, int n_lists,
                             int64_t n_q, int k, int64_t stride_s, int64_t stride_r, void *d_scores_out,
                             void *d_rows_out, void *stream, int sync);
+/* K5 of a distinct batch (kv_query_set_distinct) over lists of several indexes, e.g. the row shards' lists after the
+ * all-gather, laid out as for kv_merge_topk_device_on (1..2048 lists, k 1..32, global rows, -1 = unused).
+ * d_row_groups: device int32[n_group_rows], the group of every GLOBAL row (row_base 0), owned by the caller.  Output as
+ * the single index's distinct top-k: in (score desc, row asc) order the first entry of each group, (-inf, -1) past the
+ * last group; exact across shards, since a group of the merged top-k is in the top-k of the list holding its best row.
+ * Runs on `stream` and returns once the outputs and their validity are known.  KV_ERR_INVALID for bad counts or
+ * strides, pointers that are not device memory of `device` aligned to their element size, and -- after the fact, the
+ * outputs then undefined -- a row outside [0, n_group_rows), whose group is never read. */
+int kv_merge_topk_distinct_device_on(int device, const void *d_scores_in, const void *d_rows_in, int n_lists,
+                                     int64_t n_q, int k, int64_t stride_s, int64_t stride_r,
+                                     const void *d_row_groups, int64_t n_group_rows, void *d_scores_out,
+                                     void *d_rows_out, void *stream);
 
 /* Merge of n_runs (1..64) threshold-search results over disjoint rows -- e.g. the row shards' results after ONE
  * all-gather -- into the single result over all the rows.  Run w is a CSR as kv_range_fetch_device writes it:

@@ -12,6 +12,7 @@ from pathlib import Path
 
 KV_OK, KV_ERR_INVALID, KV_ERR_CUDA, KV_ERR_EMPTY_VOCAB, KV_ERR_NOMEM, KV_ERR_NONASCII, KV_ERR_STATE = range(7)
 KV_TEXT_RAW_ASCII, KV_TEXT_TOKENS, KV_TEXT_MIXED = 0, 1, 2
+KV_DISTINCT_MERGED_SEEDS = 2   # kv_query_set_distinct: distinct, the caller merges the shards' seed lists group-aware
 
 _LIB_PATH = Path(__file__).resolve().parent / "lib" / "libkakveda_b200.so"
 _lib = None
@@ -94,6 +95,8 @@ SIGNATURES = {
                                        C.c_void_p]),
     "kv_merge_topk_device_on": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int64,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "kv_merge_topk_distinct_device_on": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64,
+                                                   C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kv_merge_range_device_on": (C.c_int, [C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_int64, c_i64p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -199,9 +199,10 @@ struct kv_index {
   std::vector<int> h_filt_orig;
   bool has_filter = false;
   // row groups (kv_index_set_row_groups): by row for K5, the fallbacks and null queries, by scan position for the
-  // scan.  Distinct mode of the resident batch (kv_query_set_distinct), cleared by the next upload.
+  // scan.  Distinct mode of the resident batch (kv_query_set_distinct), cleared by the next upload; merged_seeds: the
+  // caller merges the shards' seed lists group-aware (KV_DISTINCT_MERGED_SEEDS), so the two-phase top-k may run.
   RowSet groups;
-  bool distinct = false;
+  bool distinct = false, merged_seeds = false;
   // deleted rows (kv_index_delete_rows).  They keep their place in the scan layout.  On the device while any row is
   // deleted, rebuilt by every finalize: by row, the live word of every chunk (by scan position) and the first LAB_FIRST
   // live rows (null queries)
@@ -1022,7 +1023,7 @@ static int build_query_tables(kv_index *ix, int64_t n_q);
 static void start_batch(kv_index *ix) {
   ix->batch_valid = false;
   drop_range(ix);
-  ix->has_excl = ix->has_filter = ix->distinct = false;
+  ix->has_excl = ix->has_filter = ix->distinct = ix->merged_seeds = false;
   ix->irr.clear();
 }
 
@@ -1455,8 +1456,8 @@ struct Batch {
 static int launch_merge(kv_index *ix, const Batch &b, int64_t n_lists) {
   if (b.distinct)
     merge_topk_distinct_kernel<<<(unsigned)((b.n_q * 32 + 255) / 256), 256, 0, ix->stream>>>(
-        ix->d_part_s.p, ix->d_part_r.p, (int)n_lists, b.n_q, b.k, b.n_q * b.k, ix->d_qperm.p, ix->groups.d_row.p, ix->row_base,
-        b.out_s, b.out_r);
+        ix->d_part_s.p, ix->d_part_r.p, (int)n_lists, b.n_q, b.k, b.n_q * b.k, b.n_q * b.k, ix->d_qperm.p, ix->groups.d_row.p,
+        ix->row_base, ix->n_rows, nullptr, b.out_s, b.out_r);
   else
     merge_topk_kernel<<<(unsigned)((b.n_q * 32 + 255) / 256), 256, 0, ix->stream>>>(
         ix->d_part_s.p, ix->d_part_r.p, (int)n_lists, b.n_q, b.k, b.n_q * b.k, b.n_q * b.k, ix->d_qperm.p, b.out_s, b.out_r);
@@ -1669,15 +1670,17 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
   if (k < 1 || k > 32) return kv_fail(KV_ERR_INVALID, "kv_topk_resident: k must be 1..32");
   int rc = check_filter(ix, "kv_topk_resident");
   if (rc != KV_OK) return rc;
-  // the thresholds peers push are those of unfiltered queries: not a bound of a filtered query's k-th score
-  if (ix->has_filter && (ix->gthr_exported || ix->n_peers))
-    return kv_fail(KV_ERR_INVALID, "kv_topk_resident: a label filter cannot be combined with the threshold exchange of a row-sharded GFKB");
+  // Filtered and distinct batches may use the threshold exchange of a row-sharded GFKB: every rank holds the same batch
+  // with the same filter and mode (kv_index_thresholds_peers), so a pushed threshold -- the k-th score of a list of the
+  // query's label, of k distinct groups in distinct mode -- bounds the query's global k-th score.
   if (ix->distinct) {
     if (!ix->groups.ready(ix->n_rows))
       return kv_fail(KV_ERR_STATE, "kv_topk_resident: the batch is distinct but the row groups are missing or stale (set them again after an append)");
-    // a shard's seed k-th score is no lower bound of the global k-th GROUP score: one group can count on several shards
-    if (phase != 0 || ix->gthr_exported || ix->n_peers)
-      return kv_fail(KV_ERR_INVALID, "kv_topk_resident: distinct mode cannot be combined with the two-phase top-k or the threshold exchange of a row-sharded GFKB");
+    // The raised seed threshold only bounds the global k-th GROUP score when the shards' seed lists were merged
+    // group-aware: one group can count on several shards.  The caller declares it with KV_DISTINCT_MERGED_SEEDS.
+    if (phase != 0 && !ix->merged_seeds)
+      return kv_fail(KV_ERR_INVALID, "kv_topk_resident: the two-phase top-k of a distinct batch needs kv_query_set_distinct(ix, KV_DISTINCT_MERGED_SEEDS) "
+                                     "(the seed k-th score is then taken over distinct groups)");
   }
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
@@ -2154,11 +2157,12 @@ int kv_query_set_distinct(kv_index *ix, int on) {
   std::lock_guard<std::mutex> g(ix->mu);
   if (on && ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_query_set_distinct: a Jaccard index (mode 1) has no distinct top-k");
   if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "kv_query_set_distinct: no query batch uploaded");
-  ix->distinct = false;
+  ix->distinct = ix->merged_seeds = false;
   if (!on) return KV_OK;
   if (!ix->groups.ready(ix->n_rows))
     return kv_fail(KV_ERR_STATE, "kv_query_set_distinct: the index has no row groups for its current rows (kv_index_set_row_groups)");
   ix->distinct = true;
+  ix->merged_seeds = on == KV_DISTINCT_MERGED_SEEDS;
   return KV_OK;
 }
 
@@ -2332,6 +2336,50 @@ int kv_merge_topk_device_on(int device, const void *d_scores_in, const void *d_r
                                                                        (float *)d_scores_out, (long long *)d_rows_out);
   KV_CUDA(cudaGetLastError());
   if (sync) KV_CUDA(cudaStreamSynchronize(s));
+  return KV_OK;
+}
+
+// K5 of a distinct batch over lists of several indexes (e.g. the row shards' lists after the all-gather): the kernel
+// launch_merge runs for one index, with the groups of every global row.  Waits for the merge: whether a row had no
+// group is only known then.  The 4-byte flag it is reported in is one per device, allocated by the first call and kept
+// for the process, so that a call allocates nothing; calls on one device take turns on it.
+int kv_merge_topk_distinct_device_on(int device, const void *d_scores_in, const void *d_rows_in, int n_lists, int64_t n_q,
+                                     int k, int64_t stride_s, int64_t stride_r, const void *d_row_groups,
+                                     int64_t n_group_rows, void *d_scores_out, void *d_rows_out, void *stream) {
+  const char *fn = "kv_merge_topk_distinct_device";
+  if (n_lists < 1 || n_lists > 2048 || n_q < 0 || k < 1 || k > 32 || n_group_rows < 0 || stride_s < n_q * k ||
+      stride_r < n_q * k)
+    return kv_fail(KV_ERR_INVALID, "%s: bad arguments (1 to 2048 lists, k 1..32, strides of at least n_q * k)", fn);
+  if (n_q == 0) return KV_OK;
+  int sm_count = 0;
+  int rc = open_device(device, fn, &sm_count);
+  if (rc != KV_OK) return rc;
+  const struct { const void *p; size_t al; const char *what; } ptrs[] = {
+      {d_scores_in, 4, "scores_in"}, {d_rows_in, 8, "rows_in"}, {d_scores_out, 4, "scores_out"}, {d_rows_out, 8, "rows_out"},
+      {d_row_groups, 4, "row_groups"}};
+  for (int j = 0; j < (n_group_rows > 0 ? 5 : 4); j++)
+    if ((rc = check_device_ptr(ptrs[j].p, device, ptrs[j].al, ptrs[j].what, fn)) != KV_OK) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  static std::mutex mu;
+  static unsigned *flags[256] = {};
+  if (device >= 256) return kv_fail(KV_ERR_INVALID, "%s: device %d", fn, device);
+  std::lock_guard<std::mutex> g(mu);
+  unsigned *&d_bad = flags[device];
+  if (!d_bad) KV_CUDA(cudaMalloc((void **)&d_bad, sizeof(unsigned)));
+  unsigned bad = 0;
+  cudaError_t e = cudaMemsetAsync(d_bad, 0, sizeof(unsigned), s);
+  if (e == cudaSuccess) {
+    merge_topk_distinct_kernel<<<(unsigned)((n_q * 32 + 255) / 256), 256, 0, s>>>(
+        (const float *)d_scores_in, (const long long *)d_rows_in, n_lists, n_q, k, stride_s, stride_r, nullptr,
+        (const int *)d_row_groups, 0, n_group_rows, d_bad, (float *)d_scores_out, (long long *)d_rows_out);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&bad, d_bad, sizeof(bad), cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) return kv_fail(KV_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e));
+  if (bad)
+    return kv_fail(KV_ERR_INVALID, "%s: a row outside the %lld rows of the group table (the outputs are undefined)", fn,
+                   (long long)n_group_rows);
   return KV_OK;
 }
 

@@ -1572,11 +1572,14 @@ __global__ void merge_topk_kernel(const float *__restrict__ in_s, const long lon
 
 // K5 of a distinct batch (kv_query_set_distinct).  Each partial list holds distinct groups; in the merged (score desc,
 // row asc) order a group's first entry is its best row, and every later entry of a taken group is skipped.  Exact: a
-// group of the global top-k is also in the top-k of the partial list that holds its best row.  groups: by local row
-// (global row - row_base).  One warp per query, as merge_topk_kernel; 256 threads per block.
+// group of the global top-k is also in the top-k of the partial list that holds its best row -- inside one index and
+// across the row shards of a sharded GFKB alike.  groups: by local row (global row - row_base), n_group_rows of them;
+// a row outside them is never looked up: it ends its list and sets *bad (when given).  stride_s / stride_r as in
+// merge_topk_kernel.  One warp per query, as merge_topk_kernel; 256 threads per block.
 __global__ void merge_topk_distinct_kernel(const float *__restrict__ in_s, const long long *__restrict__ in_r, int n_lists,
-                                           int64_t n_q, int k, int64_t stride, const int *__restrict__ out_index,
-                                           const int *__restrict__ groups, int64_t row_base, float *out_s, long long *out_r) {
+                                           int64_t n_q, int k, int64_t stride_s, int64_t stride_r,
+                                           const int *__restrict__ out_index, const int *__restrict__ groups, int64_t row_base,
+                                           int64_t n_group_rows, unsigned *bad, float *out_s, long long *out_r) {
   __shared__ int s_taken[8][32];  // per warp: the groups taken so far
   const int64_t q = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -1599,13 +1602,19 @@ __global__ void merge_topk_distinct_kernel(const float *__restrict__ in_s, const
       long long r = -1;
       int g = -1;
       for (; h < k; h++) {  // skip the entries of taken groups
-        const size_t o = (size_t)l * stride + (size_t)q * k + h;
-        r = in_r[o];
+        const size_t o = (size_t)q * k + h;
+        r = in_r[(size_t)l * stride_r + o];
         if (r < 0) break;
-        g = groups[r - row_base];
+        const long long gr = r - row_base;
+        if (gr < 0 || gr >= n_group_rows) {  // a row without a group: the list ends here, the caller reports it
+          if (bad) *bad = 1u;
+          r = -1;
+          break;
+        }
+        g = groups[gr];
         bool seen = false;
         for (int t = 0; t < j; t++) seen |= taken[t] == g;
-        if (!seen) { s = in_s[o]; break; }
+        if (!seen) { s = in_s[(size_t)l * stride_s + o]; break; }
         r = -1;
       }
       head[i] = (unsigned char)h;

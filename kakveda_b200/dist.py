@@ -8,7 +8,10 @@ only exchanges are
   TF-IDF's idf and row norms use GLOBAL df and N (``allreduce_df``);
 * once per query batch: ONE all-gather of the per-shard partial top-k (scores float32, rows int64),
   followed by a local merge ordered by (score desc, row asc) -- identical on every rank
-  (``gather_topk`` + ``kv_merge_topk_device``);
+  (``gather_topk`` + ``kv_merge_topk_device``); a distinct batch merges with ``kv_merge_topk_distinct_device_on``,
+  which keeps the first entry of each row group, and its seed exchange carries whole seed lists (scores and rows);
+* once per deletion: an all-reduce of the live document frequencies and row count, then a statistics-only finalize
+  of every shard (``ShardedGfkb.delete_rows``);
 * once per threshold search: a 16-byte all-gather of the shards' pair counts, ONE all-gather of the per-shard CSR
   results packed in equal slots, and the W-way merge of the ordered runs on the device (``gather_range_packed`` +
   ``merge_range_on_device``, ``kv_merge_range_device_on``).  The threshold is fixed, so every shard searches alone.
@@ -127,6 +130,26 @@ def merge_packed_on_device(device: int, gathered, q: int, k: int):
     return out_s, out_r
 
 
+def merge_packed_distinct_on_device(device: int, gathered, q: int, k: int, groups):
+    """The K5 of a distinct batch (``kv_merge_topk_distinct_device_on``) directly on the packed all-gather buffer ([W,
+    total] uint8): per query, in (score desc, row asc) order, the first entry of each group.  ``groups``: int32 device
+    tensor, the group of every global row.  Runs on torch's current stream and waits for it: a row without a group
+    raises ValueError."""
+    import torch
+
+    w = gathered.shape[0]
+    off_r, total = packed_layout(q, k)
+    out_s = torch.empty((q, k), dtype=torch.float32, device=gathered.device)
+    out_r = torch.empty((q, k), dtype=torch.int64, device=gathered.device)
+    stream = torch.cuda.current_stream(gathered.device).cuda_stream
+    _capi.check(_capi.load().kv_merge_topk_distinct_device_on(device, C.c_void_p(gathered.data_ptr()),
+                                                              C.c_void_p(gathered.data_ptr() + off_r), w, q, k, total // 4,
+                                                              total // 8, C.c_void_p(groups.data_ptr()), groups.numel(),
+                                                              C.c_void_p(out_s.data_ptr()), C.c_void_p(out_r.data_ptr()),
+                                                              C.c_void_p(stream)))
+    return out_s, out_r
+
+
 # ---- threshold search: variable-sized results ------------------------------------------------------------------------
 
 def range_layout(n_q: int, p_max: int, jaccard: bool = False) -> Tuple[Tuple[int, int, int, int, int], int]:
@@ -217,6 +240,21 @@ def _concat_ranges(parts):
     return (torch.cat(ips),) + tuple(torch.cat([p[j] for p in parts]) for j in range(1, len(parts[0])))
 
 
+def _drop_queries(res, drop: np.ndarray):
+    """A CSR result (torch, on one device) with no pairs for the queries where ``drop`` (bool per query) is set."""
+    import torch
+
+    if not drop.any():
+        return res
+    ip = res[0]
+    d = torch.from_numpy(drop).to(ip.device)
+    cnt = ip[1:] - ip[:-1]
+    keep = torch.repeat_interleave(~d, cnt)
+    out_ip = torch.zeros_like(ip)
+    out_ip[1:] = torch.cumsum(torch.where(d, 0, cnt), 0)
+    return (out_ip,) + tuple(t[keep] for t in res[1:])
+
+
 def _host(out, device_out: bool):
     return out if device_out else tuple(t.cpu().numpy() for t in out)
 
@@ -249,6 +287,9 @@ class ShardedGfkb:
         self.index: Optional[GfkbIndex] = None
         self.n_global = 0
         self._corpus = None   # (data, offsets, mode) of the corpus text: the queries of selfjoin_range
+        self._has_labels = self._has_groups = False   # set_row_labels / set_row_groups
+        self._groups_dev = None   # rows mode on several GPUs: the group of every global row, for the distinct merges
+        self._deleted = None      # delete_rows: bool per global row (every rank deletes the same rows)
 
     def build_packed(self, data, offsets: np.ndarray, mode: int = 0, n_threads: int = 0) -> None:
         import torch
@@ -320,13 +361,41 @@ class ShardedGfkb:
         self.index.upload_queries(qfb)
         self._exchange_thresholds(qfb.n)
 
-    def topk_resident(self, k: int, distinct: bool = False):
-        """Device-only step on the uploaded batch: local scan+merge, all-gather, global merge."""
-        no_distinct(distinct, "ShardedGfkb.topk_resident")
+    def _set_modes(self, q: int, labels: Optional[np.ndarray], distinct: bool) -> None:
+        """The filter and distinct mode of the resident batch of ``q`` queries, the same on every rank (the threshold
+        exchange relies on it).  The arguments are checked before anything is sent, so every rank raises the same error."""
+        if labels is not None:
+            labels = np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
+            if len(labels) != q:
+                raise ValueError(f"labels: {len(labels)} labels for a batch of {q} queries")
+            if q and labels.min() < -1:
+                raise ValueError("labels: a label below -1")
+            if not self._has_labels:
+                raise ValueError("labels: the sharded index has no row labels (set_row_labels)")
+        if distinct and not self._has_groups:
+            raise ValueError("distinct: the sharded index has no row groups (set_row_groups)")
+        lo, hi = self._qslice if self.mode == "queries" and self.world > 1 else (0, q)
+        if hi > lo:
+            self.index.set_filter(None if labels is None else labels[lo:hi])
+            # rows mode on several GPUs runs the two-phase top-k, whose seed lists topk_resident merges group-aware
+            self.index.set_distinct(distinct, merged_seeds=self.mode == "rows" and self.world > 1)
+
+    def _to_global(self, r) -> None:
+        """Text-range shard: local rows -> global row ids, in place (-1 stays -1)."""
+        import torch
+
+        if self.row_map is not None:
+            r.copy_(torch.where(r >= 0, self.row_map[r.clamp(min=0)], r))
+
+    def topk_resident(self, k: int, labels: Optional[np.ndarray] = None, distinct: bool = False):
+        """Device-only step on the uploaded batch: local scan+merge, all-gather, global merge.  ``labels``: per query
+        the row label its results must carry (-1: any row; ``set_row_labels``).  ``distinct``: at most one row per group
+        (``set_row_groups``), as ``GfkbIndex.topk_features``.  Both combine."""
         import torch
 
         q = self._resident_q
         dev = f"cuda:{self.device}"
+        self._set_modes(q, labels, distinct)
         if self.mode == "queries" and self.world > 1:
             import torch.distributed as dist
 
@@ -348,33 +417,49 @@ class ShardedGfkb:
         s, r = packed_views(buf, q, k)
         if self.world == 1:
             self.index.topk_resident(k, s.data_ptr(), r.data_ptr())
-            if self.row_map is not None:
-                r.copy_(torch.where(r >= 0, self.row_map[r.clamp(min=0)], r))
+            self._to_global(r)
             return s, r
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
         # phase 1: bounds + seed scan on every shard; the shards' seed lists are merged (small all-gather) and the GLOBAL
         # k-th seed score of every query becomes every shard's pruning threshold -- each shard then scans only what a
         # single index would scan of its rows
-        self.index.topk_resident_seed(k, s.data_ptr(), r.data_ptr())
-        ev[0].record()
-        # only the seed SCORES travel (6.4 MB per rank at 100k queries): the global k-th seed score of a query is the k-th
-        # largest of the W x k gathered scores (the shards hold disjoint rows)
         import torch.distributed as dist
 
-        gs = torch.empty((self.world, q, k), dtype=torch.float32, device=dev)
-        dist.all_gather_into_tensor(gs.view(-1), s.contiguous().view(-1), group=self.group)
-        kth = torch.topk(gs.permute(1, 0, 2).reshape(q, self.world * k), k, dim=1).values[:, k - 1].contiguous()
+        if distinct:
+            # One group can sit in several shards' seed lists, so the k-th of the W x k scores may count it twice: the
+            # whole seed lists travel (12 bytes an entry, rows mapped to global ids first) and the k-th seed score is
+            # slot k-1 of their distinct merge -- k distinct groups that good exist, a lower bound of the k-th group score.
+            seed = torch.empty(packed_layout(q, k)[1], dtype=torch.uint8, device=dev)
+            ss, sr = packed_views(seed, q, k)
+            ss.fill_(float("-inf"))   # null and irregular queries get no seed list
+            sr.fill_(-1)
+            torch.cuda.current_stream().synchronize()   # the seed scan writes on the index's own stream
+            self.index.topk_resident_seed(k, ss.data_ptr(), sr.data_ptr())
+            ev[0].record()
+            self._to_global(sr)
+            kth = merge_packed_distinct_on_device(self.device, gather_packed(seed, self.group), q, k,
+                                                  self._groups_dev)[0][:, k - 1].contiguous()
+        else:
+            self.index.topk_resident_seed(k, s.data_ptr(), r.data_ptr())
+            ev[0].record()
+            # only the seed SCORES travel (6.4 MB per rank at 100k queries): the global k-th seed score of a query is the
+            # k-th largest of the W x k gathered scores (the shards hold disjoint rows)
+            gs = torch.empty((self.world, q, k), dtype=torch.float32, device=dev)
+            dist.all_gather_into_tensor(gs.view(-1), s.contiguous().view(-1), group=self.group)
+            kth = torch.topk(gs.permute(1, 0, 2).reshape(q, self.world * k), k, dim=1).values[:, k - 1].contiguous()
         ev[1].record()
         torch.cuda.current_stream().synchronize()
         self.index.raise_thresholds(kth.data_ptr(), q)
         # phase 2: candidate selection + scan, then the exchange of the partial top-k
         self.index.topk_resident_finish(k, s.data_ptr(), r.data_ptr())
-        if self.row_map is not None:  # text-range shard: local row -> global row id (-1 stays -1)
-            r.copy_(torch.where(r >= 0, self.row_map[r.clamp(min=0)], r))
+        self._to_global(r)
         ev[2].record()
         gathered = gather_packed(buf, self.group)          # the all-gather of the partial top-k
         ev[3].record()
-        out = merge_packed_on_device(self.device, gathered, q, k)
+        if distinct:
+            out = merge_packed_distinct_on_device(self.device, gathered, q, k, self._groups_dev)
+        else:
+            out = merge_packed_on_device(self.device, gathered, q, k)
         ev[4].record()
         # The collective doubles as the barrier between batches for the cross-GPU threshold pushes: no rank may start
         # the next batch's scan (which resets and pushes thresholds) before every rank has finished this one's.
@@ -485,10 +570,11 @@ class ShardedGfkb:
         torch.cuda.current_stream().synchronize()
         return hs.numpy(), hr.numpy()
 
-    def topk_packed(self, data, offsets: np.ndarray, k: int, mode: int = 0, distinct: bool = False):
+    def topk_packed(self, data, offsets: np.ndarray, k: int, mode: int = 0, labels: Optional[np.ndarray] = None,
+                    distinct: bool = False):
         """End-to-end step from host text: featurise, upload, scan, exchange, merge, read back.  ``last_e2e_ms`` keeps
-        the wall-clock split of the last call (featurise / upload incl. table kernels / device step / read-back)."""
-        no_distinct(distinct, "ShardedGfkb.topk_packed")
+        the wall-clock split of the last call (featurise / upload incl. table kernels / device step / read-back).
+        ``labels`` / ``distinct`` as for ``topk_resident``."""
         import time
 
         t0 = time.perf_counter()
@@ -497,7 +583,7 @@ class ShardedGfkb:
 
             self.upload_text_sharded(data, offsets, mode)
             t2 = time.perf_counter()
-            s, r = self.topk_resident(k)
+            s, r = self.topk_resident(k, labels, distinct)
             torch.cuda.current_stream().synchronize()
             t3 = time.perf_counter()
             out = self._read_back(s, r)
@@ -512,7 +598,7 @@ class ShardedGfkb:
             self.index.upload_text(data, offsets, mode)   # featurise, classify and order on the device
             self._resident_q = n_q
             t2 = time.perf_counter()
-            s, r = self.topk_resident(k)
+            s, r = self.topk_resident(k, labels, distinct)
             torch.cuda.current_stream().synchronize()
             t3 = time.perf_counter()
             out = self._read_back(s, r)
@@ -526,7 +612,7 @@ class ShardedGfkb:
             t1 = time.perf_counter()
             self.set_resident(qfb)
             t2 = time.perf_counter()
-            s, r = self.topk_resident(k)
+            s, r = self.topk_resident(k, labels, distinct)
             import torch
 
             torch.cuda.current_stream().synchronize()
@@ -541,21 +627,95 @@ class ShardedGfkb:
             qfb.close()
 
     # ---- threshold search ------------------------------------------------------------------------------------------
+    def _local_part(self, per_row: np.ndarray) -> np.ndarray:
+        """The entries of this shard's rows of a per-global-row array: by index range, through ``row_map`` for a
+        text-order shard, all of them in queries mode."""
+        if self.row_map is not None:
+            return per_row[self._row_map_host]
+        if self.mode == "rows":
+            lo, hi = shard_bounds(self.n_global, self.world, self.rank)
+            return per_row[lo:hi]
+        return per_row
+
+    def _local_rows(self, rows: np.ndarray) -> np.ndarray:
+        """Ascending global rows -> the local rows of this shard that hold them (the others are dropped)."""
+        if self.row_map is not None:
+            m = self._row_map_host
+            pos = np.minimum(np.searchsorted(m, rows), max(len(m) - 1, 0))
+            return pos[m[pos] == rows] if len(m) else rows[:0]
+        if self.mode == "rows":
+            lo, hi = shard_bounds(self.n_global, self.world, self.rank)
+            return rows[(rows >= lo) & (rows < hi)] - lo
+        return rows
+
     def set_row_labels(self, global_labels: Optional[np.ndarray]) -> None:
         """One label >= 0 per GLOBAL row (e.g. a failure-type id): this shard keeps its rows' labels (by index range, or
-        through ``row_map`` for a text-order shard), for ``labels=`` of the threshold searches.  ``None`` clears."""
+        through ``row_map`` for a text-order shard), for ``labels=`` of the top-k and threshold searches.  ``None``
+        clears."""
         if global_labels is None:
             self.index.set_row_labels(None)
+            self._has_labels = False
             return
         lab = np.ascontiguousarray(global_labels, dtype=np.int32)
         if len(lab) != self.n_global:
             raise ValueError(f"set_row_labels: {len(lab)} labels for a corpus of {self.n_global} rows")
-        if self.row_map is not None:
-            lab = lab[self._row_map_host]
-        elif self.mode == "rows":
-            lo, hi = shard_bounds(self.n_global, self.world, self.rank)
-            lab = lab[lo:hi]
-        self.index.set_row_labels(lab)
+        self.index.set_row_labels(self._local_part(lab))
+        self._has_labels = True
+
+    def set_row_groups(self, global_groups: Optional[np.ndarray]) -> None:
+        """One group >= 0 per GLOBAL row (e.g. one id per distinct text), for ``distinct=True`` of the top-k: this shard
+        keeps its rows' groups as ``set_row_labels`` keeps labels.  In rows mode on several GPUs the rank also keeps the
+        whole table on its device (int32 per global row, 40 MB at 10M rows) for the distinct merges of the seed lists
+        and of the partial top-k.  ``None`` clears."""
+        import torch
+
+        if global_groups is None:
+            self.index.set_row_groups(None)
+            self._has_groups, self._groups_dev = False, None
+            return
+        grp = np.ascontiguousarray(global_groups, dtype=np.int32).reshape(-1)
+        if len(grp) != self.n_global:
+            raise ValueError(f"set_row_groups: {len(grp)} groups for a corpus of {self.n_global} rows")
+        if len(grp) and grp.min() < 0:
+            raise ValueError("set_row_groups: a negative group")
+        self.index.set_row_groups(self._local_part(grp))
+        self._has_groups = True
+        self._groups_dev = torch.from_numpy(grp).to(f"cuda:{self.device}") if self.mode == "rows" and self.world > 1 else None
+
+    # ---- row deletion ------------------------------------------------------------------------------------------------
+    def delete_rows(self, global_rows) -> None:
+        """Delete GLOBAL rows (any order, duplicates and rows deleted before allowed).  A collective: every rank calls it
+        with the same rows.  Each shard deletes the rows it holds; in rows mode on several GPUs the live document
+        frequencies and the live row count are then all-reduced, and every shard refreshes its statistics with a
+        statistics-only finalize, so that every search afterwards equals a single index with the same deletions.  Rows
+        outside the corpus raise ValueError on every rank before anything is deleted.  The resident batch is dropped."""
+        import torch
+
+        rows = np.unique(np.ascontiguousarray(global_rows, dtype=np.int64).reshape(-1))
+        if len(rows) and (rows[0] < 0 or rows[-1] >= self.n_global):
+            bad = rows[0] if rows[0] < 0 else rows[-1]
+            raise ValueError(f"delete_rows: row {bad} outside the corpus of {self.n_global} rows")
+        local = self._local_rows(rows)
+        if len(local):
+            self.index.delete_rows(local)
+        if self.world > 1 and self.mode == "rows":
+            cnt = torch.from_numpy(np.append(self.index.local_df().astype(np.int64), self.index.n_live_rows)).to(f"cuda:{self.device}")
+            allreduce_df(cnt, self.group)
+            cnt = cnt.cpu().numpy()
+            self.index.set_global_df(cnt[:-1].astype(np.uint32), int(cnt[-1]))
+        self.index.finalize()
+        if self._deleted is None:
+            self._deleted = np.zeros(self.n_global, dtype=bool)
+        self._deleted[rows] = True
+
+    def deleted_mask(self) -> np.ndarray:
+        """bool [n_global]: which global rows are deleted (the same on every rank)."""
+        return np.zeros(self.n_global, dtype=bool) if self._deleted is None else self._deleted.copy()
+
+    @property
+    def n_live_rows(self) -> int:
+        """The global row count minus the deleted rows."""
+        return self.n_global - (0 if self._deleted is None else int(self._deleted.sum()))
 
     def _set_resident_range(self, qfb: FeatureBatch) -> None:
         """``set_resident`` that also takes a batch whose queries-mode slice on this rank is empty."""
@@ -645,7 +805,10 @@ class ShardedGfkb:
                     pos = np.minimum(np.searchsorted(self._row_map_host, excl), max(len(self._row_map_host) - 1, 0))
                     excl = np.where(self._row_map_host[pos] == excl, pos, -1) if len(self._row_map_host) else np.full_like(excl, -1)
                 self.index.set_exclusions(excl)
-            parts.append(self.range_resident(threshold, device_out=True))
+            part = self.range_resident(threshold, device_out=True)
+            if self._deleted is not None:   # a deleted row's query has no pairs, as in GfkbIndex.selfjoin_range
+                part = _drop_queries(part, self._deleted[b0:b1])
+            parts.append(part)
         if not parts:
             return self._empty_range(device_out)
         return _host(_concat_ranges(parts), device_out)

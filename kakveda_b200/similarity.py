@@ -551,11 +551,13 @@ class GfkbIndex(_KvIndex):
         labels = np.ascontiguousarray(labels, dtype=np.int32)
         _capi.check(_capi.load().kv_query_set_filter(self._h, _ptr(labels, C.c_int32), len(labels)))
 
-    def set_distinct(self, on: bool) -> None:
+    def set_distinct(self, on: bool, merged_seeds: bool = False) -> None:
         """Distinct top-k for the resident batch (until the next upload): of the rows a query may match, the best row
         of each group (``set_row_groups``) in (score desc, row asc) order, the groups ranked by it, and the first k
-        of them.  Scores are the non-distinct ones; threshold searches ignore the mode."""
-        _capi.check(_capi.load().kv_query_set_distinct(self._h, 1 if on else 0))
+        of them.  Scores are the non-distinct ones; threshold searches ignore the mode.  ``merged_seeds``: this index
+        is a row shard whose caller merges the shards' seed lists group-aware before ``raise_thresholds``
+        (``KV_DISTINCT_MERGED_SEEDS``); only then may ``topk_resident_seed`` / ``_finish`` run the batch."""
+        _capi.check(_capi.load().kv_query_set_distinct(self._h, (_capi.KV_DISTINCT_MERGED_SEEDS if merged_seeds else 1) if on else 0))
 
     def _selfjoin_upload(self, lo: int, hi: int, same_label: bool = False) -> None:
         super()._selfjoin_upload(lo, hi)
