@@ -333,6 +333,21 @@ int kv_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_sc
 int kv_rescore_pairs(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
                      const double *q_oov_tf2, int64_t n_q, int k, const int64_t *rows, double *out_scores);
 
+/* Exact top-k of this index alone, with no candidate stage: per query K1a scores every row in float64 on the device,
+ * the block-wide selection of the irregular-query fallback takes the best k rows in (float64 score desc, row asc)
+ * order -- labels[q] >= 0: rows of that label only (kv_index_set_row_labels; labels NULL or -1: any row); distinct:
+ * the first row of each group (kv_index_set_row_groups); deleted rows never --, and K6 re-scores those rows.
+ * out_rows[n_q*k] (host) receives GLOBAL rows in that order, -1 past the last eligible row, and out_scores[n_q*k] their
+ * K6 float64 scores (-inf for unused slots).  Only the k rows of a query leave the device, not its score vector.  K6 and
+ * not K1a gives the reported scores because K1a's bits depend on the index by about 2^-50 (its fixed-point scales and
+ * folded features are per index) while K6's depend only on the row's text: identical texts on different shards or
+ * segments then tie exactly, and a merge of several indexes' lists by (score desc, row asc) reproduces
+ * services/gfkb/app.py:89's stable sort.  k 1..32; a filtered query without row labels, or distinct without row groups:
+ * KV_ERR_STATE.  The resident batch is left as it was. */
+int kv_exact_topk(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
+                  const double *q_oov_tf2, const int32_t *labels, int distinct, int64_t n_q, int k, int64_t *out_rows,
+                  double *out_scores);
+
 /* Cross-GPU pruning thresholds for a row-sharded GFKB (one process per GPU, all ranks hold the SAME resident query
  * batch).  Block-max pruning needs a lower bound of every query's GLOBAL k-th score; a shard scanning alone only knows
  * its own.  export: make this index's threshold array (int32 float bits per sorted query slot, `capacity` queries)

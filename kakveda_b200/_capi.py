@@ -80,6 +80,8 @@ SIGNATURES = {
     "kv_index_live_rows": (C.c_int64, [C.c_void_p]),
     "kv_index_deleted_rows": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint8), C.c_int64]),
     "kv_rescore_pairs": (C.c_int, [C.c_void_p, c_i64p, c_u32p, c_u32p, c_f64p, C.c_int64, C.c_int, c_i64p, c_f64p]),
+    "kv_exact_topk": (C.c_int, [C.c_void_p, c_i64p, c_u32p, c_u32p, c_f64p, C.POINTER(C.c_int32), C.c_int, C.c_int64, C.c_int,
+                                c_i64p, c_f64p]),
     "kv_range_resident": (C.c_int, [C.c_void_p, C.c_float, c_i64p]),
     "kv_range_fetch": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f32p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "kv_range_fetch_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -1787,12 +1787,12 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
     rc = score_impl(ix, irr.ids.data() + a, irr.tf.data() + a, e - a, irr.oov[i], nullptr);
     if (rc != KV_OK) return rc;
     if (b.distinct)
-      select_topk_distinct_kernel<<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
+      select_topk_distinct_kernel<float><<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
                                                      ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->labels.d_row.p,
                                                      ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix),
                                                      ix->groups.d_row.p, d_out_s + q * k, d_out_r + q * k);
     else
-      select_topk_kernel<<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
+      select_topk_kernel<float><<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
                                             ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->labels.d_row.p,
                                             ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix), d_out_s + q * k,
                                             d_out_r + q * k);
@@ -2054,6 +2054,46 @@ int kv_selfjoin_upload(kv_index *ix, int64_t q_begin, int64_t q_end) {
   return set_exclusions_locked(ix, ex.data(), n);
 }
 
+// caller holds ix->mu, the index is finalized and has rows: a query batch for K6 -- its CSR and |q|^2 exactly as K1a gets
+// them (prep_query, float64) -- in ix->d_rq_*, and room for n_q * k pairs in d_rq_rows / d_rq_out
+// (the copies read cst and ip, which the caller keeps until it synchronises the stream)
+static int rescore_upload(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
+                          const double *q_oov_tf2, int64_t n_q, int k, std::vector<double> &cst, std::vector<int64_t> &ip) {
+  const int64_t nnz = q_indptr[n_q] - q_indptr[0];
+  cudaStream_t s = ix->stream;
+  cst.resize((size_t)n_q);
+  ip.resize((size_t)n_q + 1);
+  for (int64_t q = 0; q <= n_q; q++) ip[(size_t)q] = q_indptr[q] - q_indptr[0];
+  parallel_for(n_q, n_q >= 2048 ? host_threads() : 1, [&](int, int64_t a, int64_t b) {
+    for (int64_t q = a; q < b; q++)
+      cst[(size_t)q] = host_query_norm(ix, q_ids + q_indptr[q], q_tf + q_indptr[q], q_indptr[q + 1] - q_indptr[q], q_oov_tf2 ? q_oov_tf2[q] : 0.0);
+  });
+  KV_CUDA(ix->d_rq_indptr.ensure(n_q + 1)); KV_CUDA(ix->d_rq_ids.ensure(std::max<int64_t>(nnz, 1)));
+  KV_CUDA(ix->d_rq_tf.ensure(std::max<int64_t>(nnz, 1))); KV_CUDA(ix->d_rq_const.ensure(n_q));
+  KV_CUDA(ix->d_rq_out.ensure(n_q * k)); KV_CUDA(ix->d_rq_rows.ensure(n_q * k));
+  KV_CUDA(cudaMemcpyAsync(ix->d_rq_indptr.p, ip.data(), (size_t)(n_q + 1) * 8, cudaMemcpyHostToDevice, s));
+  if (nnz) {
+    KV_CUDA(cudaMemcpyAsync(ix->d_rq_ids.p, q_ids + q_indptr[0], (size_t)nnz * 4, cudaMemcpyHostToDevice, s));
+    KV_CUDA(cudaMemcpyAsync(ix->d_rq_tf.p, q_tf + q_indptr[0], (size_t)nnz * 4, cudaMemcpyHostToDevice, s));
+  }
+  KV_CUDA(cudaMemcpyAsync(ix->d_rq_const.p, cst.data(), (size_t)n_q * 8, cudaMemcpyHostToDevice, s));
+  return KV_OK;
+}
+
+// caller holds ix->mu, after rescore_upload: K6 of the pairs (query q, global row d_rq_rows[q * k + j]) into d_rq_out
+static int rescore_launch(kv_index *ix, int64_t n_q, int k) {
+  RescoreParams P;
+  P.indptr = ix->indptr.p; P.ids = ix->ids.p; P.tf = ix->tf.p;
+  P.a64 = ix->d_a64.p; P.d64 = ix->d_d64.p; P.B64 = ix->d_B64.p; P.invperm = ix->d_invperm.p;
+  P.q_indptr = ix->d_rq_indptr.p; P.q_ids = ix->d_rq_ids.p; P.q_tf = ix->d_rq_tf.p;
+  P.q_nq = ix->d_rq_const.p;
+  P.rows = ix->d_rq_rows.p; P.n_q = n_q; P.n_rows = ix->n_rows; P.row_base = ix->row_base; P.V = ix->V;
+  P.k = k; P.jaccard = ix->jaccard; P.dead = dead_rows(ix); P.out = ix->d_rq_out.p;
+  rescore_kernel<<<(unsigned)((n_q * k * 32 + 255) / 256), 256, 0, ix->stream>>>(P);
+  KV_CUDA(cudaGetLastError());
+  return KV_OK;
+}
+
 int kv_rescore_pairs(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
                      const double *q_oov_tf2, int64_t n_q, int k, const int64_t *rows, double *out_scores) {
   if (!ix || n_q < 0 || k < 1 || (n_q > 0 && (!q_indptr || !rows || !out_scores)))
@@ -2069,33 +2109,63 @@ int kv_rescore_pairs(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_id
   }
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
-  // |q|^2 exactly as K1a gets it (prep_query, float64)
-  std::vector<double> cst((size_t)n_q);
-  std::vector<int64_t> ip((size_t)n_q + 1);
-  for (int64_t q = 0; q <= n_q; q++) ip[(size_t)q] = q_indptr[q] - q_indptr[0];
-  parallel_for(n_q, n_q >= 2048 ? host_threads() : 1, [&](int, int64_t a, int64_t b) {
-    for (int64_t q = a; q < b; q++)
-      cst[(size_t)q] = host_query_norm(ix, q_ids + q_indptr[q], q_tf + q_indptr[q], q_indptr[q + 1] - q_indptr[q], q_oov_tf2 ? q_oov_tf2[q] : 0.0);
-  });
-  KV_CUDA(ix->d_rq_indptr.ensure(n_q + 1)); KV_CUDA(ix->d_rq_ids.ensure(std::max<int64_t>(nnz, 1)));
-  KV_CUDA(ix->d_rq_tf.ensure(std::max<int64_t>(nnz, 1))); KV_CUDA(ix->d_rq_const.ensure(n_q));
-  KV_CUDA(ix->d_rq_out.ensure(n_q * k)); KV_CUDA(ix->d_rq_rows.ensure(n_q * k));
-  KV_CUDA(cudaMemcpyAsync(ix->d_rq_indptr.p, ip.data(), (size_t)(n_q + 1) * 8, cudaMemcpyHostToDevice, s));
-  if (nnz) {
-    KV_CUDA(cudaMemcpyAsync(ix->d_rq_ids.p, q_ids + q_indptr[0], (size_t)nnz * 4, cudaMemcpyHostToDevice, s));
-    KV_CUDA(cudaMemcpyAsync(ix->d_rq_tf.p, q_tf + q_indptr[0], (size_t)nnz * 4, cudaMemcpyHostToDevice, s));
-  }
-  KV_CUDA(cudaMemcpyAsync(ix->d_rq_const.p, cst.data(), (size_t)n_q * 8, cudaMemcpyHostToDevice, s));
+  std::vector<double> cst;
+  std::vector<int64_t> ip;
+  int rc = rescore_upload(ix, q_indptr, q_ids, q_tf, q_oov_tf2, n_q, k, cst, ip);
+  if (rc != KV_OK) return rc;
   KV_CUDA(cudaMemcpyAsync(ix->d_rq_rows.p, rows, (size_t)n_q * k * 8, cudaMemcpyHostToDevice, s));
-  RescoreParams P;
-  P.indptr = ix->indptr.p; P.ids = ix->ids.p; P.tf = ix->tf.p;
-  P.a64 = ix->d_a64.p; P.d64 = ix->d_d64.p; P.B64 = ix->d_B64.p; P.invperm = ix->d_invperm.p;
-  P.q_indptr = ix->d_rq_indptr.p; P.q_ids = ix->d_rq_ids.p; P.q_tf = ix->d_rq_tf.p;
-  P.q_nq = ix->d_rq_const.p;
-  P.rows = ix->d_rq_rows.p; P.n_q = n_q; P.n_rows = ix->n_rows; P.row_base = ix->row_base; P.V = ix->V;
-  P.k = k; P.jaccard = ix->jaccard; P.dead = dead_rows(ix); P.out = ix->d_rq_out.p;
-  rescore_kernel<<<(unsigned)((n_q * k * 32 + 255) / 256), 256, 0, s>>>(P);
-  KV_CUDA(cudaGetLastError());
+  if ((rc = rescore_launch(ix, n_q, k)) != KV_OK) return rc;
+  KV_CUDA(cudaMemcpyAsync(out_scores, ix->d_rq_out.p, (size_t)n_q * k * 8, cudaMemcpyDeviceToHost, s));
+  KV_CUDA(cudaStreamSynchronize(s));
+  return KV_OK;
+}
+
+int kv_exact_topk(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
+                  const double *q_oov_tf2, const int32_t *labels, int distinct, int64_t n_q, int k, int64_t *out_rows,
+                  double *out_scores) {
+  if (!ix || n_q < 0 || k < 1 || k > 32 || (n_q > 0 && (!q_indptr || !out_rows || !out_scores)))
+    return kv_fail(KV_ERR_INVALID, "kv_exact_topk: bad arguments (k must be 1..32)");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (!ix->finalized) return kv_fail(KV_ERR_STATE, "kv_exact_topk: index not finalized");
+  if (n_q == 0) return KV_OK;
+  const int64_t nnz = q_indptr[n_q] - q_indptr[0];
+  if (nnz < 0 || (nnz > 0 && (!q_ids || !q_tf))) return kv_fail(KV_ERR_INVALID, "kv_exact_topk: bad query CSR");
+  bool filtered = false;
+  for (int64_t q = 0; labels && q < n_q; q++) {
+    if (labels[q] < -1) return kv_fail(KV_ERR_INVALID, "kv_exact_topk: label %d of query %lld is below -1", labels[q], (long long)q);
+    filtered |= labels[q] >= 0;
+  }
+  if (ix->n_rows == 0) {
+    for (int64_t i = 0; i < n_q * k; i++) { out_rows[i] = -1; out_scores[i] = -INFINITY; }
+    return KV_OK;
+  }
+  if (filtered && !ix->labels.ready(ix->n_rows))
+    return kv_fail(KV_ERR_STATE, "kv_exact_topk: a filtered query needs row labels (kv_index_set_row_labels)");
+  if (distinct && !ix->groups.ready(ix->n_rows))
+    return kv_fail(KV_ERR_STATE, "kv_exact_topk: distinct needs row groups (kv_index_set_row_groups)");
+  KV_CUDA(cudaSetDevice(ix->device));
+  cudaStream_t s = ix->stream;
+  std::vector<double> cst;
+  std::vector<int64_t> ip;
+  int rc = rescore_upload(ix, q_indptr, q_ids, q_tf, q_oov_tf2, n_q, k, cst, ip);
+  if (rc != KV_OK) return rc;
+  for (int64_t q = 0; q < n_q; q++) {
+    // K1a into ix->d_scores, then the best k rows in float64 order into d_rq_rows (global) -- the K1a scores they come
+    // with land in d_rq_out, which K6 overwrites below
+    const int64_t a = q_indptr[q], e = q_indptr[q + 1];
+    if ((rc = score_impl(ix, q_ids + a, q_tf + a, e - a, q_oov_tf2 ? q_oov_tf2[q] : 0.0, nullptr)) != KV_OK) return rc;
+    const int lab = labels ? labels[q] : -1;
+    if (distinct)
+      select_topk_distinct_kernel<double><<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k, -1, ix->labels.d_row.p,
+                                                             lab, dead_rows(ix), ix->groups.d_row.p, ix->d_rq_out.p + q * k,
+                                                             ix->d_rq_rows.p + q * k);
+    else
+      select_topk_kernel<double><<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k, -1, ix->labels.d_row.p, lab,
+                                                    dead_rows(ix), ix->d_rq_out.p + q * k, ix->d_rq_rows.p + q * k);
+    KV_CUDA(cudaGetLastError());
+  }
+  if ((rc = rescore_launch(ix, n_q, k)) != KV_OK) return rc;
+  KV_CUDA(cudaMemcpyAsync(out_rows, ix->d_rq_rows.p, (size_t)n_q * k * 8, cudaMemcpyDeviceToHost, s));
   KV_CUDA(cudaMemcpyAsync(out_scores, ix->d_rq_out.p, (size_t)n_q * k * 8, cudaMemcpyDeviceToHost, s));
   KV_CUDA(cudaStreamSynchronize(s));
   return KV_OK;

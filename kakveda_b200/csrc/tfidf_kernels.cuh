@@ -1688,28 +1688,31 @@ __global__ void fill_null_kernel(const int *__restrict__ null_q, int n_null, int
 
 // Fallback selection for one (irregular) query: k passes of block-wide arg-best over float64 scores.  lab >= 0: only
 // rows with labels[row] == lab (by original row) compete; dead (NULL: none) marks deleted rows, which never do.
+// S: the precision the scores are compared and reported in -- float for the top-k (the float32 value K1b reports),
+// double for kv_exact_topk, whose order is the float64 one.
+template <typename S>
 __global__ void select_topk_kernel(const double *__restrict__ scores, int64_t n, int64_t row_base, int k, int64_t excl,
                                    const int *__restrict__ labels, int lab, const uint8_t *__restrict__ dead,
-                                   float *out_s, long long *out_r) {
-  __shared__ float s_s[32];
+                                   S *out_s, long long *out_r) {
+  __shared__ S s_s[32];
   __shared__ long long s_r[32];
-  __shared__ float prev_s;
+  __shared__ S prev_s;
   __shared__ long long prev_r;
   if (threadIdx.x == 0) { prev_s = INFINITY; prev_r = -1; }
   __syncthreads();
   for (int j = 0; j < k; j++) {
-    float bs = -INFINITY;
+    S bs = -INFINITY;
     long long br = -1;
-    const float ps = prev_s;
+    const S ps = prev_s;
     const long long pr = prev_r;
     for (int64_t r = threadIdx.x; r < n; r += blockDim.x) {
       if (r == excl || (lab >= 0 && labels[r] != lab) || (dead && dead[r])) continue;
-      float s = (float)scores[r];
+      S s = (S)scores[r];
       bool after = (s < ps) || (s == ps && r > pr);  // strictly after the previously selected pair
       if (after && (br < 0 || s > bs || (s == bs && r < br))) { bs = s; br = r; }
     }
     for (int o = 16; o; o >>= 1) {
-      float s2 = __shfl_xor_sync(FULL, bs, o);
+      S s2 = __shfl_xor_sync(FULL, bs, o);
       long long r2 = __shfl_xor_sync(FULL, br, o);
       if (r2 >= 0 && (br < 0 || s2 > bs || (s2 == bs && r2 < br))) { bs = s2; br = r2; }
     }
@@ -1720,7 +1723,7 @@ __global__ void select_topk_kernel(const double *__restrict__ scores, int64_t n,
       bs = threadIdx.x < nw ? s_s[threadIdx.x] : -INFINITY;
       br = threadIdx.x < nw ? s_r[threadIdx.x] : -1;
       for (int o = 16; o; o >>= 1) {
-        float s2 = __shfl_xor_sync(FULL, bs, o);
+        S s2 = __shfl_xor_sync(FULL, bs, o);
         long long r2 = __shfl_xor_sync(FULL, br, o);
         if (r2 >= 0 && (br < 0 || s2 > bs || (s2 == bs && r2 < br))) { bs = s2; br = r2; }
       }
@@ -1737,25 +1740,26 @@ __global__ void select_topk_kernel(const double *__restrict__ scores, int64_t n,
 // select_topk_kernel of a distinct batch: each pass takes the next row in (score desc, row asc) order whose group
 // (groups: by local row) is not taken yet.  Every row before the previous pick is a pick or of a taken group, so
 // "strictly after the previous pick" stays the only order constraint.  The <= k taken groups sit in shared memory and
-// are only consulted for a row that would beat the thread's current best.
+// are only consulted for a row that would beat the thread's current best.  S as in select_topk_kernel.
+template <typename S>
 __global__ void select_topk_distinct_kernel(const double *__restrict__ scores, int64_t n, int64_t row_base, int k, int64_t excl,
                                             const int *__restrict__ labels, int lab, const uint8_t *__restrict__ dead,
-                                            const int *__restrict__ groups, float *out_s, long long *out_r) {
-  __shared__ float s_s[32];
+                                            const int *__restrict__ groups, S *out_s, long long *out_r) {
+  __shared__ S s_s[32];
   __shared__ long long s_r[32];
   __shared__ int s_taken[32];
-  __shared__ float prev_s;
+  __shared__ S prev_s;
   __shared__ long long prev_r;
   if (threadIdx.x == 0) { prev_s = INFINITY; prev_r = -1; }
   __syncthreads();
   for (int j = 0; j < k; j++) {
-    float bs = -INFINITY;
+    S bs = -INFINITY;
     long long br = -1;
-    const float ps = prev_s;
+    const S ps = prev_s;
     const long long pr = prev_r;
     for (int64_t r = threadIdx.x; r < n; r += blockDim.x) {
       if (r == excl || (lab >= 0 && labels[r] != lab) || (dead && dead[r])) continue;
-      float s = (float)scores[r];
+      S s = (S)scores[r];
       bool after = (s < ps) || (s == ps && r > pr);
       if (after && (br < 0 || s > bs || (s == bs && r < br))) {
         const int g = groups[r];
@@ -1765,7 +1769,7 @@ __global__ void select_topk_distinct_kernel(const double *__restrict__ scores, i
       }
     }
     for (int o = 16; o; o >>= 1) {
-      float s2 = __shfl_xor_sync(FULL, bs, o);
+      S s2 = __shfl_xor_sync(FULL, bs, o);
       long long r2 = __shfl_xor_sync(FULL, br, o);
       if (r2 >= 0 && (br < 0 || s2 > bs || (s2 == bs && r2 < br))) { bs = s2; br = r2; }
     }
@@ -1776,7 +1780,7 @@ __global__ void select_topk_distinct_kernel(const double *__restrict__ scores, i
       bs = threadIdx.x < nw ? s_s[threadIdx.x] : -INFINITY;
       br = threadIdx.x < nw ? s_r[threadIdx.x] : -1;
       for (int o = 16; o; o >>= 1) {
-        float s2 = __shfl_xor_sync(FULL, bs, o);
+        S s2 = __shfl_xor_sync(FULL, bs, o);
         long long r2 = __shfl_xor_sync(FULL, br, o);
         if (r2 >= 0 && (br < 0 || s2 > bs || (s2 == bs && r2 < br))) { bs = s2; br = r2; }
       }

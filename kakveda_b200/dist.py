@@ -32,7 +32,9 @@ import numpy as np
 
 from . import _capi, _devout
 from ._capi import no_distinct
-from .similarity import FeatureBatch, GfkbIndex, Vocabulary, _featurize_on_device, gather_rows, text_order
+from .gfkb import MATCH_LIMIT
+from .similarity import FeatureBatch, GfkbIndex, Vocabulary, _featurize_on_device, gather_rows, pack_texts, text_order
+from .store import MAX_LIMIT, GfkbStore, ambiguous_candidates
 
 
 def shard_bounds(n_rows: int, world: int, rank: int) -> Tuple[int, int]:
@@ -259,6 +261,35 @@ def _host(out, device_out: bool):
     return out if device_out else tuple(t.cpu().numpy() for t in out)
 
 
+def merge_exact_lists(rows: np.ndarray, scores: np.ndarray, k: int,
+                      groups: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
+    """Per query, several ordered lists of (global row, float64 score) side by side ([Q, m] each, -1 rows unused) ->
+    the first ``k`` in (score desc, row asc) order, (-1, -inf) past the last.  ``groups`` (by global row): keep only the
+    first row of each group -- exact when each list is the distinct top-k of disjoint rows."""
+    q = rows.shape[0]
+    big = np.where(rows < 0, np.iinfo(np.int64).max, rows)
+    order = np.lexsort((big, -scores), axis=1)   # last key is primary; a -1 row carries -inf
+    rows, scores = np.take_along_axis(rows, order, axis=1), np.take_along_axis(scores, order, axis=1)
+    out_r = np.full((q, k), -1, dtype=np.int64)
+    out_s = np.full((q, k), -np.inf)
+    if groups is None:
+        m = min(k, rows.shape[1])
+        out_r[:, :m], out_s[:, :m] = rows[:, :m], scores[:, :m]
+        out_s[out_r < 0] = -np.inf
+        return out_r, out_s
+    for i in range(q):
+        seen, j = set(), 0
+        for r, sc in zip(rows[i].tolist(), scores[i].tolist()):
+            if j == k:
+                break
+            if r < 0 or groups[r] in seen:
+                continue
+            seen.add(groups[r])
+            out_r[i, j], out_s[i, j] = r, sc
+            j += 1
+    return out_r, out_s
+
+
 class ShardedGfkb:
     """This rank's share of a GFKB job spread over ``world`` GPUs.
 
@@ -289,7 +320,11 @@ class ShardedGfkb:
         self._corpus = None   # (data, offsets, mode) of the corpus text: the queries of selfjoin_range
         self._has_labels = self._has_groups = False   # set_row_labels / set_row_groups
         self._groups_dev = None   # rows mode on several GPUs: the group of every global row, for the distinct merges
+        self._groups_host = None  # set_row_groups: the group of every global row, for the merge of exact_topk
         self._deleted = None      # delete_rows: bool per global row (every rank deletes the same rows)
+        # (live df int64 by feature, live row count) of the whole sharded corpus, all-reduced by build_packed and
+        # delete_rows in rows mode on several GPUs (None: not known, the shards' own statistics when W = 1)
+        self._stats: Optional[Tuple[np.ndarray, int]] = None
 
     def build_packed(self, data, offsets: np.ndarray, mode: int = 0, n_threads: int = 0) -> None:
         import torch
@@ -308,10 +343,13 @@ class ShardedGfkb:
             self.index = GfkbIndex(device=self.device, row_base=lo, vocab=self.vocab)
             self.index.add_features(fb, lo, hi)
         fb.close()
+        self._stats = None
         if self.world > 1 and self.mode == "rows":
             df = torch.from_numpy(self.index.local_df().astype(np.int32)).to(f"cuda:{self.device}")
             allreduce_df(df, self.group)
-            self.index.set_global_df(df.cpu().numpy().astype(np.uint32), self.n_global)
+            df = df.cpu().numpy()
+            self._stats = (df.astype(np.int64), self.n_global)
+            self.index.set_global_df(df.astype(np.uint32), self.n_global)
         self.index.finalize()
 
     def _exchange_thresholds(self, n_q: int) -> None:
@@ -671,7 +709,7 @@ class ShardedGfkb:
 
         if global_groups is None:
             self.index.set_row_groups(None)
-            self._has_groups, self._groups_dev = False, None
+            self._has_groups, self._groups_dev, self._groups_host = False, None, None
             return
         grp = np.ascontiguousarray(global_groups, dtype=np.int32).reshape(-1)
         if len(grp) != self.n_global:
@@ -680,33 +718,94 @@ class ShardedGfkb:
             raise ValueError("set_row_groups: a negative group")
         self.index.set_row_groups(self._local_part(grp))
         self._has_groups = True
+        self._groups_host = grp
         self._groups_dev = torch.from_numpy(grp).to(f"cuda:{self.device}") if self.mode == "rows" and self.world > 1 else None
 
+    # ---- global statistics -------------------------------------------------------------------------------------------
+    def _reduce_stats(self) -> Tuple[np.ndarray, int]:
+        """(live df int64, live row count) of the whole sharded corpus: ONE all-reduce in rows mode on several GPUs
+        (cached until the next build or deletion), this shard's own statistics otherwise."""
+        import torch
+
+        if self.world > 1 and self.mode == "rows":
+            if self._stats is None:
+                cnt = torch.from_numpy(np.append(self.index.local_df().astype(np.int64), self.index.n_live_rows)).to(f"cuda:{self.device}")
+                allreduce_df(cnt, self.group)
+                cnt = cnt.cpu().numpy()
+                self._stats = (cnt[:-1], int(cnt[-1]))
+            return self._stats
+        return self.index.local_df().astype(np.int64), self.index.n_live_rows
+
+    @staticmethod
+    def _check_extra(extra_df: Optional[np.ndarray], extra_rows: int) -> Optional[np.ndarray]:
+        if extra_df is None:
+            if extra_rows:
+                raise ValueError("extra_rows without extra_df")
+            return None
+        extra = np.ascontiguousarray(extra_df, dtype=np.int64).reshape(-1)
+        if extra_rows < 0 or (len(extra) and extra.min() < 0):
+            raise ValueError("extra segment statistics: a negative count")
+        return extra
+
+    def _set_stats(self, extra: Optional[np.ndarray], extra_rows: int) -> Tuple[np.ndarray, int]:
+        """The corpus' statistics plus an extra segment's (df, rows) -> every shard, by a statistics-only finalize."""
+        df, n = self._reduce_stats()
+        v = max(len(self.vocab), len(df), 0 if extra is None else len(extra))
+        tot = np.zeros(v, dtype=np.int64)
+        tot[:len(df)] += df
+        if extra is not None:
+            tot[:len(extra)] += extra
+        n += extra_rows
+        self.index.set_global_df(tot.astype(np.uint32), n)
+        self.index.finalize()
+        return tot, n
+
+    def set_statistics(self, extra_df: Optional[np.ndarray] = None, extra_rows: int = 0) -> Tuple[np.ndarray, int]:
+        """Global TF-IDF statistics for a corpus that is this sharded GFKB PLUS an extra segment held elsewhere (e.g.
+        the replicated tail of ``ShardedGfkbStore``): df = the shards' live df + ``extra_df``, N = their live rows +
+        ``extra_rows``; every shard then refreshes with a statistics-only finalize.  A collective (every rank passes the
+        same arguments), but the shards' df are all-reduced only once per build or deletion and cached, so a refresh
+        after an append to the extra segment exchanges nothing.  Returns ``(df int64 [vocabulary], N)``, which the extra
+        segment needs too.  Bad arguments raise ValueError on every rank before anything is exchanged."""
+        extra = self._check_extra(extra_df, extra_rows)
+        return self._set_stats(extra, int(extra_rows))
+
     # ---- row deletion ------------------------------------------------------------------------------------------------
-    def delete_rows(self, global_rows) -> None:
+    def delete_rows(self, global_rows, extra_df: Optional[np.ndarray] = None,
+                    extra_rows: int = 0) -> Optional[Tuple[np.ndarray, int]]:
         """Delete GLOBAL rows (any order, duplicates and rows deleted before allowed).  A collective: every rank calls it
         with the same rows.  Each shard deletes the rows it holds; in rows mode on several GPUs the live document
         frequencies and the live row count are then all-reduced, and every shard refreshes its statistics with a
         statistics-only finalize, so that every search afterwards equals a single index with the same deletions.  Rows
-        outside the corpus raise ValueError on every rank before anything is deleted.  The resident batch is dropped."""
+        outside the corpus raise ValueError on every rank before anything is deleted.  The resident batch is dropped.
+        ``extra_df`` / ``extra_rows``: the statistics of an extra segment, as for ``set_statistics``, added in the same
+        refresh (one all-reduce for the whole deletion); the call then returns what ``set_statistics`` returns."""
         import torch
 
         rows = np.unique(np.ascontiguousarray(global_rows, dtype=np.int64).reshape(-1))
         if len(rows) and (rows[0] < 0 or rows[-1] >= self.n_global):
             bad = rows[0] if rows[0] < 0 else rows[-1]
             raise ValueError(f"delete_rows: row {bad} outside the corpus of {self.n_global} rows")
+        extra = self._check_extra(extra_df, extra_rows)
         local = self._local_rows(rows)
         if len(local):
             self.index.delete_rows(local)
-        if self.world > 1 and self.mode == "rows":
-            cnt = torch.from_numpy(np.append(self.index.local_df().astype(np.int64), self.index.n_live_rows)).to(f"cuda:{self.device}")
-            allreduce_df(cnt, self.group)
-            cnt = cnt.cpu().numpy()
-            self.index.set_global_df(cnt[:-1].astype(np.uint32), int(cnt[-1]))
-        self.index.finalize()
+        self._stats = None
+        out = None
+        if extra is not None:
+            out = self._set_stats(extra, int(extra_rows))
+        else:
+            if self.world > 1 and self.mode == "rows":
+                cnt = torch.from_numpy(np.append(self.index.local_df().astype(np.int64), self.index.n_live_rows)).to(f"cuda:{self.device}")
+                allreduce_df(cnt, self.group)
+                cnt = cnt.cpu().numpy()
+                self._stats = (cnt[:-1], int(cnt[-1]))
+                self.index.set_global_df(cnt[:-1].astype(np.uint32), int(cnt[-1]))
+            self.index.finalize()
         if self._deleted is None:
             self._deleted = np.zeros(self.n_global, dtype=bool)
         self._deleted[rows] = True
+        return out
 
     def deleted_mask(self) -> np.ndarray:
         """bool [n_global]: which global rows are deleted (the same on every rank)."""
@@ -716,6 +815,52 @@ class ShardedGfkb:
     def n_live_rows(self) -> int:
         """The global row count minus the deleted rows."""
         return self.n_global - (0 if self._deleted is None else int(self._deleted.sum()))
+
+    # ---- exact top-k -------------------------------------------------------------------------------------------------
+    def exact_topk(self, qfb: FeatureBatch, k: int, labels: Optional[np.ndarray] = None,
+                   distinct: bool = False) -> Tuple[np.ndarray, np.ndarray]:
+        """Every query's best ``k`` rows over the whole sharded corpus with no candidate stage: ``(rows int64 [Q,k],
+        scores float64 [Q,k])``, global rows ordered by (score desc, row asc), (-1, -inf) past the last; identical on
+        every rank.  Each shard runs ``GfkbIndex.exact_topk`` (K1a over its rows, selection on the device, K6 scores:
+        only k rows per query leave the device); in rows mode on several GPUs ONE all-gather carries the shards' lists
+        and every rank merges them.  ``labels`` / ``distinct`` as for ``topk_resident``; a distinct merge keeps the
+        first row of each group.  A collective; bad arguments raise ValueError on every rank before it starts."""
+        import torch
+
+        q = qfb.n
+        if not 1 <= k <= 32:
+            raise ValueError(f"exact_topk: k must be 1..32, not {k}")
+        if labels is not None:
+            labels = np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
+            if len(labels) != q:
+                raise ValueError(f"labels: {len(labels)} labels for a batch of {q} queries")
+            if q and labels.min() < -1:
+                raise ValueError("labels: a label below -1")
+            if not self._has_labels:
+                raise ValueError("labels: the sharded index has no row labels (set_row_labels)")
+        if distinct and not self._has_groups:
+            raise ValueError("distinct: the sharded index has no row groups (set_row_groups)")
+        rows, scores = self.index.exact_topk(qfb, k, labels, distinct)
+        if self.row_map is not None:   # text-range shard: local -> global rows (ascending, so ties keep their order)
+            rows = np.where(rows >= 0, self._row_map_host[np.clip(rows, 0, None)], -1)
+        if self.world == 1 or self.mode != "rows":
+            return rows, scores
+        dev = f"cuda:{self.device}"
+        buf = torch.empty(16 * q * k, dtype=torch.uint8)
+        buf[:8 * q * k].view(torch.float64).copy_(torch.from_numpy(scores.reshape(-1)))
+        buf[8 * q * k:].view(torch.int64).copy_(torch.from_numpy(rows.reshape(-1)))
+        got = gather_packed(buf.to(dev), self.group).cpu()
+        s_all = got[:, :8 * q * k].contiguous().view(torch.float64).numpy().reshape(self.world, q, k)
+        r_all = got[:, 8 * q * k:].contiguous().view(torch.int64).numpy().reshape(self.world, q, k)
+        s_all = s_all.transpose(1, 0, 2).reshape(q, self.world * k)
+        r_all = r_all.transpose(1, 0, 2).reshape(q, self.world * k)
+        return merge_exact_lists(r_all, s_all, k, self._groups_host if distinct else None)
+
+    def close(self) -> None:
+        """Release this shard's index (the vocabulary stays with its owner)."""
+        if self.index is not None:
+            self.index.close()
+            self.index = None
 
     def _set_resident_range(self, qfb: FeatureBatch) -> None:
         """``set_resident`` that also takes a batch whose queries-mode slice on this rank is empty."""
@@ -1000,3 +1145,149 @@ class ShardedJaccard:
         if not parts:
             return self.index._empty_range(device_out)
         return _host(_concat_ranges(parts), device_out)
+
+
+class ShardedGfkbStore(GfkbStore):
+    """``GfkbStore`` on a row-sharded GFKB: the same upsert, match, warn and purge handlers, with the main segment
+    spread over the GPUs of one box.  The record logic (versioning, quarantine, the purge's record rewriting, the match
+    post-filters and the warning strings) is inherited unchanged; only the steps that touch the device index differ.
+
+    SPMD, like ``ShardedGfkb``: every rank constructs the store with the same ``path`` and ``tail_limit`` and calls the
+    same methods in the same order with the same arguments (and a ``now`` clock that gives every rank the same time, or
+    the ranks' copies of a record differ in their timestamps).  Every rank holds all records and the same vocabulary;
+    only rank 0 writes ``failures.jsonl`` and its purge backup, the others update their records in memory; the
+    constructor and ``load`` end with a barrier, so no rank reads a file rank 0 has already changed.  Results
+    are identical on every rank, and a rejected upsert or a bad argument raises the same exception on every rank
+    before any collective starts.
+
+    Segments: MAIN is a ``ShardedGfkb`` in rows mode (contiguous ranges of record rows per rank), built from the
+    records' texts; TAIL holds the records appended since the last rebuild (at most ``tail_limit``) as a ``GfkbIndex``
+    replicated on every rank (row_base = main rows, the store's vocabulary), so an upsert exchanges nothing.  The global
+    statistics are the main shards' live df (all-reduced once per build or deletion and cached) plus the tail's,
+    N = all records; the main shards and the tail get them through statistics-only finalizes.  Queries: the sharded
+    top-k of MAIN, its candidates re-scored in float64 by every shard (K6: -inf for another shard's rows) and combined
+    with one MAX all-reduce, the tail's candidates as in ``GfkbStore``, then the same host merge.  The exact fallback
+    runs ``kv_exact_topk`` on every shard and on the tail and merges their ``limit`` rows per query (one all-gather):
+    no score vector leaves a device.  A purge deletes the main rows and refreshes every statistic in one all-reduce.
+
+    Not supported: the sidecar and the persisted layout, queries mode and text-order shards (ValueError)."""
+
+    def __init__(self, path=None, device: int = 0, rank: int = 0, world: int = 1, group=None, tail_limit: int = 65536,
+                 now=None, sidecar=None, mode: str = "rows", order: str = "index"):
+        if sidecar is not None:
+            raise ValueError("ShardedGfkbStore: the sidecar and the persisted layout are not supported on a sharded GFKB")
+        if mode != "rows":
+            raise ValueError("ShardedGfkbStore: only rows mode is supported (queries mode holds the whole index on every rank)")
+        if order != "index":
+            raise ValueError("ShardedGfkbStore: only index-order shards are supported (not text order)")
+        self.rank, self.world, self.group = rank, world, group
+        self._read_file = False
+        super().__init__(path, device=device, tail_limit=tail_limit, now=now)
+        if not self._read_file:
+            self._barrier()
+
+    def _barrier(self) -> None:
+        """Rank 0 writes the file as soon as it returns from an upsert or a purge, and the ranks run without an exchange
+        in between: every rank must have read (or found no) file before rank 0 may change it."""
+        if self.world > 1:
+            import torch.distributed as dist
+
+            dist.barrier(group=self.group)
+
+    def load(self) -> None:
+        super().load()
+        self._read_file = True
+        self._barrier()
+
+    @property
+    def _writes_file(self) -> bool:
+        return self.path is not None and self.rank == 0
+
+    def _build_main(self, texts) -> None:
+        main = ShardedGfkb(self.device, self.rank, self.world, self.group)
+        main.vocab.close()
+        main.vocab = self.vocab   # one vocabulary for both segments and every rebuild, as in GfkbStore
+        self._main = main
+        main.build_packed(*pack_texts(texts))
+
+    def _refresh_statistics(self) -> None:
+        tail = self._tail
+        extra = (tail.local_df(), tail.n_live_rows) if tail is not None else (None, 0)
+        df, n = self._main.set_statistics(*extra)
+        if tail is not None:
+            tail.set_global_df(df.astype(np.uint32), n)
+            tail.finalize()
+        self.stats["stat_refreshes" if self._main.index.last_finalize_kind == 2 else "full_rebuilds"] += 1
+
+    def _delete_dev_rows(self, gone: np.ndarray) -> bool:
+        if self._n_deleted + len(gone) > max(self.tail_limit, 0):
+            return True   # the next _sync compacts the main segment: nothing to delete or exchange now
+        main_rows = gone[gone < self._n_main]
+        tail = self._tail
+        if tail is not None and len(gone) > len(main_rows):
+            tail.delete_rows(gone[gone >= self._n_main] - self._n_main)
+        extra = (tail.local_df(), tail.n_live_rows) if tail is not None else (np.zeros(0, np.int64), 0)
+        if len(main_rows):   # the deletion's all-reduce carries the refreshed statistics
+            df, n = self._main.delete_rows(main_rows, *extra)
+        else:                # only tail rows went: the cached main statistics serve
+            df, n = self._main.set_statistics(*extra)
+        if tail is not None:
+            tail.set_global_df(df.astype(np.uint32), n)
+            tail.finalize()
+        self.stats["stat_refreshes"] += 1
+        return False
+
+    def _ensure_groups(self) -> None:
+        groups = None
+        if not self._main._has_groups:
+            groups = self._dev_groups(self._n_dev)
+            self._main.set_row_groups(groups[:self._n_main])
+        tail = self._tail
+        if tail is not None and tail.n_rows and not tail.has_row_groups:
+            groups = self._dev_groups(self._n_dev) if groups is None else groups
+            tail.set_row_groups(groups[self._n_main:self._n_main + tail.n_rows])
+
+    def _candidates(self, fb: FeatureBatch, k: int, limit: int = MATCH_LIMIT, labels: Optional[np.ndarray] = None,
+                    distinct: bool = False):
+        import torch
+        import torch.distributed as dist
+
+        kk = min(k, MAX_LIMIT)
+        if fb.n == 0:
+            return np.zeros((0, kk), np.int64), np.zeros((0, kk)), np.zeros(0, dtype=bool)
+        if distinct:
+            self._ensure_groups()
+        main = self._main
+        main.set_resident(fb)
+        s, r = main.topk_resident(kk, labels=labels, distinct=distinct)
+        s32, rows = s.cpu().numpy(), r.cpu().numpy()
+        amb = ambiguous_candidates(s32, rows, limit)
+        f64 = main.index.rescore(fb, rows)   # -inf for the rows of the other shards
+        if self.world > 1:
+            t = torch.from_numpy(f64).to(f"cuda:{self.device}")
+            dist.all_reduce(t, op=dist.ReduceOp.MAX, group=self.group)
+            f64 = t.cpu().numpy()
+        rows_all, f64_all = [rows], [f64]
+        if self._tail is not None and self._tail.n_rows:
+            s32, rows = self._segment_topk(self._tail, fb, kk, labels, distinct)
+            amb |= ambiguous_candidates(s32, rows, limit)
+            rows_all.append(rows)
+            f64_all.append(self._tail.rescore(fb, rows))
+        return self._merge_candidates(rows_all, f64_all, distinct) + (amb,)
+
+    def _exact_top(self, signature_text: str, limit: int, label: int = -1, distinct: bool = False):
+        if distinct:
+            self._ensure_groups()
+        lab = None if label < 0 else np.array([label], dtype=np.int32)
+        fb = self.vocab.featurize([signature_text], grow=False)
+        try:
+            parts = [self._main.exact_topk(fb, limit, lab, distinct)]
+            if self._tail is not None and self._tail.n_rows:
+                parts.append(self._tail.exact_topk(fb, limit, lab, distinct))
+        finally:
+            fb.close()
+        groups = self._dev_groups(self._n_dev) if distinct else None
+        rows, scores = merge_exact_lists(np.concatenate([p[0] for p in parts], axis=1),
+                                         np.concatenate([p[1] for p in parts], axis=1), limit, groups)
+        keep = rows[0] >= 0
+        return self._to_records(rows[0][keep]).tolist(), scores[0][keep].tolist()

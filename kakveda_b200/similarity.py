@@ -627,6 +627,24 @@ class GfkbIndex(_KvIndex):
                                                   _ptr(rows, C.c_int64), _ptr(out, C.c_double)))
         return out
 
+    def exact_topk(self, fb: FeatureBatch, k: int, labels: Optional[np.ndarray] = None,
+                   distinct: bool = False) -> Tuple[np.ndarray, np.ndarray]:
+        """(rows int64 [Q,k], scores float64 [Q,k]): each query's best k rows of this index with no candidate stage
+        (``kv_exact_topk``: K1a over every row, selection in float64 order on the device, K6 scores), global rows
+        ordered by (score desc, row asc), (-1, -inf) past the last.  ``labels`` / ``distinct`` as for
+        ``topk_features``.  K6 scores tie exactly for identical texts on any index, so lists of several indexes merge
+        into the stable order of one."""
+        rows = np.empty((fb.n, k), dtype=np.int64)
+        scores = np.empty((fb.n, k), dtype=np.float64)
+        lab = None if labels is None else np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
+        if lab is not None and len(lab) != fb.n:
+            raise ValueError(f"exact_topk: {len(lab)} labels for a batch of {fb.n} queries")
+        _capi.check(_capi.load().kv_exact_topk(self._h, _ptr(fb.indptr, C.c_int64), _ptr(fb.ids, C.c_uint32),
+                                               _ptr(fb.tf, C.c_uint32), _ptr(fb.oov, C.c_double),
+                                               None if lab is None else _ptr(lab, C.c_int32), int(distinct), fb.n, k,
+                                               _ptr(rows, C.c_int64), _ptr(scores, C.c_double)))
+        return rows, scores
+
     def topk_resident(self, k: int, d_scores_ptr: int, d_rows_ptr: int) -> None:
         """Device-only scan + merge of the uploaded batch into caller-owned device buffers."""
         _capi.check(_capi.load().kv_topk_resident(self._h, k, C.c_void_p(d_scores_ptr), C.c_void_p(d_rows_ptr)))

@@ -183,44 +183,7 @@ class GfkbStore:
         self._main_df = None
         n = len(self.records)
         if n:
-            texts = [self._index_text(i) for i in range(n)]
-            # the sidecar only serves a cold start (empty vocabulary); a compaction does not re-read and re-digest it
-            cold = self.sidecar_path is not None and len(self.vocab) == 0
-            cached = _sidecar.load(self.sidecar_path, texts) if cold else None
-            if cached is not None:
-                # cold start from the sidecar: the vocabulary and the first n0 rows come back as arrays
-                self.vocab.close()
-                self.vocab, head, n0 = cached
-                self._main = GfkbIndex(device=self.device, row_base=0, vocab=self.vocab)
-                self._main.add_features(head)
-                self.stats["sidecar_rows"] = n0
-                if n0 < n:
-                    rest = self.vocab.featurize(texts[n0:], grow=True)
-                    try:
-                        self._main.add_features(rest)
-                        if self.sidecar_path is not None:
-                            both = _sidecar.ArrayBatch(np.concatenate([head.indptr, rest.indptr[1:] + head.indptr[-1]]),
-                                                       np.concatenate([head.ids, rest.ids]), np.concatenate([head.tf, rest.tf]))
-                            _sidecar.save(self.sidecar_path, self.vocab, both, texts)
-                    finally:
-                        rest.close()
-            else:
-                self._main = GfkbIndex(device=self.device, row_base=0, vocab=self.vocab)
-                fb = self.vocab.featurize(texts, grow=True)
-                try:
-                    self._main.add_features(fb)
-                    if self.sidecar_path is not None:
-                        _sidecar.save(self.sidecar_path, self.vocab, fb, texts)
-                finally:
-                    fb.close()
-            # persisted scan layout next to the sidecar: a cold start then skips the host sort + block build as well
-            lay_path = Path(str(self.sidecar_path) + ".layout") if self.sidecar_path is not None else None
-            restored = lay_path is not None and self._main.load_layout(lay_path)
-            self._main.finalize()
-            if restored and self._main.last_finalize_kind == 2:
-                self.stats["layout_restored"] = self.stats.get("layout_restored", 0) + 1
-            elif lay_path is not None:
-                self._main.save_layout(lay_path)
+            self._build_main([self._index_text(i) for i in range(n)])
             self._main.set_row_labels(self._row_labels(0, n))
             self.stats["full_rebuilds"] += 1
         self._n_main = self._n_indexed = self._n_dev = n
@@ -228,6 +191,47 @@ class GfkbStore:
         self._row2rec = None
         self._n_deleted = 0
         self._dirty = False
+
+    def _build_main(self, texts: List[str]) -> None:
+        """The main segment over ``texts`` (one per record), finalized with the statistics of its own rows."""
+        n = len(texts)
+        # the sidecar only serves a cold start (empty vocabulary); a compaction does not re-read and re-digest it
+        cold = self.sidecar_path is not None and len(self.vocab) == 0
+        cached = _sidecar.load(self.sidecar_path, texts) if cold else None
+        if cached is not None:
+            # cold start from the sidecar: the vocabulary and the first n0 rows come back as arrays
+            self.vocab.close()
+            self.vocab, head, n0 = cached
+            self._main = GfkbIndex(device=self.device, row_base=0, vocab=self.vocab)
+            self._main.add_features(head)
+            self.stats["sidecar_rows"] = n0
+            if n0 < n:
+                rest = self.vocab.featurize(texts[n0:], grow=True)
+                try:
+                    self._main.add_features(rest)
+                    if self.sidecar_path is not None:
+                        both = _sidecar.ArrayBatch(np.concatenate([head.indptr, rest.indptr[1:] + head.indptr[-1]]),
+                                                   np.concatenate([head.ids, rest.ids]), np.concatenate([head.tf, rest.tf]))
+                        _sidecar.save(self.sidecar_path, self.vocab, both, texts)
+                finally:
+                    rest.close()
+        else:
+            self._main = GfkbIndex(device=self.device, row_base=0, vocab=self.vocab)
+            fb = self.vocab.featurize(texts, grow=True)
+            try:
+                self._main.add_features(fb)
+                if self.sidecar_path is not None:
+                    _sidecar.save(self.sidecar_path, self.vocab, fb, texts)
+            finally:
+                fb.close()
+        # persisted scan layout next to the sidecar: a cold start then skips the host sort + block build as well
+        lay_path = Path(str(self.sidecar_path) + ".layout") if self.sidecar_path is not None else None
+        restored = lay_path is not None and self._main.load_layout(lay_path)
+        self._main.finalize()
+        if restored and self._main.last_finalize_kind == 2:
+            self.stats["layout_restored"] = self.stats.get("layout_restored", 0) + 1
+        elif lay_path is not None:
+            self._main.save_layout(lay_path)
 
     def _dev_labels(self, n_dev: int) -> np.ndarray:
         """int32 failure-type label of the first ``n_dev`` device rows (main + tail), -1 for a deleted row."""
@@ -289,11 +293,16 @@ class GfkbStore:
                 self._row2rec = np.concatenate([self._row2rec, np.arange(self._n_indexed, len(self.records), dtype=np.int64)])
         self._n_dev += len(pending)
         self._n_indexed = len(self.records)
-        segments = [ix for ix in (self._main, self._tail) if ix is not None]
         if self._tail is not None:
             tail_labels = self._dev_labels(self._n_dev)[self._n_main:]
             self._tail.set_row_labels(np.maximum(tail_labels, 0))  # an append dropped them; a deleted row's label is moot
-        # global statistics = main + tail (the df all-reduce of a sharded GFKB, done in-process)
+        self._refresh_statistics()
+        self._dirty = False
+
+    def _refresh_statistics(self) -> None:
+        """Global statistics = main + tail (the df all-reduce of a sharded GFKB, done in-process) on both segments:
+        a statistics-only finalize of the main segment, a finalize of the tail."""
+        segments = [ix for ix in (self._main, self._tail) if ix is not None]
         v = len(self.vocab)
         if self._main_df is None:
             self._main_df = self._main.local_df().astype(np.int64)
@@ -309,7 +318,11 @@ class GfkbStore:
             self.stats["stat_refreshes"] += 1
         else:
             self.stats["full_rebuilds"] += 1
-        self._dirty = False
+
+    @property
+    def _writes_file(self) -> bool:
+        """Whether this store writes ``path`` (upserts append to it, a purge rewrites it)."""
+        return self.path is not None
 
     # -- upsert (services/gfkb/app.py:104-147) -----------------------------------------------------------------
     def upsert(self, req: Mapping[str, Any]) -> Dict[str, Any]:
@@ -347,7 +360,7 @@ class GfkbStore:
                 rec["resolution"] = req.get("resolution") or rec["resolution"]
                 rec["context_signature"] = req.get("context_signature") or rec["context_signature"]
                 created = False
-            if self.path is not None:
+            if self._writes_file:
                 with self.path.open("a", encoding="utf-8") as f:  # app.py:49-51
                     f.write(json.dumps(rec, ensure_ascii=False) + "\n")
             self.records.append(rec)
@@ -379,7 +392,7 @@ class GfkbStore:
                         continue
                 keep_idx.append(i)
                 kept += 1
-            if self.path is not None and self.path.exists():
+            if self._writes_file and self.path.exists():
                 if backup:
                     stamp = self._now().astimezone(timezone.utc).strftime("%Y%m%dT%H%M%SZ")
                     shutil.copy2(self.path, self.path.with_name(f"{self.path.name}.bak-{stamp}"))
@@ -416,16 +429,21 @@ class GfkbStore:
             row2rec = np.full(self._n_dev, -1, dtype=np.int64) if self._row2rec is None else self._row2rec.copy()
             row2rec[live_rows] = np.where(keep[:n_idx_old], new_idx[:n_idx_old], -1)
             self._row2rec = row2rec
-            main_rows = gone[gone < self._n_main]
-            if len(main_rows):
-                self._main.delete_rows(main_rows)
-                self._main_df = None  # the main segment's live df changed
-            if self._tail is not None and len(gone) > len(main_rows):
-                self._tail.delete_rows(gone[gone >= self._n_main] - self._n_main)
+            self._dirty = self._delete_dev_rows(gone)
             self._n_deleted += len(gone)
-            self._dirty = True
         if self.sidecar_path is not None:
             self._rewrite_sidecar(old_texts, keep_idx)
+
+    def _delete_dev_rows(self, gone: np.ndarray) -> bool:
+        """Delete the device rows ``gone`` (ascending) from the segments that hold them; returns whether the statistics
+        still need a refresh before the next search (here: yes, the next ``_sync`` runs it)."""
+        main_rows = gone[gone < self._n_main]
+        if len(main_rows):
+            self._main.delete_rows(main_rows)
+            self._main_df = None  # the main segment's live df changed
+        if self._tail is not None and len(gone) > len(main_rows):
+            self._tail.delete_rows(gone[gone >= self._n_main] - self._n_main)
+        return True
 
     def _rewrite_sidecar(self, old_texts: List[str], keep_idx: List[int]) -> None:
         """The sidecar of the surviving records (the vocabulary as it is, their CSR gathered from the old sidecar, the
@@ -473,14 +491,24 @@ class GfkbStore:
         for ix in (self._main, self._tail):
             if ix is None or ix.n_rows == 0:
                 continue
-            kk = min(k, MAX_LIMIT)
-            if distinct:
-                s32, rows = ix.topk_features(fb, kk, labels, distinct=True)
-            else:
-                s32, rows = ix.topk_features(fb, kk) if labels is None else ix.topk_features(fb, kk, labels)
+            s32, rows = self._segment_topk(ix, fb, min(k, MAX_LIMIT), labels, distinct)
             amb |= ambiguous_candidates(s32, rows, limit)
             rows_all.append(rows)
             f64_all.append(ix.rescore(fb, rows))
+        return self._merge_candidates(rows_all, f64_all, distinct) + (amb,)
+
+    @staticmethod
+    def _segment_topk(ix: GfkbIndex, fb: FeatureBatch, kk: int, labels: Optional[np.ndarray],
+                      distinct: bool) -> Tuple[np.ndarray, np.ndarray]:
+        """One segment's float32 candidates: (scores, global rows), each [Q, kk]."""
+        if distinct:
+            return ix.topk_features(fb, kk, labels, distinct=True)
+        return ix.topk_features(fb, kk) if labels is None else ix.topk_features(fb, kk, labels)
+
+    def _merge_candidates(self, rows_all: List[np.ndarray], f64_all: List[np.ndarray],
+                          distinct: bool) -> Tuple[np.ndarray, np.ndarray]:
+        """The segments' candidates with their float64 scores -> record indices and scores ordered (score desc, row
+        asc); ``distinct``: the first record of each group."""
         rows = np.concatenate(rows_all, axis=1)
         f64 = np.concatenate(f64_all, axis=1)
         big = np.where(rows < 0, np.iinfo(np.int64).max, rows)
@@ -488,7 +516,7 @@ class GfkbStore:
         recs, f64 = self._to_records(np.take_along_axis(rows, order, axis=1)), np.take_along_axis(f64, order, axis=1)
         if distinct:
             recs, f64 = self._first_of_groups(recs, f64)
-        return recs, f64, amb
+        return recs, f64
 
     def _first_of_groups(self, recs: np.ndarray, f64: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
         """Per query (rows ordered): the first record of each group, moved to the front; (-1, -inf) fill the rest."""
