@@ -238,6 +238,23 @@ int kv_selfjoin_upload(kv_index *ix, int64_t q_begin, int64_t q_end);
 int kv_index_set_row_labels(kv_index *ix, const int32_t *labels, int64_t n);
 int kv_query_set_filter(kv_index *ix, const int32_t *labels, int64_t n_q);
 
+/* Tag filter (e.g. a failure's affected apps).  kv_index_set_row_tags gives every local row a SET of tags >= 0, any
+ * number, possibly none: row r holds tags[indptr[r] .. indptr[r+1]), indptr[n_rows+1] starting at 0, n_rows ==
+ * kv_index_rows.  Lifetime as row labels: they survive either kind of finalize, kv_index_layout_load and deletions,
+ * kv_index_append drops them, NULL clears.  Tags touch no statistics, so setting them again on a finalized index needs
+ * no finalize.  kv_query_set_tag_filter gives each query of the resident batch a set of at most 16 tags (same CSR form,
+ * n_q == the batch; an empty set: no tag constraint), cleared by the next upload like kv_query_set_filter; NULL clears.
+ * A query with tags matches only the rows whose set meets its own (any of its tags); the label filter, exclusions,
+ * deletions and distinct mode apply as well, and scores, statistics and the order rules are those of the unfiltered
+ * search.  The scans skip the chunks whose live rows carry none of the query's tags (a 64-bit signature per chunk of
+ * bit t & 63 per tag), then test each row's mask and, when the index holds a tag >= 64, its exact set.  A null query
+ * with tags walks the index in row order until it has k eligible rows (the whole index when it has fewer).
+ * KV_ERR_INVALID: wrong lengths, indptr not starting at 0 or decreasing, a negative tag, more than 16 tags on a query,
+ * or a Jaccard index (mode 1).  KV_ERR_STATE: a query with tags on an index whose tags are missing or stale (appended
+ * rows), here or at the search. */
+int kv_index_set_row_tags(kv_index *ix, const int64_t *indptr, const int32_t *tags, int64_t n_rows);
+int kv_query_set_tag_filter(kv_index *ix, const int64_t *indptr, const int32_t *tags, int64_t n_q);
+
 /* Distinct top-k (field collapsing).  kv_index_set_row_groups gives every local row a group >= 0 (e.g. one id per
  * distinct text), groups[n] by local row; validation and lifetime as kv_index_set_row_labels: n == kv_index_rows and
  * every group >= 0 (else KV_ERR_INVALID), they survive either kind of finalize, kv_index_layout_load and deletions,
@@ -347,6 +364,12 @@ int kv_rescore_pairs(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_id
 int kv_exact_topk(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
                   const double *q_oov_tf2, const int32_t *labels, int distinct, int64_t n_q, int k, int64_t *out_rows,
                   double *out_scores);
+/* kv_exact_topk with a tag set per query (tag_indptr[n_q+1] from 0, tags; NULL: no query has tags), validated as by
+ * kv_query_set_tag_filter: a query with tags takes only the rows whose tag set meets its own.  A query with tags on an
+ * index without current row tags: KV_ERR_STATE. */
+int kv_exact_topk_tags(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
+                       const double *q_oov_tf2, const int32_t *labels, const int64_t *tag_indptr, const int32_t *tags,
+                       int distinct, int64_t n_q, int k, int64_t *out_rows, double *out_scores);
 
 /* Cross-GPU pruning thresholds for a row-sharded GFKB (one process per GPU, all ranks hold the SAME resident query
  * batch).  Block-max pruning needs a lower bound of every query's GLOBAL k-th score; a shard scanning alone only knows

@@ -74,6 +74,8 @@ SIGNATURES = {
     "kv_selfjoin_upload": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64]),
     "kv_index_set_row_labels": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int64]),
     "kv_query_set_filter": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int64]),
+    "kv_index_set_row_tags": (C.c_int, [C.c_void_p, c_i64p, C.POINTER(C.c_int32), C.c_int64]),
+    "kv_query_set_tag_filter": (C.c_int, [C.c_void_p, c_i64p, C.POINTER(C.c_int32), C.c_int64]),
     "kv_index_set_row_groups": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int64]),
     "kv_query_set_distinct": (C.c_int, [C.c_void_p, C.c_int]),
     "kv_index_delete_rows": (C.c_int, [C.c_void_p, c_i64p, C.c_int64]),
@@ -82,6 +84,8 @@ SIGNATURES = {
     "kv_rescore_pairs": (C.c_int, [C.c_void_p, c_i64p, c_u32p, c_u32p, c_f64p, C.c_int64, C.c_int, c_i64p, c_f64p]),
     "kv_exact_topk": (C.c_int, [C.c_void_p, c_i64p, c_u32p, c_u32p, c_f64p, C.POINTER(C.c_int32), C.c_int, C.c_int64, C.c_int,
                                 c_i64p, c_f64p]),
+    "kv_exact_topk_tags": (C.c_int, [C.c_void_p, c_i64p, c_u32p, c_u32p, c_f64p, C.POINTER(C.c_int32), c_i64p,
+                                     C.POINTER(C.c_int32), C.c_int, C.c_int64, C.c_int, c_i64p, c_f64p]),
     "kv_range_resident": (C.c_int, [C.c_void_p, C.c_float, c_i64p]),
     "kv_range_fetch": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f32p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "kv_range_fetch_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -63,6 +63,71 @@ struct RowSet {
   }
 };
 
+// A set of tags >= 0 per local row (kv_index_set_row_tags), CSR on the host.  Like a RowSet it describes the rows it
+// was set for (an append drops it) and every finalize rebuilds its device copies for the current scan layout: each
+// row's mask (tags_meet) and, unless every tag is < 64, its tags, by scan position; and the chunk signatures over the
+// live rows.
+struct RowTags {
+  std::vector<int64_t> indptr;
+  std::vector<int> tags;
+  bool has = false, on_device = false, masks_exact = true;  // masks_exact: every tag < 64
+  DevBuf<unsigned long long> d_mask_pos, d_chunk_sig;
+  DevBuf<int64_t> d_ptr_pos;
+  DevBuf<int> d_list_pos;
+
+  int set(const int64_t *ip, const int32_t *t, int64_t n, int64_t n_rows, const char *fn) {
+    if (n != n_rows) return kv_fail(KV_ERR_INVALID, "%s: %lld tag sets for an index of %lld rows", fn, (long long)n, (long long)n_rows);
+    if (!ip) return kv_fail(KV_ERR_INVALID, "%s: NULL indptr", fn);
+    if (ip[0] != 0) return kv_fail(KV_ERR_INVALID, "%s: indptr must start at 0", fn);
+    for (int64_t r = 0; r < n; r++)
+      if (ip[r + 1] < ip[r]) return kv_fail(KV_ERR_INVALID, "%s: indptr decreases at row %lld", fn, (long long)r);
+    if (ip[n] > 0 && !t) return kv_fail(KV_ERR_INVALID, "%s: NULL tags", fn);
+    bool exact = true;
+    for (int64_t r = 0; r < n; r++)
+      for (int64_t i = ip[r]; i < ip[r + 1]; i++) {
+        if (t[i] < 0) return kv_fail(KV_ERR_INVALID, "%s: tag %d of row %lld is negative", fn, t[i], (long long)r);
+        exact = exact && t[i] < 64;
+      }
+    indptr.assign(ip, ip + n + 1);
+    tags.assign(t, t + ip[n]);
+    masks_exact = exact;
+    has = true;
+    on_device = false;
+    return KV_OK;
+  }
+  void clear() {
+    indptr.clear();
+    tags.clear();
+    has = on_device = false;
+  }
+  bool ready(int64_t n_rows) const { return has && on_device && (int64_t)indptr.size() == n_rows + 1; }
+};
+
+// The tag filter of the resident batch (kv_query_set_tag_filter), while some query has tags: per query its mask (by
+// original query on the host, for the fallbacks; on the device by original query and by sorted slot) and its
+// ascending tags, -1 past the last (device: by original query for the fallbacks and the null fill, by sorted slot for
+// the scan).
+struct QueryTags {
+  bool on = false;
+  std::vector<unsigned long long> h_mask;
+  DevBuf<unsigned long long> d_mask_orig, d_mask_sorted;
+  DevBuf<int> d_tags_orig, d_tags_sorted;
+};
+
+// One query's tag set (tags[0, n)) as a mask and an ascending list of MAX_QTAGS slots, -1 past the last tag
+static int parse_query_tags(const int32_t *t, int64_t n, int64_t q, const char *fn, unsigned long long *mask, int *list) {
+  if (n > MAX_QTAGS) return kv_fail(KV_ERR_INVALID, "%s: query %lld has %lld tags (at most %d)", fn, (long long)q, (long long)n, MAX_QTAGS);
+  std::vector<int> v(t, t + n);
+  for (int x : v)
+    if (x < 0) return kv_fail(KV_ERR_INVALID, "%s: tag %d of query %lld is negative", fn, x, (long long)q);
+  std::sort(v.begin(), v.end());
+  v.erase(std::unique(v.begin(), v.end()), v.end());
+  *mask = 0;
+  for (int j = 0; j < MAX_QTAGS; j++) list[j] = j < (int)v.size() ? v[(size_t)j] : -1;
+  for (int x : v) *mask |= 1ull << (x & 63);
+  return KV_OK;
+}
+
 // The irregular queries of the resident batch (see classify_queries), in sorted-slot order: their original index and
 // CSR on the host, for the float64 full-scan fallback.
 struct IrregularQueries {
@@ -203,6 +268,11 @@ struct kv_index {
   // caller merges the shards' seed lists group-aware (KV_DISTINCT_MERGED_SEEDS), so the two-phase top-k may run.
   RowSet groups;
   bool distinct = false, merged_seeds = false;
+  // row tag sets (kv_index_set_row_tags) and the tag filter of the resident batch (kv_query_set_tag_filter, cleared by
+  // the next upload); the fallbacks' per-query ineligible rows
+  RowTags tags;
+  QueryTags qtags;
+  DevBuf<uint8_t> d_tagdead;
   // deleted rows (kv_index_delete_rows).  They keep their place in the scan layout.  On the device while any row is
   // deleted, rebuilt by every finalize: by row, the live word of every chunk (by scan position) and the first LAB_FIRST
   // live rows (null queries)
@@ -410,6 +480,9 @@ int kv_index_create(int device, int64_t row_base, kv_index **out) {
   KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<false, false>, smem_limit, (int)scan_smem_bytes(32)));
   KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<true, false>, smem_limit, (int)scan_smem_bytes(0)));
   KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<false, true>, smem_limit, (int)scan_smem_bytes(32, true)));
+  KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<false, false, true>, smem_limit, (int)scan_smem_bytes(32, false, true)));
+  KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<true, false, true>, smem_limit, (int)scan_smem_bytes(0, false, true)));
+  KV_CUDA(cudaFuncSetAttribute(tfidf_scan_kernel<false, true, true>, smem_limit, (int)scan_smem_bytes(32, true, true)));
   KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<true>, smem_limit, 232448));
   KV_CUDA(cudaFuncSetAttribute(tfidf_bound_kernel<false>, smem_limit, 232448));
   KV_CUDA(cudaFuncSetAttribute(jaccard_scan_kernel<false>, smem_limit, (int)jaccard_smem_bytes(32)));
@@ -475,6 +548,7 @@ int kv_index_append(kv_index *ix, const int64_t *indptr, const uint32_t *ids, co
   // again.  Deleted rows stay deleted.
   ix->labels.clear();
   ix->groups.clear();
+  ix->tags.clear();
   ix->tomb.extend(ix->n_rows);
   return KV_OK;
 }
@@ -632,17 +706,79 @@ static int upload_row_set(kv_index *ix, RowSet &rs) {
   return KV_OK;
 }
 
-// the per-row sets a finalize rebuilds on the device: labels and groups
-static int upload_row_sets(kv_index *ix) {
-  const int rc = upload_row_set(ix, ix->labels);
-  return rc != KV_OK ? rc : upload_row_set(ix, ix->groups);
+static const uint32_t *alive_words(const kv_index *ix);
+
+// The device copies of the row tags for the current layout (d_perm, and d_alive when rows are deleted, must hold it):
+// masks and tag lists by scan position, chunk signatures over the live rows.  Nothing until the index is finalized.
+static int upload_row_tags(kv_index *ix) {
+  RowTags &T = ix->tags;
+  T.on_device = false;
+  if (!T.has || !ix->finalized) return KV_OK;
+  const int64_t n = ix->n_rows, n_pos = ix->n_chunks_pad * CHUNK_ROWS;
+  if (n == 0) { T.on_device = true; return KV_OK; }
+  cudaStream_t s = ix->stream;
+  std::vector<int> perm((size_t)n);
+  KV_CUDA(cudaMemcpyAsync(perm.data(), ix->d_perm.p, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, s));
+  KV_CUDA(cudaStreamSynchronize(s));
+  std::vector<unsigned long long> mask((size_t)n_pos, 0ull);
+  std::vector<int64_t> ptr;
+  std::vector<int> list;
+  if (!T.masks_exact) { ptr.assign((size_t)n_pos + 1, 0); list.reserve(T.tags.size()); }
+  for (int64_t p = 0; p < n_pos; p++) {
+    if (p < n) {
+      const int64_t r = perm[(size_t)p];
+      for (int64_t i = T.indptr[(size_t)r]; i < T.indptr[(size_t)r + 1]; i++) {
+        mask[(size_t)p] |= 1ull << (T.tags[(size_t)i] & 63);
+        if (!T.masks_exact) list.push_back(T.tags[(size_t)i]);
+      }
+    }
+    if (!T.masks_exact) ptr[(size_t)p + 1] = (int64_t)list.size();
+  }
+  KV_CUDA(T.d_mask_pos.ensure(n_pos));
+  KV_CUDA(T.d_chunk_sig.ensure(ix->n_chunks_pad));
+  KV_CUDA(cudaMemcpyAsync(T.d_mask_pos.p, mask.data(), mask.size() * 8, cudaMemcpyHostToDevice, s));
+  if (!T.masks_exact) {
+    KV_CUDA(T.d_ptr_pos.ensure(n_pos + 1));
+    KV_CUDA(T.d_list_pos.ensure(std::max<int64_t>((int64_t)list.size(), 1)));
+    KV_CUDA(cudaMemcpyAsync(T.d_ptr_pos.p, ptr.data(), ptr.size() * 8, cudaMemcpyHostToDevice, s));
+    if (!list.empty()) KV_CUDA(cudaMemcpyAsync(T.d_list_pos.p, list.data(), list.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  }
+  chunk_tag_sig_kernel<<<(unsigned)((ix->n_chunks_pad + 255) / 256), 256, 0, s>>>(T.d_mask_pos.p, alive_words(ix), ix->n_chunks_pad,
+                                                                                T.d_chunk_sig.p);
+  KV_CUDA(cudaGetLastError());
+  KV_CUDA(cudaStreamSynchronize(s));  // the host staging vectors go out of scope
+  T.on_device = true;
+  return KV_OK;
 }
 
-// A filtered batch never runs on labels that do not describe the current rows
+// the per-row sets a finalize rebuilds on the device: labels, groups and tags
+static int upload_row_sets(kv_index *ix) {
+  int rc = upload_row_set(ix, ix->labels);
+  if (rc == KV_OK) rc = upload_row_set(ix, ix->groups);
+  return rc != KV_OK ? rc : upload_row_tags(ix);
+}
+
+// A filtered batch never runs on labels or tags that do not describe the current rows
 static int check_filter(const kv_index *ix, const char *fn) {
   if (ix->has_filter && !ix->labels.ready(ix->n_rows))
     return kv_fail(KV_ERR_STATE, "%s: the batch is filtered but the row labels are missing or stale (set them again after an append)", fn);
+  if (ix->qtags.on && !ix->tags.ready(ix->n_rows))
+    return kv_fail(KV_ERR_STATE, "%s: the batch is tag-filtered but the row tags are missing or stale (set them again after an append)", fn);
   return KV_OK;
+}
+
+int kv_index_set_row_tags(kv_index *ix, const int64_t *indptr, const int32_t *tags, int64_t n_rows) {
+  if (!ix) return kv_fail(KV_ERR_INVALID, "kv_index_set_row_tags: NULL handle");
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (!indptr) {
+    ix->tags.clear();
+    return KV_OK;
+  }
+  if (ix->jaccard) return kv_fail(KV_ERR_INVALID, "kv_index_set_row_tags: a Jaccard index (mode 1) has no tag filter");
+  const int rc = ix->tags.set(indptr, tags, n_rows, ix->n_rows, "kv_index_set_row_tags");
+  if (rc != KV_OK) return rc;
+  KV_CUDA(cudaSetDevice(ix->device));
+  return upload_row_tags(ix);
 }
 
 int kv_index_set_row_labels(kv_index *ix, const int32_t *labels, int64_t n) {
@@ -695,6 +831,28 @@ static int upload_dead(kv_index *ix) {
 // NULL while no row is deleted: the kernels' per-row and per-chunk tests are then skipped
 static const uint8_t *dead_rows(const kv_index *ix) { return ix->tomb.any() ? ix->d_dead.p : nullptr; }
 static const uint32_t *alive_words(const kv_index *ix) { return ix->tomb.any() ? ix->d_alive.p : nullptr; }
+
+// The rows a query may not match in the float64 fallbacks (*out, NULL: none): the deleted rows and, when the query has
+// tags (q_mask != 0, d_q_tags its MAX_QTAGS ascending tags on the device), the rows whose tag set misses its own --
+// those are written to d_tagdead, which the launches that follow on the stream read.
+static int fallback_dead(kv_index *ix, unsigned long long q_mask, const int *d_q_tags, const uint8_t **out) {
+  *out = dead_rows(ix);
+  if (q_mask == 0ull || ix->n_rows == 0) return KV_OK;
+  const RowTags &T = ix->tags;
+  KV_CUDA(ix->d_tagdead.ensure(ix->n_rows));
+  tag_dead_kernel<<<(unsigned)((ix->n_rows + 255) / 256), 256, 0, ix->stream>>>(
+      ix->d_invperm.p, ix->n_rows, T.d_mask_pos.p, T.masks_exact ? nullptr : T.d_ptr_pos.p,
+      T.masks_exact ? nullptr : T.d_list_pos.p, q_mask, d_q_tags, dead_rows(ix), ix->d_tagdead.p);
+  KV_CUDA(cudaGetLastError());
+  *out = ix->d_tagdead.p;
+  return KV_OK;
+}
+
+// fallback_dead for query q (original index) of the resident batch
+static int batch_fallback_dead(kv_index *ix, int64_t q, const uint8_t **out) {
+  if (!ix->qtags.on) { *out = dead_rows(ix); return KV_OK; }
+  return fallback_dead(ix, ix->qtags.h_mask[(size_t)q], ix->qtags.d_tags_orig.p + q * MAX_QTAGS, out);
+}
 
 int kv_index_delete_rows(kv_index *ix, const int64_t *rows, int64_t n) {
   if (!ix || n < 0 || (n > 0 && !rows)) return kv_fail(KV_ERR_INVALID, "kv_index_delete_rows: bad arguments");
@@ -1024,6 +1182,7 @@ static void start_batch(kv_index *ix) {
   ix->batch_valid = false;
   drop_range(ix);
   ix->has_excl = ix->has_filter = ix->distinct = ix->merged_seeds = false;
+  ix->qtags.on = false;
   ix->irr.clear();
 }
 
@@ -1482,12 +1641,23 @@ static ScanParams scan_params(const kv_index *ix, const Batch &b) {
   SP.qperm = ix->d_qperm.p; SP.range_out = ix->range.pairs.p; SP.range_count = ix->range.d_count.p;
   SP.range_cap = ix->range.capacity();
   SP.group_pos = b.distinct ? ix->groups.d_pos.p : nullptr;
+  if (ix->qtags.on) {
+    const RowTags &T = ix->tags;
+    SP.q_tmask = ix->qtags.d_mask_sorted.p; SP.q_tags = ix->qtags.d_tags_sorted.p;
+    SP.tag_mask_pos = T.d_mask_pos.p; SP.chunk_tsig = T.d_chunk_sig.p;
+    SP.tag_ptr = T.masks_exact ? nullptr : T.d_ptr_pos.p; SP.tag_list = T.masks_exact ? nullptr : T.d_list_pos.p;
+  }
   return SP;
 }
 
-// K1b-S (distinct or not), or K1b-R for a threshold search, over a grid of candidate lists
+// K1b-S (distinct or not), or K1b-R for a threshold search, over a grid of candidate lists; the tag-filtered
+// instantiations when the batch has a tag filter
 static int launch_scan(kv_index *ix, const Batch &b, const ScanParams &SP, dim3 grid) {
-  if (b.range) tfidf_scan_kernel<true, false><<<grid, S_WARPS * 32, scan_smem_bytes(0), ix->stream>>>(SP);
+  if (ix->qtags.on) {
+    if (b.range) tfidf_scan_kernel<true, false, true><<<grid, S_WARPS * 32, scan_smem_bytes(0, false, true), ix->stream>>>(SP);
+    else if (b.distinct) tfidf_scan_kernel<false, true, true><<<grid, S_WARPS * 32, scan_smem_bytes(b.k, true, true), ix->stream>>>(SP);
+    else tfidf_scan_kernel<false, false, true><<<grid, S_WARPS * 32, scan_smem_bytes(b.k, false, true), ix->stream>>>(SP);
+  } else if (b.range) tfidf_scan_kernel<true, false><<<grid, S_WARPS * 32, scan_smem_bytes(0), ix->stream>>>(SP);
   else if (b.distinct) tfidf_scan_kernel<false, true><<<grid, S_WARPS * 32, scan_smem_bytes(b.k, true), ix->stream>>>(SP);
   else tfidf_scan_kernel<false, false><<<grid, S_WARPS * 32, scan_smem_bytes(b.k), ix->stream>>>(SP);
   KV_CUDA(cudaGetLastError());
@@ -1781,20 +1951,32 @@ static int run_batch(kv_index *ix, int k, float *d_out_s, long long *d_out_r, in
     KV_CUDA(cudaGetLastError());
     b.launches++;
   }
+  if (ix->batch_null && ix->qtags.on) {  // the null queries with tags walk the index for their first eligible rows
+    const RowTags &T = ix->tags;
+    fill_null_tags_kernel<<<(unsigned)((ix->batch_null * 32 + 255) / 256), 256, 0, s>>>(
+        ix->d_qperm.p + n_q, (int)ix->batch_null, k, ix->n_rows, ix->row_base, ix->has_excl ? ix->d_excl_orig.p : nullptr,
+        ix->has_filter ? ix->d_filt_orig.p : nullptr, ix->labels.d_row.p, dead_rows(ix), b.distinct ? ix->groups.d_row.p : nullptr,
+        ix->qtags.d_mask_orig.p, ix->qtags.d_tags_orig.p, ix->d_invperm.p, T.d_mask_pos.p, T.masks_exact ? nullptr : T.d_ptr_pos.p,
+        T.masks_exact ? nullptr : T.d_list_pos.p, d_out_s, d_out_r);
+    KV_CUDA(cudaGetLastError());
+    b.launches++;
+  }
   const IrregularQueries &irr = ix->irr;
   for (size_t i = 0; i < irr.q.size(); i++) {
     const int64_t q = irr.q[i], a = irr.indptr[i], e = irr.indptr[i + 1];
     rc = score_impl(ix, irr.ids.data() + a, irr.tf.data() + a, e - a, irr.oov[i], nullptr);
     if (rc != KV_OK) return rc;
+    const uint8_t *dq = nullptr;
+    if ((rc = batch_fallback_dead(ix, q, &dq)) != KV_OK) return rc;
     if (b.distinct)
       select_topk_distinct_kernel<float><<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
                                                      ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->labels.d_row.p,
-                                                     ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix),
+                                                     ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dq,
                                                      ix->groups.d_row.p, d_out_s + q * k, d_out_r + q * k);
     else
       select_topk_kernel<float><<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k,
                                             ix->has_excl ? (int64_t)ix->h_excl_orig[(size_t)q] : -1, ix->labels.d_row.p,
-                                            ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix), d_out_s + q * k,
+                                            ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dq, d_out_s + q * k,
                                             d_out_r + q * k);
     KV_CUDA(cudaGetLastError());
     b.launches += 2;
@@ -1881,8 +2063,10 @@ static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
           jaccard_select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->d_B64.p, ix->d_invperm.p, ix->n_rows, nq, thr, excl,
                                                            (int)q, ix->jrange.pairs.p, d_count, range_cap());
         } else {
+          const uint8_t *dq = nullptr;
+          if ((rc = batch_fallback_dead(ix, q, &dq)) != KV_OK) return rc;
           select_range_kernel<<<grid, 256, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, thr, excl, ix->labels.d_row.p,
-                                                   ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dead_rows(ix), (int)q, ix->range.pairs.p,
+                                                   ix->has_filter ? ix->h_filt_orig[(size_t)q] : -1, dq, (int)q, ix->range.pairs.p,
                                                    d_count, range_cap());
         }
         KV_CUDA(cudaGetLastError());
@@ -2120,48 +2304,75 @@ int kv_rescore_pairs(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_id
   return KV_OK;
 }
 
-int kv_exact_topk(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
-                  const double *q_oov_tf2, const int32_t *labels, int distinct, int64_t n_q, int k, int64_t *out_rows,
-                  double *out_scores) {
+// kv_exact_topk and kv_exact_topk_tags (tag_indptr NULL: no query has tags; fn names the entry point)
+static int exact_topk_impl(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
+                           const double *q_oov_tf2, const int32_t *labels, const int64_t *tag_indptr, const int32_t *tags,
+                           int distinct, int64_t n_q, int k, int64_t *out_rows, double *out_scores, const char *fn) {
   if (!ix || n_q < 0 || k < 1 || k > 32 || (n_q > 0 && (!q_indptr || !out_rows || !out_scores)))
-    return kv_fail(KV_ERR_INVALID, "kv_exact_topk: bad arguments (k must be 1..32)");
+    return kv_fail(KV_ERR_INVALID, "%s: bad arguments (k must be 1..32)", fn);
   std::lock_guard<std::mutex> g(ix->mu);
-  if (!ix->finalized) return kv_fail(KV_ERR_STATE, "kv_exact_topk: index not finalized");
+  if (tag_indptr && ix->jaccard) return kv_fail(KV_ERR_INVALID, "%s: a Jaccard index (mode 1) has no tag filter", fn);
+  if (!ix->finalized) return kv_fail(KV_ERR_STATE, "%s: index not finalized", fn);
   if (n_q == 0) return KV_OK;
   const int64_t nnz = q_indptr[n_q] - q_indptr[0];
-  if (nnz < 0 || (nnz > 0 && (!q_ids || !q_tf))) return kv_fail(KV_ERR_INVALID, "kv_exact_topk: bad query CSR");
+  if (nnz < 0 || (nnz > 0 && (!q_ids || !q_tf))) return kv_fail(KV_ERR_INVALID, "%s: bad query CSR", fn);
   bool filtered = false;
   for (int64_t q = 0; labels && q < n_q; q++) {
-    if (labels[q] < -1) return kv_fail(KV_ERR_INVALID, "kv_exact_topk: label %d of query %lld is below -1", labels[q], (long long)q);
+    if (labels[q] < -1) return kv_fail(KV_ERR_INVALID, "%s: label %d of query %lld is below -1", fn, labels[q], (long long)q);
     filtered |= labels[q] >= 0;
+  }
+  std::vector<unsigned long long> tmask;
+  std::vector<int> tlist;
+  bool tagged = false;
+  if (tag_indptr) {
+    if (tag_indptr[0] != 0) return kv_fail(KV_ERR_INVALID, "%s: tag indptr must start at 0", fn);
+    tmask.assign((size_t)n_q, 0ull);
+    tlist.assign((size_t)n_q * MAX_QTAGS, -1);
+    for (int64_t q = 0; q < n_q; q++) {
+      const int64_t a = tag_indptr[q], e = tag_indptr[q + 1];
+      if (e < a) return kv_fail(KV_ERR_INVALID, "%s: tag indptr decreases at query %lld", fn, (long long)q);
+      if (e > a && !tags) return kv_fail(KV_ERR_INVALID, "%s: NULL tags", fn);
+      const int rc = parse_query_tags(tags + a, e - a, q, fn, &tmask[(size_t)q], &tlist[(size_t)q * MAX_QTAGS]);
+      if (rc != KV_OK) return rc;
+      tagged |= tmask[(size_t)q] != 0ull;
+    }
   }
   if (ix->n_rows == 0) {
     for (int64_t i = 0; i < n_q * k; i++) { out_rows[i] = -1; out_scores[i] = -INFINITY; }
     return KV_OK;
   }
   if (filtered && !ix->labels.ready(ix->n_rows))
-    return kv_fail(KV_ERR_STATE, "kv_exact_topk: a filtered query needs row labels (kv_index_set_row_labels)");
+    return kv_fail(KV_ERR_STATE, "%s: a filtered query needs row labels (kv_index_set_row_labels)", fn);
   if (distinct && !ix->groups.ready(ix->n_rows))
-    return kv_fail(KV_ERR_STATE, "kv_exact_topk: distinct needs row groups (kv_index_set_row_groups)");
+    return kv_fail(KV_ERR_STATE, "%s: distinct needs row groups (kv_index_set_row_groups)", fn);
+  if (tagged && !ix->tags.ready(ix->n_rows))
+    return kv_fail(KV_ERR_STATE, "%s: a query with tags needs row tags for the current rows (kv_index_set_row_tags)", fn);
   KV_CUDA(cudaSetDevice(ix->device));
   cudaStream_t s = ix->stream;
   std::vector<double> cst;
   std::vector<int64_t> ip;
   int rc = rescore_upload(ix, q_indptr, q_ids, q_tf, q_oov_tf2, n_q, k, cst, ip);
   if (rc != KV_OK) return rc;
+  DevBuf<int> d_tlist;
+  if (tagged) {
+    KV_CUDA(d_tlist.ensure((int64_t)tlist.size()));
+    KV_CUDA(cudaMemcpyAsync(d_tlist.p, tlist.data(), tlist.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  }
   for (int64_t q = 0; q < n_q; q++) {
     // K1a into ix->d_scores, then the best k rows in float64 order into d_rq_rows (global) -- the K1a scores they come
     // with land in d_rq_out, which K6 overwrites below
     const int64_t a = q_indptr[q], e = q_indptr[q + 1];
     if ((rc = score_impl(ix, q_ids + a, q_tf + a, e - a, q_oov_tf2 ? q_oov_tf2[q] : 0.0, nullptr)) != KV_OK) return rc;
     const int lab = labels ? labels[q] : -1;
+    const uint8_t *dq = dead_rows(ix);
+    if (tagged && (rc = fallback_dead(ix, tmask[(size_t)q], d_tlist.p + q * MAX_QTAGS, &dq)) != KV_OK) return rc;
     if (distinct)
       select_topk_distinct_kernel<double><<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k, -1, ix->labels.d_row.p,
-                                                             lab, dead_rows(ix), ix->groups.d_row.p, ix->d_rq_out.p + q * k,
+                                                             lab, dq, ix->groups.d_row.p, ix->d_rq_out.p + q * k,
                                                              ix->d_rq_rows.p + q * k);
     else
       select_topk_kernel<double><<<1, 1024, 0, s>>>(ix->d_scores.p, ix->n_rows, ix->row_base, k, -1, ix->labels.d_row.p, lab,
-                                                    dead_rows(ix), ix->d_rq_out.p + q * k, ix->d_rq_rows.p + q * k);
+                                                    dq, ix->d_rq_out.p + q * k, ix->d_rq_rows.p + q * k);
     KV_CUDA(cudaGetLastError());
   }
   if ((rc = rescore_launch(ix, n_q, k)) != KV_OK) return rc;
@@ -2169,6 +2380,20 @@ int kv_exact_topk(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, 
   KV_CUDA(cudaMemcpyAsync(out_scores, ix->d_rq_out.p, (size_t)n_q * k * 8, cudaMemcpyDeviceToHost, s));
   KV_CUDA(cudaStreamSynchronize(s));
   return KV_OK;
+}
+
+int kv_exact_topk(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
+                  const double *q_oov_tf2, const int32_t *labels, int distinct, int64_t n_q, int k, int64_t *out_rows,
+                  double *out_scores) {
+  return exact_topk_impl(ix, q_indptr, q_ids, q_tf, q_oov_tf2, labels, nullptr, nullptr, distinct, n_q, k, out_rows,
+                         out_scores, "kv_exact_topk");
+}
+
+int kv_exact_topk_tags(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
+                       const double *q_oov_tf2, const int32_t *labels, const int64_t *tag_indptr, const int32_t *tags,
+                       int distinct, int64_t n_q, int k, int64_t *out_rows, double *out_scores) {
+  return exact_topk_impl(ix, q_indptr, q_ids, q_tf, q_oov_tf2, labels, tag_indptr, tags, distinct, n_q, k, out_rows,
+                         out_scores, "kv_exact_topk_tags");
 }
 
 static int set_exclusions_locked(kv_index *ix, const int64_t *exclude_rows, int64_t n_q) {
@@ -2219,6 +2444,53 @@ int kv_query_set_filter(kv_index *ix, const int32_t *labels, int64_t n_q) {
   KV_CUDA(cudaMemcpyAsync(ix->d_filt_orig.p, ix->h_filt_orig.data(), (size_t)n_q * sizeof(int), cudaMemcpyHostToDevice, ix->stream));
   KV_CUDA(cudaStreamSynchronize(ix->stream));
   ix->has_filter = true;
+  return KV_OK;
+}
+
+int kv_query_set_tag_filter(kv_index *ix, const int64_t *indptr, const int32_t *tags, int64_t n_q) {
+  const char *fn = "kv_query_set_tag_filter";
+  if (!ix) return kv_fail(KV_ERR_INVALID, "%s: NULL handle", fn);
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (indptr && ix->jaccard) return kv_fail(KV_ERR_INVALID, "%s: a Jaccard index (mode 1) has no tag filter", fn);
+  if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "%s: no query batch uploaded", fn);
+  if (!indptr) { ix->qtags.on = false; return KV_OK; }
+  if (n_q != ix->batch_q)
+    return kv_fail(KV_ERR_INVALID, "%s: %lld tag sets for a batch of %lld queries", fn, (long long)n_q, (long long)ix->batch_q);
+  if (indptr[0] != 0) return kv_fail(KV_ERR_INVALID, "%s: indptr must start at 0", fn);
+  std::vector<unsigned long long> mask((size_t)n_q, 0ull);
+  std::vector<int> list((size_t)n_q * MAX_QTAGS, -1);
+  bool any = false;
+  for (int64_t q = 0; q < n_q; q++) {
+    const int64_t a = indptr[q], e = indptr[q + 1];
+    if (e < a) return kv_fail(KV_ERR_INVALID, "%s: indptr decreases at query %lld", fn, (long long)q);
+    if (e > a && !tags) return kv_fail(KV_ERR_INVALID, "%s: NULL tags", fn);
+    const int rc = parse_query_tags(tags + a, e - a, q, fn, &mask[(size_t)q], &list[(size_t)q * MAX_QTAGS]);
+    if (rc != KV_OK) return rc;
+    any = any || mask[(size_t)q] != 0ull;
+  }
+  QueryTags &Q = ix->qtags;
+  Q.on = false;
+  if (!any) return KV_OK;  // no query has tags: the batch without a tag filter
+  if (!ix->tags.ready(ix->n_rows))
+    return kv_fail(KV_ERR_STATE, "%s: the index has no row tags for its current rows (kv_index_set_row_tags)", fn);
+  KV_CUDA(cudaSetDevice(ix->device));
+  std::vector<unsigned long long> mask_sorted((size_t)n_q);
+  std::vector<int> list_sorted((size_t)n_q * MAX_QTAGS);
+  for (int64_t i = 0; i < n_q; i++) {
+    const int64_t q = ix->h_qperm.p[i];
+    mask_sorted[(size_t)i] = mask[(size_t)q];
+    std::copy_n(list.begin() + q * MAX_QTAGS, MAX_QTAGS, list_sorted.begin() + i * MAX_QTAGS);
+  }
+  KV_CUDA(Q.d_mask_orig.ensure(n_q)); KV_CUDA(Q.d_mask_sorted.ensure(n_q));
+  KV_CUDA(Q.d_tags_orig.ensure(n_q * MAX_QTAGS)); KV_CUDA(Q.d_tags_sorted.ensure(n_q * MAX_QTAGS));
+  cudaStream_t s = ix->stream;
+  KV_CUDA(cudaMemcpyAsync(Q.d_mask_orig.p, mask.data(), mask.size() * 8, cudaMemcpyHostToDevice, s));
+  KV_CUDA(cudaMemcpyAsync(Q.d_mask_sorted.p, mask_sorted.data(), mask_sorted.size() * 8, cudaMemcpyHostToDevice, s));
+  KV_CUDA(cudaMemcpyAsync(Q.d_tags_orig.p, list.data(), list.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  KV_CUDA(cudaMemcpyAsync(Q.d_tags_sorted.p, list_sorted.data(), list_sorted.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  KV_CUDA(cudaStreamSynchronize(s));
+  Q.h_mask = std::move(mask);
+  Q.on = true;
   return KV_OK;
 }
 
@@ -2648,7 +2920,7 @@ extern "C" int kv_index_layout_load(kv_index *ix, const char *path) {
   int rc = upload_layout(ix, SL);
   if (rc != KV_OK) return rc;
   ix->finalized = false;
-  ix->labels.on_device = ix->groups.on_device = false;  // positions changed: the finalize that follows rebuilds them
+  ix->labels.on_device = ix->groups.on_device = ix->tags.on_device = false;  // positions changed: the finalize that follows rebuilds them
   return KV_OK;
 }
 

@@ -226,6 +226,52 @@ __global__ void chunk_sig_kernel(const int *__restrict__ label_pos, int64_t n_ch
   sig[c] = m;
 }
 
+// ---- tag sets (kv_index_set_row_tags / kv_query_set_tag_filter) ----
+// A row carries a set of tags >= 0, a query at most MAX_QTAGS of them; the query matches the rows whose set meets its
+// own.  Both sides also carry a 64-bit mask, OR of 1 << (t & 63): a row whose mask misses the query's holds none of its
+// tags, and when every tag of the index is < 64 a mask hit is the exact answer.  Otherwise the row's tags (by scan
+// position, CSR tag_ptr / tag_list) are compared with the query's ascending list, -1 past its last tag.
+constexpr int MAX_QTAGS = 16;
+
+__device__ __forceinline__ bool tags_meet(unsigned long long row_mask, unsigned long long q_mask, const int64_t *__restrict__ tag_ptr,
+                                          const int *__restrict__ tag_list, int64_t pos, const int *__restrict__ q_tags) {
+  if ((row_mask & q_mask) == 0ull) return false;
+  if (!tag_ptr) return true;  // every tag < 64: the masks are the sets
+  for (int64_t i = tag_ptr[pos], e = tag_ptr[pos + 1]; i < e; i++) {
+    const int t = tag_list[i];
+    if (!((q_mask >> (t & 63)) & 1ull)) continue;
+    for (int j = 0; j < MAX_QTAGS; j++) {
+      const int u = q_tags[j];
+      if (u < 0 || u > t) break;
+      if (u == t) return true;
+    }
+  }
+  return false;
+}
+
+// chunk tag signature: OR of the masks of the chunk's live rows (alive NULL: every row is live)
+__global__ void chunk_tag_sig_kernel(const unsigned long long *__restrict__ mask_pos, const uint32_t *__restrict__ alive,
+                                     int64_t n_chunks_pad, unsigned long long *sig) {
+  const int64_t c = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (c >= n_chunks_pad) return;
+  const uint32_t live = alive ? alive[c] : FULL;
+  unsigned long long m = 0;
+  for (int i = 0; i < CHUNK_ROWS; i++)
+    if ((live >> i) & 1u) m |= mask_pos[c * CHUNK_ROWS + i];
+  sig[c] = m;
+}
+
+// The rows one tag-filtered query may not match, for the float64 fallbacks: out[row] = 1 when the row is deleted
+// (dead, NULL: none) or its tag set misses the query's (q_mask, q_tags)
+__global__ void tag_dead_kernel(const int *__restrict__ invperm, int64_t n_rows, const unsigned long long *__restrict__ mask_pos,
+                                const int64_t *__restrict__ tag_ptr, const int *__restrict__ tag_list, unsigned long long q_mask,
+                                const int *__restrict__ q_tags, const uint8_t *__restrict__ dead, uint8_t *out) {
+  const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (r >= n_rows) return;
+  const int64_t pos = invperm[r];
+  out[r] = (dead && dead[r]) || !tags_meet(mask_pos[pos], q_mask, tag_ptr, tag_list, pos, q_tags);
+}
+
 // ----------------------------------------------------------------------------------------
 // device helpers
 // ----------------------------------------------------------------------------------------
@@ -595,6 +641,9 @@ __host__ __device__ __forceinline__ uint32_t rt_slot2(uint32_t fid, uint32_t siz
 // stream in behind the scoring instead of in a separate selection pass that writes the lists to memory.
 // K1b-R (RANGE = true) is the same scan for a threshold search: the filter is the query's fixed threshold and every
 // row that reaches it is appended to a global pair buffer instead of a top-k list.
+// TAGS: the batch has a tag filter.  A record drops the filtered queries whose tags no live row of the chunk carries
+// (chunk signature), a (query, record) pair is skipped when no row's mask meets the query's, and a row enters only
+// when its set meets the query's (tags_meet).  The instantiations without it compile as before.
 // ----------------------------------------------------------------------------------------
 struct ScanParams {
   const uint32_t *blk;
@@ -645,6 +694,15 @@ struct ScanParams {
   unsigned long long range_cap;
   // distinct top-k (tfidf_scan_kernel<false, true>, kv_query_set_distinct): row group by scan position
   const int *group_pos;              // [n_chunks_pad * 32], -1 past the last row
+  // tag filter (tfidf_scan_kernel<..., true>, kv_query_set_tag_filter), see tags_meet.  By sorted slot: the query's
+  // mask (0: no tag constraint) and ascending tags; by scan position: the row masks and, unless every tag is < 64
+  // (tag_ptr NULL), the rows' tags; per chunk the OR of its live rows' masks
+  const unsigned long long *q_tmask;     // [n_q]
+  const int *q_tags;                     // [n_q][MAX_QTAGS]
+  const unsigned long long *tag_mask_pos;  // [n_chunks_pad * 32], 0 past the last row
+  const unsigned long long *chunk_tsig;  // [n_chunks_pad]
+  const int64_t *tag_ptr;                // [n_chunks_pad * 32 + 1]
+  const int *tag_list;
 };
 
 // Appends the pairs (*q, score, row) of the lanes with `hit` set: one reservation per warp
@@ -701,7 +759,7 @@ __device__ __forceinline__ void bulk_copy_g2s(void *dst, const void *src, uint32
 // found by a ballot and either kept (the new row is worse) or deleted before the new row is inserted.  A full list
 // then holds k distinct groups, so its k-th score stays a lower bound of the k-th group score: the threshold, the
 // codes snapshot and the bound passes are unchanged.
-template <bool RANGE, bool DISTINCT>
+template <bool RANGE, bool DISTINCT, bool TAGS = false>
 __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams P) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int k = P.k;
@@ -721,6 +779,9 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   unsigned int *s_next = (unsigned int *)(s_qlab + GROUP_Q);                // [1] next record of this CTA's range
   unsigned int *s_stat = s_next + 1;                                        // [4]
   int *s_lgrp = (int *)(s_stat + 4);                                        // [GROUP_Q][k] (DISTINCT only)
+  unsigned long long *s_qtm = nullptr;                                      // [GROUP_Q] tag masks (TAGS only)
+  if constexpr (TAGS)
+    s_qtm = (unsigned long long *)(((uintptr_t)(s_lgrp + (DISTINCT ? GROUP_Q * k : 0)) + 7) & ~(uintptr_t)7);
 
   const int list = blockIdx.x, ssplit = blockIdx.y;
   const int group = list / P.n_bsplits, bsplit = list - group * P.n_bsplits;
@@ -770,6 +831,7 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
       s_uc[qi] = ok ? P.q_uc[q0 + qi] : 0ull;
       s_excl[qi] = (ok && P.q_excl) ? P.q_excl[q0 + qi] : -1;
       s_qlab[qi] = (ok && P.q_label) ? P.q_label[q0 + qi] : -1;
+      if constexpr (TAGS) s_qtm[qi] = ok ? P.q_tmask[q0 + qi] : 0ull;
     }
     if (threadIdx.x == 0) { *s_next = r_lo; s_stat[0] = s_stat[1] = s_stat[2] = s_stat[3] = 0; }
     if (lane == 0) {
@@ -809,6 +871,10 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
       const unsigned long long sig = P.chunk_sig[chunk];
       const int lb = s_qlab[lane];
       mask &= __ballot_sync(FULL, lb < 0 || ((sig >> (lb & 63)) & 1ull));
+    }
+    if constexpr (TAGS) {  // the same for the tag-filtered queries
+      const unsigned long long qm = s_qtm[lane];
+      mask &= __ballot_sync(FULL, qm == 0ull || (P.chunk_tsig[chunk] & qm) != 0ull);
     }
     if (P.alive && P.alive[chunk] == 0u) mask = 0;  // every row of the chunk deleted: never staged
   };
@@ -900,6 +966,20 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
             if (lane == j) wm[i] = m;
           }
       }
+      if constexpr (TAGS) {  // lane = query: its tag mask against each chunk's signature (one broadcast load each)
+        const unsigned long long qm = s_qtm[lane];
+        if (__any_sync(FULL, qm != 0ull)) {
+          for (int i = 0; i < S_WIN / 32; i++) {
+            uint32_t keep = 0;  // lane j: the queries chunk wbase + 32 i + j keeps
+            for (int j = 0; j < 32; j++) {
+              const uint32_t m = __ballot_sync(FULL, qm == 0ull || (P.chunk_tsig[wbase + 32 * i + j] & qm) != 0ull);
+              if (lane == j) keep = m;
+            }
+            if (i == 0) wm[0] &= keep;
+            else wm[1] &= keep;
+          }
+        }
+      }
       pend = 0;
       unsigned int sel_pairs = 0, sel_recs = 0;
 #pragma unroll
@@ -977,6 +1057,10 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
         if (!(nq > 0.f)) continue;  // null / irregular query: answered elsewhere
         const int ql = s_qlab[qi];
         if (ql >= 0 && __ballot_sync(FULL, lpos == ql) == 0) continue;  // signature collision: no row of the label here
+        if constexpr (TAGS) {  // the row masks are read again (L1) where needed rather than held across the probe loop
+          const unsigned long long qtm = s_qtm[qi];
+          if (qtm && __ballot_sync(FULL, (P.tag_mask_pos[pos0 + lane] & qtm) != 0ull) == 0) continue;  // no row's mask meets the query's
+        }
         pairs_done++;
         const uint32_t *keys = s_keys + qi * QKEYS;
         const QFeat *feats = s_feats + qi * QFEATS;
@@ -1067,6 +1151,11 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
             sc = den > 0.f ? __fdiv_rn(dot, __fsqrt_rn(den)) : 0.f;
             row = P.perm[pos0 + lane];
             cand = row != s_excl[qi] && sc >= filt && (sc > ks || row < kr) && (ql < 0 || lpos == ql) && live;
+            if constexpr (TAGS) {
+              const unsigned long long qtm = s_qtm[qi];
+              if (cand && qtm)
+                cand = tags_meet(P.tag_mask_pos[pos0 + lane], qtm, P.tag_ptr, P.tag_list, pos0 + lane, P.q_tags + (q0 + qi) * MAX_QTAGS);
+            }
           }
         }
         if constexpr (RANGE) {
@@ -1196,9 +1285,10 @@ __global__ void __launch_bounds__(S_WARPS * 32, 2) tfidf_scan_kernel(ScanParams 
   }
 }
 
-static inline size_t scan_smem_bytes(int k, bool distinct = false) {
+static inline size_t scan_smem_bytes(int k, bool distinct = false, bool tags = false) {
   return (size_t)GROUP_Q * QTAB_BYTES + (size_t)S_WARPS * 2 * S_BUF_BYTES + (size_t)S_WARPS * 2 * 8 + (size_t)GROUP_Q * 8 * 3 +
-         (size_t)GROUP_Q * k * 8 + (size_t)GROUP_Q * 4 * 5 + 32 + (distinct ? (size_t)GROUP_Q * k * 4 : 0);
+         (size_t)GROUP_Q * k * 8 + (size_t)GROUP_Q * 4 * 5 + 32 + (distinct ? (size_t)GROUP_Q * k * 4 : 0) +
+         (tags ? (size_t)GROUP_Q * 8 + 8 : 0);
 }
 
 // ----------------------------------------------------------------------------------------
@@ -1817,6 +1907,58 @@ __global__ void fill_null_distinct_kernel(const int *__restrict__ null_q, int n_
     for (int t = 0; t < n; t++) fresh &= __shfl_sync(FULL, tg, t) != g;
     const uint32_t peers = __match_any_sync(FULL, g);
     fresh = fresh && __ffs(peers) - 1 == lane;  // the lowest row of its group among these 32
+    for (uint32_t fm = __ballot_sync(FULL, fresh); fm && n < k; fm &= fm - 1, n++) {
+      const int j = __ffs(fm) - 1;
+      const int gj = __shfl_sync(FULL, g, j);
+      if (lane == n) {
+        tg = gj;
+        out_s[(size_t)q * k + n] = 0.f;
+        out_r[(size_t)q * k + n] = row_base + r0 + j;
+      }
+    }
+  }
+  if (lane >= n && lane < k) {
+    out_s[(size_t)q * k + lane] = -INFINITY;
+    out_r[(size_t)q * k + lane] = -1LL;
+  }
+}
+
+// The null queries of a tag-filtered batch whose own tag set is not empty (the others keep what fill_null_kernel or
+// fill_null_distinct_kernel wrote): one warp per query walks the rows in ascending order and keeps the first k it may
+// match -- not excluded, of its label when filtered, live, tag set meeting the query's (q_tmask / q_tags by ORIGINAL
+// query, rows through invperm to their scan position) -- and in distinct mode (groups by local row, NULL: not
+// distinct) only the first row of each new group.  A query with fewer than k such rows walks the whole index.
+__global__ void fill_null_tags_kernel(const int *__restrict__ null_q, int n_null, int k, int64_t n_rows, int64_t row_base,
+                                      const int *__restrict__ excl_by_query, const int *__restrict__ label_by_query,
+                                      const int *__restrict__ labels, const uint8_t *__restrict__ dead,
+                                      const int *__restrict__ groups, const unsigned long long *__restrict__ q_tmask,
+                                      const int *__restrict__ q_tags, const int *__restrict__ invperm,
+                                      const unsigned long long *__restrict__ mask_pos, const int64_t *__restrict__ tag_ptr,
+                                      const int *__restrict__ tag_list, float *out_s, long long *out_r) {
+  const int w = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (w >= n_null) return;
+  const int q = null_q[w];
+  const unsigned long long qm = q_tmask[q];
+  if (qm == 0ull) return;
+  const int *qt = q_tags + (size_t)q * MAX_QTAGS;
+  const int ex = excl_by_query ? excl_by_query[q] : -1;
+  const int lb = label_by_query ? label_by_query[q] : -1;
+  int tg = -1;  // lane t: group of the t-th row taken
+  int n = 0;
+  for (int64_t r0 = 0; r0 < n_rows && n < k; r0 += 32) {
+    const int64_t r = r0 + lane;
+    bool elig = r < n_rows && r != ex && (lb < 0 || labels[r] == lb) && !(dead && dead[r]);
+    if (elig) {
+      const int64_t pos = invperm[r];
+      elig = tags_meet(mask_pos[pos], qm, tag_ptr, tag_list, pos, qt);
+    }
+    const int g = elig ? (groups ? groups[r] : (int)r) : -1 - lane;
+    bool fresh = elig;
+    if (groups) {
+      for (int t = 0; t < n; t++) fresh &= __shfl_sync(FULL, tg, t) != g;
+      const uint32_t peers = __match_any_sync(FULL, g);
+      fresh = fresh && __ffs(peers) - 1 == lane;  // the lowest row of its group among these 32
+    }
     for (uint32_t fm = __ballot_sync(FULL, fresh); fm && n < k; fm &= fm - 1, n++) {
       const int j = __ffs(fm) - 1;
       const int gj = __shfl_sync(FULL, g, j);

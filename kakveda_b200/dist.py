@@ -33,7 +33,8 @@ import numpy as np
 from . import _capi, _devout
 from ._capi import no_distinct
 from .gfkb import MATCH_LIMIT
-from .similarity import FeatureBatch, GfkbIndex, Vocabulary, _featurize_on_device, gather_rows, pack_texts, text_order
+from .similarity import (MAX_QUERY_TAGS, FeatureBatch, GfkbIndex, Vocabulary, _featurize_on_device, csr_rows, gather_rows,
+                         pack_texts, tag_csr, text_order)
 from .store import MAX_LIMIT, GfkbStore, ambiguous_candidates
 
 
@@ -319,6 +320,7 @@ class ShardedGfkb:
         self.n_global = 0
         self._corpus = None   # (data, offsets, mode) of the corpus text: the queries of selfjoin_range
         self._has_labels = self._has_groups = False   # set_row_labels / set_row_groups
+        self._has_tags = False                          # set_row_tags
         self._groups_dev = None   # rows mode on several GPUs: the group of every global row, for the distinct merges
         self._groups_host = None  # set_row_groups: the group of every global row, for the merge of exact_topk
         self._deleted = None      # delete_rows: bool per global row (every rank deletes the same rows)
@@ -399,9 +401,24 @@ class ShardedGfkb:
         self.index.upload_queries(qfb)
         self._exchange_thresholds(qfb.n)
 
-    def _set_modes(self, q: int, labels: Optional[np.ndarray], distinct: bool) -> None:
-        """The filter and distinct mode of the resident batch of ``q`` queries, the same on every rank (the threshold
+    def _check_tags(self, tags, q: int):
+        """``tags=`` of a batch of ``q`` queries as CSR, checked before anything is sent (every rank raises the same
+        error); None stays None."""
+        if tags is None:
+            return None
+        ip, t = tag_csr(tags, q, "tags")
+        if len(t) and t.min() < 0:
+            raise ValueError("tags: a negative tag")
+        if q and np.diff(ip).max() > MAX_QUERY_TAGS:
+            raise ValueError(f"tags: a query with more than {MAX_QUERY_TAGS} tags")
+        if not self._has_tags:
+            raise ValueError("tags: the sharded index has no row tags (set_row_tags)")
+        return ip, t
+
+    def _set_modes(self, q: int, labels: Optional[np.ndarray], distinct: bool, tags=None) -> None:
+        """The filters and distinct mode of the resident batch of ``q`` queries, the same on every rank (the threshold
         exchange relies on it).  The arguments are checked before anything is sent, so every rank raises the same error."""
+        tags = self._check_tags(tags, q)
         if labels is not None:
             labels = np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
             if len(labels) != q:
@@ -415,6 +432,7 @@ class ShardedGfkb:
         lo, hi = self._qslice if self.mode == "queries" and self.world > 1 else (0, q)
         if hi > lo:
             self.index.set_filter(None if labels is None else labels[lo:hi])
+            self.index.set_tag_filter(None if tags is None else csr_rows(*tags, np.arange(lo, hi)))
             # rows mode on several GPUs runs the two-phase top-k, whose seed lists topk_resident merges group-aware
             self.index.set_distinct(distinct, merged_seeds=self.mode == "rows" and self.world > 1)
 
@@ -425,15 +443,16 @@ class ShardedGfkb:
         if self.row_map is not None:
             r.copy_(torch.where(r >= 0, self.row_map[r.clamp(min=0)], r))
 
-    def topk_resident(self, k: int, labels: Optional[np.ndarray] = None, distinct: bool = False):
+    def topk_resident(self, k: int, labels: Optional[np.ndarray] = None, distinct: bool = False, tags=None):
         """Device-only step on the uploaded batch: local scan+merge, all-gather, global merge.  ``labels``: per query
         the row label its results must carry (-1: any row; ``set_row_labels``).  ``distinct``: at most one row per group
-        (``set_row_groups``), as ``GfkbIndex.topk_features``.  Both combine."""
+        (``set_row_groups``), as ``GfkbIndex.topk_features``.  ``tags``: per query a tag set its results' rows must
+        meet (``set_row_tags``; each shard filters its own rows, the exchanges are unchanged).  All combine."""
         import torch
 
         q = self._resident_q
         dev = f"cuda:{self.device}"
-        self._set_modes(q, labels, distinct)
+        self._set_modes(q, labels, distinct, tags)
         if self.mode == "queries" and self.world > 1:
             import torch.distributed as dist
 
@@ -609,10 +628,10 @@ class ShardedGfkb:
         return hs.numpy(), hr.numpy()
 
     def topk_packed(self, data, offsets: np.ndarray, k: int, mode: int = 0, labels: Optional[np.ndarray] = None,
-                    distinct: bool = False):
+                    distinct: bool = False, tags=None):
         """End-to-end step from host text: featurise, upload, scan, exchange, merge, read back.  ``last_e2e_ms`` keeps
         the wall-clock split of the last call (featurise / upload incl. table kernels / device step / read-back).
-        ``labels`` / ``distinct`` as for ``topk_resident``."""
+        ``labels`` / ``distinct`` / ``tags`` as for ``topk_resident``."""
         import time
 
         t0 = time.perf_counter()
@@ -621,7 +640,7 @@ class ShardedGfkb:
 
             self.upload_text_sharded(data, offsets, mode)
             t2 = time.perf_counter()
-            s, r = self.topk_resident(k, labels, distinct)
+            s, r = self.topk_resident(k, labels, distinct, tags)
             torch.cuda.current_stream().synchronize()
             t3 = time.perf_counter()
             out = self._read_back(s, r)
@@ -636,7 +655,7 @@ class ShardedGfkb:
             self.index.upload_text(data, offsets, mode)   # featurise, classify and order on the device
             self._resident_q = n_q
             t2 = time.perf_counter()
-            s, r = self.topk_resident(k, labels, distinct)
+            s, r = self.topk_resident(k, labels, distinct, tags)
             torch.cuda.current_stream().synchronize()
             t3 = time.perf_counter()
             out = self._read_back(s, r)
@@ -650,7 +669,7 @@ class ShardedGfkb:
             t1 = time.perf_counter()
             self.set_resident(qfb)
             t2 = time.perf_counter()
-            s, r = self.topk_resident(k, labels, distinct)
+            s, r = self.topk_resident(k, labels, distinct, tags)
             import torch
 
             torch.cuda.current_stream().synchronize()
@@ -699,6 +718,24 @@ class ShardedGfkb:
             raise ValueError(f"set_row_labels: {len(lab)} labels for a corpus of {self.n_global} rows")
         self.index.set_row_labels(self._local_part(lab))
         self._has_labels = True
+
+    def set_row_tags(self, global_sets) -> None:
+        """A tag set per GLOBAL row (a list of lists or an ``(indptr, tags)`` pair, as ``GfkbIndex.set_row_tags``): this
+        shard keeps its rows' sets as ``set_row_labels`` keeps labels, for ``tags=`` of the top-k, exact top-k and
+        threshold searches.  ``None`` clears."""
+        if global_sets is None:
+            self.index.set_row_tags(None)
+            self._has_tags = False
+            return
+        ip, t = tag_csr(global_sets, self.n_global, "set_row_tags")
+        if self.row_map is not None:
+            sel = self._row_map_host
+        elif self.mode == "rows":
+            sel = np.arange(*shard_bounds(self.n_global, self.world, self.rank))
+        else:
+            sel = np.arange(self.n_global)
+        self.index.set_row_tags(csr_rows(ip, t, sel))
+        self._has_tags = True
 
     def set_row_groups(self, global_groups: Optional[np.ndarray]) -> None:
         """One group >= 0 per GLOBAL row (e.g. one id per distinct text), for ``distinct=True`` of the top-k: this shard
@@ -818,13 +855,13 @@ class ShardedGfkb:
 
     # ---- exact top-k -------------------------------------------------------------------------------------------------
     def exact_topk(self, qfb: FeatureBatch, k: int, labels: Optional[np.ndarray] = None,
-                   distinct: bool = False) -> Tuple[np.ndarray, np.ndarray]:
+                   distinct: bool = False, tags=None) -> Tuple[np.ndarray, np.ndarray]:
         """Every query's best ``k`` rows over the whole sharded corpus with no candidate stage: ``(rows int64 [Q,k],
         scores float64 [Q,k])``, global rows ordered by (score desc, row asc), (-1, -inf) past the last; identical on
         every rank.  Each shard runs ``GfkbIndex.exact_topk`` (K1a over its rows, selection on the device, K6 scores:
         only k rows per query leave the device); in rows mode on several GPUs ONE all-gather carries the shards' lists
-        and every rank merges them.  ``labels`` / ``distinct`` as for ``topk_resident``; a distinct merge keeps the
-        first row of each group.  A collective; bad arguments raise ValueError on every rank before it starts."""
+        and every rank merges them.  ``labels`` / ``distinct`` / ``tags`` as for ``topk_resident``; a distinct merge keeps
+        the first row of each group.  A collective; bad arguments raise ValueError on every rank before it starts."""
         import torch
 
         q = qfb.n
@@ -840,7 +877,8 @@ class ShardedGfkb:
                 raise ValueError("labels: the sharded index has no row labels (set_row_labels)")
         if distinct and not self._has_groups:
             raise ValueError("distinct: the sharded index has no row groups (set_row_groups)")
-        rows, scores = self.index.exact_topk(qfb, k, labels, distinct)
+        tags = self._check_tags(tags, q)
+        rows, scores = self.index.exact_topk(qfb, k, labels, distinct, tags)
         if self.row_map is not None:   # text-range shard: local -> global rows (ascending, so ties keep their order)
             rows = np.where(rows >= 0, self._row_map_host[np.clip(rows, 0, None)], -1)
         if self.world == 1 or self.mode != "rows":
@@ -876,16 +914,20 @@ class ShardedGfkb:
     def _empty_range(self, device_out: bool):
         return self.index._empty_range(device_out)
 
-    def range_resident(self, threshold: float, device_out: bool = False, labels: Optional[np.ndarray] = None):
+    def range_resident(self, threshold: float, device_out: bool = False, labels: Optional[np.ndarray] = None, tags=None):
         """Threshold search of the resident batch over the whole sharded corpus: ``(indptr int64[n_q+1], rows int64[P],
         scores float32[P])`` as ``GfkbIndex.range`` returns them (global rows, each query's pairs by (score desc, row
         asc)), NumPy arrays or with ``device_out`` torch tensors on this rank's device; identical on every rank.
-        ``labels``: per query the row label its pairs must carry (-1: any row; ``set_row_labels``).  Every shard
-        searches its rows alone (the threshold is fixed); one all-gather of the results and the device merge follow."""
+        ``labels``: per query the row label its pairs must carry (-1: any row; ``set_row_labels``).  ``tags``: per query
+        a tag set its pairs' rows must meet (``set_row_tags``).  Every shard searches its rows alone (the threshold is
+        fixed); one all-gather of the results and the device merge follow."""
         q = self._resident_q
         lo, hi = self._qslice if self.mode == "queries" and self.world > 1 else (0, q)
+        tags = self._check_tags(tags, q)
         if labels is not None and hi > lo:
             self.index.set_filter(np.ascontiguousarray(labels, dtype=np.int32)[lo:hi])
+        if tags is not None and hi > lo:
+            self.index.set_tag_filter(csr_rows(*tags, np.arange(lo, hi)))
         if self.world == 1:
             return self.index._range_resident(q, threshold, device_out)
         n = self.index._range_search(threshold) if hi > lo else 0
@@ -906,7 +948,7 @@ class ShardedGfkb:
         return _host(merge_range_on_device(self.device, gathered, q, pairs), device_out)
 
     def range_packed(self, data, offsets: np.ndarray, threshold: float, mode: int = 0, labels: Optional[np.ndarray] = None,
-                     device_out: bool = False):
+                     device_out: bool = False, tags=None):
         """``range_resident`` of a batch of host text (packed as for ``topk_packed``).  Rows mode on several GPUs
         prepares the batch with ``upload_text_sharded``."""
         offsets = np.ascontiguousarray(offsets, dtype=np.int64)
@@ -920,7 +962,7 @@ class ShardedGfkb:
                 self._set_resident_range(qfb)
             finally:
                 qfb.close()
-        return self.range_resident(threshold, device_out, labels)
+        return self.range_resident(threshold, device_out, labels, tags)
 
     def selfjoin_range(self, threshold: float, device_out: bool = False, block: int = 262144):
         """All-pairs threshold search over the whole sharded corpus: for every global row every OTHER row scoring
@@ -1248,7 +1290,7 @@ class ShardedGfkbStore(GfkbStore):
             tail.set_row_groups(groups[self._n_main:self._n_main + tail.n_rows])
 
     def _candidates(self, fb: FeatureBatch, k: int, limit: int = MATCH_LIMIT, labels: Optional[np.ndarray] = None,
-                    distinct: bool = False):
+                    distinct: bool = False, tags=None):
         import torch
         import torch.distributed as dist
 
@@ -1259,7 +1301,7 @@ class ShardedGfkbStore(GfkbStore):
             self._ensure_groups()
         main = self._main
         main.set_resident(fb)
-        s, r = main.topk_resident(kk, labels=labels, distinct=distinct)
+        s, r = main.topk_resident(kk, labels=labels, distinct=distinct, tags=tags)
         s32, rows = s.cpu().numpy(), r.cpu().numpy()
         amb = ambiguous_candidates(s32, rows, limit)
         f64 = main.index.rescore(fb, rows)   # -inf for the rows of the other shards
@@ -1269,21 +1311,22 @@ class ShardedGfkbStore(GfkbStore):
             f64 = t.cpu().numpy()
         rows_all, f64_all = [rows], [f64]
         if self._tail is not None and self._tail.n_rows:
-            s32, rows = self._segment_topk(self._tail, fb, kk, labels, distinct)
+            s32, rows = self._segment_topk(self._tail, fb, kk, labels, distinct, tags)
             amb |= ambiguous_candidates(s32, rows, limit)
             rows_all.append(rows)
             f64_all.append(self._tail.rescore(fb, rows))
         return self._merge_candidates(rows_all, f64_all, distinct) + (amb,)
 
-    def _exact_top(self, signature_text: str, limit: int, label: int = -1, distinct: bool = False):
+    def _exact_top(self, signature_text: str, limit: int, label: int = -1, distinct: bool = False, app: int = -1):
         if distinct:
             self._ensure_groups()
         lab = None if label < 0 else np.array([label], dtype=np.int32)
+        tags = None if app < 0 else [[app]]
         fb = self.vocab.featurize([signature_text], grow=False)
         try:
-            parts = [self._main.exact_topk(fb, limit, lab, distinct)]
+            parts = [self._main.exact_topk(fb, limit, lab, distinct, tags)]
             if self._tail is not None and self._tail.n_rows:
-                parts.append(self._tail.exact_topk(fb, limit, lab, distinct))
+                parts.append(self._tail.exact_topk(fb, limit, lab, distinct, tags))
         finally:
             fb.close()
         groups = self._dev_groups(self._n_dev) if distinct else None

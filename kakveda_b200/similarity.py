@@ -69,6 +69,43 @@ def pack_texts(texts: Sequence[str]) -> Tuple[bytes, np.ndarray, int]:
     return b"".join(parts), offsets, _capi.KV_TEXT_MIXED
 
 
+MAX_QUERY_TAGS = 16  # tags a query's tag filter may hold
+
+
+def is_csr_pair(sets) -> bool:
+    """Whether ``sets`` is given in CSR form: a tuple of exactly two NumPy arrays ``(indptr, tags)``.  Any other
+    sequence (a list or tuple of lists, ...) holds one iterable of tags per entry."""
+    return isinstance(sets, tuple) and len(sets) == 2 and all(isinstance(x, np.ndarray) for x in sets)
+
+
+def tag_csr(sets, n: int, what: str) -> Tuple[np.ndarray, np.ndarray]:
+    """Tag sets as CSR ``(indptr int64[n+1] from 0, tags int32)``: ``sets`` is a sequence of ``n`` iterables of
+    ints, or such a pair already (``is_csr_pair``; ``what`` names the sets in the error)."""
+    if is_csr_pair(sets):
+        indptr = np.ascontiguousarray(sets[0], dtype=np.int64).reshape(-1)
+        tags = np.ascontiguousarray(sets[1], dtype=np.int32).reshape(-1)
+    else:
+        sets = list(sets)
+        indptr = np.zeros(len(sets) + 1, dtype=np.int64)
+        indptr[1:] = np.cumsum([len(t) for t in sets])
+        tags = np.fromiter((int(t) for ts in sets for t in ts), dtype=np.int32, count=int(indptr[-1]))
+    if len(indptr) != n + 1:
+        raise ValueError(f"{what}: {len(indptr) - 1} tag sets for {n} entries")
+    return indptr, tags
+
+
+def csr_rows(indptr: np.ndarray, tags: np.ndarray, sel: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
+    """The entries ``sel`` (int array) of a tag CSR, as a CSR of their own; a negative entry gives an empty set."""
+    sel = np.asarray(sel, dtype=np.int64)
+    neg = sel < 0
+    sel = np.where(neg, 0, sel)
+    lens = np.where(neg, 0, indptr[sel + 1] - indptr[sel])
+    out_ip = np.zeros(len(sel) + 1, dtype=np.int64)
+    np.cumsum(lens, out=out_ip[1:])
+    src = np.repeat(indptr[sel] - out_ip[:-1], lens) + np.arange(out_ip[-1], dtype=np.int64)
+    return out_ip, np.ascontiguousarray(tags[src], dtype=np.int32)
+
+
 class FeatureBatch:
     """CSR of a featurised batch; owns the native kv_csr and exposes zero-copy NumPy views."""
 
@@ -383,6 +420,18 @@ class GfkbIndex(_KvIndex):
         _capi.check(_capi.load().kv_index_set_row_groups(self._h, _ptr(groups, C.c_int32), len(groups)))
         self._group_rows = len(groups)
 
+    def set_row_tags(self, sets) -> None:
+        """A set of tags >= 0 per local row (e.g. a failure's affected apps as ids; any number, may be empty), for the
+        ``tags`` filter of the query methods: a sequence of iterables, or a tuple of two arrays ``(indptr, tags)``
+        (``is_csr_pair``); ``None`` clears.  Lifetime as ``set_row_labels``; tags touch no statistics, so setting them
+        again needs no finalize."""
+        if sets is None:
+            _capi.check(_capi.load().kv_index_set_row_tags(self._h, None, None, 0))
+            return
+        indptr, tags = tag_csr(sets, self.n_rows, "set_row_tags")
+        _capi.check(_capi.load().kv_index_set_row_tags(self._h, _ptr(indptr, C.c_int64), _ptr(tags, C.c_int32),
+                                                       len(indptr) - 1))
+
     @property
     def has_row_groups(self) -> bool:
         """Whether ``set_row_groups`` describes the current rows (an append drops the groups)."""
@@ -456,17 +505,23 @@ class GfkbIndex(_KvIndex):
             fb.close()
 
     def topk_features(self, fb: FeatureBatch, k: int, labels: Optional[np.ndarray] = None,
-                      distinct: bool = False) -> Tuple[np.ndarray, np.ndarray]:
+                      distinct: bool = False, tags=None) -> Tuple[np.ndarray, np.ndarray]:
         """``labels``: per query the row label its results must carry (-1: any row), see ``set_filter``.  ``distinct``:
-        at most one row per group (``set_row_groups``), see ``set_distinct``."""
+        at most one row per group (``set_row_groups``), see ``set_distinct``.  ``tags``: per query a set of at most 16
+        tags, one of which its results must carry (empty: any row), see ``set_tag_filter``."""
         if fb.n == 0:
             return np.zeros((0, k), np.float32), np.zeros((0, k), np.int64)
         self.upload_queries(fb)
-        return self._topk_uploaded(fb.n, k, labels, distinct)
+        return self._topk_uploaded(fb.n, k, labels, distinct, tags)
 
-    def _topk_uploaded(self, n_q: int, k: int, labels: Optional[np.ndarray], distinct: bool):
+    def _set_filters(self, labels: Optional[np.ndarray], tags) -> None:
         if labels is not None:
             self.set_filter(labels)
+        if tags is not None:
+            self.set_tag_filter(tags)
+
+    def _topk_uploaded(self, n_q: int, k: int, labels: Optional[np.ndarray], distinct: bool, tags=None):
+        self._set_filters(labels, tags)
         if distinct:
             self.set_distinct(True)
         return self.topk_resident_host(n_q, k)
@@ -551,6 +606,17 @@ class GfkbIndex(_KvIndex):
         labels = np.ascontiguousarray(labels, dtype=np.int32)
         _capi.check(_capi.load().kv_query_set_filter(self._h, _ptr(labels, C.c_int32), len(labels)))
 
+    def set_tag_filter(self, sets) -> None:
+        """Query q of the resident batch only matches rows whose tag set (``set_row_tags``) meets ``sets[q]`` (at most
+        16 tags; empty = any row): a sequence of iterables, or a tuple of two arrays ``(indptr, tags)``
+        (``is_csr_pair``); ``None`` clears, and so does the next upload.  Combines with ``set_filter`` and ``set_distinct``; the scores are the unfiltered ones."""
+        if sets is None:
+            _capi.check(_capi.load().kv_query_set_tag_filter(self._h, None, None, 0))
+            return
+        indptr, tags = tag_csr(sets, len(sets[0]) - 1 if is_csr_pair(sets) else len(sets), "set_tag_filter")
+        _capi.check(_capi.load().kv_query_set_tag_filter(self._h, _ptr(indptr, C.c_int64), _ptr(tags, C.c_int32),
+                                                         len(indptr) - 1))
+
     def set_distinct(self, on: bool, merged_seeds: bool = False) -> None:
         """Distinct top-k for the resident batch (until the next upload): of the rows a query may match, the best row
         of each group (``set_row_groups``) in (score desc, row asc) order, the groups ranked by it, and the first k
@@ -580,30 +646,30 @@ class GfkbIndex(_KvIndex):
         return self.topk_resident_host(hi - lo, k)
 
     def range_features(self, fb: FeatureBatch, threshold: float, device_out: bool = False,
-                       labels: Optional[np.ndarray] = None):
+                       labels: Optional[np.ndarray] = None, tags=None):
         """Threshold search: every (query, row) pair whose float32 score (the value ``topk`` reports) is >= ``threshold``,
         0 < threshold <= 1.  Returns ``(indptr int64[n_q+1], rows int64[P], scores float32[P])``: query q's pairs are
         ``[indptr[q], indptr[q+1])``, ordered by (score desc, row asc); rows are global.  ``device_out``: the same
         arrays as torch tensors on the index's device (nothing is copied to the host).  ``labels``: per query the row
-        label its pairs must carry (-1: any row), see ``set_filter``."""
+        label its pairs must carry (-1: any row), see ``set_filter``.  ``tags``: per query the tag sets its pairs' rows
+        must meet, see ``set_tag_filter``."""
         if fb.n == 0:
             return self._empty_range(device_out)
         self.upload_queries(fb)
-        return self._range_uploaded(fb.n, threshold, device_out, labels)
+        return self._range_uploaded(fb.n, threshold, device_out, labels, tags)
 
-    def _range_uploaded(self, n_q: int, threshold: float, device_out: bool, labels: Optional[np.ndarray]):
-        if labels is not None:
-            self.set_filter(labels)
+    def _range_uploaded(self, n_q: int, threshold: float, device_out: bool, labels: Optional[np.ndarray], tags=None):
+        self._set_filters(labels, tags)
         return self._range_resident(n_q, threshold, device_out)
 
     def range(self, queries: Sequence[str], threshold: float, device_out: bool = False,
-              labels: Optional[np.ndarray] = None):
+              labels: Optional[np.ndarray] = None, tags=None):
         """``range_features`` of texts."""
         if len(queries) and _featurize_on_device(len(queries)):
-            return self._range_uploaded(self.upload_text(*pack_texts(queries)), threshold, device_out, labels)
+            return self._range_uploaded(self.upload_text(*pack_texts(queries)), threshold, device_out, labels, tags)
         fb = self.vocab.featurize(queries, grow=False)
         try:
-            return self.range_features(fb, threshold, device_out, labels)
+            return self.range_features(fb, threshold, device_out, labels, tags)
         finally:
             fb.close()
 
@@ -628,10 +694,10 @@ class GfkbIndex(_KvIndex):
         return out
 
     def exact_topk(self, fb: FeatureBatch, k: int, labels: Optional[np.ndarray] = None,
-                   distinct: bool = False) -> Tuple[np.ndarray, np.ndarray]:
+                   distinct: bool = False, tags=None) -> Tuple[np.ndarray, np.ndarray]:
         """(rows int64 [Q,k], scores float64 [Q,k]): each query's best k rows of this index with no candidate stage
         (``kv_exact_topk``: K1a over every row, selection in float64 order on the device, K6 scores), global rows
-        ordered by (score desc, row asc), (-1, -inf) past the last.  ``labels`` / ``distinct`` as for
+        ordered by (score desc, row asc), (-1, -inf) past the last.  ``labels`` / ``distinct`` / ``tags`` as for
         ``topk_features``.  K6 scores tie exactly for identical texts on any index, so lists of several indexes merge
         into the stable order of one."""
         rows = np.empty((fb.n, k), dtype=np.int64)
@@ -639,10 +705,18 @@ class GfkbIndex(_KvIndex):
         lab = None if labels is None else np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
         if lab is not None and len(lab) != fb.n:
             raise ValueError(f"exact_topk: {len(lab)} labels for a batch of {fb.n} queries")
-        _capi.check(_capi.load().kv_exact_topk(self._h, _ptr(fb.indptr, C.c_int64), _ptr(fb.ids, C.c_uint32),
-                                               _ptr(fb.tf, C.c_uint32), _ptr(fb.oov, C.c_double),
-                                               None if lab is None else _ptr(lab, C.c_int32), int(distinct), fb.n, k,
-                                               _ptr(rows, C.c_int64), _ptr(scores, C.c_double)))
+        if tags is None:
+            _capi.check(_capi.load().kv_exact_topk(self._h, _ptr(fb.indptr, C.c_int64), _ptr(fb.ids, C.c_uint32),
+                                                   _ptr(fb.tf, C.c_uint32), _ptr(fb.oov, C.c_double),
+                                                   None if lab is None else _ptr(lab, C.c_int32), int(distinct), fb.n, k,
+                                                   _ptr(rows, C.c_int64), _ptr(scores, C.c_double)))
+            return rows, scores
+        t_ip, t = tag_csr(tags, fb.n, "exact_topk")
+        _capi.check(_capi.load().kv_exact_topk_tags(self._h, _ptr(fb.indptr, C.c_int64), _ptr(fb.ids, C.c_uint32),
+                                                    _ptr(fb.tf, C.c_uint32), _ptr(fb.oov, C.c_double),
+                                                    None if lab is None else _ptr(lab, C.c_int32), _ptr(t_ip, C.c_int64),
+                                                    _ptr(t, C.c_int32), int(distinct), fb.n, k,
+                                                    _ptr(rows, C.c_int64), _ptr(scores, C.c_double)))
         return rows, scores
 
     def topk_resident(self, k: int, d_scores_ptr: int, d_rows_ptr: int) -> None:
@@ -662,15 +736,15 @@ class GfkbIndex(_KvIndex):
         _capi.check(_capi.load().kv_topk_resident_finish(self._h, k, C.c_void_p(d_scores_ptr), C.c_void_p(d_rows_ptr)))
 
     def topk(self, queries: Sequence[str], k: int, labels: Optional[np.ndarray] = None,
-             distinct: bool = False) -> Tuple[np.ndarray, np.ndarray]:
+             distinct: bool = False, tags=None) -> Tuple[np.ndarray, np.ndarray]:
         """(scores float32 [Q,k], rows int64 [Q,k]) ordered by (score desc, row asc) (K1b+K5).  ``labels``: per query
         the row label its results must carry (-1: any row).  ``distinct``: at most one row per group (the best one;
-        ``set_row_groups``)."""
+        ``set_row_groups``).  ``tags``: per query the tag set its results' rows must meet (``set_tag_filter``)."""
         if len(queries) and _featurize_on_device(len(queries)):
-            return self._topk_uploaded(self.upload_text(*pack_texts(queries)), k, labels, distinct)
+            return self._topk_uploaded(self.upload_text(*pack_texts(queries)), k, labels, distinct, tags)
         fb = self.vocab.featurize(queries, grow=False)
         try:
-            return self.topk_features(fb, k, labels, distinct)
+            return self.topk_features(fb, k, labels, distinct, tags)
         finally:
             fb.close()
 

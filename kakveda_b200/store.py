@@ -37,7 +37,7 @@ import numpy as np
 from .fingerprint import signature_text as _signature_text
 from .gfkb import MATCH_LIMIT, _to_match
 from . import sidecar as _sidecar
-from .similarity import FeatureBatch, GfkbIndex, Vocabulary
+from .similarity import FeatureBatch, GfkbIndex, Vocabulary, csr_rows
 
 CANDIDATES = 16  # float32 candidates per query and segment that get re-scored in float64 (>= MATCH_LIMIT)
 MAX_LIMIT = 32   # the fused top-k of the scan holds at most 32 rows per query and segment
@@ -96,6 +96,75 @@ def check_indexable(text: str, vocab_size: int = 0) -> Optional[str]:
     return None
 
 
+class AppTags:
+    """The records' affected_apps as interned row tags, kept as one CSR over the records in record order: app ids are
+    numbered in order of first appearance, ``ip`` / ``vals`` hold each record's ids, ``count[id]`` how many list
+    entries name the app.  New records are added incrementally; a purge filters the purged ids out in NumPy and a
+    record drop keeps the surviving rows, so no call walks every record in Python again."""
+
+    def __init__(self):
+        self.ids: Dict[str, int] = {}
+        self.ip = np.zeros(1, dtype=np.int64)
+        self.vals = np.zeros(0, dtype=np.int32)
+        self.count = np.zeros(0, dtype=np.int64)
+        self._rec_of_val: Optional[np.ndarray] = None  # record of every entry (exact fallback), built on demand
+
+    @property
+    def n(self) -> int:
+        return len(self.ip) - 1
+
+    def extend(self, recs: Sequence[Mapping[str, Any]]) -> None:
+        lens, flat = [], []
+        for r in recs:
+            apps = r.get("affected_apps")
+            t = [self.ids.setdefault(a, len(self.ids)) for a in apps] if isinstance(apps, list) else []
+            lens.append(len(t))
+            flat.extend(t)
+        if not lens:
+            return
+        self.ip = np.concatenate([self.ip, self.ip[-1] + np.cumsum(lens, dtype=np.int64)])
+        self.vals = np.concatenate([self.vals, np.asarray(flat, dtype=np.int32)])
+        grown = np.zeros(len(self.ids), dtype=np.int64)
+        grown[:len(self.count)] = self.count
+        self.count = grown + np.bincount(np.asarray(flat, dtype=np.int64), minlength=len(self.ids))
+        self._rec_of_val = None
+
+    def purge(self, apps) -> None:
+        """Every list loses ``apps`` (as ``GfkbStore.purge_apps`` rewrites affected_apps)."""
+        gone = [self.ids[a] for a in apps if a in self.ids]
+        if not gone:
+            return
+        keep = ~np.isin(self.vals, gone)
+        pos = np.zeros(len(keep) + 1, dtype=np.int64)
+        np.cumsum(keep, out=pos[1:])
+        self.ip = pos[self.ip]
+        self.vals = self.vals[keep]
+        self.count[gone] = 0
+        self._rec_of_val = None
+
+    def keep(self, keep_idx) -> None:
+        """Only the records ``keep_idx`` (ascending) remain; dropped records list no app (a purge emptied them)."""
+        self.ip, self.vals = csr_rows(self.ip, self.vals, np.asarray(keep_idx, dtype=np.int64))
+        self._rec_of_val = None
+
+    def listed(self, app: str) -> int:
+        """The app's id when some record lists it, else -2."""
+        i = self.ids.get(app, -1)
+        return i if i >= 0 and self.count[i] > 0 else -2
+
+    def rows(self, recs: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
+        """CSR of the tags of records ``recs`` (-1: an empty set, e.g. a deleted device row)."""
+        return csr_rows(self.ip, self.vals, recs)
+
+    def records_with(self, tag: int) -> np.ndarray:
+        """bool [n]: which records list app id ``tag``."""
+        if self._rec_of_val is None:
+            self._rec_of_val = np.repeat(np.arange(self.n, dtype=np.int64), np.diff(self.ip))
+        out = np.zeros(self.n, dtype=bool)
+        out[self._rec_of_val[self.vals == tag]] = True
+        return out
+
+
 def _iso(dt: datetime) -> str:
     """pydantic's JSON form of an aware UTC datetime (model_dump(mode="json"), app.py:131,146)."""
     return dt.isoformat().replace("+00:00", "Z")
@@ -136,6 +205,12 @@ class GfkbStore:
         # first appearance; group of each record.  Set on the segments only when a distinct match needs them.
         self._group_ids: Dict[Tuple[str, str], int] = {}
         self._groups: List[int] = []
+        # affected_apps as row tags of the device index (app-scoped match), kept incrementally for records[:_apps.n].
+        # A device row's tags are its record's apps; set on the segments only when an app-scoped match needs them
+        # (_main_tags_ok / _tail_tag_rows: which segment's tags describe the records as they are).
+        self._apps = AppTags()
+        self._main_tags_ok = False
+        self._tail_tag_rows = -1
         self.stats = {"full_rebuilds": 0, "stat_refreshes": 0, "compactions": 0, "quarantined": 0}
         self.quarantined: List[int] = []  # indices of loaded records that cannot be indexed (they keep their row, with no features)
         if self.path is not None and self.path.exists():
@@ -167,6 +242,7 @@ class GfkbStore:
             self._latest[(r["failure_type"], r["signature_text"])] = i
         self._type_ids, self._labels = {}, []
         self._group_ids, self._groups = {}, []
+        self._apps = AppTags()
         self._rebuild_main()
 
     def _row_labels(self, lo: int, hi: int) -> np.ndarray:
@@ -187,6 +263,7 @@ class GfkbStore:
             self._main.set_row_labels(self._row_labels(0, n))
             self.stats["full_rebuilds"] += 1
         self._n_main = self._n_indexed = self._n_dev = n
+        self._main_tags_ok, self._tail_tag_rows = False, -1
         self._sidecar_rows = n if self.sidecar_path is not None else 0  # the sidecar holds the CSR of records[:n]
         self._row2rec = None
         self._n_deleted = 0
@@ -268,6 +345,28 @@ class GfkbStore:
                 if groups is None:
                     groups = self._dev_groups(self._n_dev)
                 ix.set_row_groups(groups[lo:lo + ix.n_rows])
+
+    def _sync_apps(self) -> None:
+        """Intern the apps of the records not seen yet (incremental, like ``_row_labels``)."""
+        if self._apps.n < len(self.records):
+            self._apps.extend(self.records[self._apps.n:])
+
+    def _dev_recs(self, lo: int, hi: int) -> np.ndarray:
+        """Record of device rows [lo, hi), -1 for a deleted row."""
+        if self._row2rec is None:
+            return np.arange(lo, hi, dtype=np.int64)
+        return self._row2rec[lo:hi]
+
+    def _ensure_tags(self) -> None:
+        """The segments carry their rows' app tags: only a stale segment is uploaded (a rebuild or a purge makes the
+        main segment stale, an append the tail).  Tags touch no statistics: no finalize follows."""
+        tail = self._tail
+        if not self._main_tags_ok and self._main is not None:
+            self._main.set_row_tags(self._apps.rows(self._dev_recs(0, self._n_main)))
+            self._main_tags_ok = True
+        if tail is not None and tail.n_rows and self._tail_tag_rows != tail.n_rows:
+            tail.set_row_tags(self._apps.rows(self._dev_recs(self._n_main, self._n_main + tail.n_rows)))
+            self._tail_tag_rows = tail.n_rows
 
     def _to_records(self, rows: np.ndarray) -> np.ndarray:
         """Device rows -> record indices (-1 stays -1)."""
@@ -398,6 +497,10 @@ class GfkbStore:
                     shutil.copy2(self.path, self.path.with_name(f"{self.path.name}.bak-{stamp}"))
                 lines = [json.dumps(self.records[i], ensure_ascii=False) for i in keep_idx]
                 self.path.write_text("\n".join(lines) + ("\n" if lines else ""), encoding="utf-8")
+            if updated:  # the rewritten lists change their rows' app tags
+                self._sync_apps()
+                self._apps.purge(purge)
+                self._main_tags_ok, self._tail_tag_rows = False, -1
             if removed:
                 self._drop_records(keep_idx)
             return {"kept": kept, "removed": removed, "updated": updated}
@@ -414,6 +517,8 @@ class GfkbStore:
         gone = live_rows[~keep[: self._n_indexed]]
         self.records = [self.records[i] for i in keep_idx]
         self._labels = [lab for i, lab in enumerate(self._labels) if keep[i]]
+        if self._apps.n:
+            self._apps.keep(np.flatnonzero(keep[:self._apps.n]))
         self._groups = [g for i, g in enumerate(self._groups) if keep[i]]  # survivors keep their group ids
         self.quarantined = [int(new_idx[i]) for i in self.quarantined if keep[i]]
         self._quarantine_set = set(self.quarantined)
@@ -479,11 +584,12 @@ class GfkbStore:
 
     # -- match (services/gfkb/app.py:79-102) -------------------------------------------------------------------
     def _candidates(self, fb: FeatureBatch, k: int, limit: int = MATCH_LIMIT, labels: Optional[np.ndarray] = None,
-                    distinct: bool = False) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+                    distinct: bool = False, tags=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
         """Per query: candidate rows from both segments with their float64 scores, ordered (score desc, row asc), and
         whether the candidate stage may have missed a top-``limit`` row (``ambiguous_candidates``).  ``labels``: per
         query the failure-type label its candidates must carry (-1: any).  ``distinct``: each segment returns one row
-        per (failure_type, signature_text) group, and the merge keeps the first row of each group."""
+        per (failure_type, signature_text) group, and the merge keeps the first row of each group.  ``tags``: per query
+        the app tags one of which its candidates must carry (empty: any)."""
         if distinct:
             self._ensure_groups()
         rows_all, f64_all = [], []
@@ -491,7 +597,8 @@ class GfkbStore:
         for ix in (self._main, self._tail):
             if ix is None or ix.n_rows == 0:
                 continue
-            s32, rows = self._segment_topk(ix, fb, min(k, MAX_LIMIT), labels, distinct)
+            s32, rows = (self._segment_topk(ix, fb, min(k, MAX_LIMIT), labels, distinct) if tags is None
+                         else self._segment_topk(ix, fb, min(k, MAX_LIMIT), labels, distinct, tags))
             amb |= ambiguous_candidates(s32, rows, limit)
             rows_all.append(rows)
             f64_all.append(ix.rescore(fb, rows))
@@ -499,8 +606,10 @@ class GfkbStore:
 
     @staticmethod
     def _segment_topk(ix: GfkbIndex, fb: FeatureBatch, kk: int, labels: Optional[np.ndarray],
-                      distinct: bool) -> Tuple[np.ndarray, np.ndarray]:
+                      distinct: bool, tags=None) -> Tuple[np.ndarray, np.ndarray]:
         """One segment's float32 candidates: (scores, global rows), each [Q, kk]."""
+        if tags is not None:
+            return ix.topk_features(fb, kk, labels, distinct, tags)
         if distinct:
             return ix.topk_features(fb, kk, labels, distinct=True)
         return ix.topk_features(fb, kk) if labels is None else ix.topk_features(fb, kk, labels)
@@ -539,13 +648,25 @@ class GfkbStore:
         return _to_match(self.records[self._latest[(r["failure_type"], r["signature_text"])]], score)
 
     def _exact_top(self, signature_text: str, limit: int, label: int = -1,
-                   distinct: bool = False) -> Tuple[List[int], List[float]]:
+                   distinct: bool = False, app: int = -1) -> Tuple[List[int], List[float]]:
         """Rows and float64 scores of the reference's ``sorted(..., reverse=True)[:limit]`` on the full score vector
         (K1a on both segments): no candidate stage at all.  ``label`` >= 0: over the rows of that failure-type label.
-        ``distinct``: over the first eligible row of each (failure_type, signature_text) group."""
+        ``distinct``: over the first eligible row of each (failure_type, signature_text) group.  ``app`` >= 0: over
+        the rows whose record lists that app (tag)."""
         parts = [ix.score(signature_text) for ix in (self._main, self._tail) if ix is not None and ix.n_rows]
         scores = np.concatenate(parts)  # by device row; -inf for a deleted row
-        if distinct:
+        if app >= 0:  # a deleted row lists no app
+            self._sync_apps()
+            recs = self._dev_recs(0, len(scores))
+            elig = (recs >= 0) & self._apps.records_with(app)[np.clip(recs, 0, None)]
+            if label >= 0:
+                elig &= self._dev_labels(len(scores)) == label
+            idx = np.flatnonzero(elig)  # ascending: the stable order is kept
+            if distinct:
+                _, first = np.unique(self._dev_groups(len(scores))[idx], return_index=True)
+                idx = idx[np.sort(first)]
+            order = idx[stable_top(scores[idx], limit)]
+        elif distinct:
             if label >= 0:
                 idx = np.flatnonzero(self._dev_labels(len(scores)) == label)
             elif self._row2rec is not None:
@@ -593,19 +714,61 @@ class GfkbStore:
             out[i] = [to_match(r, s) for r, s in zip(top_r, top_s) if r >= 0]
         return out
 
+    def _match_apps(self, signature_texts: Sequence[str], failure_types: Optional[Sequence[Optional[str]]],
+                    app_ids: Sequence[Optional[str]], limit: int, filter_first: bool, distinct: bool) -> List[List[dict]]:
+        """The best ``limit`` rows among the failures whose affected_apps list the query's app (all rows for a query
+        without one), searched on the device through the app tags; with ``filter_first`` also of the query's
+        failure_type, else the failure_type post-filter of the reference follows."""
+        self._row_labels(0, len(self.records))  # number every stored type
+        self._sync_apps()                        # ... and every listed app
+        apps = np.array([-1 if not a else self._apps.listed(a) for a in app_ids], dtype=np.int64)
+        labels = np.full(len(signature_texts), -1, dtype=np.int32)
+        if filter_first and failure_types is not None:
+            labels = np.array([-1 if not ft else self._type_ids.get(ft, -2) for ft in failure_types], dtype=np.int32)
+        out: List[List[dict]] = [[] for _ in signature_texts]
+        scan = np.flatnonzero((apps != -2) & (labels != -2))  # an app or type no stored row has: no match, no scan
+        if len(scan) == 0:
+            return out
+        self._ensure_tags()
+        tags = [[int(apps[i])] if apps[i] >= 0 else [] for i in scan.tolist()]
+        fb = self.vocab.featurize([signature_texts[i] for i in scan], grow=False)
+        try:
+            rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit,
+                                              labels[scan] if (labels >= 0).any() else None, distinct, tags)
+        finally:
+            fb.close()
+        to_match = self._distinct_match if distinct else (lambda r, s: _to_match(self.records[r], s))
+        for j, i in enumerate(scan.tolist()):
+            if amb[j]:
+                top_r, top_s = self._exact_top(signature_texts[i], limit, int(labels[i]), distinct, int(apps[i]))
+                self.stats["exact_fallbacks"] = self.stats.get("exact_fallbacks", 0) + 1
+            else:
+                top_r, top_s = rows[j, :limit].tolist(), f64[j, :limit].tolist()
+            ft = failure_types[i] if failure_types is not None else None
+            out[i] = [to_match(r, s) for r, s in zip(top_r, top_s)
+                      if r >= 0 and not (ft and self.records[r]["failure_type"] != ft)]
+        return out
+
     def match_batch(self, signature_texts: Sequence[str], failure_types: Optional[Sequence[Optional[str]]] = None,
-                    limit: int = MATCH_LIMIT, filter_first: bool = False, distinct: bool = False) -> List[List[dict]]:
+                    limit: int = MATCH_LIMIT, filter_first: bool = False, distinct: bool = False,
+                    app_ids: Optional[Sequence[Optional[str]]] = None) -> List[List[dict]]:
         """``filter_first=False`` (default): the reference's handler -- the best ``limit`` rows, THEN the failure_type
         filter, so rows of other types can leave fewer than ``limit`` (or no) matches.  ``filter_first=True``: the best
         ``limit`` rows of the query's failure_type, searched on the device among that type's rows only.
         ``distinct=True``: the best ``limit`` distinct failures, one per (failure_type, signature_text) key instead of
-        one per stored version, each reported with the fields of the key's newest record and the key's score."""
+        one per stored version, each reported with the fields of the key's newest record and the key's score.
+        ``app_ids``: per query an app (None: any); the search is then limited, on the device, to the failures whose
+        affected_apps list it, and an app no record lists matches nothing.  It combines with the other options."""
         if limit > MAX_LIMIT:
             raise ValueError(f"limit {limit} exceeds the {MAX_LIMIT} rows the fused top-k holds per query")
+        if app_ids is not None and len(app_ids) != len(signature_texts):
+            raise ValueError(f"app_ids: {len(app_ids)} apps for {len(signature_texts)} queries")
         with self._lock:
             if not self.records:
                 return [[] for _ in signature_texts]  # app.py:82-83
             self._sync()
+            if app_ids is not None and any(app_ids):
+                return self._match_apps(signature_texts, failure_types, app_ids, limit, filter_first, distinct)
             if filter_first and failure_types is not None and any(failure_types):
                 return self._match_filter_first(signature_texts, failure_types, limit, distinct)
             fb = self.vocab.featurize(list(signature_texts), grow=False)
@@ -637,7 +800,10 @@ class GfkbStore:
             return out
 
     def match(self, signature_text: str, failure_type: Optional[str] = None, filter_first: bool = False,
-              distinct: bool = False) -> List[dict]:
+              distinct: bool = False, app_id: Optional[str] = None) -> List[dict]:
+        if app_id is not None:
+            return self.match_batch([signature_text], [failure_type], filter_first=filter_first, distinct=distinct,
+                                    app_ids=[app_id])[0]
         return self.match_batch([signature_text], [failure_type], filter_first=filter_first, distinct=distinct)[0]
 
     def match_exact(self, signature_text: str, failure_type: Optional[str] = None, limit: int = MATCH_LIMIT) -> List[dict]:
@@ -657,10 +823,15 @@ class GfkbStore:
 
     # -- warn (services/warning_policy/app.py:19-72) ------------------------------------------------------------
     def warn_batch(self, requests: Sequence[Mapping[str, Any]], threshold: float = 0.8, default_action: str = "warn",
-                   patterns: Optional[Sequence[Mapping[str, Any]]] = None) -> List[dict]:
-        """One WarningResponse-shaped dict per request; all GFKB lookups go through ONE batched scan."""
+                   patterns: Optional[Sequence[Mapping[str, Any]]] = None, app_scoped: bool = False) -> List[dict]:
+        """One WarningResponse-shaped dict per request; all GFKB lookups go through ONE batched scan.  ``app_scoped``:
+        each request is matched against the failures of its own ``app_id`` only (default: the reference's handler,
+        which matches against every failure)."""
         sigs = [_signature_text(r["prompt"], list(r.get("tools") or []), dict(r.get("env") or {})) for r in requests]
-        all_matches = self.match_batch(sigs)
+        if app_scoped:
+            all_matches = self.match_batch(sigs, app_ids=[r.get("app_id") for r in requests])
+        else:
+            all_matches = self.match_batch(sigs)
         out = []
         for matches in all_matches:
             best = matches[0] if matches else None
