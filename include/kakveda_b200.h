@@ -570,8 +570,27 @@ int kv_dense_deleted_rows(kv_dense_index *dx, uint8_t *out, int64_t n);
  * filtered search on an index whose labels are missing or stale (appended rows). */
 int kv_dense_set_row_labels(kv_dense_index *dx, const int32_t *labels, int64_t n);
 int kv_dense_set_query_filter(kv_dense_index *dx, const int32_t *labels, int64_t n_q);
-/* Measurement and test hook: the (query tile, row tile) items the last dense search's kernel skipped and its total
- * items (q_tiles x r_tiles; skipped is 0 for an unfiltered search). */
+/* Dense tag filter (e.g. a failure's affected apps), with the semantics of kv_index_set_row_tags /
+ * kv_query_set_tag_filter.  kv_dense_set_row_tags gives every local row a SET of tags >= 0, any number, possibly none:
+ * row r holds tags[indptr[r] .. indptr[r+1]), indptr[n+1] starting at 0, n == kv_dense_rows; NULL clears.  Row tags
+ * have the lifetime of the row labels: set before or after finalize, kept by finalize and deletions, dropped by an
+ * append; setting them on a finalized index needs no finalize.
+ * kv_dense_set_tag_filter gives each query of THE NEXT SEARCH CALL on the handle a set of at most 16 tags (same CSR
+ * form; an empty set: no tag constraint), with the lifetime of kv_dense_set_query_filter: that call must have exactly
+ * n_q queries (else KV_ERR_INVALID) and clears it whether it succeeds or fails; an append or a finalize clears it too;
+ * NULL clears.  A query with tags matches only the rows whose set meets its own (any of its tags); the label filter,
+ * deletions and self-join exclusions apply as well.  Its top-k is the top-k over its eligible live rows -- (score desc,
+ * row asc), the same float32 scores as unfiltered, (-inf, -1) past the last eligible row -- and its threshold search
+ * returns the unfiltered pairs whose rows are eligible.  The kernel skips every (128-query tile, 256-row tile) item
+ * whose row tile carries no tag of a query of the query tile (a 64-bit signature of bit t & 63 per tag over the live
+ * rows; a query tile holding a query without tags skips nothing this way, since that query matches untagged rows
+ * too), then tests each row's mask and, when the index holds a tag >= 64, its exact set.
+ * KV_ERR_INVALID: wrong counts, indptr not starting at 0 or decreasing, a negative tag, more than 16 tags on a query.
+ * KV_ERR_STATE: a search with a tagged query on an index whose row tags are missing or stale (appended rows). */
+int kv_dense_set_row_tags(kv_dense_index *dx, const int64_t *indptr, const int32_t *tags, int64_t n);
+int kv_dense_set_tag_filter(kv_dense_index *dx, const int64_t *indptr, const int32_t *tags, int64_t n_q);
+/* Measurement and test hook: the (query tile, row tile) items the last dense search's kernel skipped, by the label or
+ * the tag signature, and its total items (q_tiles x r_tiles; skipped is 0 for an unfiltered search). */
 int kv_dense_last_skipped(const kv_dense_index *dx, int64_t *skipped, int64_t *items);
 
 /* ------------------------------------------------------------------------------------

@@ -136,6 +136,8 @@ SIGNATURES = {
     "kv_dense_set_row_labels": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int64]),
     "kv_dense_set_query_filter": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int64]),
     "kv_dense_last_skipped": (C.c_int, [C.c_void_p, c_i64p, c_i64p]),
+    "kv_dense_set_row_tags": (C.c_int, [C.c_void_p, c_i64p, C.POINTER(C.c_int32), C.c_int64]),
+    "kv_dense_set_tag_filter": (C.c_int, [C.c_void_p, c_i64p, C.POINTER(C.c_int32), C.c_int64]),
     "kv_hash_create": (C.c_int, [C.c_int, C.c_int64, C.POINTER(C.c_void_p)]),
     "kv_hash_destroy": (None, [C.c_void_p]),
     "kv_hash_append": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.c_int64]),

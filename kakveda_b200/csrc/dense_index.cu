@@ -24,6 +24,8 @@
 // K2-R (dense_topk_kernel<true>) is the same kernel for a threshold search: producer, ring, MMAs and register exchange
 // are unchanged; the epilogue keeps no lists and appends every pair whose score (the same float32 expression) reaches
 // the threshold to a global pair buffer, one reservation per warp and 16-column group (dense_emit).
+// FILTER and TAGS add the label and tag filters of a search (DenseFilter): items no query of the tile can match are
+// skipped, and an element outside its query's filter gets a NaN scale.
 #include "index_state.cuh"
 #include "kv_cuda.cuh"
 #include "sm90.cuh"
@@ -120,6 +122,16 @@ struct DenseFilter {
   const unsigned long long *tile_sig;   // [r_tiles] OR of 1 << (label & 63) over the tile's live rows
   const unsigned long long *qsig;       // [q_tiles] the same over the tile's queries (all ones: an unfiltered query)
   unsigned long long *skipped;          // (query tile, row tile) items skipped, counted by the producers
+  // Tag filter (dense_topk_kernel<*, true, true>; tags_meet): query p only matches the rows whose tag set meets its own
+  // (q_tmask[p] == 0: any row).  A tag-filtered call without labels runs with every query label -1 and lab_c =
+  // tile_sig = NULL.  Rows by local row, queries in kernel order (stable-sorted by (label, smallest tag)).
+  const unsigned long long *tmask_c;    // [n_rows] OR of 1 << (t & 63) over the row's tags
+  const int64_t *tag_ptr;               // [n_rows + 1] CSR of the rows' tags; NULL when every tag is < 64
+  const int *tag_list;
+  const unsigned long long *q_tmask;    // [n_q] the queries' masks (0: no tag constraint)
+  const int *q_tags;                    // [n_q][MAX_QTAGS] ascending, -1 past the last
+  const unsigned long long *tile_tsig;  // [r_tiles] OR of the masks of the tile's live rows
+  const unsigned long long *qtsig;      // [q_tiles] OR of the tile's query masks (all ones: a query without tags; no tag skip)
 };
 
 // order-preserving float <-> unsigned key (cosines may be negative)
@@ -138,19 +150,35 @@ struct __align__(1024) DenseSmem {
   float lscore[2][MAXK][BM];  // [column half][slot][query]: the 32 lanes of a warp hit 32 different banks
   int lrow[2][MAXK][BM];
   int lab_c[2][BN];  // FILTER: this tile's row labels (-1 past the end); last, so the other members keep their offsets
+  __align__(16) unsigned long long tmask_c[2][BN];  // TAGS: this tile's row tag masks (0 past the end); after lab_c for the same reason
 };
 
+// Whether the producer skips item (query tile qtile, row tile t): no live row of the tile carries a label (FILTER) or a
+// tag (TAGS) of any query of the tile.  Each signature test alone has no false negatives.
+template <bool TAGS>
+__device__ __forceinline__ bool item_skipped(const DenseFilter &F, int64_t t, int qtile) {
+  if constexpr (TAGS) {
+    // a query without tags (qtsig all ones: a tagged query sets at most MAX_QTAGS bits) matches rows without tags too,
+    // which tile_tsig does not record, so its tile takes no tag test
+    if (F.qtsig[qtile] != ~0ull && (F.tile_tsig[t] & F.qtsig[qtile]) == 0) return true;
+    if (!F.tile_sig) return false;  // no label filter in this call
+  }
+  return (F.tile_sig[t] & F.qsig[qtile]) == 0;
+}
+
 // K2-R: appends this thread's pairs of one 16-column group (columns c0 + {0, 1, 4, 5, 8, 9, 12, 13} of the tile at
-// row0): (q, tv[e] * inv_q, global row) for each element whose score reaches R.thr, whose row exists and is not the
-// excluded one.  All 32 lanes call it; the warp reserves its records with one atomic (none when no lane has a hit).
+// row0): (q, tv[e] * inv_q, global row) for each element whose score reaches R.thr, whose row exists, is not the
+// excluded one and passes keep(local row).  All 32 lanes call it; the warp reserves its records with one atomic (none
+// when no lane has a hit).
+template <class Keep>
 __device__ __forceinline__ void dense_emit(const DenseParams &P, const DenseRangeOut &R, const float (&tv)[8], float inv_q, int q,
-                                           int64_t row0, int c0, int excl) {
+                                           int64_t row0, int c0, int excl, Keep keep) {
   const int lane = threadIdx.x & 31;
   uint32_t hits = 0;
 #pragma unroll
   for (int e = 0; e < 8; e++) {
     const int64_t r = row0 + c0 + 8 * (e >> 2) + 4 * ((e >> 1) & 1) + (e & 1);
-    if (tv[e] * inv_q >= R.thr && r < P.n_rows && (int)r != excl) hits |= 1u << e;
+    if (tv[e] * inv_q >= R.thr && r < P.n_rows && (int)r != excl && keep(r)) hits |= 1u << e;
   }
   const int nh = __popc(hits);
   int incl = nh;  // inclusive prefix sum of the warp's hit counts: lane 31 holds the total
@@ -175,7 +203,11 @@ __device__ __forceinline__ void dense_emit(const DenseParams &P, const DenseRang
 // FILTER: query p only matches rows labelled F.lab_q[p] (-1: any row).  An item whose row tile holds no live row of
 // any label of its query tile (tile_sig & qsig == 0; a signature has no false negatives) is skipped by the producer
 // (no loads) and by the consumers (no MMAs, ring waits or epilogue) alike, so the ring's stage and phase stay in step.
-template <bool RANGE, bool FILTER>
+// TAGS (instantiated with FILTER only): query p also only matches rows whose tag set meets its own; the items whose row
+// tile carries no tag of any query of the tile (tile_tsig & qtsig == 0) are skipped the same way.  An element whose row
+// mask misses the query's gets a NaN scale; when some tag of the index is >= 64 a mask hit is confirmed on the row's
+// tag list (tags_meet) where an element would enter a list or be emitted, the only places its eligibility matters.
+template <bool RANGE, bool FILTER, bool TAGS = false>
 __global__ void __launch_bounds__(N_THREADS, 1)
 dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c, DenseParams P,
                   DenseRangeOut R, DenseFilter F) {
@@ -207,7 +239,7 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
         const int qtile = (int)(L / P.r_tiles);
         const int64_t t = L % P.r_tiles;
         if constexpr (FILTER) {
-          if ((F.tile_sig[t] & F.qsig[qtile]) == 0) { n_skip++; continue; }
+          if (item_skipped<TAGS>(F, t, qtile)) { n_skip++; continue; }
         }
         for (int kb = 0; kb < n_kb; kb++) {
           mbar_wait(&S.empty_bar[stage], phase ^ 1);
@@ -248,6 +280,8 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
     float lo = INFINITY;         // a row enters the list iff its score > lo
     int qlab = -1;               // FILTER: this thread's query label (-1: any row)
     int64_t qo = 0;              // FILTER: the call's index of this thread's query, qperm[q]
+    unsigned long long qtm = 0;  // TAGS: this thread's query mask (0: any row)
+    const int *qtl = nullptr;    // TAGS: its ascending tags
     auto flush = [&]() {    // publish the list of (cur_qtile, this CTA)
       if (cur_qtile < 0 || !q_ok) return;
       const int slot = (int)my_split * 2 + half;
@@ -267,7 +301,7 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
       const int qtile = (int)(L / P.r_tiles);
       const int64_t t = L % P.r_tiles;
       bool skip = false;  // (CTA-uniform) the producer issued no loads for this item
-      if constexpr (FILTER) skip = (F.tile_sig[t] & F.qsig[qtile]) == 0;
+      if constexpr (FILTER) skip = item_skipped<TAGS>(F, t, qtile);
       int prev = -1;
       if (!skip) {
         // ---- MMA over the K slices; a slice's ring slot is released once the next slice's MMAs are issued and the
@@ -304,6 +338,10 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
           qlab = q_ok ? F.lab_q[q] : -1;
           qo = q_ok ? F.qperm[q] : q;
         }
+        if constexpr (TAGS) {
+          qtm = q_ok ? F.q_tmask[q] : 0ull;
+          qtl = F.q_tags + (q_ok ? q : 0) * MAX_QTAGS;
+        }
         {
           const int64_t e = P.excl_base >= 0 ? P.excl_base + (FILTER ? qo : q) - P.row_base : -1;
           excl = (e >= 0 && e < P.n_rows) ? (int)e : -1;
@@ -325,7 +363,11 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
       const int64_t row0 = t * BN;
       for (int c = et; c < BN; c += EPI_THREADS) S.inv_c[as][c] = (row0 + c < P.n_rows) ? P.inv_norm_c[row0 + c] : -INFINITY;  // 0 * -inf = NaN: never a candidate
       if constexpr (FILTER) {
-        for (int c = et; c < BN; c += EPI_THREADS) S.lab_c[as][c] = (row0 + c < P.n_rows) ? F.lab_c[row0 + c] : -1;
+        if (!TAGS || F.lab_c)
+          for (int c = et; c < BN; c += EPI_THREADS) S.lab_c[as][c] = (row0 + c < P.n_rows) ? F.lab_c[row0 + c] : -1;
+      }
+      if constexpr (TAGS) {
+        for (int c = et; c < BN; c += EPI_THREADS) S.tmask_c[as][c] = (row0 + c < P.n_rows) ? F.tmask_c[row0 + c] : 0ull;
       }
       if constexpr (!RANGE) {
         if (q_ok) {
@@ -383,6 +425,16 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
               if (lh.y != qlab) ich.y = __int_as_float(0x7fc00000);
             }
           }
+          if constexpr (TAGS) {
+            if (qtm) {
+              const ulonglong2 ml = *reinterpret_cast<const ulonglong2 *>(&S.tmask_c[as][8 * j + cofs]);
+              const ulonglong2 mh = *reinterpret_cast<const ulonglong2 *>(&S.tmask_c[as][8 * j + 4 + cofs]);
+              if (!(ml.x & qtm)) icl.x = __int_as_float(0x7fc00000);
+              if (!(ml.y & qtm)) icl.y = __int_as_float(0x7fc00000);
+              if (!(mh.x & qtm)) ich.x = __int_as_float(0x7fc00000);
+              if (!(mh.y & qtm)) ich.y = __int_as_float(0x7fc00000);
+            }
+          }
           tv[4 * jj + 0] = acc[4 * j + 0] * icl.x;
           tv[4 * jj + 1] = acc[4 * j + 1] * icl.y;
           tv[4 * jj + 2] = acc[4 * j + 2] * ich.x;
@@ -394,14 +446,19 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
         if constexpr (RANGE) {
           // inv_q > 0 and rounding is monotone, so no score of the group reaches thr unless best does (zero and
           // padded queries have inv_q = 0: best is 0 or NaN)
-          if (__any_sync(FULL_MASK, best >= R.thr)) dense_emit(P, R, tv, inv_q, (int)(FILTER ? qo : q), row0, 16 * sb + cofs, excl);
+          if (__any_sync(FULL_MASK, best >= R.thr)) {
+            if constexpr (TAGS) {
+              dense_emit(P, R, tv, inv_q, (int)qo, row0, 16 * sb + cofs, excl, [&](int64_t r) {
+                return qtm == 0ull || tags_meet(S.tmask_c[as][r - row0], qtm, F.tag_ptr, F.tag_list, r, qtl);
+              });
+            } else {
+              dense_emit(P, R, tv, inv_q, (int)(FILTER ? qo : q), row0, 16 * sb + cofs, excl, [](int64_t) { return true; });
+            }
+          }
         } else {
           if (best > lo) {
-#pragma unroll  // static indices keep tv[] in registers
-            for (int e = 0; e < 8; e++) {
-              const float sc = tv[e] * inv_q;
-              const int col = 8 * (2 * sb + (e >> 2)) + cofs + (e & 1) + 4 * ((e >> 1) & 1);
-              if (sc > lo && (int)(row0 + col) != excl) {
+            if constexpr (TAGS) {
+              auto insert = [&](float sc, int col) {
                 int pos = cnt < k ? cnt++ : k - 1;
                 while (pos > 0 && ls[(pos - 1) * BM] < sc) {
                   ls[pos * BM] = ls[(pos - 1) * BM];
@@ -411,6 +468,44 @@ dense_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
                 ls[pos * BM] = sc;
                 lr[pos * BM] = (int)(row0 + col);
                 if (cnt == k) { thr = ls[(k - 1) * BM]; lo = fmaxf(thr, gth_pred); }
+              };
+              // the group's candidates by score and exclusion; when some tag is >= 64 a rolled loop confirms each on
+              // its row's tag list, so that the list test is compiled once per group, not once per element
+              uint32_t cb = 0;
+#pragma unroll
+              for (int e = 0; e < 8; e++) {
+                const int col = 8 * (2 * sb + (e >> 2)) + cofs + (e & 1) + 4 * ((e >> 1) & 1);
+                if (tv[e] * inv_q > lo && (int)(row0 + col) != excl) cb |= 1u << e;
+              }
+              if (cb && qtm && F.tag_ptr) {
+                for (uint32_t m = cb; m; m &= m - 1) {
+                  const int e = __ffs(m) - 1;
+                  const int col = 8 * (2 * sb + (e >> 2)) + cofs + (e & 1) + 4 * ((e >> 1) & 1);
+                  if (!tags_meet(S.tmask_c[as][col], qtm, F.tag_ptr, F.tag_list, row0 + col, qtl)) cb &= ~(1u << e);
+                }
+              }
+#pragma unroll  // static indices keep tv[] in registers
+              for (int e = 0; e < 8; e++) {
+                const float sc = tv[e] * inv_q;
+                const int col = 8 * (2 * sb + (e >> 2)) + cofs + (e & 1) + 4 * ((e >> 1) & 1);
+                if (((cb >> e) & 1u) && sc > lo) insert(sc, col);  // lo may have risen since cb was formed
+              }
+            } else {
+#pragma unroll  // static indices keep tv[] in registers
+              for (int e = 0; e < 8; e++) {
+                const float sc = tv[e] * inv_q;
+                const int col = 8 * (2 * sb + (e >> 2)) + cofs + (e & 1) + 4 * ((e >> 1) & 1);
+                if (sc > lo && (int)(row0 + col) != excl) {
+                  int pos = cnt < k ? cnt++ : k - 1;
+                  while (pos > 0 && ls[(pos - 1) * BM] < sc) {
+                    ls[pos * BM] = ls[(pos - 1) * BM];
+                    lr[pos * BM] = lr[(pos - 1) * BM];
+                    pos--;
+                  }
+                  ls[pos * BM] = sc;
+                  lr[pos * BM] = (int)(row0 + col);
+                  if (cnt == k) { thr = ls[(k - 1) * BM]; lo = fmaxf(thr, gth_pred); }
+                }
               }
             }
           }
@@ -453,6 +548,18 @@ __global__ void tile_sig_kernel(const int *__restrict__ lab, const float *__rest
   __syncthreads();
   const int64_t r = blockIdx.x * (int64_t)BN + threadIdx.x;
   if (r < n && !isnan(inv_c[r])) atomicOr(&s, 1ull << (lab[r] & 63));
+  __syncthreads();
+  if (threadIdx.x == 0) sig[blockIdx.x] = s;
+}
+
+// the same for the tag filter: OR of the tag masks of the tile's live rows
+__global__ void tile_tag_sig_kernel(const unsigned long long *__restrict__ mask, const float *__restrict__ inv_c, int64_t n,
+                                    unsigned long long *sig) {
+  __shared__ unsigned long long s;
+  if (threadIdx.x == 0) s = 0;
+  __syncthreads();
+  const int64_t r = blockIdx.x * (int64_t)BN + threadIdx.x;
+  if (r < n && !isnan(inv_c[r]) && mask[r]) atomicOr(&s, mask[r]);
   __syncthreads();
   if (threadIdx.x == 0) sig[blockIdx.x] = s;
 }
@@ -505,41 +612,76 @@ struct kv_dense_index {
   DevBuf<unsigned long long> d_qsig, d_skipped;
   DevBuf<__nv_bfloat16> d_qf;  // the filtered call's queries in kernel order (when that order is not the identity)
   int64_t last_skipped = 0, last_items = 0;
+  // row tag sets (kv_dense_set_row_tags), with the lifetime of the row labels: uploaded when set (masks by local row,
+  // and the CSR unless every tag is < 64); the tile tag signatures are rebuilt at every finalize and tag upload
+  bool has_tags = false, tags_exact = true;
+  int64_t tag_rows = 0;  // the row count they were set for
+  DevBuf<unsigned long long> d_tmask_c, d_tile_tsig;
+  DevBuf<int64_t> d_tag_ptr;
+  DevBuf<int> d_tag_list;
+  // tag filter of the next search call (kv_dense_set_tag_filter), by original query, and that call's device inputs
+  std::vector<unsigned long long> h_qtmask;
+  std::vector<int> h_qtlist;
+  bool has_qtags = false;
+  DevBuf<unsigned long long> d_q_tmask, d_qtsig;
+  DevBuf<int> d_q_tags;
 };
 
 namespace {
 
 // A search call's query filter, taken from the handle (which it leaves cleared) and then laid out in kernel order.
 struct CallFilter {
-  bool on = false;               // some query is filtered: the FILTER kernel runs
-  std::vector<int> lab;          // [n_q] by original query
-  std::vector<int64_t> perm;     // [n_q] kernel order -> original query (stable sort by label)
+  bool on = false;               // some query is filtered (label or tags): a FILTER kernel runs
+  bool labels = false;           // some query has a label
+  bool tags = false;             // some query has tags: the TAGS kernel runs
+  std::vector<int> lab;          // [n_q] by original query (all -1 when only tags were given)
+  std::vector<unsigned long long> tmask;  // tags: [n_q] by original query (0: no tag constraint)
+  std::vector<int> tlist;                 // tags: [n_q][MAX_QTAGS] by original query, ascending, -1 past the last
+  std::vector<int64_t> perm;     // [n_q] kernel order -> original query (stable sort by label, then smallest tag)
   bool identity = true;
 };
 
-// Takes (and clears) the handle's query filter for a call of n_q queries.  Caller holds dx->mu.
+// Takes (and clears) the handle's query label and tag filters for a call of n_q queries.  Caller holds dx->mu.
 int take_filter(kv_dense_index *dx, int64_t n_q, const char *fn, CallFilter &cf) {
-  const bool had = dx->has_qfilter;
-  dx->has_qfilter = false;
+  const bool had_lab = dx->has_qfilter, had_tags = dx->has_qtags;
+  dx->has_qfilter = dx->has_qtags = false;
   cf = CallFilter{};
-  if (!had) return KV_OK;
-  cf.lab.swap(dx->h_qfilter);
-  if ((int64_t)cf.lab.size() != n_q)
-    return kv_fail(KV_ERR_INVALID, "%s: the query filter has %lld labels for a call of %lld queries", fn, (long long)cf.lab.size(),
-                   (long long)n_q);
-  for (int l : cf.lab) cf.on = cf.on || l >= 0;
+  if (had_lab) {
+    cf.lab.swap(dx->h_qfilter);
+    if ((int64_t)cf.lab.size() != n_q)
+      return kv_fail(KV_ERR_INVALID, "%s: the query filter has %lld labels for a call of %lld queries", fn, (long long)cf.lab.size(),
+                     (long long)n_q);
+    for (int l : cf.lab) cf.labels = cf.labels || l >= 0;
+  }
+  if (had_tags) {
+    cf.tmask.swap(dx->h_qtmask);
+    cf.tlist.swap(dx->h_qtlist);
+    if ((int64_t)cf.tmask.size() != n_q)
+      return kv_fail(KV_ERR_INVALID, "%s: the tag filter has %lld tag sets for a call of %lld queries", fn, (long long)cf.tmask.size(),
+                     (long long)n_q);
+    for (unsigned long long m : cf.tmask) cf.tags = cf.tags || m != 0ull;
+  }
+  cf.on = cf.labels || cf.tags;
   if (!cf.on) return KV_OK;  // every query unfiltered: the unfiltered call
-  if (!dx->has_labels || (int64_t)dx->h_labels.size() != dx->n_rows)
+  if (cf.labels && (!dx->has_labels || (int64_t)dx->h_labels.size() != dx->n_rows))
     return kv_fail(KV_ERR_STATE, "%s: the index has no row labels for its current rows (kv_dense_set_row_labels)", fn);
+  if (cf.tags && (!dx->has_tags || dx->tag_rows != dx->n_rows))
+    return kv_fail(KV_ERR_STATE, "%s: the index has no row tags for its current rows (kv_dense_set_row_tags)", fn);
+  if (!cf.labels) cf.lab.assign((size_t)n_q, -1);
   cf.perm.resize((size_t)n_q);
   for (int64_t i = 0; i < n_q; i++) cf.perm[(size_t)i] = i;
-  std::stable_sort(cf.perm.begin(), cf.perm.end(), [&](int64_t a, int64_t b) { return cf.lab[(size_t)a] < cf.lab[(size_t)b]; });
+  if (cf.tags) {  // (label, smallest tag): a query tile holds few apps; the queries without tags (-1) lead their label
+    const auto key = [&](int64_t q) { return std::make_pair(cf.lab[(size_t)q], cf.tlist[(size_t)q * MAX_QTAGS]); };
+    std::stable_sort(cf.perm.begin(), cf.perm.end(), [&](int64_t a, int64_t b) { return key(a) < key(b); });
+  } else {
+    std::stable_sort(cf.perm.begin(), cf.perm.end(), [&](int64_t a, int64_t b) { return cf.lab[(size_t)a] < cf.lab[(size_t)b]; });
+  }
   for (int64_t i = 0; i < n_q && cf.identity; i++) cf.identity = cf.perm[(size_t)i] == i;
   return KV_OK;
 }
 
-// What an append of n rows changes besides the rows: the index needs a finalize, the row labels and the query filter
-// are dropped, the deleted rows stay deleted and the new rows are live.
+// What an append of n rows changes besides the rows: the index needs a finalize, the row labels and tags and the query
+// filters are dropped, the deleted rows stay deleted and the new rows are live.
 void dense_rows_appended(kv_dense_index *dx, int64_t n) {
   dx->n_rows += n;
   dx->rows.n = dx->n_rows * dx->dim;
@@ -547,6 +689,8 @@ void dense_rows_appended(kv_dense_index *dx, int64_t n) {
   dx->has_labels = false;
   dx->h_labels.clear();
   dx->has_qfilter = false;
+  dx->has_tags = false;
+  dx->has_qtags = false;
   dx->tomb.extend(dx->n_rows);
 }
 
@@ -557,6 +701,18 @@ int build_tile_sig(kv_dense_index *dx) {
   if (!r_tiles) return KV_OK;
   KV_CUDA(dx->d_tile_sig.ensure(r_tiles));
   tile_sig_kernel<<<(unsigned)r_tiles, BN, 0, dx->stream>>>(dx->d_lab_c.p, dx->d_inv_c.p, dx->n_rows, dx->d_tile_sig.p);
+  KV_CUDA(cudaGetLastError());
+  KV_CUDA(cudaStreamSynchronize(dx->stream));
+  return KV_OK;
+}
+
+// Rebuilds the tile tag signatures from the device tag masks and the inverse norms.  Needs a finalized index with row
+// tags on the device.
+int build_tile_tsig(kv_dense_index *dx) {
+  const int64_t r_tiles = (dx->n_rows + BN - 1) / BN;
+  if (!r_tiles) return KV_OK;
+  KV_CUDA(dx->d_tile_tsig.ensure(r_tiles));
+  tile_tag_sig_kernel<<<(unsigned)r_tiles, BN, 0, dx->stream>>>(dx->d_tmask_c.p, dx->d_inv_c.p, dx->n_rows, dx->d_tile_tsig.p);
   KV_CUDA(cudaGetLastError());
   KV_CUDA(cudaStreamSynchronize(dx->stream));
   return KV_OK;
@@ -595,6 +751,8 @@ int kv_dense_create(int device, int dim, int64_t row_base, kv_dense_index **out)
   KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
   KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
   KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
+  KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
+  KV_CUDA(cudaFuncSetAttribute(dense_topk_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DenseSmem) + 1024));
   *out = dx.release();
   return KV_OK;
 }
@@ -627,7 +785,7 @@ int kv_dense_finalize(kv_dense_index *dx) {
   if (!dx) return kv_fail(KV_ERR_INVALID, "kv_dense_finalize: NULL handle");
   std::lock_guard<std::mutex> g(dx->mu);
   dx->range.drop();
-  dx->has_qfilter = false;
+  dx->has_qfilter = dx->has_qtags = false;
   KV_CUDA(cudaSetDevice(dx->device));
   KV_CUDA(dx->d_inv_c.ensure(std::max<int64_t>(dx->n_rows, 1)));
   if (dx->n_rows) {
@@ -646,6 +804,10 @@ int kv_dense_finalize(kv_dense_index *dx) {
   }
   if (dx->has_labels) {
     const int rc = build_tile_sig(dx);
+    if (rc != KV_OK) return rc;
+  }
+  if (dx->has_tags) {
+    const int rc = build_tile_tsig(dx);
     if (rc != KV_OK) return rc;
   }
   dx->finalized = true;
@@ -704,6 +866,51 @@ int kv_dense_set_query_filter(kv_dense_index *dx, const int32_t *labels, int64_t
       return kv_fail(KV_ERR_INVALID, "kv_dense_set_query_filter: label %d of query %lld is below -1", labels[q], (long long)q);
   dx->h_qfilter.assign(labels, labels + n_q);
   dx->has_qfilter = true;
+  return KV_OK;
+}
+
+int kv_dense_set_row_tags(kv_dense_index *dx, const int64_t *indptr, const int32_t *tags, int64_t n) {
+  const char *fn = "kv_dense_set_row_tags";
+  if (!dx) return kv_fail(KV_ERR_INVALID, "%s: NULL handle", fn);
+  std::lock_guard<std::mutex> g(dx->mu);
+  if (!indptr) {
+    dx->has_tags = false;
+    return KV_OK;
+  }
+  bool exact = true;
+  const int rc = check_row_tags(indptr, tags, n, dx->n_rows, fn, &exact);
+  if (rc != KV_OK) return rc;
+  KV_CUDA(cudaSetDevice(dx->device));
+  dx->has_tags = false;
+  std::vector<unsigned long long> mask((size_t)n, 0ull);
+  for (int64_t r = 0; r < n; r++)
+    for (int64_t i = indptr[r]; i < indptr[r + 1]; i++) mask[(size_t)r] |= 1ull << (tags[i] & 63);
+  cudaStream_t s = dx->stream;
+  KV_CUDA(dx->d_tmask_c.ensure(std::max<int64_t>(n, 1)));
+  if (n) KV_CUDA(cudaMemcpyAsync(dx->d_tmask_c.p, mask.data(), (size_t)n * 8, cudaMemcpyHostToDevice, s));
+  if (!exact) {
+    KV_CUDA(dx->d_tag_ptr.ensure(n + 1));
+    KV_CUDA(dx->d_tag_list.ensure(std::max<int64_t>(indptr[n], 1)));
+    KV_CUDA(cudaMemcpyAsync(dx->d_tag_ptr.p, indptr, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
+    if (indptr[n]) KV_CUDA(cudaMemcpyAsync(dx->d_tag_list.p, tags, (size_t)indptr[n] * sizeof(int), cudaMemcpyHostToDevice, s));
+  }
+  KV_CUDA(cudaStreamSynchronize(s));  // the caller's arrays and the staged masks may go once this returns
+  dx->tags_exact = exact;
+  dx->tag_rows = n;
+  dx->has_tags = true;
+  return dx->finalized ? build_tile_tsig(dx) : KV_OK;  // else the next finalize builds the signatures
+}
+
+int kv_dense_set_tag_filter(kv_dense_index *dx, const int64_t *indptr, const int32_t *tags, int64_t n_q) {
+  const char *fn = "kv_dense_set_tag_filter";
+  if (!dx || n_q < 0) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
+  std::lock_guard<std::mutex> g(dx->mu);
+  dx->has_qtags = false;
+  if (!indptr) return KV_OK;
+  bool any = false;
+  const int rc = parse_query_tag_csr(indptr, tags, n_q, fn, "indptr", dx->h_qtmask, dx->h_qtlist, &any);
+  if (rc != KV_OK) return rc;
+  dx->has_qtags = true;
   return KV_OK;
 }
 
@@ -784,17 +991,41 @@ static int dense_setup(kv_dense_index *dx, const __nv_bfloat16 *d_q, int64_t n_q
     KV_CUDA(cudaMemcpyAsync(dx->d_lab_q.p, lab_q.data(), (size_t)n_q * sizeof(int), cudaMemcpyHostToDevice, s));
     KV_CUDA(cudaMemcpyAsync(dx->d_qsig.p, qsig.data(), (size_t)q_tiles * 8, cudaMemcpyHostToDevice, s));
     KV_CUDA(cudaMemsetAsync(dx->d_skipped.p, 0, 8, s));
-    F.lab_c = dx->d_lab_c.p; F.lab_q = dx->d_lab_q.p; F.qperm = dx->d_qperm.p;
-    F.tile_sig = dx->d_tile_sig.p; F.qsig = dx->d_qsig.p; F.skipped = dx->d_skipped.p;
+    F.lab_q = dx->d_lab_q.p; F.qperm = dx->d_qperm.p;
+    F.qsig = dx->d_qsig.p; F.skipped = dx->d_skipped.p;
+    if (cf.labels) { F.lab_c = dx->d_lab_c.p; F.tile_sig = dx->d_tile_sig.p; }
+  }
+  if (cf.tags) {
+    std::vector<unsigned long long> q_tmask((size_t)n_q), qtsig((size_t)q_tiles, 0ull);
+    std::vector<int> q_tags((size_t)n_q * MAX_QTAGS);
+    for (int64_t p = 0; p < n_q; p++) {
+      const int64_t q = cf.perm[(size_t)p];
+      const unsigned long long m = cf.tmask[(size_t)q];
+      q_tmask[(size_t)p] = m;
+      std::copy_n(cf.tlist.begin() + q * MAX_QTAGS, MAX_QTAGS, q_tags.begin() + p * MAX_QTAGS);
+      qtsig[(size_t)(p / BM)] |= m == 0ull ? ~0ull : m;
+    }
+    KV_CUDA(dx->d_q_tmask.ensure(n_q)); KV_CUDA(dx->d_q_tags.ensure(n_q * MAX_QTAGS)); KV_CUDA(dx->d_qtsig.ensure(q_tiles));
+    KV_CUDA(cudaMemcpyAsync(dx->d_q_tmask.p, q_tmask.data(), (size_t)n_q * 8, cudaMemcpyHostToDevice, s));
+    KV_CUDA(cudaMemcpyAsync(dx->d_q_tags.p, q_tags.data(), q_tags.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    KV_CUDA(cudaMemcpyAsync(dx->d_qtsig.p, qtsig.data(), (size_t)q_tiles * 8, cudaMemcpyHostToDevice, s));
+    KV_CUDA(cudaStreamSynchronize(s));  // the staged vectors go out of scope
+    F.tmask_c = dx->d_tmask_c.p;
+    F.tag_ptr = dx->tags_exact ? nullptr : dx->d_tag_ptr.p;
+    F.tag_list = dx->tags_exact ? nullptr : dx->d_tag_list.p;
+    F.q_tmask = dx->d_q_tmask.p; F.q_tags = dx->d_q_tags.p;
+    F.tile_tsig = dx->d_tile_tsig.p; F.qtsig = dx->d_qtsig.p;
   }
   return KV_OK;
 }
 
-// launches the top-k or the threshold (range) form of K2, filtered when F.qperm is set
+// launches the top-k or the threshold (range) form of K2, filtered when F.qperm is set, tag-filtered when F.q_tmask is
 static void dense_launch(bool range, cudaStream_t s, int64_t grid, const CUtensorMap &map_q, const CUtensorMap &map_c,
                          const DenseParams &P, const DenseRangeOut &R, const DenseFilter &F) {
   const size_t smem = sizeof(DenseSmem) + 1024;
-  if (range && F.qperm) dense_topk_kernel<true, true><<<(unsigned)grid, N_THREADS, smem, s>>>(map_q, map_c, P, R, F);
+  if (range && F.q_tmask) dense_topk_kernel<true, true, true><<<(unsigned)grid, N_THREADS, smem, s>>>(map_q, map_c, P, R, F);
+  else if (F.q_tmask) dense_topk_kernel<false, true, true><<<(unsigned)grid, N_THREADS, smem, s>>>(map_q, map_c, P, R, F);
+  else if (range && F.qperm) dense_topk_kernel<true, true><<<(unsigned)grid, N_THREADS, smem, s>>>(map_q, map_c, P, R, F);
   else if (range) dense_topk_kernel<true, false><<<(unsigned)grid, N_THREADS, smem, s>>>(map_q, map_c, P, R, F);
   else if (F.qperm) dense_topk_kernel<false, true><<<(unsigned)grid, N_THREADS, smem, s>>>(map_q, map_c, P, R, F);
   else dense_topk_kernel<false, false><<<(unsigned)grid, N_THREADS, smem, s>>>(map_q, map_c, P, R, F);

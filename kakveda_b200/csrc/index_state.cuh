@@ -1,12 +1,65 @@
 // Host-side state that both index handles (kv_index in tfidf_index.cu, kv_dense_index in dense_index.cu) keep the same
-// way: the deleted rows and the result of the last threshold search.  Each type owns the rules of its state; what a
-// handle does in reaction (drop a batch, write NaN norms) stays with the handle.
+// way: the deleted rows, the result of the last threshold search and the checks of tag sets.  Each type owns the rules
+// of its state; what a handle does in reaction (drop a batch, write NaN norms) stays with the handle.
 #pragma once
 #include "kv_cuda.cuh"
+#include "tag_sets.cuh"
 
+#include <algorithm>
 #include <cstring>
 #include <type_traits>
 #include <vector>
+
+// Checks a CSR of row tag sets, row r holding t[ip[r] .. ip[r+1]), for an index of n_rows rows (n sets given).
+// *exact: every tag is < 64 (the 64-bit masks are the sets).
+inline int check_row_tags(const int64_t *ip, const int32_t *t, int64_t n, int64_t n_rows, const char *fn, bool *exact) {
+  if (n != n_rows) return kv_fail(KV_ERR_INVALID, "%s: %lld tag sets for an index of %lld rows", fn, (long long)n, (long long)n_rows);
+  if (!ip) return kv_fail(KV_ERR_INVALID, "%s: NULL indptr", fn);
+  if (ip[0] != 0) return kv_fail(KV_ERR_INVALID, "%s: indptr must start at 0", fn);
+  for (int64_t r = 0; r < n; r++)
+    if (ip[r + 1] < ip[r]) return kv_fail(KV_ERR_INVALID, "%s: indptr decreases at row %lld", fn, (long long)r);
+  if (ip[n] > 0 && !t) return kv_fail(KV_ERR_INVALID, "%s: NULL tags", fn);
+  *exact = true;
+  for (int64_t r = 0; r < n; r++)
+    for (int64_t i = ip[r]; i < ip[r + 1]; i++) {
+      if (t[i] < 0) return kv_fail(KV_ERR_INVALID, "%s: tag %d of row %lld is negative", fn, t[i], (long long)r);
+      *exact = *exact && t[i] < 64;
+    }
+  return KV_OK;
+}
+
+// One query's tag set (tags[0, n)) as a mask and an ascending list of MAX_QTAGS slots, -1 past the last tag
+inline int parse_query_tags(const int32_t *t, int64_t n, int64_t q, const char *fn, unsigned long long *mask, int *list) {
+  if (n > MAX_QTAGS) return kv_fail(KV_ERR_INVALID, "%s: query %lld has %lld tags (at most %d)", fn, (long long)q, (long long)n, MAX_QTAGS);
+  std::vector<int> v(t, t + n);
+  for (int x : v)
+    if (x < 0) return kv_fail(KV_ERR_INVALID, "%s: tag %d of query %lld is negative", fn, x, (long long)q);
+  std::sort(v.begin(), v.end());
+  v.erase(std::unique(v.begin(), v.end()), v.end());
+  *mask = 0;
+  for (int j = 0; j < MAX_QTAGS; j++) list[j] = j < (int)v.size() ? v[(size_t)j] : -1;
+  for (int x : v) *mask |= 1ull << (x & 63);
+  return KV_OK;
+}
+
+// The tag sets of n_q queries, CSR ip[n_q+1] / t (parse_query_tags each): mask[n_q] and list[n_q * MAX_QTAGS].
+// `ip_name` names the indptr in the errors.  *any: some query has a tag.
+inline int parse_query_tag_csr(const int64_t *ip, const int32_t *t, int64_t n_q, const char *fn, const char *ip_name,
+                               std::vector<unsigned long long> &mask, std::vector<int> &list, bool *any) {
+  if (ip[0] != 0) return kv_fail(KV_ERR_INVALID, "%s: %s must start at 0", fn, ip_name);
+  mask.assign((size_t)n_q, 0ull);
+  list.assign((size_t)n_q * MAX_QTAGS, -1);
+  *any = false;
+  for (int64_t q = 0; q < n_q; q++) {
+    const int64_t a = ip[q], e = ip[q + 1];
+    if (e < a) return kv_fail(KV_ERR_INVALID, "%s: %s decreases at query %lld", fn, ip_name, (long long)q);
+    if (e > a && !t) return kv_fail(KV_ERR_INVALID, "%s: NULL tags", fn);
+    const int rc = parse_query_tags(t + a, e - a, q, fn, &mask[(size_t)q], &list[(size_t)q * MAX_QTAGS]);
+    if (rc != KV_OK) return rc;
+    *any = *any || mask[(size_t)q] != 0ull;
+  }
+  return KV_OK;
+}
 
 // Deleted rows (tombstones) by local row: no flags until the first deletion, then one per row.  A deleted row keeps
 // its row id; an append extends the flags with live rows.

@@ -76,18 +76,9 @@ struct RowTags {
   DevBuf<int> d_list_pos;
 
   int set(const int64_t *ip, const int32_t *t, int64_t n, int64_t n_rows, const char *fn) {
-    if (n != n_rows) return kv_fail(KV_ERR_INVALID, "%s: %lld tag sets for an index of %lld rows", fn, (long long)n, (long long)n_rows);
-    if (!ip) return kv_fail(KV_ERR_INVALID, "%s: NULL indptr", fn);
-    if (ip[0] != 0) return kv_fail(KV_ERR_INVALID, "%s: indptr must start at 0", fn);
-    for (int64_t r = 0; r < n; r++)
-      if (ip[r + 1] < ip[r]) return kv_fail(KV_ERR_INVALID, "%s: indptr decreases at row %lld", fn, (long long)r);
-    if (ip[n] > 0 && !t) return kv_fail(KV_ERR_INVALID, "%s: NULL tags", fn);
     bool exact = true;
-    for (int64_t r = 0; r < n; r++)
-      for (int64_t i = ip[r]; i < ip[r + 1]; i++) {
-        if (t[i] < 0) return kv_fail(KV_ERR_INVALID, "%s: tag %d of row %lld is negative", fn, t[i], (long long)r);
-        exact = exact && t[i] < 64;
-      }
+    const int rc = check_row_tags(ip, t, n, n_rows, fn, &exact);
+    if (rc != KV_OK) return rc;
     indptr.assign(ip, ip + n + 1);
     tags.assign(t, t + ip[n]);
     masks_exact = exact;
@@ -113,20 +104,6 @@ struct QueryTags {
   DevBuf<unsigned long long> d_mask_orig, d_mask_sorted;
   DevBuf<int> d_tags_orig, d_tags_sorted;
 };
-
-// One query's tag set (tags[0, n)) as a mask and an ascending list of MAX_QTAGS slots, -1 past the last tag
-static int parse_query_tags(const int32_t *t, int64_t n, int64_t q, const char *fn, unsigned long long *mask, int *list) {
-  if (n > MAX_QTAGS) return kv_fail(KV_ERR_INVALID, "%s: query %lld has %lld tags (at most %d)", fn, (long long)q, (long long)n, MAX_QTAGS);
-  std::vector<int> v(t, t + n);
-  for (int x : v)
-    if (x < 0) return kv_fail(KV_ERR_INVALID, "%s: tag %d of query %lld is negative", fn, x, (long long)q);
-  std::sort(v.begin(), v.end());
-  v.erase(std::unique(v.begin(), v.end()), v.end());
-  *mask = 0;
-  for (int j = 0; j < MAX_QTAGS; j++) list[j] = j < (int)v.size() ? v[(size_t)j] : -1;
-  for (int x : v) *mask |= 1ull << (x & 63);
-  return KV_OK;
-}
 
 // The irregular queries of the resident batch (see classify_queries), in sorted-slot order: their original index and
 // CSR on the host, for the float64 full-scan fallback.
@@ -2325,17 +2302,8 @@ static int exact_topk_impl(kv_index *ix, const int64_t *q_indptr, const uint32_t
   std::vector<int> tlist;
   bool tagged = false;
   if (tag_indptr) {
-    if (tag_indptr[0] != 0) return kv_fail(KV_ERR_INVALID, "%s: tag indptr must start at 0", fn);
-    tmask.assign((size_t)n_q, 0ull);
-    tlist.assign((size_t)n_q * MAX_QTAGS, -1);
-    for (int64_t q = 0; q < n_q; q++) {
-      const int64_t a = tag_indptr[q], e = tag_indptr[q + 1];
-      if (e < a) return kv_fail(KV_ERR_INVALID, "%s: tag indptr decreases at query %lld", fn, (long long)q);
-      if (e > a && !tags) return kv_fail(KV_ERR_INVALID, "%s: NULL tags", fn);
-      const int rc = parse_query_tags(tags + a, e - a, q, fn, &tmask[(size_t)q], &tlist[(size_t)q * MAX_QTAGS]);
-      if (rc != KV_OK) return rc;
-      tagged |= tmask[(size_t)q] != 0ull;
-    }
+    const int rc = parse_query_tag_csr(tag_indptr, tags, n_q, fn, "tag indptr", tmask, tlist, &tagged);
+    if (rc != KV_OK) return rc;
   }
   if (ix->n_rows == 0) {
     for (int64_t i = 0; i < n_q * k; i++) { out_rows[i] = -1; out_scores[i] = -INFINITY; }
@@ -2456,18 +2424,11 @@ int kv_query_set_tag_filter(kv_index *ix, const int64_t *indptr, const int32_t *
   if (!indptr) { ix->qtags.on = false; return KV_OK; }
   if (n_q != ix->batch_q)
     return kv_fail(KV_ERR_INVALID, "%s: %lld tag sets for a batch of %lld queries", fn, (long long)n_q, (long long)ix->batch_q);
-  if (indptr[0] != 0) return kv_fail(KV_ERR_INVALID, "%s: indptr must start at 0", fn);
-  std::vector<unsigned long long> mask((size_t)n_q, 0ull);
-  std::vector<int> list((size_t)n_q * MAX_QTAGS, -1);
+  std::vector<unsigned long long> mask;
+  std::vector<int> list;
   bool any = false;
-  for (int64_t q = 0; q < n_q; q++) {
-    const int64_t a = indptr[q], e = indptr[q + 1];
-    if (e < a) return kv_fail(KV_ERR_INVALID, "%s: indptr decreases at query %lld", fn, (long long)q);
-    if (e > a && !tags) return kv_fail(KV_ERR_INVALID, "%s: NULL tags", fn);
-    const int rc = parse_query_tags(tags + a, e - a, q, fn, &mask[(size_t)q], &list[(size_t)q * MAX_QTAGS]);
-    if (rc != KV_OK) return rc;
-    any = any || mask[(size_t)q] != 0ull;
-  }
+  const int prc = parse_query_tag_csr(indptr, tags, n_q, fn, "indptr", mask, list, &any);
+  if (prc != KV_OK) return prc;
   QueryTags &Q = ix->qtags;
   Q.on = false;
   if (!any) return KV_OK;  // no query has tags: the batch without a tag filter

@@ -1008,6 +1008,8 @@ class ShardedDense:
     per-shard partial top-k + K5 merge per batch -- the same exchange as the TF-IDF path, no df all-reduce needed.
     ``allpairs_topk`` makes every stored row a query: the row shards are all-gathered ONCE over NCCL (N x dim bf16,
     1.5 GB at 1M x 768) so that each rank can score all N rows against its shard, each query excluding itself.
+    The label and tag filters need no exchange of their own: every rank keeps its rows' labels and tag sets and filters
+    its own rows; the self-joins pass the global rows' labels and sets as the query filters of each block.
     """
 
     def __init__(self, dim: int, device: int, rank: int = 0, world: int = 1, group=None):
@@ -1018,6 +1020,8 @@ class ShardedDense:
         self.index = None
         self.n_global = 0
         self._local = None
+        self._labels: Optional[np.ndarray] = None                  # set_row_labels, by global row
+        self._tags: Optional[Tuple[np.ndarray, np.ndarray]] = None  # set_row_tags, CSR by global row
 
     def build(self, rows_local, n_global: int) -> None:
         """``rows_local``: this rank's rows, a torch bfloat16 CUDA tensor [n_local, dim] (shard_bounds order)."""
@@ -1028,11 +1032,57 @@ class ShardedDense:
         self.index.add_device(rows_local.contiguous())
         self.index.finalize()
         self._local = rows_local
+        self._labels = self._tags = None
 
-    def topk(self, queries, k: int = 16, exclude_base: int = -1, distinct: bool = False):
-        """queries: torch bfloat16 CUDA [Q, dim], identical on every rank -> ([Q,k] float32, [Q,k] int64) on device."""
+    def set_row_labels(self, global_labels: Optional[np.ndarray]) -> None:
+        """One label >= 0 per GLOBAL row (e.g. a failure-type id), for ``labels=`` / ``same_label=``: this rank keeps
+        its rows' labels.  ``None`` clears.  Call it with the same labels on every rank."""
+        if global_labels is None:
+            self.index.set_row_labels(None)
+            self._labels = None
+            return
+        lab = np.ascontiguousarray(global_labels, dtype=np.int32).reshape(-1)
+        if len(lab) != self.n_global:
+            raise ValueError(f"set_row_labels: {len(lab)} labels for a corpus of {self.n_global} rows")
+        lo, hi = shard_bounds(self.n_global, self.world, self.rank)
+        self.index.set_row_labels(lab[lo:hi])
+        self._labels = lab.copy()
+
+    def set_row_tags(self, global_sets) -> None:
+        """A tag set per GLOBAL row (a list of lists or an ``(indptr, tags)`` pair, as ``DenseIndex.set_row_tags``),
+        for ``tags=`` / ``same_tags=``: this rank keeps its rows' sets.  ``None`` clears.  Call it with the same sets on
+        every rank."""
+        if global_sets is None:
+            self.index.set_row_tags(None)
+            self._tags = None
+            return
+        ip, t = tag_csr(global_sets, self.n_global, "set_row_tags")
+        lo, hi = shard_bounds(self.n_global, self.world, self.rank)
+        self.index.set_row_tags(csr_rows(ip, t, np.arange(lo, hi)))
+        self._tags = (ip.copy(), t.copy())
+
+    def _block_filters(self, b0: int, b1: int, same_label: bool, same_tags: bool):
+        """The query filters of self-join block [b0, b1) of global rows: the rows' own labels and tag sets."""
+        from .denseindex import selfjoin_tags
+
+        labels = tags = None
+        if same_label:
+            if self._labels is None:
+                raise RuntimeError("same_label: the sharded index has no row labels (set_row_labels)")
+            labels = self._labels[b0:b1]
+        if same_tags:
+            if self._tags is None:
+                raise RuntimeError("same_tags: the sharded index has no row tags (set_row_tags)")
+            tags = selfjoin_tags(*self._tags, b0, b1)
+        return labels, tags
+
+    def topk(self, queries, k: int = 16, exclude_base: int = -1, distinct: bool = False,
+             labels: Optional[np.ndarray] = None, tags=None):
+        """queries: torch bfloat16 CUDA [Q, dim], identical on every rank -> ([Q,k] float32, [Q,k] int64) on device.
+        ``labels`` / ``tags``: per query the row label and the tag set its results' rows must carry / meet, as in
+        ``DenseIndex.topk`` (identical on every rank)."""
         no_distinct(distinct, "ShardedDense.topk")
-        s, r = self.index.topk_device(queries.contiguous(), k, exclude_base)
+        s, r = self.index.topk_device(queries.contiguous(), k, exclude_base, labels=labels, tags=tags)
         if self.world == 1:
             return s, r
         gs, gr = gather_topk(s, r, self.group)
@@ -1056,40 +1106,49 @@ class ShardedDense:
             parts.append(full[w * per: w * per + (hi - lo)])
         return torch.cat(parts).contiguous()
 
-    def allpairs_topk(self, k: int = 32, block: int = 262144):
-        """Every row's k nearest OTHER rows over the whole sharded GFKB: ([N,k] float32, [N,k] int64), on every rank."""
+    def allpairs_topk(self, k: int = 32, block: int = 262144, same_label: bool = False, same_tags: bool = False):
+        """Every row's k nearest OTHER rows over the whole sharded GFKB: ([N,k] float32, [N,k] int64), on every rank.
+        ``same_label`` / ``same_tags``: row i's list holds only rows with its label / sharing one of its tags (a row
+        with more than 16 tags raises ValueError), as ``DenseIndex.selfjoin_topk``."""
         import torch
 
         allrows = self.gather_rows()
         out_s, out_r = [], []
         for b0 in range(0, self.n_global, block):
             b1 = min(self.n_global, b0 + block)
-            s, r = self.topk(allrows[b0:b1], k, exclude_base=b0)
+            labels, tags = self._block_filters(b0, b1, same_label, same_tags)
+            s, r = self.topk(allrows[b0:b1], k, exclude_base=b0, labels=labels, tags=tags)
             out_s.append(s)
             out_r.append(r)
         return torch.cat(out_s), torch.cat(out_r)
 
-    def range(self, queries, threshold: float, device_out: bool = True, exclude_base: int = -1):
+    def range(self, queries, threshold: float, device_out: bool = True, exclude_base: int = -1,
+              labels: Optional[np.ndarray] = None, tags=None):
         """Threshold search over the whole sharded GFKB: queries torch bfloat16 CUDA [Q, dim], identical on every rank
         -> ``(indptr int64[Q+1], rows int64[P], scores float32[P])`` as ``DenseIndex.range_device`` returns them (torch
         tensors on the device, or NumPy arrays without ``device_out``); identical on every rank.  ``exclude_base >= 0``:
-        query q never matches GLOBAL row ``exclude_base + q``."""
+        query q never matches GLOBAL row ``exclude_base + q``.  ``labels`` / ``tags`` as in ``topk``."""
         idx = self.index
         queries = queries.contiguous()
         if self.world == 1:
-            return idx.range_device(queries, threshold, exclude_base, device_out)
+            return idx.range_device(queries, threshold, exclude_base, device_out, labels=labels, tags=tags)
         n_q = queries.shape[0]
         with idx._lock:
-            n = idx._range_search_device(queries, threshold, exclude_base)
+            n = idx._range_search_device(queries, threshold, exclude_base, labels, tags)
             gathered, pairs = gather_range_packed(self.device, n_q, n, idx._range_fetch_into, self.group)
         return _host(merge_range_on_device(self.device, gathered, n_q, pairs), device_out)
 
-    def selfjoin_range(self, threshold: float, block: int = 262144, device_out: bool = True):
+    def selfjoin_range(self, threshold: float, block: int = 262144, device_out: bool = True, same_label: bool = False,
+                       same_tags: bool = False):
         """Every row's OTHER rows scoring >= ``threshold`` over the whole sharded GFKB (query i = global row i): the row
-        shards are all-gathered once (``gather_rows``), then blocks of ``block`` rows are searched as in ``range``."""
+        shards are all-gathered once (``gather_rows``), then blocks of ``block`` rows are searched as in ``range``.
+        ``same_label`` / ``same_tags`` as in ``allpairs_topk``."""
         allrows = self.gather_rows()
-        parts = [self.range(allrows[b0:min(self.n_global, b0 + block)], threshold, True, exclude_base=b0)
-                 for b0 in range(0, self.n_global, block)]
+        parts = []
+        for b0 in range(0, self.n_global, block):
+            b1 = min(self.n_global, b0 + block)
+            labels, tags = self._block_filters(b0, b1, same_label, same_tags)
+            parts.append(self.range(allrows[b0:b1], threshold, True, exclude_base=b0, labels=labels, tags=tags))
         if not parts:
             return _host(_devout.empty_range(self.device), device_out)
         return _host(_concat_ranges(parts), device_out)
