@@ -262,6 +262,13 @@ def _host(out, device_out: bool):
     return out if device_out else tuple(t.cpu().numpy() for t in out)
 
 
+def _join_blocks(n_rows: int, block: int, part, device_out: bool, empty):
+    """A self-join of ``n_rows`` rows in query blocks of ``block`` rows: ``part(b0, b1)`` is the CSR result (torch, on
+    the device) of the queries of rows [b0, b1); the blocks' results concatenated, or ``empty()`` without rows."""
+    parts = [part(b0, min(n_rows, b0 + block)) for b0 in range(0, n_rows, block)]
+    return _host(_concat_ranges(parts), device_out) if parts else empty()
+
+
 def merge_exact_lists(rows: np.ndarray, scores: np.ndarray, k: int,
                       groups: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
     """Per query, several ordered lists of (global row, float64 score) side by side ([Q, m] each, -1 rows unused) ->
@@ -291,6 +298,53 @@ def merge_exact_lists(rows: np.ndarray, scores: np.ndarray, k: int,
     return out_r, out_s
 
 
+class _ShardRows:
+    """The global rows one ``ShardedGfkb`` shard holds, and the conversions between them and its index's row ids.
+
+    Without ``row_map`` the shard holds the index range ``[lo, hi)`` and its index has ``row_base = lo``, so the index
+    takes and reports global rows (every row in queries mode or on one GPU).  With ``row_map`` (a text-order shard,
+    ``row_base = 0``) it holds the ascending global rows ``row_map`` lists, the ``[lo, hi)`` range of the text order,
+    and its index numbers them 0, 1, ...; ``row_map_dev`` is the same array on ``device``."""
+
+    def __init__(self, lo: int, hi: int, row_map: Optional[np.ndarray] = None, device=None):
+        import torch
+
+        self.lo, self.hi, self.row_map = lo, hi, row_map
+        self.row_map_dev = None if row_map is None else torch.from_numpy(row_map).to(device)
+
+    def part(self, per_row):
+        """The entries of a per-global-row array for the local rows, in local order."""
+        return per_row[self.lo:self.hi] if self.row_map is None else per_row[self.row_map]
+
+    def local(self, rows: np.ndarray) -> np.ndarray:
+        """Ascending global rows -> the local rows that hold them; the rows of other shards are dropped."""
+        if self.row_map is None:
+            return rows[(rows >= self.lo) & (rows < self.hi)] - self.lo
+        pos = self.index_ids(rows)
+        return pos[pos >= 0]
+
+    def index_ids(self, rows: np.ndarray) -> np.ndarray:
+        """Global rows -> the ids the index takes as global rows (``set_exclusions``); -1 for a row it does not hold."""
+        m = self.row_map
+        if m is None:
+            return rows
+        if not len(m):
+            return np.full_like(rows, -1)
+        pos = np.minimum(np.searchsorted(m, rows), len(m) - 1)
+        return np.where(m[pos] == rows, pos, -1)
+
+    def to_global(self, ids):
+        """Row ids the index reports -> global rows, -1 stays -1 (ascending, so ordered lists stay ordered): a NumPy
+        array is returned mapped, a torch tensor is mapped in place."""
+        if self.row_map is None:
+            return ids
+        if isinstance(ids, np.ndarray):
+            return np.where(ids >= 0, self.row_map[np.clip(ids, 0, None)], -1)
+        import torch
+
+        return ids.copy_(torch.where(ids >= 0, self.row_map_dev[ids.clamp(min=0)], ids))
+
+
 class ShardedGfkb:
     """This rank's share of a GFKB job spread over ``world`` GPUs.
 
@@ -314,6 +368,7 @@ class ShardedGfkb:
         # its rows in ascending global order).  Host-only preparation, no kernel is involved.
         self.order = order
         self.row_map = None
+        self._rows: Optional[_ShardRows] = None   # build_packed: the global rows this shard holds
         self.device, self.rank, self.world, self.group = device, rank, world, group
         self.vocab = Vocabulary()
         self.index: Optional[GfkbIndex] = None
@@ -337,13 +392,14 @@ class ShardedGfkb:
         lo, hi = shard_bounds(fb.n, self.world, self.rank) if self.mode == "rows" else (0, fb.n)
         if self.mode == "rows" and self.order == "text" and self.world > 1:
             sel = shard_rows_by_text(fb, self.world, self.rank, n_threads)
+            self._rows = _ShardRows(lo, hi, sel, f"cuda:{self.device}")
             self.index = GfkbIndex(device=self.device, row_base=0, vocab=self.vocab)
             self.index.add_features(gather_rows(fb, sel, n_threads))
-            self.row_map = torch.from_numpy(sel).to(f"cuda:{self.device}")
-            self._row_map_host = sel
         else:
+            self._rows = _ShardRows(lo, hi)
             self.index = GfkbIndex(device=self.device, row_base=lo, vocab=self.vocab)
             self.index.add_features(fb, lo, hi)
+        self.row_map = self._rows.row_map_dev
         fb.close()
         self._stats = None
         if self.world > 1 and self.mode == "rows":
@@ -390,35 +446,31 @@ class ShardedGfkb:
         dist.barrier(group=self.group)
         self._thr_cap = cap
 
-    def upload(self, qfb: FeatureBatch) -> None:
-        if self.mode == "queries" and self.world > 1:
-            # this rank's slice of the batch: re-pack the CSR rows [lo, hi)
-            lo, hi = shard_bounds(qfb.n, self.world, self.rank)
-            self._qslice = (lo, hi)
+    def set_resident(self, qfb: FeatureBatch) -> None:
+        """Make a featurised batch the resident batch.  In queries mode on several GPUs this rank keeps only its slice
+        of the queries, which is empty when the batch has fewer queries than there are ranks."""
+        q = qfb.n
+        lo, hi = shard_bounds(q, self.world, self.rank) if self.mode == "queries" and self.world > 1 else (0, q)
+        if (lo, hi) == (0, q):
+            self.index.upload_queries(qfb)
+        elif hi > lo:   # this rank's slice of the batch: re-pack the CSR rows [lo, hi)
             self.index._upload(np.ascontiguousarray(qfb.indptr[lo:hi + 1]), qfb.ids, qfb.tf,
                                np.ascontiguousarray(qfb.oov[lo:hi]), hi - lo)
-            return
-        self.index.upload_queries(qfb)
-        self._exchange_thresholds(qfb.n)
+        self._resident_q, self._qslice = q, (lo, hi)
+        self._exchange_thresholds(q)
 
-    def _check_tags(self, tags, q: int):
-        """``tags=`` of a batch of ``q`` queries as CSR, checked before anything is sent (every rank raises the same
-        error); None stays None."""
-        if tags is None:
-            return None
-        ip, t = tag_csr(tags, q, "tags")
-        if len(t) and t.min() < 0:
-            raise ValueError("tags: a negative tag")
-        if q and np.diff(ip).max() > MAX_QUERY_TAGS:
-            raise ValueError(f"tags: a query with more than {MAX_QUERY_TAGS} tags")
-        if not self._has_tags:
-            raise ValueError("tags: the sharded index has no row tags (set_row_tags)")
-        return ip, t
-
-    def _set_modes(self, q: int, labels: Optional[np.ndarray], distinct: bool, tags=None) -> None:
-        """The filters and distinct mode of the resident batch of ``q`` queries, the same on every rank (the threshold
-        exchange relies on it).  The arguments are checked before anything is sent, so every rank raises the same error."""
-        tags = self._check_tags(tags, q)
+    def _check_filters(self, q: int, labels: Optional[np.ndarray], tags, distinct: bool):
+        """``labels=`` / ``tags=`` / ``distinct=`` of a batch of ``q`` queries, checked before anything is sent, so
+        every rank raises the same error: ``(labels int32 or None, tags CSR or None)``."""
+        if tags is not None:
+            tags = tag_csr(tags, q, "tags")
+            ip, t = tags
+            if len(t) and t.min() < 0:
+                raise ValueError("tags: a negative tag")
+            if q and np.diff(ip).max() > MAX_QUERY_TAGS:
+                raise ValueError(f"tags: a query with more than {MAX_QUERY_TAGS} tags")
+            if not self._has_tags:
+                raise ValueError("tags: the sharded index has no row tags (set_row_tags)")
         if labels is not None:
             labels = np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
             if len(labels) != q:
@@ -429,19 +481,17 @@ class ShardedGfkb:
                 raise ValueError("labels: the sharded index has no row labels (set_row_labels)")
         if distinct and not self._has_groups:
             raise ValueError("distinct: the sharded index has no row groups (set_row_groups)")
-        lo, hi = self._qslice if self.mode == "queries" and self.world > 1 else (0, q)
+        return labels, tags
+
+    def _apply_filters(self, labels: Optional[np.ndarray], tags, distinct: bool) -> None:
+        """Checked filters and distinct mode -> this rank's slice of the resident batch, the same on every rank (the
+        threshold exchange relies on it).  A filter not given is cleared, so none carries over from an earlier search."""
+        lo, hi = self._qslice
         if hi > lo:
             self.index.set_filter(None if labels is None else labels[lo:hi])
             self.index.set_tag_filter(None if tags is None else csr_rows(*tags, np.arange(lo, hi)))
             # rows mode on several GPUs runs the two-phase top-k, whose seed lists topk_resident merges group-aware
             self.index.set_distinct(distinct, merged_seeds=self.mode == "rows" and self.world > 1)
-
-    def _to_global(self, r) -> None:
-        """Text-range shard: local rows -> global row ids, in place (-1 stays -1)."""
-        import torch
-
-        if self.row_map is not None:
-            r.copy_(torch.where(r >= 0, self.row_map[r.clamp(min=0)], r))
 
     def topk_resident(self, k: int, labels: Optional[np.ndarray] = None, distinct: bool = False, tags=None):
         """Device-only step on the uploaded batch: local scan+merge, all-gather, global merge.  ``labels``: per query
@@ -452,7 +502,8 @@ class ShardedGfkb:
 
         q = self._resident_q
         dev = f"cuda:{self.device}"
-        self._set_modes(q, labels, distinct, tags)
+        labels, tags = self._check_filters(q, labels, tags, distinct)
+        self._apply_filters(labels, tags, distinct)
         if self.mode == "queries" and self.world > 1:
             import torch.distributed as dist
 
@@ -474,7 +525,7 @@ class ShardedGfkb:
         s, r = packed_views(buf, q, k)
         if self.world == 1:
             self.index.topk_resident(k, s.data_ptr(), r.data_ptr())
-            self._to_global(r)
+            self._rows.to_global(r)
             return s, r
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
         # phase 1: bounds + seed scan on every shard; the shards' seed lists are merged (small all-gather) and the GLOBAL
@@ -493,7 +544,7 @@ class ShardedGfkb:
             torch.cuda.current_stream().synchronize()   # the seed scan writes on the index's own stream
             self.index.topk_resident_seed(k, ss.data_ptr(), sr.data_ptr())
             ev[0].record()
-            self._to_global(sr)
+            self._rows.to_global(sr)
             kth = merge_packed_distinct_on_device(self.device, gather_packed(seed, self.group), q, k,
                                                   self._groups_dev)[0][:, k - 1].contiguous()
         else:
@@ -509,7 +560,7 @@ class ShardedGfkb:
         self.index.raise_thresholds(kth.data_ptr(), q)
         # phase 2: candidate selection + scan, then the exchange of the partial top-k
         self.index.topk_resident_finish(k, s.data_ptr(), r.data_ptr())
-        self._to_global(r)
+        self._rows.to_global(r)
         ev[2].record()
         gathered = gather_packed(buf, self.group)          # the all-gather of the partial top-k
         ev[3].record()
@@ -523,10 +574,6 @@ class ShardedGfkb:
         torch.cuda.current_stream().synchronize()
         self.last_exchange_ms = (ev[2].elapsed_time(ev[3]), ev[3].elapsed_time(ev[4]), ev[0].elapsed_time(ev[1]))
         return out
-
-    def set_resident(self, qfb: FeatureBatch) -> None:
-        self.upload(qfb)
-        self._resident_q = qfb.n
 
     # ---- sharded preparation of a query batch (rows mode, world > 1) -------------------------------------------------
     @staticmethod
@@ -600,7 +647,7 @@ class ShardedGfkb:
             if got != n_q:
                 raise RuntimeError(f"query-slice exchange: {got} queries assembled, {n_q} expected")
             self._exchange_thresholds(n_q)
-            self._resident_q = n_q
+            self._resident_q, self._qslice = n_q, (0, n_q)
             t3 = time.perf_counter()
             self.last_prepare_split_ms = {"featurize_slice": 1e3 * (t1 - t0), "slice_order_and_exchange": 1e3 * (t2 - t1),
                                           "assemble_and_upload": 1e3 * (t3 - t2),
@@ -634,77 +681,43 @@ class ShardedGfkb:
         ``labels`` / ``distinct`` / ``tags`` as for ``topk_resident``."""
         import time
 
+        import torch
+
         t0 = time.perf_counter()
-        if self.world > 1 and self.mode == "rows" and os.environ.get("KAKVEDA_B200_NO_SLICED_PREP") != "1":
-            import torch
-
-            self.upload_text_sharded(data, offsets, mode)
-            t2 = time.perf_counter()
-            s, r = self.topk_resident(k, labels, distinct, tags)
-            torch.cuda.current_stream().synchronize()
-            t3 = time.perf_counter()
-            out = self._read_back(s, r)
-            t4 = time.perf_counter()
-            self.last_e2e_ms = {"prepare_sharded": 1e3 * (t2 - t0), "device_step": 1e3 * (t3 - t2), "read_back": 1e3 * (t4 - t3),
-                                "prepare_split": self.last_prepare_split_ms}
-            return out
         n_q = len(offsets) - 1
-        if self.world == 1 and n_q and _featurize_on_device(n_q):
-            import torch
-
-            self.index.upload_text(data, offsets, mode)   # featurise, classify and order on the device
-            self._resident_q = n_q
-            t2 = time.perf_counter()
-            s, r = self.topk_resident(k, labels, distinct, tags)
-            torch.cuda.current_stream().synchronize()
-            t3 = time.perf_counter()
-            out = self._read_back(s, r)
-            t4 = time.perf_counter()
-            prep = self.index.last_prepare_ms()  # text upload + featurisation, classification, order, tables + copies
-            self.last_e2e_ms = {"featurize": prep[0], "upload": 1e3 * (t2 - t0) - prep[0], "device_step": 1e3 * (t3 - t2),
-                                "read_back": 1e3 * (t4 - t3), "upload_device_ms": prep}
-            return out
-        qfb = self.vocab.featurize_packed(data, offsets, mode, grow=False)
+        sliced = self.world > 1 and self.mode == "rows" and os.environ.get("KAKVEDA_B200_NO_SLICED_PREP") != "1"
+        qfb = None
         try:
-            t1 = time.perf_counter()
-            self.set_resident(qfb)
+            if sliced:
+                self.upload_text_sharded(data, offsets, mode)
+            elif self.world == 1 and n_q and _featurize_on_device(n_q):
+                self.index.upload_text(data, offsets, mode)   # featurise, classify and order on the device
+                self._resident_q, self._qslice = n_q, (0, n_q)
+            else:
+                qfb = self.vocab.featurize_packed(data, offsets, mode, grow=False)
+                t1 = time.perf_counter()
+                self.set_resident(qfb)
             t2 = time.perf_counter()
             s, r = self.topk_resident(k, labels, distinct, tags)
-            import torch
-
             torch.cuda.current_stream().synchronize()
             t3 = time.perf_counter()
             out = self._read_back(s, r)
             t4 = time.perf_counter()
-            self.last_e2e_ms = {"featurize": 1e3 * (t1 - t0), "upload": 1e3 * (t2 - t1), "device_step": 1e3 * (t3 - t2),
-                                "read_back": 1e3 * (t4 - t3),
-                                "upload_host_ms": self.index.last_prepare_ms()}  # staging, classification, order, copies+tables
-            return out
         finally:
-            qfb.close()
+            if qfb is not None:
+                qfb.close()
+        step = {"device_step": 1e3 * (t3 - t2), "read_back": 1e3 * (t4 - t3)}
+        if sliced:
+            self.last_e2e_ms = {"prepare_sharded": 1e3 * (t2 - t0), **step, "prepare_split": self.last_prepare_split_ms}
+        elif qfb is None:
+            prep = self.index.last_prepare_ms()  # text upload + featurisation, classification, order, tables + copies
+            self.last_e2e_ms = {"featurize": prep[0], "upload": 1e3 * (t2 - t0) - prep[0], **step, "upload_device_ms": prep}
+        else:
+            self.last_e2e_ms = {"featurize": 1e3 * (t1 - t0), "upload": 1e3 * (t2 - t1), **step,
+                                "upload_host_ms": self.index.last_prepare_ms()}  # staging, classification, order, copies+tables
+        return out
 
     # ---- threshold search ------------------------------------------------------------------------------------------
-    def _local_part(self, per_row: np.ndarray) -> np.ndarray:
-        """The entries of this shard's rows of a per-global-row array: by index range, through ``row_map`` for a
-        text-order shard, all of them in queries mode."""
-        if self.row_map is not None:
-            return per_row[self._row_map_host]
-        if self.mode == "rows":
-            lo, hi = shard_bounds(self.n_global, self.world, self.rank)
-            return per_row[lo:hi]
-        return per_row
-
-    def _local_rows(self, rows: np.ndarray) -> np.ndarray:
-        """Ascending global rows -> the local rows of this shard that hold them (the others are dropped)."""
-        if self.row_map is not None:
-            m = self._row_map_host
-            pos = np.minimum(np.searchsorted(m, rows), max(len(m) - 1, 0))
-            return pos[m[pos] == rows] if len(m) else rows[:0]
-        if self.mode == "rows":
-            lo, hi = shard_bounds(self.n_global, self.world, self.rank)
-            return rows[(rows >= lo) & (rows < hi)] - lo
-        return rows
-
     def set_row_labels(self, global_labels: Optional[np.ndarray]) -> None:
         """One label >= 0 per GLOBAL row (e.g. a failure-type id): this shard keeps its rows' labels (by index range, or
         through ``row_map`` for a text-order shard), for ``labels=`` of the top-k and threshold searches.  ``None``
@@ -716,7 +729,7 @@ class ShardedGfkb:
         lab = np.ascontiguousarray(global_labels, dtype=np.int32)
         if len(lab) != self.n_global:
             raise ValueError(f"set_row_labels: {len(lab)} labels for a corpus of {self.n_global} rows")
-        self.index.set_row_labels(self._local_part(lab))
+        self.index.set_row_labels(self._rows.part(lab))
         self._has_labels = True
 
     def set_row_tags(self, global_sets) -> None:
@@ -728,13 +741,7 @@ class ShardedGfkb:
             self._has_tags = False
             return
         ip, t = tag_csr(global_sets, self.n_global, "set_row_tags")
-        if self.row_map is not None:
-            sel = self._row_map_host
-        elif self.mode == "rows":
-            sel = np.arange(*shard_bounds(self.n_global, self.world, self.rank))
-        else:
-            sel = np.arange(self.n_global)
-        self.index.set_row_tags(csr_rows(ip, t, sel))
+        self.index.set_row_tags(csr_rows(ip, t, self._rows.part(np.arange(self.n_global))))
         self._has_tags = True
 
     def set_row_groups(self, global_groups: Optional[np.ndarray]) -> None:
@@ -753,7 +760,7 @@ class ShardedGfkb:
             raise ValueError(f"set_row_groups: {len(grp)} groups for a corpus of {self.n_global} rows")
         if len(grp) and grp.min() < 0:
             raise ValueError("set_row_groups: a negative group")
-        self.index.set_row_groups(self._local_part(grp))
+        self.index.set_row_groups(self._rows.part(grp))
         self._has_groups = True
         self._groups_host = grp
         self._groups_dev = torch.from_numpy(grp).to(f"cuda:{self.device}") if self.mode == "rows" and self.world > 1 else None
@@ -817,14 +824,12 @@ class ShardedGfkb:
         outside the corpus raise ValueError on every rank before anything is deleted.  The resident batch is dropped.
         ``extra_df`` / ``extra_rows``: the statistics of an extra segment, as for ``set_statistics``, added in the same
         refresh (one all-reduce for the whole deletion); the call then returns what ``set_statistics`` returns."""
-        import torch
-
         rows = np.unique(np.ascontiguousarray(global_rows, dtype=np.int64).reshape(-1))
         if len(rows) and (rows[0] < 0 or rows[-1] >= self.n_global):
             bad = rows[0] if rows[0] < 0 else rows[-1]
             raise ValueError(f"delete_rows: row {bad} outside the corpus of {self.n_global} rows")
         extra = self._check_extra(extra_df, extra_rows)
-        local = self._local_rows(rows)
+        local = self._rows.local(rows)
         if len(local):
             self.index.delete_rows(local)
         self._stats = None
@@ -833,11 +838,8 @@ class ShardedGfkb:
             out = self._set_stats(extra, int(extra_rows))
         else:
             if self.world > 1 and self.mode == "rows":
-                cnt = torch.from_numpy(np.append(self.index.local_df().astype(np.int64), self.index.n_live_rows)).to(f"cuda:{self.device}")
-                allreduce_df(cnt, self.group)
-                cnt = cnt.cpu().numpy()
-                self._stats = (cnt[:-1], int(cnt[-1]))
-                self.index.set_global_df(cnt[:-1].astype(np.uint32), int(cnt[-1]))
+                df, n = self._reduce_stats()
+                self.index.set_global_df(df.astype(np.uint32), n)
             self.index.finalize()
         if self._deleted is None:
             self._deleted = np.zeros(self.n_global, dtype=bool)
@@ -867,20 +869,9 @@ class ShardedGfkb:
         q = qfb.n
         if not 1 <= k <= 32:
             raise ValueError(f"exact_topk: k must be 1..32, not {k}")
-        if labels is not None:
-            labels = np.ascontiguousarray(labels, dtype=np.int32).reshape(-1)
-            if len(labels) != q:
-                raise ValueError(f"labels: {len(labels)} labels for a batch of {q} queries")
-            if q and labels.min() < -1:
-                raise ValueError("labels: a label below -1")
-            if not self._has_labels:
-                raise ValueError("labels: the sharded index has no row labels (set_row_labels)")
-        if distinct and not self._has_groups:
-            raise ValueError("distinct: the sharded index has no row groups (set_row_groups)")
-        tags = self._check_tags(tags, q)
+        labels, tags = self._check_filters(q, labels, tags, distinct)
         rows, scores = self.index.exact_topk(qfb, k, labels, distinct, tags)
-        if self.row_map is not None:   # text-range shard: local -> global rows (ascending, so ties keep their order)
-            rows = np.where(rows >= 0, self._row_map_host[np.clip(rows, 0, None)], -1)
+        rows = self._rows.to_global(rows)
         if self.world == 1 or self.mode != "rows":
             return rows, scores
         dev = f"cuda:{self.device}"
@@ -900,34 +891,20 @@ class ShardedGfkb:
             self.index.close()
             self.index = None
 
-    def _set_resident_range(self, qfb: FeatureBatch) -> None:
-        """``set_resident`` that also takes a batch whose queries-mode slice on this rank is empty."""
-        if self.mode == "queries" and self.world > 1:
-            lo, hi = shard_bounds(qfb.n, self.world, self.rank)
-            self._qslice = (lo, hi)
-            self._resident_q = qfb.n
-            if hi > lo:
-                self.upload(qfb)
-            return
-        self.set_resident(qfb)
-
-    def _empty_range(self, device_out: bool):
-        return self.index._empty_range(device_out)
-
     def range_resident(self, threshold: float, device_out: bool = False, labels: Optional[np.ndarray] = None, tags=None):
         """Threshold search of the resident batch over the whole sharded corpus: ``(indptr int64[n_q+1], rows int64[P],
         scores float32[P])`` as ``GfkbIndex.range`` returns them (global rows, each query's pairs by (score desc, row
         asc)), NumPy arrays or with ``device_out`` torch tensors on this rank's device; identical on every rank.
         ``labels``: per query the row label its pairs must carry (-1: any row; ``set_row_labels``).  ``tags``: per query
-        a tag set its pairs' rows must meet (``set_row_tags``).  Every shard searches its rows alone (the threshold is
-        fixed); one all-gather of the results and the device merge follow."""
+        a tag set its pairs' rows must meet (``set_row_tags``).  A search applies exactly the filters it is given: none
+        carries over from an earlier search of the same batch.  Bad arguments raise ValueError on every rank before
+        anything is exchanged.  Every shard searches its rows alone (the threshold is fixed); one all-gather of the
+        results and the device merge follow.  In queries mode a rank whose slice of the batch is empty (a batch with
+        fewer queries than ranks) contributes no pairs."""
         q = self._resident_q
-        lo, hi = self._qslice if self.mode == "queries" and self.world > 1 else (0, q)
-        tags = self._check_tags(tags, q)
-        if labels is not None and hi > lo:
-            self.index.set_filter(np.ascontiguousarray(labels, dtype=np.int32)[lo:hi])
-        if tags is not None and hi > lo:
-            self.index.set_tag_filter(csr_rows(*tags, np.arange(lo, hi)))
+        lo, hi = self._qslice
+        labels, tags = self._check_filters(q, labels, tags, False)
+        self._apply_filters(labels, tags, False)
         if self.world == 1:
             return self.index._range_resident(q, threshold, device_out)
         n = self.index._range_search(threshold) if hi > lo else 0
@@ -941,11 +918,22 @@ class ShardedGfkb:
             self.index._range_fetch_into([ip[lo:hi + 1]] + views[1:])
             ip[:lo] = 0
             ip[hi + 1:] = n
-            if self.row_map is not None:   # text-range shard: local -> global rows (ascending, so segments stay ordered)
-                views[1].copy_(self.row_map[views[1]])
+            self._rows.to_global(views[1])
 
         gathered, pairs = gather_range_packed(self.device, q, n, fill, self.group)
         return _host(merge_range_on_device(self.device, gathered, q, pairs), device_out)
+
+    def _set_resident_text(self, data, offsets: np.ndarray, mode: int) -> None:
+        """A batch of host text as the resident batch of a threshold search: ``upload_text_sharded`` in rows mode on
+        several GPUs, host featurisation and ``set_resident`` otherwise."""
+        if self.world > 1 and self.mode == "rows":
+            self.upload_text_sharded(data, offsets, mode)
+            return
+        qfb = self.vocab.featurize_packed(data, offsets, mode, grow=False)
+        try:
+            self.set_resident(qfb)
+        finally:
+            qfb.close()
 
     def range_packed(self, data, offsets: np.ndarray, threshold: float, mode: int = 0, labels: Optional[np.ndarray] = None,
                      device_out: bool = False, tags=None):
@@ -953,15 +941,8 @@ class ShardedGfkb:
         prepares the batch with ``upload_text_sharded``."""
         offsets = np.ascontiguousarray(offsets, dtype=np.int64)
         if len(offsets) <= 1:
-            return self._empty_range(device_out)
-        if self.world > 1 and self.mode == "rows":
-            self.upload_text_sharded(data, offsets, mode)
-        else:
-            qfb = self.vocab.featurize_packed(data, offsets, mode, grow=False)
-            try:
-                self._set_resident_range(qfb)
-            finally:
-                qfb.close()
+            return self.index._empty_range(device_out)
+        self._set_resident_text(data, offsets, mode)
         return self.range_resident(threshold, device_out, labels, tags)
 
     def selfjoin_range(self, threshold: float, device_out: bool = False, block: int = 262144):
@@ -973,32 +954,18 @@ class ShardedGfkb:
         if self.world == 1:
             return self.index.selfjoin_range(threshold, device_out=device_out)
         data, off, mode = self._corpus
-        parts = []
-        for b0 in range(0, self.n_global, block):
-            b1 = min(self.n_global, b0 + block)
-            if self.mode == "rows":
-                self.upload_text_sharded(data, off[b0:b1 + 1], mode)
-                lo, hi = 0, b1 - b0
-            else:
-                qfb = self.vocab.featurize_packed(data, off[b0:b1 + 1], mode, grow=False)
-                try:
-                    self._set_resident_range(qfb)
-                finally:
-                    qfb.close()
-                lo, hi = self._qslice
+
+        def part(b0: int, b1: int):
+            self._set_resident_text(data, off[b0:b1 + 1], mode)
+            lo, hi = self._qslice
             if hi > lo:
-                excl = np.arange(b0 + lo, b0 + hi, dtype=np.int64)
-                if self.row_map is not None:   # global -> local row of this text-range shard (row_base 0), -1 elsewhere
-                    pos = np.minimum(np.searchsorted(self._row_map_host, excl), max(len(self._row_map_host) - 1, 0))
-                    excl = np.where(self._row_map_host[pos] == excl, pos, -1) if len(self._row_map_host) else np.full_like(excl, -1)
-                self.index.set_exclusions(excl)
-            part = self.range_resident(threshold, device_out=True)
+                self.index.set_exclusions(self._rows.index_ids(np.arange(b0 + lo, b0 + hi, dtype=np.int64)))
+            res = self.range_resident(threshold, device_out=True)
             if self._deleted is not None:   # a deleted row's query has no pairs, as in GfkbIndex.selfjoin_range
-                part = _drop_queries(part, self._deleted[b0:b1])
-            parts.append(part)
-        if not parts:
-            return self._empty_range(device_out)
-        return _host(_concat_ranges(parts), device_out)
+                res = _drop_queries(res, self._deleted[b0:b1])
+            return res
+
+        return _join_blocks(self.n_global, block, part, device_out, lambda: self.index._empty_range(device_out))
 
 
 class ShardedDense:
@@ -1144,14 +1111,12 @@ class ShardedDense:
         shards are all-gathered once (``gather_rows``), then blocks of ``block`` rows are searched as in ``range``.
         ``same_label`` / ``same_tags`` as in ``allpairs_topk``."""
         allrows = self.gather_rows()
-        parts = []
-        for b0 in range(0, self.n_global, block):
-            b1 = min(self.n_global, b0 + block)
+
+        def part(b0: int, b1: int):
             labels, tags = self._block_filters(b0, b1, same_label, same_tags)
-            parts.append(self.range(allrows[b0:b1], threshold, True, exclude_base=b0, labels=labels, tags=tags))
-        if not parts:
-            return _host(_devout.empty_range(self.device), device_out)
-        return _host(_concat_ranges(parts), device_out)
+            return self.range(allrows[b0:b1], threshold, True, exclude_base=b0, labels=labels, tags=tags)
+
+        return _join_blocks(self.n_global, block, part, device_out, lambda: _host(_devout.empty_range(self.device), device_out))
 
 
 class ShardedJaccard:
@@ -1238,14 +1203,10 @@ class ShardedJaccard:
         if self.world == 1:
             return self.index.selfjoin_range(threshold, device_out=device_out)
         ip, ids = self._csr
-        parts = []
-        for b0 in range(0, self.n_global, block):
-            b1 = min(self.n_global, b0 + block)
-            parts.append(self._range_csr(ip[b0:b1 + 1] - ip[b0], ids[ip[b0]:ip[b1]], threshold,
-                                         np.arange(b0, b1, dtype=np.int64), True))
-        if not parts:
-            return self.index._empty_range(device_out)
-        return _host(_concat_ranges(parts), device_out)
+        return _join_blocks(self.n_global, block,
+                            lambda b0, b1: self._range_csr(ip[b0:b1 + 1] - ip[b0], ids[ip[b0]:ip[b1]], threshold,
+                                                           np.arange(b0, b1, dtype=np.int64), True),
+                            device_out, lambda: self.index._empty_range(device_out))
 
 
 class ShardedGfkbStore(GfkbStore):
@@ -1311,13 +1272,21 @@ class ShardedGfkbStore(GfkbStore):
         self._main = main
         main.build_packed(*pack_texts(texts))
 
-    def _refresh_statistics(self) -> None:
+    def _global_statistics(self, main_rows: Optional[np.ndarray] = None) -> None:
+        """The main shards' and the tail's live statistics -> every main shard and the tail, by statistics-only
+        finalizes; ``main_rows``: main rows deleted in the same exchange."""
         tail = self._tail
-        extra = (tail.local_df(), tail.n_live_rows) if tail is not None else (None, 0)
-        df, n = self._main.set_statistics(*extra)
+        extra = (tail.local_df(), tail.n_live_rows) if tail is not None else (np.zeros(0, np.int64), 0)
+        if main_rows is not None and len(main_rows):   # the deletion's all-reduce carries the refreshed statistics
+            df, n = self._main.delete_rows(main_rows, *extra)
+        else:                                           # the cached main statistics serve
+            df, n = self._main.set_statistics(*extra)
         if tail is not None:
             tail.set_global_df(df.astype(np.uint32), n)
             tail.finalize()
+
+    def _refresh_statistics(self) -> None:
+        self._global_statistics()
         self.stats["stat_refreshes" if self._main.index.last_finalize_kind == 2 else "full_rebuilds"] += 1
 
     def _delete_dev_rows(self, gone: np.ndarray) -> bool:
@@ -1327,14 +1296,7 @@ class ShardedGfkbStore(GfkbStore):
         tail = self._tail
         if tail is not None and len(gone) > len(main_rows):
             tail.delete_rows(gone[gone >= self._n_main] - self._n_main)
-        extra = (tail.local_df(), tail.n_live_rows) if tail is not None else (np.zeros(0, np.int64), 0)
-        if len(main_rows):   # the deletion's all-reduce carries the refreshed statistics
-            df, n = self._main.delete_rows(main_rows, *extra)
-        else:                # only tail rows went: the cached main statistics serve
-            df, n = self._main.set_statistics(*extra)
-        if tail is not None:
-            tail.set_global_df(df.astype(np.uint32), n)
-            tail.finalize()
+        self._global_statistics(main_rows)
         self.stats["stat_refreshes"] += 1
         return False
 

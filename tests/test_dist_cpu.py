@@ -141,6 +141,59 @@ def test_text_range_sharding_host_side(built_lib):
         gather_rows(fb, np.array([fb.n], dtype=np.int64))
 
 
+@pytest.mark.parametrize("layout", ["index", "text", "all"])
+def test_shard_rows_conversions(built_lib, layout):
+    """The rows a ``ShardedGfkb`` shard holds (dist._ShardRows) for each layout: an index range (rows mode), a range of
+    the text order (``row_map``) and every row (queries mode).  ``part``, ``local``, ``index_ids`` and ``to_global``
+    agree with each other and with ``shard_bounds`` / ``shard_rows_by_text``; the index-range and text-order shards
+    partition the rows."""
+    from kakveda_b200 import synth
+    from kakveda_b200.dist import _ShardRows, shard_bounds, shard_rows_by_text
+    from kakveda_b200.similarity import Vocabulary
+
+    v = Vocabulary()
+    for n_texts, world in ((997, 3), (40, 8)):
+        texts = synth.corpus(n_texts)
+        fb = v.featurize(texts + texts[:5], grow=True)   # duplicates: equal texts, consecutive in the text order
+        n = fb.n
+        rng = np.random.default_rng(n)
+        per_row = rng.integers(0, 1000, n)
+        probe = np.unique(rng.integers(0, n, n // 2))     # ascending global rows
+        owner = np.full(n, -1)
+        for rank in range(world):
+            lo, hi = shard_bounds(n, world, rank)
+            if layout == "index":
+                rows, held, base = _ShardRows(lo, hi), np.arange(lo, hi), lo
+            elif layout == "text":
+                held = shard_rows_by_text(fb, world, rank)
+                rows, base = _ShardRows(lo, hi, held, "cpu"), 0
+            else:
+                rows, held, base = _ShardRows(0, n), np.arange(n), 0
+            assert len(held) == hi - lo or layout == "all"
+            np.testing.assert_array_equal(rows.part(np.arange(n)), held)
+            np.testing.assert_array_equal(rows.part(per_row), per_row[held])
+            mine = probe[np.isin(probe, held)]
+            pos = np.searchsorted(held, mine)
+            np.testing.assert_array_equal(rows.local(probe), pos)
+            ids = rows.index_ids(probe)
+            if layout == "text":                          # local positions, -1 for rows of other shards
+                np.testing.assert_array_equal(ids, np.where(np.isin(probe, held), np.searchsorted(held, probe), -1))
+            else:                                         # the index takes global rows (row_base = lo)
+                np.testing.assert_array_equal(ids, probe)
+            # what the index reports for its rows (local row + row_base), and -1, back to global rows
+            reported = np.concatenate([pos + base, [-1]]).astype(np.int64)
+            want = np.concatenate([mine, [-1]])
+            np.testing.assert_array_equal(rows.to_global(reported.copy()), want)
+            t = torch.from_numpy(reported.copy())
+            assert rows.to_global(t) is t and t.tolist() == want.tolist()
+            np.testing.assert_array_equal(rows.to_global(ids[ids >= 0]), probe[ids >= 0])
+            if layout != "all":
+                assert (owner[held] == -1).all()
+                owner[held] = rank
+        assert layout == "all" or (owner >= 0).all()
+        fb.close()
+
+
 def test_query_slice_exchange_layout_is_aligned_and_disjoint():
     """Byte layout of one rank's slot in the query-slice all-gather (ShardedGfkb.upload_text_sharded): sections in
     order, 16-byte aligned, large enough for the capacities, nothing overlapping."""

@@ -24,7 +24,7 @@ import torch.distributed as tdist  # noqa: E402
 from test_gpu_scale_oracle import RTOL32, check_topk_device  # noqa: E402
 from test_gpu_shard_loopback import (TIMEOUT, Corpus, _close, _copy, _link, build_sharded, crafted_texts, lib,  # noqa: E402,F401
                                      loopback, merge_numpy, run_ranks, synth_corpus, synth_texts)
-from test_gpu_shard_range import _flags, _np  # noqa: E402
+from test_gpu_shard_range import _check_range, _flags, _np, _single_range  # noqa: E402
 
 gpu = pytest.mark.gpu
 
@@ -502,36 +502,44 @@ def test_delete_rows_equals_single_index(lib, loopback, mode, order, world):
 @pytest.mark.parametrize("mode,world", [("rows", 3), ("queries", 2)])
 def test_mode_errors_raise_on_every_rank(synth_corpus, loopback, mode, world):
     """Distinct without ``set_row_groups``, labels of the wrong length or without ``set_row_labels``: the same
-    ValueError on every rank, and the sharded index still answers afterwards."""
+    ValueError on every rank, from the top-k and (labels) from the threshold search, and the sharded index still
+    answers both afterwards."""
     c = synth_corpus
     build = build_sharded(world, "index", mode, c)
-    nq = len(c.queries)
+    nq, thr = len(c.queries), 0.6
 
     def fn(r, g):
         sh = build(r, g)
+        topk = lambda **kw: sh.topk_packed(c.qdata, c.qoff, 8, c.qmode, **kw)
+        search = lambda **kw: sh.range_packed(c.qdata, c.qoff, thr, c.qmode, **kw)
         try:
             msgs = []
-            for kw in (dict(distinct=True), dict(labels=np.full(nq, -1, np.int32))):
+            for call, kw in ((topk, dict(distinct=True)), (topk, dict(labels=np.full(nq, -1, np.int32))),
+                             (search, dict(labels=np.full(nq, -1, np.int32)))):
                 with pytest.raises(ValueError) as e:
-                    sh.topk_packed(c.qdata, c.qoff, 8, c.qmode, **kw)
+                    call(**kw)
                 msgs.append(str(e.value))
             sh.set_row_labels(np.zeros(c.n, np.int32))
             for lab in (np.zeros(nq - 1, np.int32), np.full(nq, -2, np.int32)):
-                with pytest.raises(ValueError) as e:
-                    sh.topk_packed(c.qdata, c.qoff, 8, c.qmode, labels=lab)
-                msgs.append(str(e.value))
+                for call in (topk, search):
+                    with pytest.raises(ValueError) as e:
+                        call(labels=lab)
+                    msgs.append(str(e.value))
             with pytest.raises(ValueError):
                 sh.set_row_groups(np.zeros(c.n - 1, np.int32))
-            s, rr = sh.topk_packed(c.qdata, c.qoff, 8, c.qmode)
-            return msgs, _copy(s), _copy(rr)
+            s, rr = topk()
+            return msgs, _copy(s), _copy(rr), _np(search())
         finally:
             _close([sh])
 
     out = run_ranks(world, fn)
     for o in out[1:]:
         assert o[0] == out[0][0]
-    assert "set_row_groups" in out[0][0][0] and "set_row_labels" in out[0][0][1]
+    msgs = out[0][0]
+    assert "set_row_groups" in msgs[0] and "set_row_labels" in msgs[1]
+    assert msgs[1] == msgs[2] and msgs[3] == msgs[4] and msgs[5] == msgs[6], msgs
     c.check(f"{mode} W={world} after errors", out[0][1], out[0][2], 8)
+    _check_range(c, f"{mode} W={world} after errors", out[0][3], thr, _single_range(c, thr))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
