@@ -341,6 +341,37 @@ int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores, 
  * ordering's scratch -- about the pair buffer's size again -- does not fit; the result then stays for another try. */
 int kv_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores, void *d_inter, void *d_uni);
 
+/* The relative margin of the exact threshold search's float32 stage.  It rests on the assumption the store's
+ * candidate check (AMBIGUITY_RTOL) makes too: the float32 score of a pair (K1b, and the float64 fallback of irregular
+ * queries rounded once) lies within this relative distance of its K6 float64 score; DESIGN §3 reports 6e-8 observed.
+ * So a float32 search at threshold * (1 - margin) finds every pair whose K6 score reaches threshold. */
+#define KV_RANGE_EXACT_MARGIN 4e-6
+
+/* Exact threshold search over the resident batch: every (query, row) pair whose K6 float64 score -- the value
+ * kv_rescore_pairs gives the pair, bit for bit -- is >= threshold, 0 < threshold <= 1.  It decides membership with the
+ * float64 arithmetic of the reference's scores, where kv_range_resident decides it with the float32 top-k score.
+ *   1. The float32 search of kv_range_resident (label, tag and exclusion filters, deletions) at the largest float32
+ *      <= threshold * (1 - KV_RANGE_EXACT_MARGIN): the candidates, *n_candidates (may be NULL) their count.
+ *   2. K6-R: every candidate gets its K6 score on the device, one warp per pair, and the pairs whose score is
+ *      >= threshold are kept: *n_pairs.  Rows with identical text tie exactly, on any index.
+ * q_indptr / q_ids / q_tf / q_oov_tf2 (host, n_q queries) are the resident batch's query CSR, as kv_rescore_pairs gets
+ * it; n_q must be the batch's query count.  The result stays in the handle until kv_range_fetch_exact(_device), the
+ * next upload, search, append, deletion or finalize.  The resident batch, its filters, exclusions and top-k thresholds
+ * are left as they were.  kv_index_last_kernel_ms: [0] = K6-R with its compaction, [2]-[4] as kv_range_resident.
+ * KV_ERR_INVALID: threshold NaN, <= 0 or > 1, a Jaccard index (mode 1), a batch from kv_selfjoin_upload, n_q not the
+ * batch's count, a bad CSR.  KV_ERR_STATE: not finalized, no resident batch.  KV_ERR_NOMEM as kv_range_resident. */
+int kv_range_resident_exact(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
+                            const double *q_oov_tf2, int64_t n_q, double threshold, int64_t *n_pairs,
+                            int64_t *n_candidates);
+/* The exact result: indptr[n_q+1] by original query, rows[n_pairs] (global), scores[n_pairs] (float64, K6), per query
+ * ordered by (score desc, row asc), on the device by the radix sort of the float32 results extended to a 64-bit score
+ * key (on one host core below 8192 pairs plus queries, the same bits).  Consumption, KV_ERR_NOMEM, a second fetch and,
+ * for the _device form, the device-pointer checks (d_scores aligned to 8 bytes) are those of kv_range_fetch /
+ * kv_range_fetch_device.  A float32 result (kv_range_resident) is not fetched here, nor an exact one by the float32
+ * fetches: KV_ERR_STATE, and the result stays. */
+int kv_range_fetch_exact(kv_index *ix, int64_t *indptr, int64_t *rows, double *scores);
+int kv_range_fetch_exact_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores);
+
 /* K6: float64 scores of selected (query, row) pairs: rows[n_q*k] are GLOBAL row ids (e.g. what a top-k returned;
  * -1 = unused slot), out_scores[n_q*k] (host) receives the float64 cosine of SimilarityEngine.score
  * (similarity.py:14-20) for that row, -inf for unused slots and rows that live on another shard.  Summation follows

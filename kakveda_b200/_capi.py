@@ -89,6 +89,10 @@ SIGNATURES = {
     "kv_range_resident": (C.c_int, [C.c_void_p, C.c_float, c_i64p]),
     "kv_range_fetch": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f32p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "kv_range_fetch_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kv_range_resident_exact": (C.c_int, [C.c_void_p, c_i64p, c_u32p, c_u32p, c_f64p, C.c_int64, C.c_double, c_i64p,
+                                          c_i64p]),
+    "kv_range_fetch_exact": (C.c_int, [C.c_void_p, c_i64p, c_i64p, c_f64p]),
+    "kv_range_fetch_exact_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kv_cluster_topk": (C.c_int, [C.c_int64, C.c_int, c_i64p, c_f32p, C.c_float, c_i64p, c_i64p]),
     "kv_cluster_csr": (C.c_int, [C.c_int64, c_i64p, c_i64p, c_i64p, c_i64p]),
     "kv_cluster_csr_device": (C.c_int, [C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, c_i64p]),

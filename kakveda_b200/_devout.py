@@ -5,13 +5,14 @@ from __future__ import annotations
 import ctypes as C
 
 
-def range_arrays(device: int, n_q: int, n_pairs: int, jaccard: bool = False):
-    """Uninitialised ``(indptr int64[n_q+1], rows int64[P], scores float32[P][, inter int32[P], union int32[P]])``."""
+def range_arrays(device: int, n_q: int, n_pairs: int, jaccard: bool = False, exact: bool = False):
+    """Uninitialised ``(indptr int64[n_q+1], rows int64[P], scores float32[P][, inter int32[P], union int32[P]])``;
+    ``exact``: float64 scores (an exact threshold search)."""
     import torch
 
     dev = torch.device("cuda", device)
     out = [torch.empty(n_q + 1, dtype=torch.int64, device=dev), torch.empty(n_pairs, dtype=torch.int64, device=dev),
-           torch.empty(n_pairs, dtype=torch.float32, device=dev)]
+           torch.empty(n_pairs, dtype=torch.float64 if exact else torch.float32, device=dev)]
     if jaccard:
         out += [torch.empty(n_pairs, dtype=torch.int32, device=dev), torch.empty(n_pairs, dtype=torch.int32, device=dev)]
     return tuple(out)

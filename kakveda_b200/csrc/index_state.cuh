@@ -101,7 +101,7 @@ struct Tombstones {
   }
 };
 
-// The result of a handle's last threshold search, records Rec (RangePair or JaccardPair) in emit order: the pair buffer
+// The result of a handle's last threshold search, records Rec (RangePair, JaccardPair or ExactPair) in emit order: the pair buffer
 // (65,536 records at first; it keeps its capacity across searches), the device pair count, and while the result is
 // valid its query and pair counts.  It lives until a fetch consumes it or the handle drops it.
 template <class Rec>
@@ -139,11 +139,13 @@ struct RangeResult {
   // The fetches order the pairs on the device in the pair buffer itself (range_order.cu), per query by (score desc, row
   // asc).  Once ordering has started the result is consumed whatever happens; a scratch allocation that fails first
   // (KV_ERR_NOMEM) leaves it for another try.  `search` names the entry point that makes a result, for the error of a
-  // fetch without one; row_base is added to the local rows of JaccardPair records.
+  // fetch without one; row_base is added to the local rows of JaccardPair and ExactPair records.  Scores are
+  // RecScore<Rec>: float32, float64 for ExactPair.
+  using Score = typename RecScore<Rec>::type;
 
   // Into host arrays.
   int fetch_host(const char *fn, const char *search, int device, cudaStream_t s, RangeOrderScratch &sc, int64_t row_base,
-                 int64_t *indptr, int64_t *rows, float *scores, int32_t *inter, int32_t *uni) {
+                 int64_t *indptr, int64_t *rows, Score *scores, int32_t *inter, int32_t *uni) {
     if (!valid) return kv_fail(KV_ERR_STATE, "%s: no threshold search result (%s first)", fn, search);
     if (n_pairs > 0 && (!rows || !scores)) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
     KV_CUDA(cudaSetDevice(device));
@@ -160,12 +162,12 @@ struct RangeResult {
     if (!valid) return kv_fail(KV_ERR_STATE, "%s: no threshold search result (%s first)", fn, search);
     int rc = check_device_ptr(d_indptr, device, 8, "indptr", fn);
     if (rc == KV_OK && n_pairs > 0) rc = check_device_ptr(d_rows, device, 8, "rows", fn);
-    if (rc == KV_OK && n_pairs > 0) rc = check_device_ptr(d_scores, device, 4, "scores", fn);
+    if (rc == KV_OK && n_pairs > 0) rc = check_device_ptr(d_scores, device, sizeof(Score), "scores", fn);
     if (rc == KV_OK && n_pairs > 0 && counts) rc = check_device_ptr(d_inter, device, 4, "inter", fn);
     if (rc == KV_OK && n_pairs > 0 && counts) rc = check_device_ptr(d_uni, device, 4, "uni", fn);
     if (rc != KV_OK) return rc;
     KV_CUDA(cudaSetDevice(device));
-    rc = range_order_device(pairs.p, n_pairs, n_q, row_base, (int64_t *)d_indptr, (int64_t *)d_rows, (float *)d_scores,
+    rc = range_order_device(pairs.p, n_pairs, n_q, row_base, (int64_t *)d_indptr, (int64_t *)d_rows, (Score *)d_scores,
                             (int32_t *)d_inter, (int32_t *)d_uni, sc, s, fn);
     if (rc != KV_ERR_NOMEM) valid = false;
     if (rc != KV_OK) return rc;

@@ -107,6 +107,24 @@ struct JaccardPair {
   int32_t uni;    // |q ∪ row|
 };
 
+// One match of an exact threshold search (16 bytes): a pair the float32 search emitted that K6-R re-scored in float64
+// and kept (kv_range_resident_exact).
+struct ExactPair {
+  int32_t q;     // original query
+  int32_t row;   // local original row (below 2^31: the row permutation is int)
+  double score;  // K6's float64 score
+};
+
+// The score type the fetches return for records Rec: float32, float64 for ExactPair
+template <class Rec>
+struct RecScore {
+  using type = float;
+};
+template <>
+struct RecScore<ExactPair> {
+  using type = double;
+};
+
 // Scratch of the device ordering of range records (range_order.cu), owned by an index handle: the buffers keep their
 // capacity across calls, like the pair buffer itself.
 struct RangeOrderScratch {
@@ -123,17 +141,20 @@ constexpr int64_t RANGE_HOST_ORDER_MAX = 8192;
 
 // Orders the n pairs of a threshold search over n_q queries (emit order, as the device left them; rec is reordered in
 // place) into device arrays indptr[n_q+1] / rows[n] / scores[n] (and, for JaccardPair records, inter[n] / uni[n]) on
-// stream s: per query by (score desc, row asc).  row_base is added to JaccardPair rows (RangePair rows are global
-// already).  Returns once the work is enqueued.  KV_ERR_NOMEM (with the pair count) when the scratch does not fit.
-// `fn` names the caller in error messages.  Defined for Rec = RangePair and JaccardPair.
+// stream s: per query by (score desc, row asc).  row_base is added to JaccardPair and ExactPair rows (RangePair rows
+// are global already); scores are float64 for ExactPair (RecScore).  Returns once the work is enqueued.  KV_ERR_NOMEM
+// (with the pair count) when the scratch does not fit.  `fn` names the caller in error messages.  Defined for Rec =
+// RangePair, JaccardPair and ExactPair.
 template <class Rec>
-int range_order_device(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
-                       int32_t *inter, int32_t *uni, RangeOrderScratch &sc, cudaStream_t s, const char *fn);
+int range_order_device(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows,
+                       typename RecScore<Rec>::type *scores, int32_t *inter, int32_t *uni, RangeOrderScratch &sc,
+                       cudaStream_t s, const char *fn);
 // The same into host arrays, stream synchronised: ordered on the device into sc.out and copied back, or below
 // RANGE_HOST_ORDER_MAX pairs plus queries copied back as records and ordered on the host (the same bits).
 template <class Rec>
-int range_order_to_host(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
-                        int32_t *inter, int32_t *uni, RangeOrderScratch &sc, cudaStream_t s, const char *fn);
+int range_order_to_host(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows,
+                        typename RecScore<Rec>::type *scores, int32_t *inter, int32_t *uni, RangeOrderScratch &sc,
+                        cudaStream_t s, const char *fn);
 
 // Exclusive scan of x[0, m) in place on stream s (range_order.cu); `part` is scratch.  The sums must stay below 2^32.
 int exclusive_scan_u32(unsigned *x, int64_t m, DevBuf<unsigned> &part, cudaStream_t s);

@@ -8,7 +8,8 @@
 // scatter in which every tile ranks its records digit by digit with warp match masks.  indptr then comes from a binary
 // search of each query in the sorted records.  Scores are positive (they reach a threshold in (0, 1]); the key maps
 // float32 bits to an order-preserving unsigned value all the same.  The Jaccard score is __fdiv_rn(inter, uni), the
-// bits the host's IEEE division of the two integer-valued floats gives.
+// bits the host's IEEE division of the two integer-valued floats gives.  The exact records (ExactPair) carry a float64
+// score, whose key is 64 bits wide; as for the rows, only its digits that vary are sorted.
 //
 // A host fetch of fewer than RANGE_HOST_ORDER_MAX pairs plus queries copies the records back and orders them on one
 // host core instead (host_order): below that size the device ordering's fixed cost is larger than the sort (DESIGN §6).
@@ -27,7 +28,8 @@ constexpr unsigned long long SIGN64 = 1ull << 63;
 
 enum : int { F_ROW = 0, F_SCORE = 1, F_QUERY = 2 };
 
-static_assert(sizeof(RangePair) == 16 && sizeof(JaccardPair) == 16, "records move as one 16-byte word");
+static_assert(sizeof(RangePair) == 16 && sizeof(JaccardPair) == 16 && sizeof(ExactPair) == 16,
+              "records move as one 16-byte word");
 
 template <class Rec>
 __device__ __forceinline__ Rec ld_rec(const Rec *p) {
@@ -46,16 +48,36 @@ __device__ __forceinline__ void st_rec(Rec *p, const Rec &r) {
 
 __device__ __forceinline__ float rec_score(const RangePair &p) { return p.score; }
 __device__ __forceinline__ float rec_score(const JaccardPair &p) { return __fdiv_rn((float)p.inter, (float)p.uni); }
+__device__ __forceinline__ double rec_score(const ExactPair &p) { return p.score; }
 
 // unsigned order of the result = float order of s (NaN excluded)
 __device__ __forceinline__ unsigned score_key(float s) {
   const unsigned b = __float_as_uint(s);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
+__device__ __forceinline__ unsigned long long score_key(double s) {
+  const unsigned long long b = (unsigned long long)__double_as_longlong(s);
+  return (b & SIGN64) ? ~b : (b | SIGN64);
+}
+
+// warp-wide minimum / maximum of a score key
+__device__ __forceinline__ unsigned warp_min(unsigned x) { return __reduce_min_sync(0xFFFFFFFFu, x); }
+__device__ __forceinline__ unsigned warp_max(unsigned x) { return __reduce_max_sync(0xFFFFFFFFu, x); }
+__device__ __forceinline__ unsigned long long warp_min(unsigned long long x) {
+  for (int o = 16; o; o >>= 1) x = min(x, __shfl_xor_sync(0xFFFFFFFFu, x, o));
+  return x;
+}
+__device__ __forceinline__ unsigned long long warp_max(unsigned long long x) {
+  for (int o = 16; o; o >>= 1) x = max(x, __shfl_xor_sync(0xFFFFFFFFu, x, o));
+  return x;
+}
 
 // unsigned order of the result = signed order of the row
 __device__ __forceinline__ unsigned long long row_key(const RangePair &p) { return (unsigned long long)p.row ^ SIGN64; }
 __device__ __forceinline__ unsigned long long row_key(const JaccardPair &p) {
+  return (unsigned long long)(long long)p.row ^ SIGN64;
+}
+__device__ __forceinline__ unsigned long long row_key(const ExactPair &p) {
   return (unsigned long long)(long long)p.row ^ SIGN64;
 }
 
@@ -99,18 +121,21 @@ __device__ __forceinline__ unsigned block_exclusive_scan(unsigned v, unsigned *t
 // st[0..5] = min / max of the query, of score_key and of row_key over the n records
 template <class Rec>
 __global__ void __launch_bounds__(RO_THREADS) ro_minmax_kernel(const Rec *in, int64_t n, unsigned long long *st) {
-  unsigned qlo = ~0u, qhi = 0, slo = ~0u, shi = 0;
+  using SKey = decltype(score_key(rec_score(Rec{})));  // 32 bits, 64 for a float64 score
+  unsigned qlo = ~0u, qhi = 0;
+  SKey slo = ~SKey(0), shi = 0;
   unsigned long long rlo = ~0ull, rhi = 0;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const Rec r = ld_rec(in + i);
-    const unsigned q = (unsigned)r.q, s = score_key(rec_score(r));
+    const unsigned q = (unsigned)r.q;
+    const SKey s = score_key(rec_score(r));
     const unsigned long long w = row_key(r);
     qlo = min(qlo, q); qhi = max(qhi, q);
     slo = min(slo, s); shi = max(shi, s);
     rlo = min(rlo, w); rhi = max(rhi, w);
   }
   qlo = __reduce_min_sync(0xFFFFFFFFu, qlo); qhi = __reduce_max_sync(0xFFFFFFFFu, qhi);
-  slo = __reduce_min_sync(0xFFFFFFFFu, slo); shi = __reduce_max_sync(0xFFFFFFFFu, shi);
+  slo = warp_min(slo); shi = warp_max(shi);
   for (int o = 16; o; o >>= 1) {
     rlo = min(rlo, __shfl_xor_sync(0xFFFFFFFFu, rlo, o));
     rhi = max(rhi, __shfl_xor_sync(0xFFFFFFFFu, rhi, o));
@@ -229,13 +254,16 @@ __global__ void __launch_bounds__(RO_THREADS) ro_scatter_kernel(const Rec *in, R
 // rows / scores (/ inter / uni) of the ordered records
 template <class Rec>
 __global__ void __launch_bounds__(RO_THREADS) ro_emit_kernel(const Rec *in, int64_t n, int64_t row_base, int64_t *rows,
-                                                              float *scores, int32_t *inter, int32_t *uni) {
+                                                              typename RecScore<Rec>::type *scores, int32_t *inter,
+                                                              int32_t *uni) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const Rec r = ld_rec(in + i);
     if constexpr (std::is_same_v<Rec, JaccardPair>) {
       rows[i] = row_base + r.row;
       inter[i] = r.inter;
       uni[i] = r.uni;
+    } else if constexpr (std::is_same_v<Rec, ExactPair>) {
+      rows[i] = row_base + r.row;
     } else {
       rows[i] = r.row;
     }
@@ -287,8 +315,9 @@ int exclusive_scan_u32(unsigned *x, int64_t m, DevBuf<unsigned> &part, cudaStrea
 }
 
 template <class Rec>
-int range_order_device(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
-                       int32_t *inter, int32_t *uni, RangeOrderScratch &sc, cudaStream_t s, const char *fn) {
+int range_order_device(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows,
+                       typename RecScore<Rec>::type *scores, int32_t *inter, int32_t *uni, RangeOrderScratch &sc,
+                       cudaStream_t s, const char *fn) {
   Rec *cur = rec;
   if (n > 1) {
     // offsets are 32-bit: 2^32 records would be 64 GB before any scratch
@@ -339,11 +368,12 @@ int range_order_device(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64
 namespace {
 inline float host_score(const RangePair &p) { return p.score; }
 inline float host_score(const JaccardPair &p) { return (float)p.inter / (float)p.uni; }  // IEEE: the bits of __fdiv_rn
+inline double host_score(const ExactPair &p) { return p.score; }
 
 // The ordering on one host core: a counting sort by query, then each query's segment by (score desc, row asc).
 template <class Rec>
-int host_order(const Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
-               int32_t *inter, int32_t *uni, const char *fn) {
+int host_order(const Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows,
+               typename RecScore<Rec>::type *scores, int32_t *inter, int32_t *uni, const char *fn) {
   std::vector<Rec> by_q;
   try {
     by_q.resize((size_t)n);
@@ -357,7 +387,7 @@ int host_order(const Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t
   for (int64_t i = 0; i < n; i++) by_q[(size_t)next[(size_t)rec[i].q]++] = rec[i];
   for (int64_t q = 0; q < n_q; q++)
     std::sort(by_q.begin() + indptr[q], by_q.begin() + indptr[q + 1], [](const Rec &x, const Rec &y) {
-      const float sx = host_score(x), sy = host_score(y);
+      const auto sx = host_score(x), sy = host_score(y);
       return sx != sy ? sx > sy : x.row < y.row;
     });
   for (int64_t i = 0; i < n; i++) {
@@ -367,6 +397,8 @@ int host_order(const Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t
       rows[i] = row_base + p.row;
       inter[i] = p.inter;
       uni[i] = p.uni;
+    } else if constexpr (std::is_same_v<Rec, ExactPair>) {
+      rows[i] = row_base + p.row;
     } else {
       rows[i] = p.row;
     }
@@ -376,23 +408,25 @@ int host_order(const Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t
 
 // range_order_device into sc.out, then the ordered arrays copied to the host
 template <class Rec>
-int device_order_to_host(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
-                         int32_t *inter, int32_t *uni, RangeOrderScratch &sc, cudaStream_t s, const char *fn) {
+int device_order_to_host(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows,
+                         typename RecScore<Rec>::type *scores, int32_t *inter, int32_t *uni, RangeOrderScratch &sc,
+                         cudaStream_t s, const char *fn) {
+  using Score = typename RecScore<Rec>::type;
   constexpr bool jac = std::is_same_v<Rec, JaccardPair>;
-  const int64_t bytes = (n_q + 1) * 8 + n * (jac ? 20 : 12);
+  const int64_t bytes = (n_q + 1) * 8 + n * (8 + (int64_t)sizeof(Score) + (jac ? 8 : 0));
   if (sc.out.ensure(bytes) != cudaSuccess) {
     cudaGetLastError();
     return kv_fail(KV_ERR_NOMEM, "%s: %lld pairs: their ordered arrays do not fit in device memory", fn, (long long)n);
   }
   int64_t *d_indptr = reinterpret_cast<int64_t *>(sc.out.p), *d_rows = d_indptr + (n_q + 1);
-  float *d_scores = reinterpret_cast<float *>(d_rows + n);
+  Score *d_scores = reinterpret_cast<Score *>(d_rows + n);
   int32_t *d_inter = jac ? reinterpret_cast<int32_t *>(d_scores + n) : nullptr, *d_uni = jac ? d_inter + n : nullptr;
   int rc = range_order_device(rec, n, n_q, row_base, d_indptr, d_rows, d_scores, d_inter, d_uni, sc, s, fn);
   if (rc != KV_OK) return rc;
   KV_CUDA(cudaMemcpyAsync(indptr, d_indptr, (size_t)(n_q + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
   if (n > 0) {
     KV_CUDA(cudaMemcpyAsync(rows, d_rows, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-    KV_CUDA(cudaMemcpyAsync(scores, d_scores, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, s));
+    KV_CUDA(cudaMemcpyAsync(scores, d_scores, (size_t)n * sizeof(Score), cudaMemcpyDeviceToHost, s));
     if constexpr (jac) {
       KV_CUDA(cudaMemcpyAsync(inter, d_inter, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
       KV_CUDA(cudaMemcpyAsync(uni, d_uni, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
@@ -404,8 +438,9 @@ int device_order_to_host(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int
 }  // namespace
 
 template <class Rec>
-int range_order_to_host(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows, float *scores,
-                        int32_t *inter, int32_t *uni, RangeOrderScratch &sc, cudaStream_t s, const char *fn) {
+int range_order_to_host(Rec *rec, int64_t n, int64_t n_q, int64_t row_base, int64_t *indptr, int64_t *rows,
+                        typename RecScore<Rec>::type *scores, int32_t *inter, int32_t *uni, RangeOrderScratch &sc,
+                        cudaStream_t s, const char *fn) {
   if (n + n_q >= RANGE_HOST_ORDER_MAX)
     return device_order_to_host(rec, n, n_q, row_base, indptr, rows, scores, inter, uni, sc, s, fn);
   // few pairs over few queries: the records come back (16 B each) and one host core orders them (work n + n_q) in less
@@ -427,6 +462,10 @@ template int range_order_to_host<RangePair>(RangePair *, int64_t, int64_t, int64
                                             int32_t *, RangeOrderScratch &, cudaStream_t, const char *);
 template int range_order_to_host<JaccardPair>(JaccardPair *, int64_t, int64_t, int64_t, int64_t *, int64_t *, float *,
                                               int32_t *, int32_t *, RangeOrderScratch &, cudaStream_t, const char *);
+template int range_order_device<ExactPair>(ExactPair *, int64_t, int64_t, int64_t, int64_t *, int64_t *, double *, int32_t *,
+                                           int32_t *, RangeOrderScratch &, cudaStream_t, const char *);
+template int range_order_to_host<ExactPair>(ExactPair *, int64_t, int64_t, int64_t, int64_t *, int64_t *, double *, int32_t *,
+                                            int32_t *, RangeOrderScratch &, cudaStream_t, const char *);
 
 extern "C" int kv_debug_range_order(int device, int jaccard, const void *records, int64_t n, int64_t n_q, int64_t row_base,
                                     int64_t *indptr, int64_t *rows, float *scores, int32_t *inter, int32_t *uni) {

@@ -260,9 +260,11 @@ struct kv_index {
   // threshold search over the resident batch (kv_range_resident): its own threshold array (not d_gthr, which peers push
   // into and a top-k raises) and the result of the index's mode -- on a Jaccard index (K3-R) the records carry the
   // exact counts and local rows.  Either result is dropped by the next upload, search, append, deletion or finalize.
+  // An exact search (kv_range_resident_exact) leaves its result in xrange and consumes the float32 one it started from.
   DevBuf<int> d_rthr;
   RangeResult<RangePair> range;
   RangeResult<JaccardPair> jrange;
+  RangeResult<ExactPair> xrange;
   RangeOrderScratch rsort;  // the fetches order the pairs on the device (range_order.cu)
   DevBuf<unsigned long long> d_stats;
   DevBuf<float> d_part_s, d_out_s;
@@ -274,6 +276,7 @@ struct kv_index {
 
   // query batch currently resident on the device (kv_query_upload and its variants)
   bool batch_valid = false;
+  bool batch_selfjoin = false;  // the resident batch came from kv_selfjoin_upload (no exact threshold search)
   int64_t batch_q = 0, batch_tiles = 0, batch_h2d_bytes = 0, batch_null = 0, batch_f2_outside = 0;
   IrregularQueries irr;
 
@@ -299,6 +302,7 @@ static void close_peers(kv_index *ix) {
 static void drop_range(kv_index *ix) {
   ix->range.drop();
   ix->jrange.drop();
+  ix->xrange.drop();
 }
 
 namespace {
@@ -1156,7 +1160,7 @@ static int build_query_tables(kv_index *ix, int64_t n_q);
 // An upload replaces the resident batch: the old batch and the range result are dropped, and the exclusions, label
 // filter, distinct mode and irregular queries of the old batch go with it.
 static void start_batch(kv_index *ix) {
-  ix->batch_valid = false;
+  ix->batch_valid = ix->batch_selfjoin = false;
   drop_range(ix);
   ix->has_excl = ix->has_filter = ix->distinct = ix->merged_seeds = false;
   ix->qtags.on = false;
@@ -1987,9 +1991,9 @@ static int finish_batch(kv_index *ix) {
 // Threshold search over the resident batch: every pair with score >= thr lands in ix->range (ix->jrange on a Jaccard
 // index), *n_pairs = their count.  When they do not fit, the buffer grows to the exact count and only the scan and the
 // fallbacks run again (the candidate lists depend on the threshold alone).  Events: evk[2] -> evk[3] bound pass 1,
-// evk[3] -> evk[4] scan, evk[4] -> evk[5] irregular-query fallbacks.  Caller holds ix->mu.
-static int run_range(kv_index *ix, float thr, int64_t *n_pairs) {
-  const char *fn = "kv_range_resident";
+// evk[3] -> evk[4] scan, evk[4] -> evk[5] irregular-query fallbacks.  `fn` names the entry point in errors.  Caller
+// holds ix->mu.
+static int run_range(kv_index *ix, float thr, int64_t *n_pairs, const char *fn) {
   drop_range(ix);
   if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "%s: no query batch uploaded", fn);
   int rc = check_filter(ix, fn);
@@ -2211,6 +2215,7 @@ int kv_selfjoin_upload(kv_index *ix, int64_t q_begin, int64_t q_end) {
   }
   int rc = prepare_batch_runs(ix, &R, 1);
   if (rc != KV_OK) return rc;
+  ix->batch_selfjoin = true;
   for (int64_t i = 0; i < n; i++) ex[(size_t)i] = ix->row_base + q_begin + i;
   return set_exclusions_locked(ix, ex.data(), n);
 }
@@ -2479,7 +2484,77 @@ int kv_range_resident(kv_index *ix, float threshold, int64_t *n_pairs) {
   if (!ix || !n_pairs) return kv_fail(KV_ERR_INVALID, "kv_range_resident: bad arguments");
   if (!(threshold > 0.f && threshold <= 1.f)) return kv_fail(KV_ERR_INVALID, "kv_range_resident: threshold must be in (0, 1]");
   std::lock_guard<std::mutex> g(ix->mu);
-  return run_range(ix, threshold, n_pairs);
+  return run_range(ix, threshold, n_pairs, "kv_range_resident");
+}
+
+// The float32 threshold of an exact search's first stage: the largest float32 <= thr * (1 - KV_RANGE_EXACT_MARGIN),
+// and at least the smallest positive float32 (the float32 search needs a positive threshold).
+static float exact_prefilter_threshold(double thr) {
+  const double t = thr * (1.0 - KV_RANGE_EXACT_MARGIN);
+  float f = (float)t;
+  if ((double)f > t) f = std::nextafter(f, 0.f);
+  return std::max(f, std::numeric_limits<float>::denorm_min());
+}
+
+// K6-R of the ix->range records into ix->xrange (room for all of them): events evk[0] -> evk[1] around the kernel.
+// Caller holds ix->mu, after rescore_upload.
+static int rescore_range_launch(kv_index *ix, int64_t n, double thr) {
+  RescoreRangeParams R;
+  RescoreParams &P = R.K6;
+  P.indptr = ix->indptr.p; P.ids = ix->ids.p; P.tf = ix->tf.p;
+  P.a64 = ix->d_a64.p; P.d64 = ix->d_d64.p; P.B64 = ix->d_B64.p; P.invperm = ix->d_invperm.p;
+  P.q_indptr = ix->d_rq_indptr.p; P.q_ids = ix->d_rq_ids.p; P.q_tf = ix->d_rq_tf.p;
+  P.q_nq = ix->d_rq_const.p;
+  P.rows = nullptr; P.n_q = ix->range.n_q; P.n_rows = ix->n_rows; P.row_base = ix->row_base; P.V = ix->V;
+  P.k = 0; P.jaccard = ix->jaccard; P.dead = nullptr; P.out = nullptr;
+  R.in = ix->range.pairs.p; R.n = n; R.thr = thr; R.out = ix->xrange.pairs.p; R.count = ix->xrange.d_count.p;
+  const int64_t warps = (n + 31) / 32;
+  KV_CUDA(cudaEventRecord(ix->evk[0], ix->stream));
+  rescore_range_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, ix->stream>>>(R);
+  KV_CUDA(cudaGetLastError());
+  KV_CUDA(cudaEventRecord(ix->evk[1], ix->stream));
+  return KV_OK;
+}
+
+int kv_range_resident_exact(kv_index *ix, const int64_t *q_indptr, const uint32_t *q_ids, const uint32_t *q_tf,
+                            const double *q_oov_tf2, int64_t n_q, double threshold, int64_t *n_pairs,
+                            int64_t *n_candidates) {
+  const char *fn = "kv_range_resident_exact";
+  if (!ix || !n_pairs || n_q < 1 || !q_indptr) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
+  if (!(threshold > 0.0 && threshold <= 1.0)) return kv_fail(KV_ERR_INVALID, "%s: threshold must be in (0, 1]", fn);
+  std::lock_guard<std::mutex> g(ix->mu);
+  if (ix->jaccard) return kv_fail(KV_ERR_INVALID, "%s: a Jaccard index (mode 1) has no exact threshold search", fn);
+  if (!ix->finalized) return kv_fail(KV_ERR_STATE, "%s: index not finalized", fn);
+  if (!ix->batch_valid) return kv_fail(KV_ERR_STATE, "%s: no query batch uploaded", fn);
+  if (ix->batch_selfjoin) return kv_fail(KV_ERR_INVALID, "%s: a self-join batch (kv_selfjoin_upload) has no exact threshold search", fn);
+  if (n_q != ix->batch_q)
+    return kv_fail(KV_ERR_INVALID, "%s: a query CSR of %lld queries for a batch of %lld", fn, (long long)n_q, (long long)ix->batch_q);
+  const int64_t nnz = q_indptr[n_q] - q_indptr[0];
+  if (nnz < 0 || (nnz > 0 && (!q_ids || !q_tf))) return kv_fail(KV_ERR_INVALID, "%s: bad query CSR", fn);
+  int64_t cand = 0;
+  int rc = run_range(ix, exact_prefilter_threshold(threshold), &cand, fn);
+  if (rc != KV_OK) return rc;
+  ix->range.valid = false;  // its records are K6-R's input now, not a result
+  cudaStream_t s = ix->stream;
+  unsigned long long kept = 0;
+  float ms = 0.f;
+  if ((rc = ix->xrange.prepare(s)) != KV_OK) return rc;
+  if ((unsigned long long)cand > ix->xrange.capacity() && (rc = ix->xrange.grow((unsigned long long)cand, s, fn)) != KV_OK)
+    return rc;
+  if (cand > 0) {
+    std::vector<double> cst;
+    std::vector<int64_t> ip;
+    if ((rc = rescore_upload(ix, q_indptr, q_ids, q_tf, q_oov_tf2, n_q, 1, cst, ip)) != KV_OK) return rc;
+    if ((rc = rescore_range_launch(ix, cand, threshold)) != KV_OK) return rc;
+    KV_CUDA(cudaMemcpyAsync(&kept, ix->xrange.d_count.p, sizeof(kept), cudaMemcpyDeviceToHost, s));
+    KV_CUDA(cudaStreamSynchronize(s));
+    cudaEventElapsedTime(&ms, ix->evk[0], ix->evk[1]);
+  }
+  ix->last_kernel_ms[0] = ms;
+  ix->xrange.commit(n_q, (int64_t)kept);
+  *n_pairs = (int64_t)kept;
+  if (n_candidates) *n_candidates = cand;
+  return KV_OK;
 }
 
 // The count outputs a fetch was given must fit the index's mode: required on a Jaccard index (like rows and scores, only
@@ -2499,6 +2574,7 @@ int kv_range_fetch(kv_index *ix, int64_t *indptr, int64_t *rows, float *scores, 
   const char *fn = "kv_range_fetch", *search = "kv_range_resident";
   if (!ix || !indptr) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
   std::lock_guard<std::mutex> g(ix->mu);
+  if (ix->xrange.valid) return kv_fail(KV_ERR_STATE, "%s: the last threshold search was exact (kv_range_fetch_exact)", fn);
   const int rc = check_count_outputs(ix, inter, uni, fn);
   if (rc != KV_OK) return rc;
   return ix->jaccard ? ix->jrange.fetch_host(fn, search, ix->device, ix->stream, ix->rsort, ix->row_base, indptr, rows, scores, inter, uni)
@@ -2510,12 +2586,41 @@ int kv_range_fetch_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_sc
   const char *fn = "kv_range_fetch_device", *search = "kv_range_resident";
   if (!ix) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
   std::lock_guard<std::mutex> g(ix->mu);
+  if (ix->xrange.valid)
+    return kv_fail(KV_ERR_STATE, "%s: the last threshold search was exact (kv_range_fetch_exact_device)", fn);
   const int rc = check_count_outputs(ix, d_inter, d_uni, fn);
   if (rc != KV_OK) return rc;
   return ix->jaccard ? ix->jrange.fetch_device(fn, search, ix->device, ix->stream, ix->rsort, ix->row_base, d_indptr, d_rows,
                                                d_scores, d_inter, d_uni)
                      : ix->range.fetch_device(fn, search, ix->device, ix->stream, ix->rsort, ix->row_base, d_indptr, d_rows,
                                               d_scores, d_inter, d_uni);
+}
+
+// The exact result: the same CSR with float64 scores; a float32 result is not one (KV_ERR_STATE).
+static int check_exact_result(const kv_index *ix, const char *fn) {
+  if (!ix->xrange.valid && (ix->range.valid || ix->jrange.valid))
+    return kv_fail(KV_ERR_STATE, "%s: the last threshold search was a float32 one (kv_range_fetch)", fn);
+  return KV_OK;
+}
+
+int kv_range_fetch_exact(kv_index *ix, int64_t *indptr, int64_t *rows, double *scores) {
+  const char *fn = "kv_range_fetch_exact", *search = "kv_range_resident_exact";
+  if (!ix || !indptr) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
+  std::lock_guard<std::mutex> g(ix->mu);
+  const int rc = check_exact_result(ix, fn);
+  if (rc != KV_OK) return rc;
+  return ix->xrange.fetch_host(fn, search, ix->device, ix->stream, ix->rsort, ix->row_base, indptr, rows, scores, nullptr,
+                               nullptr);
+}
+
+int kv_range_fetch_exact_device(kv_index *ix, void *d_indptr, void *d_rows, void *d_scores) {
+  const char *fn = "kv_range_fetch_exact_device", *search = "kv_range_resident_exact";
+  if (!ix) return kv_fail(KV_ERR_INVALID, "%s: bad arguments", fn);
+  std::lock_guard<std::mutex> g(ix->mu);
+  const int rc = check_exact_result(ix, fn);
+  if (rc != KV_OK) return rc;
+  return ix->xrange.fetch_device(fn, search, ix->device, ix->stream, ix->rsort, ix->row_base, d_indptr, d_rows, d_scores,
+                                 nullptr, nullptr);
 }
 
 int kv_index_thresholds_export(kv_index *ix, int64_t capacity, void *handle_out) {

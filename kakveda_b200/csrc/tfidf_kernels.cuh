@@ -1535,17 +1535,9 @@ struct RescoreParams {
   double *out;              // [n_q * k]; -inf for unused slots, rows of other shards and deleted rows
 };
 
-__global__ void __launch_bounds__(256) rescore_kernel(RescoreParams P) {
-  const int64_t pair = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (pair >= P.n_q * P.k) return;
-  const int64_t q = pair / P.k;
-  const long long gr = P.rows[pair];
-  const int64_t r = gr - P.row_base;
-  if (gr < 0 || r < 0 || r >= P.n_rows || (P.dead && P.dead[r])) {
-    if (lane == 0) P.out[pair] = -INFINITY;
-    return;
-  }
+// K6's body for one pair, shared by K6 and K6-R so that both give the same bits for the same pair: the whole warp
+// walks local row r against query q, and the lanes with `finish` set return the float64 score (the others 0).
+__device__ __forceinline__ double rescore_pair(const RescoreParams &P, int64_t q, int64_t r, int lane, bool finish) {
   const int64_t qa = P.q_indptr[q], qb = P.q_indptr[q + 1];
   double du = 0.0, dv = 0.0;
   const int64_t p1 = P.indptr[r + 1];
@@ -1574,19 +1566,73 @@ __global__ void __launch_bounds__(256) rescore_kernel(RescoreParams P) {
       dv = __dadd_rn(dv, __shfl_sync(FULL, wv, j));
     }
   }
-  if (lane == 0) {
-    const double B = P.B64[P.invperm[r]];
-    const double dot = du;
-    double sc;
-    if (P.jaccard) {
-      const double den = __dadd_rn(__dadd_rn(P.q_nq[q], B), -dot);
-      sc = (den > 0.0 && dot != 0.0) ? dot / den : 0.0;
-    } else {
-      const double den = __dmul_rn(P.q_nq[q], __dadd_rn(B, dv));
-      sc = (den > 0.0 && dot != 0.0) ? dot / sqrt(den) : 0.0;
-    }
-    P.out[pair] = sc;
+  if (!finish) return 0.0;
+  const double B = P.B64[P.invperm[r]];
+  const double dot = du;
+  double sc;
+  if (P.jaccard) {
+    const double den = __dadd_rn(__dadd_rn(P.q_nq[q], B), -dot);
+    sc = (den > 0.0 && dot != 0.0) ? dot / den : 0.0;
+  } else {
+    const double den = __dmul_rn(P.q_nq[q], __dadd_rn(B, dv));
+    sc = (den > 0.0 && dot != 0.0) ? dot / sqrt(den) : 0.0;
   }
+  return sc;
+}
+
+__global__ void __launch_bounds__(256) rescore_kernel(RescoreParams P) {
+  const int64_t pair = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (pair >= P.n_q * P.k) return;
+  const int64_t q = pair / P.k;
+  const long long gr = P.rows[pair];
+  const int64_t r = gr - P.row_base;
+  if (gr < 0 || r < 0 || r >= P.n_rows || (P.dead && P.dead[r])) {
+    if (lane == 0) P.out[pair] = -INFINITY;
+    return;
+  }
+  const double sc = rescore_pair(P, q, r, lane, lane == 0);
+  if (lane == 0) P.out[pair] = sc;
+}
+
+// ----------------------------------------------------------------------------------------
+// K6-R: K6 of the pairs a threshold search emitted (kv_range_resident_exact).  It reads the search's records in place
+// (emit order, global rows), gives each pair its K6 score through rescore_pair -- the bits K6 gives the same pair --
+// and keeps the pairs whose score reaches the float64 threshold as ExactPair records (local rows).  A warp takes 32
+// consecutive records and scores them one after the other with all its lanes, so that lane j ends with record j's
+// score; the kept ones then take one reservation per warp, as range_emit and dense_emit do.  The output has room for
+// every input record, so no pair is lost.
+// ----------------------------------------------------------------------------------------
+struct RescoreRangeParams {
+  RescoreParams K6;          // the index and the query batch; rows, k and out are not used
+  const RangePair *in;       // [n] the search's records
+  int64_t n;
+  double thr;
+  ExactPair *out;            // [n]
+  unsigned long long *count;  // kept records
+};
+
+__global__ void __launch_bounds__(256) rescore_range_kernel(RescoreRangeParams P) {
+  const int64_t i0 = ((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5) * 32;
+  const int lane = threadIdx.x & 31;
+  if (i0 >= P.n) return;
+  const int m = (int)min((int64_t)32, P.n - i0);
+  RangePair rec{0, 0.f, 0};
+  if (lane < m) rec = P.in[i0 + lane];
+  double mine = 0.0;
+  for (int j = 0; j < m; j++) {
+    const int q = __shfl_sync(FULL, rec.q, j);
+    const long long row = __shfl_sync(FULL, (long long)rec.row, j);
+    const double sc = rescore_pair(P.K6, q, row - P.K6.row_base, lane, lane == j);
+    if (lane == j) mine = sc;
+  }
+  const bool keep = lane < m && mine >= P.thr;
+  const uint32_t hm = __ballot_sync(FULL, keep);
+  if (hm == 0) return;
+  unsigned long long base = 0;
+  if (lane == 0) base = atomicAdd(P.count, (unsigned long long)__popc(hm));
+  base = __shfl_sync(FULL, base, 0);
+  if (keep) P.out[base + __popc(hm & lanemask_lt())] = ExactPair{rec.q, (int)(rec.row - P.K6.row_base), mine};
 }
 
 // ----------------------------------------------------------------------------------------

@@ -1232,7 +1232,8 @@ class ShardedGfkbStore(GfkbStore):
     runs ``kv_exact_topk`` on every shard and on the tail and merges their ``limit`` rows per query (one all-gather):
     no score vector leaves a device.  A purge deletes the main rows and refreshes every statistic in one all-reduce.
 
-    Not supported: the sidecar and the persisted layout, queries mode and text-order shards (ValueError)."""
+    Not supported: the sidecar and the persisted layout, queries mode and text-order shards (ValueError), and
+    ``match_above`` (NotImplementedError: the sharded threshold search merges float32 results)."""
 
     def __init__(self, path=None, device: int = 0, rank: int = 0, world: int = 1, group=None, tail_limit: int = 65536,
                  now=None, sidecar=None, mode: str = "rows", order: str = "index"):
@@ -1337,6 +1338,10 @@ class ShardedGfkbStore(GfkbStore):
             rows_all.append(rows)
             f64_all.append(self._tail.rescore(fb, rows))
         return self._merge_candidates(rows_all, f64_all, distinct) + (amb,)
+
+    def _above(self, fb: FeatureBatch, threshold: float, labels, tags):
+        raise NotImplementedError("ShardedGfkbStore.match_above: the exact threshold search is not built for a "
+                                  "sharded GFKB (its range merge is float32)")
 
     def _exact_top(self, signature_text: str, limit: int, label: int = -1, distinct: bool = False, app: int = -1):
         if distinct:

@@ -386,6 +386,7 @@ class GfkbIndex(_KvIndex):
         super().__init__(device, row_base)
         self._row_labels: Optional[np.ndarray] = None  # what set_row_labels gave, until the next append
         self._group_rows: Optional[int] = None  # rows set_row_groups described, until the next append
+        self.last_range_candidates = 0  # float32 candidates of the last range_exact
 
     # -- build ---------------------------------------------------------------------------
     def add_features(self, fb: FeatureBatch, lo: int = 0, hi: Optional[int] = None) -> None:
@@ -682,6 +683,38 @@ class GfkbIndex(_KvIndex):
             return self._empty_range(device_out)
         self._selfjoin_upload(lo, hi, same_label)
         return self._range_resident(hi - lo, threshold, device_out)
+
+    def range_exact(self, fb: FeatureBatch, threshold: float, labels: Optional[np.ndarray] = None, tags=None,
+                    device_out: bool = False):
+        """Exact threshold search: every (query, row) pair whose float64 score -- the value ``rescore`` gives the pair,
+        bit for bit -- is >= ``threshold``, 0 < threshold <= 1 (``kv_range_resident_exact``).  A float32 search a
+        fixed relative margin below the threshold finds the candidates; K6-R re-scores them on the device and keeps the
+        pairs that reach it.  Returns ``(indptr int64[n_q+1], rows int64[P], scores float64[P])``: query q's pairs are
+        ``[indptr[q], indptr[q+1])``, ordered by (score desc, row asc); rows are global.  ``device_out``: the same
+        arrays as torch tensors on the index's device.  ``labels`` / ``tags`` as for ``range_features``.  The float32
+        candidate count is kept in ``last_range_candidates``."""
+        lib = _capi.load()
+        if fb.n == 0:
+            self.last_range_candidates = 0
+            out = (_devout.range_arrays(self.device, 0, 0, exact=True) if device_out
+                   else (np.empty(1, np.int64), np.empty(0, np.int64), np.empty(0, np.float64)))
+            out[0][0] = 0
+            return out
+        self.upload_queries(fb)
+        self._set_filters(labels, tags)
+        n, cand = C.c_int64(0), C.c_int64(0)
+        _capi.check(lib.kv_range_resident_exact(self._h, _ptr(fb.indptr, C.c_int64), _ptr(fb.ids, C.c_uint32),
+                                                _ptr(fb.tf, C.c_uint32), _ptr(fb.oov, C.c_double), fb.n,
+                                                float(threshold), C.byref(n), C.byref(cand)))
+        self.last_range_candidates = cand.value
+        if device_out:
+            out = _devout.range_arrays(self.device, fb.n, n.value, exact=True)
+            _capi.check(lib.kv_range_fetch_exact_device(self._h, *_devout.ptrs(out)))
+            return out
+        out = (np.empty(fb.n + 1, np.int64), np.empty(n.value, np.int64), np.empty(n.value, np.float64))
+        _capi.check(lib.kv_range_fetch_exact(self._h, _ptr(out[0], C.c_int64), _ptr(out[1], C.c_int64),
+                                             _ptr(out[2], C.c_double)))
+        return out
 
     def rescore(self, fb: FeatureBatch, rows: np.ndarray) -> np.ndarray:
         """K6: float64 scores of the pairs (query q, GLOBAL row rows[q, j]); identical rows tie exactly on every shard."""

@@ -9,6 +9,8 @@ the records and their device index resident and reproduces the three handlers th
   ``F-%04d`` record; one JSON line is appended either way.
 * ``match`` / ``match_batch`` -- services/gfkb/app.py:79-102: stable sort by score descending, first 5, THEN the
   failure_type filter, mapped to FailureMatch fields.
+* ``match_above`` / ``match_above_batch`` -- the same sort with a similarity threshold instead of the first 5: every
+  record whose float64 score reaches it (the exact threshold search, ``GfkbIndex.range_exact``, on both segments).
 * ``warn_batch`` -- services/warning_policy/app.py:19-72: signature_text of the request, best match against the
   threshold, the reference's message strings.
 * ``purge_apps`` -- services/dashboard/app.py:330-375 on failures.jsonl: the purged app ids leave every record's
@@ -820,6 +822,79 @@ class GfkbStore:
                     continue
                 out.append(_to_match(rec, sc))
             return out
+
+    # -- match above a threshold (services/gfkb/app.py:88-89 without the first-5 cut) -----------------------------
+    def _above(self, fb: FeatureBatch, threshold: float, labels: Optional[np.ndarray],
+               tags) -> List[Tuple[np.ndarray, np.ndarray, np.ndarray]]:
+        """The device step of ``match_above_batch``: the exact threshold search of every segment, each
+        ``(indptr, global device rows, float64 scores)`` ordered per query by (score desc, row asc)."""
+        return [ix.range_exact(fb, threshold, labels, tags) for ix in (self._main, self._tail)
+                if ix is not None and ix.n_rows]
+
+    def match_above_batch(self, signature_texts: Sequence[str], threshold: float,
+                          failure_types: Optional[Sequence[Optional[str]]] = None,
+                          app_ids: Optional[Sequence[Optional[str]]] = None, distinct: bool = False) -> List[List[dict]]:
+        """Per query every stored failure whose similarity is >= ``threshold`` (0 < threshold <= 1), as FailureMatch
+        dicts in the reference's stable order (score desc, record asc): the handler's ``sorted(..., reverse=True)``
+        with a threshold instead of the first 5, and no result limit.  Scores are float64 and membership is decided on
+        them (the exact threshold search), so a record whose score equals the threshold is returned.  With no cut,
+        filtering before or after the sort gives the same list, so ``failure_types`` (per query a type, None: any) and
+        ``app_ids`` (per query an app its failures' affected_apps must list, None: any) are searched on the device; a
+        type or app no record has returns ``[]`` without a scan.  ``distinct``: one result per (failure_type,
+        signature_text) key, its best row, reported with the fields of the key's newest record and the key's score.
+        A threshold so low that the pairs do not fit in device memory raises ``MemoryError``."""
+        if not (0.0 < threshold <= 1.0):
+            raise ValueError(f"threshold {threshold} outside (0, 1]")
+        n = len(signature_texts)
+        for name, per_query in (("failure_types", failure_types), ("app_ids", app_ids)):
+            if per_query is not None and len(per_query) != n:
+                raise ValueError(f"{name}: {len(per_query)} entries for {n} queries")
+        out: List[List[dict]] = [[] for _ in signature_texts]
+        with self._lock:
+            if not self.records:
+                return out
+            self._sync()
+            self._row_labels(0, len(self.records))  # number every stored type
+            labels = np.full(n, -1, dtype=np.int32)
+            if failure_types is not None:
+                labels = np.array([-1 if not ft else self._type_ids.get(ft, -2) for ft in failure_types], dtype=np.int32)
+            apps = np.full(n, -1, dtype=np.int64)
+            if app_ids is not None and any(app_ids):
+                self._sync_apps()
+                apps = np.array([-1 if not a else self._apps.listed(a) for a in app_ids], dtype=np.int64)
+            scan = np.flatnonzero((labels != -2) & (apps != -2))  # an unknown type or app: no match, no scan
+            if len(scan) == 0:
+                return out
+            tags = None
+            if (apps[scan] >= 0).any():
+                self._ensure_tags()
+                tags = [[int(apps[i])] if apps[i] >= 0 else [] for i in scan.tolist()]
+            fb = self.vocab.featurize([signature_texts[i] for i in scan], grow=False)
+            try:
+                parts = self._above(fb, threshold, labels[scan] if (labels[scan] >= 0).any() else None, tags)
+            finally:
+                fb.close()
+            groups = self._rec_groups(self._n_indexed) if distinct else None
+            for j, i in enumerate(scan.tolist()):
+                rows = np.concatenate([p[1][p[0][j]:p[0][j + 1]] for p in parts] or [np.zeros(0, np.int64)])
+                scores = np.concatenate([p[2][p[0][j]:p[0][j + 1]] for p in parts] or [np.zeros(0)])
+                order = np.lexsort((rows, -scores))  # score desc, device row asc = the records' stable order
+                recs, scores = self._to_records(rows[order]).tolist(), scores[order].tolist()
+                if distinct:
+                    seen, matches = set(), []
+                    for r, sc in zip(recs, scores):
+                        if groups[r] not in seen:
+                            seen.add(groups[r])
+                            matches.append(self._distinct_match(r, sc))
+                    out[i] = matches
+                else:
+                    out[i] = [_to_match(self.records[r], sc) for r, sc in zip(recs, scores)]
+            return out
+
+    def match_above(self, signature_text: str, threshold: float, failure_type: Optional[str] = None,
+                    app_id: Optional[str] = None, distinct: bool = False) -> List[dict]:
+        """``match_above_batch`` of one query."""
+        return self.match_above_batch([signature_text], threshold, [failure_type], [app_id], distinct)[0]
 
     # -- warn (services/warning_policy/app.py:19-72) ------------------------------------------------------------
     def warn_batch(self, requests: Sequence[Mapping[str, Any]], threshold: float = 0.8, default_action: str = "warn",
