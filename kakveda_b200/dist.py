@@ -32,10 +32,9 @@ import numpy as np
 
 from . import _capi, _devout
 from ._capi import no_distinct
-from .gfkb import MATCH_LIMIT
 from .similarity import (MAX_QUERY_TAGS, FeatureBatch, GfkbIndex, Vocabulary, _featurize_on_device, csr_rows, gather_rows,
                          pack_texts, tag_csr, text_order)
-from .store import MAX_LIMIT, GfkbStore, ambiguous_candidates
+from .store import GfkbStore
 
 
 def shard_bounds(n_rows: int, world: int, rank: int) -> Tuple[int, int]:
@@ -382,6 +381,11 @@ class ShardedGfkb:
         # (live df int64 by feature, live row count) of the whole sharded corpus, all-reduced by build_packed and
         # delete_rows in rows mode on several GPUs (None: not known, the shards' own statistics when W = 1)
         self._stats: Optional[Tuple[np.ndarray, int]] = None
+
+    @property
+    def n_rows(self) -> int:
+        """Rows of the whole corpus, deleted ones included, as ``GfkbIndex.n_rows`` of one index holding them all."""
+        return self.n_global
 
     def build_packed(self, data, offsets: np.ndarray, mode: int = 0, n_threads: int = 0) -> None:
         import torch
@@ -1311,33 +1315,21 @@ class ShardedGfkbStore(GfkbStore):
             groups = self._dev_groups(self._n_dev) if groups is None else groups
             tail.set_row_groups(groups[self._n_main:self._n_main + tail.n_rows])
 
-    def _candidates(self, fb: FeatureBatch, k: int, limit: int = MATCH_LIMIT, labels: Optional[np.ndarray] = None,
-                    distinct: bool = False, tags=None):
-        import torch
-        import torch.distributed as dist
-
-        kk = min(k, MAX_LIMIT)
-        if fb.n == 0:
-            return np.zeros((0, kk), np.int64), np.zeros((0, kk)), np.zeros(0, dtype=bool)
-        if distinct:
-            self._ensure_groups()
-        main = self._main
-        main.set_resident(fb)
-        s, r = main.topk_resident(kk, labels=labels, distinct=distinct, tags=tags)
+    def _segment_candidates(self, ix, fb: FeatureBatch, kk: int, labels: Optional[np.ndarray], distinct: bool, tags):
+        if ix is not self._main:
+            return super()._segment_candidates(ix, fb, kk, labels, distinct, tags)
+        ix.set_resident(fb)
+        s, r = ix.topk_resident(kk, labels=labels, distinct=distinct, tags=tags)
         s32, rows = s.cpu().numpy(), r.cpu().numpy()
-        amb = ambiguous_candidates(s32, rows, limit)
-        f64 = main.index.rescore(fb, rows)   # -inf for the rows of the other shards
+        f64 = ix.index.rescore(fb, rows)   # -inf for the rows of the other shards
         if self.world > 1:
+            import torch
+            import torch.distributed as dist
+
             t = torch.from_numpy(f64).to(f"cuda:{self.device}")
             dist.all_reduce(t, op=dist.ReduceOp.MAX, group=self.group)
             f64 = t.cpu().numpy()
-        rows_all, f64_all = [rows], [f64]
-        if self._tail is not None and self._tail.n_rows:
-            s32, rows = self._segment_topk(self._tail, fb, kk, labels, distinct, tags)
-            amb |= ambiguous_candidates(s32, rows, limit)
-            rows_all.append(rows)
-            f64_all.append(self._tail.rescore(fb, rows))
-        return self._merge_candidates(rows_all, f64_all, distinct) + (amb,)
+        return s32, rows, f64
 
     def _above(self, fb: FeatureBatch, threshold: float, labels, tags):
         raise NotImplementedError("ShardedGfkbStore.match_above: the exact threshold search is not built for a "

@@ -66,6 +66,13 @@ def stable_top(scores: np.ndarray, limit: int) -> List[int]:
     return idx[np.lexsort((idx, -scores[idx]))].tolist()       # score descending, then row ascending
 
 
+def _first_of_each_group(groups: np.ndarray) -> np.ndarray:
+    """Ascending positions of the first entry of each group in ``groups``: a distinct result keeps its group's first
+    row in the order given."""
+    _, first = np.unique(groups, return_index=True)
+    return np.sort(first)
+
+
 def ambiguous_candidates(s32: np.ndarray, rows: np.ndarray, limit: int) -> np.ndarray:
     """Per query: could a row that did NOT make a segment's float32 candidate list belong to the float64 top-``limit``?
     Only if the list is full and its last score is within float32 rounding of its ``limit``-th score.  Exact zeros are
@@ -592,6 +599,9 @@ class GfkbStore:
         query the failure-type label its candidates must carry (-1: any).  ``distinct``: each segment returns one row
         per (failure_type, signature_text) group, and the merge keeps the first row of each group.  ``tags``: per query
         the app tags one of which its candidates must carry (empty: any)."""
+        kk = min(k, MAX_LIMIT)
+        if fb.n == 0:
+            return np.zeros((0, kk), np.int64), np.zeros((0, kk)), np.zeros(0, dtype=bool)
         if distinct:
             self._ensure_groups()
         rows_all, f64_all = [], []
@@ -599,22 +609,18 @@ class GfkbStore:
         for ix in (self._main, self._tail):
             if ix is None or ix.n_rows == 0:
                 continue
-            s32, rows = (self._segment_topk(ix, fb, min(k, MAX_LIMIT), labels, distinct) if tags is None
-                         else self._segment_topk(ix, fb, min(k, MAX_LIMIT), labels, distinct, tags))
+            s32, rows, f64 = self._segment_candidates(ix, fb, kk, labels, distinct, tags)
             amb |= ambiguous_candidates(s32, rows, limit)
             rows_all.append(rows)
-            f64_all.append(ix.rescore(fb, rows))
+            f64_all.append(f64)
         return self._merge_candidates(rows_all, f64_all, distinct) + (amb,)
 
-    @staticmethod
-    def _segment_topk(ix: GfkbIndex, fb: FeatureBatch, kk: int, labels: Optional[np.ndarray],
-                      distinct: bool, tags=None) -> Tuple[np.ndarray, np.ndarray]:
-        """One segment's float32 candidates: (scores, global rows), each [Q, kk]."""
-        if tags is not None:
-            return ix.topk_features(fb, kk, labels, distinct, tags)
-        if distinct:
-            return ix.topk_features(fb, kk, labels, distinct=True)
-        return ix.topk_features(fb, kk) if labels is None else ix.topk_features(fb, kk, labels)
+    def _segment_candidates(self, ix, fb: FeatureBatch, kk: int, labels: Optional[np.ndarray], distinct: bool,
+                            tags) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """One segment's float32 candidates and their float64 (K6) scores: (scores, global rows, K6 scores), each
+        [Q, kk].  ``ShardedGfkbStore`` replaces it for its sharded MAIN segment."""
+        s32, rows = ix.topk_features(fb, kk, labels, distinct, tags)
+        return s32, rows, ix.rescore(fb, rows)
 
     def _merge_candidates(self, rows_all: List[np.ndarray], f64_all: List[np.ndarray],
                           distinct: bool) -> Tuple[np.ndarray, np.ndarray]:
@@ -635,19 +641,26 @@ class GfkbStore:
         out_r = np.full_like(recs, -1)
         out_s = np.full_like(f64, -np.inf)
         for q in range(recs.shape[0]):
-            seen, j = set(), 0
-            for r, sc in zip(recs[q].tolist(), f64[q].tolist()):
-                if r < 0 or groups[r] in seen:
-                    continue
-                seen.add(groups[r])
-                out_r[q, j], out_s[q, j] = r, sc
-                j += 1
+            live = np.flatnonzero(recs[q] >= 0)
+            keep = live[_first_of_each_group(groups[recs[q, live]])]
+            out_r[q, :len(keep)], out_s[q, :len(keep)] = recs[q, keep], f64[q, keep]
         return out_r, out_s
 
     def _distinct_match(self, rec: int, score: float) -> dict:
         """A distinct result: its key's NEWEST record (the one the next upsert would version) with the key's score."""
         r = self.records[rec]
         return _to_match(self.records[self._latest[(r["failure_type"], r["signature_text"])]], score)
+
+    def _matches(self, recs: Sequence[int], scores: Sequence[float], distinct: bool,
+                 failure_type: Optional[str] = None) -> List[dict]:
+        """Records (-1: none) and scores -> FailureMatch dicts, after the reference's failure_type post-filter
+        (app.py:91-93); ``distinct``: each reported with its key's newest record (``_distinct_match``)."""
+        out = []
+        for r, s in zip(recs, scores):
+            if r < 0 or (failure_type and self.records[r]["failure_type"] != failure_type):
+                continue
+            out.append(self._distinct_match(r, s) if distinct else _to_match(self.records[r], s))
+        return out
 
     def _exact_top(self, signature_text: str, limit: int, label: int = -1,
                    distinct: bool = False, app: int = -1) -> Tuple[List[int], List[float]]:
@@ -657,99 +670,36 @@ class GfkbStore:
         the rows whose record lists that app (tag)."""
         parts = [ix.score(signature_text) for ix in (self._main, self._tail) if ix is not None and ix.n_rows]
         scores = np.concatenate(parts)  # by device row; -inf for a deleted row
-        if app >= 0:  # a deleted row lists no app
-            self._sync_apps()
-            recs = self._dev_recs(0, len(scores))
-            elig = (recs >= 0) & self._apps.records_with(app)[np.clip(recs, 0, None)]
+        n = len(scores)
+        if label < 0 and app < 0 and not distinct and self._row2rec is None:  # every row: no copy of the scores
+            order = np.asarray(stable_top(scores, limit), dtype=np.int64)
+        else:
+            recs = self._dev_recs(0, n)
+            elig = recs >= 0
             if label >= 0:
-                elig &= self._dev_labels(len(scores)) == label
+                elig &= self._dev_labels(n) == label
+            if app >= 0:
+                self._sync_apps()
+                elig &= self._apps.records_with(app)[np.clip(recs, 0, None)]
             idx = np.flatnonzero(elig)  # ascending: the stable order is kept
             if distinct:
-                _, first = np.unique(self._dev_groups(len(scores))[idx], return_index=True)
-                idx = idx[np.sort(first)]
+                idx = idx[_first_of_each_group(self._dev_groups(n)[idx])]
             order = idx[stable_top(scores[idx], limit)]
-        elif distinct:
-            if label >= 0:
-                idx = np.flatnonzero(self._dev_labels(len(scores)) == label)
-            elif self._row2rec is not None:
-                idx = np.flatnonzero(self._row2rec >= 0)
-            else:
-                idx = np.arange(len(scores))
-            _, first = np.unique(self._dev_groups(len(scores))[idx], return_index=True)
-            idx = idx[np.sort(first)]  # ascending: the stable order is kept
-            order = idx[stable_top(scores[idx], limit)]
-        elif label >= 0:
-            idx = np.flatnonzero(self._dev_labels(len(scores)) == label)  # ascending: the stable order is kept
-            order = idx[stable_top(scores[idx], limit)]
-        elif self._row2rec is not None:
-            idx = np.flatnonzero(self._row2rec >= 0)
-            order = idx[stable_top(scores[idx], limit)]
-        else:
-            order = np.asarray(stable_top(scores, limit), dtype=np.int64)
         return self._to_records(order).tolist(), [float(scores[i]) for i in order]
 
-    def _match_filter_first(self, signature_texts: Sequence[str], failure_types: Sequence[Optional[str]],
-                            limit: int, distinct: bool = False) -> List[List[dict]]:
-        """The best ``limit`` rows OF each query's failure type (all rows for a query without one)."""
-        self._row_labels(0, len(self.records))  # number every stored type
-        labels = np.array([-1 if not ft else self._type_ids.get(ft, -2) for ft in failure_types], dtype=np.int32)
-        out: List[List[dict]] = [[] for _ in signature_texts]
-        scan = np.flatnonzero(labels != -2)  # a type no stored row has: no match, and nothing to scan
-        if len(scan) == 0:
-            return out
-        fb = self.vocab.featurize([signature_texts[i] for i in scan], grow=False)
-        try:
-            if distinct:
-                rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit, labels[scan], True)
-            else:
-                rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit, labels[scan])
-        finally:
-            fb.close()
-        for j, i in enumerate(scan.tolist()):
-            if amb[j]:
-                top_r, top_s = (self._exact_top(signature_texts[i], limit, int(labels[i]), True) if distinct
-                                else self._exact_top(signature_texts[i], limit, int(labels[i])))
-                self.stats["exact_fallbacks"] = self.stats.get("exact_fallbacks", 0) + 1
-            else:
-                top_r, top_s = rows[j, :limit].tolist(), f64[j, :limit].tolist()
-            to_match = self._distinct_match if distinct else (lambda r, s: _to_match(self.records[r], s))
-            out[i] = [to_match(r, s) for r, s in zip(top_r, top_s) if r >= 0]
-        return out
-
-    def _match_apps(self, signature_texts: Sequence[str], failure_types: Optional[Sequence[Optional[str]]],
-                    app_ids: Sequence[Optional[str]], limit: int, filter_first: bool, distinct: bool) -> List[List[dict]]:
-        """The best ``limit`` rows among the failures whose affected_apps list the query's app (all rows for a query
-        without one), searched on the device through the app tags; with ``filter_first`` also of the query's
-        failure_type, else the failure_type post-filter of the reference follows."""
-        self._row_labels(0, len(self.records))  # number every stored type
-        self._sync_apps()                        # ... and every listed app
-        apps = np.array([-1 if not a else self._apps.listed(a) for a in app_ids], dtype=np.int64)
-        labels = np.full(len(signature_texts), -1, dtype=np.int32)
-        if filter_first and failure_types is not None:
+    def _resolve_filters(self, n: int, failure_types: Optional[Sequence[Optional[str]]],
+                         app_ids: Optional[Sequence[Optional[str]]]) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """Per query of ``n``: the failure-type label (-1: any, -2: a type no record has), the app id (-1: any, -2: an
+        app no record lists), and the queries to scan (neither -2: the others match nothing)."""
+        labels = np.full(n, -1, dtype=np.int32)
+        if failure_types is not None and any(failure_types):
+            self._row_labels(0, len(self.records))  # number every stored type
             labels = np.array([-1 if not ft else self._type_ids.get(ft, -2) for ft in failure_types], dtype=np.int32)
-        out: List[List[dict]] = [[] for _ in signature_texts]
-        scan = np.flatnonzero((apps != -2) & (labels != -2))  # an app or type no stored row has: no match, no scan
-        if len(scan) == 0:
-            return out
-        self._ensure_tags()
-        tags = [[int(apps[i])] if apps[i] >= 0 else [] for i in scan.tolist()]
-        fb = self.vocab.featurize([signature_texts[i] for i in scan], grow=False)
-        try:
-            rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit,
-                                              labels[scan] if (labels >= 0).any() else None, distinct, tags)
-        finally:
-            fb.close()
-        to_match = self._distinct_match if distinct else (lambda r, s: _to_match(self.records[r], s))
-        for j, i in enumerate(scan.tolist()):
-            if amb[j]:
-                top_r, top_s = self._exact_top(signature_texts[i], limit, int(labels[i]), distinct, int(apps[i]))
-                self.stats["exact_fallbacks"] = self.stats.get("exact_fallbacks", 0) + 1
-            else:
-                top_r, top_s = rows[j, :limit].tolist(), f64[j, :limit].tolist()
-            ft = failure_types[i] if failure_types is not None else None
-            out[i] = [to_match(r, s) for r, s in zip(top_r, top_s)
-                      if r >= 0 and not (ft and self.records[r]["failure_type"] != ft)]
-        return out
+        apps = np.full(n, -1, dtype=np.int64)
+        if app_ids is not None and any(app_ids):
+            self._sync_apps()                    # intern every listed app
+            apps = np.array([-1 if not a else self._apps.listed(a) for a in app_ids], dtype=np.int64)
+        return labels, apps, np.flatnonzero((labels != -2) & (apps != -2))
 
     def match_batch(self, signature_texts: Sequence[str], failure_types: Optional[Sequence[Optional[str]]] = None,
                     limit: int = MATCH_LIMIT, filter_first: bool = False, distinct: bool = False,
@@ -765,48 +715,39 @@ class GfkbStore:
             raise ValueError(f"limit {limit} exceeds the {MAX_LIMIT} rows the fused top-k holds per query")
         if app_ids is not None and len(app_ids) != len(signature_texts):
             raise ValueError(f"app_ids: {len(app_ids)} apps for {len(signature_texts)} queries")
+        out: List[List[dict]] = [[] for _ in signature_texts]
         with self._lock:
             if not self.records:
-                return [[] for _ in signature_texts]  # app.py:82-83
+                return out  # app.py:82-83
             self._sync()
-            if app_ids is not None and any(app_ids):
-                return self._match_apps(signature_texts, failure_types, app_ids, limit, filter_first, distinct)
-            if filter_first and failure_types is not None and any(failure_types):
-                return self._match_filter_first(signature_texts, failure_types, limit, distinct)
-            fb = self.vocab.featurize(list(signature_texts), grow=False)
+            labels, apps, scan = self._resolve_filters(len(signature_texts), failure_types if filter_first else None,
+                                                       app_ids)
+            if len(scan) == 0:
+                return out
+            tags = None
+            if (apps[scan] >= 0).any():
+                self._ensure_tags()
+                tags = [[int(apps[i])] if apps[i] >= 0 else [] for i in scan.tolist()]
+            fb = self.vocab.featurize([signature_texts[i] for i in scan], grow=False)
             try:
-                if distinct:
-                    rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit, distinct=True)
-                else:
-                    rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit)
+                rows, f64, amb = self._candidates(fb, max(CANDIDATES, limit), limit,
+                                                  labels[scan] if (labels[scan] >= 0).any() else None, distinct, tags)
             finally:
                 fb.close()
-            out = []
-            for i in range(len(signature_texts)):
-                ft = failure_types[i] if failure_types is not None else None
-                matches = []
-                if amb[i]:  # float32 candidates cannot decide this query's top rows: full float64 scan
-                    top_r, top_s = (self._exact_top(signature_texts[i], limit, distinct=True) if distinct
-                                    else self._exact_top(signature_texts[i], limit))
+            for j, i in enumerate(scan.tolist()):
+                if amb[j]:  # float32 candidates cannot decide this query's top rows: full float64 scan
+                    top_r, top_s = self._exact_top(signature_texts[i], limit, int(labels[i]), distinct, int(apps[i]))
                     self.stats["exact_fallbacks"] = self.stats.get("exact_fallbacks", 0) + 1
                 else:
-                    top_r, top_s = rows[i, :limit].tolist(), f64[i, :limit].tolist()
-                for r, s in zip(top_r, top_s):
-                    if r < 0:
-                        continue
-                    rec = self.records[r]
-                    if ft and rec["failure_type"] != ft:
-                        continue
-                    matches.append(self._distinct_match(r, s) if distinct else _to_match(rec, s))
-                out.append(matches)
+                    top_r, top_s = rows[j, :limit].tolist(), f64[j, :limit].tolist()
+                # under filter_first the rows already carry the type: the post-filter drops none of them
+                out[i] = self._matches(top_r, top_s, distinct, failure_types[i] if failure_types is not None else None)
             return out
 
     def match(self, signature_text: str, failure_type: Optional[str] = None, filter_first: bool = False,
               distinct: bool = False, app_id: Optional[str] = None) -> List[dict]:
-        if app_id is not None:
-            return self.match_batch([signature_text], [failure_type], filter_first=filter_first, distinct=distinct,
-                                    app_ids=[app_id])[0]
-        return self.match_batch([signature_text], [failure_type], filter_first=filter_first, distinct=distinct)[0]
+        return self.match_batch([signature_text], [failure_type], filter_first=filter_first, distinct=distinct,
+                                app_ids=[app_id])[0]
 
     def match_exact(self, signature_text: str, failure_type: Optional[str] = None, limit: int = MATCH_LIMIT) -> List[dict]:
         """The handler on the full float64 score vector (K1a on both segments): no candidate stage at all."""
@@ -815,13 +756,7 @@ class GfkbStore:
                 return []
             self._sync()
             order, top = self._exact_top(signature_text, limit)
-            out = []
-            for i, sc in zip(order, top):
-                rec = self.records[i]
-                if failure_type and rec["failure_type"] != failure_type:
-                    continue
-                out.append(_to_match(rec, sc))
-            return out
+            return self._matches(order, top, False, failure_type)
 
     # -- match above a threshold (services/gfkb/app.py:88-89 without the first-5 cut) -----------------------------
     def _above(self, fb: FeatureBatch, threshold: float, labels: Optional[np.ndarray],
@@ -854,15 +789,7 @@ class GfkbStore:
             if not self.records:
                 return out
             self._sync()
-            self._row_labels(0, len(self.records))  # number every stored type
-            labels = np.full(n, -1, dtype=np.int32)
-            if failure_types is not None:
-                labels = np.array([-1 if not ft else self._type_ids.get(ft, -2) for ft in failure_types], dtype=np.int32)
-            apps = np.full(n, -1, dtype=np.int64)
-            if app_ids is not None and any(app_ids):
-                self._sync_apps()
-                apps = np.array([-1 if not a else self._apps.listed(a) for a in app_ids], dtype=np.int64)
-            scan = np.flatnonzero((labels != -2) & (apps != -2))  # an unknown type or app: no match, no scan
+            labels, apps, scan = self._resolve_filters(n, failure_types, app_ids)
             if len(scan) == 0:
                 return out
             tags = None
@@ -879,16 +806,11 @@ class GfkbStore:
                 rows = np.concatenate([p[1][p[0][j]:p[0][j + 1]] for p in parts] or [np.zeros(0, np.int64)])
                 scores = np.concatenate([p[2][p[0][j]:p[0][j + 1]] for p in parts] or [np.zeros(0)])
                 order = np.lexsort((rows, -scores))  # score desc, device row asc = the records' stable order
-                recs, scores = self._to_records(rows[order]).tolist(), scores[order].tolist()
+                recs, scores = self._to_records(rows[order]), scores[order]
                 if distinct:
-                    seen, matches = set(), []
-                    for r, sc in zip(recs, scores):
-                        if groups[r] not in seen:
-                            seen.add(groups[r])
-                            matches.append(self._distinct_match(r, sc))
-                    out[i] = matches
-                else:
-                    out[i] = [_to_match(self.records[r], sc) for r, sc in zip(recs, scores)]
+                    keep = _first_of_each_group(groups[recs])
+                    recs, scores = recs[keep], scores[keep]
+                out[i] = self._matches(recs.tolist(), scores.tolist(), distinct)
             return out
 
     def match_above(self, signature_text: str, threshold: float, failure_type: Optional[str] = None,

@@ -621,7 +621,7 @@ def test_store_distinct_main_and_tail(lib):
         check_store(st, qs, ft=ft, filter_first=True)
 
 
-def test_store_distinct_ambiguous_candidates(built_lib, monkeypatch):
+def test_store_distinct_ambiguous_candidates_take_group_aware_exact_path(built_lib, monkeypatch):
     """Colliding float32 groups force the exact path, which must be group-aware: key B (rows 20..39) beats key A (rows
     0..19) in float64 only; rows 40..59 are distinct keys at 0.25.  Each key is reported with its newest record."""
     from kakveda_b200 import GfkbStore
@@ -640,7 +640,7 @@ def test_store_distinct_ambiguous_candidates(built_lib, monkeypatch):
             self.groups = np.asarray(groups)
             self.has_row_groups = True
 
-        def topk_features(self, fb, k, labels=None, distinct=False):
+        def topk_features(self, fb, k, labels=None, distinct=False, tags=None):
             assert distinct and self.has_row_groups
             s32 = f64.astype(np.float32)
             _, first = np.unique(self.groups, return_index=True)

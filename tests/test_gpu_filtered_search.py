@@ -391,7 +391,7 @@ def test_store_filter_first_main_and_tail(lib):
             np.testing.assert_allclose([m["score"] for m in ms], [s for _, s in want], rtol=1e-9)
 
 
-def test_store_filter_first_ambiguous_candidates(built_lib, monkeypatch):
+def test_store_filter_first_ambiguous_candidates_take_filtered_exact_path(built_lib, monkeypatch):
     """Colliding float32 groups of the filtered type force the exact path, which must be filter-aware: group B (rows
     20..39, type T) beats group A (rows 0..19, type T) in float64 only; rows 40..59 (type U) score higher than both."""
     from kakveda_b200 import GfkbStore
@@ -407,7 +407,7 @@ def test_store_filter_first_ambiguous_candidates(built_lib, monkeypatch):
     class FakeIndex:
         n_rows = n
 
-        def topk_features(self, fb, k, labels=None):
+        def topk_features(self, fb, k, labels=None, distinct=False, tags=None):
             s32 = np.where(allowed, f64, -np.inf).astype(np.float32) if labels is not None else f64.astype(np.float32)
             order = np.lexsort((np.arange(n), -s32))[:k]
             return np.tile(s32[order], (fb.n, 1)), np.tile(order.astype(np.int64), (fb.n, 1))

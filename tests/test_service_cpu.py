@@ -138,7 +138,7 @@ def test_sidecar_save_load_and_staleness(built_lib, tmp_path):
     assert sidecar.load(tmp_path / "bad.npz", texts) is None
 
 
-def test_store_match_and_warn_host_logic_with_canned_candidates(golden, built_lib, monkeypatch):
+def test_store_match_and_warn_host_logic_on_canned_candidate_stage(golden, built_lib, monkeypatch):
     """The host half of GfkbStore.match_batch / warn_batch (services/gfkb/app.py:88-100,
     services/warning_policy/app.py:30-72) on CPU: the device stage is replaced by candidates taken from the
     reference's recorded float64 scores, so the truncate-to-5-THEN-filter rule, the FailureMatch mapping and the
@@ -162,7 +162,7 @@ def test_store_match_and_warn_host_logic_with_canned_candidates(golden, built_li
                 pass
         return _B()
 
-    def fake_candidates(fb, k, limit=5):
+    def fake_candidates(fb, k, limit=5, labels=None, distinct=False, tags=None):
         rows, f64 = [], []
         for t in current["texts"]:
             s = by_query[t]
@@ -224,7 +224,7 @@ def test_ambiguous_candidates_rule():
     assert ambiguous_candidates(s, rows, 5).tolist() == [False, True, True, False, False, False]
 
 
-def test_store_match_takes_exact_path_when_float32_candidates_collide(built_lib, monkeypatch):
+def test_store_match_takes_exact_path_when_float32_scores_of_distinct_texts_collide(built_lib, monkeypatch):
     """ADVICE round 1: two distinct texts, each stored more than 16 times, whose float64 scores collide in float32.
     The float32 candidate list then holds only the group with the lower row ids; the reference's stable float64 top-5
     (services/gfkb/app.py:88-89) is the OTHER group.  The store must notice and take the exact path."""
@@ -241,7 +241,7 @@ def test_store_match_takes_exact_path_when_float32_candidates_collide(built_lib,
     class FakeIndex:
         n_rows = n
 
-        def topk_features(self, fb, k):
+        def topk_features(self, fb, k, labels=None, distinct=False, tags=None):
             s32 = f64.astype(np.float32)
             order = np.lexsort((np.arange(n), -s32))[:k]          # float32 score desc, row asc: what K1b returns
             return np.tile(s32[order], (fb.n, 1)), np.tile(order.astype(np.int64), (fb.n, 1))
@@ -273,6 +273,62 @@ def test_store_match_takes_exact_path_when_float32_candidates_collide(built_lib,
     assert st.stats["exact_fallbacks"] == 2
     assert [m["failure_id"] for m in st.match_exact("q0")] == [f"F-{i:04d}" for i in want]
     st._main = None
+
+
+def test_store_exact_top_eligibility_matches_brute_force(built_lib):
+    """The exact fallback (``GfkbStore._exact_top``) against Python's stable sort over the eligible records: live, of
+    the label's failure type, listing the app, and under ``distinct`` only the first record of each (failure_type,
+    signature_text) key.  Every combination of label, app and distinct, with and without deleted device rows, over two
+    segments and a score vector with heavy ties (a deleted row scores above every live one, so it must be excluded)."""
+    import itertools
+
+    from kakveda_b200 import GfkbStore
+
+    class Segment:
+        def __init__(self, scores):
+            self.scores, self.n_rows = scores, len(scores)
+
+        def score(self, text):
+            return self.scores.copy()
+
+    rng = np.random.default_rng(11)
+    n_rec, n_del = 240, 40
+    records = [{"failure_type": "ABC"[rng.integers(0, 3)], "signature_text": f"t{rng.integers(0, 25)}",
+                "affected_apps": sorted(set(rng.choice(list("wxyz"), size=rng.integers(1, 3)).tolist()))}
+               for _ in range(n_rec)]
+    for deleted in (False, True):
+        n_dev = n_rec + (n_del if deleted else 0)
+        scores = rng.integers(0, 4, size=n_dev) / 4
+        live = np.arange(n_dev)
+        st = GfkbStore()
+        st.records = records
+        st._n_indexed = n_rec
+        if deleted:
+            dead = rng.choice(n_dev, size=n_del, replace=False)
+            scores[dead] = 1.0
+            live = np.setdiff1d(live, dead)
+            st._row2rec = np.full(n_dev, -1, dtype=np.int64)
+            st._row2rec[live] = np.arange(n_rec)
+        rec_score = scores[live].tolist()
+        split = n_dev * 2 // 3
+        st._main, st._tail = Segment(scores[:split]), Segment(scores[split:])
+        st._row_labels(0, n_rec)
+        st._sync_apps()
+        app_name = {i: a for a, i in st._apps.ids.items()}
+        for label, app, distinct, limit in itertools.product([-1] + sorted(st._type_ids.values()),
+                                                             [-1] + sorted(app_name), (False, True), (1, 5, 32, 300)):
+            elig = [r for r, rec in enumerate(records)
+                    if (label < 0 or st._type_ids[rec["failure_type"]] == label)
+                    and (app < 0 or app_name[app] in rec["affected_apps"])]
+            if distinct:
+                first = {}
+                for r in elig:
+                    first.setdefault((records[r]["failure_type"], records[r]["signature_text"]), r)
+                elig = sorted(first.values())
+            want = sorted(elig, key=lambda r: rec_score[r], reverse=True)[:limit]
+            got = st._exact_top("q", limit, label, distinct, app)
+            assert got == (want, [rec_score[r] for r in want]), (deleted, label, app, distinct, limit)
+        st._main = st._tail = None
 
 
 def test_store_rejects_unindexable_rows_before_persisting(tmp_path):
